@@ -1,7 +1,7 @@
 #!/usr/bin/env python
-"""bench.py — headline benchmark of the B200-native metering engine (contract: see the task statement).
+"""bench.py — headline benchmark of the CUDA metering engine.
 
-    python bench.py [--gpus N] [--steps K] [--warmup W] [--impl b200|reference]
+    python bench.py [--gpus N] [--steps K] [--warmup W] [--impl b200|reference] [--dump-outputs DIR]
     python -m torch.distributed.run --nnodes=1 --nproc-per-node N --master-addr 127.0.0.1 ... bench.py --gpus N ...
 
 Workload (BASELINE.json `metric`: "audio-samples/sec/GPU (48 kHz stereo, 8192-ch batch) EBU R128 + true-peak"):
@@ -16,6 +16,9 @@ both channels + getters).  One "step" = one such cycle over the whole batch = 16
 `e2e`    = the same cycle through b200m_r128_run_host with pinned HOST buffers, H2D copy and D2H result read inside the
            timed region (PCIe-bound: 64 MiB per cycle cannot shrink, the LV2 contract is float32 audio).
 `--impl reference` times the reference's own CPU code (oracle/_ref, else the oracle port) on every CPU the process may use.
+`--dump-outputs DIR` writes, after the timed steps, what the headline path returns to its caller after its last timed step
+(b200m_r128_results: the EBU R128 result fields and the dBTP hold of every instance, rank 0) as DIR/<name>.npy.  The input
+ring and the block sequence are seeded, so two builds run with the same arguments can be compared output for output.
 
 The JSON line is printed (and flushed) as soon as the headline, e2e, roofline and cpu_baseline exist; the other BASELINE
 configs, the whole-mix all-reduce and the parity spot check run afterwards and the enriched line is printed again
@@ -38,7 +41,7 @@ METRIC = "audio-samples/sec/GPU (48 kHz stereo, 8192-ch batch) EBU R128 + true-p
 FS = 48000.0
 N_INST = 8192          # stereo instances per GPU
 NFRAM = 1024
-RING = 8               # distinct device-resident blocks: 8 x 64 MiB = 512 MiB > 126 MB L2
+RING = 8               # distinct device-resident blocks: 8 x 64 MiB = 512 MiB > 50 MB L2
 PRIME = 480            # untimed blocks (10.2 s of audio) so that S, I (>=50 M-points) and LRA (>=20 S-points) are live
 SAMPLES_PER_STEP = N_INST * 2 * NFRAM
 CPU_BLOCKS = 4         # blocks per CPU step
@@ -49,20 +52,13 @@ def peaks():
     if os.path.exists(p):
         d = json.load(open(p))
         return float(d["hbm_gbs"]), "measured (MEASURED_PEAKS.json)"
-    return 6650.0, "fallback (B200_PROFILING.md)"
+    return 3350.0, "data sheet (H100 SXM HBM3)"
 
 
 def bf16_peak_tflops():
     p = os.path.join(ROOT, "MEASURED_PEAKS.json")
     if os.path.exists(p):
         return float(json.load(open(p)).get("bf16_tflops", 0.0)) or None
-    return None
-
-
-def traffic_for(kernel):
-    p = os.path.join(ROOT, "profiles", "traffic.json")
-    if os.path.exists(p):
-        return json.load(open(p)).get(kernel)
     return None
 
 
@@ -181,6 +177,8 @@ def run_b200(args):
     ms = timed_loop(torch, dist, ws, step, K)
     launches = B.launch_count() - l0
     sampler.stop_flag = True; sampler.join()
+    if args.dump_outputs and rank == 0:
+        dump_outputs(args.dump_outputs, *bank.results())
     value = ws * SAMPLES_PER_STEP * K / (ms * 1e-3)
     bank.set_precision(B.PREC_EXACT)
     for s in range(W):
@@ -275,16 +273,16 @@ def run_b200(args):
     eb_gbs = alg_bytes / (ms_eb / K * 1e-3) / 1e9
     # fp32 instructions the FIR executes per input sample: tolerance mode 120 (72 FFMA + 48 FADD, csrc/tpk.cu fir16_fma);
     # exact mode 288 unfused FMUL/FADD for phases 1-3 (+96 for phase 0 where the exact-delay guard fails: never on this noise)
-    out["roofline"] = {"kernel": "tpmax_tc_kernel (4x polyphase FIR as a Toeplitz GEMM on tcgen05 kind::tf32 with the 3xTF32 split, + max; tolerance mode)",
+    out["roofline"] = {"kernel": "tpmax_tc_kernel (4x polyphase FIR as a Toeplitz GEMM on wgmma tf32 with the 3xTF32 split, + max; tolerance mode)",
                        "bound": "hbm", "achieved": tp_gbs, "peak": hbm_peak,
-                       "unit": "GB/s", "frac": tp_gbs / hbm_peak, "traffic": traffic_for("tpmax_tc_kernel"), "peak_source": peak_src,
+                       "unit": "GB/s", "frac": tp_gbs / hbm_peak, "peak_source": peak_src,
                        "ms_per_launch": ms_tp / K, "algorithmic_bytes_per_launch": alg_bytes,
-                       "note": "bound by its producer / epilogue warps (window -> {hi, lo} -> TMEM, TMEM -> maxima), not by HBM or the tensor pipe, see roofline_tensor and DESIGN.md; share of the cycle: %.0f%%" % (100.0 * ms_tp / ms)}
+                       "note": "share of the cycle: %.0f%%" % (100.0 * ms_tp / ms)}
     # executed tensor-core work: per [8 channels x 256 samples] tile 8 K-steps x (128 x 96 x 8 + 128 x 48 x 8) MACs (25 % of the Toeplitz B is zero,
     # and the three products of the split count three times): 1152 flop per input sample, of which 288 (3 phases x 48 taps x 2) are the FIR's own
     tf32_peak = (bf16_peak / 2.0) if bf16_peak else None
     tc_tflops = SAMPLES_PER_STEP * 1152.0 / (ms_tp / K * 1e-3) / 1e12
-    out["roofline_tensor"] = {"kernel": "tpmax_tc_kernel", "bound": "tensor (kind::tf32)", "achieved": tc_tflops, "peak": tf32_peak, "unit": "TFLOP/s",
+    out["roofline_tensor"] = {"kernel": "tpmax_tc_kernel", "bound": "tensor (tf32)", "achieved": tc_tflops, "peak": tf32_peak, "unit": "TFLOP/s",
                               "frac": (tc_tflops / tf32_peak) if tf32_peak else None, "executed_flop_per_sample": 1152, "fir_flop_per_sample": 288,
                               "peak_source": "half of MEASURED_PEAKS.json's dense bf16 rate (tf32 runs at half the bf16 rate)" if tf32_peak else "none"}
     out["roofline_alu"] = {"kernel": "tpmax_kernel<IMM,FMA> (the same FIR on the CUDA cores: B200M_TPK_TC=0, and every bank too small for the tensor-core grid)",
@@ -296,7 +294,7 @@ def run_b200(args):
                                               "frac": SAMPLES_PER_STEP * 288.0 / (ms_tpx / K * 1e-3) / 1e9 / fp32_peak}}
     out["roofline_kernels"] = [
         {"kernel": "ebu_kweight_frag (+ebu_fragment_kernel every 2400 frames)", "bound": "hbm", "achieved": eb_gbs, "peak": hbm_peak, "unit": "GB/s",
-         "frac": eb_gbs / hbm_peak, "traffic": traffic_for("ebu_kweight_frag"), "ms_per_block": ms_eb / K, "launches_per_block": eb_launch / K,
+         "frac": eb_gbs / hbm_peak, "ms_per_block": ms_eb / K, "launches_per_block": eb_launch / K,
          "samples_per_s": SAMPLES_PER_STEP * K / (ms_eb * 1e-3)}]
     del tpb, ebb
 
@@ -346,6 +344,15 @@ def run_b200(args):
             emit(out)
     if ws > 1:
         dist.destroy_process_group()
+
+
+def dump_outputs(d, res, tp):
+    """the arrays b200m_r128_results hands its caller, one .npy per field (integer counts as float64)"""
+    os.makedirs(d, exist_ok=True)
+    for name in res.dtype.names:
+        a = res[name]
+        np.save(os.path.join(d, name + ".npy"), a.astype(np.float64) if a.dtype.kind == "i" else a.astype(np.float32))
+    np.save(os.path.join(d, "tp_max.npy"), tp.astype(np.float32))
 
 
 def spot_check(B, bank, x, blocks_run, ni=2):
@@ -513,6 +520,7 @@ def main():
     ap.add_argument("--e2e-steps", type=int, default=100)
     ap.add_argument("--no-cpu", action="store_true", help="skip the cpu_baseline leg")
     ap.add_argument("--headline-only", action="store_true", help="skip the other BASELINE configs, whole-mix and spot check")
+    ap.add_argument("--dump-outputs", metavar="DIR", help="write the headline path's outputs after its last timed step to DIR/<name>.npy")
     args = ap.parse_args()
     if args.impl == "reference":
         run_reference(args)

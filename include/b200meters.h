@@ -1,4 +1,4 @@
-/* b200meters.h — C ABI of the B200-native batched audio-metering engine.
+/* b200meters.h — C ABI of the CUDA batched audio-metering engine (H100, sm_90a).
  *
  * One "bank" = N independent instances of one reference DSP class, all processed by one CUDA
  * kernel launch per process() call.  Entry points mirror, one for one, the methods an LV2 host
@@ -18,7 +18,7 @@
  *    reset-latch side effects) and stores the values in a device result block;
  *    `*_results` copies that block to the host (synchronises the stream it was given).
  *  - there is NO CPU fallback: a bank cannot be created without a CUDA device, and every
- *    sample is processed by the sm_100a kernels in meters.lv2_b200/csrc/.
+ *    sample is processed by the sm_90a kernels in meters.lv2_b200/csrc/.
  */
 #ifndef B200METERS_H
 #define B200METERS_H
@@ -56,8 +56,8 @@ int         b200m_host_free (void* p);
 /* number of kernel launches issued by this library since load (bench.py's gpu_launches) */
 uint64_t    b200m_launch_count (void);
 
-/* ALU ceilings measured on the device (the driver's MEASURED_PEAKS.json has only HBM and bf16 GEMM):
- * kind 0 = fp32 unfused FMUL+FADD issue rate, kind 1 = fp64 DMUL+DADD, kind 2 = packed fp32x2 FMUL2+FADD2;
+/* ALU ceilings measured on the device:
+ * kind 0 = fp32 unfused FMUL+FADD issue rate, kind 1 = fp64 DMUL+DADD;
  * result in 1e9 lane-operations/s. */
 int         b200m_peak_probe (int device, int kind, double* gops);
 
@@ -158,7 +158,7 @@ int b200m_tpk_process_host (b200m_tpk* h, const float* in, size_t stride, uint32
 /* Arithmetic of the 4x polyphase FIR (zita-resampler/resampler.cc:213-230).
  *   B200M_PREC_EXACT (default): the reference's operation order, unfused -- every float bit-identical to the reference build.
  *   B200M_PREC_FMA: fused multiply-add accumulation using the table's symmetry, phase 0 taken as the pure delay it is to
- *     7.7e-16: 2.4x fewer instructions; true-peak / dBTP readings stay within +-1e-4 dB of the reference (measured <= 2e-5 dB),
+ *     7.7e-16: 2.4x fewer instructions; true-peak / dBTP readings stay within +-1e-4 dB of the reference,
  *     the K-meter and every integer result are unaffected.  Default can be preset with B200M_TPK_PRECISION=fma. */
 enum { B200M_PREC_EXACT = 0, B200M_PREC_FMA = 1 };
 int b200m_tpk_set_precision (b200m_tpk* h, int mode);
@@ -258,7 +258,7 @@ int b200m_cor_results (b200m_cor* h, float* out, void* stream);           /* Stc
 /* B200M_PREC_EXACT (default): the five recurrences run serially in time, one lane per pair, bit-identical to the reference.
  * B200M_PREC_FMA: time-parallel evaluation -- the recurrences are linear one-pole filters, so a warp owns ONE pair, its lanes take
  * consecutive time segments and an affine warp scan stitches them: 32x more parallelism for small banks (2048 pairs are 64 warps
- * in exact mode); the correlation stays within 1e-5 of the reference (measured ~1e-7). */
+ * in exact mode); the correlation stays within 1e-5 of the reference. */
 int b200m_cor_set_precision (b200m_cor* h, int mode);
 int b200m_cor_state (b200m_cor* h, float* state5, void* stream);          /* [n][5] zl zr zlr zll zrr */
 int b200m_cor_coeffs (const b200m_cor* h, float w[2]);
@@ -322,7 +322,7 @@ int b200m_spec_destroy (b200m_spec* h);
 int b200m_spec_process_device (b200m_spec* h, const float* d_in, size_t stride, uint32_t nfram, float speed, float reset, void* stream);
 int b200m_spec_process_host (b200m_spec* h, const float* in, size_t stride, uint32_t nfram, float speed, float reset);
 /* B200M_PREC_EXACT (default): the reference's fp64 rounding sequence, ports bit-identical.  B200M_PREC_FMA: fused multiply-adds in the
- * biquad cascade (25 instead of 39 fp64 instructions per frame and band); band levels within +-1e-4 dB (measured ~1e-12 dB). */
+ * biquad cascade (25 instead of 39 fp64 instructions per frame and band); band levels within +-1e-4 dB. */
 int b200m_spec_set_precision (b200m_spec* h, int mode);
 /* ports 0..59 of every instance: 30 band levels (dB), 30 band maxima (dB) */
 int b200m_spec_results (b200m_spec* h, float* out60, void* stream);

@@ -1,13 +1,13 @@
-"""In-tree build of libb200meters.so (C ABI of include/b200meters.h) for sm_100a.
+"""In-tree build of libb200meters.so (C ABI of include/b200meters.h) for the H100 (sm_90a).
 
     python meters.lv2_b200/build.py [--force] [--verbose]
 
 Every .cu under csrc/ is compiled with
-    nvcc -gencode arch=compute_100a,code=sm_100a -O3 -lineinfo -fmad=false
+    nvcc -gencode arch=compute_90a,code=sm_90a -O3 -lineinfo -fmad=false
 (no FMA contraction: the per-sample pipelines must round exactly like the reference's SSE2 build,
 Makefile:35 of the reference; kernels that want FMA call fmaf()/__fma_rn explicitly) and linked into
-meters.lv2_b200/libb200meters.so next to this file, so that the .so travels with the repo snapshot
-to the GPU box.  nvcc cross-compiles without a GPU.
+meters.lv2_b200/libb200meters.so next to this file, where the package loads it from.  nvcc cross-compiles
+without a GPU.
 """
 import concurrent.futures as cf
 import os
@@ -21,7 +21,7 @@ OBJ = os.path.join(HERE, "build")
 LIB = os.path.join(HERE, "libb200meters.so")
 NVCC = shutil.which("nvcc") or "/usr/local/cuda/bin/nvcc"
 FLAGS = [
-    "-gencode", "arch=compute_100a,code=sm_100a", "-O3", "-lineinfo", "-std=c++17",
+    "-gencode", "arch=compute_90a,code=sm_90a", "-O3", "-lineinfo", "-std=c++17",
     "-fmad=false", "-prec-div=true", "-prec-sqrt=true", "-ftz=false",
     "-Xcompiler", "-fPIC,-O2,-ffp-contract=off,-fno-fast-math,-fvisibility=hidden",
     "-Xptxas", "-v", "-I", os.path.join(HERE, "..", "include"),
@@ -65,7 +65,7 @@ def build(force=False, verbose=False):
                     sys.stderr.write(log)
     objs = [os.path.join(OBJ, s[:-3] + ".o") for s in srcs]
     if jobs or not os.path.exists(LIB):
-        cmd = [NVCC, "-shared", "-o", LIB, *objs, "-gencode", "arch=compute_100a,code=sm_100a",
+        cmd = [NVCC, "-shared", "-o", LIB, *objs, "-gencode", "arch=compute_90a,code=sm_90a",
                "-Xcompiler", "-fPIC", "-Xlinker", "--no-undefined"]
         p = subprocess.run(cmd, capture_output=True, text=True)
         if p.returncode != 0:

@@ -1,4 +1,4 @@
-// common.cuh — shared host/device helpers of the b200meters CUDA library (sm_100a only).
+// common.cuh — shared host/device helpers of the b200meters CUDA library (sm_90a only).
 #pragma once
 #include <cuda_runtime.h>
 #include <stdint.h>

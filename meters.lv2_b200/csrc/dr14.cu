@@ -5,7 +5,7 @@
 // (:285-352: silence gate, 8000-bin RMS histogram in 0.01 dB steps, mean of the loudest 20 % of the windows, second
 // highest window peak), then read() of both meters and the port arithmetic (:418-462).
 //
-// B200 mapping: the window sums ride on the process() kernel as an extra lane role (TpkDr, tpk_internal.cuh) so the
+// Mapping: the window sums ride on the process() kernel as an extra lane role (TpkDr, tpk_internal.cuh) so the
 // input is still read once; the window clock is host-tracked and shared by all instances (reset_peaks is bank-wide),
 // so a window end is a launch-time constant `cut`.  The scoring is one warp per instance: the top-down histogram walk
 // is a ballot over 32 bins at a time, accumulated in exactly the reference's bin order.  Port values are computed on

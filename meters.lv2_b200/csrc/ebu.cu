@@ -130,8 +130,7 @@ struct PaddedStage {
         for (int t = 0; t < EBU_STAGES - 1; ++t) issue (t);
     }
     B200M_DEV void acquire (int) { cp_async_wait<EBU_STAGES - 2> (); __syncwarp (); }
-    // requested after tile t is consumed, not before: measured 178 vs 183 us per EBUr128 cycle (the earlier request competes
-    // with the recurrence for issue slots), 64-sample tiles x 3 stages vs 128 x 2: +5 us per cycle for -1.5 us standalone
+    // requested after tile t is consumed, not before (the earlier request competes with the recurrence for issue slots)
     B200M_DEV void release (int t) { __syncwarp (); issue (t + EBU_STAGES - 1); }
     B200M_DEV void drain () { cp_async_wait<0> (); }
     B200M_DEV const float* row (int t) const { return tile + (t % EBU_STAGES) * (32 * EBU_ROWP) + lane * EBU_ROWP; }
@@ -256,7 +255,7 @@ B200M_DEV void kw_warp (Stage& sg, int lane, int k, bool live, int nchans, int n
         if (b - a == EBU_TILE && cend >= b) {
             // fast path: a whole tile inside one chunk; float4 groups with a one-group register prefetch
             float4 cur = sg.ld4 (t, 0);
-#pragma unroll Stage::UNROLL                     // cp.async staging, measured: unroll 4 26.7 us/block, 2: 29.1, 8: 27.9
+#pragma unroll Stage::UNROLL
             for (int q = 0; q < EBU_TILE / 4; ++q) {
                 const float4 nxt = sg.ld4 (t, (q + 1) & (EBU_TILE / 4 - 1));
                 kw_step (cur.x, cf, z1, z2, z3, z4, sj);
@@ -318,17 +317,15 @@ ebu_kweight_frag (const float* __restrict__ in, size_t stride, int nchans, int k
 // ---- K1 split over two warps per 32 channels -------------------------------------------------------------------------------
 // The recurrence is two biquad-like stages in series (:321-322): stage 1  x = p - b1 z1 - b2 z2 + 1e-15  feeds stage 2
 // y = a0 x + a1 z1 + a2 z2 - c3 z3 - c4 z4;  z4 += z3;  z3 += y;  sj += y y.  Each stage is a 16-cycle dependent chain per sample, and
-// one warp per SM sub-partition (all a 16384-channel bank offers) cannot hide either behind the other: 36 cycles per sample measured.
+// one warp per SM sub-partition (all a 16384-channel bank offers) cannot hide either behind the other.
 // Here warp A runs stage 1 and hands the x stream to warp B (same sub-partition: warps w and w + 4 of the CTA) through a
 // double-buffered shared-memory tile; the two chains then interleave on one scheduler.  Every channel sees exactly the same
 // operations in the same order as in kw_warp, so the results stay bit-identical.  Named barriers (bar.arrive / bar.sync on 64
 // threads) hand the tiles over: a waiting warp is parked by the hardware and takes no issue slots from its partner.
-// MEASURED (round 2, profiles/r2_ncu_ebu_kweight_split.txt): 27.2 us under ncu against 22.8 us for the one-warp kernel, 28.6 vs 26.2 us
-// live -- slower, so it is opt-in (B200M_EBU_SPLIT=1) and kept for the record.  The premise was wrong: ncu's stall breakdown of
-// the one-warp kernel shows 21.5 issue cycles + 6.5 dependency-wait cycles + 8 other per sample, i.e. the warp is limited by the
-// ~21.5 instructions it must ISSUE per sample on its scheduler, not by the 16-cycle chains; a second warp on the SAME scheduler
-// adds hand-over instructions and barrier waits (0.54 cycles per instruction) without adding issue slots, and every scheduler of
-// the 128 SMs in use already hosts a warp.  Only more channels per scheduler help (0.65 of HBM at 32768 instances).
+// It is slower than the one-warp kernel, so it is opt-in (B200M_EBU_SPLIT=1) and kept for the record: the one-warp kernel is limited
+// by the ~21.5 instructions it must ISSUE per sample on its scheduler, not by the 16-cycle chains; a second warp on the SAME scheduler
+// adds hand-over instructions and barrier waits without adding issue slots, and every scheduler in use already hosts a warp.
+// Only more channels per scheduler help.
 constexpr int EBU_SPLIT_PAIRS = 4;
 constexpr int EBU_SPLIT_PAIR_FLOATS = (EBU_STAGES + 2) * 32 * EBU_ROWP;
 constexpr int EBU_SPLIT_SMEM = EBU_SPLIT_PAIRS * EBU_SPLIT_PAIR_FLOATS * 4;
@@ -879,9 +876,9 @@ int b200m_ebu_create (b200m_ebu** out, int device, uint32_t n_inst, uint32_t nch
     if (e == cudaSuccess) e = cudaFuncSetAttribute (ebu_kweight_tma<2>, cudaFuncAttributeMaxDynamicSharedMemorySize, EBU_TMA_SMEM);
     if (e == cudaSuccess) e = cudaFuncSetAttribute (ebu_kweight_tma<1>, cudaFuncAttributePreferredSharedMemoryCarveout, cudaSharedmemCarveoutMaxShared);
     if (e == cudaSuccess) e = cudaFuncSetAttribute (ebu_kweight_tma<2>, cudaFuncAttributePreferredSharedMemoryCarveout, cudaSharedmemCarveoutMaxShared);
-    // TMA staging is bit-identical and removes ~120 address instructions per tile, but measured no faster standalone (26.0 vs
-    // 25.8 us per block) and 3 % slower inside the EBUr128 cycle (the mbarrier try_wait spin takes issue slots from the
-    // co-running true-peak kernel, a scoreboard wait does not): opt-in with B200M_EBU_TMA=1
+    // TMA staging is bit-identical and removes ~120 address instructions per tile, but is no faster standalone and slower inside the
+    // EBUr128 cycle (the mbarrier try_wait spin takes issue slots from the co-running true-peak kernel, a scoreboard wait does not):
+    // opt-in with B200M_EBU_TMA=1
 #define EBU_SATTR(NC, AL) if (e == cudaSuccess) e = cudaFuncSetAttribute (ebu_kweight_split<NC, AL>, cudaFuncAttributeMaxDynamicSharedMemorySize, EBU_SPLIT_SMEM); \
     if (e == cudaSuccess) e = cudaFuncSetAttribute (ebu_kweight_split<NC, AL>, cudaFuncAttributePreferredSharedMemoryCarveout, cudaSharedmemCarveoutMaxShared)
     EBU_SATTR (1, true); EBU_SATTR (1, false); EBU_SATTR (2, true); EBU_SATTR (2, false);

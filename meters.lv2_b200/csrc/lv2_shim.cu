@@ -52,7 +52,7 @@ struct Shim {
 
 // ---- batched mode (opt-in: B200M_LV2_BATCH=<slots>) ---------------------------------------------------------------------
 // By default every instance is a synchronous bank of one: exact per-cycle semantics, but one upload / launch / download round
-// trip (~70 us) per instance and cycle.  With B200M_LV2_BATCH=N the instances of one plugin type and sample rate share ONE bank
+// trip per instance and cycle.  With B200M_LV2_BATCH=N the instances of one plugin type and sample rate share ONE bank
 // of N slots, as the EBUr128 instances do (lv2_ebur128.cu): run() copies its input into its rows of a pinned staging block and
 // publishes the readings of the PREVIOUS cycle (one declared cycle of latency on the control ports; the audio pass-through is
 // not delayed); the instance whose run() completes the cycle launches the bank asynchronously.  Host contract: every instance

@@ -1,7 +1,6 @@
 // peaks.cu — on-device probes of the two ALU ceilings that bound the compute-bound metering kernels.
 //
-// MEASURED_PEAKS.json (driver-written) carries only the HBM copy and bf16 GEMM peaks; the true-peak FIR is
-// bound by fp32 *instruction issue* (unfused FMUL + FADD, the reference's rounding sequence forbids FMA) and the
+// The true-peak FIR is bound by fp32 *instruction issue* (unfused FMUL + FADD, the reference's rounding sequence forbids FMA) and the
 // 1/3-octave bank by the fp64 pipe (SURVEY.md §8d).  bench.py reports each such kernel against these probes as
 // well as against the HBM roofline.  Each probe runs independent dependent-chains of unfused multiply + add.
 #include "common.cuh"
@@ -30,36 +29,13 @@ __global__ void __launch_bounds__ (256) peak_probe_kernel (T* out, int iters, T 
     if (s == (T)123.456) out[0] = s;            // never true: keeps the chains alive
 }
 
-// packed fp32x2 probe (Blackwell FMUL2 / FADD2): independent multiply-only and add-only chains so that ptxas
-// cannot contract them into FFMA2 (it does contract mul.rn.f32x2 + add.rn.f32x2, unlike the scalar forms)
-__global__ void __launch_bounds__ (256) peak_probe_x2_kernel (unsigned long long* out, int iters, unsigned long long k1, unsigned long long k2)
-{
-    unsigned long long a[4], b[4];
-#pragma unroll
-    for (int i = 0; i < 4; ++i) { a[i] = 0x3f8000003f800000ull + threadIdx.x + i; b[i] = 0x3f0000003f000000ull + threadIdx.x * 3 + i; }
-    for (int it = 0; it < iters; ++it) {
-#pragma unroll
-        for (int u = 0; u < 4; ++u) {
-#pragma unroll
-            for (int i = 0; i < 4; ++i) {
-                asm volatile ("mul.rn.f32x2 %0, %0, %1;" : "+l"(a[i]) : "l"(k1));
-                asm volatile ("add.rn.f32x2 %0, %0, %1;" : "+l"(b[i]) : "l"(k2));
-            }
-        }
-    }
-    unsigned long long s = 0;
-#pragma unroll
-    for (int i = 0; i < 4; ++i) s += a[i] ^ b[i];
-    if (s == 0x123456789ull) out[0] = s;
-}
-
 }  // namespace b200m
 
 using namespace b200m;
 
 extern "C" int b200m_peak_probe (int device, int kind, double* gops)
 {
-    if (!gops || kind < 0 || kind > 2) return set_err (B200M_E_INVAL, "bad argument");
+    if (!gops || kind < 0 || kind > 1) return set_err (B200M_E_INVAL, "bad argument");
     if (b200m_device_count () <= 0) return set_err (B200M_E_NODEVICE, "no CUDA device");
     DeviceGuard g (device);
     cudaDeviceProp pr; B200M_CUDA (cudaGetDeviceProperties (&pr, device));
@@ -70,7 +46,6 @@ extern "C" int b200m_peak_probe (int device, int kind, double* gops)
     for (int rep = 0; rep < 4; ++rep) {
         cudaEventRecord (e0);
         if (kind == 0) peak_probe_kernel<float><<<blocks, 256>>> ((float*)d, iters, 0.999f, 1e-3f);
-        else if (kind == 2) peak_probe_x2_kernel<<<blocks, 256>>> ((unsigned long long*)d, iters, 0x3f7fbe773f7fbe77ull, 0x3a83126f3a83126full);
         else peak_probe_kernel<double><<<blocks, 256>>> ((double*)d, iters, 0.999, 1e-3);
         B200M_LAUNCHED (1);
         cudaEventRecord (e1); cudaEventSynchronize (e1);
@@ -80,7 +55,6 @@ extern "C" int b200m_peak_probe (int device, int kind, double* gops)
     cudaEventDestroy (e0); cudaEventDestroy (e1); cudaFree (d);
     B200M_CUDA (cudaGetLastError ());
     // lane-operations (one FMUL or FADD of one lane) per second, in units of 1e9
-    // kind 2 issues 4 x (4 FMUL2 + 4 FADD2) packed instructions per iteration = 64 lane-operations per thread
     *gops = (double)blocks * 256.0 * iters * 4 * 8 * 2 / (best * 1e-3) / 1e9;
     return 0;
 }

@@ -9,7 +9,7 @@
 // Every size the reference GUI offers is provided: fft_bins 64 .. 8192 and 6144 (N = 128 .. 16384 and 12288 = 3 * 4096,
 // gui/phasewheel.c:1108-1116).
 //
-// B200 design: the ring buffers of all instances advance in lock step, so the host tracks the write
+// Design: the ring buffers of all instances advance in lock step, so the host tracks the write
 // offset and the 25 Hz analysis clock; one CTA per instance runs, per channel, an N/2-point complex autosort
 // (Stockham) FFT in shared memory (radix-3 pass when 3 | N, radix-4 passes, one radix-2 pass when needed), splits it
 // into the real spectrum, and writes phase difference / level bins with coalesced stores.  The block append can be

@@ -3,7 +3,7 @@
 // b200m_selftest_log10f evaluates the engine's glibc-exact log10f (common.cuh: log10f_glibc, the function every loudness
 // value, dB port and histogram bin of the engine goes through; reference call sites ebumeter/ebu_r128_proc.cc:116-141,259)
 // on a contiguous range of float BIT PATTERNS, so that a test can sweep all 2^31 non-negative floats against the host
-// libm's log10f (tests/test_log10f_sweep_gpu.py, result log in profiles/).
+// libm's log10f (tests/test_log10f_sweep_gpu.py).
 #include "common.cuh"
 
 namespace b200m {

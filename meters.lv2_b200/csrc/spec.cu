@@ -2,7 +2,7 @@
 //
 // Replaces spectrum_instantiate / spectrum_run (src/spectrumlv2.c:73-121,159-257) over
 // bandpass_setup / bandpass_process / proc_one (src/spectr.c:68-206) for N plugin instances.
-// B200 design: one warp per instance, lane = band (30 of 32 lanes), the six transposed-DF-II
+// Design: one warp per instance, lane = band (30 of 32 lanes), the six transposed-DF-II
 // biquad states and the band's coefficients live in fp64 registers, the (L+R)/2 input (plus the
 // alternating +-1e-12 anti-denormal bias) is converted to double once per frame by the staging
 // lanes and broadcast from shared memory.  The filter design itself runs on the host in complex

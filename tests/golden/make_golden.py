@@ -7,6 +7,9 @@ The reference ships no golden vectors or tests (SURVEY.md §4), so these fixture
 reference itself, run here — are the pin for the oracle port on machines where /root/reference is absent.
 `compute(kind)` is also what tests/test_oracle_port.py::test_golden_vectors replays.
 The phasewheel entries come from the port (FFTW3 is absent: that path has no reference build).
+It also writes ebur128_plugin.npz and goniometer_ref.npz (the reference side of two GPU tests).  lv2_ref.npz, what the
+reference's LV2 plugins write to their ports in the GPU tests, is recorded by those tests on a GPU machine with oracle/_ref built:
+    B200M_LV2_REF_RECORD=$PWD/tests/golden/lv2_ref.npz python -m pytest -m gpu tests/test_lv2_*.py tests/test_dr14_gpu.py
 """
 import os
 import sys
@@ -106,8 +109,39 @@ def compute(kind):
     return out
 
 
+def ebur128_plugin_input():
+    """the input of tests/test_ebu_gpu.py::test_r128_bank_vs_reference_ebur128_plugin: 10 stereo instances, 140 blocks"""
+    x = S.white(2 * 10, 1024 * 140, seed=68)
+    x[3] = 0
+    return x
+
+
+def ebur128_plugin_reads():
+    """the reference's EBUr128 plugin (ebur128_run) on that input: its output ports after every 20th block, [7, 10, 10]"""
+    x = ebur128_plugin_input()
+    o = O.EbuPlugin(10, 48000.0, True)
+    reads = []
+    for b in range(140):
+        o.run(np.ascontiguousarray(x[:, b * 1024:(b + 1) * 1024]), nthreads=8)
+        if b % 20 == 19:
+            reads.append(o.read())
+    return np.stack(reads)
+
+
 if __name__ == "__main__":
     assert O.available("reference"), "build oracle/_ref first (make -C oracle ref)"
     d = compute("reference")
     np.savez_compressed(os.path.join(HERE, "golden_v1.npz"), **d)
     print("wrote golden_v1.npz:", {k: v.shape for k, v in d.items()})
+    np.savez_compressed(os.path.join(HERE, "ebur128_plugin.npz"), reads=ebur128_plugin_reads())
+    print("wrote ebur128_plugin.npz")
+    import test_lv2_gon_gpu as GON
+    feed, rings = GON.reference_feed()
+    state = GON.reference_saved_state()
+    d = dict(layout=np.array([GON._layout(O.load("reference"), "refgon_layout")[k] for k in GON.FIELDS], np.int64),
+             feed=feed, feed_rings=np.array(rings), state_keys=np.array(list(state), dtype=object).astype(bytes),
+             state_types=np.array([v[1] for v in state.values()]), state_flags=np.array([v[2] for v in state.values()], np.int64))
+    for i, v in enumerate(state.values()):
+        d["state_value_%d" % i] = np.frombuffer(v[0], np.uint8)
+    np.savez_compressed(os.path.join(HERE, "goniometer_ref.npz"), **d)
+    print("wrote goniometer_ref.npz")

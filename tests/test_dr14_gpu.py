@@ -10,7 +10,7 @@ import pytest
 import _oracle as O
 import _signals as S
 from test_lv2_ebur128_gpu import ATOM, MTR, obj, position, sequence
-from test_lv2_shim_gpu import descriptors, Plugin, u32
+from test_lv2_shim_gpu import descriptors, Plugin, RefPlugin, u32
 
 pytestmark = pytest.mark.gpu
 OUT_ST = [3, 6, 7, 8, 9, 10, 13, 14, 15, 16, 17, 18]          # DRPortIndex outputs (src/dr14.c:27-43)
@@ -37,8 +37,7 @@ def _connect(p, nch, ctl, ctrl, bufs, outs):
 def _side_by_side(name, nch, nblocks, block, script=None, x=None, rate=48000.0):
     import meters_lv2_b200 as B
     mine, l1 = descriptors(B.LIB_PATH)
-    ref, l2 = descriptors(O.PATHS["reference"])
-    g, r = Plugin(mine[name], rate), Plugin(ref[name], rate)
+    g, r = Plugin(mine[name], rate), RefPlugin(name, rate)
     ports = OUT_ST if nch == 2 else OUT_MONO
     if x is None:
         x = _music(nch, nblocks * block, 3, 0.7)
@@ -110,13 +109,12 @@ def test_dr14_bank_vs_reference_instances(wide, monkeypatch):
         monkeypatch.setenv("B200M_TPK_SLAB", "192"); monkeypatch.setenv("B200M_TPK_SPLIT", "2")   # 8192-frame blocks in 43 slabs: DR window ends fall inside slabs
     elif wide:
         monkeypatch.setenv("B200M_TPK_WIDE", "2"); monkeypatch.setenv("B200M_TPK_SPLIT", "0")
-    ref, l2 = descriptors(O.PATHS["reference"])
     ninst, nblocks, blk = 5, 150, 8192
     gains = [0.9, 0.3, 0.05, 1e-5, 0.6]                          # instance 3 stays below the silence gate
     x = np.concatenate([_music(2, nblocks * blk, 10 + i, gains[i]) for i in range(ninst)], axis=0)
     bank = B.DR14(ninst, 2, 48000.0, True)
     xd = torch.from_numpy(x).cuda()
-    plugs = [Plugin(ref["dr14stereo"], 48000.0) for _ in range(ninst)]
+    plugs = [RefPlugin("dr14stereo", 48000.0) for _ in range(ninst)]
     empty = sequence([])
     outs = [{i: np.zeros(1, np.float32) for i in OUT_ST} for _ in range(ninst)]
     ctrl = [np.ones(1, np.float32), np.zeros(1, np.float32)]

@@ -1,4 +1,6 @@
 """GPU parity: b200m_ebu_* (CUDA) vs the CPU oracle, same seeded inputs, same block sequence."""
+import os
+
 import numpy as np
 import pytest
 
@@ -238,19 +240,23 @@ def test_ebur128_plugin_cycle_with_dbtp():
 
 def test_r128_bank_vs_reference_ebur128_plugin():
     """b200m_r128_* against the reference's EBUr128 PLUGIN driven through its own ebur128_run (oracle/_ref compiles
-    src/meters.cc unmodified): the nine loudness values and the dBTP hold tp_max must be bit-identical."""
+    src/meters.cc unmodified; without that build, its readings stored in tests/golden/ebur128_plugin.npz by
+    tests/golden/make_golden.py): the nine loudness values and the dBTP hold tp_max must be bit-identical."""
     import torch
     import meters_lv2_b200 as B
+    import golden.make_golden as G
     n = 10
-    x = S.white(2 * n, 1024 * 140, seed=68)
-    x[3] = 0
+    x = G.ebur128_plugin_input()
+    if O.available("reference"):
+        refs = G.ebur128_plugin_reads()
+    else:
+        refs = np.load(os.path.join(os.path.dirname(os.path.abspath(__file__)), "golden", "ebur128_plugin.npz"))["reads"]
     xd = torch.from_numpy(x).cuda()
     g = B.EBUr128(n, 48000.0, True); g.control(B.EBUr128.START)
-    o = O.EbuPlugin(n, 48000.0, True)
     for b in range(140):
-        g.run(xd[:, b * 1024:(b + 1) * 1024]); o.run(np.ascontiguousarray(x[:, b * 1024:(b + 1) * 1024]), nthreads=8)
+        g.run(xd[:, b * 1024:(b + 1) * 1024])
         if b % 20 == 19:
-            res, tp = g.results(); ref = o.read()
+            res, tp = g.results(); ref = refs[b // 20]
             for i, name in enumerate(RES):
                 assert np.array_equal(res[name].view(np.uint32), ref[:, i].view(np.uint32)), (b, name)
             assert np.array_equal(tp.view(np.uint32), ref[:, 9].view(np.uint32)), (b, tp, ref[:, 9])

@@ -12,7 +12,7 @@ import pytest
 
 import _oracle as O
 import _signals as S
-from test_lv2_shim_gpu import Feature, _map, descriptors, Plugin
+from test_lv2_shim_gpu import Feature, _map, descriptors, Plugin, RefPlugin
 
 pytestmark = pytest.mark.gpu
 ATOM = b"http://lv2plug.in/ns/ext/atom#"
@@ -55,8 +55,7 @@ def drive(script, nblocks, block=1024, x=None, cap=CAP, rate=48000.0, name="EBUr
     """script: {block index: [events]} fed to the control port of both plugins; asserts byte parity of the notify port"""
     import meters_lv2_b200 as B
     mine, l1 = descriptors(B.LIB_PATH)
-    ref, l2 = descriptors(O.PATHS["reference"])
-    g, r = Plugin(mine[name], rate), Plugin(ref[name], rate)
+    g, r = Plugin(mine[name], rate), RefPlugin(name, rate)
     if x is None:
         x = S.white(2, block * nblocks, seed=17) * np.float32(4.0)
     empty = sequence([])
@@ -157,9 +156,8 @@ def test_batched_mode_one_cycle_latency(monkeypatch):
     monkeypatch.setenv("B200M_LV2_BATCH", "6")
     n, nb, blk = 6, 140, 1024
     mine, l1 = descriptors(B.LIB_PATH)
-    ref, l2 = descriptors(O.PATHS["reference"])
     gs = [Plugin(mine["EBUr128"]) for _ in range(n)]
-    rs = [Plugin(ref["EBUr128"]) for _ in range(n)]
+    rs = [RefPlugin("EBUr128") for _ in range(n)]
     x = S.white(2 * n, blk * nb, seed=61) * np.float32(3.0)
     x[2:4] *= np.float32(0.05)
     keys = [urid(MTR + k) for k in (b"ebu_loudnessM", b"ebu_maxloudnM", b"ebu_loudnessS", b"ebu_maxloudnS", b"ebu_integrated",

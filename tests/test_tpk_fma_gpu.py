@@ -167,7 +167,7 @@ def test_fma_process_max_tensor_core_path(monkeypatch):
     import torch
     import meters_lv2_b200 as B
     monkeypatch.setenv("B200M_TPK_TC", "1")
-    C = 148 * 8 + 21
+    C = torch.cuda.get_device_properties(0).multi_processor_count * 8 + 21
     sizes = [1024, 1000, 512, 260, 4, 2048, 1024]
     total = sum(sizes)
     x = S.white(C, total, seed=11)
