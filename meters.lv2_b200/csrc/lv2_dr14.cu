@@ -7,8 +7,7 @@
 #include <stdio.h>
 #include <stdlib.h>
 #include <string.h>
-#include "common.cuh"
-#include "lv2_abi.cuh"
+#include "lv2_hub.cuh"
 
 namespace {
 
@@ -19,7 +18,7 @@ enum { DR_CONTROL = 0, DR_HOST_TRANSPORT, DR_RESET, DR_BLKCNT, DR_INPUT0, DR_OUT
 
 struct DrPlugin {
     b200m_dr14* bank = nullptr; uint32_t nch = 1; bool dr_mode = false;
-    float* stage = nullptr; size_t stage_cap = 0;
+    PinnedStage stage;
     void* port[DR_NPORTS] = {nullptr};
     LV2_URID atom_Blank = 0, atom_Object = 0, atom_Float = 0, time_Position = 0, time_speed = 0, dr14reset = 0, meteron = 0, meteroff = 0;
     bool transport_rolling = false, reinit_gui = false;
@@ -36,8 +35,7 @@ LV2_Handle dr_instantiate (const LV2_Descriptor* d, double rate, const char*, co
     else if (!strcmp (u, "TPnRMSstereo")) { nch = 2; dr_mode = false; }
     else if (!strcmp (u, "TPnRMSmono")) { nch = 1; dr_mode = false; }
     else return nullptr;
-    const LV2_URID_Map* map = nullptr;
-    for (int i = 0; features && features[i]; ++i) if (!strcmp (features[i]->URI, B200M_LV2_URID_MAP)) map = (const LV2_URID_Map*)features[i]->data;
+    const LV2_URID_Map* map = find_urid_map (features);
     if (!map) { fprintf (stderr, "DR14LV2 error: Host does not support urid:map\n"); return nullptr; }      // :133-136
     DrPlugin* p = new (std::nothrow) DrPlugin;
     if (!p) return nullptr;
@@ -47,7 +45,7 @@ LV2_Handle dr_instantiate (const LV2_Descriptor* d, double rate, const char*, co
     p->time_Position = M (B200M_LV2_TIME "Position"); p->time_speed = M (B200M_LV2_TIME "speed");
     p->dr14reset = M (MTR_URI "dr14reset"); p->meteron = M (MTR_URI "meteron"); p->meteroff = M (MTR_URI "meteroff");
     if (b200m_dr14_create (&p->bank, 0, 1, nch, rate, dr_mode)) { delete p; return nullptr; }
-    if (b200m_host_alloc ((void**)&p->stage, (size_t)nch * B200M_MAX_BLOCK * sizeof (float)) == 0) p->stage_cap = B200M_MAX_BLOCK;   // pinned staging for the largest cycle, allocated here so that run() never allocates (it stays lazy only as a fallback)
+    p->stage.reserve (nch);
     return p;
 }
 
@@ -59,7 +57,7 @@ void dr_run (LV2_Handle h, uint32_t n)
     float* in[2] = {fport (p, DR_INPUT0), fport (p, DR_INPUT1)}; float* out[2] = {fport (p, DR_OUTPUT0), fport (p, DR_OUTPUT1)};
     // audio first (dr14_run ends with this copy, src/dr14.c:477-481): no metering failure may drop it.  TruePeakdsp::process
     // itself is limited to 8192 frames (jmeters/truepeakdsp.cc:43-44), so longer cycles are forwarded but not metered.
-    for (uint32_t c = 0; c < p->nch; ++c) if (out[c] && in[c] && in[c] != out[c]) memcpy (out[c], in[c], sizeof (float) * n);
+    forward_audio (in, out, p->nch, n);
     if (!in[0] || (p->nch == 2 && !in[1]) || n < 1 || n > B200M_MAX_BLOCK) return;
     const bool follow_host_transport = fport (p, DR_HOST_TRANSPORT) && *fport (p, DR_HOST_TRANSPORT) != 0;
     bool reset = false;
@@ -85,16 +83,8 @@ void dr_run (LV2_Handle h, uint32_t n)
     if (fport (p, DR_RESET) && *fport (p, DR_RESET) != 0) reset = true;
     if (reset) b200m_dr14_reset (p->bank, nullptr);           // reset_peaks is idempotent: several triggers in one cycle = one reset
 
-    if (n > p->stage_cap) {
-        if (p->stage) b200m_host_free (p->stage);
-        p->stage = nullptr; p->stage_cap = 0;
-        const size_t cap = n < 1024 ? 1024 : B200M_MAX_BLOCK;
-        if (b200m_host_alloc ((void**)&p->stage, (size_t)p->nch * cap * sizeof (float))) return;
-        p->stage_cap = cap;
-    }
-    for (uint32_t c = 0; c < p->nch; ++c) memcpy (p->stage + (size_t)c * p->stage_cap, in[c], n * sizeof (float));
     b200m_dr14_result r;
-    if (b200m_dr14_run_host (p->bank, p->stage, p->stage_cap, n) || b200m_dr14_results (p->bank, &r, nullptr)) return;
+    if (!p->stage.fill (in, p->nch, n) || b200m_dr14_run_host (p->bank, p->stage.data, p->stage.cap, n) || b200m_dr14_results (p->bank, &r, nullptr)) return;
 
     static const int pv_peak[2] = {DR_V_PEAK0, DR_V_PEAK1}, pm_peak[2] = {DR_M_PEAK0, DR_M_PEAK1}, pv_rms[2] = {DR_V_RMS0, DR_V_RMS1},
                      pm_rms[2] = {DR_M_RMS0, DR_M_RMS1}, p_dr[2] = {DR_DR0, DR_DR1};
@@ -116,7 +106,7 @@ void dr_cleanup (LV2_Handle h)
 {
     DrPlugin* p = (DrPlugin*)h;
     b200m_dr14_destroy (p->bank);
-    if (p->stage) b200m_host_free (p->stage);
+    p->stage.release ();
     delete p;
 }
 

@@ -15,10 +15,7 @@
 #include <stdio.h>
 #include <stdlib.h>
 #include <string.h>
-#include <mutex>
-#include <vector>
-#include "common.cuh"
-#include "lv2_abi.cuh"
+#include "lv2_hub.cuh"
 
 namespace {
 
@@ -41,7 +38,7 @@ struct Urids {
 struct EbuHub;
 struct EbuPlugin {
     b200m_r128* bank = nullptr; EbuHub* hub = nullptr; int slot = -1;       // private bank of one, or slot `slot` of a shared bank
-    float* stage = nullptr; size_t stage_cap = 0;             // pinned [2][cap] planar staging
+    PinnedStage stage;                                         // private bank only
     Urids u; AtomWriter out;
     const void* control = nullptr; void* notify = nullptr;
     float* input[2] = {nullptr, nullptr}; float* output[2] = {nullptr, nullptr};
@@ -57,99 +54,43 @@ struct EbuPlugin {
     int32_t histM[HIST_LEN], histS[HIST_LEN];
 };
 
-// ---- batched mode (opt-in: B200M_LV2_BATCH=<slots>) ---------------------------------------------------------------------
-// Every EBUr128 instance a host loads is by default a synchronous bank of one: exact, but one upload / launch / download
-// round trip per instance and cycle.  With B200M_LV2_BATCH=N the instances of one sample rate share ONE bank of N slots:
-// run() copies its two input buffers into its rows of a pinned staging block and publishes the results of the PREVIOUS
-// cycle (one declared cycle of latency on every notify message; audio pass-through is not delayed); the instance whose
-// run() completes the cycle (all members have submitted) launches the bank asynchronously.  Host contract: every instance
-// runs once per cycle with the same n_samples; if one is skipped, the next double submission launches the cycle anyway.
-// dBTP is processed for every slot as soon as one member enables it; after a disable/enable the oversampler history is
-// current rather than frozen (the reference does not run the meter while disabled).
-struct EbuHub {
-    std::mutex mu;
-    double rate = 0; uint32_t slots = 0, members = 0;
-    b200m_r128* bank = nullptr; float* stage = nullptr;       // pinned [2 * slots][B200M_MAX_BLOCK]
-    std::vector<EbuPlugin*> member; std::vector<uint8_t> submitted; uint32_t n_submitted = 0, cycle_n = 0;
-    bool inflight = false;
+// batched mode (lv2_hub.cuh): the instances of one sample rate share one bank.  dBTP is processed for every slot as soon as one
+// member enables it; after a disable/enable the oversampler history is current rather than frozen (the reference does not run
+// the meter while disabled).
+struct EbuHub : SlotHub {
+    b200m_r128* bank = nullptr;
     std::vector<b200m_ebu_result> res; std::vector<float> tp;  // results of the last completed cycle
-};
-std::mutex g_hub_mu;
-std::vector<EbuHub*> g_hubs;
 
-void hub_fetch (EbuHub* hub)                                  // results of the cycle in flight (waits for it)
-{
-    if (!hub->inflight) return;
-    b200m_r128_results (hub->bank, hub->res.data (), hub->tp.data (), nullptr);
-    hub->inflight = false;
-}
+    EbuHub (const HubKey& k, uint32_t n) : SlotHub (k, n), res (n), tp (n, -INFINITY) {}
+    ~EbuHub () { b200m_r128_destroy (bank); }
 
-void hub_launch (EbuHub* hub)
-{
-    bool any_dbtp = false;
-    for (EbuPlugin* m : hub->member) if (m && m->dbtp_enable) any_dbtp = true;
-    b200m_r128_set_dbtp (hub->bank, any_dbtp);
-    // a forced launch (contract broken, see ebur_run): rows of members that did not submit this cycle still hold their previous
-    // block -- they meter silence rather than the same audio twice
-    if (hub->n_submitted < hub->members)
-        for (uint32_t i = 0; i < hub->slots; ++i)
-            if (hub->member[i] && !hub->submitted[i]) memset (hub->stage + (size_t)2 * i * B200M_MAX_BLOCK, 0, (size_t)2 * B200M_MAX_BLOCK * sizeof (float));
-    if (hub->cycle_n && b200m_r128_run_host (hub->bank, hub->stage, B200M_MAX_BLOCK, hub->cycle_n) == 0) hub->inflight = true;
-    std::fill (hub->submitted.begin (), hub->submitted.end (), 0);
-    hub->n_submitted = 0; hub->cycle_n = 0;
-}
-
-EbuHub* hub_join (EbuPlugin* p, double rate)
-{
-    const char* v = getenv ("B200M_LV2_BATCH");
-    const int want = v ? atoi (v) : 0;
-    if (want < 2) return nullptr;
-    std::lock_guard<std::mutex> lk (g_hub_mu);
-    EbuHub* hub = nullptr;
-    for (EbuHub* h : g_hubs) if (h->rate == rate && h->members < h->slots) hub = h;
-    if (!hub) {
-        hub = new (std::nothrow) EbuHub;
-        if (!hub) return nullptr;
-        hub->rate = rate; hub->slots = (uint32_t)want;
-        if (b200m_r128_create (&hub->bank, 0, hub->slots, (float)rate, 0) ||
-            b200m_host_alloc ((void**)&hub->stage, (size_t)2 * hub->slots * B200M_MAX_BLOCK * sizeof (float))) {
-            b200m_r128_destroy (hub->bank); delete hub; return nullptr;
-        }
-        memset (hub->stage, 0, (size_t)2 * hub->slots * B200M_MAX_BLOCK * sizeof (float));
-        hub->member.assign (hub->slots, nullptr); hub->submitted.assign (hub->slots, 0);
-        hub->res.resize (hub->slots); hub->tp.assign (hub->slots, -INFINITY);
-        b200m_r128_results (hub->bank, hub->res.data (), hub->tp.data (), nullptr);     // the getters' initial values
-        g_hubs.push_back (hub);
-    }
-    std::lock_guard<std::mutex> lh (hub->mu);
-    for (uint32_t i = 0; i < hub->slots; ++i)
-        if (!hub->member[i]) { hub->member[i] = p; p->slot = (int)i; ++hub->members; return hub; }
-    return nullptr;
-}
-
-void hub_leave (EbuPlugin* p)
-{
-    EbuHub* hub = p->hub;
-    std::lock_guard<std::mutex> lk (g_hub_mu);
-    bool empty;
+    static SlotHub* create (const HubKey& k, uint32_t n)
     {
-        std::lock_guard<std::mutex> lh (hub->mu);
-        hub_fetch (hub);
-        if (hub->submitted[p->slot]) { hub->submitted[p->slot] = 0; --hub->n_submitted; }
-        hub->member[p->slot] = nullptr; --hub->members;
+        EbuHub* h = new (std::nothrow) EbuHub (k, n);
+        if (!h) return nullptr;
+        if (b200m_r128_create (&h->bank, 0, n, (float)k.rate, 0)) { delete h; return nullptr; }
+        b200m_r128_results (h->bank, h->res.data (), h->tp.data (), nullptr);     // the getters' initial values
+        return h;
+    }
+    int launch_bank (uint32_t n) override
+    {
+        bool any_dbtp = false;
+        for (void* m : member) if (m && ((EbuPlugin*)m)->dbtp_enable) any_dbtp = true;
+        b200m_r128_set_dbtp (bank, any_dbtp);
+        return b200m_r128_run_host (bank, stage.data, B200M_MAX_BLOCK, n);
+    }
+    void collect () override { b200m_r128_results (bank, res.data (), tp.data (), nullptr); }
+    void vacate (uint32_t slot) override
+    {
         // the slot's next tenant starts from a freshly created instance and silence: filters, 64-fragment ring, loudness values,
         // histograms, true-peak history and hold all cleared; only the bank's shared 50 ms fragment phase is inherited
-        b200m_r128_control (hub->bank, p->slot, B200M_R128_CLEAR, nullptr);
-        hub->tp[p->slot] = -INFINITY;
-        { b200m_ebu_result z; memset (&z, 0, sizeof (z)); z.loudness_M = z.maxloudn_M = z.loudness_S = z.maxloudn_S = z.integrated = z.integ_thr = z.range_min = z.range_max = z.range_thr = -200.0f; hub->res[p->slot] = z; }
-        memset (hub->stage + (size_t)2 * p->slot * B200M_MAX_BLOCK, 0, (size_t)2 * B200M_MAX_BLOCK * sizeof (float));
-        empty = hub->members == 0;
+        b200m_r128_control (bank, (int)slot, B200M_R128_CLEAR, nullptr);
+        tp[slot] = -INFINITY;
+        b200m_ebu_result z; memset (&z, 0, sizeof (z));
+        z.loudness_M = z.maxloudn_M = z.loudness_S = z.maxloudn_S = z.integrated = z.integ_thr = z.range_min = z.range_max = z.range_thr = -200.0f;
+        res[slot] = z;
     }
-    if (empty) {
-        for (size_t i = 0; i < g_hubs.size (); ++i) if (g_hubs[i] == hub) { g_hubs.erase (g_hubs.begin () + i); break; }
-        b200m_r128_destroy (hub->bank); b200m_host_free (hub->stage); delete hub;
-    }
-}
+};
 
 // bank control for this instance (all of a private bank, one slot of a shared one)
 void bank_control (EbuPlugin* p, int cmd)
@@ -256,8 +197,7 @@ void on_config (EbuPlugin* p, const AtomObject& obj, uint32_t n_samples)      //
 LV2_Handle ebur_instantiate (const LV2_Descriptor* d, double rate, const char*, const LV2_Feature* const* features)
 {
     if (strcmp (d->URI, MTR_URI "EBUr128")) return nullptr;
-    const LV2_URID_Map* map = nullptr;
-    for (int i = 0; features && features[i]; ++i) if (!strcmp (features[i]->URI, B200M_LV2_URID_MAP)) map = (const LV2_URID_Map*)features[i]->data;
+    const LV2_URID_Map* map = find_urid_map (features);
     if (!map) { fprintf (stderr, "EBUrLV2 error: Host does not support urid:map\n"); return nullptr; }      // :140-144
     EbuPlugin* p = new (std::nothrow) EbuPlugin;
     if (!p) return nullptr;
@@ -280,9 +220,11 @@ LV2_Handle ebur_instantiate (const LV2_Descriptor* d, double rate, const char*, 
     for (int i = 0; i < RADAR_POINTS; ++i) { p->radarS[i] = -INFINITY; p->radarM[i] = -INFINITY; }
     set_radarspeed (p, 2.0 * 60.0);
     forget_sent_histogram (p);
-    p->hub = hub_join (p, rate);
-    if (!p->hub && b200m_r128_create (&p->bank, 0, 1, (float)rate, 0)) { delete p; return nullptr; }     // ebu->init (2, rate); 2 x TruePeakdsp (:189-196)
-    if (!p->hub && b200m_host_alloc ((void**)&p->stage, (size_t)2 * B200M_MAX_BLOCK * sizeof (float)) == 0) p->stage_cap = B200M_MAX_BLOCK;   // pinned staging for the largest cycle, allocated here so that run() never allocates (it stays lazy only as a fallback)
+    p->hub = (EbuHub*)SlotHub::join (HubKey{HUB_EBUR128, 0, 2, 0, rate}, p, &p->slot, EbuHub::create);
+    if (!p->hub) {
+        if (b200m_r128_create (&p->bank, 0, 1, (float)rate, 0)) { delete p; return nullptr; }     // ebu->init (2, rate); 2 x TruePeakdsp (:189-196)
+        p->stage.reserve (2);
+    }
     return p;
 }
 
@@ -312,8 +254,7 @@ void ebur_run (LV2_Handle h, uint32_t n_samples)
     EbuPlugin* p = (EbuPlugin*)h;
     // audio first, whatever happens to the metering below (the reference ends ebur128_run with this copy, src/ebulv2.cc:484-491;
     // doing it first means an engine failure, a missing notify port or an over-long cycle can never drop audio)
-    for (int c = 0; c < 2; ++c)
-        if (p->output[c] && p->input[c] && p->input[c] != p->output[c]) memcpy (p->output[c], p->input[c], sizeof (float) * n_samples);
+    forward_audio (p->input, p->output, 2, n_samples);
     if (!p->notify || !p->input[0] || !p->input[1]) return;
     const uint32_t capacity = ((const AtomHead*)p->notify)->size;      // host convention: capacity of the output port
     p->out.begin_sequence (p->notify, capacity);
@@ -326,12 +267,10 @@ void ebur_run (LV2_Handle h, uint32_t n_samples)
     }
 
     if (p->hub && n_samples >= 1 && n_samples <= B200M_MAX_BLOCK) {
-        // contract broken (this instance already submitted, or the block size changed): close the open cycle as it is BEFORE this
-        // cycle's control messages reach the bank, so that a RESET / START meant for the new cycle does not land ahead of the old audio
-        EbuHub* hub = p->hub;
-        std::lock_guard<std::mutex> lh (hub->mu);
-        hub_fetch (hub);
-        if (hub->submitted[p->slot] || (hub->cycle_n && hub->cycle_n != n_samples)) { hub_launch (hub); hub_fetch (hub); }
+        // close a cycle this run() breaks BEFORE this cycle's control messages reach the bank, so that a RESET / START meant for
+        // the new cycle does not land ahead of the old audio
+        std::lock_guard<std::mutex> lh (p->hub->mu);
+        p->hub->close_if_broken (p->slot, n_samples);
     }
     if (p->control) {                                          // messages from the GUI / host (:258-331)
         for (AtomEvents ev (p->control); ev.valid (); ev.next ()) {
@@ -353,28 +292,12 @@ void ebur_run (LV2_Handle h, uint32_t n_samples)
     if (p->hub && n_samples >= 1 && n_samples <= B200M_MAX_BLOCK) {
         EbuHub* hub = p->hub;
         std::lock_guard<std::mutex> lh (hub->mu);
-        hub_fetch (hub);                                       // first caller of a cycle: collect the previous cycle (the staging block is free again)
-        if (hub->submitted[p->slot] || (hub->cycle_n && hub->cycle_n != n_samples)) hub_launch (hub), hub_fetch (hub);   // contract broken: close the cycle as it is
-        r = hub->res[p->slot]; tp_max = p->dbtp_enable ? hub->tp[p->slot] : -INFINITY;
-        float* rows = hub->stage + (size_t)2 * p->slot * B200M_MAX_BLOCK;
-        memcpy (rows, p->input[0], n_samples * sizeof (float));
-        memcpy (rows + B200M_MAX_BLOCK, p->input[1], n_samples * sizeof (float));
-        hub->submitted[p->slot] = 1; ++hub->n_submitted; hub->cycle_n = n_samples;
-        if (hub->n_submitted == hub->members) hub_launch (hub);
+        hub->submit (p->slot, p->input, n_samples);
+        r = hub->res[p->slot]; tp_max = p->dbtp_enable ? hub->tp[p->slot] : -INFINITY;      // the previous cycle's
         ran = true;
-    } else if (n_samples >= 1 && n_samples <= B200M_MAX_BLOCK) {
-        if (n_samples > p->stage_cap) {
-            if (p->stage) b200m_host_free (p->stage);
-            p->stage = nullptr; p->stage_cap = 0;
-            const size_t cap = n_samples < 1024 ? 1024 : B200M_MAX_BLOCK;
-            if (b200m_host_alloc ((void**)&p->stage, 2 * cap * sizeof (float)) == 0) p->stage_cap = cap;
-        }
-        if (p->stage_cap) {
-            memcpy (p->stage, p->input[0], n_samples * sizeof (float));
-            memcpy (p->stage + p->stage_cap, p->input[1], n_samples * sizeof (float));
-            b200m_r128_set_dbtp (p->bank, p->dbtp_enable);
-            ran = b200m_r128_run_host (p->bank, p->stage, p->stage_cap, n_samples) == 0 && b200m_r128_results (p->bank, &r, &tp_max, nullptr) == 0;
-        }
+    } else if (n_samples >= 1 && n_samples <= B200M_MAX_BLOCK && p->stage.fill (p->input, 2, n_samples)) {
+        b200m_r128_set_dbtp (p->bank, p->dbtp_enable);
+        ran = b200m_r128_run_host (p->bank, p->stage.data, p->stage.cap, n_samples) == 0 && b200m_r128_results (p->bank, &r, &tp_max, nullptr) == 0;
     }
     if (!ran) return;                                          // run() never fails: leave the (empty) sequence
     const float lm = r.loudness_M, mm = r.maxloudn_M, ls = r.loudness_S, ms = r.maxloudn_S, il = r.integrated, rn = r.range_min, rx = r.range_max;
@@ -446,8 +369,8 @@ void ebur_run (LV2_Handle h, uint32_t n_samples)
 void ebur_cleanup (LV2_Handle h)
 {
     EbuPlugin* p = (EbuPlugin*)h;
-    if (p->hub) hub_leave (p); else b200m_r128_destroy (p->bank);
-    if (p->stage) b200m_host_free (p->stage);
+    if (p->hub) p->hub->leave (p->slot); else b200m_r128_destroy (p->bank);
+    p->stage.release ();
     delete p;
 }
 

@@ -14,8 +14,7 @@
 #include <pthread.h>
 #include <stdlib.h>
 #include <string.h>
-#include "common.cuh"
-#include "lv2_abi.cuh"
+#include "lv2_hub.cuh"
 
 namespace {
 
@@ -46,7 +45,7 @@ struct LV2gmLayout {                                                          //
 struct GonPlugin {
     LV2gmLayout g;                          // MUST stay first: the GUI casts the instance handle to LV2gm*
     b200m_cor* bank = nullptr;
-    float* stage = nullptr; size_t stage_cap = 0;
+    PinnedStage stage;
 };
 
 size_t ring_write_space (const GmRing* rb) { return rb->rp == rb->wp ? rb->len - 1 : ((rb->len + rb->rp - rb->wp) % rb->len) - 1; }   // :52-55
@@ -67,8 +66,7 @@ int ring_write (GmRing* rb, const float* c0, const float* c1, size_t len)     //
 
 LV2_Handle gon_instantiate (const LV2_Descriptor*, double rate, const char*, const LV2_Feature* const* features)
 {
-    LV2_URID_Map* map = nullptr;
-    for (int i = 0; features && features[i]; ++i) if (!strcmp (features[i]->URI, B200M_LV2_URID_MAP)) map = (LV2_URID_Map*)features[i]->data;
+    LV2_URID_Map* map = find_urid_map (features);
     if (!map) { fprintf (stderr, "Goniometer error: Host does not support urid:map\n"); return nullptr; }      // :60-64
     GonPlugin* p = (GonPlugin*)calloc (1, sizeof (GonPlugin));
     if (!p) return nullptr;
@@ -93,7 +91,7 @@ LV2_Handle gon_instantiate (const LV2_Descriptor*, double rate, const char*, con
     if (rb) { rb->c0 = (float*)malloc (rbsize * sizeof (float)); rb->c1 = (float*)malloc (rbsize * sizeof (float)); rb->len = rbsize; rb->rp = 0; rb->wp = 0; }
     if (!rb || !rb->c0 || !rb->c1) { if (rb) { free (rb->c0); free (rb->c1); free (rb); } b200m_cor_destroy (p->bank); free (p); return nullptr; }
     g.rb = rb;
-    if (b200m_host_alloc ((void**)&p->stage, (size_t)2 * B200M_MAX_BLOCK * sizeof (float)) == 0) p->stage_cap = B200M_MAX_BLOCK;   // pinned staging for the largest cycle, allocated here so that run() never allocates (it stays lazy only as a fallback)
+    p->stage.reserve (2);
     return p;
 }
 
@@ -116,21 +114,14 @@ void gon_run (LV2_Handle h, uint32_t n)
 {
     GonPlugin* p = (GonPlugin*)h; LV2gmLayout& g = p->g;
     // audio first: a metering failure never drops it (the reference copies last, :177-182)
-    for (int c = 0; c < 2; ++c) if (g.input[c] && g.output[c] && g.input[c] != g.output[c]) memcpy (g.output[c], g.input[c], sizeof (float) * n);
+    forward_audio (g.input, g.output, 2, n);
     if (!g.input[0] || !g.input[1] || n == 0) return;
     // self->cor->process (in0, in1, n) every cycle, GUI open or not (:147); cycles longer than the engine's block go in pieces
     bool ok = true;
     for (uint32_t off = 0; off < n && ok; off += B200M_MAX_BLOCK) {
         const uint32_t k = n - off < B200M_MAX_BLOCK ? n - off : B200M_MAX_BLOCK;
-        if (k > p->stage_cap) {
-            if (p->stage) b200m_host_free (p->stage);
-            p->stage = nullptr; p->stage_cap = 0;
-            const size_t cap = k < 1024 ? 1024 : B200M_MAX_BLOCK;
-            if (b200m_host_alloc ((void**)&p->stage, 2 * cap * sizeof (float)) == 0) p->stage_cap = cap;
-        }
-        if (!p->stage_cap) { ok = false; break; }
-        memcpy (p->stage, g.input[0] + off, k * sizeof (float)); memcpy (p->stage + p->stage_cap, g.input[1] + off, k * sizeof (float));
-        ok = b200m_cor_process_host (p->bank, p->stage, p->stage_cap, k) == 0;
+        const float* in[2] = {g.input[0] + off, g.input[1] + off};
+        ok = p->stage.fill (in, 2, k) && b200m_cor_process_host (p->bank, p->stage.data, p->stage.cap, k) == 0;
         if (ok && off + k < n) { float tmp; ok = b200m_cor_results (p->bank, &tmp, nullptr) == 0; }      // `stage` is reused by the next piece: wait for its upload
     }
     float cv = 0;
@@ -155,7 +146,7 @@ void gon_cleanup (LV2_Handle h)
     GonPlugin* p = (GonPlugin*)h;
     free (p->g.rb->c0); free (p->g.rb->c1); free (p->g.rb);
     b200m_cor_destroy (p->bank);
-    if (p->stage) b200m_host_free (p->stage);
+    p->stage.release ();
     free (p);
 }
 

@@ -16,10 +16,7 @@
 #include <math.h>
 #include <stdlib.h>
 #include <string.h>
-#include <mutex>
-#include <vector>
-#include "common.cuh"
-#include "lv2_abi.cuh"
+#include "lv2_hub.cuh"
 
 namespace b200m {
 const LV2_Descriptor* lv2_ebur128_descriptor ();        // lv2_ebur128.cu
@@ -32,6 +29,8 @@ const LV2_Descriptor* lv2_goniometer_descriptor ();       // lv2_gon.cu
 
 namespace {
 
+using namespace b200m;
+
 enum Kind { K_COR, K_DBTP, K_KMETER, K_SPEC, K_NEEDLE, K_BBCM6, K_SUR };
 // port enums: src/meters.cc:59-70 (MTR_*), src/spectrumlv2.c:35-44 (SA_*)
 enum { MTR_REFLEVEL = 0, MTR_INPUT0, MTR_OUTPUT0, MTR_LEVEL0, MTR_INPUT1, MTR_OUTPUT1, MTR_LEVEL1, MTR_PEAK0, MTR_PEAK1, MTR_HOLD };
@@ -43,161 +42,84 @@ struct Shim {
     b200m_cor* cor = nullptr; b200m_tpk* tpk = nullptr; b200m_spec* spec = nullptr; b200m_ppm* ppm = nullptr;
     float rlgain = 1.0f;                  // needle meters: reference-level gain (src/meters.cc:243,303-306)
     float* port[68] = {nullptr};          // raw port pointers, indexed as in the reference's enums
-    float* stage = nullptr; size_t stage_cap = 0;   // pinned [chn][cap] planar staging
-    float* stage2 = nullptr; size_t stage2_cap = 0; // surround meters: [8][cap] = the 4 correlation pairs
+    PinnedStage stage;                    // [chn] rows, private banks only
+    PinnedStage stage2;                   // surround meters: [8] rows = the 4 correlation pairs
     float p_refl = -9999, peak_max[2] = {0, 0}, peak_hold = 0;   // src/meters.cc:245-251
-    struct ShimHub* hub = nullptr; int slot = -1;     // batched mode (B200M_LV2_BATCH): a slot of a shared bank instead of a private one
-    int ppm_kind = 0; double rate = 0;
+    struct ShimHub* hub = nullptr; int slot = -1;     // batched mode: a slot of a shared bank instead of a private one
 };
 
-// ---- batched mode (opt-in: B200M_LV2_BATCH=<slots>) ---------------------------------------------------------------------
-// By default every instance is a synchronous bank of one: exact per-cycle semantics, but one upload / launch / download round
-// trip per instance and cycle.  With B200M_LV2_BATCH=N the instances of one plugin type and sample rate share ONE bank
-// of N slots, as the EBUr128 instances do (lv2_ebur128.cu): run() copies its input into its rows of a pinned staging block and
-// publishes the readings of the PREVIOUS cycle (one declared cycle of latency on the control ports; the audio pass-through is
-// not delayed); the instance whose run() completes the cycle launches the bank asynchronously.  Host contract: every instance
-// runs once per cycle with the same n_samples (a skipped instance: the next double submission launches the cycle anyway).
-// Batched: COR, dBTP, K-meters, needle meters (VU/BBC/EBU/DIN/NOR), spectr30.  spectr30's speed / reset ports are bank-wide in
-// the engine: the values of the instance that launches the cycle apply to all.  BBCM6 and the surround meters keep private banks.
-struct ShimHub {
-    std::mutex mu;
-    Kind kind; int ppm_kind = 0; uint32_t chn = 1, tpk_flags = 0; double rate = 0; uint32_t slots = 0, members = 0;
+// batched mode (lv2_hub.cuh): COR, dBTP, K-meters, needle meters (VU/BBC/EBU/DIN/NOR), spectr30.  spectr30's speed / reset ports
+// are bank-wide in the engine: the values of the instance that launches the cycle apply to all.  BBCM6 and the surround meters
+// keep private banks.
+struct ShimHub : SlotHub {
     b200m_cor* cor = nullptr; b200m_tpk* tpk = nullptr; b200m_spec* spec = nullptr; b200m_ppm* ppm = nullptr;
-    float* stage = nullptr;                                    // pinned [slots * chn][B200M_MAX_BLOCK]
-    std::vector<Shim*> member; std::vector<uint8_t> submitted; uint32_t n_submitted = 0, cycle_n = 0; bool inflight = false;
     std::vector<b200m_tpk_result> tpk_res; std::vector<float> f_res;      // results of the last completed cycle
     float spec_speed = 1.0f, spec_reset = -4.0f;
-};
-std::mutex g_shub_mu;
-std::vector<ShimHub*> g_shubs;
 
-void shub_destroy_banks (ShimHub* h) { b200m_cor_destroy (h->cor); b200m_tpk_destroy (h->tpk); b200m_spec_destroy (h->spec); b200m_ppm_destroy (h->ppm); }
+    ShimHub (const HubKey& k, uint32_t n) : SlotHub (k, n) {}
+    ~ShimHub () { b200m_cor_destroy (cor); b200m_tpk_destroy (tpk); b200m_spec_destroy (spec); b200m_ppm_destroy (ppm); }
 
-void shub_fetch (ShimHub* h)                                   // results of the cycle in flight (waits for it)
-{
-    if (!h->inflight) return;
-    switch (h->kind) {
-    case K_COR: b200m_cor_results (h->cor, h->f_res.data (), nullptr); break;
-    case K_DBTP: case K_KMETER: b200m_tpk_results (h->tpk, h->tpk_res.data (), nullptr); break;
-    case K_NEEDLE: b200m_ppm_results (h->ppm, h->f_res.data (), nullptr); break;
-    case K_SPEC: b200m_spec_results (h->spec, h->f_res.data (), nullptr); break;
-    default: break;
+    static SlotHub* create (const HubKey& k, uint32_t n)
+    {
+        ShimHub* h = new (std::nothrow) ShimHub (k, n);
+        if (!h) return nullptr;
+        const uint32_t rows = n * k.chn;
+        int rc = -1;
+        switch (k.family) {
+        case K_COR: rc = b200m_cor_create (&h->cor, 0, n, (int)k.rate, 2e3f, 0.3f); h->f_res.assign (n, 0.0f); break;
+        case K_DBTP: case K_KMETER: rc = b200m_tpk_create (&h->tpk, 0, rows, (float)k.rate, k.tpk_flags); h->tpk_res.assign (rows, b200m_tpk_result{0, 0, 0, 0}); break;
+        case K_NEEDLE: rc = b200m_ppm_create (&h->ppm, 0, rows, (float)k.rate, k.ppm_kind); h->f_res.assign (rows, 0.0f); break;
+        case K_SPEC:
+            rc = b200m_spec_create (&h->spec, 0, n, k.chn, k.rate); h->f_res.assign ((size_t)n * 60, -100.0f);
+            if (!rc) b200m_spec_results (h->spec, h->f_res.data (), nullptr);        // the ports' initial values
+            break;
+        }
+        if (rc) { delete h; return nullptr; }
+        return h;
     }
-    h->inflight = false;
-}
-
-void shub_launch (ShimHub* h)
-{
-    int rc = -1;
-    if (h->cycle_n) {
-        switch (h->kind) {
-        case K_COR: rc = b200m_cor_process_host (h->cor, h->stage, B200M_MAX_BLOCK, h->cycle_n); break;
+    int launch_bank (uint32_t n) override
+    {
+        int rc = -1;
+        switch (key.family) {
+        case K_COR: rc = b200m_cor_process_host (cor, stage.data, B200M_MAX_BLOCK, n); break;
         case K_DBTP: case K_KMETER:
-            rc = b200m_tpk_process_host (h->tpk, h->stage, B200M_MAX_BLOCK, h->cycle_n, B200M_TP_MODE_PROCESS);
-            if (!rc) rc = b200m_tpk_read_device (h->tpk, nullptr);
+            rc = b200m_tpk_process_host (tpk, stage.data, B200M_MAX_BLOCK, n, B200M_TP_MODE_PROCESS);
+            if (!rc) rc = b200m_tpk_read_device (tpk, nullptr);
             break;
         case K_NEEDLE:
-            rc = b200m_ppm_process_host (h->ppm, h->stage, B200M_MAX_BLOCK, h->cycle_n);
-            if (!rc) rc = b200m_ppm_read_device (h->ppm, nullptr);
+            rc = b200m_ppm_process_host (ppm, stage.data, B200M_MAX_BLOCK, n);
+            if (!rc) rc = b200m_ppm_read_device (ppm, nullptr);
             break;
-        case K_SPEC: rc = b200m_spec_process_host (h->spec, h->stage, B200M_MAX_BLOCK, h->cycle_n, h->spec_speed, h->spec_reset); break;
-        default: break;
+        case K_SPEC: rc = b200m_spec_process_host (spec, stage.data, B200M_MAX_BLOCK, n, spec_speed, spec_reset); break;
         }
+        return rc;
     }
-    h->inflight = rc == 0;
-    std::fill (h->submitted.begin (), h->submitted.end (), 0);
-    h->n_submitted = 0; h->cycle_n = 0;
-}
-
-ShimHub* shub_join (Shim* s, uint32_t tpk_flags)
-{
-    const char* v = getenv ("B200M_LV2_BATCH");
-    const int want = v ? atoi (v) : 0;
-    if (want < 2 || s->kind == K_BBCM6 || s->kind == K_SUR) return nullptr;
-    std::lock_guard<std::mutex> lk (g_shub_mu);
-    ShimHub* hub = nullptr;
-    for (ShimHub* h : g_shubs)
-        if (h->kind == s->kind && h->ppm_kind == s->ppm_kind && h->chn == s->chn && h->tpk_flags == tpk_flags && h->rate == s->rate && h->members < h->slots) hub = h;
-    if (!hub) {
-        hub = new (std::nothrow) ShimHub;
-        if (!hub) return nullptr;
-        hub->kind = s->kind; hub->ppm_kind = s->ppm_kind; hub->chn = s->chn; hub->tpk_flags = tpk_flags; hub->rate = s->rate; hub->slots = (uint32_t)want;
-        const uint32_t rows = hub->slots * hub->chn;
-        int rc = -1;
-        switch (s->kind) {
-        case K_COR: rc = b200m_cor_create (&hub->cor, 0, hub->slots, (int)s->rate, 2e3f, 0.3f); hub->f_res.assign (hub->slots, 0.0f); break;
-        case K_DBTP: case K_KMETER: rc = b200m_tpk_create (&hub->tpk, 0, rows, (float)s->rate, tpk_flags); hub->tpk_res.assign (rows, b200m_tpk_result{0, 0, 0, 0}); break;
-        case K_NEEDLE: rc = b200m_ppm_create (&hub->ppm, 0, rows, (float)s->rate, s->ppm_kind); hub->f_res.assign (rows, 0.0f); break;
-        case K_SPEC: rc = b200m_spec_create (&hub->spec, 0, hub->slots, hub->chn, s->rate); hub->f_res.assign ((size_t)hub->slots * 60, -100.0f); break;
-        default: break;
-        }
-        if (!rc) rc = b200m_host_alloc ((void**)&hub->stage, (size_t)rows * B200M_MAX_BLOCK * sizeof (float));
-        if (rc) { shub_destroy_banks (hub); delete hub; return nullptr; }
-        memset (hub->stage, 0, (size_t)rows * B200M_MAX_BLOCK * sizeof (float));
-        hub->member.assign (hub->slots, nullptr); hub->submitted.assign (hub->slots, 0);
-        if (hub->spec) b200m_spec_results (hub->spec, hub->f_res.data (), nullptr);      // the ports' initial values
-        g_shubs.push_back (hub);
-    }
-    std::lock_guard<std::mutex> lh (hub->mu);
-    for (uint32_t i = 0; i < hub->slots; ++i)
-        if (!hub->member[i]) { hub->member[i] = s; s->slot = (int)i; ++hub->members; return hub; }
-    return nullptr;
-}
-
-void shub_leave (Shim* s)
-{
-    ShimHub* hub = s->hub;
-    std::lock_guard<std::mutex> lk (g_shub_mu);
-    bool empty;
+    void collect () override
     {
-        std::lock_guard<std::mutex> lh (hub->mu);
-        shub_fetch (hub);
-        if (hub->submitted[s->slot]) { hub->submitted[s->slot] = 0; --hub->n_submitted; }
-        hub->member[s->slot] = nullptr; --hub->members;
-        memset (hub->stage + (size_t)s->slot * hub->chn * B200M_MAX_BLOCK, 0, (size_t)hub->chn * B200M_MAX_BLOCK * sizeof (float));   // the slot idles on silence
-        if (hub->tpk) for (uint32_t c = 0; c < hub->chn; ++c) b200m_tpk_reset (hub->tpk, (int32_t)(s->slot * hub->chn + c), nullptr);
-        empty = hub->members == 0;
+        switch (key.family) {
+        case K_COR: b200m_cor_results (cor, f_res.data (), nullptr); break;
+        case K_DBTP: case K_KMETER: b200m_tpk_results (tpk, tpk_res.data (), nullptr); break;
+        case K_NEEDLE: b200m_ppm_results (ppm, f_res.data (), nullptr); break;
+        case K_SPEC: b200m_spec_results (spec, f_res.data (), nullptr); break;
+        }
     }
-    if (empty) {
-        for (size_t i = 0; i < g_shubs.size (); ++i) if (g_shubs[i] == hub) { g_shubs.erase (g_shubs.begin () + i); break; }
-        shub_destroy_banks (hub); b200m_host_free (hub->stage); delete hub;
+    void vacate (uint32_t slot) override
+    {
+        if (tpk) for (uint32_t c = 0; c < key.chn; ++c) b200m_tpk_reset (tpk, (int32_t)(slot * key.chn + c), nullptr);
     }
-}
+};
 
-// one cycle of a batched instance: collect the previous cycle's results of this slot, hand in this cycle's audio, launch when complete.
-// Returns false when there is nothing to publish.
-bool shub_cycle (Shim* s, const float* const* in, uint32_t n, b200m_tpk_result* tr, float* fr, uint32_t nf)
+// one cycle of a batched instance: collect the previous cycle's results of this slot, hand in this cycle's audio, launch when complete
+void shub_cycle (Shim* s, const float* const* in, uint32_t n, b200m_tpk_result* tr, float* fr, uint32_t nf)
 {
     ShimHub* hub = s->hub;
+    const uint32_t chn = hub->key.chn;
     std::lock_guard<std::mutex> lh (hub->mu);
-    shub_fetch (hub);                                          // first caller of a cycle collects the previous one (the staging block is free again)
-    if (hub->submitted[s->slot] || (hub->cycle_n && hub->cycle_n != n)) { shub_launch (hub); shub_fetch (hub); }     // contract broken: close the cycle as it is
-    if (tr) for (uint32_t c = 0; c < hub->chn; ++c) tr[c] = hub->tpk_res[(size_t)s->slot * hub->chn + c];
+    hub->close_if_broken (s->slot, n);
+    if (tr) for (uint32_t c = 0; c < chn; ++c) tr[c] = hub->tpk_res[(size_t)s->slot * chn + c];
     if (fr) for (uint32_t k = 0; k < nf; ++k) fr[k] = hub->f_res[(size_t)s->slot * nf + k];
-    for (uint32_t c = 0; c < hub->chn; ++c) memcpy (hub->stage + ((size_t)s->slot * hub->chn + c) * B200M_MAX_BLOCK, in[c], n * sizeof (float));
-    hub->submitted[s->slot] = 1; ++hub->n_submitted; hub->cycle_n = n;
-    if (s->kind == K_SPEC) { hub->spec_speed = *s->port[SA_SPEED]; hub->spec_reset = *s->port[SA_RESET]; }
-    if (hub->n_submitted == hub->members) shub_launch (hub);
-    return true;
-}
-
-
-bool stage_in (Shim* s, const float* const* in, uint32_t n)
-{
-    if (n > s->stage_cap) {
-        if (s->stage) b200m_host_free (s->stage);
-        s->stage = nullptr; s->stage_cap = 0;
-        const size_t cap = n < 1024 ? 1024 : B200M_MAX_BLOCK;
-        if (b200m_host_alloc ((void**)&s->stage, (size_t)s->chn * cap * sizeof (float))) return false;
-        s->stage_cap = cap;
-    }
-    for (uint32_t c = 0; c < s->chn; ++c) memcpy (s->stage + (size_t)c * s->stage_cap, in[c], n * sizeof (float));
-    return true;
-}
-
-void pass_through (float* const* in, float* const* out, uint32_t chn, uint32_t n)
-{
-    for (uint32_t c = 0; c < chn; ++c) if (in[c] != out[c] && in[c] && out[c]) memcpy (out[c], in[c], sizeof (float) * n);
+    if (s->kind == K_SPEC) { hub->spec_speed = *s->port[SA_SPEED]; hub->spec_reset = *s->port[SA_RESET]; }   // before a launch by this submit
+    hub->submit (s->slot, in, n);
 }
 
 LV2_Handle shim_instantiate (const LV2_Descriptor* d, double rate, const char*, const LV2_Feature* const*)
@@ -205,27 +127,28 @@ LV2_Handle shim_instantiate (const LV2_Descriptor* d, double rate, const char*, 
     Shim* s = new (std::nothrow) Shim;
     if (!s) return nullptr;
     const char* u = d->URI + strlen (MTR_URI);
-    s->rate = rate;
-    uint32_t tpk_flags = 0; bool known = true;
+    uint32_t tpk_flags = 0; int ppm_kind = 0; bool known = true;
     if (!strcmp (u, "COR")) { s->kind = K_COR; s->chn = 2; }                                                   // :204-207
     else if (!strncmp (u, "dBTP", 4)) { s->kind = K_DBTP; s->chn = strstr (u, "stereo") ? 2 : 1; tpk_flags = B200M_TPK_TRUEPEAK; }
     else if (u[0] == 'K') { s->kind = K_KMETER; s->chn = strstr (u, "stereo") ? 2 : 1; tpk_flags = B200M_TPK_KMETER; }
-    else if (!strcmp (u, "BBCM6")) { s->kind = K_BBCM6; s->chn = 2; s->ppm_kind = B200M_PPM_MS; }               // :208-214
+    else if (!strcmp (u, "BBCM6")) { s->kind = K_BBCM6; s->chn = 2; }               // :208-214
     else if (!strncmp (u, "VU", 2) || !strncmp (u, "BBC", 3) || !strncmp (u, "EBU", 3) || !strncmp (u, "DIN", 3) || !strncmp (u, "NOR", 3)) {
         // MTRDEF (src/meters.cc:172-190,215-219): VU -> Vumeterdsp, BBC/EBU -> Iec2ppmdsp, DIN/NOR -> Iec1ppmdsp
         s->kind = K_NEEDLE; s->chn = strstr (u, "stereo") ? 2 : 1;
-        s->ppm_kind = !strncmp (u, "VU", 2) ? B200M_PPM_VU : (!strncmp (u, "DIN", 3) || !strncmp (u, "NOR", 3)) ? B200M_PPM_IEC1 : B200M_PPM_IEC2;
+        ppm_kind = !strncmp (u, "VU", 2) ? B200M_PPM_VU : (!strncmp (u, "DIN", 3) || !strncmp (u, "NOR", 3)) ? B200M_PPM_IEC1 : B200M_PPM_IEC2;
     }
     else if (!strncmp (u, "surround", 8) && u[8] >= '3' && u[8] <= '8' && !u[9]) { s->kind = K_SUR; s->chn = (uint32_t)(u[8] - '0'); tpk_flags = B200M_TPK_KMETER; }   // src/surmeter.c:24-70
     else if (!strncmp (u, "spectr30", 8)) { s->kind = K_SPEC; s->chn = strstr (u, "stereo") ? 2 : 1; }
     else known = false;
     int rc = known ? 0 : -1;
-    if (known && !(s->hub = shub_join (s, tpk_flags))) {      // a private bank of one instance unless B200M_LV2_BATCH puts it into a shared one
+    if (known && s->kind != K_BBCM6 && s->kind != K_SUR)
+        s->hub = (ShimHub*)SlotHub::join (HubKey{s->kind, ppm_kind, s->chn, tpk_flags, rate}, s, &s->slot, ShimHub::create);
+    if (known && !s->hub) {                                    // a private bank of one instance unless batched mode puts it into a shared one
         switch (s->kind) {
         case K_COR: rc = b200m_cor_create (&s->cor, 0, 1, (int)rate, 2e3f, 0.3f); break;
         case K_DBTP: case K_KMETER: rc = b200m_tpk_create (&s->tpk, 0, s->chn, (float)rate, tpk_flags); break;
         case K_BBCM6: rc = b200m_ppm_create (&s->ppm, 0, 1, (float)rate, B200M_PPM_MS); break;
-        case K_NEEDLE: rc = b200m_ppm_create (&s->ppm, 0, s->chn, (float)rate, s->ppm_kind); break;
+        case K_NEEDLE: rc = b200m_ppm_create (&s->ppm, 0, s->chn, (float)rate, ppm_kind); break;
         case K_SUR:
             rc = b200m_tpk_create (&s->tpk, 0, s->chn, (float)rate, B200M_TPK_KMETER);
             if (!rc) rc = b200m_cor_create (&s->cor, 0, 4, (int)rate, 2e3f, 0.3f);
@@ -233,12 +156,10 @@ LV2_Handle shim_instantiate (const LV2_Descriptor* d, double rate, const char*, 
             break;
         case K_SPEC: rc = b200m_spec_create (&s->spec, 0, 1, s->chn, rate); break;
         }
+        if (!rc) s->stage.reserve (s->chn);
+        if (!rc && s->kind == K_SUR) s->stage2.reserve (8);
     }
     if (rc) { delete s; return nullptr; }                  // instantiate() -> NULL, as the reference does on failure
-    if (!s->hub) {   // pinned staging for the largest cycle, allocated here so that run() never allocates (it stays lazy only as a fallback)
-        if (b200m_host_alloc ((void**)&s->stage, (size_t)s->chn * B200M_MAX_BLOCK * sizeof (float)) == 0) s->stage_cap = B200M_MAX_BLOCK;
-        if (s->kind == K_SUR && b200m_host_alloc ((void**)&s->stage2, (size_t)8 * B200M_MAX_BLOCK * sizeof (float)) == 0) s->stage2_cap = B200M_MAX_BLOCK;
-    }
     return s;
 }
 
@@ -251,10 +172,9 @@ void shim_connect (LV2_Handle h, uint32_t port, void* data)
 void shim_cleanup (LV2_Handle h)
 {
     Shim* s = (Shim*)h;
-    if (s->hub) shub_leave (s);
+    if (s->hub) s->hub->leave (s->slot);
     b200m_cor_destroy (s->cor); b200m_tpk_destroy (s->tpk); b200m_spec_destroy (s->spec); b200m_ppm_destroy (s->ppm);
-    if (s->stage) b200m_host_free (s->stage);
-    if (s->stage2) b200m_host_free (s->stage2);
+    s->stage.release (); s->stage2.release ();
     delete s;
 }
 
@@ -264,9 +184,9 @@ void run_cor (Shim* s, uint32_t off, uint32_t n)
 {
     float* in[2] = {s->port[MTR_INPUT0] + off, s->port[MTR_INPUT1] + off};
     float v = 0;
-    if (s->hub) { if (shub_cycle (s, in, n, nullptr, &v, 1)) *s->port[MTR_LEVEL0] = v; return; }
-    if (!stage_in (s, in, n)) return;
-    if (b200m_cor_process_host (s->cor, s->stage, s->stage_cap, n) == 0 && b200m_cor_results (s->cor, &v, nullptr) == 0)
+    if (s->hub) { shub_cycle (s, in, n, nullptr, &v, 1); *s->port[MTR_LEVEL0] = v; return; }
+    if (!s->stage.fill (in, s->chn, n)) return;
+    if (b200m_cor_process_host (s->cor, s->stage.data, s->stage.cap, n) == 0 && b200m_cor_results (s->cor, &v, nullptr) == 0)
         *s->port[MTR_LEVEL0] = v;                          // *level[0] = cor->read() (:516-517)
 }
 
@@ -296,11 +216,8 @@ void run_tpk (Shim* s, uint32_t off, uint32_t n)
     // a mono meter re-uses the second channel's port slots for its peak values: only chn audio pointers exist
     float* in[2] = {s->port[MTR_INPUT0] + off, s->chn == 2 ? s->port[MTR_INPUT1] + off : nullptr};
     b200m_tpk_result r[2];
-    if (s->hub) { if (!shub_cycle (s, in, n, r, nullptr, 0)) return; }
-    else {
-        if (!stage_in (s, in, n)) return;
-        if (b200m_tpk_process_host (s->tpk, s->stage, s->stage_cap, n, B200M_TP_MODE_PROCESS)) return;
-    }
+    if (s->hub) shub_cycle (s, in, n, r, nullptr, 0);
+    else if (!s->stage.fill (in, s->chn, n) || b200m_tpk_process_host (s->tpk, s->stage.data, s->stage.cap, n, B200M_TP_MODE_PROCESS)) return;
     if (reinit) {                                          // force parameter change (:381-389, :476-489); no read() in such a cycle
         b200m_tpk_result sync[2];
         if (!s->hub) b200m_tpk_results (s->tpk, sync, nullptr);   // stream sync only: run() must not return while the upload of `stage` is in flight
@@ -347,11 +264,9 @@ void run_needle (Shim* s, uint32_t off, uint32_t n)
         b200m_ppm_set_gain (s->ppm, -6, s20 ? +14 : -6);
     }
     float v[2] = {0, 0};
-    if (s->hub) { if (!shub_cycle (s, in, n, nullptr, v, s->chn)) return; }
-    else {
-        if (!stage_in (s, in, n)) return;
-        if (b200m_ppm_process_host (s->ppm, s->stage, s->stage_cap, n) || b200m_ppm_read_device (s->ppm, nullptr) || b200m_ppm_results (s->ppm, v, nullptr)) return;
-    }
+    if (s->hub) shub_cycle (s, in, n, nullptr, v, s->chn);
+    else if (!s->stage.fill (in, s->chn, n) || b200m_ppm_process_host (s->ppm, s->stage.data, s->stage.cap, n) || b200m_ppm_read_device (s->ppm, nullptr) ||
+             b200m_ppm_results (s->ppm, v, nullptr)) return;
     *s->port[MTR_LEVEL0] = s->rlgain * v[0];
     if (s->chn == 2) *s->port[MTR_LEVEL1] = s->rlgain * v[1];
 }
@@ -360,12 +275,9 @@ void run_spec (Shim* s, uint32_t off, uint32_t n)
 {
     float* in[2] = {s->port[SA_INPUT0] + off, s->chn == 2 ? s->port[SA_INPUT1] + off : nullptr};
     float ports[60];
-    if (s->hub) { if (!shub_cycle (s, in, n, nullptr, ports, 60)) return; }
-    else {
-        if (!stage_in (s, in, n)) return;
-        if (b200m_spec_process_host (s->spec, s->stage, s->stage_cap, n, *s->port[SA_SPEED], *s->port[SA_RESET])) return;
-        if (b200m_spec_results (s->spec, ports, nullptr)) return;
-    }
+    if (s->hub) shub_cycle (s, in, n, nullptr, ports, 60);
+    else if (!s->stage.fill (in, s->chn, n) || b200m_spec_process_host (s->spec, s->stage.data, s->stage.cap, n, *s->port[SA_SPEED], *s->port[SA_RESET]) ||
+             b200m_spec_results (s->spec, ports, nullptr)) return;
     for (int i = 0; i < 30; ++i) {
         if (s->port[i]) *s->port[i] = ports[i];
         if (s->port[30 + i]) *s->port[30 + i] = ports[30 + i] <= -500.0f ? -500.0f - (rand () & 0xffff) : ports[30 + i];   // :243-246
@@ -377,29 +289,21 @@ void run_sur (Shim* s, uint32_t off, uint32_t n)
 {
     float* in[8];
     for (uint32_t c = 0; c < s->chn; ++c) { in[c] = s->port[13 + 4 * c]; if (!in[c]) return; in[c] += off; }
-    if (n > s->stage2_cap) {
-        if (s->stage2) b200m_host_free (s->stage2);
-        s->stage2 = nullptr; s->stage2_cap = 0;
-        const size_t cap = n < 1024 ? 1024 : B200M_MAX_BLOCK;
-        if (b200m_host_alloc ((void**)&s->stage2, 8 * cap * sizeof (float))) return;
-        s->stage2_cap = cap;
-    }
     const uint32_t cors = s->chn > 3 ? 4 : 3;
-    for (uint32_t c = 0; c < 4; ++c) {
-        float* a = s->stage2 + (size_t)(2 * c) * s->stage2_cap; float* b = a + s->stage2_cap;
-        if (c < cors && s->port[1 + 3 * c] && s->port[2 + 3 * c]) {
-            uint32_t in_a = (uint32_t)rintf (*s->port[1 + 3 * c]), in_b = (uint32_t)rintf (*s->port[2 + 3 * c]);
-            if (in_a >= s->chn) in_a = s->chn - 1;
-            if (in_b >= s->chn) in_b = s->chn - 1;
-            memcpy (a, in[in_a], n * sizeof (float)); memcpy (b, in[in_b], n * sizeof (float));
-        } else { memset (a, 0, n * sizeof (float)); memset (b, 0, n * sizeof (float)); }     // cor4[3] idles on a 3-channel meter
+    const float* pair[8] = {nullptr};                      // NULL rows stage silence: cor4[3] idles on a 3-channel meter
+    for (uint32_t c = 0; c < cors; ++c) {
+        if (!s->port[1 + 3 * c] || !s->port[2 + 3 * c]) continue;
+        uint32_t in_a = (uint32_t)rintf (*s->port[1 + 3 * c]), in_b = (uint32_t)rintf (*s->port[2 + 3 * c]);
+        if (in_a >= s->chn) in_a = s->chn - 1;
+        if (in_b >= s->chn) in_b = s->chn - 1;
+        pair[2 * c] = in[in_a]; pair[2 * c + 1] = in[in_b];
     }
     float cv[4] = {0, 0, 0, 0};
-    if (b200m_cor_process_host (s->cor, s->stage2, s->stage2_cap, n) || b200m_cor_results (s->cor, cv, nullptr)) return;
+    if (!s->stage2.fill (pair, 8, n) || b200m_cor_process_host (s->cor, s->stage2.data, s->stage2.cap, n) || b200m_cor_results (s->cor, cv, nullptr)) return;
     for (uint32_t c = 0; c < cors; ++c) if (s->port[3 + 3 * c]) *s->port[3 + 3 * c] = cv[c];
-    if (!stage_in (s, in, n)) return;
+    if (!s->stage.fill (in, s->chn, n)) return;
     b200m_tpk_result r[8];
-    if (b200m_tpk_process_host (s->tpk, s->stage, s->stage_cap, n, B200M_TP_MODE_PROCESS) || b200m_tpk_read_device (s->tpk, nullptr) ||
+    if (b200m_tpk_process_host (s->tpk, s->stage.data, s->stage.cap, n, B200M_TP_MODE_PROCESS) || b200m_tpk_read_device (s->tpk, nullptr) ||
         b200m_tpk_results (s->tpk, r, nullptr)) return;
     for (uint32_t c = 0; c < s->chn; ++c) {
         if (s->port[15 + 4 * c]) *s->port[15 + 4 * c] = r[c].km_rms;         // Kmeterdsp::read (m, p): *level = m, *peak = p
@@ -419,7 +323,7 @@ void shim_run (LV2_Handle h, uint32_t n)
         if (s->kind == K_SUR) for (uint32_t c = 0; c < s->chn; ++c) { in[c] = s->port[13 + 4 * c]; out[c] = s->port[14 + 4 * c]; }
         else if (s->kind == K_SPEC) { in[0] = s->port[SA_INPUT0]; out[0] = s->port[SA_OUTPUT0]; if (s->chn == 2) { in[1] = s->port[SA_INPUT1]; out[1] = s->port[SA_OUTPUT1]; } }
         else { in[0] = s->port[MTR_INPUT0]; out[0] = s->port[MTR_OUTPUT0]; if (s->chn == 2) { in[1] = s->port[MTR_INPUT1]; out[1] = s->port[MTR_OUTPUT1]; } }
-        pass_through (in, out, s->chn, n);
+        forward_audio (in, out, s->chn, n);
         for (uint32_t c = 0; c < s->chn; ++c) if (!in[c]) return;          // unconnected input: nothing to meter
     }
     // the engine's block limit is 8192 frames (B200M_MAX_BLOCK = the hosts' MAXPERIOD); the reference's needle / COR / K-meter /

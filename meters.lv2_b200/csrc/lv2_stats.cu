@@ -7,8 +7,7 @@
 #include <stdio.h>
 #include <stdlib.h>
 #include <string.h>
-#include "common.cuh"
-#include "lv2_abi.cuh"
+#include "lv2_hub.cuh"
 
 namespace {
 
@@ -22,7 +21,7 @@ constexpr int BIM_LAST = 584, DIST_BIN = 361;                  // src/uris.h:49,
 struct StatsPlugin {
     bool is_bim = false;
     b200m_bim* bim = nullptr; b200m_sdh* sdh = nullptr;
-    float* stage = nullptr; size_t stage_cap = 0;
+    PinnedStage stage;
     AtomWriter out;
     const void* control = nullptr; void* notify = nullptr;
     float* input[2] = {nullptr, nullptr}; float* output[2] = {nullptr, nullptr};
@@ -86,8 +85,7 @@ LV2_Handle stats_instantiate (const LV2_Descriptor* d, double rate, const char*,
 {
     const bool is_bim = !strcmp (d->URI, MTR_URI "bitmeter");
     if (!is_bim && strcmp (d->URI, MTR_URI "SigDistHist")) return nullptr;
-    const LV2_URID_Map* map = nullptr;
-    for (int i = 0; features && features[i]; ++i) if (!strcmp (features[i]->URI, B200M_LV2_URID_MAP)) map = (const LV2_URID_Map*)features[i]->data;
+    const LV2_URID_Map* map = find_urid_map (features);
     if (!map) { fprintf (stderr, "%s error: Host does not support urid:map\n", is_bim ? "Bitmeter" : "SigDistHist"); return nullptr; }
     StatsPlugin* p = new (std::nothrow) StatsPlugin;
     if (!p) return nullptr;
@@ -113,7 +111,7 @@ LV2_Handle stats_instantiate (const LV2_Descriptor* d, double rate, const char*,
     if (is_bim) { p->integrating = true; rc = b200m_bim_create (&p->bim, 0, 1, rate); }       // src/bitmeter.c:150-151
     else rc = b200m_sdh_create (&p->sdh, 0, 1, rate);
     if (rc) { delete p; return nullptr; }
-    if (b200m_host_alloc ((void**)&p->stage, (size_t)B200M_MAX_BLOCK * sizeof (float)) == 0) p->stage_cap = B200M_MAX_BLOCK;   // pinned staging for the largest cycle, allocated here so that run() never allocates (it stays lazy only as a fallback)
+    p->stage.reserve (1);
     return p;
 }
 
@@ -133,16 +131,7 @@ void stats_connect (LV2_Handle h, uint32_t port, void* data)
 
 bool stage_block (StatsPlugin* p, uint32_t n)
 {
-    if (n < 1 || n > B200M_MAX_BLOCK) return false;
-    if (n > p->stage_cap) {
-        if (p->stage) b200m_host_free (p->stage);
-        p->stage = nullptr; p->stage_cap = 0;
-        const size_t cap = n < 1024 ? 1024 : B200M_MAX_BLOCK;
-        if (b200m_host_alloc ((void**)&p->stage, cap * sizeof (float))) return false;
-        p->stage_cap = cap;
-    }
-    memcpy (p->stage, p->input[0], n * sizeof (float));
-    return true;
+    return n >= 1 && n <= B200M_MAX_BLOCK && p->stage.fill (p->input, 1, n);
 }
 
 void bim_run (StatsPlugin* p, uint32_t n)
@@ -170,7 +159,7 @@ void bim_run (StatsPlugin* p, uint32_t n)
             }
         }
     }
-    if (!stage_block (p, n) || b200m_bim_run_host (p->bim, p->stage, p->stage_cap, n)) return;
+    if (!stage_block (p, n) || b200m_bim_run_host (p->bim, p->stage.data, p->stage.cap, n)) return;
     // run() is synchronous for the host: the staging block is rewritten next cycle, so the asynchronous upload and the scan
     // must have finished before we return even when nothing is published (a results call with no outputs = stream sync)
     if (b200m_bim_results (p->bim, 0, nullptr, nullptr, nullptr, nullptr, nullptr)) return;
@@ -238,7 +227,7 @@ void sdh_run (StatsPlugin* p, uint32_t n)
             }
         }
     }
-    if (!stage_block (p, n) || b200m_sdh_run_host (p->sdh, p->stage, p->stage_cap, n)) return;
+    if (!stage_block (p, n) || b200m_sdh_run_host (p->sdh, p->stage.data, p->stage.cap, n)) return;
     if (b200m_sdh_results (p->sdh, 0, nullptr, nullptr, nullptr, nullptr, nullptr)) return;      // synchronous run(), see bim_run
     const double lim = p->rate / 25.f;                         // const int fps_limit = MAX (rate / 25.f, n_samples)  (:329)
     const int fps_limit = (int)(lim > n ? lim : (double)n);
@@ -268,7 +257,7 @@ void stats_run (LV2_Handle h, uint32_t n)
 {
     StatsPlugin* p = (StatsPlugin*)h;
     // audio first (src/bitmeter.c:330-334, src/sigdistlv2.c:372-376 end with this copy): a metering failure never drops it
-    if (p->output[0] && p->input[0] && p->input[0] != p->output[0]) memcpy (p->output[0], p->input[0], sizeof (float) * n);
+    forward_audio (p->input, p->output, 1, n);
     if (!p->notify || !p->input[0]) return;
     p->out.begin_sequence (p->notify, ((const AtomHead*)p->notify)->size);
     if (p->is_bim) bim_run (p, n); else sdh_run (p, n);
@@ -278,7 +267,7 @@ void stats_cleanup (LV2_Handle h)
 {
     StatsPlugin* p = (StatsPlugin*)h;
     b200m_bim_destroy (p->bim); b200m_sdh_destroy (p->sdh);
-    if (p->stage) b200m_host_free (p->stage);
+    p->stage.release ();
     delete p;
 }
 

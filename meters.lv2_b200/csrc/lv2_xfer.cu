@@ -6,8 +6,7 @@
 #include <stdio.h>
 #include <stdlib.h>
 #include <string.h>
-#include "common.cuh"
-#include "lv2_abi.cuh"
+#include "lv2_hub.cuh"
 
 namespace {
 
@@ -17,7 +16,7 @@ enum { SPR_CONTROL = 0, SPR_NOTIFY, SPR_INPUT0, SPR_OUTPUT0, SPR_INPUT1, SPR_OUT
 
 struct XferPlugin {
     b200m_cor* cor = nullptr;                                  // phasewheel only (:93-95)
-    float* stage = nullptr; size_t stage_cap = 0;
+    PinnedStage stage;
     AtomWriter out;
     const void* control = nullptr; void* notify = nullptr;
     float* input[2] = {nullptr, nullptr}; float* output[2] = {nullptr, nullptr}; float* p_phase = nullptr;
@@ -27,8 +26,7 @@ struct XferPlugin {
 
 LV2_Handle xfer_instantiate (const LV2_Descriptor* d, double rate, const char*, const LV2_Feature* const* features)
 {
-    const LV2_URID_Map* map = nullptr;
-    for (int i = 0; features && features[i]; ++i) if (!strcmp (features[i]->URI, B200M_LV2_URID_MAP)) map = (const LV2_URID_Map*)features[i]->data;
+    const LV2_URID_Map* map = find_urid_map (features);
     if (!map) { fprintf (stderr, "meters.lv2 error: Host does not support urid:map\n"); return nullptr; }
     const bool wheel = !strcmp (d->URI, MTR_URI "phasewheel");
     if (!wheel && strcmp (d->URI, MTR_URI "stereoscope")) return nullptr;
@@ -42,7 +40,7 @@ LV2_Handle xfer_instantiate (const LV2_Descriptor* d, double rate, const char*, 
     p->out.t_float = M (B200M_LV2_ATOM "Float"); p->out.t_int = M (B200M_LV2_ATOM "Int");
     p->rawstereo = M (MTR_URI "rawstereo"); p->audioleft = M (MTR_URI "audioleft"); p->audioright = M (MTR_URI "audioright");
     p->samplerate = M (MTR_URI "samplerate"); p->ui_on = M (MTR_URI "ui_on"); p->ui_off = M (MTR_URI "ui_off"); p->ui_state = M (MTR_URI "ui_state");
-    if (p->cor && b200m_host_alloc ((void**)&p->stage, (size_t)2 * B200M_MAX_BLOCK * sizeof (float)) == 0) p->stage_cap = B200M_MAX_BLOCK;   // pinned staging for the largest cycle, allocated here so that run() never allocates (it stays lazy only as a fallback)
+    if (p->cor) p->stage.reserve (2);
     return p;
 }
 
@@ -66,7 +64,7 @@ void xfer_run (LV2_Handle h, uint32_t n)
     XferPlugin* p = (XferPlugin*)h;
     // audio first: the reference forwards it at the end of xfer_run (src/xfer.c:262-275) and therefore DROPS it in a cycle whose
     // atom buffer is too small (:192-205); here a metering / messaging problem never costs audio
-    for (int c = 0; c < 2; ++c) if (p->output[c] && p->input[c] && p->input[c] != p->output[c]) memcpy (p->output[c], p->input[c], sizeof (float) * n);
+    forward_audio (p->input, p->output, 2, n);
     if (!p->notify || !p->input[0] || !p->input[1]) return;
     const size_t size = (sizeof (float) * n + 64) * 2;
     const uint32_t capacity = ((const AtomHead*)p->notify)->size;
@@ -90,18 +88,9 @@ void xfer_run (LV2_Handle h, uint32_t n)
             else if (obj.otype () == p->ui_off) p->ui_active = false;
         }
     }
-    if (p->cor && n >= 1 && n <= B200M_MAX_BLOCK) {            // stcor->process; *p_phase = stcor->read () (:248-251)
-        if (n > p->stage_cap) {
-            if (p->stage) b200m_host_free (p->stage);
-            p->stage = nullptr; p->stage_cap = 0;
-            const size_t cap = n < 1024 ? 1024 : B200M_MAX_BLOCK;
-            if (b200m_host_alloc ((void**)&p->stage, 2 * cap * sizeof (float)) == 0) p->stage_cap = cap;
-        }
-        if (p->stage_cap) {
-            memcpy (p->stage, p->input[0], n * sizeof (float)); memcpy (p->stage + p->stage_cap, p->input[1], n * sizeof (float));
-            float v = 0;
-            if (b200m_cor_process_host (p->cor, p->stage, p->stage_cap, n) == 0 && b200m_cor_results (p->cor, &v, nullptr) == 0 && p->p_phase) *p->p_phase = v;
-        }
+    if (p->cor && n >= 1 && n <= B200M_MAX_BLOCK && p->stage.fill (p->input, 2, n)) {      // stcor->process; *p_phase = stcor->read () (:248-251)
+        float v = 0;
+        if (b200m_cor_process_host (p->cor, p->stage.data, p->stage.cap, n) == 0 && b200m_cor_results (p->cor, &v, nullptr) == 0 && p->p_phase) *p->p_phase = v;
     }
     if (p->ui_active) {                                        // tx_rawstereo (:162-178)
         p->out.begin_event_object (p->rawstereo);
@@ -115,7 +104,7 @@ void xfer_cleanup (LV2_Handle h)
 {
     XferPlugin* p = (XferPlugin*)h;
     b200m_cor_destroy (p->cor);
-    if (p->stage) b200m_host_free (p->stage);
+    p->stage.release ();
     delete p;
 }
 

@@ -416,7 +416,7 @@ def test_audio_is_forwarded_whatever_the_cycle_length(name, level_port):
     ("spectr30stereo", list(range(64)), [(64, 65), (66, 67)]),
 ])
 def test_batched_mode_of_the_control_port_plugins(name, ports, audio, monkeypatch):
-    """B200M_LV2_BATCH: the instances of one plugin type share one bank (csrc/lv2_shim.cu ShimHub).  What an instance's control
+    """B200M_LV2_BATCH: the instances of one plugin type share one bank (SlotHub, csrc/lv2_hub.cuh).  What an instance's control
     ports show after cycle k + 1 is bit for bit what the reference plugin shows after cycle k (one declared cycle of latency)."""
     import meters_lv2_b200 as B
     monkeypatch.setenv("B200M_LV2_BATCH", "8")
@@ -459,3 +459,59 @@ def test_batched_mode_of_the_control_port_plugins(name, ports, audio, monkeypatc
     assert checked >= n * (nb - 3)
     for p in gs + rs:
         p.close()
+
+
+@pytest.mark.timeout(180)
+@pytest.mark.parametrize("name,compared", [("K20stereo", [3, 6, 7, 8]), ("dBTPstereo", [3, 6])])
+def test_batched_control_port_plugins_survive_a_host_that_breaks_the_contract(name, compared, monkeypatch):
+    """a skipped instance, a changing block size and an instance leaving must neither hang nor corrupt the others.  A cycle that
+    a double submission closes early meters silence for the member that skipped it: one cycle late, that member reads bit for
+    bit what a private instance fed its audio with the skipped cycles zeroed reads.  Compared: the ports that carry the bank's
+    reading (levels, and the K-meter's peaks); the plugins' own holds depend on which cycles an instance published."""
+    import meters_lv2_b200 as B
+    mine, l1 = descriptors(B.LIB_PATH)
+    monkeypatch.delenv("B200M_LV2_BATCH", raising=False)
+    private = Plugin(mine[name])                                         # the variable is read at instantiate: a bank of its own
+    monkeypatch.setenv("B200M_LV2_BATCH", "4")
+    ps = [Plugin(mine[name]) for _ in range(3)]                          # 3 members of a 4-slot hub
+    x = S.white(6, 1024 * 60, seed=5)
+    silence = np.zeros(1024, np.float32)
+
+    def connect(p):
+        p.ctl = {i: np.zeros(1, np.float32) for i in (0, 3, 6, 7, 8, 9)}
+        p.ctl[0][0] = 20.0                                               # |port 0| >= 3: no re-init handshake
+        for i, a in p.ctl.items():
+            p.port(i, a)
+
+    def cycle(p, bufs, n):
+        p.port(1, bufs[0]); p.port(2, bufs[0]); p.port(4, bufs[1]); p.port(5, bufs[1])
+        p.run(n)
+        return {i: u32(p.ctl[i])[0] for i in compared}
+
+    for p in ps + [private]:
+        connect(p)
+    got, want = {}, {}
+    for b in range(60):
+        n = 512 if 30 <= b < 34 else 1024                                # the host changes its block size for a few cycles
+        for i, p in enumerate(ps):
+            if p is None or (i == 1 and 10 <= b < 20):                   # instance 1 is bypassed for ten cycles
+                continue
+            bufs = [np.ascontiguousarray(x[2 * i + c, b * 1024:b * 1024 + n]) for c in range(2)]
+            r = cycle(p, bufs, n)
+            if i == 1:
+                got[b] = r
+            if i == 2 and b > 0:
+                assert all(np.isfinite(p.ctl[k][0]) for k in compared), (b, p.ctl)
+        skipped = 10 <= b < 20
+        want[b] = cycle(private, [silence[:n] if skipped else np.ascontiguousarray(x[2 + c, b * 1024:b * 1024 + n]) for c in range(2)], n)
+        if b == 45:
+            ps[0].close(); ps[0] = None                                  # leaves while the others keep running
+    for k in list(range(9)) + list(range(19, 30)):
+        assert got[k + 1] == want[k], (name, k, got[k + 1], want[k])
+    for p in ps[1:] + [private]:
+        p.close()
+    late = Plugin(mine[name])                                            # a fresh hub can be created after the old one emptied
+    connect(late)
+    cycle(late, [np.ascontiguousarray(x[c, :1024]) for c in range(2)], 1024)
+    assert all(np.isfinite(late.ctl[k][0]) for k in compared)
+    late.close()
