@@ -136,17 +136,21 @@ _PROTOS = {
     "b200m_bim_create": (C.c_int, [C.POINTER(_v), C.c_int, C.c_uint32, C.c_double]),
     "b200m_bim_destroy": (C.c_int, [_v]),
     "b200m_bim_control": (C.c_int, [_v, C.c_int, _v]),
+    "b200m_bim_control_inst": (C.c_int, [_v, C.c_int32, C.c_int, _v]),
     "b200m_bim_run_device": (C.c_int, [_v, _v, C.c_size_t, C.c_uint32, _v]),
     "b200m_bim_run_host": (C.c_int, [_v, _v, C.c_size_t, C.c_uint32]),
     "b200m_bim_results": (C.c_int, [_v, C.c_uint32, _v, _v, _v, _v, _v]),
     "b200m_bim_window_closed": (C.c_int, [_v]),
     "b200m_bim_published": (C.c_int, [_v, C.c_uint32, _v, _v, _v, _v, _v]),
+    "b200m_bim_results_all": (C.c_int, [_v, _v, _v, _v, _v, _v, _v, _v, _v, _v, _v]),
     "b200m_sdh_create": (C.c_int, [C.POINTER(_v), C.c_int, C.c_uint32, C.c_double]),
     "b200m_sdh_destroy": (C.c_int, [_v]),
     "b200m_sdh_control": (C.c_int, [_v, C.c_int, _v]),
+    "b200m_sdh_control_inst": (C.c_int, [_v, C.c_int32, C.c_int, _v]),
     "b200m_sdh_run_device": (C.c_int, [_v, _v, C.c_size_t, C.c_uint32, _v]),
     "b200m_sdh_run_host": (C.c_int, [_v, _v, C.c_size_t, C.c_uint32]),
     "b200m_sdh_results": (C.c_int, [_v, C.c_uint32, _v, _v, _v, _v, _v]),
+    "b200m_sdh_results_all": (C.c_int, [_v, _v, _v, _v, _v, _v]),
     # spectr30
     "b200m_spec_create": (C.c_int, [C.POINTER(_v), C.c_int, C.c_uint32, C.c_uint32, C.c_double]),
     "b200m_spec_destroy": (C.c_int, [_v]),
@@ -526,7 +530,7 @@ class NeedleMeters(_Bank):
         return s
 
 
-CTL_START, CTL_PAUSE, CTL_RESET, CTL_AVERAGE, CTL_WINDOWED = 1, 2, 3, 4, 5
+CTL_START, CTL_PAUSE, CTL_RESET, CTL_AVERAGE, CTL_WINDOWED, CTL_CLEAR = 1, 2, 3, 4, 5, 6
 
 
 class _StatBank(_Bank):
@@ -537,8 +541,9 @@ class _StatBank(_Bank):
         self.n_inst = n_inst
         _ck(getattr(lib(), self._pfx + "create")(C.byref(self.h), device, n_inst, rate))
 
-    def control(self, cmd, stream=None):
-        _ck(getattr(lib(), self._pfx + "control")(self.h, cmd, _stream_ptr(stream)))
+    def control(self, cmd, stream=None, inst=-1):
+        """CTL_* on one instance, or on every instance with inst = -1"""
+        _ck(getattr(lib(), self._pfx + "control_inst")(self.h, inst, cmd, _stream_ptr(stream)))
 
     def run(self, x, stream=None):
         if isinstance(x, np.ndarray) or not x.is_cuda:
@@ -563,6 +568,17 @@ class Bitmeter(_StatBank):
         _ck(lib().b200m_bim_results(self.h, inst, _np_ptr(h), _np_ptr(c), _np_ptr(mm), C.byref(it), _stream_ptr(stream)))
         return h, c, mm, it.value
 
+    def results_all(self, stream=None):
+        """every instance in one synchronisation: dict of hist [n, 584], cnt [n, 5], minmax [n, 2], itime [n], closed [n] (the
+        last run closed that instance's window) and pub_hist, pub_cnt, pub_minmax, pub_itime (its last published snapshot)"""
+        n = self.n_inst
+        r = dict(hist=np.empty((n, 584), np.int32), cnt=np.empty((n, 5), np.int32), minmax=np.empty((n, 2), np.float32),
+                 itime=np.empty(n, np.int64), closed=np.empty(n, np.int32), pub_hist=np.empty((n, 584), np.int32),
+                 pub_cnt=np.empty((n, 5), np.int32), pub_minmax=np.empty((n, 2), np.float32), pub_itime=np.empty(n, np.int64))
+        _ck(lib().b200m_bim_results_all(self.h, *(_np_ptr(r[k]) for k in ("hist", "cnt", "minmax", "itime", "closed", "pub_hist", "pub_cnt",
+                                                                            "pub_minmax", "pub_itime")), _stream_ptr(stream)))
+        return r
+
 
 class SigDistHist(_StatBank):
     """N x the signal-distribution-histogram plugin's statistics (src/sigdistlv2.c:287-327)."""
@@ -572,6 +588,13 @@ class SigDistHist(_StatBank):
         h = np.empty(361, np.int32); mp = np.empty(2, np.int32); av = np.empty(3, np.float64); it = C.c_int64(0)
         _ck(lib().b200m_sdh_results(self.h, inst, _np_ptr(h), _np_ptr(mp), _np_ptr(av), C.byref(it), _stream_ptr(stream)))
         return h, mp, av, it.value
+
+    def results_all(self, stream=None):
+        """every instance in one synchronisation: (hist [n, 361], max_peak [n, 2], avg_tmp_var [n, 3] fp64, itime [n])"""
+        n = self.n_inst
+        h = np.empty((n, 361), np.int32); mp = np.empty((n, 2), np.int32); av = np.empty((n, 3), np.float64); it = np.empty(n, np.int64)
+        _ck(lib().b200m_sdh_results_all(self.h, _np_ptr(h), _np_ptr(mp), _np_ptr(av), _np_ptr(it), _stream_ptr(stream)))
+        return h, mp, av, it
 
 
 DR14_RESULT_DTYPE = np.dtype([("v_rms", "<f4", 2), ("v_peak", "<f4", 2), ("m_peak", "<f4", 2), ("m_rms", "<f4", 2), ("dr", "<f4", 2),

@@ -65,14 +65,14 @@ inline void forward_audio (float* const* in, float* const* out, uint32_t chn, ui
 // or n_samples changes) the open cycle is launched as it is, and the rows of the members that did not submit are zeroed
 // first: a skipped instance meters silence for that cycle rather than its previous block again.
 struct HubKey {
-    int family;                                                // lv2_shim.cu: its Kind; lv2_ebur128.cu: HUB_EBUR128
+    int family;                                                // lv2_shim.cu: its Kind; lv2_ebur128.cu, lv2_stats.cu: HUB_*
     int ppm_kind; uint32_t chn, tpk_flags; double rate;        // chn: staged rows per slot
     bool operator== (const HubKey& o) const
     {
         return family == o.family && ppm_kind == o.ppm_kind && chn == o.chn && tpk_flags == o.tpk_flags && rate == o.rate;
     }
 };
-constexpr int HUB_EBUR128 = -1;
+constexpr int HUB_EBUR128 = -1, HUB_BITMETER = -2, HUB_SIGDIST = -3;
 
 class SlotHub {
 public:

@@ -14,6 +14,7 @@
  *   EBUr128 (src/ebulv2.cc:31-38): 0 control atom in, 1 notify atom out, 2 inL, 3 outL, 4 inR, 5 outR
  *   needle / COR / dBTP / K-meters (src/meters.cc:59-70): 0 reflevel, 1 in0, 2 out0, 3 level0, 4 in1, 5 out1, 6 level1, 7 peak0, 8 peak1, 9 hold
  *   spectr30 (src/spectrumlv2.c:35-44): 0-59 band / max outputs, 60 speed, 61 reset, 62 amp, 63 state, 64 in0, 65 out0, 66 in1, 67 out1
+ *   bitmeter / SigDistHist (src/bitmeter.c, src/sigdistlv2.c port enums): 0 control atom in, 1 notify atom out, 2 in, 3 out
  */
 #define _GNU_SOURCE
 #include <dlfcn.h>
@@ -56,13 +57,13 @@ typedef struct {
     LV2_Handle h;
     float *in[2], *out[2];
     float ctl[68];                          /* control ports (in and out) */
-    uint8_t *atom_in, *atom_out;            /* EBUr128 */
+    uint8_t *atom_in, *atom_out;            /* EBUr128, bitmeter, SigDistHist */
 } Inst;
 
 typedef struct { const LV2_Descriptor* d; Inst* inst; int first, last; uint32_t nframes; int kind; uint32_t seq_t, chunk_t; pthread_barrier_t *start, *done; int cycles;
                  int cycle; const uint8_t* first_msgs; uint32_t first_len; } Worker;
 
-enum { KIND_MTR, KIND_EBUR, KIND_SPEC };
+enum { KIND_MTR, KIND_EBUR, KIND_SPEC, KIND_STATS };
 #define ATOM_CAP 8192
 
 /* one event at frame 0: object {otype; controlkey = key (Int); controlval = val (Float)} -- forge_kvcontrolmessage, src/uris.h:279-294 */
@@ -87,7 +88,7 @@ static void run_range (const Worker* w)
 {
     for (int i = w->first; i < w->last; ++i) {
         Inst* p = &w->inst[i];
-        if (w->kind == KIND_EBUR) {           /* host convention: empty input sequence, output buffer announced as a chunk of its capacity */
+        if (w->kind == KIND_EBUR || w->kind == KIND_STATS) {   /* host convention: empty input sequence, output buffer announced as a chunk of its capacity */
             uint32_t* a = (uint32_t*)p->atom_in; a[0] = 8; a[1] = w->seq_t; a[2] = 0; a[3] = 0;
             if (w->cycle == 0 && w->first_len) { memcpy (p->atom_in + 16, w->first_msgs, w->first_len); a[0] = 8 + w->first_len; }   /* the GUI's opening messages */
             uint32_t* o = (uint32_t*)p->atom_out; o[0] = ATOM_CAP - 8; o[1] = w->chunk_t;
@@ -122,7 +123,7 @@ int main (int argc, char** argv)
         else if (!strcmp (argv[i], "--rate")) rate = atof (argv[i + 1]);
         else if (!strcmp (argv[i], "--threads")) threads = atoi (argv[i + 1]);
         else if (!strcmp (argv[i], "--dbtp")) dbtp = atoi (argv[i + 1]);       /* EBUr128: enable the true-peak meters (CTL_UISETTINGS bit 64) */
-        else if (!strcmp (argv[i], "--ui")) ui = atoi (argv[i + 1]);           /* EBUr128: a GUI is attached (meteron): level messages every cycle */
+        else if (!strcmp (argv[i], "--ui")) ui = atoi (argv[i + 1]);           /* EBUr128, bitmeter, SigDistHist: a GUI is attached (meteron) */
         else { fprintf (stderr, "unknown option %s\n", argv[i]); return 2; }
     }
     if (threads < 1) threads = 1;
@@ -135,7 +136,8 @@ int main (int argc, char** argv)
     const LV2_Descriptor* d = NULL;
     for (uint32_t i = 0; (d = get (i)) != NULL; ++i) if (!strcmp (d->URI, full)) break;
     if (!d) { fprintf (stderr, "%s not served by %s\n", full, lib); return 1; }
-    const int kind = !strcmp (uri, "EBUr128") ? KIND_EBUR : !strncmp (uri, "spectr30", 8) ? KIND_SPEC : KIND_MTR;
+    const int kind = !strcmp (uri, "EBUr128") ? KIND_EBUR : !strncmp (uri, "spectr30", 8) ? KIND_SPEC
+                   : !strcmp (uri, "bitmeter") || !strcmp (uri, "SigDistHist") ? KIND_STATS : KIND_MTR;
     const int stereo = kind == KIND_EBUR || strstr (uri, "stereo") || !strcmp (uri, "COR") || !strcmp (uri, "BBCM6");
 
     LV2_URID_Map map = {NULL, urid_map};
@@ -144,14 +146,15 @@ int main (int argc, char** argv)
     const uint32_t seq_t = urid_map (NULL, "http://lv2plug.in/ns/ext/atom#Sequence"), chunk_t = urid_map (NULL, "http://lv2plug.in/ns/ext/atom#Chunk");
 
     /* EBUr128: what the GUI sends when it opens -- integration on, dBTP on, optionally "meteron" (src/ebulv2.cc:258-331) */
+    /* bitmeter / SigDistHist (ports 0 control, 1 notify, 2 in, 3 out): "meteron" with --ui 1, and SigDistHist's CTL_START */
     uint8_t first_msgs[512]; uint32_t first_len = 0;
-    if (kind == KIND_EBUR) {
+    if (kind == KIND_EBUR || kind == KIND_STATS) {
         const uint32_t t_obj = urid_map (NULL, "http://lv2plug.in/ns/ext/atom#Object"), t_int = urid_map (NULL, "http://lv2plug.in/ns/ext/atom#Int"),
                        t_flt = urid_map (NULL, "http://lv2plug.in/ns/ext/atom#Float"), cfg = urid_map (NULL, MTR_URI "metercfg"),
                        kk = urid_map (NULL, MTR_URI "controlkey"), kv = urid_map (NULL, MTR_URI "controlval"), on = urid_map (NULL, MTR_URI "meteron");
         if (ui) first_len += forge_kv (first_msgs + first_len, t_obj, on, t_int, t_flt, kk, kv, 0, 0, 0);
-        first_len += forge_kv (first_msgs + first_len, t_obj, cfg, t_int, t_flt, kk, kv, 7 /* CTL_UISETTINGS */, dbtp ? 64.0f : 0.0f, 1);
-        first_len += forge_kv (first_msgs + first_len, t_obj, cfg, t_int, t_flt, kk, kv, 1 /* CTL_START */, 0.0f, 1);
+        if (kind == KIND_EBUR) first_len += forge_kv (first_msgs + first_len, t_obj, cfg, t_int, t_flt, kk, kv, 7 /* CTL_UISETTINGS */, dbtp ? 64.0f : 0.0f, 1);
+        if (kind == KIND_EBUR || !strcmp (uri, "SigDistHist")) first_len += forge_kv (first_msgs + first_len, t_obj, cfg, t_int, t_flt, kk, kv, 1 /* CTL_START */, 0.0f, 1);
     }
     Inst* inst = (Inst*)calloc ((size_t)n_inst, sizeof (Inst));
     uint64_t s = 0x42B200;
@@ -163,10 +166,11 @@ int main (int argc, char** argv)
             p->in[c] = (float*)malloc (sizeof (float) * nframes); p->out[c] = (float*)malloc (sizeof (float) * nframes);
             for (uint32_t k = 0; k < nframes; ++k) { s ^= s << 13; s ^= s >> 7; s ^= s << 17; p->in[c][k] = ((float)(s >> 40) * (1.0f / 8388608.0f) - 1.0f) * 0.25f; }
         }
-        if (kind == KIND_EBUR) {
+        if (kind == KIND_EBUR || kind == KIND_STATS) {
             p->atom_in = (uint8_t*)calloc (1, 1024); p->atom_out = (uint8_t*)calloc (1, ATOM_CAP);
             d->connect_port (p->h, 0, p->atom_in); d->connect_port (p->h, 1, p->atom_out);
-            d->connect_port (p->h, 2, p->in[0]); d->connect_port (p->h, 3, p->out[0]); d->connect_port (p->h, 4, p->in[1]); d->connect_port (p->h, 5, p->out[1]);
+            d->connect_port (p->h, 2, p->in[0]); d->connect_port (p->h, 3, p->out[0]);
+            if (kind == KIND_EBUR) { d->connect_port (p->h, 4, p->in[1]); d->connect_port (p->h, 5, p->out[1]); }
         } else if (kind == KIND_SPEC) {
             for (uint32_t k = 0; k < 64; ++k) d->connect_port (p->h, k, &p->ctl[k]);
             p->ctl[60] = 1.0f; p->ctl[61] = -4.0f; p->ctl[62] = 0.0f;
@@ -199,7 +203,7 @@ int main (int argc, char** argv)
     }
     for (int t = 0; t < threads; ++t) pthread_join (th[t], NULL);
     const double mean = sum / cycles, budget = nframes / rate;
-    float probe = kind == KIND_EBUR ? 0.0f : inst[0].ctl[3];
+    float probe = kind == KIND_EBUR || kind == KIND_STATS ? 0.0f : inst[0].ctl[3];
     const char* batch = getenv ("B200M_LV2_BATCH");
     printf ("{\"lv2_host\": \"%s\", \"lib\": \"%s\", \"instances\": %d, \"threads\": %d, \"nframes\": %u, \"rate\": %.0f, \"cycles\": %d, "
             "\"dbtp\": %d, \"ui\": %d, \"batch_slots\": %s, \"cycle_ms_mean\": %.4f, \"cycle_ms_max\": %.4f, \"us_per_instance\": %.3f, \"budget_ms\": %.3f, \"fits_realtime\": %s, "
