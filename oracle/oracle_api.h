@@ -40,6 +40,11 @@ void  orc_ebu_hist    (void* h, int inst, int* histM, int* histS, int* counts4);
 void  orc_ebu_coeffs  (void* h, float* out7);          /* a0 a1 a2 b1 b2 c3 c4 */
 void  orc_ebu_state   (void* h, int inst, float* z, float* power64, float* frpwr, int* counters4);
                        /* z: [nchan][4]; counters: frcnt wrind div1 div2 */
+/* Ebu_r128_hist::calc_integ + calc_range (:105-150) on caller-given counts: 751 bins and the count word of each
+ * histogram.  out5 = integrated, integ_thr, range_min, range_max, range_thr, all pre-set to -200 (what a reset
+ * instance reports: calc_integ leaves the threshold unchanged below 50 points).  The range walks have no upper
+ * bound: the caller guarantees that the bins sum to the count word and that both walks end by bin 750. */
+void  orc_ebu_hist_calc (const int* histM751, int cntM, const int* histS751, int cntS, float* out5);
 
 /* ---- True peak (jmeters/truepeakdsp.h:28-61), one mono meter per channel ---- */
 void* orc_tp_create   (int n, float fsamp);

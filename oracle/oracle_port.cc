@@ -760,6 +760,15 @@ void orc_ebu_hist (void* h, int inst, int* hm, int* hs, int* c4) {
     memcpy (hm, e.hM.bins, sizeof (e.hM.bins)); memcpy (hs, e.hS.bins, sizeof (e.hS.bins));
     c4[0] = e.hM.count; c4[1] = e.hS.count; c4[2] = e.hM.error; c4[3] = e.hS.error;
 }
+void orc_ebu_hist_calc (const int* hm, int cm, const int* hs, int cs, float* o) {   // calc_integ + calc_range (:105-150) on given counts
+    Hist M, S;
+    memcpy (M.bins, hm, sizeof (M.bins)); M.count = cm; M.error = 0;
+    memcpy (S.bins, hs, sizeof (S.bins)); S.count = cs; S.error = 0;
+    binpow_init ();
+    for (int q = 0; q < 5; ++q) o[q] = -200.0f;
+    hist_integ (M, o + 0, o + 1);
+    hist_range (S, o + 2, o + 3, o + 4);
+}
 void orc_ebu_coeffs (void* h, float* o) { const Ebu& e = ((Bank<Ebu>*)h)->v[0]; o[0] = e.a0; o[1] = e.a1; o[2] = e.a2; o[3] = e.b1; o[4] = e.b2; o[5] = e.c3; o[6] = e.c4; }
 void orc_ebu_state (void* h, int inst, float* z, float* pw, float* frpwr, int* c4) {
     auto* b = (Bank<Ebu>*)h; const Ebu& e = b->v[inst];

@@ -110,6 +110,15 @@ void orc_ebu_hist (void* h, int inst, int* hm, int* hs, int* c4)
     memcpy (hm, e->histogram_M (), 751 * sizeof (int)); memcpy (hs, e->histogram_S (), 751 * sizeof (int));
     c4[0] = e->hist_M_count (); c4[1] = e->hist_S_count (); c4[2] = e->_hist_M._error; c4[3] = e->_hist_S._error;
 }
+void orc_ebu_hist_calc (const int* hm, int cm, const int* hs, int cs, float* o)
+{
+    Ebu_r128_hist M, S;
+    memcpy (M._histc, hm, 751 * sizeof (int)); M._count = cm;
+    memcpy (S._histc, hs, 751 * sizeof (int)); S._count = cs;
+    for (int q = 0; q < 5; ++q) o[q] = -200.0f;
+    M.calc_integ (o + 0, o + 1);
+    S.calc_range (o + 2, o + 3, o + 4);
+}
 void orc_ebu_coeffs (void* h, float* o)
 {
     Ebu_r128_proc* e = ((EbuB*)h)->p[0];

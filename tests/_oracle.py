@@ -36,6 +36,7 @@ def _proto(lib):
         "orc_ebu_hist": (None, [_v, C.c_int, _v, _v, _v]),
         "orc_ebu_coeffs": (None, [_v, _v]),
         "orc_ebu_state": (None, [_v, C.c_int, _v, _v, _v, _v]),
+        "orc_ebu_hist_calc": (None, [_v, C.c_int, _v, C.c_int, _v]),
         "orc_r128_cycle": (None, [_v, _v, _v, C.c_size_t, C.c_int, C.c_int, C.c_int]),
         "orc_tp_create": (_v, [C.c_int, C.c_float]),
         "orc_tp_destroy": (None, [_v]),
@@ -100,10 +101,16 @@ def _proto(lib):
         "orc_cpu_info": (C.c_int, [_v, _v, _v]),
         "orc_r128_bench": (C.c_int, [C.c_int, C.c_int, C.c_int, C.c_int, C.c_int, C.c_int, C.c_int, C.c_float, _v]),
     }
+    # a prebuilt reference library from before an entry was added lacks it: the other entries stay usable, and
+    # exports() says which ones the library has
+    lib.orc_exports = set()
     for name, (res, args) in P.items():
-        fn = getattr(lib, name)
+        fn = getattr(lib, name, None)
+        if fn is None:
+            continue
         fn.restype = res
         fn.argtypes = args
+        lib.orc_exports.add(name)
     return lib
 
 
@@ -116,6 +123,11 @@ def load(kind="best"):
     if kind not in _cache:
         _cache[kind] = _proto(C.CDLL(PATHS[kind]))
     return _cache[kind]
+
+
+def exports(kind, name):
+    """True if the `kind` oracle is built and exports `name`"""
+    return available(kind) and name in load(kind).orc_exports
 
 
 def ptr(a):
@@ -186,6 +198,48 @@ class Ebu:
         fr = np.empty(1, np.float32); c = np.empty(4, np.int32)
         self.L.orc_ebu_state(self.h, inst, ptr(z), ptr(pw), ptr(fr), ptr(c))
         return z, pw, fr[0], c
+
+
+def _range_walks_end(h):
+    """True if both percentile walks of Ebu_r128_hist::calc_range (ebu_r128_proc.cc:143-147) stop by bin 750 for every
+    start bin k: `for (i = k, s = 0; s < a; i++) s += h[i]` and `for (j = 750, s = n; s > b; j--) s -= h[j]` in float,
+    with n the int sum of h[k:], a = 0.10f * n, b = 0.95f * n.  Vectorised over k; float32 numpy arithmetic rounds as
+    the reference's SSE float code does."""
+    h = np.asarray(h, np.int64)
+    f = h.astype(np.float32)
+    ks = np.arange(751)
+    n = np.cumsum(h[::-1])[::-1]                       # n[k] = sum h[k:] (exact)
+    nf = n.astype(np.float32)
+    a = np.float32(0.10) * nf
+    b = np.float32(0.95) * nf
+    up = np.zeros(751, np.float32)
+    for i in range(751):
+        up = np.where(ks <= i, up + f[i], up)
+    dn = nf.copy()
+    for j in range(750, -1, -1):
+        dn = np.where(dn > b, dn - f[j], dn)
+    return bool(np.all(~(up < a)) and np.all(~(dn > b)))
+
+
+def hist_calc(hist_m, cnt_m, hist_s, cnt_s, kind="best"):
+    """Ebu_r128_hist::calc_integ + calc_range on given counts -> float32[5]: integrated, integ_thr, range_min,
+    range_max, range_thr (-200 where the reference leaves a value unset).  The reference's range walks have no
+    upper bound, so the counts are checked first: each histogram's bins must sum to its count word, and above
+    2^24 points (where float partial sums stop being exact) both walks must provably end by bin 750.
+    kind "best" is the reference build when it has this entry, else the port (pinned to the reference's outputs stored
+    in tests/golden/ebu_hist_calc.npz by tests/test_oracle_port.py)."""
+    if kind == "best":
+        kind = "reference" if exports("reference", "orc_ebu_hist_calc") else "port"
+    hm = np.ascontiguousarray(hist_m, np.int32); hs = np.ascontiguousarray(hist_s, np.int32)
+    assert hm.shape == (751,) and hs.shape == (751,)
+    assert (hm >= 0).all() and (hs >= 0).all()
+    assert int(hm.astype(np.int64).sum()) == cnt_m and int(hs.astype(np.int64).sum()) == cnt_s, "bins must sum to the count words"
+    assert cnt_m < 2 ** 31 and cnt_s < 2 ** 31
+    if cnt_s > 2 ** 24:
+        assert _range_walks_end(hs), "calc_range would walk past bin 750"
+    out = np.empty(5, np.float32)
+    load(kind).orc_ebu_hist_calc(ptr(hm), int(cnt_m), ptr(hs), int(cnt_s), ptr(out))
+    return out
 
 
 def r128_cycle(ebu, tp, x, nfram, nblocks, nthreads):

@@ -7,7 +7,8 @@ The reference ships no golden vectors or tests (SURVEY.md §4), so these fixture
 reference itself, run here — are the pin for the oracle port on machines where /root/reference is absent.
 `compute(kind)` is also what tests/test_oracle_port.py::test_golden_vectors replays.
 The phasewheel entries come from the port (FFTW3 is absent: that path has no reference build).
-It also writes ebur128_plugin.npz and goniometer_ref.npz (the reference side of two GPU tests).  lv2_ref.npz, what the
+It also writes ebur128_plugin.npz and goniometer_ref.npz (the reference side of two GPU tests) and ebu_hist_calc.npz (the
+reference's calc_integ / calc_range on the synthetic histograms of tests/test_ebu_gating_gpu.py).  lv2_ref.npz, what the
 reference's LV2 plugins write to their ports in the GPU tests, is recorded by those tests on a GPU machine with oracle/_ref built:
     B200M_LV2_REF_RECORD=$PWD/tests/golden/lv2_ref.npz python -m pytest -m gpu tests/test_lv2_*.py tests/test_dr14_gpu.py
 """
@@ -128,6 +129,13 @@ def ebur128_plugin_reads():
     return np.stack(reads)
 
 
+def ebu_hist_calc_reads(kind="reference"):
+    """Ebu_r128_hist::calc_integ / calc_range of the reference on the synthetic histogram families of
+    tests/test_ebu_gating_gpu.py: [n, 5] float32 (integrated, integ_thr, range_min, range_max, range_thr)"""
+    import test_ebu_gating_gpu as GG
+    return np.stack([O.hist_calc(hm, int(hm.sum()), hs, int(hs.sum()), kind=kind) for _, hm, hs in GG.hist_families()])
+
+
 if __name__ == "__main__":
     assert O.available("reference"), "build oracle/_ref first (make -C oracle ref)"
     d = compute("reference")
@@ -145,3 +153,5 @@ if __name__ == "__main__":
         d["state_value_%d" % i] = np.frombuffer(v[0], np.uint8)
     np.savez_compressed(os.path.join(HERE, "goniometer_ref.npz"), **d)
     print("wrote goniometer_ref.npz")
+    np.savez_compressed(os.path.join(HERE, "ebu_hist_calc.npz"), out5=ebu_hist_calc_reads())
+    print("wrote ebu_hist_calc.npz")

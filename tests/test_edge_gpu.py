@@ -19,6 +19,9 @@ def u32(a):
     (96000.0, 33, [1024] * 40 + [8192] * 8),
     (48000.0, 130, [1] * 5 + [8192] * 3 + [2400] * 4 + [2399, 2401]),
     (22050.0, 3, [512] * 200),
+    (4000.0, 7, [8192] * 4 + [1] + [8192] * 4 + [3, 4097]),   # fragment = 200 frames: 41 fragment edges in 8192 frames, more than
+                                                               # K1's 32 pieces per launch; after the 1-frame block the second
+                                                               # launch starts at an unaligned offset
 ])
 def test_ebu_rates_and_sizes(fs, n_inst, blocks):
     import torch

@@ -45,6 +45,28 @@ def test_ebu_port_equals_reference(nchan):
         assert np.array_equal(u32(sa[0]), u32(sb[0])) and np.array_equal(u32(sa[1]), u32(sb[1])) and list(sa[3]) == list(sb[3])
 
 
+HIST_CALC_GOLD = os.path.join(os.path.dirname(__file__), "golden", "ebu_hist_calc.npz")
+
+
+@needs_port
+@pytest.mark.parametrize("kind", ["port"] + (["reference"] if HAVE_REF else []))
+def test_ebu_hist_calc_equals_reference(kind):
+    """Ebu_r128_hist::calc_integ / calc_range on the synthetic histogram families of tests/test_ebu_gating_gpu.py
+    (thresholds, single bins at the decade edges, gated clusters, k < 0, every bin, sparse, counts near 2^27), all five
+    floats bit for bit: against the reference's outputs stored in tests/golden/ebu_hist_calc.npz (generated from
+    oracle/_ref by tests/golden/make_golden.py) and, where the reference build has the entry, against it directly."""
+    import golden.make_golden as G
+    if kind == "reference" and not O.exports("reference", "orc_ebu_hist_calc"):
+        pytest.skip("the prebuilt oracle/_ref predates orc_ebu_hist_calc (`make -C oracle ref` with the reference tree)")
+    got = G.ebu_hist_calc_reads(kind)
+    want = np.load(HIST_CALC_GOLD)["out5"]
+    assert got.shape == want.shape
+    bad = np.nonzero((u32(got) != u32(want)).any(axis=1))[0]
+    assert bad.size == 0, (kind, bad[:5], got[bad[:3]], want[bad[:3]])
+    if kind == "port" and O.exports("reference", "orc_ebu_hist_calc"):
+        assert np.array_equal(u32(got), u32(G.ebu_hist_calc_reads("reference")))
+
+
 @needs_both
 def test_truepeak_kmeter_port_equals_reference():
     x = S.nasty(7, sum(BLOCKS), seed=102)
