@@ -255,6 +255,10 @@ int b200m_cor_destroy (b200m_cor* h);
 int b200m_cor_process_device (b200m_cor* h, const float* d_in, size_t stride, uint32_t nfram, void* stream);
 int b200m_cor_process_host (b200m_cor* h, const float* in, size_t stride, uint32_t nfram);
 int b200m_cor_results (b200m_cor* h, float* out, void* stream);           /* Stcorrdsp::read (:79-82) */
+/* pair inst (-1: all) back to a newly constructed Stcorrdsp (stcorrdsp.cc:33-37): the five filter states and the reading zero, in
+ * both precision modes.  Ordered with the bank's runs on the stream it currently runs on.  A phasewheel ring fed from this bank
+ * (b200m_pw_attach_cor) is not touched. */
+int b200m_cor_clear (b200m_cor* h, int32_t inst, void* stream);
 /* B200M_PREC_EXACT (default): the five recurrences run serially in time, one lane per pair, bit-identical to the reference.
  * B200M_PREC_FMA: time-parallel evaluation -- the recurrences are linear one-pole filters, so a warp owns ONE pair, its lanes take
  * consecutive time segments and an affine warp scan stitches them: 32x more parallelism for small banks (2048 pairs are 64 warps
@@ -275,6 +279,14 @@ enum { B200M_PPM_VU = 0, B200M_PPM_IEC1 = 1, B200M_PPM_IEC2 = 2, B200M_PPM_MS = 
 int b200m_ppm_create (b200m_ppm** out, int device, uint32_t n_units, float fsamp, int kind);
 int b200m_ppm_destroy (b200m_ppm* h);
 int b200m_ppm_set_gain (b200m_ppm* h, float db_m, float db_s);       /* Msppmdsp::set_gain of the M and S meters (default -6, -6) */
+/* Msppmdsp::set_gain (msppmdsp.cc:135-143) of one pair's M and S meters (unit = -1: every pair, exactly b200m_ppm_set_gain).  The
+ * gains are designed on the host, skipped per meter when the dB value is unchanged, and reach the bank with its next process call,
+ * on that call's stream. */
+int b200m_ppm_set_gain_inst (b200m_ppm* h, int32_t unit, float db_m, float db_s);
+/* unit (-1: all) back to newly constructed meters (vumeterdsp.cc / iec1ppmdsp.cc / iec2ppmdsp.cc / msppmdsp.cc constructors):
+ * z1 z2 m = 0, _res = true, both meters of an M/S pair, whose gains return to -6 / -6 dB.  Ordered with the bank's runs on the
+ * stream it currently runs on. */
+int b200m_ppm_clear (b200m_ppm* h, int32_t unit, void* stream);
 int b200m_ppm_process_device (b200m_ppm* h, const float* d_in, size_t stride, uint32_t nfram, void* stream);
 int b200m_ppm_process_host (b200m_ppm* h, const float* in, size_t stride, uint32_t nfram);
 int b200m_ppm_read_device (b200m_ppm* h, void* stream);                /* read(): _res = true, value = _g * _m */
@@ -344,6 +356,16 @@ int b200m_spec_destroy (b200m_spec* h);
 /* one spectrum_run(): speed = *port 60, reset = *port 61 (same value for every instance) */
 int b200m_spec_process_device (b200m_spec* h, const float* d_in, size_t stride, uint32_t nfram, float speed, float reset, void* stream);
 int b200m_spec_process_host (b200m_spec* h, const float* in, size_t stride, uint32_t nfram, float speed, float reset);
+/* one spectrum_run() with every instance's own controls: ctl = host array [n_inst][2] = {*port 60, *port 61} of this cycle.  Each
+ * instance keeps its own speed / reset handshake state (src/spectrumlv2.c:170-205), fall-off coefficient and `ac` dither phase;
+ * the two calls above are this one with the same pair for every instance.  Only instances whose run parameters changed are
+ * uploaded, on the call's stream. */
+int b200m_spec_process_ctl_device (b200m_spec* h, const float* d_in, size_t stride, uint32_t nfram, const float* ctl, void* stream);
+int b200m_spec_process_ctl_host (b200m_spec* h, const float* in, size_t stride, uint32_t nfram, const float* ctl);
+/* instance inst (-1: all) back to what b200m_spec_create gives (spectrum_instantiate, src/spectrumlv2.c:73-121): filter states,
+ * val, max and ports zero, rst_h = -4, spd_h = 1, `ac` restarting with the next frame.  Ordered with the bank's runs on the stream
+ * it currently runs on. */
+int b200m_spec_clear (b200m_spec* h, int32_t inst, void* stream);
 /* B200M_PREC_EXACT (default): the reference's fp64 rounding sequence, ports bit-identical.  B200M_PREC_FMA: fused multiply-adds in the
  * biquad cascade (25 instead of 39 fp64 instructions per frame and band); band levels within +-1e-4 dB. */
 int b200m_spec_set_precision (b200m_spec* h, int mode);

@@ -122,10 +122,13 @@ _PROTOS = {
     "b200m_cor_results": (C.c_int, [_v, _v, _v]),
     "b200m_cor_state": (C.c_int, [_v, _v, _v]),
     "b200m_cor_coeffs": (C.c_int, [_v, _v]),
+    "b200m_cor_clear": (C.c_int, [_v, C.c_int32, _v]),
     # needle-meter ballistics
     "b200m_ppm_create": (C.c_int, [C.POINTER(_v), C.c_int, C.c_uint32, C.c_float, C.c_int]),
     "b200m_ppm_destroy": (C.c_int, [_v]),
     "b200m_ppm_set_gain": (C.c_int, [_v, C.c_float, C.c_float]),
+    "b200m_ppm_set_gain_inst": (C.c_int, [_v, C.c_int32, C.c_float, C.c_float]),
+    "b200m_ppm_clear": (C.c_int, [_v, C.c_int32, _v]),
     "b200m_ppm_process_device": (C.c_int, [_v, _v, C.c_size_t, C.c_uint32, _v]),
     "b200m_ppm_process_host": (C.c_int, [_v, _v, C.c_size_t, C.c_uint32]),
     "b200m_ppm_read_device": (C.c_int, [_v, _v]),
@@ -156,6 +159,9 @@ _PROTOS = {
     "b200m_spec_destroy": (C.c_int, [_v]),
     "b200m_spec_process_device": (C.c_int, [_v, _v, C.c_size_t, C.c_uint32, C.c_float, C.c_float, _v]),
     "b200m_spec_process_host": (C.c_int, [_v, _v, C.c_size_t, C.c_uint32, C.c_float, C.c_float]),
+    "b200m_spec_process_ctl_device": (C.c_int, [_v, _v, C.c_size_t, C.c_uint32, _v, _v]),
+    "b200m_spec_process_ctl_host": (C.c_int, [_v, _v, C.c_size_t, C.c_uint32, _v]),
+    "b200m_spec_clear": (C.c_int, [_v, C.c_int32, _v]),
     "b200m_spec_results": (C.c_int, [_v, _v, _v]),
     "b200m_spec_state": (C.c_int, [_v, C.c_uint32, _v, _v, _v, _v]),
     "b200m_spec_coeffs": (C.c_int, [_v, _v]),
@@ -484,6 +490,10 @@ class Stcorrdsp(_Bank):
         _ck(lib().b200m_cor_coeffs(self.h, _np_ptr(w)))
         return w
 
+    def clear(self, inst=-1, stream=None):
+        """pair inst (-1: all) back to a newly constructed Stcorrdsp; an attached phasewheel ring is not touched"""
+        _ck(lib().b200m_cor_clear(self.h, inst, _stream_ptr(stream)))
+
 
 PPM_VU, PPM_IEC1, PPM_IEC2, PPM_MS = 0, 1, 2, 3
 
@@ -505,8 +515,13 @@ class NeedleMeters(_Bank):
         self.n_meters = self.rows
         _ck(lib().b200m_ppm_create(C.byref(self.h), device, n_units, fsamp, kind))
 
-    def set_gain(self, db_m, db_s):
-        _ck(lib().b200m_ppm_set_gain(self.h, db_m, db_s))
+    def set_gain(self, db_m, db_s, unit=-1):
+        """Msppmdsp::set_gain of pair `unit`'s M and S meters (-1: every pair); applied with the next process()"""
+        _ck(lib().b200m_ppm_set_gain_inst(self.h, unit, db_m, db_s))
+
+    def clear(self, unit=-1, stream=None):
+        """unit (-1: all) back to newly constructed meters (M/S: gains -6 / -6 dB)"""
+        _ck(lib().b200m_ppm_clear(self.h, unit, _stream_ptr(stream)))
 
     def process(self, x, stream=None):
         if isinstance(x, np.ndarray) or not x.is_cuda:
@@ -647,14 +662,29 @@ class Spectr30(_Bank):
         _ck(lib().b200m_spec_create(C.byref(self.h), device, n_inst, nchan, rate))
 
     def process(self, x, speed=1.0, reset=-4.0, stream=None):
+        """speed / reset: ports 60 / 61, one value for every instance or an array of n_inst (each instance its own)"""
+        ctl = None
+        if np.ndim(speed) or np.ndim(reset):
+            ctl = np.empty((self.n_inst, 2), np.float32)
+            ctl[:, 0] = speed; ctl[:, 1] = reset
         if isinstance(x, np.ndarray) or not x.is_cuda:
             p, s, rows, n = _host_planar(x)
             assert rows == self.n_inst * self.nchan
-            _ck(lib().b200m_spec_process_host(self.h, p, s, n, speed, reset))
+            if ctl is None:
+                _ck(lib().b200m_spec_process_host(self.h, p, s, n, speed, reset))
+            else:
+                _ck(lib().b200m_spec_process_ctl_host(self.h, p, s, n, _np_ptr(ctl)))
         else:
             p, s, rows, n = _dev_ptr(x)
             assert rows == self.n_inst * self.nchan
-            _ck(lib().b200m_spec_process_device(self.h, p, s, n, speed, reset, _stream_ptr(stream)))
+            if ctl is None:
+                _ck(lib().b200m_spec_process_device(self.h, p, s, n, speed, reset, _stream_ptr(stream)))
+            else:
+                _ck(lib().b200m_spec_process_ctl_device(self.h, p, s, n, _np_ptr(ctl), _stream_ptr(stream)))
+
+    def clear(self, inst=-1, stream=None):
+        """instance inst (-1: all) back to a freshly created spectr30"""
+        _ck(lib().b200m_spec_clear(self.h, inst, _stream_ptr(stream)))
 
     def set_precision(self, mode):
         """PREC_EXACT: ports bit-identical to the reference; PREC_FMA: fused multiply-adds, band levels within +-1e-4 dB"""

@@ -238,6 +238,16 @@ cor_scan_kernel (const float* __restrict__ in, size_t stride, int n_inst, int nf
     }
 }
 
+// pairs [i0, i0 + n) back to a newly constructed Stcorrdsp (stcorrdsp.cc:33-37): the five filter states and the reading zero
+__global__ void cor_clear_kernel (int n_inst, int i0, int n, float* __restrict__ st, float* __restrict__ res)
+{
+    const int i = blockIdx.x * blockDim.x + threadIdx.x;
+    if (i >= n) return;
+#pragma unroll
+    for (int q = 0; q < 5; ++q) st[q * (size_t)n_inst + i0 + i] = 0.0f;
+    res[i0 + i] = 0.0f;
+}
+
 }  // namespace b200m
 
 using namespace b200m;
@@ -339,6 +349,17 @@ int b200m_cor_set_precision (b200m_cor* h, int mode)
 {
     if (!h || (mode != B200M_PREC_EXACT && mode != B200M_PREC_FMA)) return set_err (B200M_E_INVAL, "bad argument");
     h->scan = mode == B200M_PREC_FMA;                       // takes effect with the next process call
+    return 0;
+}
+
+int b200m_cor_clear (b200m_cor* h, int32_t inst, void* stream)
+{
+    if (!h || inst < -1 || inst >= (int32_t)h->n_inst) return set_err (B200M_E_INVAL, "bad argument");
+    DeviceGuard g (h->device);
+    const int i0 = inst < 0 ? 0 : inst, n = inst < 0 ? (int)h->n_inst : 1;
+    cor_clear_kernel<<<(n + 127) / 128, 128, 0, cor_stream (h, stream)>>> ((int)h->n_inst, i0, n, h->d_st, h->d_res);
+    B200M_LAUNCHED (1);
+    B200M_CUDA (cudaGetLastError ());
     return 0;
 }
 

@@ -48,16 +48,22 @@ struct Shim {
     struct ShimHub* hub = nullptr; int slot = -1;     // batched mode: a slot of a shared bank instead of a private one
 };
 
-// batched mode (lv2_hub.cuh): COR, dBTP, K-meters, needle meters (VU/BBC/EBU/DIN/NOR), spectr30.  spectr30's speed / reset ports
-// are bank-wide in the engine: the values of the instance that launches the cycle apply to all.  BBCM6 and the surround meters
-// keep private banks.
+// batched mode (lv2_hub.cuh): every plugin of this file.  Per-instance controls are stored per slot at submit and reach the bank
+// with the cycle's launch: spectr30's speed / reset (b200m_spec_process_ctl_host), BBCM6's S gain (b200m_ppm_set_gain_inst), a
+// surround meter's pair selection (the launch gathers the selected rows into the correlation bank's stage).  A vacated or newly
+// joined slot is cleared to a freshly instantiated plugin.
+constexpr uint8_t SUR_IDLE = 0xff;                        // a correlation pair that meters silence (4th pair of surround3, unconnected)
+
 struct ShimHub : SlotHub {
     b200m_cor* cor = nullptr; b200m_tpk* tpk = nullptr; b200m_spec* spec = nullptr; b200m_ppm* ppm = nullptr;
     std::vector<b200m_tpk_result> tpk_res; std::vector<float> f_res;      // results of the last completed cycle
-    float spec_speed = 1.0f, spec_reset = -4.0f;
+    std::vector<float> spec_ctl;                          // spectr30: [slot] {port 60, port 61} as last submitted
+    std::vector<float> s_gain;                            // BBCM6: [slot] S meter gain (dB) as last submitted
+    std::vector<uint8_t> sur_sel;                         // surround: [slot][8] input channel of each pair's L and R row, or SUR_IDLE
+    PinnedStage pairs;                                    // surround: [slots * 8] rows, the correlation bank's input
 
     ShimHub (const HubKey& k, uint32_t n) : SlotHub (k, n) {}
-    ~ShimHub () { b200m_cor_destroy (cor); b200m_tpk_destroy (tpk); b200m_spec_destroy (spec); b200m_ppm_destroy (ppm); }
+    ~ShimHub () { b200m_cor_destroy (cor); b200m_tpk_destroy (tpk); b200m_spec_destroy (spec); b200m_ppm_destroy (ppm); pairs.release (); }
 
     static SlotHub* create (const HubKey& k, uint32_t n)
     {
@@ -69,9 +75,17 @@ struct ShimHub : SlotHub {
         case K_COR: rc = b200m_cor_create (&h->cor, 0, n, (int)k.rate, 2e3f, 0.3f); h->f_res.assign (n, 0.0f); break;
         case K_DBTP: case K_KMETER: rc = b200m_tpk_create (&h->tpk, 0, rows, (float)k.rate, k.tpk_flags); h->tpk_res.assign (rows, b200m_tpk_result{0, 0, 0, 0}); break;
         case K_NEEDLE: rc = b200m_ppm_create (&h->ppm, 0, rows, (float)k.rate, k.ppm_kind); h->f_res.assign (rows, 0.0f); break;
+        case K_BBCM6: rc = b200m_ppm_create (&h->ppm, 0, n, (float)k.rate, B200M_PPM_MS); h->f_res.assign (2 * n, 0.0f); h->s_gain.assign (n, -6.0f); break;
+        case K_SUR:
+            rc = b200m_tpk_create (&h->tpk, 0, rows, (float)k.rate, B200M_TPK_KMETER);
+            if (!rc) rc = b200m_cor_create (&h->cor, 0, 4 * n, (int)k.rate, 2e3f, 0.3f);
+            if (!rc) { h->pairs.reserve (8 * n); if (!h->pairs.cap) rc = -1; }
+            h->tpk_res.assign (rows, b200m_tpk_result{0, 0, 0, 0}); h->f_res.assign (4 * n, 0.0f); h->sur_sel.assign (8 * n, SUR_IDLE);
+            break;
         case K_SPEC:
             rc = b200m_spec_create (&h->spec, 0, n, k.chn, k.rate); h->f_res.assign ((size_t)n * 60, -100.0f);
             if (!rc) b200m_spec_results (h->spec, h->f_res.data (), nullptr);        // the ports' initial values
+            for (uint32_t i = 0; i < n; ++i) { h->spec_ctl.push_back (1.0f); h->spec_ctl.push_back (-4.0f); }   // spectrum_instantiate (:95-98)
             break;
         }
         if (rc) { delete h; return nullptr; }
@@ -86,11 +100,27 @@ struct ShimHub : SlotHub {
             rc = b200m_tpk_process_host (tpk, stage.data, B200M_MAX_BLOCK, n, B200M_TP_MODE_PROCESS);
             if (!rc) rc = b200m_tpk_read_device (tpk, nullptr);
             break;
+        case K_BBCM6:
+            for (uint32_t i = 0; i < slots; ++i) b200m_ppm_set_gain_inst (ppm, (int32_t)i, -6, s_gain[i]);     // bbcm_run (src/meters.cc:557-560)
+            /* fall through */
         case K_NEEDLE:
             rc = b200m_ppm_process_host (ppm, stage.data, B200M_MAX_BLOCK, n);
             if (!rc) rc = b200m_ppm_read_device (ppm, nullptr);
             break;
-        case K_SPEC: rc = b200m_spec_process_host (spec, stage.data, B200M_MAX_BLOCK, n, spec_speed, spec_reset); break;
+        case K_SUR:
+            // the selected input rows of every slot -> its 4 correlation pairs; rows of members that skipped the cycle are zero already
+            for (uint32_t i = 0; i < slots; ++i)
+                for (uint32_t r = 0; r < 8; ++r) {
+                    float* dst = pairs.data + (size_t)(8 * i + r) * B200M_MAX_BLOCK;
+                    const uint8_t c = sur_sel[8 * i + r];
+                    if (c == SUR_IDLE) memset (dst, 0, n * sizeof (float));
+                    else memcpy (dst, stage.data + (size_t)(i * key.chn + c) * B200M_MAX_BLOCK, n * sizeof (float));
+                }
+            rc = b200m_cor_process_host (cor, pairs.data, B200M_MAX_BLOCK, n);
+            if (!rc) rc = b200m_tpk_process_host (tpk, stage.data, B200M_MAX_BLOCK, n, B200M_TP_MODE_PROCESS);
+            if (!rc) rc = b200m_tpk_read_device (tpk, nullptr);
+            break;
+        case K_SPEC: rc = b200m_spec_process_ctl_host (spec, stage.data, B200M_MAX_BLOCK, n, spec_ctl.data ()); break;
         }
         return rc;
     }
@@ -99,18 +129,30 @@ struct ShimHub : SlotHub {
         switch (key.family) {
         case K_COR: b200m_cor_results (cor, f_res.data (), nullptr); break;
         case K_DBTP: case K_KMETER: b200m_tpk_results (tpk, tpk_res.data (), nullptr); break;
-        case K_NEEDLE: b200m_ppm_results (ppm, f_res.data (), nullptr); break;
+        case K_NEEDLE: case K_BBCM6: b200m_ppm_results (ppm, f_res.data (), nullptr); break;
+        case K_SUR: b200m_cor_results (cor, f_res.data (), nullptr); b200m_tpk_results (tpk, tpk_res.data (), nullptr); break;
         case K_SPEC: b200m_spec_results (spec, f_res.data (), nullptr); break;
         }
     }
-    void vacate (uint32_t slot) override
+    // the slot as a freshly instantiated plugin has it; also at join, because a vacant slot meters silence until it is taken
+    void clear (uint32_t slot)
     {
-        if (tpk) for (uint32_t c = 0; c < key.chn; ++c) b200m_tpk_reset (tpk, (int32_t)(slot * key.chn + c), nullptr);
+        if (tpk) for (uint32_t c = 0; c < key.chn; ++c) b200m_tpk_clear (tpk, (int32_t)(slot * key.chn + c), nullptr);
+        const uint32_t pairs_per_slot = key.family == K_SUR ? 4 : 1;
+        if (cor) for (uint32_t c = 0; c < pairs_per_slot; ++c) b200m_cor_clear (cor, (int32_t)(slot * pairs_per_slot + c), nullptr);
+        if (ppm) {
+            if (key.family == K_BBCM6) { b200m_ppm_clear (ppm, (int32_t)slot, nullptr); s_gain[slot] = -6.0f; }
+            else for (uint32_t c = 0; c < key.chn; ++c) b200m_ppm_clear (ppm, (int32_t)(slot * key.chn + c), nullptr);
+        }
+        if (spec) { b200m_spec_clear (spec, (int32_t)slot, nullptr); spec_ctl[2 * slot] = 1.0f; spec_ctl[2 * slot + 1] = -4.0f; }
+        if (!sur_sel.empty ()) memset (&sur_sel[8 * slot], SUR_IDLE, 8);
     }
+    void vacate (uint32_t slot) override { clear (slot); }
 };
 
-// one cycle of a batched instance: collect the previous cycle's results of this slot, hand in this cycle's audio, launch when complete
-void shub_cycle (Shim* s, const float* const* in, uint32_t n, b200m_tpk_result* tr, float* fr, uint32_t nf)
+// one cycle of a batched instance: collect the previous cycle's results of this slot, store its controls, hand in this cycle's
+// audio, launch when complete.  ctl: spectr30 {speed, reset}, BBCM6 {S gain}, surround uint8_t[8] pair rows; NULL for the others.
+void shub_cycle (Shim* s, const float* const* in, uint32_t n, b200m_tpk_result* tr, float* fr, uint32_t nf, const void* ctl = nullptr)
 {
     ShimHub* hub = s->hub;
     const uint32_t chn = hub->key.chn;
@@ -118,7 +160,10 @@ void shub_cycle (Shim* s, const float* const* in, uint32_t n, b200m_tpk_result* 
     hub->close_if_broken (s->slot, n);
     if (tr) for (uint32_t c = 0; c < chn; ++c) tr[c] = hub->tpk_res[(size_t)s->slot * chn + c];
     if (fr) for (uint32_t k = 0; k < nf; ++k) fr[k] = hub->f_res[(size_t)s->slot * nf + k];
-    if (s->kind == K_SPEC) { hub->spec_speed = *s->port[SA_SPEED]; hub->spec_reset = *s->port[SA_RESET]; }   // before a launch by this submit
+    // before a launch by this submit; a member that misses a cycle keeps its previous controls
+    if (s->kind == K_SPEC) memcpy (&hub->spec_ctl[2 * s->slot], ctl, 2 * sizeof (float));
+    else if (s->kind == K_BBCM6) hub->s_gain[s->slot] = *(const float*)ctl;
+    else if (s->kind == K_SUR) memcpy (&hub->sur_sel[8 * s->slot], ctl, 8);
     hub->submit (s->slot, in, n);
 }
 
@@ -141,8 +186,8 @@ LV2_Handle shim_instantiate (const LV2_Descriptor* d, double rate, const char*, 
     else if (!strncmp (u, "spectr30", 8)) { s->kind = K_SPEC; s->chn = strstr (u, "stereo") ? 2 : 1; }
     else known = false;
     int rc = known ? 0 : -1;
-    if (known && s->kind != K_BBCM6 && s->kind != K_SUR)
-        s->hub = (ShimHub*)SlotHub::join (HubKey{s->kind, ppm_kind, s->chn, tpk_flags, rate}, s, &s->slot, ShimHub::create);
+    if (known) s->hub = (ShimHub*)SlotHub::join (HubKey{s->kind, ppm_kind, s->chn, tpk_flags, rate}, s, &s->slot, ShimHub::create);
+    if (s->hub) { std::lock_guard<std::mutex> lh (s->hub->mu); s->hub->clear ((uint32_t)s->slot); }
     if (known && !s->hub) {                                    // a private bank of one instance unless batched mode puts it into a shared one
         switch (s->kind) {
         case K_COR: rc = b200m_cor_create (&s->cor, 0, 1, (int)rate, 2e3f, 0.3f); break;
@@ -259,12 +304,14 @@ void run_needle (Shim* s, uint32_t off, uint32_t n)
     const float r = *s->port[MTR_REFLEVEL];
     if (s->p_refl != r) { s->p_refl = r; s->rlgain = powf (10.0f, 0.05f * (s->p_refl + 18.0)); }
     float* in[2] = {s->port[MTR_INPUT0] + off, s->chn == 2 ? s->port[MTR_INPUT1] + off : nullptr};
+    float s_gain = -6;
     if (s->kind == K_BBCM6) {
         const bool s20 = (*s->port[MTR_PEAK0] > 0.5) ? true : false;           // port 7
-        b200m_ppm_set_gain (s->ppm, -6, s20 ? +14 : -6);
+        s_gain = s20 ? +14 : -6;
+        if (!s->hub) b200m_ppm_set_gain (s->ppm, -6, s_gain);
     }
     float v[2] = {0, 0};
-    if (s->hub) shub_cycle (s, in, n, nullptr, v, s->chn);
+    if (s->hub) shub_cycle (s, in, n, nullptr, v, s->chn, &s_gain);
     else if (!s->stage.fill (in, s->chn, n) || b200m_ppm_process_host (s->ppm, s->stage.data, s->stage.cap, n) || b200m_ppm_read_device (s->ppm, nullptr) ||
              b200m_ppm_results (s->ppm, v, nullptr)) return;
     *s->port[MTR_LEVEL0] = s->rlgain * v[0];
@@ -275,7 +322,8 @@ void run_spec (Shim* s, uint32_t off, uint32_t n)
 {
     float* in[2] = {s->port[SA_INPUT0] + off, s->chn == 2 ? s->port[SA_INPUT1] + off : nullptr};
     float ports[60];
-    if (s->hub) shub_cycle (s, in, n, nullptr, ports, 60);
+    const float ctl[2] = {*s->port[SA_SPEED], *s->port[SA_RESET]};
+    if (s->hub) shub_cycle (s, in, n, nullptr, ports, 60, ctl);
     else if (!s->stage.fill (in, s->chn, n) || b200m_spec_process_host (s->spec, s->stage.data, s->stage.cap, n, *s->port[SA_SPEED], *s->port[SA_RESET]) ||
              b200m_spec_results (s->spec, ports, nullptr)) return;
     for (int i = 0; i < 30; ++i) {
@@ -290,21 +338,26 @@ void run_sur (Shim* s, uint32_t off, uint32_t n)
     float* in[8];
     for (uint32_t c = 0; c < s->chn; ++c) { in[c] = s->port[13 + 4 * c]; if (!in[c]) return; in[c] += off; }
     const uint32_t cors = s->chn > 3 ? 4 : 3;
-    const float* pair[8] = {nullptr};                      // NULL rows stage silence: cor4[3] idles on a 3-channel meter
+    uint8_t sel[8];                                        // SUR_IDLE rows stage silence: cor4[3] idles on a 3-channel meter
+    memset (sel, SUR_IDLE, sizeof (sel));
     for (uint32_t c = 0; c < cors; ++c) {
         if (!s->port[1 + 3 * c] || !s->port[2 + 3 * c]) continue;
         uint32_t in_a = (uint32_t)rintf (*s->port[1 + 3 * c]), in_b = (uint32_t)rintf (*s->port[2 + 3 * c]);
         if (in_a >= s->chn) in_a = s->chn - 1;
         if (in_b >= s->chn) in_b = s->chn - 1;
-        pair[2 * c] = in[in_a]; pair[2 * c + 1] = in[in_b];
+        sel[2 * c] = (uint8_t)in_a; sel[2 * c + 1] = (uint8_t)in_b;
     }
     float cv[4] = {0, 0, 0, 0};
-    if (!s->stage2.fill (pair, 8, n) || b200m_cor_process_host (s->cor, s->stage2.data, s->stage2.cap, n) || b200m_cor_results (s->cor, cv, nullptr)) return;
-    for (uint32_t c = 0; c < cors; ++c) if (s->port[3 + 3 * c]) *s->port[3 + 3 * c] = cv[c];
-    if (!s->stage.fill (in, s->chn, n)) return;
     b200m_tpk_result r[8];
-    if (b200m_tpk_process_host (s->tpk, s->stage.data, s->stage.cap, n, B200M_TP_MODE_PROCESS) || b200m_tpk_read_device (s->tpk, nullptr) ||
-        b200m_tpk_results (s->tpk, r, nullptr)) return;
+    if (s->hub) shub_cycle (s, in, n, r, cv, 4, sel);
+    else {
+        const float* pair[8];
+        for (int k = 0; k < 8; ++k) pair[k] = sel[k] == SUR_IDLE ? nullptr : in[sel[k]];
+        if (!s->stage2.fill (pair, 8, n) || b200m_cor_process_host (s->cor, s->stage2.data, s->stage2.cap, n) || b200m_cor_results (s->cor, cv, nullptr)) return;
+    }
+    for (uint32_t c = 0; c < cors; ++c) if (s->port[3 + 3 * c]) *s->port[3 + 3 * c] = cv[c];
+    if (!s->hub && (!s->stage.fill (in, s->chn, n) || b200m_tpk_process_host (s->tpk, s->stage.data, s->stage.cap, n, B200M_TP_MODE_PROCESS) ||
+                    b200m_tpk_read_device (s->tpk, nullptr) || b200m_tpk_results (s->tpk, r, nullptr))) return;
     for (uint32_t c = 0; c < s->chn; ++c) {
         if (s->port[15 + 4 * c]) *s->port[15 + 4 * c] = r[c].km_rms;         // Kmeterdsp::read (m, p): *level = m, *peak = p
         if (s->port[16 + 4 * c]) *s->port[16 + 4 * c] = r[c].km_peak;

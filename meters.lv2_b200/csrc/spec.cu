@@ -12,6 +12,7 @@
 #include <math.h>
 #include <stdlib.h>
 #include <complex>
+#include <vector>
 #include "common.cuh"
 
 namespace b200m {
@@ -20,7 +21,10 @@ constexpr int SPEC_BANDS = 30;
 constexpr int SPEC_TC = 64;               // frames per staged chunk
 constexpr int SPEC_WARPS = 4;             // instances per CTA
 
-struct SpecRun { float omega; int ac0; int clear_max; int reinit_gui; int nchan; };
+struct SpecRun { int ac0; int nchan; };
+// per-instance run parameters of one call, designed on the host from the instance's control ports (spec_control)
+struct SpecCtl { float omega; int flags; };
+constexpr int SPEC_CLEAR_MAX = 1, SPEC_REINIT_GUI = 2, SPEC_PARITY = 4;   // SPEC_PARITY: the instance's `ac` phase against the bank's frame count
 
 // coef[band][16]: stage0 {b0,b1,b2,a1,a2}, stages 1..5 {a1,a2}; pad to 16
 // FMA = B200M_PREC_FMA: the same transposed-DF-II cascade with fused multiply-adds (25 instead of 39 fp64 instructions per frame and
@@ -28,7 +32,7 @@ struct SpecRun { float omega; int ac0; int clear_max; int reinit_gui; int nchan;
 // contract's +-1e-4 dB (tests/test_cor_spec_gpu.py::test_spec_fma_mode_within_tolerance).
 template <bool FMA>
 __global__ void __launch_bounds__ (SPEC_WARPS * 32)
-spec_kernel (const float* __restrict__ in, size_t stride, int n_inst, int nfram, SpecRun rp, const double* __restrict__ coef,
+spec_kernel (const float* __restrict__ in, size_t stride, int n_inst, int nfram, SpecRun rp, const SpecCtl* __restrict__ ctl, const double* __restrict__ coef,
              double* __restrict__ zst /* [inst][12][32] */, float* __restrict__ valf /* [inst][2][32] */, float* __restrict__ ports /* [inst][60] */)
 {
     __shared__ float raw[SPEC_WARPS][2][2][SPEC_TC];      // [warp][stage][channel][frame]
@@ -67,8 +71,10 @@ spec_kernel (const float* __restrict__ in, size_t stride, int n_inst, int nfram,
 #pragma unroll
     for (int s = 0; s < 6; ++s) { z1[s] = zp[(2 * s) * 32]; z2[s] = zp[(2 * s + 1) * 32]; }
     float val = valf[(size_t)inst * 64 + lane], mx = valf[(size_t)inst * 64 + 32 + lane];
-    if (rp.clear_max) mx = 0.0f;                           // peak-hold reset (src/spectrumlv2.c:192-203)
-    const float omega = rp.omega;
+    const SpecCtl cp = ctl[inst];
+    if (cp.flags & SPEC_CLEAR_MAX) mx = 0.0f;              // peak-hold reset (src/spectrumlv2.c:192-203)
+    const float omega = cp.omega;
+    const int ac0 = rp.ac0 ^ ((cp.flags & SPEC_PARITY) ? 1 : 0);
 
     for (int c = 0; c < nchunks; ++c) {
         const int s0 = c * SPEC_TC;
@@ -81,7 +87,7 @@ spec_kernel (const float* __restrict__ in, size_t stride, int n_inst, int nfram,
             const int j = lane + 32 * h;
             const float l = raw[w][c & 1][0][j], r = raw[w][c & 1][1][j];
             const float x = rp.nchan == 2 ? __fmul_rn (__fadd_rn (l, r), 0.5f) : l;      // x/2.0f == x*0.5f exactly
-            const bool ac = (((rp.ac0 + s0 + j) & 1) == 0);
+            const bool ac = (((ac0 + s0 + j) & 1) == 0);
             dd[w][j] = __dadd_rn ((double)x, ac ? 1e-12 : -1e-12);
         }
         __syncwarp ();
@@ -148,7 +154,7 @@ spec_kernel (const float* __restrict__ in, size_t stride, int n_inst, int nfram,
         ports[(size_t)inst * 60 + lane] = vs > .00001f ? __double2float_rn (__dmul_rn (20.0, (double)log10f_glibc (vs))) : -100.0f;
         // while a peak-reset handshake is pending the reference emits -500 - (rand() & 0xffff) to force a
         // GUI parameter change (:243-246); the engine emits the deterministic -500
-        ports[(size_t)inst * 60 + 30 + lane] = rp.reinit_gui ? -500.0f
+        ports[(size_t)inst * 60 + 30 + lane] = (cp.flags & SPEC_REINIT_GUI) ? -500.0f
                                              : (ms > .00001f ? __double2float_rn (__dmul_rn (20.0, (double)log10f_glibc (ms))) : -100.0f);
     }
 }
@@ -159,7 +165,10 @@ using namespace b200m;
 
 struct b200m_spec {
     int device; uint32_t n_inst, nchan; double rate;
-    float rst_h, spd_h, omega; uint64_t frames;           // uniform control state (src/spectrumlv2.c:52-62)
+    uint64_t frames;                                      // frames processed by the bank: the `ac` phase of an instance never cleared
+    std::vector<float> rst_h, spd_h;                      // per-instance control state (src/spectrumlv2.c:52-62)
+    std::vector<SpecCtl> ctl;                             // host copy of d_ctl; [ctl_lo, ctl_hi) not uploaded yet
+    SpecCtl* d_ctl = nullptr; uint32_t ctl_lo = 0, ctl_hi = 0;
     double W[30][6][6];                                   // a0 a1 a2 b0 b1 b2 per stage, as the reference stores them
     double *d_coef = nullptr, *d_z = nullptr; float *d_val = nullptr, *d_ports = nullptr;
     cudaStream_t own = nullptr; HostStage stage; bool last_host = false;
@@ -240,30 +249,59 @@ static float spec_omega (float speed, double rate)
 
 static cudaStream_t spec_stream (b200m_spec* h, void* stream) { return h->last_host ? h->own : (cudaStream_t)stream; }
 
-static int spec_process (b200m_spec* h, const float* d_in, size_t stride, uint32_t nfram, float speed, float reset, cudaStream_t st)
+// control-port handling at the top of spectrum_run (:170-205) for one instance: updates its state, returns its run parameters
+static SpecCtl spec_control (b200m_spec* h, uint32_t i, float speed, float reset)
 {
-    // control-port handling at the top of spectrum_run (:170-205), uniform over the bank
-    SpecRun rp; rp.clear_max = 0; rp.reinit_gui = 0; rp.nchan = (int)h->nchan;
-    if (h->spd_h != speed) {
-        h->spd_h = speed;
-        float v = h->spd_h;
+    SpecCtl c = {h->ctl[i].omega, h->ctl[i].flags & SPEC_PARITY};
+    if (h->spd_h[i] != speed) {
+        h->spd_h[i] = speed;
+        float v = h->spd_h[i];
         if (v < 0.01) v = 0.01;
         if (v > 15.0) v = 15.0;
-        h->omega = spec_omega (v, h->rate);
-        h->rst_h = 0;
+        c.omega = spec_omega (v, h->rate);
+        h->rst_h[i] = 0;
     }
-    if (h->rst_h != reset) {
-        if (fabsf (reset) < 3 || h->rst_h == 0) { rp.reinit_gui = 1; rp.clear_max = 1; }
-        if (fabsf (reset) != 3) h->rst_h = reset;
+    if (h->rst_h[i] != reset) {
+        if (fabsf (reset) < 3 || h->rst_h[i] == 0) c.flags |= SPEC_REINIT_GUI | SPEC_CLEAR_MAX;
+        if (fabsf (reset) != 3) h->rst_h[i] = reset;
     }
-    if (fabsf (reset) == 3) rp.reinit_gui = 1;
-    rp.omega = h->omega;
+    if (fabsf (reset) == 3) c.flags |= SPEC_REINIT_GUI;
+    return c;
+}
+
+static void spec_mark (b200m_spec* h, uint32_t lo, uint32_t hi)
+{
+    if (h->ctl_lo >= h->ctl_hi) { h->ctl_lo = lo; h->ctl_hi = hi; }
+    else { if (lo < h->ctl_lo) h->ctl_lo = lo; if (hi > h->ctl_hi) h->ctl_hi = hi; }
+}
+
+// an instance as b200m_spec_create leaves it (:95-98): rst_h = -4, spd_h = 1, `ac` from false at its next frame
+static void spec_reset_ctl (b200m_spec* h, uint32_t i)
+{
+    h->rst_h[i] = -4; h->spd_h[i] = 1.0f;
+    h->ctl[i].omega = spec_omega (1.0f, h->rate);
+    h->ctl[i].flags = (h->frames & 1) ? SPEC_PARITY : 0;
+}
+
+// ctl[i * cstride] = {speed, reset} of instance i; cstride = 0: the same pair for every instance.  Only the instances whose run
+// parameters changed are uploaded (one copy of the changed range, on the call's stream).
+static int spec_process (b200m_spec* h, const float* d_in, size_t stride, uint32_t nfram, const float* ctl, size_t cstride, cudaStream_t st)
+{
+    for (uint32_t i = 0; i < h->n_inst; ++i) {
+        const SpecCtl c = spec_control (h, i, ctl[i * cstride], ctl[i * cstride + 1]);
+        if (memcmp (&c, &h->ctl[i], sizeof (c))) { h->ctl[i] = c; spec_mark (h, i, i + 1); }
+    }
+    if (h->ctl_lo < h->ctl_hi) {
+        B200M_CUDA (cudaMemcpyAsync (h->d_ctl + h->ctl_lo, h->ctl.data () + h->ctl_lo, (h->ctl_hi - h->ctl_lo) * sizeof (SpecCtl), cudaMemcpyHostToDevice, st));
+        h->ctl_lo = h->ctl_hi = 0;
+    }
+    SpecRun rp; rp.nchan = (int)h->nchan;
     rp.ac0 = (int)(h->frames & 1);
     h->frames += nfram;
     if (h->fma) spec_kernel<true><<<(h->n_inst + SPEC_WARPS - 1) / SPEC_WARPS, SPEC_WARPS * 32, 0, st>>> (
-        d_in, stride, (int)h->n_inst, (int)nfram, rp, h->d_coef, h->d_z, h->d_val, h->d_ports);
+        d_in, stride, (int)h->n_inst, (int)nfram, rp, h->d_ctl, h->d_coef, h->d_z, h->d_val, h->d_ports);
     else spec_kernel<false><<<(h->n_inst + SPEC_WARPS - 1) / SPEC_WARPS, SPEC_WARPS * 32, 0, st>>> (
-        d_in, stride, (int)h->n_inst, (int)nfram, rp, h->d_coef, h->d_z, h->d_val, h->d_ports);
+        d_in, stride, (int)h->n_inst, (int)nfram, rp, h->d_ctl, h->d_coef, h->d_z, h->d_val, h->d_ports);
     B200M_LAUNCHED (1);
     B200M_CUDA (cudaGetLastError ());
     return 0;
@@ -288,9 +326,9 @@ int b200m_spec_create (b200m_spec** out, int device, uint32_t n_inst, uint32_t n
     if (!g.ok) return set_err (B200M_E_NODEVICE, "cannot select CUDA device %d", device);
     b200m_spec* h = new (std::nothrow) b200m_spec;
     if (!h) return set_err (B200M_E_NOMEM, "host allocation failed");
-    h->device = device; h->n_inst = n_inst; h->nchan = nchan; h->rate = rate;
-    h->rst_h = -4; h->spd_h = 1.0; h->frames = 0;       // :95-98
-    h->omega = spec_omega (h->spd_h, rate);
+    h->device = device; h->n_inst = n_inst; h->nchan = nchan; h->rate = rate; h->frames = 0;
+    h->rst_h.resize (n_inst); h->spd_h.resize (n_inst); h->ctl.resize (n_inst);
+    for (uint32_t i = 0; i < n_inst; ++i) spec_reset_ctl (h, i);
     double coef[SPEC_BANDS][16];
     memset (coef, 0, sizeof (coef));
     design_bank (h->W, rate);
@@ -304,7 +342,9 @@ int b200m_spec_create (b200m_spec** out, int device, uint32_t n_inst, uint32_t n
     A ((void**)&h->d_z, (size_t)n_inst * 12 * 32 * sizeof (double));
     A ((void**)&h->d_val, (size_t)n_inst * 64 * sizeof (float));
     A ((void**)&h->d_ports, (size_t)n_inst * 60 * sizeof (float));
+    A ((void**)&h->d_ctl, (size_t)n_inst * sizeof (SpecCtl));
     if (e == cudaSuccess) e = cudaMemcpy (h->d_coef, coef, sizeof (coef), cudaMemcpyHostToDevice);
+    if (e == cudaSuccess) e = cudaMemcpy (h->d_ctl, h->ctl.data (), (size_t)n_inst * sizeof (SpecCtl), cudaMemcpyHostToDevice);
     if (e == cudaSuccess) e = cudaStreamCreateWithFlags (&h->own, cudaStreamNonBlocking);
     if (e != cudaSuccess) { int rc = cuda_fail (e, "spec_create", __FILE__, __LINE__); b200m_spec_destroy (h); return rc; }
     *out = h;
@@ -316,10 +356,19 @@ int b200m_spec_destroy (b200m_spec* h)
     if (!h) return 0;
     DeviceGuard g (h->device);
     cudaDeviceSynchronize ();
-    cudaFree (h->d_coef); cudaFree (h->d_z); cudaFree (h->d_val); cudaFree (h->d_ports); h->stage.release ();
+    cudaFree (h->d_coef); cudaFree (h->d_z); cudaFree (h->d_val); cudaFree (h->d_ports); cudaFree (h->d_ctl); h->stage.release ();
     if (h->own) cudaStreamDestroy (h->own);
     delete h;
     return 0;
+}
+
+int b200m_spec_process_ctl_device (b200m_spec* h, const float* d_in, size_t stride, uint32_t nfram, const float* ctl, void* stream)
+{
+    if (int rc = check_block_args (h, d_in, stride, nfram)) return rc;
+    if (!ctl) return set_err (B200M_E_INVAL, "NULL ctl");
+    DeviceGuard g (h->device);
+    h->last_host = false;
+    return spec_process (h, d_in, stride, nfram, ctl, 2, (cudaStream_t)stream);
 }
 
 int b200m_spec_process_device (b200m_spec* h, const float* d_in, size_t stride, uint32_t nfram, float speed, float reset, void* stream)
@@ -327,10 +376,11 @@ int b200m_spec_process_device (b200m_spec* h, const float* d_in, size_t stride, 
     if (int rc = check_block_args (h, d_in, stride, nfram)) return rc;
     DeviceGuard g (h->device);
     h->last_host = false;
-    return spec_process (h, d_in, stride, nfram, speed, reset, (cudaStream_t)stream);
+    const float c[2] = {speed, reset};
+    return spec_process (h, d_in, stride, nfram, c, 0, (cudaStream_t)stream);
 }
 
-int b200m_spec_process_host (b200m_spec* h, const float* in, size_t stride, uint32_t nfram, float speed, float reset)
+static int spec_process_host (b200m_spec* h, const float* in, size_t stride, uint32_t nfram, const float* ctl, size_t cstride)
 {
     if (int rc = check_block_args (h, in, stride, nfram)) return rc;
     DeviceGuard g (h->device);
@@ -340,7 +390,34 @@ int b200m_spec_process_host (b200m_spec* h, const float* in, size_t stride, uint
     B200M_CUDA (cudaMemcpy2DAsync (h->stage.d, h->stage.cap * sizeof (float), in, stride * sizeof (float),
                                    (size_t)nfram * sizeof (float), nch, cudaMemcpyHostToDevice, h->own));
     h->last_host = true;
-    return spec_process (h, h->stage.d, h->stage.cap, nfram, speed, reset, h->own);
+    return spec_process (h, h->stage.d, h->stage.cap, nfram, ctl, cstride, h->own);
+}
+
+int b200m_spec_process_ctl_host (b200m_spec* h, const float* in, size_t stride, uint32_t nfram, const float* ctl)
+{
+    if (!ctl) return set_err (B200M_E_INVAL, "NULL ctl");
+    return spec_process_host (h, in, stride, nfram, ctl, 2);
+}
+
+int b200m_spec_process_host (b200m_spec* h, const float* in, size_t stride, uint32_t nfram, float speed, float reset)
+{
+    const float c[2] = {speed, reset};
+    return spec_process_host (h, in, stride, nfram, c, 0);
+}
+
+int b200m_spec_clear (b200m_spec* h, int32_t inst, void* stream)
+{
+    if (!h || inst < -1 || inst >= (int32_t)h->n_inst) return set_err (B200M_E_INVAL, "bad argument");
+    DeviceGuard g (h->device);
+    cudaStream_t st = spec_stream (h, stream);
+    const uint32_t i0 = inst < 0 ? 0 : (uint32_t)inst, n = inst < 0 ? h->n_inst : 1;
+    // filter states, val / max and the ports as b200m_spec_create zeroes them
+    B200M_CUDA (cudaMemsetAsync (h->d_z + (size_t)i0 * 12 * 32, 0, (size_t)n * 12 * 32 * sizeof (double), st));
+    B200M_CUDA (cudaMemsetAsync (h->d_val + (size_t)i0 * 64, 0, (size_t)n * 64 * sizeof (float), st));
+    B200M_CUDA (cudaMemsetAsync (h->d_ports + (size_t)i0 * 60, 0, (size_t)n * 60 * sizeof (float), st));
+    for (uint32_t i = i0; i < i0 + n; ++i) spec_reset_ctl (h, i);
+    spec_mark (h, i0, i0 + n);                             // uploaded by the next process call, on its stream
+    return 0;
 }
 
 int b200m_spec_set_precision (b200m_spec* h, int mode)

@@ -15,6 +15,8 @@
  *   needle / COR / dBTP / K-meters (src/meters.cc:59-70): 0 reflevel, 1 in0, 2 out0, 3 level0, 4 in1, 5 out1, 6 level1, 7 peak0, 8 peak1, 9 hold
  *   spectr30 (src/spectrumlv2.c:35-44): 0-59 band / max outputs, 60 speed, 61 reset, 62 amp, 63 state, 64 in0, 65 out0, 66 in1, 67 out1
  *   bitmeter / SigDistHist (src/bitmeter.c, src/sigdistlv2.c port enums): 0 control atom in, 1 notify atom out, 2 in, 3 out
+ *   surround3..8 (src/surmeter.c:24-70): pair c: 1 + 3c, 2 + 3c input selectors, 3 + 3c correlation; channel c: 13 + 4c in, 14 + 4c out,
+ *                15 + 4c level, 16 + 4c peak
  */
 #define _GNU_SOURCE
 #include <dlfcn.h>
@@ -55,7 +57,7 @@ static uint32_t urid_map (void* h, const char* uri)
 
 typedef struct {
     LV2_Handle h;
-    float *in[2], *out[2];
+    float *in[8], *out[8];
     float ctl[68];                          /* control ports (in and out) */
     uint8_t *atom_in, *atom_out;            /* EBUr128, bitmeter, SigDistHist */
 } Inst;
@@ -63,7 +65,7 @@ typedef struct {
 typedef struct { const LV2_Descriptor* d; Inst* inst; int first, last; uint32_t nframes; int kind; uint32_t seq_t, chunk_t; pthread_barrier_t *start, *done; int cycles;
                  int cycle; const uint8_t* first_msgs; uint32_t first_len; } Worker;
 
-enum { KIND_MTR, KIND_EBUR, KIND_SPEC, KIND_STATS };
+enum { KIND_MTR, KIND_EBUR, KIND_SPEC, KIND_STATS, KIND_SUR };
 #define ATOM_CAP 8192
 
 /* one event at frame 0: object {otype; controlkey = key (Int); controlval = val (Float)} -- forge_kvcontrolmessage, src/uris.h:279-294 */
@@ -137,8 +139,9 @@ int main (int argc, char** argv)
     for (uint32_t i = 0; (d = get (i)) != NULL; ++i) if (!strcmp (d->URI, full)) break;
     if (!d) { fprintf (stderr, "%s not served by %s\n", full, lib); return 1; }
     const int kind = !strcmp (uri, "EBUr128") ? KIND_EBUR : !strncmp (uri, "spectr30", 8) ? KIND_SPEC
-                   : !strcmp (uri, "bitmeter") || !strcmp (uri, "SigDistHist") ? KIND_STATS : KIND_MTR;
+                   : !strcmp (uri, "bitmeter") || !strcmp (uri, "SigDistHist") ? KIND_STATS : !strncmp (uri, "surround", 8) ? KIND_SUR : KIND_MTR;
     const int stereo = kind == KIND_EBUR || strstr (uri, "stereo") || !strcmp (uri, "COR") || !strcmp (uri, "BBCM6");
+    const int chn = kind == KIND_SUR ? uri[8] - '0' : stereo ? 2 : 1;
 
     LV2_URID_Map map = {NULL, urid_map};
     LV2_Feature fmap = {"http://lv2plug.in/ns/ext/urid#map", &map};
@@ -162,7 +165,7 @@ int main (int argc, char** argv)
         Inst* p = &inst[i];
         p->h = d->instantiate (d, rate, "", feats);
         if (!p->h) { fprintf (stderr, "instantiate failed at instance %d (no GPU? B200M_LV2_BATCH smaller than --instances is fine: more hubs are made)\n", i); return 1; }
-        for (int c = 0; c < 2; ++c) {
+        for (int c = 0; c < chn; ++c) {
             p->in[c] = (float*)malloc (sizeof (float) * nframes); p->out[c] = (float*)malloc (sizeof (float) * nframes);
             for (uint32_t k = 0; k < nframes; ++k) { s ^= s << 13; s ^= s >> 7; s ^= s << 17; p->in[c][k] = ((float)(s >> 40) * (1.0f / 8388608.0f) - 1.0f) * 0.25f; }
         }
@@ -176,6 +179,13 @@ int main (int argc, char** argv)
             p->ctl[60] = 1.0f; p->ctl[61] = -4.0f; p->ctl[62] = 0.0f;
             d->connect_port (p->h, 64, p->in[0]); d->connect_port (p->h, 65, p->out[0]);
             if (stereo) { d->connect_port (p->h, 66, p->in[1]); d->connect_port (p->h, 67, p->out[1]); }
+        } else if (kind == KIND_SUR) {
+            for (uint32_t k = 0; k < 13; ++k) d->connect_port (p->h, k, &p->ctl[k]);
+            for (int c = 0; c < 4; ++c) { p->ctl[1 + 3 * c] = (float)c; p->ctl[2 + 3 * c] = (float)((c + 1) % chn); }   /* adjacent channel pairs */
+            for (int c = 0; c < chn; ++c) {
+                d->connect_port (p->h, 13 + 4 * c, p->in[c]); d->connect_port (p->h, 14 + 4 * c, p->out[c]);
+                d->connect_port (p->h, 15 + 4 * c, &p->ctl[15 + 4 * c]); d->connect_port (p->h, 16 + 4 * c, &p->ctl[16 + 4 * c]);
+            }
         } else {
             for (uint32_t k = 0; k < 10; ++k) d->connect_port (p->h, k, &p->ctl[k]);
             p->ctl[0] = -18.0f;
