@@ -15,58 +15,9 @@
 #include <algorithm>
 #include <vector>
 #include "common.cuh"
+#include "ebu_kw.cuh"
 
 namespace b200m {
-
-#ifndef B200M_EBU_TILE
-#define B200M_EBU_TILE 64
-#endif
-#ifndef B200M_EBU_TMA_UNROLL
-#define B200M_EBU_TMA_UNROLL 8
-#endif
-#ifndef B200M_EBU_STAGES
-#define B200M_EBU_STAGES 3
-#endif
-constexpr int EBU_TILE   = B200M_EBU_TILE;   // samples per smem tile (64 or 128)
-constexpr int EBU_ROWP   = EBU_TILE + 4;  // padded row pitch (floats): = 4 mod 32 -> LDS.128 conflict free
-constexpr int EBU_STAGES = B200M_EBU_STAGES; // cp.async pipeline depth (2 tiles = 128 samples in flight per channel)
-static_assert (EBU_TILE == 64 || EBU_TILE == 128, "tile geometry");
-constexpr int EBU_WARPS  = 4;             // warps per CTA: one per SM sub-partition, each an independent 32-channel pipeline
-constexpr int EBU_WARP_FLOATS = EBU_STAGES * 32 * EBU_ROWP;
-constexpr int EBU_SMEM_BYTES = EBU_WARPS * EBU_WARP_FLOATS * 4;
-constexpr int EBU_MAXCHUNK = 32;          // chunks (block/fragment edges) handled per K1 launch
-constexpr int HIST_PITCH = 752;           // 751 bins padded to a 16-byte multiple
-
-struct EbuCoef { float a0, a1, a2, b1, b2, c3, c4; };
-
-struct EbuChunks {                        // bit31: chunk ends a 50 ms fragment
-    int n;
-    uint32_t v[EBU_MAXCHUNK];
-};
-
-// ---- K1: K-weighting recurrence + per-chunk power sums ------------------------------------
-// One warp = 32 consecutive mono channels (lane = channel).  Tiles of [32 ch x 64 samples] are
-// copied global->shared with cp.async (each row of the planar input is contiguous, so every
-// 16-byte copy is fully coalesced), two tiles in flight behind the one being consumed; lane l
-// walks row l with LDS.128, the next float4 always loaded one group ahead (the recurrence is a
-// pure dependent chain: an exposed LDS latency costs as much as two samples).
-// The kernel is bound by per-warp instruction issue, not HBM (DESIGN.md §3): a CTA therefore
-// carries exactly one warp per SM sub-partition.
-B200M_DEV void kw_step (float p, const EbuCoef& c, float& z1, float& z2, float& z3, float& z4, float& sj)
-{
-    // x = p - b1*z1 - b2*z2 + 1e-15f;  y = a0*x + a1*z1 + a2*z2 - c3*z3 - c4*z4   (:321-322)
-    float x = __fsub_rn (p, __fmul_rn (c.b1, z1));
-    x = __fsub_rn (x, __fmul_rn (c.b2, z2));
-    x = __fadd_rn (x, 1e-15f);
-    float y = __fadd_rn (__fmul_rn (c.a0, x), __fmul_rn (c.a1, z1));
-    y = __fadd_rn (y, __fmul_rn (c.a2, z2));
-    y = __fsub_rn (y, __fmul_rn (c.c3, z3));
-    y = __fsub_rn (y, __fmul_rn (c.c4, z4));
-    z2 = z1; z1 = x;
-    z4 = __fadd_rn (z4, z3);
-    z3 = __fadd_rn (z3, y);
-    sj = __fadd_rn (sj, __fmul_rn (y, y));
-}
 
 // ---- staging policies: how a warp's [32 channels x 64 samples] tiles reach shared memory and how lane = channel reads them ----
 
@@ -143,7 +94,6 @@ struct PaddedStage {
 // swizzle) completing on an mbarrier -- no per-lane address arithmetic, no zero-fill logic (out-of-range rows / columns
 // read as 0).  The 128B swizzle stores 16-byte chunk c of row r at chunk c ^ (r & 7), so the eight lanes of an LDS.128
 // phase (rows r..r+7, same logical chunk) hit eight different bank groups: conflict-free without padding.
-B200M_DEV uint32_t smem_u32 (const void* p) { return (uint32_t)__cvta_generic_to_shared (p); }
 
 struct TmaStage {
     static constexpr int UNROLL = B200M_EBU_TMA_UNROLL;       // 8 float4 = one 128-byte row segment: the swizzled offsets are then compile-time
@@ -206,93 +156,6 @@ struct TmaStage {
         return *reinterpret_cast<const float*> (p);
     }
 };
-
-// The recurrence over one block for the 32 channels of a warp; `sg` supplies the tiles.
-template <int NCHAN, class Stage>
-B200M_DEV void kw_warp (Stage& sg, int lane, int k, bool live, int nchans, int nfram, const EbuCoef& cf, const EbuChunks& ck, float fragm_f,
-                        float* __restrict__ zst, float* __restrict__ frpwr, float* __restrict__ fragpw, int n_inst)
-{
-    const int ntiles = (nfram + EBU_TILE - 1) / EBU_TILE;
-    float z1 = zst[0 * (size_t)nchans + k], z2 = zst[1 * (size_t)nchans + k];
-    float z3 = zst[2 * (size_t)nchans + k], z4 = zst[3 * (size_t)nchans + k];
-    const int inst = k / NCHAN;
-    float fp = frpwr[inst];
-    float sj = 0.0f;
-    int ci = 0, nfr = 0;
-    int cend = (int)(ck.v[0] & 0x7fffffffu);           // end position (exclusive) of the current chunk
-    bool cfrag = (ck.v[0] >> 31) != 0;
-
-    // end of one detect_process() call (:324-335): state scrub, channel sum, _frpwr +=, fragment hand-over (:217-221)
-    auto chunk_end = [&] () {
-        z1 = scrub (z1); z2 = scrub (z2); z3 = scrub (z3); z4 = scrub (z4);
-        float si;
-        if (NCHAN == 1) si = __fmul_rn (2.0f, sj);
-        else if (NCHAN == 2) si = __fadd_rn (sj, __shfl_xor_sync (0xffffffffu, sj, 1));   // 1.0f*sjL + 1.0f*sjR
-        else {
-            // si = sum_i _chan_gain[i] * sj_i in channel order, gains 1 1 1 1.41 1.41 (:29,328-329); the instance's lanes are contiguous
-            const int lead = lane - lane % NCHAN;
-            si = __fmul_rn (1.0f, __shfl_sync (0xffffffffu, sj, lead));
-#pragma unroll
-            for (int c = 1; c < NCHAN; ++c) si = __fadd_rn (si, __fmul_rn (c >= 3 ? 1.41f : 1.0f, __shfl_sync (0xffffffffu, sj, (lead + c) & 31)));
-        }
-        fp = __fadd_rn (fp, si);
-        if (cfrag) {
-            if (live && (k % NCHAN) == 0) fragpw[(size_t)nfr * n_inst + inst] = __fdiv_rn (fp, fragm_f);
-            fp = 1e-30f;
-            ++nfr;
-        }
-        sj = 0.0f;
-        ++ci;
-        if (ci < ck.n) { cend = (int)(ck.v[ci] & 0x7fffffffu); cfrag = (ck.v[ci] >> 31) != 0; }
-        else cend = 0x7fffffff;
-    };
-
-    sg.prologue ();
-    for (int t = 0; t < ntiles; ++t) {
-        sg.acquire (t);
-        int a = t * EBU_TILE;
-        const int b = min (a + EBU_TILE, nfram);
-        if (b - a == EBU_TILE && cend >= b) {
-            // fast path: a whole tile inside one chunk; float4 groups with a one-group register prefetch
-            float4 cur = sg.ld4 (t, 0);
-#pragma unroll Stage::UNROLL
-            for (int q = 0; q < EBU_TILE / 4; ++q) {
-                const float4 nxt = sg.ld4 (t, (q + 1) & (EBU_TILE / 4 - 1));
-                kw_step (cur.x, cf, z1, z2, z3, z4, sj);
-                kw_step (cur.y, cf, z1, z2, z3, z4, sj);
-                kw_step (cur.z, cf, z1, z2, z3, z4, sj);
-                kw_step (cur.w, cf, z1, z2, z3, z4, sj);
-                cur = nxt;
-            }
-            a = b;
-            if (a == cend) chunk_end ();
-        } else {
-            while (a < b) {
-                const int e = min (b, cend);
-                int j = a;
-                // scalar head up to a 4-aligned position, vector body, scalar tail
-                for (; j < e && (j & 3); ++j) kw_step (sg.ld (t, j - t * EBU_TILE), cf, z1, z2, z3, z4, sj);
-                for (; j + 4 <= e; j += 4) {
-                    const float4 v = sg.ld4_dyn (t, (j - t * EBU_TILE) >> 2);
-                    kw_step (v.x, cf, z1, z2, z3, z4, sj);
-                    kw_step (v.y, cf, z1, z2, z3, z4, sj);
-                    kw_step (v.z, cf, z1, z2, z3, z4, sj);
-                    kw_step (v.w, cf, z1, z2, z3, z4, sj);
-                }
-                for (; j < e; ++j) kw_step (sg.ld (t, j - t * EBU_TILE), cf, z1, z2, z3, z4, sj);
-                a = e;
-                if (a == cend) chunk_end ();
-            }
-        }
-        sg.release (t);
-    }
-    sg.drain ();
-    if (live) {
-        zst[0 * (size_t)nchans + k] = z1; zst[1 * (size_t)nchans + k] = z2;
-        zst[2 * (size_t)nchans + k] = z3; zst[3 * (size_t)nchans + k] = z4;
-        if ((k % NCHAN) == 0) frpwr[inst] = fp;
-    }
-}
 
 template <int NCHAN, bool ALIGNED>
 __global__ void __launch_bounds__ (EBU_WARPS * 32)
@@ -747,13 +610,19 @@ static TmaEncodeFn tma_encoder ()
     }();
     return fn;
 }
+bool ebu_tma_map (CUtensorMap* tm, const float* base, size_t stride, uint32_t rows, uint32_t cols, uint32_t box_cols, uint32_t box_rows, bool swizzle128)
+{
+    if (!tma_encoder ()) return false;
+    const cuuint64_t gdim[2] = {cols, rows}; const cuuint64_t gstr[1] = {(cuuint64_t)stride * sizeof (float)};
+    const cuuint32_t box[2] = {box_cols, box_rows}, es[2] = {1, 1};
+    return tma_encoder () (tm, CU_TENSOR_MAP_DATA_TYPE_FLOAT32, 2, const_cast<float*> (base), gdim, gstr, box, es, CU_TENSOR_MAP_INTERLEAVE_NONE,
+                           swizzle128 ? CU_TENSOR_MAP_SWIZZLE_128B : CU_TENSOR_MAP_SWIZZLE_NONE, CU_TENSOR_MAP_L2_PROMOTION_L2_128B,
+                           CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE) == CUDA_SUCCESS;
+}
 // [rows x cols] float32 view of the planar input for K1: boxes of 32 rows x 32 floats, 128B swizzle, zeros outside
 static bool tma_input_map (CUtensorMap* tm, const float* base, size_t stride, uint32_t rows, uint32_t cols)
 {
-    const cuuint64_t gdim[2] = {cols, rows}; const cuuint64_t gstr[1] = {(cuuint64_t)stride * sizeof (float)};
-    const cuuint32_t box[2] = {32, 32}, es[2] = {1, 1};
-    return tma_encoder () (tm, CU_TENSOR_MAP_DATA_TYPE_FLOAT32, 2, const_cast<float*> (base), gdim, gstr, box, es, CU_TENSOR_MAP_INTERLEAVE_NONE,
-                           CU_TENSOR_MAP_SWIZZLE_128B, CU_TENSOR_MAP_L2_PROMOTION_L2_128B, CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE) == CUDA_SUCCESS;
+    return ebu_tma_map (tm, base, stride, rows, cols, 32, 32, true);
 }
 
 struct b200m_ebu {
@@ -932,32 +801,54 @@ int b200m_ebu_integr_start (b200m_ebu* h, int32_t inst, void* stream) { return e
 int b200m_ebu_integr_pause (b200m_ebu* h, int32_t inst, void* stream) { return ebu_ctl (h, inst, 0, stream); }
 int b200m_ebu_integr_reset (b200m_ebu* h, int32_t inst, void* stream) { return ebu_ctl (h, inst, 2, stream); }
 
+// Cut the next `rem` frames at fragment edges, at most EBU_MAXCHUNK pieces (one K1 launch, :212-216), advancing the fragment
+// counter `frcnt`; returns the frames the chunk list covers.
+static uint32_t ebu_plan_chunks (int& frcnt, int fragm, uint32_t rem, EbuChunks& ck, int& nfrag)
+{
+    ck.n = 0; nfrag = 0;
+    uint32_t pos = 0;
+    while (pos < rem && ck.n < EBU_MAXCHUNK) {
+        const uint32_t left = rem - pos;
+        const uint32_t k = (uint32_t)frcnt < left ? (uint32_t)frcnt : left;
+        pos += k; frcnt -= (int)k;
+        uint32_t v = pos;
+        if (frcnt == 0) { v |= 0x80000000u; frcnt = fragm; ++nfrag; }
+        ck.v[ck.n++] = v;
+    }
+    return pos;
+}
+
+bool ebu_single_k1 (const b200m_ebu* h, uint32_t nfram)
+{
+    int frcnt = h->frcnt, nfrag; EbuChunks ck;
+    return ebu_plan_chunks (frcnt, h->fragm, nfram, ck, nfrag) == nfram;
+}
+
 // One Ebu_r128_proc::process call for every instance.  `nsl` instance slices [bounds[s], bounds[s+1]) are launched
 // separately, slice s after event ready[s] (the host->device copy of its rows) when `ready` is given; the
 // fragment/gating kernels run once, after the last slice.
+// `k1_fused`, when given (one slice, a block whose chunk list fits one launch: ebu_single_k1), launches a kernel that does
+// K1's work over the whole bank in its place; `after_k1` is enqueued right behind the first K1 launch.
 int ebu_process_sliced (b200m_ebu* h, const float* d_in, size_t stride, uint32_t nfram, cudaStream_t st,
-                        int nsl, const uint32_t* bounds, cudaEvent_t* ready, int (*after_k1) (void*), void* after_arg)
+                        int nsl, const uint32_t* bounds, cudaEvent_t* ready, int (*after_k1) (void*), void* after_arg,
+                        int (*k1_fused) (void*, const EbuK1Args&))
 {
     const int nch = (int)(h->n_inst * h->nchan);
     const bool aligned = ((uintptr_t)d_in % 16 == 0) && (stride % 4 == 0);
     uint32_t done = 0;
     while (done < nfram) {
-        // cut [done, nfram) at fragment edges, at most EBU_MAXCHUNK pieces per launch (:212-216)
-        EbuChunks ck; ck.n = 0;
-        int nfrag = 0; uint32_t pos = 0;
-        while (done + pos < nfram && ck.n < EBU_MAXCHUNK) {
-            const uint32_t rem = nfram - done - pos;
-            const uint32_t k = (uint32_t)h->frcnt < rem ? (uint32_t)h->frcnt : rem;
-            pos += k; h->frcnt -= (int)k;
-            uint32_t v = pos;
-            if (h->frcnt == 0) { v |= 0x80000000u; h->frcnt = h->fragm; ++nfrag; }
-            ck.v[ck.n++] = v;
-        }
+        EbuChunks ck; int nfrag;
+        const uint32_t pos = ebu_plan_chunks (h->frcnt, h->fragm, nfram - done, ck, nfrag);
         const float* src = d_in + done;
+        const bool fused = k1_fused && done == 0 && pos == nfram && nsl == 1 && bounds[0] == 0 && bounds[1] == h->n_inst;
+        if (fused) {
+            const EbuK1Args a = {src, stride, nch, (int)pos, h->cf, ck, (float)h->fragm, h->d_z, h->d_frpwr, h->d_fragpw, (int)h->n_inst};
+            if (int rc = k1_fused (after_arg, a)) return rc;
+        }
         const bool al = aligned && (done % 4 == 0);
         CUtensorMap tmap;
-        const bool tma = al && h->use_tma && h->nchan <= 2 && tma_input_map (&tmap, src, stride, (uint32_t)nch, pos);
-        for (int sl = 0; sl < nsl; ++sl) {
+        const bool tma = !fused && al && h->use_tma && h->nchan <= 2 && tma_input_map (&tmap, src, stride, (uint32_t)nch, pos);
+        for (int sl = 0; !fused && sl < nsl; ++sl) {
             const int kf = (int)(bounds[sl] * h->nchan), ke = (int)(bounds[sl + 1] * h->nchan);
             if (ke <= kf) continue;
             if (ready && done == 0) B200M_CUDA (cudaStreamWaitEvent (st, ready[sl], 0));
@@ -1008,7 +899,7 @@ int ebu_process_sliced (b200m_ebu* h, const float* d_in, size_t stride, uint32_t
 static int ebu_process (b200m_ebu* h, const float* d_in, size_t stride, uint32_t nfram, cudaStream_t st)
 {
     const uint32_t bounds[2] = {0, h->n_inst};
-    return ebu_process_sliced (h, d_in, stride, nfram, st, 1, bounds, nullptr, nullptr, nullptr);
+    return ebu_process_sliced (h, d_in, stride, nfram, st, 1, bounds, nullptr, nullptr, nullptr, nullptr);
 }
 
 int b200m_ebu_process_device (b200m_ebu* h, const float* d_in, size_t stride, uint32_t nfram, void* stream)

@@ -7,6 +7,7 @@
 #include <math.h>
 #include <stdlib.h>
 #include "common.cuh"
+#include "ebu_kw.cuh"
 
 namespace b200m {
 
@@ -15,11 +16,11 @@ __global__ void r128_fill_kernel (int n, float* p, float v) { const int i = bloc
 
 }  // namespace b200m
 
-// sliced process entry points of the two banks (ebu.cu, tpk.cu)
-extern "C" int ebu_process_sliced (b200m_ebu* h, const float* d_in, size_t stride, uint32_t nfram, cudaStream_t st, int nsl, const uint32_t* bounds, cudaEvent_t* ready,
-                                   int (*after_k1) (void*), void* after_arg);
+// sliced process entry point of the true-peak bank and the fused K-weighting + true-peak kernel (tpk.cu); the EBU bank's: ebu_kw.cuh
 int tpk_process_sliced (b200m_tpk* h, const float* d_in, size_t stride, uint32_t nfram, uint32_t tp_mode, cudaStream_t st, int nsl, const uint32_t* bounds, cudaEvent_t* ready,
                         float* r128_tpmax, bool pdl, const void* dr);
+bool tpk_r128_fused_ok (const b200m_tpk* h, const float* d_in, size_t stride, uint32_t nfram);
+int tpk_r128_fused (b200m_tpk* h, const b200m::EbuK1Args& a, float* r128_tpmax, cudaStream_t st);
 
 using namespace b200m;
 
@@ -48,6 +49,13 @@ static int r128_tp_behind_k1 (void* p)
     return tpk_process_sliced (a->h->tpk, a->d_in, a->stride, a->nfram, B200M_TP_MODE_MAX, a->st, 1, a->bc, nullptr, a->h->d_tpmax, true, nullptr);
 }
 
+// device path, fused: one kernel does K1's work and the true-peak maximum over one shared-memory copy of the block (tpk.cu)
+static int r128_fused_k1 (void* p, const EbuK1Args& a)
+{
+    R128Step* s = (R128Step*)p;
+    return tpk_r128_fused (s->h->tpk, a, s->h->d_tpmax, s->st);
+}
+
 static int r128_run (b200m_r128* h, const float* d_in, size_t stride, uint32_t nfram, cudaStream_t st, int nsl, cudaEvent_t* ready)
 {
     uint32_t bi[R128_SLICES + 1], bc[R128_SLICES + 1];
@@ -61,12 +69,17 @@ static int r128_run (b200m_r128* h, const float* d_in, size_t stride, uint32_t n
     //    tp_max hold per instance and ends with griddepcontrol.wait, so everything queued behind it is ordered after both.
     //  * sliced host path (>= 1): true-peak kernels on the side stream, each slice behind its copy event.
     // B200M_R128_CONCURRENT=0 serialises everything on one stream.
-    const bool pdl = h->dbtp && h->concurrent >= 2 && !ready;
+    // Tolerance mode on the device path runs neither: one fused kernel takes K1's place (r128_fused_kernel, tpk.cu) when the
+    // true-peak bank would take the tensor-core path, the block is 16-byte aligned with nfram % 4 == 0, its chunk list fits one K1
+    // launch and the bank is large enough to fill the GPU with 128-channel slabs.
+    const bool fused = !ready && h->dbtp && tpk_r128_fused_ok (h->tpk, d_in, stride, nfram) && ebu_single_k1 (h->ebu, nfram);
+    const bool pdl = !fused && h->dbtp && h->concurrent >= 2 && !ready;
     const bool conc = h->dbtp && h->concurrent >= 1 && ready;
     R128Step step = {h, d_in, stride, nfram, st, bc};
-    if (int rc = ebu_process_sliced (h->ebu, d_in, stride, nfram, st, nsl, bi, ready, pdl ? r128_tp_behind_k1 : nullptr, &step)) return rc;
+    if (int rc = ebu_process_sliced (h->ebu, d_in, stride, nfram, st, nsl, bi, ready, pdl ? r128_tp_behind_k1 : nullptr, &step,
+                                     fused ? r128_fused_k1 : nullptr)) return rc;
     if (h->dbtp) {
-        if (!pdl) {
+        if (!pdl && !fused) {
             if (int rc = tpk_process_sliced (h->tpk, d_in, stride, nfram, B200M_TP_MODE_MAX, conc ? h->side : st, nsl, bc, conc ? ready : nullptr, h->d_tpmax, false, nullptr)) return rc;
             if (conc) { B200M_CUDA (cudaEventRecord (h->ev_tp, h->side)); B200M_CUDA (cudaStreamWaitEvent (st, h->ev_tp, 0)); }
         }

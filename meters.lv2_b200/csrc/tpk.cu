@@ -22,6 +22,7 @@
 #include <algorithm>
 #include "common.cuh"
 #include "tpk_internal.cuh"
+#include "ebu_kw.cuh"
 
 namespace b200m {
 
@@ -1540,6 +1541,72 @@ B200M_DEV void tcf_wgmma_n48 (float (&d)[48], const uint32_t (&a)[4], uint64_t d
                   : "r"(a[0]), "r"(a[1]), "r"(a[2]), "r"(a[3]), "l"(db), "r"(scale_d) : "memory");
 }
 
+// ---- the tile arithmetic, shared by tpmax_tc_kernel and r128_fused_kernel: one thread's part of one 64-row tile, rows g and g + 8
+// of its warp, which are two consecutive 16-sample blocks of one channel.  xw = window element t of row g in the input stage.
+// A fragment of K step s: a0 = A[g][8s + t], a1 = A[g + 8][8s + t], a2 = A[g][8s + t + 4], a3 = A[g + 8][8s + t + 4]
+B200M_DEV void tcf_load (const float* xw, float (&v)[8][4])
+{
+#pragma unroll
+    for (int s = 0; s < 8; ++s) { v[s][0] = xw[8 * s]; v[s][1] = xw[16 + 8 * s]; v[s][2] = xw[8 * s + 4]; v[s][3] = xw[16 + 8 * s + 4]; }
+}
+// window elements k >= nin[h] (row g: h = 0, row g + 8: h = 1) lie beyond the block's end, where the stage holds stale data: zeroed.
+// Returns phase 0's maximum: |window element 24 + j| over the valid output positions j < vj[h].
+B200M_DEV float tcf_mask_p0 (float (&v)[8][4], int t, const int (&vj)[2], const int (&nin)[2])
+{
+    if (nin[1] < 64) {
+#pragma unroll
+        for (int s = 0; s < 8; ++s)
+#pragma unroll
+            for (int e = 0; e < 4; ++e)
+                if (8 * s + t + 4 * (e >> 1) >= nin[e & 1]) v[s][e] = 0.0f;
+    }
+    float p0 = 0.0f;
+#pragma unroll
+    for (int s = 3; s < 5; ++s)
+#pragma unroll
+        for (int e = 0; e < 4; ++e)
+            if (8 * (s - 3) + t + 4 * (e >> 1) < vj[e & 1]) p0 = fmaxf (p0, fabsf (v[s][e]));
+    return p0;
+}
+// x = hi + lo: hi = the top 11 significand bits (what a tf32 operand keeps), lo = the exact remainder
+B200M_DEV void tcf_split (const float (&v)[8][4], uint32_t (&ahi)[8][4], uint32_t (&alo)[8][4])
+{
+#pragma unroll
+    for (int s = 0; s < 8; ++s)
+#pragma unroll
+        for (int e = 0; e < 4; ++e) {
+            const uint32_t hbits = __float_as_uint (v[s][e]) & 0xffffe000u;
+            ahi[s][e] = hbits; alo[s][e] = __float_as_uint (__fsub_rn (v[s][e], __uint_as_float (hbits)));
+        }
+}
+// the tile's 16 wgmmas, committed as one group; the first starts the accumulators with scale-d = 0 (no zeroing moves)
+B200M_DEV void tcf_mma (float (&d)[48], const uint32_t (&ahi)[8][4], const uint32_t (&alo)[8][4], uint32_t bb)
+{
+    asm volatile ("wgmma.fence.sync.aligned;" ::: "memory");
+#pragma unroll
+    for (int s = 0; s < 8; ++s) {
+        const uint64_t db = tcf_desc (bb + 2 * s * TCF_BLBO, TCF_BLBO, 128);
+        tcf_wgmma_n96 (d, ahi[s], db, s == 0 ? 0u : 1u);                 // A_hi x [B_hi | B_lo]
+        tcf_wgmma_n48 (d, alo[s], db, 1u);                               // A_lo x B_hi
+    }
+    asm volatile ("wgmma.commit_group.sync.aligned;" ::: "memory");
+}
+B200M_DEV void tcf_mma_wait () { asm volatile ("wgmma.wait_group.sync.aligned 0;" ::: "memory"); }
+// max (mx, |output|) over the valid positions of rows g and g + 8; accumulator registers: d[4i + e] = (row g, column 8i + 2t + e),
+// d[4i + 2 + e] = (row g + 8, same column), an output is column n + column 48 + n
+B200M_DEV float tcf_tile_max (const float (&d)[48], int t, const int (&vj)[2], float mx)
+{
+#pragma unroll
+    for (int i = 0; i < 6; ++i)
+#pragma unroll
+        for (int e = 0; e < 2; ++e) {
+            const int j = 8 * (i & 1) + 2 * t + e;
+            if (j < vj[0]) mx = fmaxf (mx, fabsf (__fadd_rn (d[4 * i + e], d[4 * (i + 6) + e])));
+            if (j < vj[1]) mx = fmaxf (mx, fabsf (__fadd_rn (d[4 * i + 2 + e], d[4 * (i + 6) + 2 + e])));
+        }
+    return mx;
+}
+
 __global__ void __launch_bounds__ (TCF_THREADS, 1)
 tpmax_tc_kernel (const float* __restrict__ in, size_t stride, int c_first, int n_chan, int nfram, int nchunks, const float* __restrict__ bcanon,
                  TpkState st, float* __restrict__ r128_tpmax)
@@ -1604,10 +1671,8 @@ tpmax_tc_kernel (const float* __restrict__ in, size_t stride, int c_first, int n
             tcf_wait (tcf_smem_u32 (&xfull[sg]), (uint32_t)((it / TCF_XSTAGES) & 1));
             const float* xt = xbuf + (size_t)sg * 8 * TCF_XPITCH;
             const float* xw = xt + g * TCF_XPITCH + 16 * tb0 + t;
-            // fragment of K step s: a0 = A[g][8s + t], a1 = A[g + 8][8s + t], a2 = A[g][8s + t + 4], a3 = A[g + 8][8s + t + 4]
             float v[8][4];
-#pragma unroll
-            for (int s = 0; s < 8; ++s) { v[s][0] = xw[8 * s]; v[s][1] = xw[16 + 8 * s]; v[s][2] = xw[8 * s + 4]; v[s][3] = xw[16 + 8 * s + 4]; }
+            tcf_load (xw, v);
             if (chunk == nchunks - 1 && tid < 96) {
                 // history of the next block = the 48 samples that end this one: stage positions nfram - s0 + j (prefix + chunk >= 48 samples)
                 const int rr = tid / 12, k4 = (tid - 12 * rr) * 4;
@@ -1621,49 +1686,13 @@ tpmax_tc_kernel (const float* __restrict__ in, size_t stride, int c_first, int n
                 vj[h] = min (16, max (0, nfram - (s0 + 16 * (tb0 + h))));
                 nin[h] = nfram - (s0 - 48) - 16 * (tb0 + h);
             }
-            if (nin[1] < 64) {                                                    // the stage holds stale data beyond the block's end
-#pragma unroll
-                for (int s = 0; s < 8; ++s)
-#pragma unroll
-                    for (int e = 0; e < 4; ++e)
-                        if (8 * s + t + 4 * (e >> 1) >= nin[e & 1]) v[s][e] = 0.0f;
-            }
-            float p0 = 0.0f;                                                     // phase 0: window element 24 + j for output position j
-#pragma unroll
-            for (int s = 3; s < 5; ++s)
-#pragma unroll
-                for (int e = 0; e < 4; ++e)
-                    if (8 * (s - 3) + t + 4 * (e >> 1) < vj[e & 1]) p0 = fmaxf (p0, fabsf (v[s][e]));
+            const float p0 = tcf_mask_p0 (v, t, vj, nin);
             uint32_t ahi[8][4], alo[8][4];
-#pragma unroll
-            for (int s = 0; s < 8; ++s)
-#pragma unroll
-                for (int e = 0; e < 4; ++e) {
-                    const uint32_t hbits = __float_as_uint (v[s][e]) & 0xffffe000u;
-                    ahi[s][e] = hbits; alo[s][e] = __float_as_uint (__fsub_rn (v[s][e], __uint_as_float (hbits)));
-                }
+            tcf_split (v, ahi, alo);
             float d[48];
-#pragma unroll
-            for (int i = 0; i < 48; ++i) d[i] = 0.0f;
-            asm volatile ("wgmma.fence.sync.aligned;" ::: "memory");
-#pragma unroll
-            for (int s = 0; s < 8; ++s) {
-                const uint64_t db = tcf_desc (bb + 2 * s * TCF_BLBO, TCF_BLBO, 128);
-                tcf_wgmma_n96 (d, ahi[s], db, 1u);                               // A_hi x [B_hi | B_lo]
-                tcf_wgmma_n48 (d, alo[s], db, 1u);                               // A_lo x B_hi
-            }
-            asm volatile ("wgmma.commit_group.sync.aligned;" ::: "memory");
-            asm volatile ("wgmma.wait_group.sync.aligned 0;" ::: "memory");
-            // accumulator registers: d[4i + e] = (row g, column 8i + 2t + e), d[4i + 2 + e] = (row g + 8, same column)
-            float mx = p0;
-#pragma unroll
-            for (int i = 0; i < 6; ++i)
-#pragma unroll
-                for (int e = 0; e < 2; ++e) {
-                    const int j = 8 * (i & 1) + 2 * t + e;
-                    if (j < vj[0]) mx = fmaxf (mx, fabsf (__fadd_rn (d[4 * i + e], d[4 * (i + 6) + e])));
-                    if (j < vj[1]) mx = fmaxf (mx, fabsf (__fadd_rn (d[4 * i + 2 + e], d[4 * (i + 6) + 2 + e])));
-                }
+            tcf_mma (d, ahi, alo, bb);
+            tcf_mma_wait ();
+            float mx = tcf_tile_max (d, t, vj, p0);
             mx = fmaxf (mx, __shfl_xor_sync (0xffffffffu, mx, 1));
             mx = fmaxf (mx, __shfl_xor_sync (0xffffffffu, mx, 2));
             if (t == 0 && mx > 0.0f) atomicMax (&s_gmax[g], __float_as_uint (mx));
@@ -1700,6 +1729,211 @@ tpmax_tc_kernel (const float* __restrict__ in, size_t stride, int c_first, int n
         // launched with programmatic serialization behind the K-weighting kernel (r128.cu): see tpmax_kernel
         const unsigned dn = atomicAdd (st.done_cnt, 1u);
         if (dn == gridDim.x - 1) { *st.done_cnt = 0u; asm volatile ("griddepcontrol.wait;" ::: "memory"); }
+    }
+}
+
+// ---- the EBUr128 cycle's K-weighting and true-peak maximum in one persistent kernel (tolerance mode, device path, r128.cu) --------
+// One CTA per slab of 128 channels (64 stereo instances; slabs blockIdx.x, + gridDim.x, ...) walks the block in 64-sample stages
+// [128 channels][48 history + 64 new + 4 pad] held in a 3-slot shared-memory ring, so the input is read from HBM once for both jobs.
+//   warps 0-7   two FIR warpgroups.  Per stage the slab is 512 rows (128 channels x 4 blocks of 16 samples) = 8 m64 tiles, four per
+//               warpgroup, computed by tpmax_tc_kernel's tile arithmetic (tcf_*): every maximum is bit-identical to it.  In tile m,
+//               warp w of warpgroup wg takes channel 64 wg + 16 m + 8 (w >> 1) + g in rows g / g + 8 and blocks 2 (w & 1), 2 (w & 1) + 1,
+//               so a thread meets the same four channels in every stage and keeps their running maxima in registers until the slab
+//               ends.  The two warpgroups take turns on the tensor cores (named barriers 2 and 3): one's 16 wgmmas run while the
+//               other loads, splits and reduces.
+//   warps 8-11  K-weighting: kw_warp<2> unchanged (lane = channel) through FusedStage, so the EBU floats stay bit-exact.
+// A slot is refilled by the last of the 12 warps to release it (a shared counter), so no role waits for another to finish reading:
+// stages >= 1 by one 2-D TMA box [128 rows x 116 floats] from sample 64 t - 48 (rows and samples outside the block read as zero),
+// stage 0 by per-row bulk copies of the 48-sample history and the block's first 68 samples.
+// Banks: the row pitch 116 = 20 (mod 32) floats puts the rows g = 0..7 of a fragment load (8 consecutive channels, one column) at
+// banks 0 20 8 28 16 4 24 12 (+ t = 0..3): 32 different banks.  An LDS.128 phase of a K-weighting warp (8 lanes = 8 consecutive rows,
+// one column) covers the same 8 offsets x 4 consecutive banks: conflict-free as well.
+constexpr int R128F_CH = 128, R128F_PITCH = 116, R128F_SLOTS = 3, R128F_WARPS = 12;
+constexpr int R128F_STAGE_BYTES = R128F_CH * R128F_PITCH * 4;                    // 59392
+constexpr int R128F_SMEM = 128 + TCF_BBYTES + R128F_SLOTS * R128F_STAGE_BYTES + 64 + R128F_CH * 4;
+static_assert (EBU_TILE == 64, "a stage is one K1 tile");
+
+struct R128fRing {
+    uint8_t* stage; uint32_t full, cnt;          // slot 0; full[3] mbarriers, cnt[3] release counters (shared addresses)
+    const CUtensorMap* tmap; const float* in; size_t stride; const float* hist; int nch, nfram, ntiles, nslabs;
+
+    B200M_DEV uint8_t* slot (int j) const { return stage + (j % R128F_SLOTS) * R128F_STAGE_BYTES; }
+    B200M_DEV void wait (int j) const { tcf_wait (full + 8 * (j % R128F_SLOTS), (uint32_t)(j / R128F_SLOTS) & 1u); }
+    // stage j = tile j % ntiles of this CTA's slab j / ntiles into its slot; called by a whole warp
+    B200M_DEV void produce (int j, int lane) const
+    {
+        const int i = j / ntiles, t = j - i * ntiles;
+        if (i >= nslabs) return;
+        const int c0 = ((int)blockIdx.x + i * (int)gridDim.x) * R128F_CH;
+        const uint32_t dst = smem_u32 (slot (j)), bar = full + 8 * (j % R128F_SLOTS);
+        if (t == 0) {
+            // the 48 samples before the block are the bank's history: per-row bulk copies (a TMA box lands densely)
+            const uint32_t nb = (uint32_t)min (68, nfram) * 4u;
+            if (lane == 0) asm volatile ("mbarrier.arrive.expect_tx.shared::cta.b64 _, [%0], %1;" :: "r"(bar), "r"((uint32_t)R128F_CH * (192u + nb)) : "memory");
+            __syncwarp ();
+            asm volatile ("fence.proxy.async.shared::cta;" ::: "memory");
+            for (int r = lane; r < R128F_CH; r += 32) {
+                const size_t ch = (size_t)min (c0 + r, nch - 1);
+                const uint32_t d = dst + (uint32_t)(r * R128F_PITCH * 4);
+                asm volatile ("cp.async.bulk.shared::cluster.global.mbarrier::complete_tx::bytes [%0], [%1], %2, [%3];"
+                              :: "r"(d), "l"(hist + ch * 48), "r"(192u), "r"(bar) : "memory");
+                asm volatile ("cp.async.bulk.shared::cluster.global.mbarrier::complete_tx::bytes [%0], [%1], %2, [%3];"
+                              :: "r"(d + 192u), "l"(in + ch * stride), "r"(nb), "r"(bar) : "memory");
+            }
+        } else if (lane == 0) {
+            asm volatile ("fence.proxy.async.shared::cta;" ::: "memory");
+            asm volatile ("mbarrier.arrive.expect_tx.shared::cta.b64 _, [%0], %1;" :: "r"(bar), "r"((uint32_t)R128F_STAGE_BYTES) : "memory");
+            asm volatile ("cp.async.bulk.tensor.2d.shared::cluster.global.tile.mbarrier::complete_tx::bytes [%0], [%1, {%2, %3}], [%4];"
+                          :: "r"(dst), "l"(tmap), "r"(64 * t - 48), "r"(c0), "r"(bar) : "memory");
+        }
+    }
+    // a warp is done reading stage j; the last of the 12 warps refills the slot with stage j + 3
+    B200M_DEV void release (int j, int lane) const
+    {
+        __syncwarp ();
+        uint32_t old = 0;
+        if (lane == 0) asm volatile ("atom.acq_rel.cta.shared::cta.add.u32 %0, [%1], 1;" : "=r"(old) : "r"(cnt + 4 * (j % R128F_SLOTS)) : "memory");
+        old = __shfl_sync (0xffffffffu, old, 0);
+        if (old % R128F_WARPS == R128F_WARPS - 1) produce (j + R128F_SLOTS, lane);
+    }
+};
+
+// kw_warp's staging policy in the fused kernel: tile t of slab i is ring stage j0 + t (j0 = i * ntiles), the lane's row from offset 48
+struct FusedStage {
+    static constexpr int UNROLL = 4;
+    R128fRing ring; int j0, lane, row;             // row: byte offset of the lane's first new sample in a slot
+    B200M_DEV void prologue () {}
+    B200M_DEV void acquire (int t) { ring.wait (j0 + t); }
+    B200M_DEV void release (int t) { ring.release (j0 + t, lane); }
+    B200M_DEV void drain () {}
+    B200M_DEV const float* rowp (int t) const { return reinterpret_cast<const float*> (ring.slot (j0 + t) + row); }
+    B200M_DEV float4 ld4 (int t, int q) const { return reinterpret_cast<const float4*> (rowp (t))[q]; }
+    B200M_DEV float4 ld4_dyn (int t, int q) const { return ld4 (t, q); }
+    B200M_DEV float ld (int t, int e) const { return rowp (t)[e]; }
+};
+
+__global__ void __launch_bounds__ (R128F_WARPS * 32, 1)
+r128_fused_kernel (const __grid_constant__ CUtensorMap tmap, const float* __restrict__ in, size_t stride, int nch, int nfram,
+                   const float* __restrict__ bcanon, TpkState st, float* __restrict__ r128_tpmax,
+                   EbuCoef cf, EbuChunks ck, float fragm_f, float* __restrict__ zst, float* __restrict__ frpwr, float* __restrict__ fragpw, int n_inst)
+{
+    extern __shared__ uint8_t r128f_smem[];
+    uint8_t* sB = r128f_smem + ((128u - (smem_u32 (r128f_smem) & 127u)) & 127u);            // TMA destinations: 128-byte aligned
+    uint8_t* stages = sB + TCF_BBYTES;
+    uint64_t* full = reinterpret_cast<uint64_t*> (stages + R128F_SLOTS * R128F_STAGE_BYTES);
+    unsigned* cnt = reinterpret_cast<unsigned*> (full + 4);
+    unsigned* s_gmax = reinterpret_cast<unsigned*> (full + 8);
+    const int tid = threadIdx.x, warp = tid >> 5, lane = tid & 31;
+    const int ntiles = (nfram + EBU_TILE - 1) / EBU_TILE, nslabs = (nch + R128F_CH - 1) / R128F_CH;
+    R128fRing ring;
+    ring.stage = stages; ring.full = smem_u32 (full); ring.cnt = smem_u32 (cnt); ring.tmap = &tmap; ring.in = in; ring.stride = stride;
+    ring.hist = st.hist; ring.nch = nch; ring.nfram = nfram; ring.ntiles = ntiles;
+    ring.nslabs = (nslabs - (int)blockIdx.x + (int)gridDim.x - 1) / (int)gridDim.x;
+
+    for (int i = tid; i < TCF_BBYTES / 16; i += R128F_WARPS * 32) reinterpret_cast<float4*> (sB)[i] = reinterpret_cast<const float4*> (bcanon)[i];
+    if (tid < R128F_CH) s_gmax[tid] = 0u;
+    if (tid < R128F_SLOTS) cnt[tid] = 0u;
+    if (tid == 0) {
+        for (int s = 0; s < R128F_SLOTS; ++s) asm volatile ("mbarrier.init.shared::cta.b64 [%0], 1;" :: "r"(ring.full + 8 * s));
+        asm volatile ("fence.mbarrier_init.release.cluster;" ::: "memory");
+    }
+    asm volatile ("fence.proxy.async.shared::cta;" ::: "memory");             // B: generic-proxy stores, read by the tensor core (async proxy)
+    __syncthreads ();
+
+    if (warp >= 8) {
+        // ---------------- K-weighting warpgroup: warp kw = 32 channels of the slab; the first one also fills the ring
+        const int kw = warp - 8;
+        if (kw == 0)
+            for (int j = 0; j < R128F_SLOTS; ++j) ring.produce (j, lane);
+        FusedStage sg;
+        sg.ring = ring; sg.lane = lane; sg.row = ((32 * kw + lane) * R128F_PITCH + 48) * 4;
+        for (int i = 0; i < ring.nslabs; ++i) {
+            const int k = ((int)blockIdx.x + i * (int)gridDim.x) * R128F_CH + 32 * kw + lane;
+            sg.j0 = i * ntiles;
+            // rows beyond the bank read as zeros (stage 0: the last channel's): those lanes never store
+            kw_warp<2> (sg, lane, min (k, nch - 1), k < nch, nch, nfram, cf, ck, fragm_f, zst, frpwr, fragpw, n_inst);
+        }
+        return;
+    }
+
+    // ---------------- FIR warpgroups
+    const int wg = warp >> 2, w = warp & 3, g = lane >> 2, t4 = lane & 3, b0 = 2 * (w & 1);
+    const int rowc = 64 * wg + 8 * (w >> 1) + g;                              // the thread's channel in tile m: rowc + 16 m
+    const uint32_t bb = smem_u32 (sB);
+    if (wg == 1) bar_arrive_i<2, 256> ();                                     // warpgroup 0 takes the tensor cores first (barrier 2 + wg: its turn)
+    for (int i = 0; i < ring.nslabs; ++i) {
+        const int c0 = ((int)blockIdx.x + i * (int)gridDim.x) * R128F_CH;
+        float rm0 = 0.0f, rm1 = 0.0f, rm2 = 0.0f, rm3 = 0.0f;                   // running maxima of channels rowc + 16 m, m = 0..3
+        for (int t = 0; t < ntiles; ++t) {
+            const int j = i * ntiles + t;
+            ring.wait (j);
+            const float* xs = reinterpret_cast<const float*> (ring.slot (j));
+            int vj[2], nin[2];                                                // valid output positions; window elements k < nin lie inside the block
+#pragma unroll
+            for (int h = 0; h < 2; ++h) {
+                vj[h] = min (16, max (0, nfram - (64 * t + 16 * (b0 + h))));
+                nin[h] = nfram + 48 - 64 * t - 16 * (b0 + h);
+            }
+#pragma unroll 1
+            for (int m = 0; m < 4; ++m) {
+                float v[8][4];
+                tcf_load (xs + (rowc + 16 * m) * R128F_PITCH + 16 * b0 + t4, v);
+                if (m == 3) {
+                    if (t == ntiles - 1) {
+                        // history of the next block = the 48 samples that end this one (stage positions nfram - 64 t + k); a warp copies 16 rows
+                        for (int q = lane; q < 16 * 12; q += 32) {
+                            const int r = 16 * warp + q / 12, k4 = (q % 12) * 4;
+                            if (c0 + r < nch)
+                                *reinterpret_cast<float4*> (st.hist_alt + (size_t)(c0 + r) * 48 + k4) = *reinterpret_cast<const float4*> (xs + r * R128F_PITCH + (nfram - 64 * t) + k4);
+                        }
+                    }
+                    ring.release (j, lane);
+                }
+                const float p0 = tcf_mask_p0 (v, t4, vj, nin);
+                uint32_t ahi[8][4], alo[8][4];
+                tcf_split (v, ahi, alo);
+                float d[48];
+                // no branch between the wgmmas and their wait (ptxas would serialise them): barrier ids in registers, a predicated arrive
+                const uint32_t pass = wg == 0 || i < ring.nslabs - 1 || t < ntiles - 1 || m < 3;
+                asm volatile ("bar.sync %0, 256;" :: "r"(2 + wg) : "memory");
+                tcf_mma (d, ahi, alo, bb);
+                asm volatile ("{ .reg .pred p; setp.ne.b32 p, %1, 0; @p bar.arrive %0, 256; }" :: "r"(3 - wg), "r"(pass) : "memory");
+                tcf_mma_wait ();
+                // the four maxima rotate: rm0 is always tile m's channel
+                const float mx = tcf_tile_max (d, t4, vj, fmaxf (rm0, p0));
+                rm0 = rm1; rm1 = rm2; rm2 = rm3; rm3 = mx;
+            }
+        }
+        // the slab's block is complete: one maximum per channel, then process_max's m = max (m, v) (truepeakdsp.cc:108-123) and the
+        // EBUr128 epilogue, as in tpmax_tc_kernel
+        const float rm[4] = {rm0, rm1, rm2, rm3};
+#pragma unroll
+        for (int m = 0; m < 4; ++m) {
+            float mx = fmaxf (rm[m], __shfl_xor_sync (0xffffffffu, rm[m], 1));
+            mx = fmaxf (mx, __shfl_xor_sync (0xffffffffu, mx, 2));
+            if (t4 == 0 && mx > 0.0f) atomicMax (&s_gmax[rowc + 16 * m], __float_as_uint (mx));
+        }
+        bar_sync_i<1, 256> ();
+        if (wg == 0) {
+            const int cc = c0 + tid;
+            const bool own = cc < nch;
+            float mm = __uint_as_float (s_gmax[tid]);
+            s_gmax[tid] = 0u;
+            if (own) {
+                const float m0 = st.tp_res[cc] ? 0.0f : st.tp_m[cc];
+                if (!(mm > m0)) mm = m0;
+                st.tp_m[cc] = mm;
+            }
+            // src/ebulv2.cc:227-230,360-367, one thread per stereo instance: read() both meters, coef_to_db, hold
+            const float bo = __shfl_xor_sync (0xffffffffu, mm, 1);
+            if (own && (tid & 1) == 0 && cc + 1 < nch) {
+                const float vv = mm > bo ? mm : bo;
+                const float tp = (vv == 0) ? -INFINITY : __double2float_rn (__dmul_rn (20.0, (double)log10f_glibc (vv)));
+                if (tp > r128_tpmax[cc >> 1]) r128_tpmax[cc >> 1] = tp;
+                st.tp_res[cc] = 1; st.tp_res[cc + 1] = 1;
+            }
+        }
+        bar_sync_i<1, 256> ();                                                // s_gmax is reset before the next slab's maxima arrive
     }
 }
 
@@ -1904,6 +2138,35 @@ static int tpk_process (b200m_tpk* h, const float* d_in, size_t stride, uint32_t
     return tpk_process_sliced (h, d_in, stride, nfram, tp_mode, st, 1, bounds, nullptr, nullptr, false, h->dr_on ? &h->dr : nullptr);
 }
 
+// ---- the EBUr128 cycle's fused K-weighting + true-peak kernel (r128_fused_kernel), launched by the EBU bank in place of K1 (r128.cu)
+// It walks time with one CTA per 128-channel slab, so its cycle costs about the same from a few dozen slabs up to one slab per SM,
+// while K1 + tpmax_tc_kernel spread any bank over every SM and scale with it.  Cycle of 1024 frames, median of 3 x 300 cycles on an
+// H100 80GB HBM3 (SXM, 700 W power limit): two kernels 51.9 / 77.4 / 84.7 / 89.0 / 101.2 / 129.6 us, fused 81.8 / 82.9 / 83.8 / 82.8 /
+// 82.5 / 83.4 us for 2048 / 4096 / 4608 / 5120 / 6144 / 8192 stereo instances.  They tie near 4608 instances: banks of at least 10240
+// channels (5120 stereo instances) run fused.
+constexpr uint32_t R128F_MIN_CH = 10240;
+
+bool tpk_r128_fused_ok (const b200m_tpk* h, const float* d_in, size_t stride, uint32_t nfram)
+{
+    return (h->flags & B200M_TPK_TRUEPEAK) && !(h->flags & B200M_TPK_KMETER) && h->chunked && h->tc && h->fma && h->imm && h->d_btc && !h->d_dbg
+        && (uintptr_t)d_in % 16 == 0 && stride % 4 == 0 && nfram % 4 == 0 && h->n_chan >= R128F_MIN_CH;
+}
+
+int tpk_r128_fused (b200m_tpk* h, const EbuK1Args& a, float* r128_tpmax, cudaStream_t st)
+{
+    if (a.nchans != (int)h->n_chan) return set_err (B200M_E_INVAL, "r128: EBU and true-peak banks disagree on the channel count");
+    CUtensorMap tm;
+    if (!ebu_tma_map (&tm, a.in, a.stride, h->n_chan, (uint32_t)a.nfram, R128F_PITCH, R128F_CH, false))
+        return set_err (B200M_E_CUDA, "r128: the driver rejected the input block's tensor map");
+    const int nslabs = ((int)h->n_chan + R128F_CH - 1) / R128F_CH;
+    r128_fused_kernel<<<std::min (nslabs, h->n_sm), R128F_WARPS * 32, R128F_SMEM, st>>> (
+        tm, a.in, a.stride, (int)h->n_chan, a.nfram, h->d_btc, h->st, r128_tpmax, a.cf, a.ck, a.fragm_f, a.zst, a.frpwr, a.fragpw, a.n_inst);
+    B200M_LAUNCHED (1);
+    B200M_CUDA (cudaGetLastError ());
+    float* t = h->st.hist; h->st.hist = h->st.hist_alt; h->st.hist_alt = t;          // the kernel wrote the next block's history
+    return 0;
+}
+
 extern "C" {
 
 int b200m_design_tpk (float fsamp, float w[4], float ctab[120], float km[2])
@@ -1985,6 +2248,7 @@ int b200m_tpk_create (b200m_tpk** out, int device, uint32_t n_chan, float fsamp,
         if (e == cudaSuccess) e = cudaFuncSetAttribute (tpmax_tc_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, TCF_SMEM);
         // it shares SMs with the K-weighting kernel in the EBUr128 cycle (106 KB + 104 KB): same (maximum) carveout as that one
         if (e == cudaSuccess) e = cudaFuncSetAttribute (tpmax_tc_kernel, cudaFuncAttributePreferredSharedMemoryCarveout, cudaSharedmemCarveoutMaxShared);
+        if (e == cudaSuccess) e = cudaFuncSetAttribute (r128_fused_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, R128F_SMEM);
         if (e == cudaSuccess) e = cudaDeviceGetAttribute (&h->n_sm, cudaDevAttrMultiProcessorCount, device);
     }
     if (const char* v = getenv ("B200M_TPK_DEC")) h->dec = atoi (v) != 0;
