@@ -227,8 +227,9 @@ b200m_tpk* b200m_r128_tpk (b200m_r128* h);
  * DR-14 / TPnRMS bank (SURVEY §8f rank 2) — replaces dr14_run (src/dr14.c:354-482) for n_inst instances of
  * n_channels (1 or 2): Kmeterdsp::process + TruePeakdsp::process + read() per channel and, with dr_mode, the 3 s
  * window statistics of dr14_calc_rms_score (:285-352).  The result block mirrors the plugin's output ports
- * (DRPortIndex :27-43): all values in dB as the reference writes them.  Every instance shares the 3 s window clock, so
- * reset_peaks (:241-258) is bank-wide.  dr_mode needs rate >= 2731 Hz (a window longer than the largest block).
+ * (DRPortIndex :27-43): all values in dB as the reference writes them.  Every instance has its own 3 s window phase,
+ * which restarts when that instance is reset, so each instance behaves as a plugin of its own.  dr_mode needs
+ * rate >= 2731 Hz (a window longer than the largest block).
  * ====================================================================================== */
 typedef struct b200m_dr14 b200m_dr14;
 typedef struct b200m_dr14_result {
@@ -242,6 +243,13 @@ int b200m_dr14_destroy (b200m_dr14* h);
 int b200m_dr14_run_device (b200m_dr14* h, const float* d_in, size_t stride, uint32_t nfram, void* stream);   /* rows: inst * n_channels + c */
 int b200m_dr14_run_host (b200m_dr14* h, const float* in, size_t stride, uint32_t nfram);
 int b200m_dr14_reset (b200m_dr14* h, void* stream);                                       /* reset_peaks, every instance */
+/* B200M_DR14_RESET: reset_peaks (:246-262) of the listed instances: K-meter reset, m_peak = m_rms = -81, m_dbtp = 0, window
+ * sums, second-peak pair, histogram, num_fragments, and the instance's 3 s window restarts with the next block.
+ * B200M_DR14_CLEAR: the instance as a freshly instantiated plugin (:139-165): RESET plus b200m_tpk_clear of its channels.
+ * inst = NULL, count = 0: every instance; a listed instance may repeat.  One upload and two kernels per call, ordered with the
+ * bank's runs on the stream the bank currently runs on. */
+enum { B200M_DR14_RESET = 1, B200M_DR14_CLEAR = 2 };
+int b200m_dr14_control (b200m_dr14* h, const uint32_t* inst, uint32_t count, int cmd, void* stream);
 int b200m_dr14_results (b200m_dr14* h, b200m_dr14_result* out, void* stream);
 int b200m_dr14_histogram (b200m_dr14* h, uint32_t inst, uint32_t chan, uint32_t* hist8000, void* stream);   /* hist[c] (:46,309-311) */
 

@@ -113,6 +113,7 @@ _PROTOS = {
     "b200m_dr14_run_device": (C.c_int, [_v, _v, C.c_size_t, C.c_uint32, _v]),
     "b200m_dr14_run_host": (C.c_int, [_v, _v, C.c_size_t, C.c_uint32]),
     "b200m_dr14_reset": (C.c_int, [_v, _v]),
+    "b200m_dr14_control": (C.c_int, [_v, _v, C.c_uint32, C.c_int, _v]),
     "b200m_dr14_results": (C.c_int, [_v, _v, _v]),
     "b200m_dr14_histogram": (C.c_int, [_v, C.c_uint32, C.c_uint32, _v, _v]),
     "b200m_cor_create": (C.c_int, [C.POINTER(_v), C.c_int, C.c_uint32, C.c_int, C.c_float, C.c_float]),
@@ -616,6 +617,9 @@ DR14_RESULT_DTYPE = np.dtype([("v_rms", "<f4", 2), ("v_peak", "<f4", 2), ("m_pea
                               ("dr_total", "<f4"), ("block_count", "<f4")])
 
 
+DR14_RESET, DR14_CLEAR = 1, 2
+
+
 class DR14(_Bank):
     """N x dr14_run (src/dr14.c:354-482): DR-14 mode (dr_mode=True) or TPnRMS (False); results = the plugin's output ports."""
     _destroy = "b200m_dr14_destroy"
@@ -640,6 +644,14 @@ class DR14(_Bank):
 
     def reset(self, stream=None):
         _ck(lib().b200m_dr14_reset(self.h, _stream_ptr(stream)))
+
+    def control(self, cmd, inst=None, stream=None):
+        """DR14_RESET / DR14_CLEAR of the listed instances (a sequence of indices), or of every instance with inst=None"""
+        if inst is None:
+            _ck(lib().b200m_dr14_control(self.h, None, 0, cmd, _stream_ptr(stream)))
+        else:
+            sel = np.ascontiguousarray(inst, np.uint32)
+            _ck(lib().b200m_dr14_control(self.h, _np_ptr(sel), sel.size, cmd, _stream_ptr(stream)))
 
     def results(self, stream=None):
         out = np.empty(self.n_inst, DR14_RESULT_DTYPE)

@@ -6,12 +6,16 @@
 // highest window peak), then read() of both meters and the port arithmetic (:418-462).
 //
 // Mapping: the window sums ride on the process() kernel as an extra lane role (TpkDr, tpk_internal.cuh) so the
-// input is still read once; the window clock is host-tracked and shared by all instances (reset_peaks is bank-wide),
-// so a window end is a launch-time constant `cut`.  The scoring is one warp per instance: the top-down histogram walk
-// is a ballot over 32 bins at a time, accumulated in exactly the reference's bin order.  Port values are computed on
-// the device with the glibc-exact log10f (common.cuh), so every float equals the reference's.
+// input is still read once.  The bank keeps one sample clock on the host; each instance's window phase (the bank time of
+// its last reset_peaks, mod the window length) is device state written only by the control kernel, and each DR lane
+// derives its instance's window end in the block from it.  The host mirrors the phases (an ordered count of the distinct
+// ones), so the scoring kernel is launched only in blocks where some window closes.  The scoring is one warp per instance:
+// the top-down histogram walk is a ballot over 32 bins at a time, accumulated in exactly the reference's bin order.  Port
+// values are computed on the device with the glibc-exact log10f (common.cuh), so every float equals the reference's.
 #include <math.h>
 #include <stdlib.h>
+#include <map>
+#include <vector>
 #include "common.cuh"
 #include "tpk_internal.cuh"
 
@@ -36,16 +40,18 @@ struct Dr14State {
     float *emit_rms, *emit_peak; int* emit_valid;
     float *peak_hist, *m_rms, *m_peak, *m_dbtp;                // per channel (peak_hist: 2 per channel)
     unsigned long long* numfrag;                               // per instance
+    uint32_t* phase;                                           // per instance: bank time of its last reset_peaks, mod the window length
     uint32_t* hist;                                            // [n_ch][8000]
     const float* cd;                                           // db_to_coeff ((b - 7999) / 100.0) for b = 0..7999, host libm
 };
 
-// dr14_calc_rms_score (:285-352) for the window that just closed; one warp per instance
-__global__ void dr14_score_kernel (int n_inst, int nch, float n_sample_cnt_f, Dr14State s)
+// dr14_calc_rms_score (:285-352) of the instances whose window closed in this block; one warp per instance
+__global__ void dr14_score_kernel (int n_inst, int nch, float n_sample_cnt_f, Dr14State s, TpkDr dr, int nfram)
 {
     const int inst = (blockIdx.x * blockDim.x + threadIdx.x) >> 5, lane = threadIdx.x & 31;
     if (inst >= n_inst) return;
     const int ch0 = inst * nch;
+    if (tpk_dr_cut (dr, inst, nfram) < 0) return;             // no window end in this block: emit_* still hold an older window's
     if (!s.emit_valid[ch0]) return;                            // silent window: nothing recorded (:287-297)
     unsigned long long nf = 0;
     if (lane == 0) { nf = s.numfrag[inst] + 1; s.numfrag[inst] = nf; }
@@ -126,12 +132,20 @@ __global__ void dr14_ports_kernel (int n_inst, int nch, int dr_mode, const b200m
     out[inst] = o;
 }
 
-__global__ void dr14_reset_kernel (size_t n_ch, size_t n_inst, int dr_mode, float* rms_sum, float* peak_cur, Dr14State s)
+// reset_peaks (:246-262) of the instances inst[0 .. n_sel) (inst == nullptr: instances 0 .. n_sel - 1): their next window
+// starts at bank time `tmod` (mod the window length).  The K-meter part is tpk_reset_inst.
+__global__ void dr14_reset_kernel (const uint32_t* inst, size_t n_sel, int nch, int dr_mode, uint32_t tmod, float* rms_sum, float* peak_cur, Dr14State s)
 {
-    const size_t i = (size_t)blockIdx.x * blockDim.x + threadIdx.x;
-    if (i < n_ch) { s.m_peak[i] = -81.0f; s.m_rms[i] = -81.0f; s.m_dbtp[i] = 0.0f; rms_sum[i] = 0.0f; peak_cur[i] = 0.0f; s.peak_hist[2 * i] = 0.0f; s.peak_hist[2 * i + 1] = 0.0f; s.emit_valid[i] = 0; }
-    if (i < n_inst) s.numfrag[i] = 0;
-    if (dr_mode) for (size_t k = i; k < n_ch * DR_HISTBINS; k += (size_t)gridDim.x * blockDim.x) s.hist[k] = 0;
+    const size_t t = (size_t)blockIdx.x * blockDim.x + threadIdx.x, n_ch = n_sel * nch;
+    auto chan = [&] (size_t k) { return inst ? (size_t)inst[k / nch] * nch + k % nch : k; };
+    if (t < n_ch) { const size_t i = chan (t); s.m_peak[i] = -81.0f; s.m_rms[i] = -81.0f; s.m_dbtp[i] = 0.0f; rms_sum[i] = 0.0f; peak_cur[i] = 0.0f; s.peak_hist[2 * i] = 0.0f; s.peak_hist[2 * i + 1] = 0.0f; s.emit_valid[i] = 0; }
+    if (t < n_sel) { const size_t j = inst ? inst[t] : t; s.numfrag[j] = 0; s.phase[j] = tmod; }
+    if (dr_mode)
+        for (size_t k = t; k < n_ch * DR_HISTBINS; k += (size_t)gridDim.x * blockDim.x) {
+            if (!inst) { s.hist[k] = 0; continue; }
+            const size_t r = k / DR_HISTBINS;
+            s.hist[chan (r) * DR_HISTBINS + (k - r * DR_HISTBINS)] = 0;
+        }
 }
 
 }  // namespace b200m
@@ -141,38 +155,59 @@ using namespace b200m;
 struct b200m_dr14 {
     int device; uint32_t n_inst, nch; double rate; int dr_mode;
     b200m_tpk* tpk = nullptr;
-    uint64_t n_sample_cnt = 0, sample_count = 0;               // 3 s window clock (:149-150), shared by every instance
+    uint64_t n_sample_cnt = 0;                                 // rintf (rate * 3.0) (:149)
+    uint32_t w = 0, tmod = 0;                                  // window length n_sample_cnt + 1; bank sample clock mod w
+    std::vector<uint32_t> phase;                               // host mirror of st.phase
+    std::map<uint32_t, uint32_t> phases;                       // distinct phases -> number of instances on each
+    uint32_t* d_sel = nullptr;                                 // instance list of a control call
     float *d_rms_sum = nullptr, *d_peak_cur = nullptr, *d_cd = nullptr;
     Dr14State st{}; b200m_dr14_result* d_out = nullptr;
     cudaStream_t own = nullptr; HostStage stage; bool last_host = false;
 };
 
-static int dr14_reset_all (b200m_dr14* h, cudaStream_t st)
+// reset_peaks of the instances d_inst[0 .. n_sel) (d_inst == nullptr: every instance), clear: and b200m_tpk_clear of their
+// channels.  The host mirror of the phases is updated by the caller.
+static int dr14_reset (b200m_dr14* h, const uint32_t* d_inst, uint32_t n_sel, bool clear, cudaStream_t st)
 {
-    const size_t n_ch = (size_t)h->n_inst * h->nch;
-    dr14_reset_kernel<<<(unsigned)((n_ch + 255) / 256), 256, 0, st>>> (n_ch, h->n_inst, h->dr_mode, h->d_rms_sum, h->d_peak_cur, h->st);
+    const size_t n_ch = (size_t)n_sel * h->nch;
+    dr14_reset_kernel<<<(unsigned)((n_ch + 255) / 256), 256, 0, st>>> (d_inst, n_sel, (int)h->nch, h->dr_mode, h->tmod, h->d_rms_sum, h->d_peak_cur, h->st);
     B200M_LAUNCHED (1);
     B200M_CUDA (cudaGetLastError ());
-    h->sample_count = 0;
-    return b200m_tpk_reset_kmeter (h->tpk, st);                // km[c]->reset () (:249)
+    return tpk_reset_inst (h->tpk, d_inst, n_sel, h->nch, clear, st);     // km[c]->reset () (:249)
+}
+
+static void dr14_set_phase (b200m_dr14* h, uint32_t inst, uint32_t p)
+{
+    auto it = h->phases.find (h->phase[inst]);
+    if (--it->second == 0) h->phases.erase (it);
+    h->phase[inst] = p;
+    ++h->phases[p];
+}
+
+// does some instance's window close in the next block of nfram samples?  Phase p closes at block sample (p - tmod - 1) mod w.
+static bool dr14_closes (const b200m_dr14* h, uint32_t nfram)
+{
+    const uint32_t a = (h->tmod + 1) % h->w, b = a + nfram;   // phases in [a, b), taken mod w
+    auto it = h->phases.lower_bound (a);
+    if (it != h->phases.end () && it->first < b) return true;
+    return b > h->w && h->phases.begin ()->first < b - h->w;
 }
 
 static int dr14_run (b200m_dr14* h, const float* d_in, size_t stride, uint32_t nfram, cudaStream_t st)
 {
-    int cut = -1;
+    bool closes = false;
+    TpkDr dr = {};
     if (h->dr_mode) {
-        // "if (++scnt > slmt)" (:410): the window closes after sample index slmt - scnt of this block
-        const uint64_t left = h->n_sample_cnt - h->sample_count;
-        if (left < nfram) { cut = (int)left; h->sample_count = nfram - left - 1; }
-        else h->sample_count += nfram;
-        TpkDr dr = {h->d_rms_sum, h->d_peak_cur, h->st.emit_rms, h->st.emit_peak, h->st.emit_valid, cut, (int)h->nch,
-                    1e-9 * (double)(float)h->n_sample_cnt};
+        closes = dr14_closes (h, nfram);
+        dr = {h->d_rms_sum, h->d_peak_cur, h->st.emit_rms, h->st.emit_peak, h->st.emit_valid, h->st.phase, h->tmod, h->w, (int)h->nch,
+              1e-9 * (double)(float)h->n_sample_cnt};
         tpk_set_dr (h->tpk, &dr);
+        h->tmod = (uint32_t)((h->tmod + (uint64_t)nfram) % h->w);
     }
     int rc = b200m_tpk_process_device (h->tpk, d_in, stride, nfram, B200M_TP_MODE_PROCESS, st);
     if (rc) return rc;
-    if (cut >= 0) {
-        dr14_score_kernel<<<(h->n_inst * 32 + 127) / 128, 128, 0, st>>> ((int)h->n_inst, (int)h->nch, (float)h->n_sample_cnt, h->st);
+    if (closes) {
+        dr14_score_kernel<<<(h->n_inst * 32 + 127) / 128, 128, 0, st>>> ((int)h->n_inst, (int)h->nch, (float)h->n_sample_cnt, h->st, dr, (int)nfram);
         B200M_LAUNCHED (1);
     }
     if ((rc = b200m_tpk_read_device (h->tpk, st))) return rc;
@@ -195,6 +230,9 @@ int b200m_dr14_create (b200m_dr14** out, int device, uint32_t n_inst, uint32_t n
     if (!h) return set_err (B200M_E_NOMEM, "host allocation failed");
     h->device = device; h->n_inst = n_inst; h->nch = n_channels; h->rate = rate; h->dr_mode = dr_mode ? 1 : 0;
     h->n_sample_cnt = (uint64_t)rintf ((float)(rate * 3.0));   // n_sample_cnt = rintf (rate * 3.0) (:149)
+    h->w = (uint32_t)(h->n_sample_cnt + 1);                    // "if (++scnt > slmt)" (:411): a window every n_sample_cnt + 1 samples
+    h->phase.assign (n_inst, 0);
+    h->phases[0] = n_inst;
     const size_t n_ch = (size_t)n_inst * n_channels;
     int rc = b200m_tpk_create (&h->tpk, device, (uint32_t)n_ch, (float)rate, B200M_TPK_TRUEPEAK | B200M_TPK_KMETER);
     if (rc) { delete h; return rc; }
@@ -204,7 +242,7 @@ int b200m_dr14_create (b200m_dr14** out, int device, uint32_t n_inst, uint32_t n
     A ((void**)&h->d_rms_sum, n_ch * 4); A ((void**)&h->d_peak_cur, n_ch * 4);
     A ((void**)&h->st.emit_rms, n_ch * 4); A ((void**)&h->st.emit_peak, n_ch * 4); A ((void**)&h->st.emit_valid, n_ch * 4);
     A ((void**)&h->st.peak_hist, n_ch * 8); A ((void**)&h->st.m_rms, n_ch * 4); A ((void**)&h->st.m_peak, n_ch * 4); A ((void**)&h->st.m_dbtp, n_ch * 4);
-    A ((void**)&h->st.numfrag, (size_t)n_inst * 8);
+    A ((void**)&h->st.numfrag, (size_t)n_inst * 8); A ((void**)&h->st.phase, (size_t)n_inst * 4); A ((void**)&h->d_sel, (size_t)n_inst * 4);
     if (h->dr_mode) A ((void**)&h->st.hist, n_ch * DR_HISTBINS * 4);
     A ((void**)&h->d_cd, DR_HISTBINS * 4); A ((void**)&h->d_out, (size_t)n_inst * sizeof (b200m_dr14_result));
     if (e == cudaSuccess) {
@@ -220,7 +258,7 @@ int b200m_dr14_create (b200m_dr14** out, int device, uint32_t n_inst, uint32_t n
     }
     if (e == cudaSuccess) e = cudaStreamCreateWithFlags (&h->own, cudaStreamNonBlocking);
     if (e == cudaSuccess) {                                    // instantiate: m_rms = m_peak = -81 (:157-158)
-        dr14_reset_kernel<<<(unsigned)((n_ch + 255) / 256), 256>>> (n_ch, n_inst, h->dr_mode, h->d_rms_sum, h->d_peak_cur, h->st);
+        dr14_reset_kernel<<<(unsigned)((n_ch + 255) / 256), 256>>> (nullptr, n_inst, (int)n_channels, h->dr_mode, 0u, h->d_rms_sum, h->d_peak_cur, h->st);
         B200M_LAUNCHED (1);
         e = cudaDeviceSynchronize ();
     }
@@ -236,7 +274,7 @@ int b200m_dr14_destroy (b200m_dr14* h)
     DeviceGuard g (h->device);
     cudaDeviceSynchronize ();
     void* ps[] = {h->d_rms_sum, h->d_peak_cur, h->st.emit_rms, h->st.emit_peak, h->st.emit_valid, h->st.peak_hist, h->st.m_rms, h->st.m_peak,
-                  h->st.m_dbtp, h->st.numfrag, h->st.hist, h->d_cd, h->d_out};
+                  h->st.m_dbtp, h->st.numfrag, h->st.phase, h->d_sel, h->st.hist, h->d_cd, h->d_out};
     for (void* p : ps) cudaFree (p);
     h->stage.release ();
     if (h->own) cudaStreamDestroy (h->own);
@@ -268,9 +306,31 @@ int b200m_dr14_run_host (b200m_dr14* h, const float* in, size_t stride, uint32_t
 
 int b200m_dr14_reset (b200m_dr14* h, void* stream)              // reset_peaks (:241-258), every instance
 {
+    return b200m_dr14_control (h, nullptr, 0, B200M_DR14_RESET, stream);
+}
+
+int b200m_dr14_control (b200m_dr14* h, const uint32_t* inst, uint32_t count, int cmd, void* stream)
+{
     if (!h) return set_err (B200M_E_INVAL, "NULL handle");
+    if (cmd != B200M_DR14_RESET && cmd != B200M_DR14_CLEAR) return set_err (B200M_E_INVAL, "unknown control %d", cmd);
+    if (!inst && count) return set_err (B200M_E_INVAL, "NULL instance list");
     DeviceGuard g (h->device);
-    return dr14_reset_all (h, h->last_host ? h->own : (cudaStream_t)stream);
+    cudaStream_t st = h->last_host ? h->own : (cudaStream_t)stream;
+    if (!inst) {
+        h->phase.assign (h->n_inst, h->tmod);
+        h->phases.clear (); h->phases[h->tmod] = h->n_inst;
+        return dr14_reset (h, nullptr, h->n_inst, cmd == B200M_DR14_CLEAR, st);
+    }
+    std::vector<uint32_t> sel;                                 // the listed instances, each once
+    std::vector<uint8_t> seen (h->n_inst, 0);
+    for (uint32_t k = 0; k < count; ++k) {
+        if (inst[k] >= h->n_inst) return set_err (B200M_E_INVAL, "bad instance %u", inst[k]);
+        if (!seen[inst[k]]) { seen[inst[k]] = 1; sel.push_back (inst[k]); }
+    }
+    if (sel.empty ()) return 0;
+    B200M_CUDA (cudaMemcpyAsync (h->d_sel, sel.data (), sel.size () * sizeof (uint32_t), cudaMemcpyHostToDevice, st));
+    for (uint32_t i : sel) dr14_set_phase (h, i, h->tmod);
+    return dr14_reset (h, h->d_sel, (uint32_t)sel.size (), cmd == B200M_DR14_CLEAR, st);
 }
 
 int b200m_dr14_results (b200m_dr14* h, b200m_dr14_result* out, void* stream)

@@ -66,13 +66,13 @@ inline void forward_audio (float* const* in, float* const* out, uint32_t chn, ui
 // first: a skipped instance meters silence for that cycle rather than its previous block again.
 struct HubKey {
     int family;                                                // lv2_shim.cu: its Kind; lv2_ebur128.cu, lv2_stats.cu: HUB_*
-    int ppm_kind; uint32_t chn, tpk_flags; double rate;        // chn: staged rows per slot
+    int ppm_kind; uint32_t chn, tpk_flags; double rate;        // chn: staged rows per slot; HUB_DR14: tpk_flags = DR mode
     bool operator== (const HubKey& o) const
     {
         return family == o.family && ppm_kind == o.ppm_kind && chn == o.chn && tpk_flags == o.tpk_flags && rate == o.rate;
     }
 };
-constexpr int HUB_EBUR128 = -1, HUB_BITMETER = -2, HUB_SIGDIST = -3;
+constexpr int HUB_EBUR128 = -1, HUB_BITMETER = -2, HUB_SIGDIST = -3, HUB_DR14 = -4;
 
 class SlotHub {
 public:

@@ -404,7 +404,9 @@ tpk_kernel (const float* __restrict__ in, size_t stride, int c_first, int n_chan
     // ballistics lanes come in groups of 16 channels x 2 filters = one warp: a 16-channel CTA has one such warp (the other three do the
     // K-meter / DR roles or idle during the serial phase), a 64-channel CTA ("wide") keeps ALL four warps busy in the serial phase.
     // 87 KB of shared memory per CTA leave two CTAs = eight warps per SM, too few to hide the FIR's latencies (the 16-channel form
-    // keeps seven CTAs resident and lets other CTAs' FIR phases run under a CTA's serial phase).  Kept opt-in, bit-identical, tested.
+    // keeps seven CTAs resident and lets other CTAs' FIR phases run under a CTA's serial phase; its DR form takes 94 registers and
+    // keeps five, measured faster than the same code bounded to seven, meters.lv2_b200/host/dr14_run_cost.py).  Kept opt-in,
+    // bit-identical, tested.
     static_assert (!BAL || CH == 16 || CH == 64, "split ballistics lanes assume 16 channels per warp");
     constexpr bool ALLW = BAL && CH == 64;
     constexpr int LPR = TPK_THREADS / CH;         // lanes that share one channel row in the FIR phase (an aligned lane group)
@@ -495,8 +497,11 @@ tpk_kernel (const float* __restrict__ in, size_t stride, int c_first, int n_chan
     const int drow = wbase + (lane & 15);
     const int dch = min (c0 + drow, n_chan - 1);
     const bool dr_live = dr_warp && lane < 16 && (c0 + drow) < n_chan;
-    float drs = 0, drp = 0;
-    if (dr_warp) { drs = dr.rms_sum[dch]; drp = dr.peak_cur[dch]; }
+    float drs = 0, drp = 0; int dcut = -1;
+    if (dr_warp) { drs = dr.rms_sum[dch]; drp = dr.peak_cur[dch]; dcut = tpk_dr_cut (dr, dch / dr.nch, nfram); }
+    // the first window end of the warp's lanes in this block (each lane's instance has its own); the warp reaches it together, so
+    // the silence test's partner exchange is a convergent shuffle
+    int wcut = dr_warp ? __reduce_min_sync (0xffffffffu, dcut >= 0 ? dcut : INT_MAX) : INT_MAX;
     float vmax = 0.0f;                                                    // process_max: plain running max (:109-122), per FIR lane
     const int km_n = (nfram / 4) * 4;                                     // "n /= 4" drops n mod 4 samples (:79)
 
@@ -654,15 +659,18 @@ tpk_kernel (const float* __restrict__ in, size_t stride, int c_first, int n_chan
                 const float v = xr[j];
                 drs = __fadd_rn (drs, __fmul_rn (v, v));
                 drp = drp > v ? drp : v;                    // MAX (peak_cur, v) on the RAW sample (:408), NaN-transparent like the macro
-                if (s0 + j == dr.cut) {                      // ++scnt > slmt (:410): the 3 s window closes after this sample
+                if (s0 + j == wcut) {                        // warp-uniform: the whole warp exchanges, the lanes whose window ends here close
                     const float other = dr.nch == 2 ? __shfl_xor_sync (0xffffffffu, drs, 1) : drs;
-                    const bool silent = !((double)drs > dr.silent_thr) && !((double)other > dr.silent_thr);
-                    if (dr_live) {
-                        dr.emit_valid[dch] = silent ? 0 : 1;
-                        if (!silent) { dr.emit_rms[dch] = drs; dr.emit_peak[dch] = drp; }
+                    if (dcut == wcut) {                      // ++scnt > slmt (:410): this lane's 3 s window closes after this sample
+                        const bool silent = !((double)drs > dr.silent_thr) && !((double)other > dr.silent_thr);
+                        if (dr_live) {
+                            dr.emit_valid[dch] = silent ? 0 : 1;
+                            if (!silent) { dr.emit_rms[dch] = drs; dr.emit_peak[dch] = drp; }
+                        }
+                        drs = 0.0f;                          // silent windows keep peak_cur (:293-296)
+                        if (!silent) drp = 0.0f;
                     }
-                    drs = 0.0f;                              // silent windows keep peak_cur (:293-296)
-                    if (!silent) drp = 0.0f;
+                    wcut = __reduce_min_sync (0xffffffffu, dcut > wcut ? dcut : INT_MAX);
                 }
             }
         }
@@ -1133,6 +1141,10 @@ tpbal_kernel (const float4* __restrict__ scr, int scr_pitch, const float* __rest
         const bool is_km = lane < 16;
         const bool is_dr = DR && dr.rms_sum != nullptr && lane >= 16;
         float kz1 = 0, kz2 = 0, kt = 0, drs = 0, drp = 0;
+        // window end of this lane's instance in the block (lanes k and k + 16 share a channel), and the warp's first one at or after
+        // this launch's slab: the warp reaches it together, so the silence test's partner exchange is a convergent shuffle
+        const int dcut = DR && dr.rms_sum != nullptr ? tpk_dr_cut (dr, ch / dr.nch, nfram) : -1;
+        int wcut = DR && dr.rms_sum != nullptr ? __reduce_min_sync (0xffffffffu, dcut >= s_begin ? dcut : INT_MAX) : INT_MAX;
         if (is_km) {
             if (first) {
                 const float a = st.km_z1[ch], b = st.km_z2[ch];
@@ -1189,18 +1201,21 @@ tpbal_kernel (const float4* __restrict__ scr, int scr_pitch, const float* __rest
                     kz2 = __fadd_rn (kz2, __fmul_rn (om4, __fsub_rn (kz1, kz2)));
                 }
             }
-            if (DR && dr.rms_sum != nullptr) {                      // both half warps take the branch: the window close shuffles within lanes 16..31
+            if (DR && dr.rms_sum != nullptr) {
                 for (int j = 0; j < len; ++j) {
                     const float v = xr[j];
                     if (is_dr) { drs = __fadd_rn (drs, __fmul_rn (v, v)); drp = drp > v ? drp : v; }
-                    if (a0 + j == dr.cut) {
+                    if (a0 + j == wcut) {                           // warp-uniform: both half warps exchange, the lanes whose window ends here close
                         const float other = dr.nch == 2 ? __shfl_xor_sync (0xffffffffu, drs, 1) : drs;
-                        const bool silent = !((double)drs > dr.silent_thr) && !((double)other > dr.silent_thr);
-                        if (is_dr && live) {
-                            dr.emit_valid[ch] = silent ? 0 : 1;
-                            if (!silent) { dr.emit_rms[ch] = drs; dr.emit_peak[ch] = drp; }
+                        if (dcut == wcut) {
+                            const bool silent = !((double)drs > dr.silent_thr) && !((double)other > dr.silent_thr);
+                            if (is_dr && live) {
+                                dr.emit_valid[ch] = silent ? 0 : 1;
+                                if (!silent) { dr.emit_rms[ch] = drs; dr.emit_peak[ch] = drp; }
+                            }
+                            if (is_dr) { drs = 0.0f; if (!silent) drp = 0.0f; }
                         }
-                        if (is_dr) { drs = 0.0f; if (!silent) drp = 0.0f; }
+                        wcut = __reduce_min_sync (0xffffffffu, dcut > wcut ? dcut : INT_MAX);
                     }
                 }
             }
@@ -1952,9 +1967,11 @@ __global__ void tpk_read_kernel (int n_chan, uint32_t flags, TpkState st, b200m_
     out[i] = r;
 }
 
-__global__ void tpk_reset_kernel (int n_chan, int sel, uint32_t flags, TpkState st)
+// channel `sel`, every channel (sel = -1), or with a list the channels inst[k] * per .. inst[k] * per + per - 1 for k < n_sel
+__global__ void tpk_reset_kernel (int n_chan, int sel, uint32_t flags, TpkState st, const uint32_t* inst, int n_sel, int per)
 {
-    const int i = blockIdx.x * blockDim.x + threadIdx.x;
+    int i = blockIdx.x * blockDim.x + threadIdx.x;
+    if (inst) { if (i >= n_sel * per) return; i = (int)inst[i / per] * per + i % per; }
     if (i >= n_chan || (sel >= 0 && i != sel)) return;
     if (flags & B200M_TPK_TRUEPEAK) { st.tp_res[i] = 1; st.tp_m[i] = 0; st.tp_p[i] = 0; }                 // :140-145
     if (flags & B200M_TPK_KMETER) { st.km_z1[i] = st.km_z2[i] = st.km_rms[i] = st.km_peak[i] = 0; st.km_cnt[i] = 0; st.km_flag[i] = 0; }
@@ -2028,6 +2045,14 @@ static void tpk_design (float fsamp, TpkParams& prm, float* ctab)
 namespace b200m {
 void tpk_set_dr (b200m_tpk* h, const TpkDr* dr) { h->dr_on = dr != nullptr; if (dr) h->dr = *dr; }
 const b200m_tpk_result* tpk_device_results (b200m_tpk* h) { return h->d_res; }
+int tpk_reset_inst (b200m_tpk* h, const uint32_t* d_inst, uint32_t n_sel, uint32_t per, bool clear, cudaStream_t st)
+{
+    const uint32_t flags = clear ? h->flags | 4u : h->flags & B200M_TPK_KMETER, n = d_inst ? n_sel * per : h->n_chan;
+    tpk_reset_kernel<<<(n + 127) / 128, 128, 0, st>>> ((int)h->n_chan, -1, flags, h->st, d_inst, (int)n_sel, (int)per);
+    B200M_LAUNCHED (1);
+    B200M_CUDA (cudaGetLastError ());
+    return 0;
+}
 }
 
 static cudaStream_t tpk_stream (b200m_tpk* h, void* stream) { return h->last_host ? h->own : (cudaStream_t)stream; }
@@ -2294,7 +2319,7 @@ int b200m_tpk_create (b200m_tpk** out, int device, uint32_t n_chan, float fsamp,
     if (e == cudaSuccess) {
         // constructors: TruePeakdsp _res(true) (:29); Kmeterdsp _flag(false), all zero (kmeterdsp.cc:30-40);
         // the 8192-zero pre-roll (:159-168) leaves an all-zero history, which the memset above provides
-        tpk_reset_kernel<<<(n_chan + 127) / 128, 128>>> ((int)n_chan, -1, B200M_TPK_TRUEPEAK, h->st);
+        tpk_reset_kernel<<<(n_chan + 127) / 128, 128>>> ((int)n_chan, -1, B200M_TPK_TRUEPEAK, h->st, nullptr, 0, 1);
         B200M_LAUNCHED (1);
         e = cudaDeviceSynchronize ();
     }
@@ -2374,7 +2399,7 @@ int b200m_tpk_reset (b200m_tpk* h, int32_t chan, void* stream)
 {
     if (!h || chan >= (int32_t)h->n_chan) return set_err (B200M_E_INVAL, "bad argument");
     DeviceGuard g (h->device);
-    tpk_reset_kernel<<<(h->n_chan + 127) / 128, 128, 0, tpk_stream (h, stream)>>> ((int)h->n_chan, chan, h->flags, h->st);
+    tpk_reset_kernel<<<(h->n_chan + 127) / 128, 128, 0, tpk_stream (h, stream)>>> ((int)h->n_chan, chan, h->flags, h->st, nullptr, 0, 1);
     B200M_LAUNCHED (1);
     B200M_CUDA (cudaGetLastError ());
     return 0;
@@ -2386,7 +2411,7 @@ int b200m_tpk_clear (b200m_tpk* h, int32_t chan, void* stream)
     // TruePeakdsp::init's pre-roll, truepeakdsp.cc:159-168).  For slot reuse in shared banks.
     if (!h || chan >= (int32_t)h->n_chan) return set_err (B200M_E_INVAL, "bad argument");
     DeviceGuard g (h->device);
-    tpk_reset_kernel<<<(h->n_chan + 127) / 128, 128, 0, tpk_stream (h, stream)>>> ((int)h->n_chan, chan, h->flags | 4u, h->st);
+    tpk_reset_kernel<<<(h->n_chan + 127) / 128, 128, 0, tpk_stream (h, stream)>>> ((int)h->n_chan, chan, h->flags | 4u, h->st, nullptr, 0, 1);
     B200M_LAUNCHED (1);
     B200M_CUDA (cudaGetLastError ());
     return 0;
@@ -2397,7 +2422,7 @@ int b200m_tpk_reset_kmeter (b200m_tpk* h, void* stream)
     // reset_peaks of the TPnRMS/DR14 plugin resets only its K-meters (src/dr14.c:241-258)
     if (!h) return set_err (B200M_E_INVAL, "NULL handle");
     DeviceGuard g (h->device);
-    tpk_reset_kernel<<<(h->n_chan + 127) / 128, 128, 0, tpk_stream (h, stream)>>> ((int)h->n_chan, -1, h->flags & B200M_TPK_KMETER, h->st);
+    tpk_reset_kernel<<<(h->n_chan + 127) / 128, 128, 0, tpk_stream (h, stream)>>> ((int)h->n_chan, -1, h->flags & B200M_TPK_KMETER, h->st, nullptr, 0, 1);
     B200M_LAUNCHED (1);
     B200M_CUDA (cudaGetLastError ());
     return 0;

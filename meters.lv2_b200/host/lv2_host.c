@@ -15,6 +15,8 @@
  *   needle / COR / dBTP / K-meters (src/meters.cc:59-70): 0 reflevel, 1 in0, 2 out0, 3 level0, 4 in1, 5 out1, 6 level1, 7 peak0, 8 peak1, 9 hold
  *   spectr30 (src/spectrumlv2.c:35-44): 0-59 band / max outputs, 60 speed, 61 reset, 62 amp, 63 state, 64 in0, 65 out0, 66 in1, 67 out1
  *   bitmeter / SigDistHist (src/bitmeter.c, src/sigdistlv2.c port enums): 0 control atom in, 1 notify atom out, 2 in, 3 out
+ *   dr14mono/stereo, TPnRMSmono/stereo (src/dr14.c:27-43): 0 control atom in, 1 follow host transport, 2 reset, 3 block count,
+ *                4 in0, 5 out0, 6-10 outputs of channel 0, 11 in1, 12 out1, 13-17 outputs of channel 1, 18 DR total (no notify port)
  *   surround3..8 (src/surmeter.c:24-70): pair c: 1 + 3c, 2 + 3c input selectors, 3 + 3c correlation; channel c: 13 + 4c in, 14 + 4c out,
  *                15 + 4c level, 16 + 4c peak
  */
@@ -65,7 +67,7 @@ typedef struct {
 typedef struct { const LV2_Descriptor* d; Inst* inst; int first, last; uint32_t nframes; int kind; uint32_t seq_t, chunk_t; pthread_barrier_t *start, *done; int cycles;
                  int cycle; const uint8_t* first_msgs; uint32_t first_len; } Worker;
 
-enum { KIND_MTR, KIND_EBUR, KIND_SPEC, KIND_STATS, KIND_SUR };
+enum { KIND_MTR, KIND_EBUR, KIND_SPEC, KIND_STATS, KIND_SUR, KIND_DR };
 #define ATOM_CAP 8192
 
 /* one event at frame 0: object {otype; controlkey = key (Int); controlval = val (Float)} -- forge_kvcontrolmessage, src/uris.h:279-294 */
@@ -90,6 +92,7 @@ static void run_range (const Worker* w)
 {
     for (int i = w->first; i < w->last; ++i) {
         Inst* p = &w->inst[i];
+        if (w->kind == KIND_DR) { uint32_t* a = (uint32_t*)p->atom_in; a[0] = 8; a[1] = w->seq_t; a[2] = 0; a[3] = 0; }   /* empty input sequence */
         if (w->kind == KIND_EBUR || w->kind == KIND_STATS) {   /* host convention: empty input sequence, output buffer announced as a chunk of its capacity */
             uint32_t* a = (uint32_t*)p->atom_in; a[0] = 8; a[1] = w->seq_t; a[2] = 0; a[3] = 0;
             if (w->cycle == 0 && w->first_len) { memcpy (p->atom_in + 16, w->first_msgs, w->first_len); a[0] = 8 + w->first_len; }   /* the GUI's opening messages */
@@ -139,7 +142,8 @@ int main (int argc, char** argv)
     for (uint32_t i = 0; (d = get (i)) != NULL; ++i) if (!strcmp (d->URI, full)) break;
     if (!d) { fprintf (stderr, "%s not served by %s\n", full, lib); return 1; }
     const int kind = !strcmp (uri, "EBUr128") ? KIND_EBUR : !strncmp (uri, "spectr30", 8) ? KIND_SPEC
-                   : !strcmp (uri, "bitmeter") || !strcmp (uri, "SigDistHist") ? KIND_STATS : !strncmp (uri, "surround", 8) ? KIND_SUR : KIND_MTR;
+                   : !strcmp (uri, "bitmeter") || !strcmp (uri, "SigDistHist") ? KIND_STATS : !strncmp (uri, "surround", 8) ? KIND_SUR
+                   : !strncmp (uri, "dr14", 4) || !strncmp (uri, "TPnRMS", 6) ? KIND_DR : KIND_MTR;
     const int stereo = kind == KIND_EBUR || strstr (uri, "stereo") || !strcmp (uri, "COR") || !strcmp (uri, "BBCM6");
     const int chn = kind == KIND_SUR ? uri[8] - '0' : stereo ? 2 : 1;
 
@@ -179,6 +183,13 @@ int main (int argc, char** argv)
             p->ctl[60] = 1.0f; p->ctl[61] = -4.0f; p->ctl[62] = 0.0f;
             d->connect_port (p->h, 64, p->in[0]); d->connect_port (p->h, 65, p->out[0]);
             if (stereo) { d->connect_port (p->h, 66, p->in[1]); d->connect_port (p->h, 67, p->out[1]); }
+        } else if (kind == KIND_DR) {
+            p->atom_in = (uint8_t*)calloc (1, 1024);
+            d->connect_port (p->h, 0, p->atom_in);
+            for (uint32_t k = 1; k < 19; ++k) if (k != 4 && k != 5 && k != 11 && k != 12) d->connect_port (p->h, k, &p->ctl[k]);
+            p->ctl[1] = 1.0f;                                   /* follow host transport (the plugin's default) */
+            d->connect_port (p->h, 4, p->in[0]); d->connect_port (p->h, 5, p->out[0]);
+            if (stereo) { d->connect_port (p->h, 11, p->in[1]); d->connect_port (p->h, 12, p->out[1]); }
         } else if (kind == KIND_SUR) {
             for (uint32_t k = 0; k < 13; ++k) d->connect_port (p->h, k, &p->ctl[k]);
             for (int c = 0; c < 4; ++c) { p->ctl[1 + 3 * c] = (float)c; p->ctl[2 + 3 * c] = (float)((c + 1) % chn); }   /* adjacent channel pairs */
@@ -213,7 +224,7 @@ int main (int argc, char** argv)
     }
     for (int t = 0; t < threads; ++t) pthread_join (th[t], NULL);
     const double mean = sum / cycles, budget = nframes / rate;
-    float probe = kind == KIND_EBUR || kind == KIND_STATS ? 0.0f : inst[0].ctl[3];
+    float probe = kind == KIND_EBUR || kind == KIND_STATS ? 0.0f : inst[0].ctl[kind == KIND_DR ? 6 : 3];
     const char* batch = getenv ("B200M_LV2_BATCH");
     printf ("{\"lv2_host\": \"%s\", \"lib\": \"%s\", \"instances\": %d, \"threads\": %d, \"nframes\": %u, \"rate\": %.0f, \"cycles\": %d, "
             "\"dbtp\": %d, \"ui\": %d, \"batch_slots\": %s, \"cycle_ms_mean\": %.4f, \"cycle_ms_max\": %.4f, \"us_per_instance\": %.3f, \"budget_ms\": %.3f, \"fits_realtime\": %s, "
