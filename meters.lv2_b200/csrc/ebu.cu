@@ -13,6 +13,7 @@
 #include <stdlib.h>
 #include <cuda.h>
 #include <algorithm>
+#include <map>
 #include <vector>
 #include "common.cuh"
 #include "ebu_kw.cuh"
@@ -157,7 +158,8 @@ struct TmaStage {
     }
 };
 
-template <int NCHAN, bool ALIGNED>
+// PHASES: the bank's instances have several fragment phases (ck.fph); without it the chunk-list policy is compiled alone
+template <int NCHAN, bool ALIGNED, bool PHASES>
 __global__ void __launch_bounds__ (EBU_WARPS * 32)
 ebu_kweight_frag (const float* __restrict__ in, size_t stride, int nchans, int k_first, int k_end, int nfram, EbuCoef cf, EbuChunks ck,
                   float fragm_f, float* __restrict__ zst, float* __restrict__ frpwr, float* __restrict__ fragpw, int n_inst, int pdl_trigger)
@@ -173,8 +175,8 @@ ebu_kweight_frag (const float* __restrict__ in, size_t stride, int nchans, int k
     if (k0 >= k_end) return;                           // warp-uniform; warps never synchronise with each other
     PaddedStage<ALIGNED> sg;
     sg.init (in, stride, ebu_smem + warp * EBU_WARP_FLOATS, lane, k0, k_end, nfram);
-    kw_warp<NCHAN> (sg, lane, min (k0 + lane, k_end - 1) /* tail lanes shadow the last channel (no stores) */, lane < CPW && (k0 + lane) < k_end,
-                    nchans, nfram, cf, ck, fragm_f, zst, frpwr, fragpw, n_inst);
+    kw_warp<NCHAN, PHASES> (sg, lane, min (k0 + lane, k_end - 1) /* tail lanes shadow the last channel (no stores) */, lane < CPW && (k0 + lane) < k_end,
+                            nchans, nfram, cf, ck, fragm_f, zst, frpwr, fragpw, n_inst);
 }
 
 // ---- K1 split over two warps per 32 channels -------------------------------------------------------------------------------
@@ -185,6 +187,7 @@ ebu_kweight_frag (const float* __restrict__ in, size_t stride, int nchans, int k
 // double-buffered shared-memory tile; the two chains then interleave on one scheduler.  Every channel sees exactly the same
 // operations in the same order as in kw_warp, so the results stay bit-identical.  Named barriers (bar.arrive / bar.sync on 64
 // threads) hand the tiles over: a waiting warp is parked by the hardware and takes no issue slots from its partner.
+// It knows the warp-uniform chunk list only: a bank whose instances have several fragment phases runs ebu_kweight_frag instead.
 // It is slower than the one-warp kernel, so it is opt-in (B200M_EBU_SPLIT=1) and kept for the record: the one-warp kernel is limited
 // by the ~21.5 instructions it must ISSUE per sample on its scheduler, not by the 16-cycle chains; a second warp on the SAME scheduler
 // adds hand-over instructions and barrier waits without adding issue slots, and every scheduler in use already hosts a warp.
@@ -331,7 +334,8 @@ ebu_kweight_split (const float* __restrict__ in, size_t stride, int nchans, int 
     }
 }
 
-// the same kernel fed by TMA (16-byte aligned input with a 16-byte multiple row pitch: every bank-sized call in practice)
+// the same kernel fed by TMA (16-byte aligned input with a 16-byte multiple row pitch: every bank-sized call in practice); the chunk
+// list only, like ebu_kweight_split: a bank with several fragment phases runs ebu_kweight_frag
 constexpr int EBU_TMA_SMEM = EBU_WARPS * EBU_STAGES * TmaStage::STAGE_BYTES + EBU_WARPS * EBU_STAGES * 8 + 1024;
 template <int NCHAN>
 __global__ void __launch_bounds__ (EBU_WARPS * 32)
@@ -349,11 +353,12 @@ ebu_kweight_tma (const __grid_constant__ CUtensorMap tmap, int nchans, int k_fir
     TmaStage sg;
     sg.init (&tmap, base + warp * EBU_STAGES * TmaStage::STAGE_BYTES, bars, lane, k0, nfram);
     // rows >= k_end read as zeros (or as the neighbouring slice's channels): those lanes never store
-    kw_warp<NCHAN> (sg, lane, min (k0 + lane, k_end - 1), (k0 + lane) < k_end, nchans, nfram, cf, ck, fragm_f, zst, frpwr, fragpw, n_inst);
+    kw_warp<NCHAN, false> (sg, lane, min (k0 + lane, k_end - 1), (k0 + lane) < k_end, nchans, nfram, cf, ck, fragm_f, zst, frpwr, fragpw, n_inst);
 }
 
 // ---- K2: per-fragment loudness, histograms, gated integration ------------------------------
-struct EbuCtl { int div1, div2, integr, calc; };
+// wrind: the instance's 64-slot ring write index (_wrind); padded to 32 bytes so that K2a moves it with two 16-byte accesses
+struct __align__ (16) EbuCtl { int div1, div2, integr, calc, wrind, pad[3]; };
 
 // Ebu_r128_hist::integrate (:82-102).  `c[t]` holds bin t*32+lane.  Only non-zero bins change the
 // running float sum, so the warp walks them in bin order (ballot) and applies the "/= 10 after
@@ -447,17 +452,23 @@ B200M_DEV void hist_calc_range (const int* row, int count, const float* bp, int 
 // K2a: one THREAD per instance, one completed 50 ms fragment (process :217-243 minus the gated statistics).
 // ring layout [64][n_inst] so that lane = instance accesses coalesce; each thread parks its 64-slot ring column
 // in shared memory (column private to the thread: no barrier needed) for the two ordered sums.
+// Launch `frag` handles row `frag` of fragpw: with one phase for the bank every instance's fragment `frag` of the K1 launch; with
+// per-instance phases (fph) each instance's fragment `frag` of the block, if the block of `nfram` frames from bank time tmod has one.
 constexpr int K2A_THREADS = 128;
 
 __global__ void __launch_bounds__ (K2A_THREADS)
-ebu_fragment_kernel (int n_inst, int frag, int wrind, const float* __restrict__ fragpw, float* __restrict__ ring,
-                     EbuCtl* __restrict__ ctl, b200m_ebu_result* __restrict__ res, int* __restrict__ histM,
+ebu_fragment_kernel (int n_inst, int frag, const int* __restrict__ fph, int tmod, int fragm, int nfram, const float* __restrict__ fragpw,
+                     float* __restrict__ ring, EbuCtl* __restrict__ ctl, b200m_ebu_result* __restrict__ res, int* __restrict__ histM,
                      int* __restrict__ histS, int* __restrict__ cnt)
 {
     __shared__ float sring[64][K2A_THREADS];
     const int tid = threadIdx.x;
     const int i = blockIdx.x * K2A_THREADS + tid;
     if (i >= n_inst) return;
+    if (fph) {
+        int el = (tmod - fph[i]) % fragm; if (el < 0) el += fragm;
+        if (fragm - el + frag * fragm > nfram) return;     // the instance's edge `frag` lies beyond this block
+    }
     // all 64 ring slots in flight at once (one round of memory latency, not 64): cp.async straight into the column
 #pragma unroll
     for (int w = 0; w < 64; ++w) cp_async4 (&sring[w][tid], ring + (size_t)w * n_inst + i, 4);
@@ -465,10 +476,12 @@ ebu_fragment_kernel (int n_inst, int frag, int wrind, const float* __restrict__ 
     EbuCtl c = ctl[i];
     b200m_ebu_result r = res[i];
     const float p = fragpw[(size_t)frag * n_inst + i];
+    const int wrind = c.wrind;
     cp_async_wait<0> ();
     sring[wrind][tid] = p;                                 // _power[_wrind++] = _frpwr / _fragm (:218)
     ring[(size_t)wrind * n_inst + i] = p;
     const int wr = (wrind + 1) & 63;
+    c.wrind = wr;
     r.frag_power = p;
     // addfrags (8), addfrags (60) (:251-260): sequential sums, oldest fragment first
     float s8 = 0.0f, s60 = 0.0f;
@@ -535,9 +548,10 @@ ebu_gate_kernel (int n_inst, EbuCtl* __restrict__ ctl, b200m_ebu_result* __restr
     }
 }
 
-// reset / integration control, one thread per instance
+// reset / integration control, one thread per instance.  tph >= 0 (cmd 3 only): the instance's clock restarts at bank time tph --
+// fragment phase and ring write index -- as in reset(); tph = -1 keeps both (b200m_ebu_clear)
 __global__ void ebu_ctl_kernel (int n_inst, int inst_sel, int cmd, int nchan, float* zst, float* frpwr, float* ring,
-                                EbuCtl* ctl, b200m_ebu_result* res, int* histM, int* histS, int* cnt)
+                                EbuCtl* ctl, b200m_ebu_result* res, int* histM, int* histS, int* cnt, int* fph, int tph)
 {
     const int i = blockIdx.x * blockDim.x + threadIdx.x;
     if (i >= n_inst || (inst_sel >= 0 && i != inst_sel)) return;
@@ -558,6 +572,7 @@ __global__ void ebu_ctl_kernel (int n_inst, int inst_sel, int cmd, int nchan, fl
         for (int b = 0; b < 64; ++b) ring[(size_t)b * n_inst + i] = 0.0f;
         const size_t nch = (size_t)n_inst * nchan;
         for (int c = 0; c < nchan; ++c) for (int z = 0; z < 4; ++z) zst[z * nch + (size_t)i * nchan + c] = 0.0f;
+        if (tph >= 0) { fph[i] = tph; ctl[i].wrind = 0; }
     }
     res[i] = r;
 }
@@ -625,31 +640,57 @@ static bool tma_input_map (CUtensorMap* tm, const float* base, size_t stride, ui
     return ebu_tma_map (tm, base, stride, rows, cols, 32, 32, true);
 }
 
+// The bank's sample clock T is kept on the host as tmod = T mod fragm.  Instance i's 50 ms fragment clock last started at bank
+// time fph[i] (mod fragm): a device value that only the control kernel writes, mirrored on the host in ph[i].  Its next edge
+// lies fragm - ((T - fph[i]) mod fragm) frames ahead.
+struct EbuPhase { int n = 0, G = 0; int cnt10[10] = {0}; };   // one phase class: members, fragment counter mod 10, S-period census
+
 struct b200m_ebu {
     int device; uint32_t n_inst, nchan; float fsamp; int fragm;
-    int frcnt, wrind;                    // shared 50 ms fragment clock (host-tracked, see b200meters.h)
+    int tmod = 0;                        // bank time mod fragm
+    int fragrows = EBU_MAXCHUNK;         // rows of d_fragpw: the most fragments one K1 launch completes per instance
     EbuCoef cf;
     float *d_z = nullptr, *d_frpwr = nullptr, *d_fragpw = nullptr, *d_ring = nullptr, *d_binpow = nullptr, *d_out5 = nullptr;
     EbuCtl* d_ctl = nullptr; b200m_ebu_result* d_res = nullptr;
-    int *d_histM = nullptr, *d_histS = nullptr, *d_cnt = nullptr;
+    int *d_histM = nullptr, *d_histS = nullptr, *d_cnt = nullptr, *d_fph = nullptr;
     cudaStream_t own = nullptr; HostStage stage; bool last_host = false;
     bool use_tma = false;                // K1 tiles by TMA (opt-in, 16-byte aligned input only) instead of cp.async
     bool split = false;                  // K1 as two warps per 32 channels (ebu_kweight_split), opt-in with B200M_EBU_SPLIT=1: measured slower, see the kernel
-    // Host mirror of every instance's S-histogram period (_div2, :234-241), kept in O(1) per fragment: an
-    // integrating instance has div2 = (G - base) mod 10 where G counts fragments; cnt10[r] = number of integrating
-    // instances with base = r.  The gated-statistics kernel (K2b) is launched only for fragments where some
-    // instance wraps, i.e. cnt10[G] > 0.
-    std::vector<uint8_t> integ, base, frozen; int cnt10[10]; int G = 0;
-    void phase_reset () { integ.assign (n_inst, 0); base.assign (n_inst, 0); frozen.assign (n_inst, 0); for (int& c : cnt10) c = 0; G = 0; }
+    // Host mirror of every instance's S-histogram period (_div2, :234-241), kept in O(1) per fragment and phase class: the
+    // instances that share a fragment phase form a class whose G counts their fragments; an integrating instance has
+    // div2 = (G - base) mod 10 and cnt10[r] = number of integrating members with base = r.  The gated-statistics kernel (K2b)
+    // is launched only behind fragments where some class has cnt10[G] > 0.  The classes are ordered by phase.
+    std::vector<uint8_t> integ, base, frozen; std::vector<int> ph;
+    std::map<int, EbuPhase> cls;
+    std::vector<int> nf;                 // per class: fragments it completes in the block being launched (scratch)
+    void phase_reset () {
+        integ.assign (n_inst, 0); base.assign (n_inst, 0); frozen.assign (n_inst, 0); ph.assign (n_inst, tmod);
+        cls.clear (); cls[tmod].n = (int)n_inst;
+    }
     void phase_ctl (int32_t inst, int cmd) {
         for (uint32_t i = 0; i < n_inst; ++i) {
             if (inst >= 0 && (uint32_t)inst != i) continue;
-            if (cmd == 0 && integ[i]) { frozen[i] = (uint8_t)((G - base[i] + 10) % 10); cnt10[base[i]]--; integ[i] = 0; }
-            else if (cmd == 1 && !integ[i]) { base[i] = (uint8_t)((G - frozen[i] + 10) % 10); cnt10[base[i]]++; integ[i] = 1; }
-            else if (cmd == 2) { if (integ[i]) { cnt10[base[i]]--; base[i] = (uint8_t)G; cnt10[base[i]]++; } else frozen[i] = 0; }
+            EbuPhase& c = cls[ph[i]];
+            if (cmd == 0 && integ[i]) { frozen[i] = (uint8_t)((c.G - base[i] + 10) % 10); c.cnt10[base[i]]--; integ[i] = 0; }
+            else if (cmd == 1 && !integ[i]) { base[i] = (uint8_t)((c.G - frozen[i] + 10) % 10); c.cnt10[base[i]]++; integ[i] = 1; }
+            else if (cmd == 2) { if (integ[i]) { c.cnt10[base[i]]--; base[i] = (uint8_t)c.G; c.cnt10[base[i]]++; } else frozen[i] = 0; }
         }
     }
-    bool phase_tick () { G = (G + 1) % 10; return cnt10[G] > 0; }     // one fragment completed: does anyone wrap?
+    // reset() of one instance: integration off, div counters cleared, its clock restarted now
+    void phase_restart (uint32_t i) {
+        phase_ctl ((int32_t)i, 0); phase_ctl ((int32_t)i, 2);
+        auto it = cls.find (ph[i]);
+        if (--it->second.n == 0) cls.erase (it);
+        ph[i] = tmod; cls[tmod].n++;
+    }
+    // fragments that instances of phase p complete in the next nfram frames
+    int frags_in (int p, uint32_t nfram) const {
+        int el = (tmod - p) % fragm; if (el < 0) el += fragm;
+        const int e0 = fragm - el;
+        return e0 <= (int)nfram ? 1 + ((int)nfram - e0) / fragm : 0;
+    }
+    int frcnt_of (int p) const { int el = (tmod - p) % fragm; if (el < 0) el += fragm; return fragm - el; }
+    static bool phase_tick (EbuPhase& c) { c.G = (c.G + 1) % 10; return c.cnt10[c.G] > 0; }   // one fragment of the class: does anyone wrap?
 };
 
 // Host-side coefficient design; restates Ebu_r128_proc::detect_init (ebu_r128_proc.cc:263-293).
@@ -681,10 +722,12 @@ static int ebu_ctl (b200m_ebu* h, int32_t inst, int cmd, void* stream)
     if (!h) return set_err (B200M_E_INVAL, "NULL handle");
     if (inst >= (int32_t)h->n_inst) return set_err (B200M_E_INVAL, "instance %d out of range", inst);
     DeviceGuard g (h->device);
-    if (cmd == 3) h->phase_reset (); else h->phase_ctl (inst, cmd);
+    if (cmd == 3) { if (inst < 0) h->phase_reset (); else h->phase_restart ((uint32_t)inst); }
+    else h->phase_ctl (inst, cmd);
     // after process_host the bank runs on its own stream: a control on any other stream would race with the kernels in flight
     ebu_ctl_kernel<<<(h->n_inst + 127) / 128, 128, 0, h->last_host ? h->own : (cudaStream_t)stream>>> (
-        (int)h->n_inst, inst, cmd, (int)h->nchan, h->d_z, h->d_frpwr, h->d_ring, h->d_ctl, h->d_res, h->d_histM, h->d_histS, h->d_cnt);
+        (int)h->n_inst, inst, cmd, (int)h->nchan, h->d_z, h->d_frpwr, h->d_ring, h->d_ctl, h->d_res, h->d_histM, h->d_histS, h->d_cnt,
+        h->d_fph, cmd == 3 ? h->tmod : -1);
     B200M_LAUNCHED (1);
     B200M_CUDA (cudaGetLastError ());
     return 0;
@@ -713,7 +756,8 @@ int b200m_ebu_create (b200m_ebu** out, int device, uint32_t n_inst, uint32_t nch
     if (!h) return set_err (B200M_E_NOMEM, "host allocation failed");
     h->device = device; h->n_inst = n_inst; h->nchan = nchan; h->fsamp = fsamp;
     h->fragm = (int)fsamp / 20;                     // :170
-    h->frcnt = h->fragm; h->wrind = 0;
+    // with per-instance phases one K1 launch covers a whole block (a split would add a cut the reference does not make)
+    h->fragrows = std::max<int> (EBU_MAXCHUNK, (int)(B200M_MAX_BLOCK / (uint32_t)h->fragm) + 2);
     ebu_design (fsamp, h->cf);
     const size_t nch = (size_t)n_inst * nchan;
     float bp[100];
@@ -722,7 +766,7 @@ int b200m_ebu_create (b200m_ebu** out, int device, uint32_t n_inst, uint32_t nch
     auto A = [&] (void** p, size_t bytes) { if (e == cudaSuccess) { e = cudaMalloc (p, bytes); if (e == cudaSuccess) e = cudaMemset (*p, 0, bytes); } };
     A ((void**)&h->d_z, 4 * nch * sizeof (float));
     A ((void**)&h->d_frpwr, n_inst * sizeof (float));
-    A ((void**)&h->d_fragpw, (size_t)EBU_MAXCHUNK * n_inst * sizeof (float));
+    A ((void**)&h->d_fragpw, (size_t)h->fragrows * n_inst * sizeof (float));
     A ((void**)&h->d_ring, (size_t)64 * n_inst * sizeof (float));
     A ((void**)&h->d_binpow, 100 * sizeof (float));
     A ((void**)&h->d_out5, 8 * sizeof (float));
@@ -731,16 +775,19 @@ int b200m_ebu_create (b200m_ebu** out, int device, uint32_t n_inst, uint32_t nch
     A ((void**)&h->d_histM, (size_t)HIST_PITCH * n_inst * sizeof (int));
     A ((void**)&h->d_histS, (size_t)HIST_PITCH * n_inst * sizeof (int));
     A ((void**)&h->d_cnt, (size_t)4 * n_inst * sizeof (int));
+    A ((void**)&h->d_fph, n_inst * sizeof (int));
     if (e == cudaSuccess) e = cudaMemcpy (h->d_binpow, bp, sizeof (bp), cudaMemcpyHostToDevice);
     if (e == cudaSuccess) e = cudaStreamCreateWithFlags (&h->own, cudaStreamNonBlocking);
     // K1 carries 102 KB of dynamic shared memory per CTA
     // ... and asks for the largest shared-memory carveout: with the default the driver configures the SM for just what this kernel
     // needs (132 KB), which leaves room for ONE CTA of the true-peak kernel that is meant to share the SM with it (r128.cu)
-#define EBU_ATTR(NC, AL) if (e == cudaSuccess) e = cudaFuncSetAttribute (ebu_kweight_frag<NC, AL>, cudaFuncAttributeMaxDynamicSharedMemorySize, EBU_SMEM_BYTES); \
-    if (e == cudaSuccess) e = cudaFuncSetAttribute (ebu_kweight_frag<NC, AL>, cudaFuncAttributePreferredSharedMemoryCarveout, cudaSharedmemCarveoutMaxShared)
+#define EBU_ATTR1(NC, AL, PH) if (e == cudaSuccess) e = cudaFuncSetAttribute (ebu_kweight_frag<NC, AL, PH>, cudaFuncAttributeMaxDynamicSharedMemorySize, EBU_SMEM_BYTES); \
+    if (e == cudaSuccess) e = cudaFuncSetAttribute (ebu_kweight_frag<NC, AL, PH>, cudaFuncAttributePreferredSharedMemoryCarveout, cudaSharedmemCarveoutMaxShared)
+#define EBU_ATTR(NC, AL) EBU_ATTR1 (NC, AL, false); EBU_ATTR1 (NC, AL, true)
     EBU_ATTR (1, true); EBU_ATTR (1, false); EBU_ATTR (2, true); EBU_ATTR (2, false);
     EBU_ATTR (3, true); EBU_ATTR (3, false); EBU_ATTR (4, true); EBU_ATTR (4, false); EBU_ATTR (5, true); EBU_ATTR (5, false);
 #undef EBU_ATTR
+#undef EBU_ATTR1
     if (e == cudaSuccess) e = cudaFuncSetAttribute (ebu_kweight_tma<1>, cudaFuncAttributeMaxDynamicSharedMemorySize, EBU_TMA_SMEM);
     if (e == cudaSuccess) e = cudaFuncSetAttribute (ebu_kweight_tma<2>, cudaFuncAttributeMaxDynamicSharedMemorySize, EBU_TMA_SMEM);
     if (e == cudaSuccess) e = cudaFuncSetAttribute (ebu_kweight_tma<1>, cudaFuncAttributePreferredSharedMemoryCarveout, cudaSharedmemCarveoutMaxShared);
@@ -770,7 +817,7 @@ int b200m_ebu_destroy (b200m_ebu* h)
     DeviceGuard g (h->device);
     cudaDeviceSynchronize ();
     cudaFree (h->d_z); cudaFree (h->d_frpwr); cudaFree (h->d_fragpw); cudaFree (h->d_ring); cudaFree (h->d_binpow);
-    cudaFree (h->d_out5); cudaFree (h->d_ctl); cudaFree (h->d_res); cudaFree (h->d_histM); cudaFree (h->d_histS); cudaFree (h->d_cnt);
+    cudaFree (h->d_out5); cudaFree (h->d_ctl); cudaFree (h->d_res); cudaFree (h->d_histM); cudaFree (h->d_histS); cudaFree (h->d_cnt); cudaFree (h->d_fph);
     h->stage.release ();
     if (h->own) cudaStreamDestroy (h->own);
     delete h;
@@ -780,19 +827,19 @@ int b200m_ebu_destroy (b200m_ebu* h)
 int b200m_ebu_reset (b200m_ebu* h, int32_t inst, void* stream)
 {
     if (!h) return set_err (B200M_E_INVAL, "NULL handle");
-    if (inst != -1) return set_err (B200M_E_UNSUPPORTED, "reset() restarts the shared fragment clock: only inst = -1");
-    h->frcnt = h->fragm; h->wrind = 0;
-    return ebu_ctl (h, -1, 3, stream);
+    if (inst < -1) return set_err (B200M_E_INVAL, "instance %d out of range", inst);
+    return ebu_ctl (h, inst, 3, stream);         // the instance's (every instance's) clock restarts at the current bank time
 }
 int b200m_ebu_clear (b200m_ebu* h, int32_t inst, void* stream)
 {
     // what reset() does to ONE instance -- integration off, filter states, 64-fragment ring, loudness values, histograms -- without
-    // restarting the bank's shared 50 ms fragment clock
+    // restarting its 50 ms fragment clock
     if (!h || inst < 0 || inst >= (int32_t)h->n_inst) return set_err (B200M_E_INVAL, "bad argument");
     DeviceGuard g (h->device);
     h->phase_ctl (inst, 0); h->phase_ctl (inst, 2);
     ebu_ctl_kernel<<<(h->n_inst + 127) / 128, 128, 0, h->last_host ? h->own : (cudaStream_t)stream>>> (
-        (int)h->n_inst, inst, 3, (int)h->nchan, h->d_z, h->d_frpwr, h->d_ring, h->d_ctl, h->d_res, h->d_histM, h->d_histS, h->d_cnt);
+        (int)h->n_inst, inst, 3, (int)h->nchan, h->d_z, h->d_frpwr, h->d_ring, h->d_ctl, h->d_res, h->d_histM, h->d_histS, h->d_cnt,
+        h->d_fph, -1);
     B200M_LAUNCHED (1);
     B200M_CUDA (cudaGetLastError ());
     return 0;
@@ -820,7 +867,8 @@ static uint32_t ebu_plan_chunks (int& frcnt, int fragm, uint32_t rem, EbuChunks&
 
 bool ebu_single_k1 (const b200m_ebu* h, uint32_t nfram)
 {
-    int frcnt = h->frcnt, nfrag; EbuChunks ck;
+    if (h->cls.size () > 1) return true;             // per-instance phases: always one launch per block
+    int frcnt = h->frcnt_of (h->cls.begin ()->first), nfrag; EbuChunks ck;
     return ebu_plan_chunks (frcnt, h->fragm, nfram, ck, nfrag) == nfram;
 }
 
@@ -835,10 +883,21 @@ int ebu_process_sliced (b200m_ebu* h, const float* d_in, size_t stride, uint32_t
 {
     const int nch = (int)(h->n_inst * h->nchan);
     const bool aligned = ((uintptr_t)d_in % 16 == 0) && (stride % 4 == 0);
+    // one phase class: the warp-uniform chunk list, split over launches of at most EBU_MAXCHUNK chunks; several: one launch per
+    // block, every lane cutting at its own instance's fragment edges
+    const bool multi = h->cls.size () > 1;
+    int frcnt = multi ? 0 : h->frcnt_of (h->cls.begin ()->first);
     uint32_t done = 0;
     while (done < nfram) {
-        EbuChunks ck; int nfrag;
-        const uint32_t pos = ebu_plan_chunks (h->frcnt, h->fragm, nfram - done, ck, nfrag);
+        EbuChunks ck; int nfrag = 0;
+        uint32_t pos = nfram;
+        ck.tmod = h->tmod; ck.fragm = h->fragm; ck.fph = nullptr;
+        if (multi) {
+            ck.n = 0; ck.v[0] = 0; ck.fph = h->d_fph;
+            h->nf.clear ();
+            for (const auto& c : h->cls) { h->nf.push_back (h->frags_in (c.first, nfram)); nfrag = std::max (nfrag, h->nf.back ()); }
+        }
+        else pos = ebu_plan_chunks (frcnt, h->fragm, nfram - done, ck, nfrag);
         const float* src = d_in + done;
         const bool fused = k1_fused && done == 0 && pos == nfram && nsl == 1 && bounds[0] == 0 && bounds[1] == h->n_inst;
         if (fused) {
@@ -847,7 +906,7 @@ int ebu_process_sliced (b200m_ebu* h, const float* d_in, size_t stride, uint32_t
         }
         const bool al = aligned && (done % 4 == 0);
         CUtensorMap tmap;
-        const bool tma = !fused && al && h->use_tma && h->nchan <= 2 && tma_input_map (&tmap, src, stride, (uint32_t)nch, pos);
+        const bool tma = !fused && !multi && al && h->use_tma && h->nchan <= 2 && tma_input_map (&tmap, src, stride, (uint32_t)nch, pos);
         for (int sl = 0; !fused && sl < nsl; ++sl) {
             const int kf = (int)(bounds[sl] * h->nchan), ke = (int)(bounds[sl + 1] * h->nchan);
             if (ke <= kf) continue;
@@ -855,7 +914,8 @@ int ebu_process_sliced (b200m_ebu* h, const float* d_in, size_t stride, uint32_t
             const int cpw = (32 / (int)h->nchan) * (int)h->nchan;          // a warp takes whole instances only
             const int nwarps = (ke - kf + cpw - 1) / cpw;
             dim3 grid ((nwarps + EBU_WARPS - 1) / EBU_WARPS), blk (EBU_WARPS * 32);
-#define EBU_K1(NC, AL) ebu_kweight_frag<NC, AL><<<grid, blk, EBU_SMEM_BYTES, st>>> (src, stride, nch, kf, ke, (int)pos, h->cf, ck, (float)h->fragm, h->d_z, h->d_frpwr, h->d_fragpw, (int)h->n_inst, (after_k1 && done == 0) ? 1 : 0)
+#define EBU_K1P(NC, AL, PH) ebu_kweight_frag<NC, AL, PH><<<grid, blk, EBU_SMEM_BYTES, st>>> (src, stride, nch, kf, ke, (int)pos, h->cf, ck, (float)h->fragm, h->d_z, h->d_frpwr, h->d_fragpw, (int)h->n_inst, (after_k1 && done == 0) ? 1 : 0)
+#define EBU_K1(NC, AL) do { if (multi) EBU_K1P (NC, AL, true); else EBU_K1P (NC, AL, false); } while (0)
 #define EBU_K1T(NC) ebu_kweight_tma<NC><<<grid, blk, EBU_TMA_SMEM, st>>> (tmap, nch, kf, ke, (int)pos, h->cf, ck, (float)h->fragm, h->d_z, h->d_frpwr, h->d_fragpw, (int)h->n_inst, (after_k1 && done == 0) ? 1 : 0)
             if (h->nchan > 2) {                                  // surround banks (3..5 channels): the one-warp kernel, lanes grouped per instance
                 switch (h->nchan * 2 + (al ? 1 : 0)) {
@@ -864,7 +924,7 @@ int ebu_process_sliced (b200m_ebu* h, const float* d_in, size_t stride, uint32_t
                 case 11: EBU_K1 (5, true); break; default: EBU_K1 (5, false); break;
                 }
             }
-            else if (h->split && !tma) {
+            else if (h->split && !tma && !multi) {           // the opt-in variants know the chunk list only
                 dim3 sgrid ((nwarps + EBU_SPLIT_PAIRS - 1) / EBU_SPLIT_PAIRS), sblk (2 * EBU_SPLIT_PAIRS * 32);
 #define EBU_K1S(NC, AL) ebu_kweight_split<NC, AL><<<sgrid, sblk, EBU_SPLIT_SMEM, st>>> (src, stride, nch, kf, ke, (int)pos, h->cf, ck, (float)h->fragm, h->d_z, h->d_frpwr, h->d_fragpw, (int)h->n_inst, (after_k1 && done == 0) ? 1 : 0)
                 if (h->nchan == 1) { if (al) EBU_K1S (1, true); else EBU_K1S (1, false); }
@@ -875,16 +935,24 @@ int ebu_process_sliced (b200m_ebu* h, const float* d_in, size_t stride, uint32_t
             else if (h->nchan == 1) { if (al) EBU_K1 (1, true); else EBU_K1 (1, false); }
             else               { if (al) EBU_K1 (2, true); else EBU_K1 (2, false); }
 #undef EBU_K1
+#undef EBU_K1P
 #undef EBU_K1T
             B200M_LAUNCHED (1);
         }
         if (after_k1 && done == 0) { if (int rc = after_k1 (after_arg)) return rc; }      // work to enqueue right behind the first K1
         for (int f = 0; f < nfrag; ++f) {                    // fragments complete in order; each may trigger gating
             ebu_fragment_kernel<<<(h->n_inst + K2A_THREADS - 1) / K2A_THREADS, K2A_THREADS, 0, st>>> (
-                (int)h->n_inst, f, h->wrind, h->d_fragpw, h->d_ring, h->d_ctl, h->d_res, h->d_histM, h->d_histS, h->d_cnt);
+                (int)h->n_inst, f, ck.fph, h->tmod, h->fragm, (int)nfram, h->d_fragpw, h->d_ring, h->d_ctl, h->d_res, h->d_histM, h->d_histS, h->d_cnt);
             B200M_LAUNCHED (1);
-            h->wrind = (h->wrind + 1) & 63;
-            if (h->phase_tick ()) {
+            // K2b behind fragment f only if some class completing its fragment f has an integrating member whose S period wraps
+            // there: a later addpoint in the same block would otherwise be gated into the statistics
+            bool wrap = false;
+            int q = 0;
+            for (auto& c : h->cls) {
+                if (!multi || f < h->nf[q]) wrap |= b200m_ebu::phase_tick (c.second);
+                ++q;
+            }
+            if (wrap) {
                 ebu_gate_kernel<<<(h->n_inst + K2B_WARPS - 1) / K2B_WARPS, K2B_WARPS * 32, 0, st>>> (
                     (int)h->n_inst, h->d_ctl, h->d_res, h->d_histM, h->d_histS, h->d_cnt, h->d_binpow);
                 B200M_LAUNCHED (1);
@@ -892,6 +960,7 @@ int ebu_process_sliced (b200m_ebu* h, const float* d_in, size_t stride, uint32_t
         }
         done += pos;
     }
+    h->tmod = (int)((h->tmod + nfram) % (uint32_t)h->fragm);
     B200M_CUDA (cudaGetLastError ());
     return 0;
 }
@@ -947,10 +1016,13 @@ int b200m_ebu_histogram (b200m_ebu* h, uint32_t inst, int32_t* hist_M, int32_t* 
 }
 
 // ---- snapshot / restore (SURVEY §5: the reference never saves DSP state; a batch engine integrating for hours should) ----
-// blob = header, the host-side clocks and phase book-keeping, then every device state array in a fixed order
+// blob = header (the bank time mod fragm), the host-side phase book-keeping per instance (phase int32, then integ, base, frozen
+// and its phase class's fragment counter G as bytes), then every device state array in a fixed order.  The class census is
+// rebuilt from the per-instance entries.
 namespace {
-struct EbuSnapHead { uint32_t magic, n_inst, nchan; float fsamp; int32_t frcnt, wrind, G, cnt10[10]; };
-constexpr uint32_t EBU_SNAP_MAGIC = 0x42453031u;              // "BE01"
+struct EbuSnapHead { uint32_t magic, n_inst, nchan; float fsamp; int32_t tmod, pad[3]; };
+constexpr uint32_t EBU_SNAP_MAGIC = 0x42453032u;              // "BE02": per-instance fragment phases
+constexpr size_t EBU_SNAP_HOST_PER_INST = 8;
 struct EbuSeg { void* p; size_t bytes; };
 int ebu_segments (b200m_ebu* h, EbuSeg* seg)
 {
@@ -959,7 +1031,7 @@ int ebu_segments (b200m_ebu* h, EbuSeg* seg)
     seg[k++] = {h->d_z, 4 * nch * sizeof (float)}; seg[k++] = {h->d_frpwr, n * sizeof (float)}; seg[k++] = {h->d_ring, 64 * n * sizeof (float)};
     seg[k++] = {h->d_ctl, n * sizeof (EbuCtl)}; seg[k++] = {h->d_res, n * sizeof (b200m_ebu_result)};
     seg[k++] = {h->d_histM, (size_t)HIST_PITCH * n * sizeof (int)}; seg[k++] = {h->d_histS, (size_t)HIST_PITCH * n * sizeof (int)};
-    seg[k++] = {h->d_cnt, 4 * n * sizeof (int)};
+    seg[k++] = {h->d_cnt, 4 * n * sizeof (int)}; seg[k++] = {h->d_fph, n * sizeof (int)};
     return k;
 }
 }
@@ -967,8 +1039,8 @@ int ebu_segments (b200m_ebu* h, EbuSeg* seg)
 size_t b200m_ebu_snapshot_size (b200m_ebu* h)
 {
     if (!h) return 0;
-    EbuSeg seg[8]; const int k = ebu_segments (h, seg);
-    size_t b = sizeof (EbuSnapHead) + 3 * (size_t)h->n_inst;
+    EbuSeg seg[9]; const int k = ebu_segments (h, seg);
+    size_t b = sizeof (EbuSnapHead) + EBU_SNAP_HOST_PER_INST * (size_t)h->n_inst;
     b = (b + 15) & ~size_t (15);
     for (int i = 0; i < k; ++i) b += (seg[i].bytes + 15) & ~size_t (15);
     return b;
@@ -980,12 +1052,14 @@ int b200m_ebu_snapshot (b200m_ebu* h, void* buf, size_t bytes, void* stream)
     DeviceGuard g (h->device);
     cudaStream_t st = ebu_stream (h, stream);
     uint8_t* o = (uint8_t*)buf;
-    EbuSnapHead hd = {EBU_SNAP_MAGIC, h->n_inst, h->nchan, h->fsamp, h->frcnt, h->wrind, h->G, {0}};
-    memcpy (hd.cnt10, h->cnt10, sizeof (hd.cnt10));
+    EbuSnapHead hd = {EBU_SNAP_MAGIC, h->n_inst, h->nchan, h->fsamp, h->tmod, {0, 0, 0}};
     memcpy (o, &hd, sizeof (hd)); o += sizeof (hd);
-    memcpy (o, h->integ.data (), h->n_inst); o += h->n_inst; memcpy (o, h->base.data (), h->n_inst); o += h->n_inst; memcpy (o, h->frozen.data (), h->n_inst); o += h->n_inst;
-    o = (uint8_t*)buf + ((sizeof (hd) + 3 * (size_t)h->n_inst + 15) & ~size_t (15));
-    EbuSeg seg[8]; const int k = ebu_segments (h, seg);
+    const size_t n = h->n_inst;
+    memcpy (o, h->ph.data (), 4 * n); o += 4 * n;
+    memcpy (o, h->integ.data (), n); o += n; memcpy (o, h->base.data (), n); o += n; memcpy (o, h->frozen.data (), n); o += n;
+    for (size_t i = 0; i < n; ++i) *o++ = (uint8_t)h->cls.find (h->ph[i])->second.G;
+    o = (uint8_t*)buf + ((sizeof (hd) + EBU_SNAP_HOST_PER_INST * n + 15) & ~size_t (15));
+    EbuSeg seg[9]; const int k = ebu_segments (h, seg);
     for (int i = 0; i < k; ++i) { B200M_CUDA (cudaMemcpyAsync (o, seg[i].p, seg[i].bytes, cudaMemcpyDeviceToHost, st)); o += (seg[i].bytes + 15) & ~size_t (15); }
     B200M_CUDA (cudaStreamSynchronize (st));
     return 0;
@@ -1000,10 +1074,18 @@ int b200m_ebu_restore (b200m_ebu* h, const void* buf, size_t bytes, void* stream
     DeviceGuard g (h->device);
     cudaStream_t st = ebu_stream (h, stream);
     const uint8_t* o = (const uint8_t*)buf + sizeof (hd);
-    h->frcnt = hd.frcnt; h->wrind = hd.wrind; h->G = hd.G; memcpy (h->cnt10, hd.cnt10, sizeof (hd.cnt10));
-    memcpy (h->integ.data (), o, h->n_inst); o += h->n_inst; memcpy (h->base.data (), o, h->n_inst); o += h->n_inst; memcpy (h->frozen.data (), o, h->n_inst);
-    o = (const uint8_t*)buf + ((sizeof (hd) + 3 * (size_t)h->n_inst + 15) & ~size_t (15));
-    EbuSeg seg[8]; const int k = ebu_segments (h, seg);
+    const size_t n = h->n_inst;
+    h->tmod = hd.tmod;
+    memcpy (h->ph.data (), o, 4 * n); o += 4 * n;
+    memcpy (h->integ.data (), o, n); o += n; memcpy (h->base.data (), o, n); o += n; memcpy (h->frozen.data (), o, n); o += n;
+    h->cls.clear ();
+    for (size_t i = 0; i < n; ++i) {
+        EbuPhase& c = h->cls[h->ph[i]];
+        c.n++; c.G = o[i];
+        if (h->integ[i]) c.cnt10[h->base[i]]++;
+    }
+    o = (const uint8_t*)buf + ((sizeof (hd) + EBU_SNAP_HOST_PER_INST * n + 15) & ~size_t (15));
+    EbuSeg seg[9]; const int k = ebu_segments (h, seg);
     for (int i = 0; i < k; ++i) { B200M_CUDA (cudaMemcpyAsync (seg[i].p, o, seg[i].bytes, cudaMemcpyHostToDevice, st)); o += (seg[i].bytes + 15) & ~size_t (15); }
     B200M_CUDA (cudaStreamSynchronize (st));
     return 0;
@@ -1030,7 +1112,7 @@ int b200m_ebu_state (b200m_ebu* h, uint32_t inst, float* z, float* power64, floa
     EbuCtl c;
     B200M_CUDA (cudaMemcpyAsync (&c, h->d_ctl + inst, sizeof (c), cudaMemcpyDeviceToHost, st));
     B200M_CUDA (cudaStreamSynchronize (st));
-    c4[0] = h->frcnt; c4[1] = h->wrind; c4[2] = c.div1; c4[3] = c.div2;
+    c4[0] = h->frcnt_of (h->ph[inst]); c4[1] = c.wrind; c4[2] = c.div1; c4[3] = c.div2;
     return 0;
 }
 

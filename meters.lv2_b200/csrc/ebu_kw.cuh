@@ -27,9 +27,15 @@ constexpr int HIST_PITCH = 752;           // 751 bins padded to a 16-byte multip
 
 struct EbuCoef { float a0, a1, a2, b1, b2, c3, c4; };
 
-struct EbuChunks {                        // bit31: chunk ends a 50 ms fragment
+// How K1 cuts a block into detect_process() calls.  fph == nullptr: the warp-uniform chunk list v[0..n) (bit31: the chunk ends a
+// 50 ms fragment), for a bank whose instances share one fragment phase.  fph != nullptr: every instance has its own phase
+// (fph[i]: the bank time mod fragm at which its clock last started; tmod: the bank time mod fragm at the launch's first frame)
+// and the launch covers the whole block.
+struct EbuChunks {
     int n;
     uint32_t v[EBU_MAXCHUNK];
+    int tmod, fragm;
+    const int* fph;
 };
 
 // Everything one K1 launch over a whole bank needs: the block's first `nfram` frames, its chunk list and the bank's state arrays.
@@ -66,8 +72,8 @@ B200M_DEV void kw_step (float p, const EbuCoef& c, float& z1, float& z2, float& 
 B200M_DEV uint32_t smem_u32 (const void* p) { return (uint32_t)__cvta_generic_to_shared (p); }
 
 // The recurrence over one block for the 32 channels of a warp; `sg` supplies the tiles (a staging policy: PaddedStage and
-// TmaStage in ebu.cu, FusedStage in tpk.cu).
-template <int NCHAN, class Stage>
+// TmaStage in ebu.cu, FusedStage in tpk.cu).  PHASES = false compiles the chunk-list policy alone (ck.fph is ignored).
+template <int NCHAN, bool PHASES, class Stage>
 B200M_DEV void kw_warp (Stage& sg, int lane, int k, bool live, int nchans, int nfram, const EbuCoef& cf, const EbuChunks& ck, float fragm_f,
                         float* __restrict__ zst, float* __restrict__ frpwr, float* __restrict__ fragpw, int n_inst)
 {
@@ -78,12 +84,20 @@ B200M_DEV void kw_warp (Stage& sg, int lane, int k, bool live, int nchans, int n
     float fp = frpwr[inst];
     float sj = 0.0f;
     int ci = 0, nfr = 0;
-    int cend = (int)(ck.v[0] & 0x7fffffffu);           // end position (exclusive) of the current chunk
+    int cend = (int)(ck.v[0] & 0x7fffffffu);           // end position (exclusive) of the current chunk (warp-uniform)
     bool cfrag = (ck.v[0] >> 31) != 0;
+    // per-instance phases: the warp cuts at the nearest of its lanes' own fragment edges and the block end; a lane's
+    // detect_process() call ends only at its own edges and the block end (:207-216), so at another lane's edge it carries on
+    int mynext = 0x7fffffff;                           // this lane's next own fragment edge
+    if (PHASES && ck.fph) {
+        if (live) { int el = (ck.tmod - ck.fph[inst]) % ck.fragm; if (el < 0) el += ck.fragm; mynext = ck.fragm - el; }
+        cend = min (__reduce_min_sync (0xffffffffu, mynext), nfram);
+    }
 
     // end of one detect_process() call (:324-335): state scrub, channel sum, _frpwr +=, fragment hand-over (:217-221)
     auto chunk_end = [&] () {
-        z1 = scrub (z1); z2 = scrub (z2); z3 = scrub (z3); z4 = scrub (z4);
+        bool cut = true;
+        if (PHASES && ck.fph) { cfrag = mynext == cend; cut = cfrag || cend == nfram; }
         float si;
         if (NCHAN == 1) si = __fmul_rn (2.0f, sj);
         else if (NCHAN == 2) si = __fadd_rn (sj, __shfl_xor_sync (0xffffffffu, sj, 1));   // 1.0f*sjL + 1.0f*sjR
@@ -94,16 +108,23 @@ B200M_DEV void kw_warp (Stage& sg, int lane, int k, bool live, int nchans, int n
 #pragma unroll
             for (int c = 1; c < NCHAN; ++c) si = __fadd_rn (si, __fmul_rn (c >= 3 ? 1.41f : 1.0f, __shfl_sync (0xffffffffu, sj, (lead + c) & 31)));
         }
-        fp = __fadd_rn (fp, si);
-        if (cfrag) {
-            if (live && (k % NCHAN) == 0) fragpw[(size_t)nfr * n_inst + inst] = __fdiv_rn (fp, fragm_f);
-            fp = 1e-30f;
-            ++nfr;
+        if (cut) {                                     // the channel sums above are shuffles: every lane took part
+            z1 = scrub (z1); z2 = scrub (z2); z3 = scrub (z3); z4 = scrub (z4);
+            fp = __fadd_rn (fp, si);
+            if (cfrag) {
+                if (live && (k % NCHAN) == 0) fragpw[(size_t)nfr * n_inst + inst] = __fdiv_rn (fp, fragm_f);
+                fp = 1e-30f;
+                ++nfr;
+                mynext += ck.fragm;
+            }
+            sj = 0.0f;
         }
-        sj = 0.0f;
-        ++ci;
-        if (ci < ck.n) { cend = (int)(ck.v[ci] & 0x7fffffffu); cfrag = (ck.v[ci] >> 31) != 0; }
-        else cend = 0x7fffffff;
+        if (PHASES && ck.fph) cend = cend == nfram ? 0x7fffffff : min (__reduce_min_sync (0xffffffffu, mynext), nfram);
+        else {
+            ++ci;
+            if (ci < ck.n) { cend = (int)(ck.v[ci] & 0x7fffffffu); cfrag = (ck.v[ci] >> 31) != 0; }
+            else cend = 0x7fffffff;
+        }
     };
 
     sg.prologue ();

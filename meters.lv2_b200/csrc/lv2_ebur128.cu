@@ -54,14 +54,17 @@ struct EbuPlugin {
     int32_t histM[HIST_LEN], histS[HIST_LEN];
 };
 
-// batched mode (lv2_hub.cuh): the instances of one sample rate share one bank.  dBTP is processed for every slot as soon as one
-// member enables it; after a disable/enable the oversampler history is current rather than frozen (the reference does not run
-// the meter while disabled).
+// batched mode (lv2_hub.cuh): the instances of one sample rate share one bank.  A slot's tenant gets a fresh instance whose own
+// 50 ms fragment clock starts with its first run() (B200M_R128_NEW, applied ahead of that run's control messages and audio).
+// Each slot's dBTP switch is its member's own (b200m_r128_set_dbtp_inst at the launch of the cycle): while it is off the slot's
+// true-peak histories stay frozen and its hold reads -inf, as the plugin's do.
 struct EbuHub : SlotHub {
     b200m_r128* bank = nullptr;
     std::vector<b200m_ebu_result> res; std::vector<float> tp;  // results of the last completed cycle
+    std::vector<uint8_t> fresh;                                // per slot: its tenant has not run yet
+    std::vector<uint8_t> dbtp;                                 // per slot: the dBTP switch the bank has
 
-    EbuHub (const HubKey& k, uint32_t n) : SlotHub (k, n), res (n), tp (n, -INFINITY) {}
+    EbuHub (const HubKey& k, uint32_t n) : SlotHub (k, n), res (n), tp (n, -INFINITY), fresh (n, 1), dbtp (n, 0) {}
     ~EbuHub () { b200m_r128_destroy (bank); }
 
     static SlotHub* create (const HubKey& k, uint32_t n)
@@ -74,16 +77,26 @@ struct EbuHub : SlotHub {
     }
     int launch_bank (uint32_t n) override
     {
-        bool any_dbtp = false;
-        for (void* m : member) if (m && ((EbuPlugin*)m)->dbtp_enable) any_dbtp = true;
-        b200m_r128_set_dbtp (bank, any_dbtp);
+        for (uint32_t s = 0; s < slots; ++s) {                 // a vacant slot keeps its last switch
+            const EbuPlugin* m = (const EbuPlugin*)member[s];
+            if (m && m->dbtp_enable != (dbtp[s] != 0)) { dbtp[s] = m->dbtp_enable; b200m_r128_set_dbtp_inst (bank, (int32_t)s, m->dbtp_enable); }
+        }
         return b200m_r128_run_host (bank, stage.data, B200M_MAX_BLOCK, n);
     }
     void collect () override { b200m_r128_results (bank, res.data (), tp.data (), nullptr); }
+    // with mu held, after close_if_broken, before the run()'s control messages: the instance the plugin's constructor made
+    // (Ebu_r128_proc::reset, src/ebulv2.cc:190) starts at the cycle this run() joins
+    void first_run (int slot)
+    {
+        if (!fresh[slot]) return;
+        fresh[slot] = 0;
+        b200m_r128_control (bank, slot, B200M_R128_NEW, nullptr);
+    }
     void vacate (uint32_t slot) override
     {
-        // the slot's next tenant starts from a freshly created instance and silence: filters, 64-fragment ring, loudness values,
-        // histograms, true-peak history and hold all cleared; only the bank's shared 50 ms fragment phase is inherited
+        // the vacated slot idles as a freshly created instance on silence: filters, 64-fragment ring, loudness values, histograms,
+        // true-peak history and hold all cleared; its next tenant restarts the fragment clock at its first run()
+        fresh[slot] = 1;
         b200m_r128_control (bank, (int)slot, B200M_R128_CLEAR, nullptr);
         tp[slot] = -INFINITY;
         b200m_ebu_result z; memset (&z, 0, sizeof (z));
@@ -187,7 +200,6 @@ void on_config (EbuPlugin* p, const AtomObject& obj, uint32_t n_samples)      //
         break;
     case CTL_UISETTINGS:
         p->ui_settings = (uint32_t)v;
-        if (p->hub && !p->dbtp_enable && (p->ui_settings & 64)) bank_control (p, B200M_R128_CLEAR_TPMAX);   // the hold restarts, as after disabled cycles
         p->dbtp_enable = (p->ui_settings & 64) != 0;
         break;
     default: break;
@@ -271,6 +283,7 @@ void ebur_run (LV2_Handle h, uint32_t n_samples)
         // the new cycle does not land ahead of the old audio
         std::lock_guard<std::mutex> lh (p->hub->mu);
         p->hub->close_if_broken (p->slot, n_samples);
+        p->hub->first_run (p->slot);
     }
     if (p->control) {                                          // messages from the GUI / host (:258-331)
         for (AtomEvents ev (p->control); ev.valid (); ev.next ()) {
@@ -293,7 +306,7 @@ void ebur_run (LV2_Handle h, uint32_t n_samples)
         EbuHub* hub = p->hub;
         std::lock_guard<std::mutex> lh (hub->mu);
         hub->submit (p->slot, p->input, n_samples);
-        r = hub->res[p->slot]; tp_max = p->dbtp_enable ? hub->tp[p->slot] : -INFINITY;      // the previous cycle's
+        r = hub->res[p->slot]; tp_max = hub->tp[p->slot];      // the previous cycle's (-inf if the slot's dBTP was off in it)
         ran = true;
     } else if (n_samples >= 1 && n_samples <= B200M_MAX_BLOCK && p->stage.fill (p->input, 2, n_samples)) {
         b200m_r128_set_dbtp (p->bank, p->dbtp_enable);

@@ -1756,7 +1756,7 @@ tpmax_tc_kernel (const float* __restrict__ in, size_t stride, int c_first, int n
 //               so a thread meets the same four channels in every stage and keeps their running maxima in registers until the slab
 //               ends.  The two warpgroups take turns on the tensor cores (named barriers 2 and 3): one's 16 wgmmas run while the
 //               other loads, splits and reduces.
-//   warps 8-11  K-weighting: kw_warp<2> unchanged (lane = channel) through FusedStage, so the EBU floats stay bit-exact.
+//   warps 8-11  K-weighting: kw_warp<2, PHASES> (lane = channel) through FusedStage, so the EBU floats stay bit-exact.
 // A slot is refilled by the last of the 12 warps to release it (a shared counter), so no role waits for another to finish reading:
 // stages >= 1 by one 2-D TMA box [128 rows x 116 floats] from sample 64 t - 48 (rows and samples outside the block read as zero),
 // stage 0 by per-row bulk copies of the 48-sample history and the block's first 68 samples.
@@ -1827,6 +1827,8 @@ struct FusedStage {
     B200M_DEV float ld (int t, int e) const { return rowp (t)[e]; }
 };
 
+// PHASES: the EBU bank's instances have several fragment phases (kw_warp's per-instance cut policy)
+template <bool PHASES>
 __global__ void __launch_bounds__ (R128F_WARPS * 32, 1)
 r128_fused_kernel (const __grid_constant__ CUtensorMap tmap, const float* __restrict__ in, size_t stride, int nch, int nfram,
                    const float* __restrict__ bcanon, TpkState st, float* __restrict__ r128_tpmax,
@@ -1866,7 +1868,7 @@ r128_fused_kernel (const __grid_constant__ CUtensorMap tmap, const float* __rest
             const int k = ((int)blockIdx.x + i * (int)gridDim.x) * R128F_CH + 32 * kw + lane;
             sg.j0 = i * ntiles;
             // rows beyond the bank read as zeros (stage 0: the last channel's): those lanes never store
-            kw_warp<2> (sg, lane, min (k, nch - 1), k < nch, nch, nfram, cf, ck, fragm_f, zst, frpwr, fragpw, n_inst);
+            kw_warp<2, PHASES> (sg, lane, min (k, nch - 1), k < nch, nch, nfram, cf, ck, fragm_f, zst, frpwr, fragpw, n_inst);
         }
         return;
     }
@@ -2171,6 +2173,9 @@ static int tpk_process (b200m_tpk* h, const float* d_in, size_t stride, uint32_t
 // channels (5120 stereo instances) run fused.
 constexpr uint32_t R128F_MIN_CH = 10240;
 
+// the history the next block reads (48 floats per channel): after a block, the buffer its kernels left current
+float* tpk_hist (b200m_tpk* h) { return h->st.hist; }
+
 bool tpk_r128_fused_ok (const b200m_tpk* h, const float* d_in, size_t stride, uint32_t nfram)
 {
     return (h->flags & B200M_TPK_TRUEPEAK) && !(h->flags & B200M_TPK_KMETER) && h->chunked && h->tc && h->fma && h->imm && h->d_btc && !h->d_dbg
@@ -2184,7 +2189,7 @@ int tpk_r128_fused (b200m_tpk* h, const EbuK1Args& a, float* r128_tpmax, cudaStr
     if (!ebu_tma_map (&tm, a.in, a.stride, h->n_chan, (uint32_t)a.nfram, R128F_PITCH, R128F_CH, false))
         return set_err (B200M_E_CUDA, "r128: the driver rejected the input block's tensor map");
     const int nslabs = ((int)h->n_chan + R128F_CH - 1) / R128F_CH;
-    r128_fused_kernel<<<std::min (nslabs, h->n_sm), R128F_WARPS * 32, R128F_SMEM, st>>> (
+    (a.ck.fph ? r128_fused_kernel<true> : r128_fused_kernel<false>)<<<std::min (nslabs, h->n_sm), R128F_WARPS * 32, R128F_SMEM, st>>> (
         tm, a.in, a.stride, (int)h->n_chan, a.nfram, h->d_btc, h->st, r128_tpmax, a.cf, a.ck, a.fragm_f, a.zst, a.frpwr, a.fragpw, a.n_inst);
     B200M_LAUNCHED (1);
     B200M_CUDA (cudaGetLastError ());
@@ -2273,7 +2278,8 @@ int b200m_tpk_create (b200m_tpk** out, int device, uint32_t n_chan, float fsamp,
         if (e == cudaSuccess) e = cudaFuncSetAttribute (tpmax_tc_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, TCF_SMEM);
         // it shares SMs with the K-weighting kernel in the EBUr128 cycle (106 KB + 104 KB): same (maximum) carveout as that one
         if (e == cudaSuccess) e = cudaFuncSetAttribute (tpmax_tc_kernel, cudaFuncAttributePreferredSharedMemoryCarveout, cudaSharedmemCarveoutMaxShared);
-        if (e == cudaSuccess) e = cudaFuncSetAttribute (r128_fused_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, R128F_SMEM);
+        if (e == cudaSuccess) e = cudaFuncSetAttribute (r128_fused_kernel<false>, cudaFuncAttributeMaxDynamicSharedMemorySize, R128F_SMEM);
+        if (e == cudaSuccess) e = cudaFuncSetAttribute (r128_fused_kernel<true>, cudaFuncAttributeMaxDynamicSharedMemorySize, R128F_SMEM);
         if (e == cudaSuccess) e = cudaDeviceGetAttribute (&h->n_sm, cudaDevAttrMultiProcessorCount, device);
     }
     if (const char* v = getenv ("B200M_TPK_DEC")) h->dec = atoi (v) != 0;
