@@ -193,6 +193,8 @@ int b200m_tpk_debug_timeline (b200m_tpk* h, unsigned long long* out, int n);
  * EBUr128 plugin cycle — the audio part of ebur128_run (src/ebulv2.cc:341-367) for N stereo
  * instances: Ebu_r128_proc::process + (if dbtp_enable) TruePeakdsp::process_max on both channels,
  * the getters, and the dBTP hold  tp_max = max (tp_max, coef_to_db (max (tp0, tp1)))  (:227-230,360-367).
+ * b200m_r128_create_nch: the same cycle for instances of 1..5 channels (the maximum of the reads of all
+ * the instance's channels, taken before coef_to_db).
  * One host->device copy per block feeds both meters.  Atom/radar/GUI messaging is out of scope.
  * ====================================================================================== */
 typedef struct b200m_r128 b200m_r128;
@@ -204,6 +206,11 @@ enum { B200M_R128_START = 1, B200M_R128_PAUSE = 2, B200M_R128_RESET = 3, B200M_R
  * NEW (inst >= 0): CLEAR with the instance's own fragment clock restarted: a freshly instantiated plugin whose first run() is the
  *   next block (b200m_ebu_reset of the instance). */
 int b200m_r128_create (b200m_r128** out, int device, uint32_t n_inst, float fsamp, int dbtp_enable);
+/* n_inst instances of nchan = 1..5 channels (b200m_r128_create: nchan = 2).  Input rows are inst * nchan + c, channels in
+ * Ebu_r128_proc's order L R C Ls Rs (gains 1 1 1 1.41 1.41, ebumeter/ebu_r128_proc.cc:29); LFE is not an input (BS.1770 leaves
+ * it out): pass the non-LFE rows.  Every other b200m_r128_* call works on such a bank; CLEAR / NEW and a disabled dBTP cover all
+ * the instance's channels, and a snapshot restores only into a bank with the same nchan. */
+int b200m_r128_create_nch (b200m_r128** out, int device, uint32_t n_inst, uint32_t nchan, float fsamp, int dbtp_enable);
 int b200m_r128_destroy (b200m_r128* h);
 int b200m_r128_control (b200m_r128* h, int32_t inst, int cmd, void* stream);      /* inst = -1: all */
 int b200m_r128_run_device (b200m_r128* h, const float* d_in, size_t stride, uint32_t nfram, void* stream);

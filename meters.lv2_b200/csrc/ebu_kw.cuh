@@ -1,5 +1,5 @@
 // ebu_kw.cuh — the K-weighting recurrence of the EBU R128 bank (K1's per-channel body), shared by the K1 kernels of ebu.cu
-// and the fused K-weighting + true-peak kernel of the EBUr128 cycle (tpk.cu).
+// and the fused K-weighting + true-peak kernel of the EBUr128 cycle (tpk.cu); the cycle's dBTP hold (tpk.cu, r128.cu).
 #pragma once
 #include <cuda.h>
 #include "common.cuh"
@@ -44,6 +44,19 @@ struct EbuK1Args {
     EbuCoef cf; EbuChunks ck; float fragm_f;
     float *zst, *frpwr, *fragpw; int n_inst;
 };
+
+// The EBUr128 cycle's dBTP hold (src/ebulv2.cc:227-230,360-367) as the true-peak kernels' epilogue sees it: nch channels per
+// instance, instance i on channels nch i .. nch i + nch - 1.  tpmax == nullptr: no EBUr128 epilogue.  lin == nullptr (nch = 1, 2, 4:
+// an instance never leaves an 8-channel true-peak group): the group folds its instances into tpmax[] itself.  Otherwise (nch = 3, 5:
+// instances straddle groups and host slices) every channel's read() goes to lin[channel] and r128_hold_kernel folds them.
+struct R128Hold { float* tpmax; float* lin; int nch; };
+
+// coef_to_db (src/ebulv2.cc:227-230) of the larger read() t, then tp_max = max (tp_max, tp)
+B200M_DEV void r128_hold (float* tpmax, float t)
+{
+    const float tp = (t == 0) ? -INFINITY : __double2float_rn (__dmul_rn (20.0, (double)log10f_glibc (t)));
+    if (tp > *tpmax) *tpmax = tp;
+}
 
 // ---- K1: K-weighting recurrence + per-chunk power sums ------------------------------------
 // One warp = 32 consecutive mono channels (lane = channel).  Tiles of [32 ch x 64 samples] are
