@@ -283,6 +283,13 @@ int b200m_cor_results (b200m_cor* h, float* out, void* stream);           /* Stc
  * both precision modes.  Ordered with the bank's runs on the stream it currently runs on.  A phasewheel ring fed from this bank
  * (b200m_pw_attach_cor) is not touched. */
 int b200m_cor_clear (b200m_cor* h, int32_t inst, void* stream);
+/* b200m_cor_process_* with a per-pair hold: run = n_inst flags, NULL = every pair runs (exactly b200m_cor_process_*).  A pair
+ * with run[i] == 0 is left as if the call had not been made for it: its five filter states and its reading stay bit-identical,
+ * without the end-of-process scrub and bias, and its input rows are not read (they may hold anything, NaN included).  Each pair's
+ * arithmetic is independent of its neighbours', so the others advance exactly as in a bank called only in their own active
+ * cycles, in both precision modes.  The mask is uploaded only when it differs from the previous call's. */
+int b200m_cor_process_ctl_device (b200m_cor* h, const float* d_in, size_t stride, uint32_t nfram, const uint8_t* run, void* stream);
+int b200m_cor_process_ctl_host (b200m_cor* h, const float* in, size_t stride, uint32_t nfram, const uint8_t* run);
 /* B200M_PREC_EXACT (default): the five recurrences run serially in time, one lane per pair, bit-identical to the reference.
  * B200M_PREC_FMA: time-parallel evaluation -- the recurrences are linear one-pole filters, so a warp owns ONE pair, its lanes take
  * consecutive time segments and an affine warp scan stitches them: 32x more parallelism for small banks (2048 pairs are 64 warps

@@ -122,6 +122,8 @@ _PROTOS = {
     "b200m_cor_destroy": (C.c_int, [_v]),
     "b200m_cor_process_device": (C.c_int, [_v, _v, C.c_size_t, C.c_uint32, _v]),
     "b200m_cor_process_host": (C.c_int, [_v, _v, C.c_size_t, C.c_uint32]),
+    "b200m_cor_process_ctl_device": (C.c_int, [_v, _v, C.c_size_t, C.c_uint32, _v, _v]),
+    "b200m_cor_process_ctl_host": (C.c_int, [_v, _v, C.c_size_t, C.c_uint32, _v]),
     "b200m_cor_results": (C.c_int, [_v, _v, _v]),
     "b200m_cor_state": (C.c_int, [_v, _v, _v]),
     "b200m_cor_coeffs": (C.c_int, [_v, _v]),
@@ -466,15 +468,24 @@ class Stcorrdsp(_Bank):
         self.n_inst = n_inst
         _ck(lib().b200m_cor_create(C.byref(self.h), device, n_inst, int(fsamp), flp, tcf))
 
-    def process(self, x, stream=None):
+    def process(self, x, run=None, stream=None):
+        """run: None (every pair) or n_inst flags; a pair whose flag is 0 is held, its state and reading left as they are"""
+        mask = None if run is None else np.ascontiguousarray(run, np.uint8)
+        assert mask is None or mask.shape == (self.n_inst,)
         if isinstance(x, np.ndarray) or not x.is_cuda:
             p, s, rows, n = _host_planar(x)
             assert rows == 2 * self.n_inst
-            _ck(lib().b200m_cor_process_host(self.h, p, s, n))
+            if mask is None:
+                _ck(lib().b200m_cor_process_host(self.h, p, s, n))
+            else:
+                _ck(lib().b200m_cor_process_ctl_host(self.h, p, s, n, _np_ptr(mask)))
         else:
             p, s, rows, n = _dev_ptr(x)
             assert rows == 2 * self.n_inst
-            _ck(lib().b200m_cor_process_device(self.h, p, s, n, _stream_ptr(stream)))
+            if mask is None:
+                _ck(lib().b200m_cor_process_device(self.h, p, s, n, _stream_ptr(stream)))
+            else:
+                _ck(lib().b200m_cor_process_ctl_device(self.h, p, s, n, _np_ptr(mask), _stream_ptr(stream)))
 
     def set_precision(self, mode):
         """PREC_EXACT: serial, bit-identical; PREC_FMA: time-parallel warp scan, correlation within 1e-5"""

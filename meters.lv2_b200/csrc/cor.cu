@@ -7,15 +7,20 @@
 // Operation order is the reference's, without FMA contraction (bit-identical state).
 #include <math.h>
 #include <stdlib.h>
+#include <vector>
 #include "common.cuh"
 
 namespace b200m {
 
 constexpr int COR_T = 32, COR_P = COR_T + 4, COR_STAGES = 4;
 
+// HOLD (b200m_cor_process_ctl_*): pairs with run[i] == 0 are held -- their rows are never loaded and their state and reading are
+// not written back.  The plain process calls and the phasewheel ring feed are the HOLD = false instantiation.
+template <bool HOLD>
 __global__ void __launch_bounds__ (32)
 cor_kernel (const float* __restrict__ in, size_t stride, int n_inst, int nfram, int aligned, float w1, float w2,
-            float* __restrict__ st /* [5][n_inst] */, float* __restrict__ res, float* __restrict__ ring, int N, int rboff)
+            float* __restrict__ st /* [5][n_inst] */, float* __restrict__ res, float* __restrict__ ring, int N, int rboff,
+            const uint8_t* __restrict__ run)
 {
     __shared__ __align__ (16) float tile[COR_STAGES][2][32 * COR_P];
     const int lane = threadIdx.x;
@@ -23,6 +28,9 @@ cor_kernel (const float* __restrict__ in, size_t stride, int n_inst, int nfram, 
     const int inst = min (i0 + lane, n_inst - 1);
     const bool live = (i0 + lane) < n_inst;
     const int ntiles = (nfram + COR_T - 1) / COR_T;
+    // bit p: pair i0 + p is held (lanes past the bank repeat its last pair); a warp of held pairs has nothing to do
+    const unsigned held = HOLD ? __ballot_sync (0xffffffffu, !run[inst]) : 0u;
+    if (HOLD && held == 0xffffffffu) return;
 
     auto issue = [&] (int t) {
         if (t < ntiles) {
@@ -37,13 +45,14 @@ cor_kernel (const float* __restrict__ in, size_t stride, int n_inst, int nfram, 
                     const int row = 4 * i + (lane >> 3);       // 0..63 : pair = row>>1, channel = row&1
                     const int pr = min (i0 + (row >> 1), n_inst - 1);
                     const float* src = in + (size_t)(2 * pr + (row & 1)) * stride + s0 + c4;
-                    cp_async16 (d0 + (row & 1) * (32 * COR_P) + (row >> 1) * COR_P + c4, nb ? src : in, nb);
+                    const int nr = (held >> (row >> 1)) & 1 ? 0 : nb;
+                    cp_async16 (d0 + (row & 1) * (32 * COR_P) + (row >> 1) * COR_P + c4, nr ? src : in, nr);
                 }
             } else {
 #pragma unroll 4
                 for (int row = 0; row < 64; ++row) {
                     const int pr = min (i0 + (row >> 1), n_inst - 1);
-                    const bool ok = (s0 + lane) < nfram;
+                    const bool ok = (s0 + lane) < nfram && !((held >> (row >> 1)) & 1);
                     cp_async4 (d0 + (row & 1) * (32 * COR_P) + (row >> 1) * COR_P + lane,
                                ok ? in + (size_t)(2 * pr + (row & 1)) * stride + s0 + lane : in, ok ? 4 : 0);
                 }
@@ -71,7 +80,7 @@ cor_kernel (const float* __restrict__ in, size_t stride, int n_inst, int nfram, 
         const float* pl = tile[t % COR_STAGES][0] + lane * COR_P;
         const float* pr = tile[t % COR_STAGES][1] + lane * COR_P;
         const int len = min (COR_T, nfram - t * COR_T);
-        if (ring && lane < len) {
+        if (!HOLD && ring && lane < len) {
             // fused phasewheel feed (b200m_pw_attach_cor): r_buf[(i + n_off) % n_siz] = data[i] (gui/fft.c:302-305) for the 64 rows
             // of this tile, one 128-byte row segment per store instruction
             int o = rboff + t * COR_T + lane; if (o >= N) o -= N;
@@ -95,7 +104,7 @@ cor_kernel (const float* __restrict__ in, size_t stride, int n_inst, int nfram, 
     // end of process(): non-finite scrub, anti-denormal bias on the three products (:65-75)
     zl = scrub (zl); zr = scrub (zr); zlr = scrub (zlr); zll = scrub (zll); zrr = scrub (zrr);
     zlr = __fadd_rn (zlr, 1e-10f); zll = __fadd_rn (zll, 1e-10f); zrr = __fadd_rn (zrr, 1e-10f);
-    if (live) {
+    if (live && !((held >> lane) & 1)) {
         st[0 * (size_t)n_inst + inst] = zl;  st[1 * (size_t)n_inst + inst] = zr;
         st[2 * (size_t)n_inst + inst] = zlr; st[3 * (size_t)n_inst + inst] = zll; st[4 * (size_t)n_inst + inst] = zrr;
         // Stcorrdsp::read (:79-82)
@@ -134,14 +143,17 @@ B200M_DEV void affine_scan (float& A, float& B, int lane)
     }
 }
 
+template <bool HOLD>
 __global__ void __launch_bounds__ (CSC_WARPS * 32)
 cor_scan_kernel (const float* __restrict__ in, size_t stride, int n_inst, int nfram, int aligned, float w1, float w2,
-                 float* __restrict__ st /* [5][n_inst] */, float* __restrict__ res, float* __restrict__ ring, int N, int rboff)
+                 float* __restrict__ st /* [5][n_inst] */, float* __restrict__ res, float* __restrict__ ring, int N, int rboff,
+                 const uint8_t* __restrict__ run)
 {
     __shared__ float sm[CSC_WARPS][2][32 * CSC_PITCH];
     const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
     const int inst = blockIdx.x * CSC_WARPS + warp;
-    if (inst >= n_inst) return;                              // warp-uniform; warps never synchronise with each other
+    if (inst >= n_inst || (HOLD && !run[inst])) return;      // warp-uniform; warps never synchronise with each other
+    if (HOLD) ring = nullptr;                                // the phasewheel ring feed never holds: compiled out of this variant
     float* sl = sm[warp][0]; float* sr = sm[warp][1];
     const float* gl = in + (size_t)(2 * inst) * stride; const float* gr = gl + stride;
     float* rl = ring ? ring + (size_t)(2 * inst) * N : nullptr; float* rr = rl ? rl + N : nullptr;
@@ -256,30 +268,46 @@ struct b200m_cor {
     int device; uint32_t n_inst; float w1, w2;
     int scan = 0;                          // B200M_PREC_FMA: time-parallel cor_scan_kernel
     float *d_st = nullptr, *d_res = nullptr;
+    std::vector<uint8_t> run;              // b200m_cor_process_ctl_*: the run mask as last uploaded to d_run (all 1 at create)
+    uint8_t* d_run = nullptr;
     cudaStream_t own = nullptr; HostStage stage; bool last_host = false;
 };
 
 static cudaStream_t cor_stream (b200m_cor* h, void* stream) { return h->last_host ? h->own : (cudaStream_t)stream; }
 
-namespace b200m {
-int cor_feed (b200m_cor* h, const float* d_in, size_t stride, uint32_t nfram, cudaStream_t st, float* ring, int N, int rboff)
+template <bool HOLD>
+static int cor_launch (b200m_cor* h, const float* d_in, size_t stride, uint32_t nfram, cudaStream_t st, float* ring, int N, int rboff)
 {
     const int aligned = ((uintptr_t)d_in % 16 == 0) && (stride % 4 == 0);
+    const uint8_t* run = HOLD ? h->d_run : nullptr;
     if (h->scan)
-        cor_scan_kernel<<<(h->n_inst + CSC_WARPS - 1) / CSC_WARPS, CSC_WARPS * 32, 0, st>>> (d_in, stride, (int)h->n_inst, (int)nfram, aligned, h->w1, h->w2,
-                                                                                              h->d_st, h->d_res, ring, N, rboff);
+        cor_scan_kernel<HOLD><<<(h->n_inst + CSC_WARPS - 1) / CSC_WARPS, CSC_WARPS * 32, 0, st>>> (
+            d_in, stride, (int)h->n_inst, (int)nfram, aligned, h->w1, h->w2, h->d_st, h->d_res, ring, N, rboff, run);
     else
-        cor_kernel<<<(h->n_inst + 31) / 32, 32, 0, st>>> (d_in, stride, (int)h->n_inst, (int)nfram, aligned, h->w1, h->w2, h->d_st, h->d_res, ring, N, rboff);
+        cor_kernel<HOLD><<<(h->n_inst + 31) / 32, 32, 0, st>>> (d_in, stride, (int)h->n_inst, (int)nfram, aligned, h->w1, h->w2, h->d_st, h->d_res,
+                                                                ring, N, rboff, run);
     B200M_LAUNCHED (1);
     B200M_CUDA (cudaGetLastError ());
     return 0;
 }
+
+namespace b200m {
+int cor_feed (b200m_cor* h, const float* d_in, size_t stride, uint32_t nfram, cudaStream_t st, float* ring, int N, int rboff)
+{
+    return cor_launch<false> (h, d_in, stride, nfram, st, ring, N, rboff);
+}
 uint32_t cor_instances (const b200m_cor* h) { return h ? h->n_inst : 0; }
 }
 
-static int cor_process (b200m_cor* h, const float* d_in, size_t stride, uint32_t nfram, cudaStream_t st)
+// run: NULL (every pair runs) or n_inst flags; the mask is uploaded only when it differs from the last one
+static int cor_process (b200m_cor* h, const float* d_in, size_t stride, uint32_t nfram, const uint8_t* run, cudaStream_t st)
 {
-    return cor_feed (h, d_in, stride, nfram, st, nullptr, 0, 0);
+    if (!run) return cor_launch<false> (h, d_in, stride, nfram, st, nullptr, 0, 0);
+    if (memcmp (run, h->run.data (), h->n_inst)) {
+        for (uint32_t i = 0; i < h->n_inst; ++i) h->run[i] = run[i] != 0;
+        B200M_CUDA (cudaMemcpyAsync (h->d_run, h->run.data (), h->n_inst, cudaMemcpyHostToDevice, st));
+    }
+    return cor_launch<true> (h, d_in, stride, nfram, st, nullptr, 0, 0);
 }
 
 extern "C" {
@@ -303,11 +331,14 @@ int b200m_cor_create (b200m_cor** out, int device, uint32_t n_inst, int fsamp, f
     b200m_cor* h = new (std::nothrow) b200m_cor;
     if (!h) return set_err (B200M_E_NOMEM, "host allocation failed");
     h->device = device; h->n_inst = n_inst;
+    h->run.assign (n_inst, 1);
     { float w[2]; b200m_design_cor (fsamp, flp, tcf, w); h->w1 = w[0]; h->w2 = w[1]; }
     cudaError_t e = cudaMalloc ((void**)&h->d_st, (size_t)5 * n_inst * sizeof (float));
     if (e == cudaSuccess) e = cudaMemset (h->d_st, 0, (size_t)5 * n_inst * sizeof (float));
     if (e == cudaSuccess) e = cudaMalloc ((void**)&h->d_res, n_inst * sizeof (float));
     if (e == cudaSuccess) e = cudaMemset (h->d_res, 0, n_inst * sizeof (float));
+    if (e == cudaSuccess) e = cudaMalloc ((void**)&h->d_run, n_inst);
+    if (e == cudaSuccess) e = cudaMemset (h->d_run, 1, n_inst);
     if (e == cudaSuccess) e = cudaStreamCreateWithFlags (&h->own, cudaStreamNonBlocking);
     if (e != cudaSuccess) { int rc = cuda_fail (e, "cor_create", __FILE__, __LINE__); b200m_cor_destroy (h); return rc; }
     *out = h;
@@ -319,21 +350,26 @@ int b200m_cor_destroy (b200m_cor* h)
     if (!h) return 0;
     DeviceGuard g (h->device);
     cudaDeviceSynchronize ();
-    cudaFree (h->d_st); cudaFree (h->d_res); h->stage.release ();
+    cudaFree (h->d_st); cudaFree (h->d_res); cudaFree (h->d_run); h->stage.release ();
     if (h->own) cudaStreamDestroy (h->own);
     delete h;
     return 0;
 }
 
-int b200m_cor_process_device (b200m_cor* h, const float* d_in, size_t stride, uint32_t nfram, void* stream)
+int b200m_cor_process_ctl_device (b200m_cor* h, const float* d_in, size_t stride, uint32_t nfram, const uint8_t* run, void* stream)
 {
     if (int rc = check_block_args (h, d_in, stride, nfram)) return rc;
     DeviceGuard g (h->device);
     h->last_host = false;
-    return cor_process (h, d_in, stride, nfram, (cudaStream_t)stream);
+    return cor_process (h, d_in, stride, nfram, run, (cudaStream_t)stream);
 }
 
-int b200m_cor_process_host (b200m_cor* h, const float* in, size_t stride, uint32_t nfram)
+int b200m_cor_process_device (b200m_cor* h, const float* d_in, size_t stride, uint32_t nfram, void* stream)
+{
+    return b200m_cor_process_ctl_device (h, d_in, stride, nfram, nullptr, stream);
+}
+
+int b200m_cor_process_ctl_host (b200m_cor* h, const float* in, size_t stride, uint32_t nfram, const uint8_t* run)
 {
     if (int rc = check_block_args (h, in, stride, nfram)) return rc;
     DeviceGuard g (h->device);
@@ -342,7 +378,12 @@ int b200m_cor_process_host (b200m_cor* h, const float* in, size_t stride, uint32
     B200M_CUDA (cudaMemcpy2DAsync (h->stage.d, h->stage.cap * sizeof (float), in, stride * sizeof (float),
                                    (size_t)nfram * sizeof (float), (size_t)2 * h->n_inst, cudaMemcpyHostToDevice, h->own));
     h->last_host = true;
-    return cor_process (h, h->stage.d, h->stage.cap, nfram, h->own);
+    return cor_process (h, h->stage.d, h->stage.cap, nfram, run, h->own);
+}
+
+int b200m_cor_process_host (b200m_cor* h, const float* in, size_t stride, uint32_t nfram)
+{
+    return b200m_cor_process_ctl_host (h, in, stride, nfram, nullptr);
 }
 
 int b200m_cor_set_precision (b200m_cor* h, int mode)

@@ -10,6 +10,9 @@
 // exactly like `LV2gm` (src/goniometer.h:113-169, restated below member for member; x86-64 SysV layout) and whose ring buffer
 // is a `gmringbuf` (:33-39) with the reference's index discipline (:52-113); this library's own state follows after it.
 // tests/test_lv2_gon_gpu.py drives both plugins side by side through that struct, the way the GUI does.
+// Batched mode (B200M_LV2_BATCH): the instance takes a slot in the COR plugin's hub of its sample rate (cor_hub_cycle,
+// lv2_shim.cu).  The ring buffer, its overrun flag and the redraw notification stay on the host in their own cycle; the
+// correlation port of run k + 1 gets cycle k's reading if the GUI was open (ui_active) in run k, the reference's rule one cycle late.
 #include <math.h>
 #include <pthread.h>
 #include <stdlib.h>
@@ -46,6 +49,8 @@ struct GonPlugin {
     LV2gmLayout g;                          // MUST stay first: the GUI casts the instance handle to LV2gm*
     b200m_cor* bank = nullptr;
     PinnedStage stage;
+    SlotHub* hub; int slot;                 // batched: a slot of the COR hub instead of `bank`
+    bool last_ui;                           // batched: ui_active in the previous run(), which publishes its reading now
 };
 
 size_t ring_write_space (const GmRing* rb) { return rb->rp == rb->wp ? rb->len - 1 : ((rb->len + rb->rp - rb->wp) % rb->len) - 1; }   // :52-55
@@ -77,7 +82,8 @@ LV2_Handle gon_instantiate (const LV2_Descriptor*, double rate, const char*, con
     g.atom_Float = map->map (map->handle, B200M_LV2_ATOM "Float");
     g.gon_State_F = map->map (map->handle, MTR_URI "gon_stateF");
     g.gon_State_I = map->map (map->handle, MTR_URI "gon_stateI");
-    if (b200m_cor_create (&p->bank, 0, 1, (int)rate, 2e3f, 0.3f)) { free (p); return nullptr; }             // cor->init (rate, 2e3f, 0.3f) :73-74
+    p->hub = cor_hub_join (rate, p, &p->slot);
+    if (!p->hub && b200m_cor_create (&p->bank, 0, 1, (int)rate, 2e3f, 0.3f)) { free (p); return nullptr; }    // cor->init (rate, 2e3f, 0.3f) :73-74
     g.rate = rate; g.ui_active = false; g.rb_overrun = false;
     g.apv = (uint32_t)rint (rate / 25.0);                                      // UPDATE_FPS :25,80
     g.sample_cnt = 0; g.ntfy = 0;
@@ -89,9 +95,13 @@ LV2_Handle gon_instantiate (const LV2_Descriptor*, double rate, const char*, con
     if (rbsize < 2 * g.apv) rbsize = 2 * g.apv;
     GmRing* rb = (GmRing*)malloc (sizeof (GmRing));                            // gmrb_alloc :41-49 (plain malloc: the GUI never frees it)
     if (rb) { rb->c0 = (float*)malloc (rbsize * sizeof (float)); rb->c1 = (float*)malloc (rbsize * sizeof (float)); rb->len = rbsize; rb->rp = 0; rb->wp = 0; }
-    if (!rb || !rb->c0 || !rb->c1) { if (rb) { free (rb->c0); free (rb->c1); free (rb); } b200m_cor_destroy (p->bank); free (p); return nullptr; }
+    if (!rb || !rb->c0 || !rb->c1) {
+        if (rb) { free (rb->c0); free (rb->c1); free (rb); }
+        if (p->hub) p->hub->leave (p->slot);
+        b200m_cor_destroy (p->bank); free (p); return nullptr;
+    }
     g.rb = rb;
-    p->stage.reserve (2);
+    if (!p->hub) p->stage.reserve (2);
     return p;
 }
 
@@ -117,16 +127,21 @@ void gon_run (LV2_Handle h, uint32_t n)
     forward_audio (g.input, g.output, 2, n);
     if (!g.input[0] || !g.input[1] || n == 0) return;
     // self->cor->process (in0, in1, n) every cycle, GUI open or not (:147); cycles longer than the engine's block go in pieces
-    bool ok = true;
+    bool ok = true; float cv = 0;
     for (uint32_t off = 0; off < n && ok; off += B200M_MAX_BLOCK) {
         const uint32_t k = n - off < B200M_MAX_BLOCK ? n - off : B200M_MAX_BLOCK;
         const float* in[2] = {g.input[0] + off, g.input[1] + off};
+        if (p->hub) { cv = cor_hub_cycle (p->hub, p->slot, in, k, false); continue; }
         ok = p->stage.fill (in, 2, k) && b200m_cor_process_host (p->bank, p->stage.data, p->stage.cap, k) == 0;
         if (ok && off + k < n) { float tmp; ok = b200m_cor_results (p->bank, &tmp, nullptr) == 0; }      // `stage` is reused by the next piece: wait for its upload
     }
-    float cv = 0;
-    const bool have = ok && b200m_cor_results (p->bank, &cv, nullptr) == 0;     // also the stream sync: `stage` is free when run() returns
-    if (g.ui_active) {
+    // cor->read () reaches the port while the GUI is open (:174); batched: the previous cycle's reading, if the GUI was open in
+    // that cycle.  Private: the results call is also the stream sync (`stage` is free when run() returns)
+    const bool ui = g.ui_active;
+    const bool show = p->hub ? p->last_ui : ok && b200m_cor_results (p->bank, &cv, nullptr) == 0 && ui;
+    p->last_ui = ui;
+    if (g.correlation && show) *g.correlation = cv;
+    if (ui) {
         if (ring_write (g.rb, g.input[0], g.input[1], n) < 0) g.rb_overrun = true;                    // reset by UI (:150-152)
         g.sample_cnt += n;                                                     // notify UI about new data (:155-172)
         if (g.sample_cnt >= g.apv) {
@@ -137,13 +152,13 @@ void gon_run (LV2_Handle h, uint32_t n)
             g.sample_cnt = g.sample_cnt % g.apv;
         }
         if (g.notify) *g.notify = (float)g.ntfy;
-        if (g.correlation && have) *g.correlation = cv;                        // cor->read () (:174)
     } else g.rb_overrun = false;
 }
 
 void gon_cleanup (LV2_Handle h)
 {
     GonPlugin* p = (GonPlugin*)h;
+    if (p->hub) p->hub->leave (p->slot);
     free (p->g.rb->c0); free (p->g.rb->c1); free (p->g.rb);
     b200m_cor_destroy (p->bank);
     p->stage.release ();

@@ -184,4 +184,11 @@ private:
     }
 };
 
+// Batched phasewheel and goniometer instances (lv2_xfer.cu, lv2_gon.cu) share the COR plugin's hub of their sample rate
+// (lv2_shim.cu).  cor_hub_join: a slot cleared to a fresh Stcorrdsp, or NULL when batched mode is off; leave with hub->leave (slot).
+// cor_hub_cycle: returns the slot's reading of the previous cycle and submits this cycle's n frames of in[0], in[1]; a held cycle
+// leaves the slot's Stcorrdsp untouched, as a private instance that does not call process () in it.
+SlotHub* cor_hub_join (double rate, void* who, int* slot);
+float cor_hub_cycle (SlotHub* hub, int slot, const float* const* in, uint32_t n, bool hold);
+
 }  // namespace b200m

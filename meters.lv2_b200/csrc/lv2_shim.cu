@@ -9,13 +9,15 @@
 // (dr14mono/stereo, TPnRMSmono/stereo).
 // lv2_xfer.cu adds phasewheel and stereoscope (raw-audio forwarding to the GUI + correlation), lv2_gon.cu the goniometer, whose
 // GUI reaches into the plugin's C struct through LV2 instance-access (ring buffer, mutex: src/goniometer.h): its instance
-// handle points at a struct laid out like the reference's.  All 38 descriptors of the reference are served.
+// handle points at a struct laid out like the reference's.  All 38 descriptors of the reference are served.  In batched mode
+// phasewheel and goniometer instances take slots in the COR plugin's hub (cor_hub_join / cor_hub_cycle below).
 // Each LV2 instance owns a bank of one instance; run() is synchronous (host buffers in, ports out), exactly the
 // reference's calling convention (robtk/jackwrap.c:531-544).  LV2 core types are restated from the LV2
 // specification (the SDK is not installed); the struct layout is the stable public C ABI.
 #include <math.h>
 #include <stdlib.h>
 #include <string.h>
+#include <algorithm>
 #include "lv2_hub.cuh"
 
 namespace b200m {
@@ -50,8 +52,9 @@ struct Shim {
 
 // batched mode (lv2_hub.cuh): every plugin of this file.  Per-instance controls are stored per slot at submit and reach the bank
 // with the cycle's launch: spectr30's speed / reset (b200m_spec_process_ctl_host), BBCM6's S gain (b200m_ppm_set_gain_inst), a
-// surround meter's pair selection (the launch gathers the selected rows into the correlation bank's stage).  A vacated or newly
-// joined slot is cleared to a freshly instantiated plugin.
+// surround meter's pair selection (the launch gathers the selected rows into the correlation bank's stage), and in the COR hub the
+// hold of a phasewheel whose cycle is skipped (b200m_cor_process_ctl_host).  A vacated or newly joined slot is cleared to a
+// freshly instantiated plugin.
 constexpr uint8_t SUR_IDLE = 0xff;                        // a correlation pair that meters silence (4th pair of surround3, unconnected)
 
 struct ShimHub : SlotHub {
@@ -60,6 +63,7 @@ struct ShimHub : SlotHub {
     std::vector<float> spec_ctl;                          // spectr30: [slot] {port 60, port 61} as last submitted
     std::vector<float> s_gain;                            // BBCM6: [slot] S meter gain (dB) as last submitted
     std::vector<uint8_t> sur_sel;                         // surround: [slot][8] input channel of each pair's L and R row, or SUR_IDLE
+    std::vector<uint8_t> cor_run;                         // COR: [slot] 0 = held in the open cycle (its bank state left untouched)
     PinnedStage pairs;                                    // surround: [slots * 8] rows, the correlation bank's input
 
     ShimHub (const HubKey& k, uint32_t n) : SlotHub (k, n) {}
@@ -72,7 +76,7 @@ struct ShimHub : SlotHub {
         const uint32_t rows = n * k.chn;
         int rc = -1;
         switch (k.family) {
-        case K_COR: rc = b200m_cor_create (&h->cor, 0, n, (int)k.rate, 2e3f, 0.3f); h->f_res.assign (n, 0.0f); break;
+        case K_COR: rc = b200m_cor_create (&h->cor, 0, n, (int)k.rate, 2e3f, 0.3f); h->f_res.assign (n, 0.0f); h->cor_run.assign (n, 1); break;
         case K_DBTP: case K_KMETER: rc = b200m_tpk_create (&h->tpk, 0, rows, (float)k.rate, k.tpk_flags); h->tpk_res.assign (rows, b200m_tpk_result{0, 0, 0, 0}); break;
         case K_NEEDLE: rc = b200m_ppm_create (&h->ppm, 0, rows, (float)k.rate, k.ppm_kind); h->f_res.assign (rows, 0.0f); break;
         case K_BBCM6: rc = b200m_ppm_create (&h->ppm, 0, n, (float)k.rate, B200M_PPM_MS); h->f_res.assign (2 * n, 0.0f); h->s_gain.assign (n, -6.0f); break;
@@ -95,7 +99,13 @@ struct ShimHub : SlotHub {
     {
         int rc = -1;
         switch (key.family) {
-        case K_COR: rc = b200m_cor_process_host (cor, stage.data, B200M_MAX_BLOCK, n); break;
+        case K_COR: {
+            // the mask reaches the bank only in cycles where a slot holds; every slot runs again in the next cycle unless held anew
+            const bool hold = std::find (cor_run.begin (), cor_run.end (), 0) != cor_run.end ();
+            rc = b200m_cor_process_ctl_host (cor, stage.data, B200M_MAX_BLOCK, n, hold ? cor_run.data () : nullptr);
+            std::fill (cor_run.begin (), cor_run.end (), 1);
+            break;
+        }
         case K_DBTP: case K_KMETER:
             rc = b200m_tpk_process_host (tpk, stage.data, B200M_MAX_BLOCK, n, B200M_TP_MODE_PROCESS);
             if (!rc) rc = b200m_tpk_read_device (tpk, nullptr);
@@ -146,25 +156,41 @@ struct ShimHub : SlotHub {
         }
         if (spec) { b200m_spec_clear (spec, (int32_t)slot, nullptr); spec_ctl[2 * slot] = 1.0f; spec_ctl[2 * slot + 1] = -4.0f; }
         if (!sur_sel.empty ()) memset (&sur_sel[8 * slot], SUR_IDLE, 8);
+        if (!cor_run.empty ()) cor_run[slot] = 1;
     }
     void vacate (uint32_t slot) override { clear (slot); }
 };
 
-// one cycle of a batched instance: collect the previous cycle's results of this slot, store its controls, hand in this cycle's
-// audio, launch when complete.  ctl: spectr30 {speed, reset}, BBCM6 {S gain}, surround uint8_t[8] pair rows; NULL for the others.
-void shub_cycle (Shim* s, const float* const* in, uint32_t n, b200m_tpk_result* tr, float* fr, uint32_t nf, const void* ctl = nullptr)
+// a slot in a hub with this key, cleared to a freshly instantiated plugin; NULL when batched mode is off
+ShimHub* shub_join (const HubKey& key, void* who, int* slot)
 {
-    ShimHub* hub = s->hub;
+    ShimHub* hub = (ShimHub*)SlotHub::join (key, who, slot, ShimHub::create);
+    if (hub) { std::lock_guard<std::mutex> lh (hub->mu); hub->clear ((uint32_t)*slot); }
+    return hub;
+}
+
+// one cycle of a batched instance: collect the previous cycle's results of this slot, store its controls, hand in this cycle's
+// audio, launch when complete.  ctl: spectr30 {speed, reset}, BBCM6 {S gain}, surround uint8_t[8] pair rows, COR uint8_t hold
+// (NULL: runs); NULL for the others.
+void hub_cycle (ShimHub* hub, int slot, Kind kind, const float* const* in, uint32_t n, b200m_tpk_result* tr, float* fr, uint32_t nf,
+                const void* ctl)
+{
     const uint32_t chn = hub->key.chn;
     std::lock_guard<std::mutex> lh (hub->mu);
-    hub->close_if_broken (s->slot, n);
-    if (tr) for (uint32_t c = 0; c < chn; ++c) tr[c] = hub->tpk_res[(size_t)s->slot * chn + c];
-    if (fr) for (uint32_t k = 0; k < nf; ++k) fr[k] = hub->f_res[(size_t)s->slot * nf + k];
+    hub->close_if_broken (slot, n);
+    if (tr) for (uint32_t c = 0; c < chn; ++c) tr[c] = hub->tpk_res[(size_t)slot * chn + c];
+    if (fr) for (uint32_t k = 0; k < nf; ++k) fr[k] = hub->f_res[(size_t)slot * nf + k];
     // before a launch by this submit; a member that misses a cycle keeps its previous controls
-    if (s->kind == K_SPEC) memcpy (&hub->spec_ctl[2 * s->slot], ctl, 2 * sizeof (float));
-    else if (s->kind == K_BBCM6) hub->s_gain[s->slot] = *(const float*)ctl;
-    else if (s->kind == K_SUR) memcpy (&hub->sur_sel[8 * s->slot], ctl, 8);
-    hub->submit (s->slot, in, n);
+    if (kind == K_SPEC) memcpy (&hub->spec_ctl[2 * slot], ctl, 2 * sizeof (float));
+    else if (kind == K_BBCM6) hub->s_gain[slot] = *(const float*)ctl;
+    else if (kind == K_SUR) memcpy (&hub->sur_sel[8 * slot], ctl, 8);
+    else if (kind == K_COR && ctl) hub->cor_run[slot] = !*(const uint8_t*)ctl;
+    hub->submit (slot, in, n);
+}
+
+void shub_cycle (Shim* s, const float* const* in, uint32_t n, b200m_tpk_result* tr, float* fr, uint32_t nf, const void* ctl = nullptr)
+{
+    hub_cycle (s->hub, s->slot, s->kind, in, n, tr, fr, nf, ctl);
 }
 
 LV2_Handle shim_instantiate (const LV2_Descriptor* d, double rate, const char*, const LV2_Feature* const*)
@@ -186,8 +212,7 @@ LV2_Handle shim_instantiate (const LV2_Descriptor* d, double rate, const char*, 
     else if (!strncmp (u, "spectr30", 8)) { s->kind = K_SPEC; s->chn = strstr (u, "stereo") ? 2 : 1; }
     else known = false;
     int rc = known ? 0 : -1;
-    if (known) s->hub = (ShimHub*)SlotHub::join (HubKey{s->kind, ppm_kind, s->chn, tpk_flags, rate}, s, &s->slot, ShimHub::create);
-    if (s->hub) { std::lock_guard<std::mutex> lh (s->hub->mu); s->hub->clear ((uint32_t)s->slot); }
+    if (known) s->hub = shub_join (HubKey{s->kind, ppm_kind, s->chn, tpk_flags, rate}, s, &s->slot);
     if (known && !s->hub) {                                    // a private bank of one instance unless batched mode puts it into a shared one
         switch (s->kind) {
         case K_COR: rc = b200m_cor_create (&s->cor, 0, 1, (int)rate, 2e3f, 0.3f); break;
@@ -404,6 +429,19 @@ const LV2_Descriptor g_desc[] = {
 };
 
 }  // namespace
+
+namespace b200m {
+// phasewheel and goniometer run the COR plugin's Stcorrdsp, init (rate, 2e3f, 0.3f) on two rows (src/xfer.c:93, src/goniometerlv2.c:73-74)
+SlotHub* cor_hub_join (double rate, void* who, int* slot) { return shub_join (HubKey{K_COR, 0, 2, 0, rate}, who, slot); }
+
+float cor_hub_cycle (SlotHub* hub, int slot, const float* const* in, uint32_t n, bool hold)
+{
+    float v = 0;
+    const uint8_t h = hold;
+    hub_cycle ((ShimHub*)hub, slot, K_COR, in, n, nullptr, &v, 1, &h);
+    return v;
+}
+}
 
 // The one symbol meters.so exports (src/meters.cc:739-792).  Hosts look plugins up by URI; the indices here are
 // the covered subset in the reference's order.

@@ -3,6 +3,9 @@
 // float) while the UI is open, answers ui_on with a ui_state {samplerate} message, and -- phasewheel only -- runs the
 // stereo correlation meter whose value goes to control port 6.  The correlation runs on the GPU (b200m_cor_*); the FFT
 // analysis the reference's GUI performs on the forwarded audio is available GPU-side through b200m_pw_* (pw.cu).
+// Batched mode (B200M_LV2_BATCH): a phasewheel takes a slot in the COR plugin's hub of its sample rate (cor_hub_cycle,
+// lv2_shim.cu); its phase port gets the previous cycle's reading, and a skipped cycle is held in the bank.  The notify messages
+// and the audio stay in their own cycle.  The stereoscope has no DSP and no bank.
 #include <stdio.h>
 #include <stdlib.h>
 #include <string.h>
@@ -16,6 +19,8 @@ enum { SPR_CONTROL = 0, SPR_NOTIFY, SPR_INPUT0, SPR_OUTPUT0, SPR_INPUT1, SPR_OUT
 
 struct XferPlugin {
     b200m_cor* cor = nullptr;                                  // phasewheel only (:93-95)
+    SlotHub* hub = nullptr; int slot = -1;                     // batched phasewheel: a slot of the COR hub instead of `cor`
+    bool last_ran = false;                                     // batched: the previous run() metered its cycle
     PinnedStage stage;
     AtomWriter out;
     const void* control = nullptr; void* notify = nullptr;
@@ -32,7 +37,8 @@ LV2_Handle xfer_instantiate (const LV2_Descriptor* d, double rate, const char*, 
     if (!wheel && strcmp (d->URI, MTR_URI "stereoscope")) return nullptr;
     XferPlugin* p = new (std::nothrow) XferPlugin;
     if (!p) return nullptr;
-    if (wheel && b200m_cor_create (&p->cor, 0, 1, (int)rate, 2e3f, 0.3f)) { delete p; return nullptr; }
+    if (wheel) p->hub = cor_hub_join (rate, p, &p->slot);
+    if (wheel && !p->hub && b200m_cor_create (&p->cor, 0, 1, (int)rate, 2e3f, 0.3f)) { delete p; return nullptr; }
     p->rate = rate;
     auto M = [&] (const char* uri) { return map->map (map->handle, uri); };
     p->atom_Blank = M (B200M_LV2_ATOM "Blank"); p->atom_Object = M (B200M_LV2_ATOM "Object");
@@ -59,6 +65,21 @@ void xfer_connect (LV2_Handle h, uint32_t port, void* data)
     }
 }
 
+// stcor->process; *p_phase = stcor->read () (:248-251).  Batched: the phase port gets the reading of the previous cycle unless
+// that one was skipped, and a skipped cycle (atom buffer too small: no process () in the reference) is submitted held.
+void xfer_meter (XferPlugin* p, uint32_t n, bool skipped)
+{
+    if (n < 1 || n > B200M_MAX_BLOCK) { p->last_ran = false; return; }
+    if (p->hub) {
+        const float v = cor_hub_cycle (p->hub, p->slot, p->input, n, skipped);
+        if (p->last_ran && p->p_phase) *p->p_phase = v;
+        p->last_ran = !skipped;
+    } else if (p->cor && !skipped && p->stage.fill (p->input, 2, n)) {
+        float v = 0;
+        if (b200m_cor_process_host (p->cor, p->stage.data, p->stage.cap, n) == 0 && b200m_cor_results (p->cor, &v, nullptr) == 0 && p->p_phase) *p->p_phase = v;
+    }
+}
+
 void xfer_run (LV2_Handle h, uint32_t n)
 {
     XferPlugin* p = (XferPlugin*)h;
@@ -70,6 +91,7 @@ void xfer_run (LV2_Handle h, uint32_t n)
     const uint32_t capacity = ((const AtomHead*)p->notify)->size;
     if (capacity < size + 128) {                               // the whole cycle is skipped, as in the reference (:190-205)
         if (!p->warned) { fprintf (stderr, "meters.lv2 error: LV2 comm-buffersize is insufficient %u/%zu bytes.\n", capacity, size + 160); p->warned = true; }
+        xfer_meter (p, n, true);
         return;
     }
     p->out.begin_sequence (p->notify, capacity);
@@ -88,10 +110,7 @@ void xfer_run (LV2_Handle h, uint32_t n)
             else if (obj.otype () == p->ui_off) p->ui_active = false;
         }
     }
-    if (p->cor && n >= 1 && n <= B200M_MAX_BLOCK && p->stage.fill (p->input, 2, n)) {      // stcor->process; *p_phase = stcor->read () (:248-251)
-        float v = 0;
-        if (b200m_cor_process_host (p->cor, p->stage.data, p->stage.cap, n) == 0 && b200m_cor_results (p->cor, &v, nullptr) == 0 && p->p_phase) *p->p_phase = v;
-    }
+    xfer_meter (p, n, false);
     if (p->ui_active) {                                        // tx_rawstereo (:162-178)
         p->out.begin_event_object (p->rawstereo);
         p->out.prop_vector_f32 (p->audioleft, p->input[0], n);
@@ -103,6 +122,7 @@ void xfer_run (LV2_Handle h, uint32_t n)
 void xfer_cleanup (LV2_Handle h)
 {
     XferPlugin* p = (XferPlugin*)h;
+    if (p->hub) p->hub->leave (p->slot);
     b200m_cor_destroy (p->cor);
     p->stage.release ();
     delete p;

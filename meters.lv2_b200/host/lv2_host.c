@@ -19,6 +19,11 @@
  *                4 in0, 5 out0, 6-10 outputs of channel 0, 11 in1, 12 out1, 13-17 outputs of channel 1, 18 DR total (no notify port)
  *   surround3..8 (src/surmeter.c:24-70): pair c: 1 + 3c, 2 + 3c input selectors, 3 + 3c correlation; channel c: 13 + 4c in, 14 + 4c out,
  *                15 + 4c level, 16 + 4c peak
+ *   phasewheel / stereoscope (src/xfer.c:50-60): 0 control atom in, 1 notify atom out, 2 in0, 3 out0, 4 in1, 5 out1, 6 phase, 7 gain, 8 range;
+ *                the notify buffer holds one rawstereo message of both channels per cycle, (4 n + 64) * 2 + 128 bytes (:188-205)
+ *   goniometer (src/goniometerlv2.c:27-35): 0 in0, 1 out0, 2 in1, 3 out1, 4 gain, 5 correlation, 6 notify
+ * --ui 1 opens the GUI: meteron (EBUr128, bitmeter, SigDistHist), ui_on (phasewheel, stereoscope); the goniometer's GUI sets ui_active
+ * in the plugin's instance struct (LV2gm, src/goniometer.h:113-169) and drains its ring buffer every cycle, which this host does too.
  */
 #define _GNU_SOURCE
 #include <dlfcn.h>
@@ -61,14 +66,18 @@ typedef struct {
     LV2_Handle h;
     float *in[8], *out[8];
     float ctl[68];                          /* control ports (in and out) */
-    uint8_t *atom_in, *atom_out;            /* EBUr128, bitmeter, SigDistHist */
+    uint8_t *atom_in, *atom_out;            /* EBUr128, bitmeter, SigDistHist, phasewheel, stereoscope */
 } Inst;
 
-typedef struct { const LV2_Descriptor* d; Inst* inst; int first, last; uint32_t nframes; int kind; uint32_t seq_t, chunk_t; pthread_barrier_t *start, *done; int cycles;
-                 int cycle; const uint8_t* first_msgs; uint32_t first_len; } Worker;
+typedef struct { const LV2_Descriptor* d; Inst* inst; int first, last; uint32_t nframes; int kind; uint32_t seq_t, chunk_t, atom_cap; pthread_barrier_t *start, *done;
+                 int cycles; int cycle; const uint8_t* first_msgs; uint32_t first_len; int ui; } Worker;
 
-enum { KIND_MTR, KIND_EBUR, KIND_SPEC, KIND_STATS, KIND_SUR, KIND_DR };
+enum { KIND_MTR, KIND_EBUR, KIND_SPEC, KIND_STATS, KIND_SUR, KIND_DR, KIND_XFER, KIND_GON };
 #define ATOM_CAP 8192
+/* goniometer: the GUI-shared head of LV2gm (src/goniometer.h:33-39,113-116): gmringbuf* rb, then bool ui_active; the ring is
+ * {float* c0, c1; size_t rp, wp, len} */
+typedef struct { float *c0, *c1; size_t rp, wp, len; } GmRing;
+typedef struct { GmRing* rb; _Bool ui_active; } GmHead;
 
 /* one event at frame 0: object {otype; controlkey = key (Int); controlval = val (Float)} -- forge_kvcontrolmessage, src/uris.h:279-294 */
 static uint32_t forge_kv (uint8_t* dst, uint32_t t_object, uint32_t otype, uint32_t t_int, uint32_t t_float, uint32_t k_key, uint32_t k_val, int key, float val, int with_props)
@@ -93,11 +102,12 @@ static void run_range (const Worker* w)
     for (int i = w->first; i < w->last; ++i) {
         Inst* p = &w->inst[i];
         if (w->kind == KIND_DR) { uint32_t* a = (uint32_t*)p->atom_in; a[0] = 8; a[1] = w->seq_t; a[2] = 0; a[3] = 0; }   /* empty input sequence */
-        if (w->kind == KIND_EBUR || w->kind == KIND_STATS) {   /* host convention: empty input sequence, output buffer announced as a chunk of its capacity */
+        if (w->kind == KIND_EBUR || w->kind == KIND_STATS || w->kind == KIND_XFER) {   /* host convention: empty input sequence, output buffer announced as a chunk of its capacity */
             uint32_t* a = (uint32_t*)p->atom_in; a[0] = 8; a[1] = w->seq_t; a[2] = 0; a[3] = 0;
             if (w->cycle == 0 && w->first_len) { memcpy (p->atom_in + 16, w->first_msgs, w->first_len); a[0] = 8 + w->first_len; }   /* the GUI's opening messages */
-            uint32_t* o = (uint32_t*)p->atom_out; o[0] = ATOM_CAP - 8; o[1] = w->chunk_t;
+            uint32_t* o = (uint32_t*)p->atom_out; o[0] = w->atom_cap - 8; o[1] = w->chunk_t;
         }
+        if (w->kind == KIND_GON && w->ui) { GmHead* g = (GmHead*)p->h; g->ui_active = 1; g->rb->rp = g->rb->wp; }   /* the GUI's open / gmrb_read_clear */
         w->d->run (p->h, w->nframes);
     }
 }
@@ -128,7 +138,7 @@ int main (int argc, char** argv)
         else if (!strcmp (argv[i], "--rate")) rate = atof (argv[i + 1]);
         else if (!strcmp (argv[i], "--threads")) threads = atoi (argv[i + 1]);
         else if (!strcmp (argv[i], "--dbtp")) dbtp = atoi (argv[i + 1]);       /* EBUr128: enable the true-peak meters (CTL_UISETTINGS bit 64) */
-        else if (!strcmp (argv[i], "--ui")) ui = atoi (argv[i + 1]);           /* EBUr128, bitmeter, SigDistHist: a GUI is attached (meteron) */
+        else if (!strcmp (argv[i], "--ui")) ui = atoi (argv[i + 1]);           /* a GUI is attached (EBUr128, bitmeter, SigDistHist, phasewheel, stereoscope, goniometer) */
         else { fprintf (stderr, "unknown option %s\n", argv[i]); return 2; }
     }
     if (threads < 1) threads = 1;
@@ -143,8 +153,10 @@ int main (int argc, char** argv)
     if (!d) { fprintf (stderr, "%s not served by %s\n", full, lib); return 1; }
     const int kind = !strcmp (uri, "EBUr128") ? KIND_EBUR : !strncmp (uri, "spectr30", 8) ? KIND_SPEC
                    : !strcmp (uri, "bitmeter") || !strcmp (uri, "SigDistHist") ? KIND_STATS : !strncmp (uri, "surround", 8) ? KIND_SUR
-                   : !strncmp (uri, "dr14", 4) || !strncmp (uri, "TPnRMS", 6) ? KIND_DR : KIND_MTR;
-    const int stereo = kind == KIND_EBUR || strstr (uri, "stereo") || !strcmp (uri, "COR") || !strcmp (uri, "BBCM6");
+                   : !strncmp (uri, "dr14", 4) || !strncmp (uri, "TPnRMS", 6) ? KIND_DR
+                   : !strcmp (uri, "phasewheel") || !strcmp (uri, "stereoscope") ? KIND_XFER : !strcmp (uri, "goniometer") ? KIND_GON : KIND_MTR;
+    const int stereo = kind == KIND_EBUR || kind == KIND_XFER || kind == KIND_GON || strstr (uri, "stereo") || !strcmp (uri, "COR") || !strcmp (uri, "BBCM6");
+    const uint32_t atom_cap = kind == KIND_XFER ? (4 * nframes + 64) * 2 + 1024 : ATOM_CAP;
     const int chn = kind == KIND_SUR ? uri[8] - '0' : stereo ? 2 : 1;
 
     LV2_URID_Map map = {NULL, urid_map};
@@ -163,6 +175,8 @@ int main (int argc, char** argv)
         if (kind == KIND_EBUR) first_len += forge_kv (first_msgs + first_len, t_obj, cfg, t_int, t_flt, kk, kv, 7 /* CTL_UISETTINGS */, dbtp ? 64.0f : 0.0f, 1);
         if (kind == KIND_EBUR || !strcmp (uri, "SigDistHist")) first_len += forge_kv (first_msgs + first_len, t_obj, cfg, t_int, t_flt, kk, kv, 1 /* CTL_START */, 0.0f, 1);
     }
+    if (kind == KIND_XFER && ui)                        /* phasewheel / stereoscope GUI: ui_on (gui/phasewheel.c:263-270) */
+        first_len += forge_kv (first_msgs, urid_map (NULL, "http://lv2plug.in/ns/ext/atom#Object"), urid_map (NULL, MTR_URI "ui_on"), 0, 0, 0, 0, 0, 0, 0);
     Inst* inst = (Inst*)calloc ((size_t)n_inst, sizeof (Inst));
     uint64_t s = 0x42B200;
     for (int i = 0; i < n_inst; ++i) {
@@ -173,11 +187,17 @@ int main (int argc, char** argv)
             p->in[c] = (float*)malloc (sizeof (float) * nframes); p->out[c] = (float*)malloc (sizeof (float) * nframes);
             for (uint32_t k = 0; k < nframes; ++k) { s ^= s << 13; s ^= s >> 7; s ^= s << 17; p->in[c][k] = ((float)(s >> 40) * (1.0f / 8388608.0f) - 1.0f) * 0.25f; }
         }
-        if (kind == KIND_EBUR || kind == KIND_STATS) {
-            p->atom_in = (uint8_t*)calloc (1, 1024); p->atom_out = (uint8_t*)calloc (1, ATOM_CAP);
+        if (kind == KIND_EBUR || kind == KIND_STATS || kind == KIND_XFER) {
+            p->atom_in = (uint8_t*)calloc (1, 1024); p->atom_out = (uint8_t*)calloc (1, atom_cap);
             d->connect_port (p->h, 0, p->atom_in); d->connect_port (p->h, 1, p->atom_out);
             d->connect_port (p->h, 2, p->in[0]); d->connect_port (p->h, 3, p->out[0]);
-            if (kind == KIND_EBUR) { d->connect_port (p->h, 4, p->in[1]); d->connect_port (p->h, 5, p->out[1]); }
+            if (stereo) { d->connect_port (p->h, 4, p->in[1]); d->connect_port (p->h, 5, p->out[1]); }
+            if (kind == KIND_XFER) for (uint32_t k = 6; k < 9; ++k) d->connect_port (p->h, k, &p->ctl[k]);
+        } else if (kind == KIND_GON) {
+            d->connect_port (p->h, 0, p->in[0]); d->connect_port (p->h, 1, p->out[0]);
+            d->connect_port (p->h, 2, p->in[1]); d->connect_port (p->h, 3, p->out[1]);
+            p->ctl[4] = 1.0f;
+            for (uint32_t k = 4; k < 7; ++k) d->connect_port (p->h, k, &p->ctl[k]);
         } else if (kind == KIND_SPEC) {
             for (uint32_t k = 0; k < 64; ++k) d->connect_port (p->h, k, &p->ctl[k]);
             p->ctl[60] = 1.0f; p->ctl[61] = -4.0f; p->ctl[62] = 0.0f;
@@ -211,7 +231,7 @@ int main (int argc, char** argv)
     Worker* w = (Worker*)calloc ((size_t)threads, sizeof (Worker)); pthread_t* th = (pthread_t*)calloc ((size_t)threads, sizeof (pthread_t));
     for (int t = 0; t < threads; ++t) {
         w[t].d = d; w[t].inst = inst; w[t].first = (int)((long long)n_inst * t / threads); w[t].last = (int)((long long)n_inst * (t + 1) / threads);
-        w[t].nframes = nframes; w[t].kind = kind; w[t].seq_t = seq_t; w[t].chunk_t = chunk_t; w[t].start = &b_start; w[t].done = &b_done; w[t].cycles = warm + cycles; w[t].first_msgs = first_msgs; w[t].first_len = first_len;
+        w[t].nframes = nframes; w[t].kind = kind; w[t].seq_t = seq_t; w[t].chunk_t = chunk_t; w[t].atom_cap = atom_cap; w[t].ui = ui; w[t].start = &b_start; w[t].done = &b_done; w[t].cycles = warm + cycles; w[t].first_msgs = first_msgs; w[t].first_len = first_len;
         pthread_create (&th[t], NULL, worker_main, &w[t]);
     }
     double sum = 0, worst = 0;
@@ -224,7 +244,7 @@ int main (int argc, char** argv)
     }
     for (int t = 0; t < threads; ++t) pthread_join (th[t], NULL);
     const double mean = sum / cycles, budget = nframes / rate;
-    float probe = kind == KIND_EBUR || kind == KIND_STATS ? 0.0f : inst[0].ctl[kind == KIND_DR ? 6 : 3];
+    float probe = kind == KIND_EBUR || kind == KIND_STATS ? 0.0f : inst[0].ctl[kind == KIND_DR || kind == KIND_XFER ? 6 : kind == KIND_GON ? 5 : 3];
     const char* batch = getenv ("B200M_LV2_BATCH");
     printf ("{\"lv2_host\": \"%s\", \"lib\": \"%s\", \"instances\": %d, \"threads\": %d, \"nframes\": %u, \"rate\": %.0f, \"cycles\": %d, "
             "\"dbtp\": %d, \"ui\": %d, \"batch_slots\": %s, \"cycle_ms_mean\": %.4f, \"cycle_ms_max\": %.4f, \"us_per_instance\": %.3f, \"budget_ms\": %.3f, \"fits_realtime\": %s, "
