@@ -96,6 +96,16 @@ typedef struct b200m_ebu_result {          /* getters, ebumeter/ebu_r128_proc.h:
 /* Ebu_r128_proc() + init(nchan, fsamp) (:166-173) for n_inst instances.  nchan 1..5 (the EBUr128 plugin uses 2, src/ebulv2.cc:190;
  * 3..5: surround layouts with the channel gains 1 1 1 1.41 1.41 of ebu_r128_proc.cc:29). */
 int b200m_ebu_create (b200m_ebu** out, int device, uint32_t n_inst, uint32_t nchan, float fsamp);
+/* The same bank with nchan = 1..32 channels per instance and caller-given channel weights: the per-chunk channel sum is
+ * si = gains[0] * sj0, then si += gains[c] * sj_c in channel order, in fp32 (detect_process, ebu_r128_proc.cc:328-330, with these
+ * weights; mono {2.0f} is the reference's 2 * sj).  Gains must be finite and >= 0 with at least one > 0, else B200M_E_INVAL and
+ * *out = NULL.  The reference's own weights for 1..5 channels (mono {2}, else 1 1 1 1.41 1.41) give exactly b200m_ebu_create's bank;
+ * any other set runs the run-time channel-count K-weighting kernel.  Snapshots of a weighted bank record nchan and the gains and
+ * restore only into a bank with the same ones (bitwise). */
+int b200m_ebu_create_weighted (b200m_ebu** out, int device, uint32_t n_inst, uint32_t nchan, const float* gains, float fsamp);
+/* ITU-R BS.1770-4 channel weights from loudspeaker positions in degrees: 1.41 when |elevation| < 30 and 60 <= |azimuth| <= 120
+ * (azimuth taken modulo 360 into -180 .. 180), 1.0 otherwise.  Host only: needs no device.  Non-finite positions: B200M_E_INVAL. */
+int b200m_bs1770_weights (uint32_t n, const float* azimuth_deg, const float* elevation_deg, float* gains);
 int b200m_ebu_destroy (b200m_ebu* h);
 /* Ebu_r128_proc::reset (:176-190) of one instance, or of every instance with inst = -1.  Every instance has its own 50 ms
  * fragment clock: reset() restarts it, so the instance's next fragment ends fragm frames into the next processed block. */
@@ -211,6 +221,13 @@ int b200m_r128_create (b200m_r128** out, int device, uint32_t n_inst, float fsam
  * it out): pass the non-LFE rows.  Every other b200m_r128_* call works on such a bank; CLEAR / NEW and a disabled dBTP cover all
  * the instance's channels, and a snapshot restores only into a bank with the same nchan. */
 int b200m_r128_create_nch (b200m_r128** out, int device, uint32_t n_inst, uint32_t nchan, float fsamp, int dbtp_enable);
+/* Immersive and custom layouts: n_inst instances of nchan = 1..32 channels with per-channel loudness weights gains[c]
+ * (b200m_ebu_create_weighted; b200m_bs1770_weights gives the BS.1770-4 weights of a layout).  Rows are inst * nchan + c.  A gain
+ * of 0 keeps a channel out of the loudness but not out of the dBTP hold: pass an LFE row in place to get BS.1770 loudness and the
+ * true peak of every channel.  The reference's weights for 1..5 channels give exactly b200m_r128_create_nch's bank (same kernels
+ * and snapshot bytes).  Every other b200m_r128_* call works on such a bank unchanged; its snapshot restores only into a bank with
+ * the same nchan and gains. */
+int b200m_r128_create_weighted (b200m_r128** out, int device, uint32_t n_inst, uint32_t nchan, const float* gains, float fsamp, int dbtp_enable);
 int b200m_r128_destroy (b200m_r128* h);
 int b200m_r128_control (b200m_r128* h, int32_t inst, int cmd, void* stream);      /* inst = -1: all */
 int b200m_r128_run_device (b200m_r128* h, const float* d_in, size_t stride, uint32_t nfram, void* stream);

@@ -49,6 +49,8 @@ _PROTOS = {
     "b200m_design_spec": (C.c_int, [C.c_double, _v]),
     # EBU
     "b200m_ebu_create": (C.c_int, [C.POINTER(_v), C.c_int, C.c_uint32, C.c_uint32, C.c_float]),
+    "b200m_ebu_create_weighted": (C.c_int, [C.POINTER(_v), C.c_int, C.c_uint32, C.c_uint32, _v, C.c_float]),
+    "b200m_bs1770_weights": (C.c_int, [C.c_uint32, _v, _v, _v]),
     "b200m_ebu_destroy": (C.c_int, [_v]),
     "b200m_ebu_reset": (C.c_int, [_v, C.c_int32, _v]),
     "b200m_ebu_integr_start": (C.c_int, [_v, C.c_int32, _v]),
@@ -89,6 +91,7 @@ _PROTOS = {
     # EBUr128 plugin cycle
     "b200m_r128_create": (C.c_int, [C.POINTER(_v), C.c_int, C.c_uint32, C.c_float, C.c_int]),
     "b200m_r128_create_nch": (C.c_int, [C.POINTER(_v), C.c_int, C.c_uint32, C.c_uint32, C.c_float, C.c_int]),
+    "b200m_r128_create_weighted": (C.c_int, [C.POINTER(_v), C.c_int, C.c_uint32, C.c_uint32, _v, C.c_float, C.c_int]),
     "b200m_r128_destroy": (C.c_int, [_v]),
     "b200m_r128_control": (C.c_int, [_v, C.c_int32, C.c_int, _v]),
     "b200m_r128_run_device": (C.c_int, [_v, _v, C.c_size_t, C.c_uint32, _v]),
@@ -273,6 +276,24 @@ def design_spec(rate):
     return W
 
 
+def bs1770_weights(azimuth, elevation):
+    """ITU-R BS.1770-4 channel weights of a layout from its loudspeaker positions in degrees (b200m_bs1770_weights): 1.41 where
+    |elevation| < 30 and 60 <= |azimuth| <= 120, else 1.0.  Needs no GPU."""
+    az = np.ascontiguousarray(azimuth, np.float32).ravel(); el = np.ascontiguousarray(elevation, np.float32).ravel()
+    assert az.shape == el.shape, "one elevation per azimuth"
+    g = np.empty(az.size, np.float32)
+    _ck(lib().b200m_bs1770_weights(az.size, _np_ptr(az), _np_ptr(el), _np_ptr(g)))
+    return g
+
+
+def _gains(gains, nchan):
+    """caller weights as a float32 array of nchan entries (the C side validates their values)"""
+    g = np.ascontiguousarray(gains, np.float32).ravel()
+    if g.size != nchan:
+        raise B200MError("%d gains for %d channels" % (g.size, nchan))
+    return g
+
+
 def host_alloc(rows, cols):
     """[rows, cols] float32 numpy array in pinned host memory from b200m_host_alloc (placed on the GPU-local NUMA node);
     freed with b200m_host_free when the array is garbage-collected."""
@@ -320,10 +341,15 @@ class Ebu_r128_proc(_Bank):
     """N x LV2M::Ebu_r128_proc (ebumeter/ebu_r128_proc.h:66-125)."""
     _destroy = "b200m_ebu_destroy"
 
-    def __init__(self, n_inst, nchan=2, fsamp=48000.0, device=0):
+    def __init__(self, n_inst, nchan=2, fsamp=48000.0, device=0, gains=None):
+        """gains: None for the reference's weights (nchan 1..5), or nchan per-channel weights (nchan 1..32, b200m_ebu_create_weighted)"""
         super().__init__()
         self.n_inst, self.nchan = n_inst, nchan
-        _ck(lib().b200m_ebu_create(C.byref(self.h), device, n_inst, nchan, fsamp))
+        if gains is None:
+            _ck(lib().b200m_ebu_create(C.byref(self.h), device, n_inst, nchan, fsamp))
+        else:
+            self.gains = _gains(gains, nchan)
+            _ck(lib().b200m_ebu_create_weighted(C.byref(self.h), device, n_inst, nchan, _np_ptr(self.gains), fsamp))
 
     def reset(self, inst=-1, stream=None):
         """Ebu_r128_proc::reset of one instance (its 50 ms fragment clock restarts with the next block), or of all with inst=-1"""
@@ -792,14 +818,20 @@ class Phasewheel(_Bank):
 
 class EBUr128(_Bank):
     """N x the EBUr128 plugin's audio cycle (ebur128_run, src/ebulv2.cc:341-367): EBU R128 + optional dBTP.
-    nchan 1..5 channels per instance (rows inst * nchan + c, order L R C Ls Rs, no LFE); the plugin itself is stereo."""
+    nchan 1..5 channels per instance (rows inst * nchan + c, order L R C Ls Rs, no LFE); the plugin itself is stereo.
+    gains: nchan per-channel loudness weights for any layout of 1..32 channels (b200m_r128_create_weighted; bs1770_weights gives
+    the BS.1770-4 ones); a zero weight keeps a row (an LFE) out of the loudness but in the dBTP hold."""
     _destroy = "b200m_r128_destroy"
     START, PAUSE, RESET, CLEAR_TPMAX, CLEAR, NEW = 1, 2, 3, 4, 5, 6
 
-    def __init__(self, n_inst, fsamp=48000.0, dbtp_enable=True, device=0, nchan=2):
+    def __init__(self, n_inst, fsamp=48000.0, dbtp_enable=True, device=0, nchan=2, gains=None):
         super().__init__()
         self.n_inst, self.nchan = n_inst, nchan
-        _ck(lib().b200m_r128_create_nch(C.byref(self.h), device, n_inst, nchan, fsamp, int(dbtp_enable)))
+        if gains is None:
+            _ck(lib().b200m_r128_create_nch(C.byref(self.h), device, n_inst, nchan, fsamp, int(dbtp_enable)))
+        else:
+            self.gains = _gains(gains, nchan)
+            _ck(lib().b200m_r128_create_weighted(C.byref(self.h), device, n_inst, nchan, _np_ptr(self.gains), fsamp, int(dbtp_enable)))
         self.ebu = Ebu_r128_proc.__new__(Ebu_r128_proc)
         self.ebu.h = _v(lib().b200m_r128_ebu(self.h)); self.ebu.n_inst = n_inst; self.ebu.nchan = nchan
         self.ebu._destroy = None

@@ -11,6 +11,8 @@
 // histogram bins that must be bit-exact.
 #include <math.h>
 #include <stdlib.h>
+#include <string.h>
+#include <cmath>
 #include <cuda.h>
 #include <algorithm>
 #include <map>
@@ -177,6 +179,26 @@ ebu_kweight_frag (const float* __restrict__ in, size_t stride, int nchans, int k
     sg.init (in, stride, ebu_smem + warp * EBU_WARP_FLOATS, lane, k0, k_end, nfram);
     kw_warp<NCHAN, PHASES> (sg, lane, min (k0 + lane, k_end - 1) /* tail lanes shadow the last channel (no stores) */, lane < CPW && (k0 + lane) < k_end,
                             nchans, nfram, cf, ck, fragm_f, zst, frpwr, fragpw, n_inst);
+}
+
+// the same kernel for a weighted bank (b200m_ebu_create_weighted): gw.nch = 1..32 channels per instance, known at run time, a warp
+// takes CPW = (32 / nch) nch channels (whole instances), and the channel sum uses the bank's weights gw.g
+template <bool ALIGNED, bool PHASES>
+__global__ void __launch_bounds__ (EBU_WARPS * 32)
+ebu_kweight_frag_w (const float* __restrict__ in, size_t stride, int nchans, int k_first, int k_end, int nfram, EbuCoef cf, EbuChunks ck,
+                    float fragm_f, float* __restrict__ zst, float* __restrict__ frpwr, float* __restrict__ fragpw, int n_inst, int pdl_trigger,
+                    const __grid_constant__ EbuGains gw)
+{
+    extern __shared__ __align__ (16) float ebu_smem[];
+    if (pdl_trigger) asm volatile ("griddepcontrol.launch_dependents;");
+    const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
+    const int cpw = (32 / gw.nch) * gw.nch;
+    const int k0 = k_first + (blockIdx.x * EBU_WARPS + warp) * cpw;
+    if (k0 >= k_end) return;
+    PaddedStage<ALIGNED> sg;
+    sg.init (in, stride, ebu_smem + warp * EBU_WARP_FLOATS, lane, k0, k_end, nfram);
+    kw_warp<0, PHASES> (sg, lane, min (k0 + lane, k_end - 1), lane < cpw && (k0 + lane) < k_end,
+                        nchans, nfram, cf, ck, fragm_f, zst, frpwr, fragpw, n_inst, &gw);
 }
 
 // ---- K1 split over two warps per 32 channels -------------------------------------------------------------------------------
@@ -647,6 +669,7 @@ struct EbuPhase { int n = 0, G = 0; int cnt10[10] = {0}; };   // one phase class
 
 struct b200m_ebu {
     int device; uint32_t n_inst, nchan; float fsamp; int fragm;
+    bool weighted = false; EbuGains gw = {};   // b200m_ebu_create_weighted with other than the default weights: ebu_kweight_frag_w
     int tmod = 0;                        // bank time mod fragm
     int fragrows = EBU_MAXCHUNK;         // rows of d_fragpw: the most fragments one K1 launch completes per instance
     EbuCoef cf;
@@ -743,18 +766,39 @@ int b200m_design_ebu (float fsamp, float o[7])
     return 0;
 }
 
-int b200m_ebu_create (b200m_ebu** out, int device, uint32_t n_inst, uint32_t nchan, float fsamp)
+}  // extern "C"
+
+bool ebu_default_gains (uint32_t nchan, const float* gains)
 {
-    if (!out) return set_err (B200M_E_INVAL, "NULL out pointer");
-    *out = nullptr;
+    static const float dflt[5] = {1.0f, 1.0f, 1.0f, 1.41f, 1.41f};          // ebu_r128_proc.cc:29; mono: 2 * sj (:327)
+    if (nchan < 1 || nchan > 5) return false;
+    if (nchan == 1) { const float two = 2.0f; return memcmp (gains, &two, 4) == 0; }
+    return memcmp (gains, dflt, 4 * nchan) == 0;
+}
+
+int ebu_check_gains (uint32_t nchan, const float* gains)
+{
+    if (nchan < 1 || nchan > (uint32_t)EBU_MAXCH_W) return set_err (B200M_E_INVAL, "nchan %u outside 1..%d", nchan, EBU_MAXCH_W);
+    if (!gains) return set_err (B200M_E_INVAL, "NULL gains");
+    bool any = false;
+    for (uint32_t c = 0; c < nchan; ++c) {
+        if (!std::isfinite (gains[c]) || gains[c] < 0.0f) return set_err (B200M_E_INVAL, "gain %u is not finite and >= 0", c);
+        any |= gains[c] > 0.0f;
+    }
+    return any ? 0 : set_err (B200M_E_INVAL, "every gain is zero");
+}
+
+// gains == nullptr: the default weights of a 1..5-channel bank (the compile-time K1 instantiations); otherwise a weighted bank
+static int ebu_create (b200m_ebu** out, int device, uint32_t n_inst, uint32_t nchan, float fsamp, const float* gains)
+{
     if (n_inst == 0 || !(fsamp >= 1000.0f)) return set_err (B200M_E_INVAL, "bad n_inst/fsamp");
-    if (nchan < 1 || nchan > 5) return set_err (B200M_E_INVAL, "nchan %u outside 1..5", nchan);
     if (b200m_device_count () <= 0) return set_err (B200M_E_NODEVICE, "no CUDA device: b200meters has no CPU path");
     DeviceGuard g (device);
     if (!g.ok) return set_err (B200M_E_NODEVICE, "cannot select CUDA device %d", device);
     b200m_ebu* h = new (std::nothrow) b200m_ebu;
     if (!h) return set_err (B200M_E_NOMEM, "host allocation failed");
     h->device = device; h->n_inst = n_inst; h->nchan = nchan; h->fsamp = fsamp;
+    if (gains) { h->weighted = true; h->gw.nch = (int)nchan; memcpy (h->gw.g, gains, 4 * nchan); }
     h->fragm = (int)fsamp / 20;                     // :170
     // with per-instance phases one K1 launch covers a whole block (a split would add a cut the reference does not make)
     h->fragrows = std::max<int> (EBU_MAXCHUNK, (int)(B200M_MAX_BLOCK / (uint32_t)h->fragm) + 2);
@@ -788,6 +832,11 @@ int b200m_ebu_create (b200m_ebu** out, int device, uint32_t n_inst, uint32_t nch
     EBU_ATTR (3, true); EBU_ATTR (3, false); EBU_ATTR (4, true); EBU_ATTR (4, false); EBU_ATTR (5, true); EBU_ATTR (5, false);
 #undef EBU_ATTR
 #undef EBU_ATTR1
+    if (gains)
+        for (const auto k : {ebu_kweight_frag_w<true, false>, ebu_kweight_frag_w<true, true>, ebu_kweight_frag_w<false, false>, ebu_kweight_frag_w<false, true>}) {
+            if (e == cudaSuccess) e = cudaFuncSetAttribute (k, cudaFuncAttributeMaxDynamicSharedMemorySize, EBU_SMEM_BYTES);
+            if (e == cudaSuccess) e = cudaFuncSetAttribute (k, cudaFuncAttributePreferredSharedMemoryCarveout, cudaSharedmemCarveoutMaxShared);
+        }
     if (e == cudaSuccess) e = cudaFuncSetAttribute (ebu_kweight_tma<1>, cudaFuncAttributeMaxDynamicSharedMemorySize, EBU_TMA_SMEM);
     if (e == cudaSuccess) e = cudaFuncSetAttribute (ebu_kweight_tma<2>, cudaFuncAttributeMaxDynamicSharedMemorySize, EBU_TMA_SMEM);
     if (e == cudaSuccess) e = cudaFuncSetAttribute (ebu_kweight_tma<1>, cudaFuncAttributePreferredSharedMemoryCarveout, cudaSharedmemCarveoutMaxShared);
@@ -808,6 +857,41 @@ int b200m_ebu_create (b200m_ebu** out, int device, uint32_t n_inst, uint32_t nch
     if (rc == 0 && cudaDeviceSynchronize () != cudaSuccess) rc = set_err (B200M_E_CUDA, "reset kernel failed");
     if (rc) { b200m_ebu_destroy (h); return rc; }
     *out = h;
+    return 0;
+}
+
+extern "C" {
+
+int b200m_ebu_create (b200m_ebu** out, int device, uint32_t n_inst, uint32_t nchan, float fsamp)
+{
+    if (!out) return set_err (B200M_E_INVAL, "NULL out pointer");
+    *out = nullptr;
+    if (nchan < 1 || nchan > 5) return set_err (B200M_E_INVAL, "nchan %u outside 1..5", nchan);
+    return ebu_create (out, device, n_inst, nchan, fsamp, nullptr);
+}
+
+int b200m_ebu_create_weighted (b200m_ebu** out, int device, uint32_t n_inst, uint32_t nchan, const float* gains, float fsamp)
+{
+    if (!out) return set_err (B200M_E_INVAL, "NULL out pointer");
+    *out = nullptr;
+    if (int rc = ebu_check_gains (nchan, gains)) return rc;
+    return ebu_create (out, device, n_inst, nchan, fsamp, ebu_default_gains (nchan, gains) ? nullptr : gains);
+}
+
+// ITU-R BS.1770-4 channel weights from loudspeaker positions: 1.41 for |elevation| < 30 degrees and 60 <= |azimuth| <= 120 degrees
+// (azimuth taken modulo 360 into -180 .. 180), 1.0 otherwise.  Host only.
+int b200m_bs1770_weights (uint32_t n, const float* azimuth_deg, const float* elevation_deg, float* gains)
+{
+    if (n && (!azimuth_deg || !elevation_deg || !gains)) return set_err (B200M_E_INVAL, "NULL argument");
+    for (uint32_t c = 0; c < n; ++c)
+        if (!std::isfinite (azimuth_deg[c]) || !std::isfinite (elevation_deg[c])) return set_err (B200M_E_INVAL, "position %u is not finite", c);
+    for (uint32_t c = 0; c < n; ++c) {
+        double az = fmod ((double)azimuth_deg[c], 360.0);
+        if (az > 180.0) az -= 360.0;
+        else if (az < -180.0) az += 360.0;
+        az = fabs (az);
+        gains[c] = (fabs ((double)elevation_deg[c]) < 30.0 && az >= 60.0 && az <= 120.0) ? 1.41f : 1.0f;
+    }
     return 0;
 }
 
@@ -906,7 +990,7 @@ int ebu_process_sliced (b200m_ebu* h, const float* d_in, size_t stride, uint32_t
         }
         const bool al = aligned && (done % 4 == 0);
         CUtensorMap tmap;
-        const bool tma = !fused && !multi && al && h->use_tma && h->nchan <= 2 && tma_input_map (&tmap, src, stride, (uint32_t)nch, pos);
+        const bool tma = !fused && !multi && al && h->use_tma && h->nchan <= 2 && !h->weighted && tma_input_map (&tmap, src, stride, (uint32_t)nch, pos);
         for (int sl = 0; !fused && sl < nsl; ++sl) {
             const int kf = (int)(bounds[sl] * h->nchan), ke = (int)(bounds[sl + 1] * h->nchan);
             if (ke <= kf) continue;
@@ -917,7 +1001,14 @@ int ebu_process_sliced (b200m_ebu* h, const float* d_in, size_t stride, uint32_t
 #define EBU_K1P(NC, AL, PH) ebu_kweight_frag<NC, AL, PH><<<grid, blk, EBU_SMEM_BYTES, st>>> (src, stride, nch, kf, ke, (int)pos, h->cf, ck, (float)h->fragm, h->d_z, h->d_frpwr, h->d_fragpw, (int)h->n_inst, (after_k1 && done == 0) ? 1 : 0)
 #define EBU_K1(NC, AL) do { if (multi) EBU_K1P (NC, AL, true); else EBU_K1P (NC, AL, false); } while (0)
 #define EBU_K1T(NC) ebu_kweight_tma<NC><<<grid, blk, EBU_TMA_SMEM, st>>> (tmap, nch, kf, ke, (int)pos, h->cf, ck, (float)h->fragm, h->d_z, h->d_frpwr, h->d_fragpw, (int)h->n_inst, (after_k1 && done == 0) ? 1 : 0)
-            if (h->nchan > 2) {                                  // surround banks (3..5 channels): the one-warp kernel, lanes grouped per instance
+            if (h->weighted) {                                   // weighted banks: the run-time channel count, lanes grouped per instance
+                const int pt = (after_k1 && done == 0) ? 1 : 0;
+#define EBU_K1W(AL, PH) ebu_kweight_frag_w<AL, PH><<<grid, blk, EBU_SMEM_BYTES, st>>> (src, stride, nch, kf, ke, (int)pos, h->cf, ck, (float)h->fragm, h->d_z, h->d_frpwr, h->d_fragpw, (int)h->n_inst, pt, h->gw)
+                if (al) { if (multi) EBU_K1W (true, true); else EBU_K1W (true, false); }
+                else    { if (multi) EBU_K1W (false, true); else EBU_K1W (false, false); }
+#undef EBU_K1W
+            }
+            else if (h->nchan > 2) {                             // surround banks (3..5 channels): the one-warp kernel, lanes grouped per instance
                 switch (h->nchan * 2 + (al ? 1 : 0)) {
                 case 7: EBU_K1 (3, true); break; case 6: EBU_K1 (3, false); break;
                 case 9: EBU_K1 (4, true); break; case 8: EBU_K1 (4, false); break;
@@ -1022,7 +1113,9 @@ int b200m_ebu_histogram (b200m_ebu* h, uint32_t inst, int32_t* hist_M, int32_t* 
 namespace {
 struct EbuSnapHead { uint32_t magic, n_inst, nchan; float fsamp; int32_t tmod, pad[3]; };
 constexpr uint32_t EBU_SNAP_MAGIC = 0x42453032u;              // "BE02": per-instance fragment phases
+constexpr uint32_t EBU_SNAP_MAGIC_W = 0x42573032u;            // "BW02": the same for a weighted bank, its EBU_MAXCH_W gains follow the header
 constexpr size_t EBU_SNAP_HOST_PER_INST = 8;
+size_t ebu_head_bytes (const b200m_ebu* h) { return sizeof (EbuSnapHead) + (h->weighted ? sizeof (h->gw.g) : 0); }
 struct EbuSeg { void* p; size_t bytes; };
 int ebu_segments (b200m_ebu* h, EbuSeg* seg)
 {
@@ -1040,7 +1133,7 @@ size_t b200m_ebu_snapshot_size (b200m_ebu* h)
 {
     if (!h) return 0;
     EbuSeg seg[9]; const int k = ebu_segments (h, seg);
-    size_t b = sizeof (EbuSnapHead) + EBU_SNAP_HOST_PER_INST * (size_t)h->n_inst;
+    size_t b = ebu_head_bytes (h) + EBU_SNAP_HOST_PER_INST * (size_t)h->n_inst;
     b = (b + 15) & ~size_t (15);
     for (int i = 0; i < k; ++i) b += (seg[i].bytes + 15) & ~size_t (15);
     return b;
@@ -1052,13 +1145,14 @@ int b200m_ebu_snapshot (b200m_ebu* h, void* buf, size_t bytes, void* stream)
     DeviceGuard g (h->device);
     cudaStream_t st = ebu_stream (h, stream);
     uint8_t* o = (uint8_t*)buf;
-    EbuSnapHead hd = {EBU_SNAP_MAGIC, h->n_inst, h->nchan, h->fsamp, h->tmod, {0, 0, 0}};
+    EbuSnapHead hd = {h->weighted ? EBU_SNAP_MAGIC_W : EBU_SNAP_MAGIC, h->n_inst, h->nchan, h->fsamp, h->tmod, {0, 0, 0}};
     memcpy (o, &hd, sizeof (hd)); o += sizeof (hd);
+    if (h->weighted) { memcpy (o, h->gw.g, sizeof (h->gw.g)); o += sizeof (h->gw.g); }
     const size_t n = h->n_inst;
     memcpy (o, h->ph.data (), 4 * n); o += 4 * n;
     memcpy (o, h->integ.data (), n); o += n; memcpy (o, h->base.data (), n); o += n; memcpy (o, h->frozen.data (), n); o += n;
     for (size_t i = 0; i < n; ++i) *o++ = (uint8_t)h->cls.find (h->ph[i])->second.G;
-    o = (uint8_t*)buf + ((sizeof (hd) + EBU_SNAP_HOST_PER_INST * n + 15) & ~size_t (15));
+    o = (uint8_t*)buf + ((ebu_head_bytes (h) + EBU_SNAP_HOST_PER_INST * n + 15) & ~size_t (15));
     EbuSeg seg[9]; const int k = ebu_segments (h, seg);
     for (int i = 0; i < k; ++i) { B200M_CUDA (cudaMemcpyAsync (o, seg[i].p, seg[i].bytes, cudaMemcpyDeviceToHost, st)); o += (seg[i].bytes + 15) & ~size_t (15); }
     B200M_CUDA (cudaStreamSynchronize (st));
@@ -1069,11 +1163,13 @@ int b200m_ebu_restore (b200m_ebu* h, const void* buf, size_t bytes, void* stream
 {
     if (!h || !buf || bytes < b200m_ebu_snapshot_size (h)) return set_err (B200M_E_INVAL, "bad argument / buffer too small");
     EbuSnapHead hd; memcpy (&hd, buf, sizeof (hd));
-    if (hd.magic != EBU_SNAP_MAGIC || hd.n_inst != h->n_inst || hd.nchan != h->nchan || hd.fsamp != h->fsamp)
-        return set_err (B200M_E_INVAL, "snapshot does not match this bank (instances / channels / sample rate)");
+    if (hd.magic != (h->weighted ? EBU_SNAP_MAGIC_W : EBU_SNAP_MAGIC) || hd.n_inst != h->n_inst || hd.nchan != h->nchan || hd.fsamp != h->fsamp)
+        return set_err (B200M_E_INVAL, "snapshot does not match this bank (weights / instances / channels / sample rate)");
+    if (h->weighted && memcmp ((const uint8_t*)buf + sizeof (hd), h->gw.g, sizeof (h->gw.g)) != 0)
+        return set_err (B200M_E_INVAL, "snapshot of a bank with other channel weights");
     DeviceGuard g (h->device);
     cudaStream_t st = ebu_stream (h, stream);
-    const uint8_t* o = (const uint8_t*)buf + sizeof (hd);
+    const uint8_t* o = (const uint8_t*)buf + ebu_head_bytes (h);
     const size_t n = h->n_inst;
     h->tmod = hd.tmod;
     memcpy (h->ph.data (), o, 4 * n); o += 4 * n;
@@ -1084,7 +1180,7 @@ int b200m_ebu_restore (b200m_ebu* h, const void* buf, size_t bytes, void* stream
         c.n++; c.G = o[i];
         if (h->integ[i]) c.cnt10[h->base[i]]++;
     }
-    o = (const uint8_t*)buf + ((sizeof (hd) + EBU_SNAP_HOST_PER_INST * n + 15) & ~size_t (15));
+    o = (const uint8_t*)buf + ((ebu_head_bytes (h) + EBU_SNAP_HOST_PER_INST * n + 15) & ~size_t (15));
     EbuSeg seg[9]; const int k = ebu_segments (h, seg);
     for (int i = 0; i < k; ++i) { B200M_CUDA (cudaMemcpyAsync (seg[i].p, o, seg[i].bytes, cudaMemcpyHostToDevice, st)); o += (seg[i].bytes + 15) & ~size_t (15); }
     B200M_CUDA (cudaStreamSynchronize (st));

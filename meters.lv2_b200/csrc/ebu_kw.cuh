@@ -27,6 +27,12 @@ constexpr int HIST_PITCH = 752;           // 751 bins padded to a 16-byte multip
 
 struct EbuCoef { float a0, a1, a2, b1, b2, c3, c4; };
 
+// A weighted bank's channel count and per-channel weights (b200m_ebu_create_weighted): kw_warp's run-time form (NCHAN = 0) reads
+// them in chunk_end, once per detect_process() call.  Kernels take it as a __grid_constant__ parameter: g[c] is then an indexed
+// parameter-space load, not a local copy.
+constexpr int EBU_MAXCH_W = 32;           // a K-weighting warp always holds at least one whole instance
+struct EbuGains { int nch; float g[EBU_MAXCH_W]; };
+
 // How K1 cuts a block into detect_process() calls.  fph == nullptr: the warp-uniform chunk list v[0..n) (bit31: the chunk ends a
 // 50 ms fragment), for a bank whose instances share one fragment phase.  fph != nullptr: every instance has its own phase
 // (fph[i]: the bank time mod fragm at which its clock last started; tmod: the bank time mod fragm at the launch's first frame)
@@ -47,8 +53,9 @@ struct EbuK1Args {
 
 // The EBUr128 cycle's dBTP hold (src/ebulv2.cc:227-230,360-367) as the true-peak kernels' epilogue sees it: nch channels per
 // instance, instance i on channels nch i .. nch i + nch - 1.  tpmax == nullptr: no EBUr128 epilogue.  lin == nullptr (nch = 1, 2, 4:
-// an instance never leaves an 8-channel true-peak group): the group folds its instances into tpmax[] itself.  Otherwise (nch = 3, 5:
-// instances straddle groups and host slices) every channel's read() goes to lin[channel] and r128_hold_kernel folds them.
+// an instance never leaves an 8-channel true-peak group): the group folds its instances into tpmax[] itself.  Otherwise (nch = 3, 5
+// and every weighted bank: instances straddle groups and host slices) every channel's read() goes to lin[channel] and
+// r128_hold_kernel folds them.
 struct R128Hold { float* tpmax; float* lin; int nch; };
 
 // coef_to_db (src/ebulv2.cc:227-230) of the larger read() t, then tp_max = max (tp_max, tp)
@@ -86,14 +93,17 @@ B200M_DEV uint32_t smem_u32 (const void* p) { return (uint32_t)__cvta_generic_to
 
 // The recurrence over one block for the 32 channels of a warp; `sg` supplies the tiles (a staging policy: PaddedStage and
 // TmaStage in ebu.cu, FusedStage in tpk.cu).  PHASES = false compiles the chunk-list policy alone (ck.fph is ignored).
+// NCHAN = 0: a weighted bank, gw->nch channels per instance with the weights gw->g (the instance's lanes are lane - lane % nch ..
+// + nch - 1); gw is read only in that form.
 template <int NCHAN, bool PHASES, class Stage>
 B200M_DEV void kw_warp (Stage& sg, int lane, int k, bool live, int nchans, int nfram, const EbuCoef& cf, const EbuChunks& ck, float fragm_f,
-                        float* __restrict__ zst, float* __restrict__ frpwr, float* __restrict__ fragpw, int n_inst)
+                        float* __restrict__ zst, float* __restrict__ frpwr, float* __restrict__ fragpw, int n_inst, const EbuGains* gw = nullptr)
 {
     const int ntiles = (nfram + EBU_TILE - 1) / EBU_TILE;
     float z1 = zst[0 * (size_t)nchans + k], z2 = zst[1 * (size_t)nchans + k];
     float z3 = zst[2 * (size_t)nchans + k], z4 = zst[3 * (size_t)nchans + k];
-    const int inst = k / NCHAN;
+    const int nch = NCHAN ? NCHAN : gw->nch;
+    const int inst = k / nch;
     float fp = frpwr[inst];
     float sj = 0.0f;
     int ci = 0, nfr = 0;
@@ -112,11 +122,18 @@ B200M_DEV void kw_warp (Stage& sg, int lane, int k, bool live, int nchans, int n
         bool cut = true;
         if (PHASES && ck.fph) { cfrag = mynext == cend; cut = cfrag || cend == nfram; }
         float si;
-        if (NCHAN == 1) si = __fmul_rn (2.0f, sj);
+        if constexpr (NCHAN == 0) {
+            // si = g0 sj0, then si += g_c sj_c in channel order (:328-330 with the caller's weights; 0 + g0 sj0 is g0 sj0 exactly).
+            // nch is warp-uniform: every lane runs every shuffle
+            const int lead = lane - lane % nch;
+            si = __fmul_rn (gw->g[0], __shfl_sync (0xffffffffu, sj, lead));
+            for (int c = 1; c < nch; ++c) si = __fadd_rn (si, __fmul_rn (gw->g[c], __shfl_sync (0xffffffffu, sj, (lead + c) & 31)));
+        }
+        else if (NCHAN == 1) si = __fmul_rn (2.0f, sj);
         else if (NCHAN == 2) si = __fadd_rn (sj, __shfl_xor_sync (0xffffffffu, sj, 1));   // 1.0f*sjL + 1.0f*sjR
         else {
             // si = sum_i _chan_gain[i] * sj_i in channel order, gains 1 1 1 1.41 1.41 (:29,328-329); the instance's lanes are contiguous
-            const int lead = lane - lane % NCHAN;
+            const int lead = lane - lane % nch;
             si = __fmul_rn (1.0f, __shfl_sync (0xffffffffu, sj, lead));
 #pragma unroll
             for (int c = 1; c < NCHAN; ++c) si = __fadd_rn (si, __fmul_rn (c >= 3 ? 1.41f : 1.0f, __shfl_sync (0xffffffffu, sj, (lead + c) & 31)));
@@ -125,7 +142,7 @@ B200M_DEV void kw_warp (Stage& sg, int lane, int k, bool live, int nchans, int n
             z1 = scrub (z1); z2 = scrub (z2); z3 = scrub (z3); z4 = scrub (z4);
             fp = __fadd_rn (fp, si);
             if (cfrag) {
-                if (live && (k % NCHAN) == 0) fragpw[(size_t)nfr * n_inst + inst] = __fdiv_rn (fp, fragm_f);
+                if (live && (k % nch) == 0) fragpw[(size_t)nfr * n_inst + inst] = __fdiv_rn (fp, fragm_f);
                 fp = 1e-30f;
                 ++nfr;
                 mynext += ck.fragm;
@@ -183,7 +200,7 @@ B200M_DEV void kw_warp (Stage& sg, int lane, int k, bool live, int nchans, int n
     if (live) {
         zst[0 * (size_t)nchans + k] = z1; zst[1 * (size_t)nchans + k] = z2;
         zst[2 * (size_t)nchans + k] = z3; zst[3 * (size_t)nchans + k] = z4;
-        if ((k % NCHAN) == 0) frpwr[inst] = fp;
+        if ((k % nch) == 0) frpwr[inst] = fp;
     }
 }
 
@@ -192,6 +209,10 @@ B200M_DEV void kw_warp (Stage& sg, int lane, int k, bool live, int nchans, int n
 // host side, ebu.cu: a [rows x cols] float32 tensor map of the planar input with boxes of box_rows x box_cols floats, zeros outside
 // (128B swizzle or none); false when the driver offers no encoder or rejects the geometry
 bool ebu_tma_map (CUtensorMap* tm, const float* base, size_t stride, uint32_t rows, uint32_t cols, uint32_t box_cols, uint32_t box_rows, bool swizzle128);
+// host side, ebu.cu: are these the reference's weights for nchan = 1..5 (mono {2}, else 1 1 1 1.41 1.41), compared bitwise?  And the
+// validation of b200m_ebu_create_weighted's arguments (nchan 1..32, finite gains >= 0, one > 0): 0 or B200M_E_INVAL
+bool ebu_default_gains (uint32_t nchan, const float* gains);
+int ebu_check_gains (uint32_t nchan, const float* gains);
 // host side, ebu.cu: does the next `nfram` frames' chunk list fit ONE K1 launch (EBU_MAXCHUNK chunks)?
 extern "C" bool ebu_single_k1 (const b200m_ebu* h, uint32_t nfram);
 // host side, ebu.cu: one Ebu_r128_proc::process call of every instance, launched per instance slice (see the definition)

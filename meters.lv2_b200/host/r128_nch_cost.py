@@ -4,8 +4,13 @@ in exact mode (K-weighting + tpmax_kernel, and for 3 and 5 channels r128_hold_ke
 warm-up blocks; --runs runs, the libraries given with --lib alternated (order reversed on every other run).  A library without
 b200m_r128_create_nch is timed at 2 channels only.  The GPU's name and power limit are read at the start and printed with the
 results (one JSON line).
+Weighted layouts (b200m_r128_create_weighted, --weighted, default 7, 11, 22 and 32 channels per instance) are timed in the same
+session, in both modes, as floor (channels / nchan) instances with BS.1770-4-style weights (1.41 on two of every eight channels):
+these banks run the run-time channel-count K-weighting kernel and, in tolerance mode, the tensor-core FIR behind it (they have no
+fused form).  A library without b200m_r128_create_weighted skips them.
 
     python meters.lv2_b200/host/r128_nch_cost.py [--lib meters.lv2_b200/libb200meters.so ...] [--channels 16380] [--nframes 1024]
+                                                 [--weighted 7,11,22,32]
 """
 import argparse
 import ctypes as C
@@ -26,6 +31,8 @@ def _load(path):
     L.b200m_r128_create.argtypes = [C.POINTER(_v), C.c_int, C.c_uint32, C.c_float, C.c_int]
     if hasattr(L, "b200m_r128_create_nch"):
         L.b200m_r128_create_nch.argtypes = [C.POINTER(_v), C.c_int, C.c_uint32, C.c_uint32, C.c_float, C.c_int]
+    if hasattr(L, "b200m_r128_create_weighted"):
+        L.b200m_r128_create_weighted.argtypes = [C.POINTER(_v), C.c_int, C.c_uint32, C.c_uint32, _v, C.c_float, C.c_int]
     L.b200m_r128_run_device.argtypes = [_v, _v, C.c_size_t, C.c_uint32, _v]
     L.b200m_r128_control.argtypes = [_v, C.c_int32, C.c_int, _v]
     L.b200m_r128_set_precision.argtypes = [_v, C.c_int]
@@ -33,12 +40,17 @@ def _load(path):
     return L
 
 
-def _time(L, x, nchan, nframes, mode, iters):
-    """us per block, or None when the library has no b200m_r128_create_nch and nchan != 2"""
+def _time(L, x, nchan, nframes, mode, iters, weighted=False):
+    """us per block, or None when the library has no b200m_r128_create_nch and nchan != 2 (weighted: no b200m_r128_create_weighted)"""
     st = _v(torch.cuda.current_stream().cuda_stream)
     h = _v()
     n_inst = x.shape[0] // nchan
-    if hasattr(L, "b200m_r128_create_nch"):
+    if weighted:
+        if not hasattr(L, "b200m_r128_create_weighted"):
+            return None
+        g = (C.c_float * nchan)(*[1.41 if c % 8 in (3, 4) else 1.0 for c in range(nchan)])
+        assert L.b200m_r128_create_weighted(C.byref(h), 0, n_inst, nchan, C.cast(g, _v), 48000.0, 1) == 0
+    elif hasattr(L, "b200m_r128_create_nch"):
         assert L.b200m_r128_create_nch(C.byref(h), 0, n_inst, nchan, 48000.0, 1) == 0
     elif nchan == 2:
         assert L.b200m_r128_create(C.byref(h), 0, n_inst, 48000.0, 1) == 0
@@ -67,6 +79,7 @@ def main():
     ap.add_argument("--channels", type=int, default=16380)
     ap.add_argument("--nframes", type=int, default=1024)
     ap.add_argument("--iters", type=int, default=300)
+    ap.add_argument("--weighted", default="7,11,22,32", help="channels per instance of the weighted layouts ('' for none)")
     a = ap.parse_args()
     libs = {p: _load(p) for p in (a.lib or [os.path.join(HERE, "..", "libb200meters.so")])}
     gpu = subprocess.run(["nvidia-smi", "--query-gpu=name,power.limit", "--format=csv,noheader"], capture_output=True, text=True).stdout.strip()
@@ -82,6 +95,10 @@ def main():
                     t = _time(L, x, nchan, a.nframes, mode, a.iters)
                     if t is not None:
                         res.setdefault(f"{p} {mode} nchan={nchan}", []).append(round(t, 2))
+                for nchan in [int(v) for v in a.weighted.split(",") if v]:
+                    t = _time(L, x, nchan, a.nframes, mode, a.iters, weighted=True)
+                    if t is not None:
+                        res.setdefault(f"{p} {mode} weighted nchan={nchan} x {a.channels // nchan}", []).append(round(t, 2))
     print(json.dumps({"gpu": gpu, "channels": a.channels, "nframes": a.nframes, "us_per_block": res}))
 
 
