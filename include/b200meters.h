@@ -120,6 +120,14 @@ int b200m_ebu_integr_reset (b200m_ebu* h, int32_t inst, void* stream);
 /* Ebu_r128_proc::process(nfram, input[]) (:207-248) for every instance. 0 < nfram <= 8192. */
 int b200m_ebu_process_device (b200m_ebu* h, const float* d_in, size_t stride, uint32_t nfram, void* stream);
 int b200m_ebu_process_host (b200m_ebu* h, const float* in, size_t stride, uint32_t nfram);
+/* Ragged blocks: Ebu_r128_proc::process (len[i], rows of i) for every instance i, over the first len[i] <= nfram frames of its
+ * rows; len[i] == 0: process is not called for i at all.  len: host array of n_inst; NULL (or every len[i] == nfram) is exactly
+ * b200m_ebu_process_*.  Instance i ends up bit-identical to a private Ebu_r128_proc fed only its own len[i] > 0 blocks, in order:
+ * its 50 ms fragment clock advances by len[i], not nfram.  Frames at or after len[i] never reach a result (they may hold anything,
+ * NaN included).  A len[i] > nfram is B200M_E_INVAL and enqueues nothing.  Controls, snapshots and the whole-mix reduce keep
+ * their meaning.  Loudness of many clips of different lengths: feed each clip's frames and a 0 length once it has ended. */
+int b200m_ebu_process_ragged_device (b200m_ebu* h, const float* d_in, size_t stride, uint32_t nfram, const uint32_t* len, void* stream);
+int b200m_ebu_process_ragged_host (b200m_ebu* h, const float* in, size_t stride, uint32_t nfram, const uint32_t* len);
 /* getters -> host array of n_inst results.  stream = the stream last used for processing
  * (ignored after process_host, which uses the bank's stream). */
 int b200m_ebu_results (b200m_ebu* h, b200m_ebu_result* out, void* stream);
@@ -232,6 +240,14 @@ int b200m_r128_destroy (b200m_r128* h);
 int b200m_r128_control (b200m_r128* h, int32_t inst, int cmd, void* stream);      /* inst = -1: all */
 int b200m_r128_run_device (b200m_r128* h, const float* d_in, size_t stride, uint32_t nfram, void* stream);
 int b200m_r128_run_host (b200m_r128* h, const float* in, size_t stride, uint32_t nfram);
+/* Ragged blocks: the EBUr128 cycle of instance i over its first len[i] <= nfram frames -- Ebu process (len[i]), process_max
+ * (len[i]) on each of its channels, the reads and the tp_max hold; len[i] == 0: the plugin did not run this cycle (no process,
+ * no read, hold unchanged).  len: host array of n_inst; NULL (or every len[i] == nfram) is exactly b200m_r128_run_* (same kernels,
+ * launches and bits).  Parity, unread frames and B200M_E_INVAL as for b200m_ebu_process_ragged_*; a dBTP-disabled instance stays
+ * frozen whatever its length.  A ragged block runs the chunk-parallel true-peak FIR in either precision mode, never the
+ * tensor-core or fused kernels. */
+int b200m_r128_run_ragged_device (b200m_r128* h, const float* d_in, size_t stride, uint32_t nfram, const uint32_t* len, void* stream);
+int b200m_r128_run_ragged_host (b200m_r128* h, const float* in, size_t stride, uint32_t nfram, const uint32_t* len);
 /* ebu_out: n_inst getter blocks (may be NULL); tp_max_db: n_inst floats, -inf when dBTP is disabled (may be NULL) */
 int b200m_r128_results (b200m_r128* h, b200m_ebu_result* ebu_out, float* tp_max_db, void* stream);
 /* self->dbtp_enable (CTL_UISETTINGS bit 64, src/ebulv2.cc:316-317): the true-peak meters only run while enabled; while

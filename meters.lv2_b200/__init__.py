@@ -58,6 +58,8 @@ _PROTOS = {
     "b200m_ebu_integr_reset": (C.c_int, [_v, C.c_int32, _v]),
     "b200m_ebu_process_device": (C.c_int, [_v, _v, C.c_size_t, C.c_uint32, _v]),
     "b200m_ebu_process_host": (C.c_int, [_v, _v, C.c_size_t, C.c_uint32]),
+    "b200m_ebu_process_ragged_device": (C.c_int, [_v, _v, C.c_size_t, C.c_uint32, _v, _v]),
+    "b200m_ebu_process_ragged_host": (C.c_int, [_v, _v, C.c_size_t, C.c_uint32, _v]),
     "b200m_ebu_results": (C.c_int, [_v, _v, _v]),
     "b200m_ebu_histogram": (C.c_int, [_v, C.c_uint32, _v, _v, _v]),
     "b200m_ebu_coeffs": (C.c_int, [_v, _v]),
@@ -96,6 +98,8 @@ _PROTOS = {
     "b200m_r128_control": (C.c_int, [_v, C.c_int32, C.c_int, _v]),
     "b200m_r128_run_device": (C.c_int, [_v, _v, C.c_size_t, C.c_uint32, _v]),
     "b200m_r128_run_host": (C.c_int, [_v, _v, C.c_size_t, C.c_uint32]),
+    "b200m_r128_run_ragged_device": (C.c_int, [_v, _v, C.c_size_t, C.c_uint32, _v, _v]),
+    "b200m_r128_run_ragged_host": (C.c_int, [_v, _v, C.c_size_t, C.c_uint32, _v]),
     "b200m_r128_results": (C.c_int, [_v, _v, _v, _v]),
     "b200m_r128_set_dbtp": (C.c_int, [_v, C.c_int]),
     "b200m_r128_set_dbtp_inst": (C.c_int, [_v, C.c_int32, C.c_int]),
@@ -294,6 +298,16 @@ def _gains(gains, nchan):
     return g
 
 
+def _lengths(lengths, n_inst):
+    """per-instance frame counts as a uint32 array of n_inst entries (the C side checks them against nfram)"""
+    a = np.asarray(lengths).ravel()
+    if a.size != n_inst:
+        raise B200MError("%d lengths for %d instances" % (a.size, n_inst))
+    if a.size and (a.min() < 0 or a.max() > 0xffffffff):
+        raise B200MError("lengths must be frame counts >= 0")
+    return np.ascontiguousarray(a, np.uint32)
+
+
 def host_alloc(rows, cols):
     """[rows, cols] float32 numpy array in pinned host memory from b200m_host_alloc (placed on the GPU-local NUMA node);
     freed with b200m_host_free when the array is garbage-collected."""
@@ -368,16 +382,26 @@ class Ebu_r128_proc(_Bank):
     def integr_reset(self, inst=-1, stream=None):
         _ck(lib().b200m_ebu_integr_reset(self.h, inst, _stream_ptr(stream)))
 
-    def process(self, x, stream=None):
-        """x: [n_inst*nchan, nfram] float32 CUDA tensor (device path) or numpy/pinned CPU (host path)."""
+    def process(self, x, stream=None, lengths=None):
+        """x: [n_inst*nchan, nfram] float32 CUDA tensor (device path) or numpy/pinned CPU (host path).
+        lengths: None, or n_inst frame counts <= nfram: instance i processes only the first lengths[i] frames of its rows (0: it is
+        not called at all), as a private Ebu_r128_proc fed just those frames (b200m_ebu_process_ragged_*)."""
         if isinstance(x, np.ndarray) or not x.is_cuda:
             p, s, rows, n = _host_planar(x)
             assert rows == self.n_inst * self.nchan
-            _ck(lib().b200m_ebu_process_host(self.h, p, s, n))
+            if lengths is None:
+                _ck(lib().b200m_ebu_process_host(self.h, p, s, n))
+            else:
+                ln = _lengths(lengths, self.n_inst)
+                _ck(lib().b200m_ebu_process_ragged_host(self.h, p, s, n, _np_ptr(ln)))
         else:
             p, s, rows, n = _dev_ptr(x)
             assert rows == self.n_inst * self.nchan
-            _ck(lib().b200m_ebu_process_device(self.h, p, s, n, _stream_ptr(stream)))
+            if lengths is None:
+                _ck(lib().b200m_ebu_process_device(self.h, p, s, n, _stream_ptr(stream)))
+            else:
+                ln = _lengths(lengths, self.n_inst)
+                _ck(lib().b200m_ebu_process_ragged_device(self.h, p, s, n, _np_ptr(ln), _stream_ptr(stream)))
 
     def process_ptr(self, ptr, stride, nfram, stream=None):
         _ck(lib().b200m_ebu_process_device(self.h, C.c_void_p(ptr), stride, nfram, _stream_ptr(stream)))
@@ -844,15 +868,26 @@ class EBUr128(_Bank):
     def control(self, cmd, inst=-1, stream=None):
         _ck(lib().b200m_r128_control(self.h, inst, cmd, _stream_ptr(stream)))
 
-    def run(self, x, stream=None):
+    def run(self, x, stream=None, lengths=None):
+        """one cycle of every instance over x [n_inst*nchan, nfram] (CUDA tensor: device path; numpy / CPU tensor: host path).
+        lengths: None, or n_inst frame counts <= nfram: instance i runs its cycle over its first lengths[i] frames only (0: the
+        plugin did not run this cycle: no process, no read, hold unchanged), b200m_r128_run_ragged_*."""
         if isinstance(x, np.ndarray) or not x.is_cuda:
             p, s, rows, n = _host_planar(x)
             assert rows == self.nchan * self.n_inst
-            _ck(lib().b200m_r128_run_host(self.h, p, s, n))
+            if lengths is None:
+                _ck(lib().b200m_r128_run_host(self.h, p, s, n))
+            else:
+                ln = _lengths(lengths, self.n_inst)
+                _ck(lib().b200m_r128_run_ragged_host(self.h, p, s, n, _np_ptr(ln)))
         else:
             p, s, rows, n = _dev_ptr(x)
             assert rows == self.nchan * self.n_inst
-            _ck(lib().b200m_r128_run_device(self.h, p, s, n, _stream_ptr(stream)))
+            if lengths is None:
+                _ck(lib().b200m_r128_run_device(self.h, p, s, n, _stream_ptr(stream)))
+            else:
+                ln = _lengths(lengths, self.n_inst)
+                _ck(lib().b200m_r128_run_ragged_device(self.h, p, s, n, _np_ptr(ln), _stream_ptr(stream)))
 
     def run_ptr(self, ptr, stride, nfram, stream=None, host=False):
         if host:
@@ -890,3 +925,47 @@ class EBUr128(_Bank):
         m = np.empty(751, np.int32); s = np.empty(751, np.int32)
         _ck(lib().b200m_r128_histogram(self.h, int(inst), _np_ptr(m), _np_ptr(s), _stream_ptr(stream)))
         return m, s
+
+
+PROGRAMME_FIELDS = ("integrated", "integ_thr", "range_min", "range_max", "maxloudn_M", "maxloudn_S")
+
+
+def programme_loudness(x, lengths, fsamp=48000.0, nchan=2, gains=None, block=1024, dbtp=True, precision=PREC_EXACT, device=0):
+    """Whole-programme EBU R128 loudness and true peak of N clips of different lengths, in one bank.
+
+    x: rows i * nchan + c of clip i (nchan channels, or len(gains) with per-channel weights as in EBUr128), clip i valid for its
+    first lengths[i] frames: a [N * nchan, >= max(lengths)] float32 numpy array / CPU tensor (host path) or CUDA tensor (device
+    path), or a callable f(offset, nfram) that returns frames offset .. offset + nfram - 1 of every row as such an array (clips
+    produced block by block).  Frames past a clip's length are never read into a result.
+    Integration starts before the first frame.  The clips are fed in blocks of `block` frames: block k has
+    nfram = min(block, longest remaining) and clip i's length in it is clamp(lengths[i] - k * block, 0, block) (EBUr128.run with
+    lengths).  Clip i's numbers are therefore bit-identical (exact mode) to a private Ebu_r128_proc + TruePeakdsp instance fed the
+    clip in blocks of `block` frames with a short last block -- the reference's results depend on where blocks are cut
+    (ebu_r128_proc.cc:212-216).  No padding is metered: a short clip's loudness, maxima, histograms and range stop at its end.
+    Returns a dict of float32 arrays of N: integrated, integ_thr, range_min, range_max, maxloudn_M, maxloudn_S (LUFS / LU, -200
+    where the reference reports nothing) and tp_max (dBTP, -inf when dbtp is False or the clip is empty)."""
+    ln = np.asarray(lengths, np.int64).ravel()
+    n = ln.size
+    if n == 0:
+        raise B200MError("no clips")
+    if ln.min() < 0:
+        raise B200MError("lengths must be frame counts >= 0")
+    if not 1 <= int(block) <= 8192:
+        raise B200MError("block must be 1..8192 frames")
+    if gains is not None:
+        nchan = np.asarray(gains).size
+    bank = EBUr128(n, fsamp, dbtp, device, nchan=nchan, gains=gains)
+    try:
+        bank.set_precision(precision)
+        bank.control(EBUr128.START)
+        total = int(ln.max())
+        for off in range(0, total, int(block)):
+            nfram = min(int(block), total - off)
+            xb = x(off, nfram) if callable(x) else x[:, off:off + nfram]
+            bank.run(xb, lengths=np.clip(ln - off, 0, nfram))
+        r, tp = bank.results()
+    finally:
+        bank.close()
+    out = {k: np.ascontiguousarray(r[k], np.float32) for k in PROGRAMME_FIELDS}
+    out["tp_max"] = tp
+    return out

@@ -160,11 +160,13 @@ struct TmaStage {
     }
 };
 
-// PHASES: the bank's instances have several fragment phases (ck.fph); without it the chunk-list policy is compiled alone
-template <int NCHAN, bool ALIGNED, bool PHASES>
+// PHASES: the bank's instances have several fragment phases (ck.fph); without it the chunk-list policy is compiled alone.
+// RAG (with PHASES): a ragged block, instance i's rows are read for their first rlen[i] frames only (kw_warp); rlen is not read otherwise
+template <int NCHAN, bool ALIGNED, bool PHASES, bool RAG = false>
 __global__ void __launch_bounds__ (EBU_WARPS * 32)
 ebu_kweight_frag (const float* __restrict__ in, size_t stride, int nchans, int k_first, int k_end, int nfram, EbuCoef cf, EbuChunks ck,
-                  float fragm_f, float* __restrict__ zst, float* __restrict__ frpwr, float* __restrict__ fragpw, int n_inst, int pdl_trigger)
+                  float fragm_f, float* __restrict__ zst, float* __restrict__ frpwr, float* __restrict__ fragpw, int n_inst, int pdl_trigger,
+                  const uint32_t* __restrict__ rlen)
 {
     // channels [k_first, k_end) of the bank's nchans (a slice: *_run_host overlaps the copy of slice s+1 with slice s)
     extern __shared__ __align__ (16) float ebu_smem[];
@@ -177,17 +179,17 @@ ebu_kweight_frag (const float* __restrict__ in, size_t stride, int nchans, int k
     if (k0 >= k_end) return;                           // warp-uniform; warps never synchronise with each other
     PaddedStage<ALIGNED> sg;
     sg.init (in, stride, ebu_smem + warp * EBU_WARP_FLOATS, lane, k0, k_end, nfram);
-    kw_warp<NCHAN, PHASES> (sg, lane, min (k0 + lane, k_end - 1) /* tail lanes shadow the last channel (no stores) */, lane < CPW && (k0 + lane) < k_end,
-                            nchans, nfram, cf, ck, fragm_f, zst, frpwr, fragpw, n_inst);
+    kw_warp<NCHAN, PHASES, PaddedStage<ALIGNED>, RAG> (sg, lane, min (k0 + lane, k_end - 1) /* tail lanes shadow the last channel (no stores) */,
+                                                      lane < CPW && (k0 + lane) < k_end, nchans, nfram, cf, ck, fragm_f, zst, frpwr, fragpw, n_inst, nullptr, rlen);
 }
 
 // the same kernel for a weighted bank (b200m_ebu_create_weighted): gw.nch = 1..32 channels per instance, known at run time, a warp
 // takes CPW = (32 / nch) nch channels (whole instances), and the channel sum uses the bank's weights gw.g
-template <bool ALIGNED, bool PHASES>
+template <bool ALIGNED, bool PHASES, bool RAG = false>
 __global__ void __launch_bounds__ (EBU_WARPS * 32)
 ebu_kweight_frag_w (const float* __restrict__ in, size_t stride, int nchans, int k_first, int k_end, int nfram, EbuCoef cf, EbuChunks ck,
                     float fragm_f, float* __restrict__ zst, float* __restrict__ frpwr, float* __restrict__ fragpw, int n_inst, int pdl_trigger,
-                    const __grid_constant__ EbuGains gw)
+                    const __grid_constant__ EbuGains gw, const uint32_t* __restrict__ rlen)
 {
     extern __shared__ __align__ (16) float ebu_smem[];
     if (pdl_trigger) asm volatile ("griddepcontrol.launch_dependents;");
@@ -197,8 +199,8 @@ ebu_kweight_frag_w (const float* __restrict__ in, size_t stride, int nchans, int
     if (k0 >= k_end) return;
     PaddedStage<ALIGNED> sg;
     sg.init (in, stride, ebu_smem + warp * EBU_WARP_FLOATS, lane, k0, k_end, nfram);
-    kw_warp<0, PHASES> (sg, lane, min (k0 + lane, k_end - 1), lane < cpw && (k0 + lane) < k_end,
-                        nchans, nfram, cf, ck, fragm_f, zst, frpwr, fragpw, n_inst, &gw);
+    kw_warp<0, PHASES, PaddedStage<ALIGNED>, RAG> (sg, lane, min (k0 + lane, k_end - 1), lane < cpw && (k0 + lane) < k_end,
+                                                  nchans, nfram, cf, ck, fragm_f, zst, frpwr, fragpw, n_inst, &gw, rlen);
 }
 
 // ---- K1 split over two warps per 32 channels -------------------------------------------------------------------------------
@@ -475,13 +477,14 @@ B200M_DEV void hist_calc_range (const int* row, int count, const float* bp, int 
 // ring layout [64][n_inst] so that lane = instance accesses coalesce; each thread parks its 64-slot ring column
 // in shared memory (column private to the thread: no barrier needed) for the two ordered sums.
 // Launch `frag` handles row `frag` of fragpw: with one phase for the bank every instance's fragment `frag` of the K1 launch; with
-// per-instance phases (fph) each instance's fragment `frag` of the block, if the block of `nfram` frames from bank time tmod has one.
+// per-instance phases (fph) each instance's fragment `frag` of the block, if the block of `nfram` frames from bank time tmod has one
+// -- in a ragged block (rlen), if the instance's first rlen[i] frames have one.
 constexpr int K2A_THREADS = 128;
 
 __global__ void __launch_bounds__ (K2A_THREADS)
 ebu_fragment_kernel (int n_inst, int frag, const int* __restrict__ fph, int tmod, int fragm, int nfram, const float* __restrict__ fragpw,
                      float* __restrict__ ring, EbuCtl* __restrict__ ctl, b200m_ebu_result* __restrict__ res, int* __restrict__ histM,
-                     int* __restrict__ histS, int* __restrict__ cnt)
+                     int* __restrict__ histS, int* __restrict__ cnt, const uint32_t* __restrict__ rlen)
 {
     __shared__ float sring[64][K2A_THREADS];
     const int tid = threadIdx.x;
@@ -489,7 +492,7 @@ ebu_fragment_kernel (int n_inst, int frag, const int* __restrict__ fph, int tmod
     if (i >= n_inst) return;
     if (fph) {
         int el = (tmod - fph[i]) % fragm; if (el < 0) el += fragm;
-        if (fragm - el + frag * fragm > nfram) return;     // the instance's edge `frag` lies beyond this block
+        if (fragm - el + frag * fragm > (rlen ? (int)rlen[i] : nfram)) return;     // the instance's edge `frag` lies beyond its block
     }
     // all 64 ring slots in flight at once (one round of memory latency, not 64): cp.async straight into the column
 #pragma unroll
@@ -568,6 +571,15 @@ ebu_gate_kernel (int n_inst, EbuCtl* __restrict__ ctl, b200m_ebu_result* __restr
         res[inst].range_min = v0; res[inst].range_max = v1; res[inst].range_thr = rt;
         ctl[inst].calc = 0;
     }
+}
+
+// a ragged block moves every instance's clock on by its own length, not by the block's nfram: its phase (the bank time at which
+// the clock last started) advances by nfram - rlen[i].  Launched behind the block's fragment kernels, which read the old phase.
+__global__ void ebu_ragged_clock_kernel (int n_inst, const uint32_t* __restrict__ rlen, int nfram, int fragm, int* __restrict__ fph)
+{
+    const int i = blockIdx.x * blockDim.x + threadIdx.x;
+    if (i >= n_inst) return;
+    fph[i] = (fph[i] + (nfram - (int)rlen[i])) % fragm;
 }
 
 // reset / integration control, one thread per instance.  tph >= 0 (cmd 3 only): the instance's clock restarts at bank time tph --
@@ -663,8 +675,9 @@ static bool tma_input_map (CUtensorMap* tm, const float* base, size_t stride, ui
 }
 
 // The bank's sample clock T is kept on the host as tmod = T mod fragm.  Instance i's 50 ms fragment clock last started at bank
-// time fph[i] (mod fragm): a device value that only the control kernel writes, mirrored on the host in ph[i].  Its next edge
-// lies fragm - ((T - fph[i]) mod fragm) frames ahead.
+// time fph[i] (mod fragm): a device value mirrored on the host in ph[i], written by the control kernel (the clock restarts) and by
+// ebu_ragged_clock_kernel (a ragged block: the instance's clock ran rlen[i] frames, not nfram).  Its next edge lies
+// fragm - ((T - fph[i]) mod fragm) frames ahead.
 struct EbuPhase { int n = 0, G = 0; int cnt10[10] = {0}; };   // one phase class: members, fragment counter mod 10, S-period census
 
 struct b200m_ebu {
@@ -686,6 +699,12 @@ struct b200m_ebu {
     std::vector<uint8_t> integ, base, frozen; std::vector<int> ph;
     std::map<int, EbuPhase> cls;
     std::vector<int> nf;                 // per class: fragments it completes in the block being launched (scratch)
+    // a ragged block (b200m_ebu_process_ragged_*): its per-instance lengths on the device, pinned staging for their upload (two
+    // slots, each reused only after its previous copy ran), and the instances whose length differs from nfram (scratch: index,
+    // fragments in the block, S-period position div2)
+    uint32_t* d_len = nullptr; uint32_t* h_len[2] = {nullptr, nullptr}; cudaEvent_t ev_len[2] = {nullptr, nullptr}; int len_slot = 0;
+    struct Rag { uint32_t i; int nf, d2; };
+    std::vector<Rag> rg;
     void phase_reset () {
         integ.assign (n_inst, 0); base.assign (n_inst, 0); frozen.assign (n_inst, 0); ph.assign (n_inst, tmod);
         cls.clear (); cls[tmod].n = (int)n_inst;
@@ -714,6 +733,39 @@ struct b200m_ebu {
     }
     int frcnt_of (int p) const { int el = (tmod - p) % fragm; if (el < 0) el += fragm; return fragm - el; }
     static bool phase_tick (EbuPhase& c) { c.G = (c.G + 1) % 10; return c.cnt10[c.G] > 0; }   // one fragment of the class: does anyone wrap?
+    // A ragged block: instance i with len[i] != nfram completes another number of fragments than its class, so it leaves the class
+    // for the block and is ticked on its own, its S-period position kept as div2 = (G - base) mod 10 (integrating) or in frozen
+    // (paused).  O(classes + such instances) besides the scan of len.
+    void ragged_leave (const uint32_t* len, uint32_t nfram) {
+        rg.clear ();
+        for (uint32_t i = 0; i < n_inst; ++i) {
+            if (len[i] == nfram) continue;
+            auto it = cls.find (ph[i]);
+            EbuPhase& c = it->second;
+            int d2 = 0;
+            if (integ[i]) { d2 = (c.G - base[i] + 10) % 10; c.cnt10[base[i]]--; }
+            rg.push_back ({i, frags_in (ph[i], len[i]), d2});
+            if (--c.n == 0) cls.erase (it);
+        }
+    }
+    // ... one fragment f of the block for the instances that left: does an integrating one wrap its S period?
+    bool ragged_tick (int f) {
+        bool wrap = false;
+        for (auto& r : rg)
+            if (f < r.nf && integ[r.i]) { r.d2 = (r.d2 + 1) % 10; wrap |= r.d2 == 0; }
+        return wrap;
+    }
+    // ... and after it each joins the class of its new phase ph + nfram - len (ebu_ragged_clock_kernel), keeping its S-period position
+    void ragged_join (const uint32_t* len, uint32_t nfram) {
+        for (const auto& r : rg) {
+            const uint32_t i = r.i;
+            ph[i] = (int)(((uint32_t)ph[i] + (nfram - len[i])) % (uint32_t)fragm);
+            EbuPhase& c = cls[ph[i]];
+            c.n++;
+            if (integ[i]) { base[i] = (uint8_t)((c.G - r.d2 + 10) % 10); c.cnt10[base[i]]++; }
+        }
+        rg.clear ();
+    }
 };
 
 // Host-side coefficient design; restates Ebu_r128_proc::detect_init (ebu_r128_proc.cc:263-293).
@@ -820,6 +872,11 @@ static int ebu_create (b200m_ebu** out, int device, uint32_t n_inst, uint32_t nc
     A ((void**)&h->d_histS, (size_t)HIST_PITCH * n_inst * sizeof (int));
     A ((void**)&h->d_cnt, (size_t)4 * n_inst * sizeof (int));
     A ((void**)&h->d_fph, n_inst * sizeof (int));
+    A ((void**)&h->d_len, n_inst * sizeof (uint32_t));
+    for (int s = 0; s < 2; ++s) {
+        if (e == cudaSuccess) e = cudaHostAlloc ((void**)&h->h_len[s], n_inst * sizeof (uint32_t), cudaHostAllocDefault);
+        if (e == cudaSuccess) e = cudaEventCreateWithFlags (&h->ev_len[s], cudaEventDisableTiming);
+    }
     if (e == cudaSuccess) e = cudaMemcpy (h->d_binpow, bp, sizeof (bp), cudaMemcpyHostToDevice);
     if (e == cudaSuccess) e = cudaStreamCreateWithFlags (&h->own, cudaStreamNonBlocking);
     // K1 carries 102 KB of dynamic shared memory per CTA
@@ -827,13 +884,17 @@ static int ebu_create (b200m_ebu** out, int device, uint32_t n_inst, uint32_t nc
     // needs (132 KB), which leaves room for ONE CTA of the true-peak kernel that is meant to share the SM with it (r128.cu)
 #define EBU_ATTR1(NC, AL, PH) if (e == cudaSuccess) e = cudaFuncSetAttribute (ebu_kweight_frag<NC, AL, PH>, cudaFuncAttributeMaxDynamicSharedMemorySize, EBU_SMEM_BYTES); \
     if (e == cudaSuccess) e = cudaFuncSetAttribute (ebu_kweight_frag<NC, AL, PH>, cudaFuncAttributePreferredSharedMemoryCarveout, cudaSharedmemCarveoutMaxShared)
-#define EBU_ATTR(NC, AL) EBU_ATTR1 (NC, AL, false); EBU_ATTR1 (NC, AL, true)
+#define EBU_ATTR2(NC, AL) if (e == cudaSuccess) e = cudaFuncSetAttribute (ebu_kweight_frag<NC, AL, true, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, EBU_SMEM_BYTES); \
+    if (e == cudaSuccess) e = cudaFuncSetAttribute (ebu_kweight_frag<NC, AL, true, true>, cudaFuncAttributePreferredSharedMemoryCarveout, cudaSharedmemCarveoutMaxShared)
+#define EBU_ATTR(NC, AL) EBU_ATTR1 (NC, AL, false); EBU_ATTR1 (NC, AL, true); EBU_ATTR2 (NC, AL)
     EBU_ATTR (1, true); EBU_ATTR (1, false); EBU_ATTR (2, true); EBU_ATTR (2, false);
     EBU_ATTR (3, true); EBU_ATTR (3, false); EBU_ATTR (4, true); EBU_ATTR (4, false); EBU_ATTR (5, true); EBU_ATTR (5, false);
 #undef EBU_ATTR
 #undef EBU_ATTR1
+#undef EBU_ATTR2
     if (gains)
-        for (const auto k : {ebu_kweight_frag_w<true, false>, ebu_kweight_frag_w<true, true>, ebu_kweight_frag_w<false, false>, ebu_kweight_frag_w<false, true>}) {
+        for (const auto k : {ebu_kweight_frag_w<true, false>, ebu_kweight_frag_w<true, true>, ebu_kweight_frag_w<false, false>, ebu_kweight_frag_w<false, true>,
+                             ebu_kweight_frag_w<true, true, true>, ebu_kweight_frag_w<false, true, true>}) {
             if (e == cudaSuccess) e = cudaFuncSetAttribute (k, cudaFuncAttributeMaxDynamicSharedMemorySize, EBU_SMEM_BYTES);
             if (e == cudaSuccess) e = cudaFuncSetAttribute (k, cudaFuncAttributePreferredSharedMemoryCarveout, cudaSharedmemCarveoutMaxShared);
         }
@@ -902,6 +963,8 @@ int b200m_ebu_destroy (b200m_ebu* h)
     cudaDeviceSynchronize ();
     cudaFree (h->d_z); cudaFree (h->d_frpwr); cudaFree (h->d_fragpw); cudaFree (h->d_ring); cudaFree (h->d_binpow);
     cudaFree (h->d_out5); cudaFree (h->d_ctl); cudaFree (h->d_res); cudaFree (h->d_histM); cudaFree (h->d_histS); cudaFree (h->d_cnt); cudaFree (h->d_fph);
+    cudaFree (h->d_len);
+    for (int s = 0; s < 2; ++s) { if (h->h_len[s]) cudaFreeHost (h->h_len[s]); if (h->ev_len[s]) cudaEventDestroy (h->ev_len[s]); }
     h->stage.release ();
     if (h->own) cudaStreamDestroy (h->own);
     delete h;
@@ -961,15 +1024,18 @@ bool ebu_single_k1 (const b200m_ebu* h, uint32_t nfram)
 // fragment/gating kernels run once, after the last slice.
 // `k1_fused`, when given (one slice, a block whose chunk list fits one launch: ebu_single_k1), launches a kernel that does
 // K1's work over the whole bank in its place; `after_k1` is enqueued right behind the first K1 launch.
+// `len` (host) / `d_len` (its copy on the device, ebu_upload_len): a ragged block, instance i processes its first len[i] frames (some
+// len[i] differs from nfram: ebu_ragged_check); nullptr: every instance processes nfram.
 int ebu_process_sliced (b200m_ebu* h, const float* d_in, size_t stride, uint32_t nfram, cudaStream_t st,
                         int nsl, const uint32_t* bounds, cudaEvent_t* ready, int (*after_k1) (void*), void* after_arg,
-                        int (*k1_fused) (void*, const EbuK1Args&))
+                        int (*k1_fused) (void*, const EbuK1Args&), const uint32_t* len, const uint32_t* d_len)
 {
     const int nch = (int)(h->n_inst * h->nchan);
     const bool aligned = ((uintptr_t)d_in % 16 == 0) && (stride % 4 == 0);
-    // one phase class: the warp-uniform chunk list, split over launches of at most EBU_MAXCHUNK chunks; several: one launch per
-    // block, every lane cutting at its own instance's fragment edges
-    const bool multi = h->cls.size () > 1;
+    // one phase class: the warp-uniform chunk list, split over launches of at most EBU_MAXCHUNK chunks; several, or a ragged block:
+    // one launch per block, every lane cutting at its own instance's fragment edges (and its own end)
+    if (d_len) h->ragged_leave (len, nfram);
+    const bool multi = d_len || h->cls.size () > 1;
     int frcnt = multi ? 0 : h->frcnt_of (h->cls.begin ()->first);
     uint32_t done = 0;
     while (done < nfram) {
@@ -980,10 +1046,11 @@ int ebu_process_sliced (b200m_ebu* h, const float* d_in, size_t stride, uint32_t
             ck.n = 0; ck.v[0] = 0; ck.fph = h->d_fph;
             h->nf.clear ();
             for (const auto& c : h->cls) { h->nf.push_back (h->frags_in (c.first, nfram)); nfrag = std::max (nfrag, h->nf.back ()); }
+            for (const auto& r : h->rg) nfrag = std::max (nfrag, r.nf);
         }
         else pos = ebu_plan_chunks (frcnt, h->fragm, nfram - done, ck, nfrag);
         const float* src = d_in + done;
-        const bool fused = k1_fused && done == 0 && pos == nfram && nsl == 1 && bounds[0] == 0 && bounds[1] == h->n_inst;
+        const bool fused = k1_fused && !d_len && done == 0 && pos == nfram && nsl == 1 && bounds[0] == 0 && bounds[1] == h->n_inst;
         if (fused) {
             const EbuK1Args a = {src, stride, nch, (int)pos, h->cf, ck, (float)h->fragm, h->d_z, h->d_frpwr, h->d_fragpw, (int)h->n_inst};
             if (int rc = k1_fused (after_arg, a)) return rc;
@@ -998,14 +1065,14 @@ int ebu_process_sliced (b200m_ebu* h, const float* d_in, size_t stride, uint32_t
             const int cpw = (32 / (int)h->nchan) * (int)h->nchan;          // a warp takes whole instances only
             const int nwarps = (ke - kf + cpw - 1) / cpw;
             dim3 grid ((nwarps + EBU_WARPS - 1) / EBU_WARPS), blk (EBU_WARPS * 32);
-#define EBU_K1P(NC, AL, PH) ebu_kweight_frag<NC, AL, PH><<<grid, blk, EBU_SMEM_BYTES, st>>> (src, stride, nch, kf, ke, (int)pos, h->cf, ck, (float)h->fragm, h->d_z, h->d_frpwr, h->d_fragpw, (int)h->n_inst, (after_k1 && done == 0) ? 1 : 0)
-#define EBU_K1(NC, AL) do { if (multi) EBU_K1P (NC, AL, true); else EBU_K1P (NC, AL, false); } while (0)
+#define EBU_K1P(NC, AL, PH, RG) ebu_kweight_frag<NC, AL, PH, RG><<<grid, blk, EBU_SMEM_BYTES, st>>> (src, stride, nch, kf, ke, (int)pos, h->cf, ck, (float)h->fragm, h->d_z, h->d_frpwr, h->d_fragpw, (int)h->n_inst, (after_k1 && done == 0) ? 1 : 0, d_len)
+#define EBU_K1(NC, AL) do { if (d_len) EBU_K1P (NC, AL, true, true); else if (multi) EBU_K1P (NC, AL, true, false); else EBU_K1P (NC, AL, false, false); } while (0)
 #define EBU_K1T(NC) ebu_kweight_tma<NC><<<grid, blk, EBU_TMA_SMEM, st>>> (tmap, nch, kf, ke, (int)pos, h->cf, ck, (float)h->fragm, h->d_z, h->d_frpwr, h->d_fragpw, (int)h->n_inst, (after_k1 && done == 0) ? 1 : 0)
             if (h->weighted) {                                   // weighted banks: the run-time channel count, lanes grouped per instance
                 const int pt = (after_k1 && done == 0) ? 1 : 0;
-#define EBU_K1W(AL, PH) ebu_kweight_frag_w<AL, PH><<<grid, blk, EBU_SMEM_BYTES, st>>> (src, stride, nch, kf, ke, (int)pos, h->cf, ck, (float)h->fragm, h->d_z, h->d_frpwr, h->d_fragpw, (int)h->n_inst, pt, h->gw)
-                if (al) { if (multi) EBU_K1W (true, true); else EBU_K1W (true, false); }
-                else    { if (multi) EBU_K1W (false, true); else EBU_K1W (false, false); }
+#define EBU_K1W(AL, PH, RG) ebu_kweight_frag_w<AL, PH, RG><<<grid, blk, EBU_SMEM_BYTES, st>>> (src, stride, nch, kf, ke, (int)pos, h->cf, ck, (float)h->fragm, h->d_z, h->d_frpwr, h->d_fragpw, (int)h->n_inst, pt, h->gw, d_len)
+                if (al) { if (d_len) EBU_K1W (true, true, true); else if (multi) EBU_K1W (true, true, false); else EBU_K1W (true, false, false); }
+                else    { if (d_len) EBU_K1W (false, true, true); else if (multi) EBU_K1W (false, true, false); else EBU_K1W (false, false, false); }
 #undef EBU_K1W
             }
             else if (h->nchan > 2) {                             // surround banks (3..5 channels): the one-warp kernel, lanes grouped per instance
@@ -1033,7 +1100,7 @@ int ebu_process_sliced (b200m_ebu* h, const float* d_in, size_t stride, uint32_t
         if (after_k1 && done == 0) { if (int rc = after_k1 (after_arg)) return rc; }      // work to enqueue right behind the first K1
         for (int f = 0; f < nfrag; ++f) {                    // fragments complete in order; each may trigger gating
             ebu_fragment_kernel<<<(h->n_inst + K2A_THREADS - 1) / K2A_THREADS, K2A_THREADS, 0, st>>> (
-                (int)h->n_inst, f, ck.fph, h->tmod, h->fragm, (int)nfram, h->d_fragpw, h->d_ring, h->d_ctl, h->d_res, h->d_histM, h->d_histS, h->d_cnt);
+                (int)h->n_inst, f, ck.fph, h->tmod, h->fragm, (int)nfram, h->d_fragpw, h->d_ring, h->d_ctl, h->d_res, h->d_histM, h->d_histS, h->d_cnt, d_len);
             B200M_LAUNCHED (1);
             // K2b behind fragment f only if some class completing its fragment f has an integrating member whose S period wraps
             // there: a later addpoint in the same block would otherwise be gated into the statistics
@@ -1043,6 +1110,7 @@ int ebu_process_sliced (b200m_ebu* h, const float* d_in, size_t stride, uint32_t
                 if (!multi || f < h->nf[q]) wrap |= b200m_ebu::phase_tick (c.second);
                 ++q;
             }
+            if (d_len) wrap |= h->ragged_tick (f);
             if (wrap) {
                 ebu_gate_kernel<<<(h->n_inst + K2B_WARPS - 1) / K2B_WARPS, K2B_WARPS * 32, 0, st>>> (
                     (int)h->n_inst, h->d_ctl, h->d_res, h->d_histM, h->d_histS, h->d_cnt, h->d_binpow);
@@ -1051,15 +1119,44 @@ int ebu_process_sliced (b200m_ebu* h, const float* d_in, size_t stride, uint32_t
         }
         done += pos;
     }
+    if (d_len) {                                             // behind the fragment kernels, which read the clocks the block began with
+        ebu_ragged_clock_kernel<<<(h->n_inst + 255) / 256, 256, 0, st>>> ((int)h->n_inst, d_len, (int)nfram, h->fragm, h->d_fph);
+        B200M_LAUNCHED (1);
+        h->ragged_join (len, nfram);
+    }
     h->tmod = (int)((h->tmod + nfram) % (uint32_t)h->fragm);
     B200M_CUDA (cudaGetLastError ());
     return 0;
 }
 
-static int ebu_process (b200m_ebu* h, const float* d_in, size_t stride, uint32_t nfram, cudaStream_t st)
+static int ebu_process (b200m_ebu* h, const float* d_in, size_t stride, uint32_t nfram, cudaStream_t st, const uint32_t* len = nullptr)
 {
     const uint32_t bounds[2] = {0, h->n_inst};
-    return ebu_process_sliced (h, d_in, stride, nfram, st, 1, bounds, nullptr, nullptr, nullptr, nullptr);
+    const uint32_t* d_len = len ? ebu_upload_len (h, len, st) : nullptr;
+    if (len && !d_len) return B200M_E_CUDA;
+    return ebu_process_sliced (h, d_in, stride, nfram, st, 1, bounds, nullptr, nullptr, nullptr, nullptr, len, d_len);
+}
+
+int ebu_ragged_check (const b200m_ebu* h, uint32_t nfram, const uint32_t* len)
+{
+    if (!len) return 0;
+    bool rag = false;
+    for (uint32_t i = 0; i < h->n_inst; ++i) {
+        if (len[i] > nfram) return set_err (B200M_E_INVAL, "len[%u] = %u exceeds nfram = %u", i, len[i], nfram);
+        rag |= len[i] != nfram;
+    }
+    return rag ? 1 : 0;
+}
+
+const uint32_t* ebu_upload_len (b200m_ebu* h, const uint32_t* len, cudaStream_t st)
+{
+    // pinned staging: the copy is truly asynchronous, and the slot's previous copy has run before it is overwritten
+    const int s = h->len_slot; h->len_slot ^= 1;
+    cudaError_t e = cudaEventSynchronize (h->ev_len[s]);
+    if (e == cudaSuccess) { memcpy (h->h_len[s], len, h->n_inst * sizeof (uint32_t)); e = cudaMemcpyAsync (h->d_len, h->h_len[s], h->n_inst * sizeof (uint32_t), cudaMemcpyHostToDevice, st); }
+    if (e == cudaSuccess) e = cudaEventRecord (h->ev_len[s], st);
+    if (e != cudaSuccess) { cuda_fail (e, "ebu_upload_len", __FILE__, __LINE__); return nullptr; }
+    return h->d_len;
 }
 
 int b200m_ebu_process_device (b200m_ebu* h, const float* d_in, size_t stride, uint32_t nfram, void* stream)
@@ -1081,6 +1178,33 @@ int b200m_ebu_process_host (b200m_ebu* h, const float* in, size_t stride, uint32
                                    (size_t)nfram * sizeof (float), nch, cudaMemcpyHostToDevice, h->own));
     h->last_host = true;
     return ebu_process (h, h->stage.d, h->stage.cap, nfram, h->own);
+}
+
+int b200m_ebu_process_ragged_device (b200m_ebu* h, const float* d_in, size_t stride, uint32_t nfram, const uint32_t* len, void* stream)
+{
+    if (int rc = check_block_args (h, d_in, stride, nfram)) return rc;
+    const int rag = ebu_ragged_check (h, nfram, len);
+    if (rag < 0) return rag;
+    if (!rag) return b200m_ebu_process_device (h, d_in, stride, nfram, stream);      // every length is nfram: the plain call
+    DeviceGuard g (h->device);
+    h->last_host = false;
+    return ebu_process (h, d_in, stride, nfram, (cudaStream_t)stream, len);
+}
+
+int b200m_ebu_process_ragged_host (b200m_ebu* h, const float* in, size_t stride, uint32_t nfram, const uint32_t* len)
+{
+    if (int rc = check_block_args (h, in, stride, nfram)) return rc;
+    const int rag = ebu_ragged_check (h, nfram, len);
+    if (rag < 0) return rag;
+    if (!rag) return b200m_ebu_process_host (h, in, stride, nfram);
+    DeviceGuard g (h->device);
+    B200M_ENTER_HOST_PATH (h);
+    const size_t nch = (size_t)h->n_inst * h->nchan;
+    if (h->stage.ensure (nch, nfram)) return set_err (B200M_E_NOMEM, "staging buffer allocation failed");
+    B200M_CUDA (cudaMemcpy2DAsync (h->stage.d, h->stage.cap * sizeof (float), in, stride * sizeof (float),
+                                   (size_t)nfram * sizeof (float), nch, cudaMemcpyHostToDevice, h->own));
+    h->last_host = true;
+    return ebu_process (h, h->stage.d, h->stage.cap, nfram, h->own, len);
 }
 
 static cudaStream_t ebu_stream (b200m_ebu* h, void* stream) { return h->last_host ? h->own : (cudaStream_t)stream; }

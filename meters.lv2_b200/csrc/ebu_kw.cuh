@@ -95,10 +95,16 @@ B200M_DEV uint32_t smem_u32 (const void* p) { return (uint32_t)__cvta_generic_to
 // TmaStage in ebu.cu, FusedStage in tpk.cu).  PHASES = false compiles the chunk-list policy alone (ck.fph is ignored).
 // NCHAN = 0: a weighted bank, gw->nch channels per instance with the weights gw->g (the instance's lanes are lane - lane % nch ..
 // + nch - 1); gw is read only in that form.
-template <int NCHAN, bool PHASES, class Stage>
+// RAG (a ragged block, per-instance phases only): instance i processes only its first rlen[i] frames.  Its end is one more
+// candidate of the warp's next cut; there its detect_process() call ends (scrub, channel sum, _frpwr +=, and the fragment if an
+// edge falls on it) and its state goes to memory at once.  Past that cut the lane keeps stepping through whatever the input holds
+// (no per-sample predicate) but never cuts, emits or stores again; rlen[i] = 0: it never does.
+template <int NCHAN, bool PHASES, class Stage, bool RAG = false>
 B200M_DEV void kw_warp (Stage& sg, int lane, int k, bool live, int nchans, int nfram, const EbuCoef& cf, const EbuChunks& ck, float fragm_f,
-                        float* __restrict__ zst, float* __restrict__ frpwr, float* __restrict__ fragpw, int n_inst, const EbuGains* gw = nullptr)
+                        float* __restrict__ zst, float* __restrict__ frpwr, float* __restrict__ fragpw, int n_inst, const EbuGains* gw = nullptr,
+                        const uint32_t* __restrict__ rlen = nullptr)
 {
+    static_assert (!RAG || PHASES, "a ragged block runs the per-instance phase policy");
     const int ntiles = (nfram + EBU_TILE - 1) / EBU_TILE;
     float z1 = zst[0 * (size_t)nchans + k], z2 = zst[1 * (size_t)nchans + k];
     float z3 = zst[2 * (size_t)nchans + k], z4 = zst[3 * (size_t)nchans + k];
@@ -112,15 +118,21 @@ B200M_DEV void kw_warp (Stage& sg, int lane, int k, bool live, int nchans, int n
     // per-instance phases: the warp cuts at the nearest of its lanes' own fragment edges and the block end; a lane's
     // detect_process() call ends only at its own edges and the block end (:207-216), so at another lane's edge it carries on
     int mynext = 0x7fffffff;                           // this lane's next own fragment edge
+    int myend = 0x7fffffff;                            // RAG: this lane's own block end until its lane has cut there
     if (PHASES && ck.fph) {
         if (live) { int el = (ck.tmod - ck.fph[inst]) % ck.fragm; if (el < 0) el += ck.fragm; mynext = ck.fragm - el; }
-        cend = min (__reduce_min_sync (0xffffffffu, mynext), nfram);
+        if constexpr (RAG) {
+            if (live) { myend = (int)rlen[inst]; if (myend == 0) mynext = myend = 0x7fffffff; }
+            cend = min (__reduce_min_sync (0xffffffffu, min (mynext, myend)), nfram);
+        }
+        else cend = min (__reduce_min_sync (0xffffffffu, mynext), nfram);
     }
 
     // end of one detect_process() call (:324-335): state scrub, channel sum, _frpwr +=, fragment hand-over (:217-221)
     auto chunk_end = [&] () {
         bool cut = true;
-        if (PHASES && ck.fph) { cfrag = mynext == cend; cut = cfrag || cend == nfram; }
+        if constexpr (RAG) { cfrag = mynext == cend; cut = cfrag || cend == myend; }
+        else if (PHASES && ck.fph) { cfrag = mynext == cend; cut = cfrag || cend == nfram; }
         float si;
         if constexpr (NCHAN == 0) {
             // si = g0 sj0, then si += g_c sj_c in channel order (:328-330 with the caller's weights; 0 + g0 sj0 is g0 sj0 exactly).
@@ -148,8 +160,17 @@ B200M_DEV void kw_warp (Stage& sg, int lane, int k, bool live, int nchans, int n
                 mynext += ck.fragm;
             }
             sj = 0.0f;
+            if constexpr (RAG) {
+                if (cend == myend) {                   // the instance's process() call ends here: its state is final
+                    zst[0 * (size_t)nchans + k] = z1; zst[1 * (size_t)nchans + k] = z2;
+                    zst[2 * (size_t)nchans + k] = z3; zst[3 * (size_t)nchans + k] = z4;
+                    if ((k % nch) == 0) frpwr[inst] = fp;
+                    mynext = myend = 0x7fffffff;
+                }
+            }
         }
-        if (PHASES && ck.fph) cend = cend == nfram ? 0x7fffffff : min (__reduce_min_sync (0xffffffffu, mynext), nfram);
+        if constexpr (RAG) cend = cend == nfram ? 0x7fffffff : min (__reduce_min_sync (0xffffffffu, min (mynext, myend)), nfram);
+        else if (PHASES && ck.fph) cend = cend == nfram ? 0x7fffffff : min (__reduce_min_sync (0xffffffffu, mynext), nfram);
         else {
             ++ci;
             if (ci < ck.n) { cend = (int)(ck.v[ci] & 0x7fffffffu); cfrag = (ck.v[ci] >> 31) != 0; }
@@ -197,7 +218,7 @@ B200M_DEV void kw_warp (Stage& sg, int lane, int k, bool live, int nchans, int n
         sg.release (t);
     }
     sg.drain ();
-    if (live) {
+    if (!RAG && live) {                                // RAG: every live lane stored its state at its own end
         zst[0 * (size_t)nchans + k] = z1; zst[1 * (size_t)nchans + k] = z2;
         zst[2 * (size_t)nchans + k] = z3; zst[3 * (size_t)nchans + k] = z4;
         if ((k % nch) == 0) frpwr[inst] = fp;
@@ -217,4 +238,10 @@ int ebu_check_gains (uint32_t nchan, const float* gains);
 extern "C" bool ebu_single_k1 (const b200m_ebu* h, uint32_t nfram);
 // host side, ebu.cu: one Ebu_r128_proc::process call of every instance, launched per instance slice (see the definition)
 extern "C" int ebu_process_sliced (b200m_ebu* h, const float* d_in, size_t stride, uint32_t nfram, cudaStream_t st, int nsl, const uint32_t* bounds,
-                                   cudaEvent_t* ready, int (*after_k1) (void*), void* after_arg, int (*k1_fused) (void*, const b200m::EbuK1Args&));
+                                   cudaEvent_t* ready, int (*after_k1) (void*), void* after_arg, int (*k1_fused) (void*, const b200m::EbuK1Args&),
+                                   const uint32_t* len = nullptr, const uint32_t* d_len = nullptr);
+// host side, ebu.cu: per-instance lengths of a ragged block (b200m_ebu_process_ragged_*).  ebu_ragged_check: 1 if some len[i] differs
+// from nfram, 0 if none does (or len is NULL: the plain call), B200M_E_INVAL if one exceeds nfram.  ebu_upload_len: enqueue the
+// copy of len[0 .. n_inst) on st into the bank's device array, which it returns (nullptr on a CUDA error, reported by set_err)
+extern "C" int ebu_ragged_check (const b200m_ebu* h, uint32_t nfram, const uint32_t* len);
+extern "C" const uint32_t* ebu_upload_len (b200m_ebu* h, const uint32_t* len, cudaStream_t st);

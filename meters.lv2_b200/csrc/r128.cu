@@ -18,31 +18,39 @@ namespace b200m {
 // coef_to_db (src/ebulv2.cc:227-230) and the tp_max hold (:360-367) run in the epilogue of the true-peak kernels (tpk.cu) when an
 // instance's channels never leave an 8-channel true-peak group (1, 2, 4 channels).  With 3 or 5 they leave every channel's read()
 // in lin[] (R128Hold) and this kernel, one thread per instance behind them, folds the instance's reads in channel order.
+// rlen (a ragged block): an instance with length 0 did not run, its hold stays.
 template <int NCHAN>
-__global__ void r128_hold_kernel (int n_inst, const float* __restrict__ lin, float* __restrict__ tpmax)
+__global__ void r128_hold_kernel (int n_inst, const float* __restrict__ lin, float* __restrict__ tpmax, const uint32_t* __restrict__ rlen)
 {
     const int i = blockIdx.x * blockDim.x + threadIdx.x;
-    if (i >= n_inst) return;
+    if (i >= n_inst || (rlen && rlen[i] == 0)) return;
     float t = lin[(size_t)i * NCHAN];
 #pragma unroll
     for (int c = 1; c < NCHAN; ++c) { const float v = lin[(size_t)i * NCHAN + c]; t = t > v ? t : v; }
     r128_hold (tpmax + i, t);
 }
 // the same fold for a weighted bank: nch = 1..32 channels per instance, known at run time
-__global__ void r128_hold_kernel_w (int n_inst, int nch, const float* __restrict__ lin, float* __restrict__ tpmax)
+__global__ void r128_hold_kernel_w (int n_inst, int nch, const float* __restrict__ lin, float* __restrict__ tpmax, const uint32_t* __restrict__ rlen)
 {
     const int i = blockIdx.x * blockDim.x + threadIdx.x;
-    if (i >= n_inst) return;
+    if (i >= n_inst || (rlen && rlen[i] == 0)) return;
     float t = lin[(size_t)i * nch];
     for (int c = 1; c < nch; ++c) { const float v = lin[(size_t)i * nch + c]; t = t > v ? t : v; }
     r128_hold (tpmax + i, t);
 }
 __global__ void r128_fill_kernel (int n, float* p, float v) { const int i = blockIdx.x * blockDim.x + threadIdx.x; if (i < n) p[i] = v; }
+// the same for the instances of a ragged block that ran (rlen[i] > 0)
+__global__ void r128_fill_ran_kernel (int n, float* p, float v, const uint32_t* __restrict__ rlen)
+{
+    const int i = blockIdx.x * blockDim.x + threadIdx.x;
+    if (i < n && rlen[i] != 0) p[i] = v;
+}
 
 // Per-instance dBTP.  An instance with dBTP off runs no process_max (src/ebulv2.cc:344-347): its nchan TruePeakdsp histories
 // stay frozen and its hold is -inf after the cycle (:365-366).  In a cycle with a mixed mask the true-peak kernels process every
 // channel; behind them r128_dbtp_fix_kernel puts the frozen histories (stash) back into the history the next block reads and
-// clears the hold of the disabled instances.  One thread per (instance, history float); nh = nchan x 48 history floats per instance.
+// clears the hold of the disabled instances (in a ragged block: of those that ran; a disabled instance's histories stay frozen whatever
+// its length).  One thread per (instance, history float); nh = nchan x 48 history floats per instance.
 __global__ void r128_dbtp_stash_kernel (int n_inst, int nh, const uint8_t* __restrict__ off, const float* __restrict__ hist, float* __restrict__ stash)
 {
     const int t = blockIdx.x * blockDim.x + threadIdx.x;
@@ -50,21 +58,21 @@ __global__ void r128_dbtp_stash_kernel (int n_inst, int nh, const uint8_t* __res
     stash[t] = hist[t];                           // the channels of instance i are nchan i .. nchan i + nchan - 1: its floats are contiguous
 }
 __global__ void r128_dbtp_fix_kernel (int n_inst, int nh, const uint8_t* __restrict__ off, const float* __restrict__ stash, float* __restrict__ hist,
-                                      float* __restrict__ tpmax)
+                                      float* __restrict__ tpmax, const uint32_t* __restrict__ rlen)
 {
     const int t = blockIdx.x * blockDim.x + threadIdx.x;
     if (t >= n_inst * nh) return;
     const int i = t / nh;
     if (!off[i]) return;
     hist[t] = stash[t];
-    if (t % nh == 0) tpmax[i] = -INFINITY;
+    if (t % nh == 0 && !(rlen && rlen[i] == 0)) tpmax[i] = -INFINITY;
 }
 
 }  // namespace b200m
 
 // sliced process entry point of the true-peak bank and the fused K-weighting + true-peak kernel (tpk.cu); the EBU bank's: ebu_kw.cuh
 int tpk_process_sliced (b200m_tpk* h, const float* d_in, size_t stride, uint32_t nfram, uint32_t tp_mode, cudaStream_t st, int nsl, const uint32_t* bounds, cudaEvent_t* ready,
-                        b200m::R128Hold r128, bool pdl, const void* dr);
+                        b200m::R128Hold r128, bool pdl, const void* dr, const uint32_t* rlen);
 bool tpk_r128_fused_ok (const b200m_tpk* h, const float* d_in, size_t stride, uint32_t nfram);
 float* tpk_hist (b200m_tpk* h);
 int tpk_r128_fused (b200m_tpk* h, const b200m::EbuK1Args& a, float* r128_tpmax, cudaStream_t st);
@@ -94,14 +102,14 @@ struct b200m_r128 {
 
 static int env_int (const char* name, int dflt) { const char* v = getenv (name); return v ? atoi (v) : dflt; }
 
-struct R128Step { b200m_r128* h; const float* d_in; size_t stride; uint32_t nfram; cudaStream_t st; const uint32_t* bc; };
+struct R128Step { b200m_r128* h; const float* d_in; size_t stride; uint32_t nfram; cudaStream_t st; const uint32_t* bc; const uint32_t* d_len; };
 
 // device path: the true-peak kernel goes onto the caller's stream right behind the first K-weighting launch, with
 // programmatic dependent launch, so that the two kernels share the SMs (see r128_run)
 static int r128_tp_behind_k1 (void* p)
 {
     R128Step* a = (R128Step*)p;
-    return tpk_process_sliced (a->h->tpk, a->d_in, a->stride, a->nfram, B200M_TP_MODE_MAX, a->st, 1, a->bc, nullptr, a->h->hold (), true, nullptr);
+    return tpk_process_sliced (a->h->tpk, a->d_in, a->stride, a->nfram, B200M_TP_MODE_MAX, a->st, 1, a->bc, nullptr, a->h->hold (), true, nullptr, a->d_len);
 }
 
 // device path, fused: one kernel does K1's work and the true-peak maximum over one shared-memory copy of the block (tpk.cu)
@@ -111,7 +119,9 @@ static int r128_fused_k1 (void* p, const EbuK1Args& a)
     return tpk_r128_fused (s->h->tpk, a, s->h->d_tpmax, s->st);
 }
 
-static int r128_run (b200m_r128* h, const float* d_in, size_t stride, uint32_t nfram, cudaStream_t st, int nsl, cudaEvent_t* ready)
+// len (host, every entry <= nfram, some != nfram): a ragged block, instance i runs its cycle over its first len[i] frames; nullptr: all nfram
+static int r128_run (b200m_r128* h, const float* d_in, size_t stride, uint32_t nfram, cudaStream_t st, int nsl, cudaEvent_t* ready,
+                     const uint32_t* len = nullptr)
 {
     uint32_t bi[R128_SLICES + 1], bc[R128_SLICES + 1];
     for (int s = 0; s <= nsl; ++s) { bi[s] = (uint32_t)((uint64_t)h->n_inst * s / nsl); bc[s] = h->nchan * bi[s]; }
@@ -129,6 +139,10 @@ static int r128_run (b200m_r128* h, const float* d_in, size_t stride, uint32_t n
     // true-peak bank would take the tensor-core path, the block is 16-byte aligned with nfram % 4 == 0, its chunk list fits one K1
     // launch and the bank is large enough to fill the GPU with 128-channel (3 and 5 channels: 120-channel) slabs.
     // 3 and 5 channels outside the fused kernel: r128_hold_kernel behind the true-peak kernels folds the hold.
+    // A ragged block: one upload of the lengths, read by the K-weighting, fragment and true-peak kernels.  The true-peak FIR is
+    // tpmax_kernel in both precision modes (tpk_process_sliced): no fused kernel.
+    const uint32_t* d_len = nullptr;
+    if (len && !(d_len = ebu_upload_len (h->ebu, len, st))) return B200M_E_CUDA;
     const bool mixed = h->n_off && h->n_off < h->n_inst;
     if (mixed) {
         // the first mixed cycle after a change: device mask, then the frozen histories of the disabled instances.  Until now every
@@ -143,34 +157,35 @@ static int r128_run (b200m_r128* h, const float* d_in, size_t stride, uint32_t n
         }
     }
     // weighted banks have no fused form: they keep the two-kernel cycle (K1 + the true-peak kernel behind it), see DESIGN.md §3
-    const bool fused = !ready && h->dbtp && !h->weighted && tpk_r128_fused_ok (h->tpk, d_in, stride, nfram) && ebu_single_k1 (h->ebu, nfram);
+    const bool fused = !ready && !d_len && h->dbtp && !h->weighted && tpk_r128_fused_ok (h->tpk, d_in, stride, nfram) && ebu_single_k1 (h->ebu, nfram);
     const bool pdl = !fused && h->dbtp && h->concurrent >= 2 && !ready;
     const bool conc = h->dbtp && h->concurrent >= 1 && ready;
     // the side stream's true-peak kernels read the history that the stash / fix-up kernels on st touch
-    if (conc && (mixed || h->fixed)) { B200M_CUDA (cudaEventRecord (h->ev_pre, st)); B200M_CUDA (cudaStreamWaitEvent (h->side, h->ev_pre, 0)); }
+    if (conc && (mixed || h->fixed || d_len)) { B200M_CUDA (cudaEventRecord (h->ev_pre, st)); B200M_CUDA (cudaStreamWaitEvent (h->side, h->ev_pre, 0)); }
     h->fixed = mixed && h->dbtp;
-    R128Step step = {h, d_in, stride, nfram, st, bc};
+    R128Step step = {h, d_in, stride, nfram, st, bc, d_len};
     if (int rc = ebu_process_sliced (h->ebu, d_in, stride, nfram, st, nsl, bi, ready, pdl ? r128_tp_behind_k1 : nullptr, &step,
-                                     fused ? r128_fused_k1 : nullptr)) return rc;
+                                     fused ? r128_fused_k1 : nullptr, len, d_len)) return rc;
     if (h->dbtp) {
         if (!pdl && !fused) {
-            if (int rc = tpk_process_sliced (h->tpk, d_in, stride, nfram, B200M_TP_MODE_MAX, conc ? h->side : st, nsl, bc, conc ? ready : nullptr, h->hold (), false, nullptr)) return rc;
+            if (int rc = tpk_process_sliced (h->tpk, d_in, stride, nfram, B200M_TP_MODE_MAX, conc ? h->side : st, nsl, bc, conc ? ready : nullptr, h->hold (), false, nullptr, d_len)) return rc;
             if (conc) { B200M_CUDA (cudaEventRecord (h->ev_tp, h->side)); B200M_CUDA (cudaStreamWaitEvent (st, h->ev_tp, 0)); }
         }
         if (h->d_tplin && !fused) {                        // behind every slice's true-peak kernel, before the fix-up clears holds
             const int nb = (h->n_inst + 255) / 256;
-            if (h->weighted) r128_hold_kernel_w<<<nb, 256, 0, st>>> ((int)h->n_inst, (int)h->nchan, h->d_tplin, h->d_tpmax);
-            else if (h->nchan == 3) r128_hold_kernel<3><<<nb, 256, 0, st>>> ((int)h->n_inst, h->d_tplin, h->d_tpmax);
-            else r128_hold_kernel<5><<<nb, 256, 0, st>>> ((int)h->n_inst, h->d_tplin, h->d_tpmax);
+            if (h->weighted) r128_hold_kernel_w<<<nb, 256, 0, st>>> ((int)h->n_inst, (int)h->nchan, h->d_tplin, h->d_tpmax, d_len);
+            else if (h->nchan == 3) r128_hold_kernel<3><<<nb, 256, 0, st>>> ((int)h->n_inst, h->d_tplin, h->d_tpmax, d_len);
+            else r128_hold_kernel<5><<<nb, 256, 0, st>>> ((int)h->n_inst, h->d_tplin, h->d_tpmax, d_len);
             B200M_LAUNCHED (1);
         }
         if (mixed) {                                       // behind the true-peak kernels on st, and behind the history swap on the host
             const int nh = (int)h->nchan * 48, nt = (int)h->n_inst * nh;
-            r128_dbtp_fix_kernel<<<(nt + 255) / 256, 256, 0, st>>> ((int)h->n_inst, nh, h->d_off, h->d_stash, tpk_hist (h->tpk), h->d_tpmax);
+            r128_dbtp_fix_kernel<<<(nt + 255) / 256, 256, 0, st>>> ((int)h->n_inst, nh, h->d_off, h->d_stash, tpk_hist (h->tpk), h->d_tpmax, d_len);
             B200M_LAUNCHED (1);
         }
     } else {
-        r128_fill_kernel<<<(h->n_inst + 255) / 256, 256, 0, st>>> ((int)h->n_inst, h->d_tpmax, -INFINITY);   // :365-366
+        if (d_len) r128_fill_ran_kernel<<<(h->n_inst + 255) / 256, 256, 0, st>>> ((int)h->n_inst, h->d_tpmax, -INFINITY, d_len);
+        else r128_fill_kernel<<<(h->n_inst + 255) / 256, 256, 0, st>>> ((int)h->n_inst, h->d_tpmax, -INFINITY);   // :365-366
         B200M_LAUNCHED (1);
     }
     B200M_CUDA (cudaGetLastError ());
@@ -308,7 +323,35 @@ int b200m_r128_run_device (b200m_r128* h, const float* d_in, size_t stride, uint
     return r128_run (h, d_in, stride, nfram, (cudaStream_t)stream, 1, nullptr);
 }
 
+int b200m_r128_run_ragged_device (b200m_r128* h, const float* d_in, size_t stride, uint32_t nfram, const uint32_t* len, void* stream)
+{
+    if (int rc = check_block_args (h, d_in, stride, nfram)) return rc;
+    const int rag = ebu_ragged_check (h->ebu, nfram, len);
+    if (rag < 0) return rag;
+    if (!rag) return b200m_r128_run_device (h, d_in, stride, nfram, stream);        // every length is nfram: the plain call
+    DeviceGuard g (h->device);
+    h->last_host = false;
+    return r128_run (h, d_in, stride, nfram, (cudaStream_t)stream, 1, nullptr, len);
+}
+
+static int r128_run_host (b200m_r128* h, const float* in, size_t stride, uint32_t nfram, const uint32_t* len);
+
 int b200m_r128_run_host (b200m_r128* h, const float* in, size_t stride, uint32_t nfram)
+{
+    return r128_run_host (h, in, stride, nfram, nullptr);
+}
+
+int b200m_r128_run_ragged_host (b200m_r128* h, const float* in, size_t stride, uint32_t nfram, const uint32_t* len)
+{
+    if (int rc = check_block_args (h, in, stride, nfram)) return rc;
+    const int rag = ebu_ragged_check (h->ebu, nfram, len);
+    if (rag < 0) return rag;
+    return r128_run_host (h, in, stride, nfram, rag ? len : nullptr);
+}
+
+}  // extern "C"
+
+static int r128_run_host (b200m_r128* h, const float* in, size_t stride, uint32_t nfram, const uint32_t* len)
 {
     if (int rc = check_block_args (h, in, stride, nfram)) return rc;
     DeviceGuard g (h->device);
@@ -328,10 +371,12 @@ int b200m_r128_run_host (b200m_r128* h, const float* in, size_t stride, uint32_t
         B200M_CUDA (cudaEventRecord (h->ev_ready[s], h->copy));
     }
     h->last_host = true;
-    if (int rc = r128_run (h, h->stage.d, h->stage.cap, nfram, h->own, nsl, h->ev_ready)) return rc;
+    if (int rc = r128_run (h, h->stage.d, h->stage.cap, nfram, h->own, nsl, h->ev_ready, len)) return rc;
     B200M_CUDA (cudaEventRecord (h->ev_done, h->own));
     return 0;
 }
+
+extern "C" {
 
 int b200m_r128_results (b200m_r128* h, b200m_ebu_result* ebu_out, float* tp_max_db, void* stream)
 {

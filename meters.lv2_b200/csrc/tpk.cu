@@ -788,10 +788,15 @@ tpk_kernel (const float* __restrict__ in, size_t stride, int c_first, int n_chan
 // (all values are >= +0, so unsigned order = float order); the CTA that finishes a channel group last applies
 // `m = _res ? 0 : _m; if (v > m) m = v; _m = m` and, in the EBUr128 cycle, the plugin's read() x 2 + coef_to_db + tp_max hold.
 // The history of the NEXT block goes to the alternate buffer (the group's chunk-0 CTA may still be reading the current one).
-template <bool IMM, bool FMA, int HOLD>
+// RAG: a ragged EBUr128 block, row c belongs to instance c / r128.nch, which ran for its first rlen[instance] frames.  The maximum
+// excludes positions at or after that length (the FIR is causal: the positions before it never see the unread frames); the CTA
+// whose chunk holds the row's end writes the row's next history from xs (its 48-sample prefix covers lengths < 48; length 0: chunk 0
+// copies the current history, which the host swap would otherwise lose); the epilogue leaves tp_m, tp_res and the hold of a
+// length-0 instance untouched (the plugin did not run).
+template <bool IMM, bool FMA, int HOLD, bool RAG = false>
 __global__ void __launch_bounds__ (TPK_THREADS)
 tpmax_kernel (const float* __restrict__ in, size_t stride, int c_first, int n_chan, int nfram, int nchunks, int aligned, int elide0,
-              TpkState st, float* __restrict__ dbg, R128Hold r128)
+              TpkState st, float* __restrict__ dbg, R128Hold r128, const uint32_t* __restrict__ rlen)
 {
     constexpr int CH = 8, TC = 256;
     constexpr int XP = 48 + TC + 4;
@@ -841,6 +846,8 @@ tpmax_kernel (const float* __restrict__ in, size_t stride, int c_first, int n_ch
     __syncthreads ();
 
     const int r = tid / LPR, ql = tid % LPR;
+    // positions of this thread's row that count in this chunk
+    const int rl = RAG ? max (0, min (len, (int)rlen[(unsigned)min (c0 + r, n_chan - 1) / (unsigned)r128.nch] - s0)) : len;
     float vmax = 0.0f, vmax2 = 0.0f;                        // vmax2: max (|P| + |Q|) = 2 max (|ph1|, |ph3|), tolerance mode
     {
         float M = 0.0f;
@@ -856,7 +863,7 @@ tpmax_kernel (const float* __restrict__ in, size_t stride, int c_first, int n_ch
         } else
 #pragma unroll 1
         for (int q = ql; q < GPC; q += LPR) {
-            const bool act = 4 * q < len;
+            const bool act = 4 * q < rl;
             bool full0 = !FMA;
             if (!FMA && elide0) {
                 const float4 xm = *reinterpret_cast<const float4*> (&xs[r][act ? 4 * q + 24 : 0]);
@@ -868,7 +875,7 @@ tpmax_kernel (const float* __restrict__ in, size_t stride, int c_first, int n_ch
 #pragma unroll
                 for (int i = 0; i < 13; ++i) { const float4 v = xr[i]; w[4 * i] = v.x; w[4 * i + 1] = v.y; w[4 * i + 2] = v.z; w[4 * i + 3] = v.w; }
 #if B200M_TPK_SYM
-                if (FMA && !dbg) { fir16_fma_max<IMM> (w, min (4, len - 4 * q), vmax, vmax2); continue; }      // maxima only (dbg: warp-uniform)
+                if (FMA && !dbg) { fir16_fma_max<IMM> (w, min (4, rl - 4 * q), vmax, vmax2); continue; }      // maxima only (dbg: warp-uniform)
 #endif
                 float o[16];
                 if (FMA) fir16_fma<IMM> (w, o); else fir16<IMM> (w, &xs[r][4 * q], o, full0);
@@ -880,7 +887,7 @@ tpmax_kernel (const float* __restrict__ in, size_t stride, int c_first, int n_ch
                 // positions beyond len inside the last group come from zero-filled input: exclude them
 #pragma unroll
                 for (int i = 0; i < 4; ++i)
-                    if (4 * q + i < len)
+                    if (4 * q + i < rl)
                         vmax = fmaxf (fmaxf (vmax, fmaxf (fabsf (o[4 * i]), fabsf (o[4 * i + 1]))), fmaxf (fabsf (o[4 * i + 2]), fabsf (o[4 * i + 3])));
             }
         }
@@ -891,7 +898,15 @@ tpmax_kernel (const float* __restrict__ in, size_t stride, int c_first, int n_ch
     if (ql == 0) s_rowmax[r] = vmax;
 
     // history of the next block = the 48 samples that end this one (the last chunk holds them: prefix + chunk >= 48 samples)
-    if (chunk == nchunks - 1)
+    if constexpr (RAG) {
+        for (int idx = tid; idx < CH * 48; idx += TPK_THREADS) {
+            const int rr = idx / 48, j = idx % 48;
+            if (c0 + rr >= n_chan) continue;
+            const int L = (int)rlen[(unsigned)(c0 + rr) / (unsigned)r128.nch];
+            if (chunk == (L > 0 ? (L - 1) / TC : 0)) st.hist_alt[(size_t)(c0 + rr) * 48 + j] = xs[rr][L - s0 + j];
+        }
+    }
+    else if (chunk == nchunks - 1)
         for (int idx = tid; idx < CH * 48; idx += TPK_THREADS) {
             const int rr = idx / 48, j = idx % 48;
             if (c0 + rr < n_chan) st.hist_alt[(size_t)(c0 + rr) * 48 + j] = xs[rr][len + j];
@@ -900,7 +915,8 @@ tpmax_kernel (const float* __restrict__ in, size_t stride, int c_first, int n_ch
     if (tid >= 32) return;                                  // the group / grid book-keeping is warp 0's: one fence per CTA, not one per warp
 
     const int cc = c0 + lane;
-    const bool own = lane < CH && cc < n_chan;
+    bool own = lane < CH && cc < n_chan;
+    if constexpr (RAG) own = own && rlen[(unsigned)cc / (unsigned)r128.nch] != 0;
     if (own && s_rowmax[lane] > 0.0f) atomicMax (st.blk_max + cc, __float_as_uint (s_rowmax[lane]));
     __threadfence ();                                       // the maxima are visible before this CTA's arrival is
     unsigned prev = 0;
@@ -2084,9 +2100,10 @@ int tpk_reset_inst (b200m_tpk* h, const uint32_t* d_inst, uint32_t n_sel, uint32
 static cudaStream_t tpk_stream (b200m_tpk* h, void* stream) { return h->last_host ? h->own : (cudaStream_t)stream; }
 
 // the instantiations of the EBUr128 epilogue's HOLD (r128_group_hold)
-template <bool IMM, bool FMA> static decltype (&tpmax_kernel<IMM, FMA, 2>) tpmax_kernel_for (int hold)
+template <bool IMM, bool FMA, bool RAG = false> static decltype (&tpmax_kernel<IMM, FMA, 2, RAG>) tpmax_kernel_for (int hold)
 {
-    return hold == 0 ? tpmax_kernel<IMM, FMA, 0> : hold == 1 ? tpmax_kernel<IMM, FMA, 1> : hold == 4 ? tpmax_kernel<IMM, FMA, 4> : tpmax_kernel<IMM, FMA, 2>;
+    return hold == 0 ? tpmax_kernel<IMM, FMA, 0, RAG> : hold == 1 ? tpmax_kernel<IMM, FMA, 1, RAG> : hold == 4 ? tpmax_kernel<IMM, FMA, 4, RAG>
+                                                                                                       : tpmax_kernel<IMM, FMA, 2, RAG>;
 }
 static decltype (&tpmax_tc_kernel<2>) tpmax_tc_kernel_for (int hold)
 {
@@ -2096,8 +2113,11 @@ static const int R128_HOLDS[4] = {0, 1, 2, 4};
 
 // process()/process_max() of every meter; channel slices [bounds[s], bounds[s+1]) are launched separately, slice s
 // after event ready[s] when `ready` is given (see ebu_process_sliced).
+// rlen (device, one length per EBUr128 instance, r128.nch channels each): a ragged block of the EBUr128 cycle.  It always runs
+// tpmax_kernel, exact or FMA: the tensor-core and fused kernels walk whole 8-channel groups through every chunk of the block with
+// no per-row end, so only the chunk-parallel kernel has the per-row mask and the per-row history hand-over.
 int tpk_process_sliced (b200m_tpk* h, const float* d_in, size_t stride, uint32_t nfram, uint32_t tp_mode, cudaStream_t st,
-                        int nsl, const uint32_t* bounds, cudaEvent_t* ready, R128Hold r128, bool pdl, const void* dr_v)
+                        int nsl, const uint32_t* bounds, cudaEvent_t* ready, R128Hold r128, bool pdl, const void* dr_v, const uint32_t* rlen)
 {
     const TpkDr* dr = (const TpkDr*)dr_v;
     const bool tp = h->flags & B200M_TPK_TRUEPEAK, km = h->flags & B200M_TPK_KMETER;
@@ -2123,7 +2143,16 @@ int tpk_process_sliced (b200m_tpk* h, const float* d_in, size_t stride, uint32_t
             if (h->imm && h->fma) B200M_CUDA (cudaLaunchKernelEx (&cfg, tpk_kernel<CH, TC, TP, MX, KM, true, DRM, true>, d_in, stride, cf, ce, (int)nfram, aligned, h->elide0, prm, h->st, h->d_dbg, r128, drp)); \
             else if (h->imm) B200M_CUDA (cudaLaunchKernelEx (&cfg, tpk_kernel<CH, TC, TP, MX, KM, true, DRM>, d_in, stride, cf, ce, (int)nfram, aligned, h->elide0, prm, h->st, h->d_dbg, r128, drp)); \
             else B200M_CUDA (cudaLaunchKernelEx (&cfg, tpk_kernel<CH, TC, TP, MX, KM, false, DRM>, d_in, stride, cf, ce, (int)nfram, aligned, h->elide0, prm, h->st, h->d_dbg, r128, drp)); } while (0)
-        if (tp && tp_mode == B200M_TP_MODE_MAX && !km && h->chunked && h->tc && h->fma && h->imm && h->d_btc && aligned && nfram % 4 == 0 && !h->d_dbg
+        if (rlen) {
+            const int nchunks = ((int)nfram + 255) / 256;
+            cfg.gridDim = dim3 ((unsigned)(((ce - cf + 7) / 8) * nchunks));
+            const int hold = r128_hold_of (r128);
+            const auto k = h->imm && h->fma ? tpmax_kernel_for<true, true, true> (hold) : h->imm ? tpmax_kernel_for<true, false, true> (hold)
+                                                                                                 : tpmax_kernel_for<false, false, true> (hold);
+            B200M_CUDA (cudaLaunchKernelEx (&cfg, k, d_in, stride, cf, ce, (int)nfram, nchunks, aligned, h->elide0, h->st, h->d_dbg, r128, rlen));
+            swap_hist = true;
+        }
+        else if (tp && tp_mode == B200M_TP_MODE_MAX && !km && h->chunked && h->tc && h->fma && h->imm && h->d_btc && aligned && nfram % 4 == 0 && !h->d_dbg
             && (ce - cf + 7) / 8 >= h->n_sm) {
             // tensor-core path: persistent CTAs, each takes whole 8-channel groups (a bank too small to give every SM a group runs tpmax_kernel)
             const int nchunks = ((int)nfram + 255) / 256;
@@ -2138,7 +2167,7 @@ int tpk_process_sliced (b200m_tpk* h, const float* d_in, size_t stride, uint32_t
             cfg.gridDim = dim3 ((unsigned)(((ce - cf + 7) / 8) * nchunks));
             const int hold = r128_hold_of (r128);
             const auto k = h->imm && h->fma ? tpmax_kernel_for<true, true> (hold) : h->imm ? tpmax_kernel_for<true, false> (hold) : tpmax_kernel_for<false, false> (hold);
-            B200M_CUDA (cudaLaunchKernelEx (&cfg, k, d_in, stride, cf, ce, (int)nfram, nchunks, aligned, h->elide0, h->st, h->d_dbg, r128));
+            B200M_CUDA (cudaLaunchKernelEx (&cfg, k, d_in, stride, cf, ce, (int)nfram, nchunks, aligned, h->elide0, h->st, h->d_dbg, r128, (const uint32_t*)nullptr));
             swap_hist = true;
         }
         else if (tp && tp_mode == B200M_TP_MODE_MAX) { if (km) TPK_GO (8, 256, true, true, true, false); else TPK_GO (8, 256, true, true, false, false); }
@@ -2197,7 +2226,7 @@ int tpk_process_sliced (b200m_tpk* h, const float* d_in, size_t stride, uint32_t
 static int tpk_process (b200m_tpk* h, const float* d_in, size_t stride, uint32_t nfram, uint32_t tp_mode, cudaStream_t st)
 {
     const uint32_t bounds[2] = {0, h->n_chan};
-    return tpk_process_sliced (h, d_in, stride, nfram, tp_mode, st, 1, bounds, nullptr, R128Hold {}, false, h->dr_on ? &h->dr : nullptr);
+    return tpk_process_sliced (h, d_in, stride, nfram, tp_mode, st, 1, bounds, nullptr, R128Hold {}, false, h->dr_on ? &h->dr : nullptr, nullptr);
 }
 
 // ---- the EBUr128 cycle's fused K-weighting + true-peak kernel (r128_fused_kernel), launched by the EBU bank in place of K1 (r128.cu)
@@ -2285,7 +2314,8 @@ int b200m_tpk_create (b200m_tpk** out, int device, uint32_t n_chan, float fsamp,
     if (e == cudaSuccess) e = cudaFuncSetAttribute (tpdec_kernel<true, false>, cudaFuncAttributePreferredSharedMemoryCarveout, cudaSharedmemCarveoutMaxShared);
     if (e == cudaSuccess) e = cudaFuncSetAttribute (tpdec_kernel<false, false>, cudaFuncAttributePreferredSharedMemoryCarveout, cudaSharedmemCarveoutMaxShared);
     for (const int hold : R128_HOLDS)
-        for (const auto k : {tpmax_kernel_for<true, true> (hold), tpmax_kernel_for<true, false> (hold), tpmax_kernel_for<false, false> (hold)})
+        for (const auto k : {tpmax_kernel_for<true, true> (hold), tpmax_kernel_for<true, false> (hold), tpmax_kernel_for<false, false> (hold),
+                             tpmax_kernel_for<true, true, true> (hold), tpmax_kernel_for<true, false, true> (hold), tpmax_kernel_for<false, false, true> (hold)})
             if (e == cudaSuccess) e = cudaFuncSetAttribute (k, cudaFuncAttributePreferredSharedMemoryCarveout, cudaSharedmemCarveoutMaxShared);
     auto A = [&] (void** p, size_t bytes) { if (e == cudaSuccess) { e = cudaMalloc (p, bytes); if (e == cudaSuccess) e = cudaMemset (*p, 0, bytes); } };
     const size_t n = n_chan;
