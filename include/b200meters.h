@@ -300,6 +300,19 @@ int b200m_dr14_create (b200m_dr14** out, int device, uint32_t n_inst, uint32_t n
 int b200m_dr14_destroy (b200m_dr14* h);
 int b200m_dr14_run_device (b200m_dr14* h, const float* d_in, size_t stride, uint32_t nfram, void* stream);   /* rows: inst * n_channels + c */
 int b200m_dr14_run_host (b200m_dr14* h, const float* in, size_t stride, uint32_t nfram);
+/* Ragged blocks: instance i runs dr14_run over the first len[i] <= nfram frames of its rows, bit-identical to a private plugin
+ * instance fed only those frames (DR-14 and TPnRMS mode, mono and stereo, device and host path).  len: host array of n_inst.
+ * - Frames at or after len[i] may hold anything, NaN and Inf included: they reach no result and no state.  A window that the
+ *   instance's frames do not complete is not scored, as the reference never scores a track's partial last window.
+ * - len[i] == 0: the instance is not called at all: no process and no read() (the meters' read latches stay), its result row and
+ *   m_dbtp are unchanged, and its 3 s window clock does not advance.
+ * - A length above nfram returns B200M_E_INVAL and enqueues nothing.
+ * - NULL, or every len[i] == nfram, is exactly b200m_dr14_run_* (same kernels, launches and bits).
+ * - Controls, path switches and streams are ordered between ragged blocks as between plain ones.
+ * A ragged block always runs the exact fused process() kernel (whatever B200M_TPK_SPLIT / B200M_TPK_WIDE select for plain blocks),
+ * plus one clock kernel in DR mode. */
+int b200m_dr14_run_ragged_device (b200m_dr14* h, const float* d_in, size_t stride, uint32_t nfram, const uint32_t* len, void* stream);
+int b200m_dr14_run_ragged_host (b200m_dr14* h, const float* in, size_t stride, uint32_t nfram, const uint32_t* len);
 int b200m_dr14_reset (b200m_dr14* h, void* stream);                                       /* reset_peaks, every instance */
 /* B200M_DR14_RESET: reset_peaks (:246-262) of the listed instances: K-meter reset, m_peak = m_rms = -81, m_dbtp = 0, window
  * sums, second-peak pair, histogram, num_fragments, and the instance's 3 s window restarts with the next block.

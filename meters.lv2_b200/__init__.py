@@ -121,6 +121,8 @@ _PROTOS = {
     "b200m_dr14_destroy": (C.c_int, [_v]),
     "b200m_dr14_run_device": (C.c_int, [_v, _v, C.c_size_t, C.c_uint32, _v]),
     "b200m_dr14_run_host": (C.c_int, [_v, _v, C.c_size_t, C.c_uint32]),
+    "b200m_dr14_run_ragged_device": (C.c_int, [_v, _v, C.c_size_t, C.c_uint32, _v, _v]),
+    "b200m_dr14_run_ragged_host": (C.c_int, [_v, _v, C.c_size_t, C.c_uint32, _v]),
     "b200m_dr14_reset": (C.c_int, [_v, _v]),
     "b200m_dr14_control": (C.c_int, [_v, _v, C.c_uint32, C.c_int, _v]),
     "b200m_dr14_results": (C.c_int, [_v, _v, _v]),
@@ -697,15 +699,26 @@ class DR14(_Bank):
         self.n_inst, self.nchan = n_inst, n_channels
         _ck(lib().b200m_dr14_create(C.byref(self.h), device, n_inst, n_channels, rate, int(bool(dr_mode))))
 
-    def run(self, x, stream=None):
+    def run(self, x, stream=None, lengths=None):
+        """one dr14_run of every instance over x [n_inst*nchan, nfram] (CUDA tensor: device path; numpy / CPU tensor: host path).
+        lengths: None, or n_inst frame counts <= nfram: instance i runs over its first lengths[i] frames only (0: the plugin did not
+        run: no process, no read, its window clock stands still), b200m_dr14_run_ragged_*."""
         if isinstance(x, np.ndarray) or not x.is_cuda:
             p, s, rows, n = _host_planar(x)
             assert rows == self.n_inst * self.nchan
-            _ck(lib().b200m_dr14_run_host(self.h, p, s, n))
+            if lengths is None:
+                _ck(lib().b200m_dr14_run_host(self.h, p, s, n))
+            else:
+                ln = _lengths(lengths, self.n_inst)
+                _ck(lib().b200m_dr14_run_ragged_host(self.h, p, s, n, _np_ptr(ln)))
         else:
             p, s, rows, n = _dev_ptr(x)
             assert rows == self.n_inst * self.nchan
-            _ck(lib().b200m_dr14_run_device(self.h, p, s, n, _stream_ptr(stream)))
+            if lengths is None:
+                _ck(lib().b200m_dr14_run_device(self.h, p, s, n, _stream_ptr(stream)))
+            else:
+                ln = _lengths(lengths, self.n_inst)
+                _ck(lib().b200m_dr14_run_ragged_device(self.h, p, s, n, _np_ptr(ln), _stream_ptr(stream)))
 
     def run_ptr(self, ptr, stride, nfram, stream=None):
         _ck(lib().b200m_dr14_run_device(self.h, C.c_void_p(ptr), stride, nfram, _stream_ptr(stream)))
@@ -969,3 +982,37 @@ def programme_loudness(x, lengths, fsamp=48000.0, nchan=2, gains=None, block=102
     out = {k: np.ascontiguousarray(r[k], np.float32) for k in PROGRAMME_FIELDS}
     out["tp_max"] = tp
     return out
+
+
+def programme_dr14(x, lengths, rate=48000.0, n_channels=2, dr_mode=True, block=1024, device=0):
+    """DR-14 (dr_mode=True) or TPnRMS meter readings of N whole tracks of different lengths, in one bank.
+
+    x: rows i * n_channels + c of track i, track i valid for its first lengths[i] frames: a [N * n_channels, >= max(lengths)]
+    float32 numpy array / CPU tensor (host path) or CUDA tensor (device path), or a callable f(offset, nfram) that returns frames
+    offset .. offset + nfram - 1 of every row as such an array (tracks produced block by block).  Frames past a track's length are
+    never read into a result.  The tracks are fed in blocks of `block` frames: block k has nfram = min(block, longest remaining)
+    and track i's length in it is clamp(lengths[i] - k * block, 0, block) (DR14.run with lengths), so track i's numbers are
+    bit-identical to a private dr14 plugin instance fed the track in blocks of `block` frames with a short last block.
+    A track's DR counts only its whole 3 s windows (rintf (3 * rate) + 1 frames each), as the reference's does: a partial last
+    window is never scored, and a track shorter than three windows reads dr 21 ("not valid").  dr_mode needs rate >= 2731 Hz
+    (b200m_dr14_create: a window longer than the largest block).
+    Returns a DR14_RESULT_DTYPE array of N: each track's b200m_dr14_result after its last frame (all zero for an empty track,
+    which never runs)."""
+    ln = np.asarray(lengths, np.int64).ravel()
+    n = ln.size
+    if n == 0:
+        raise B200MError("no tracks")
+    if ln.min() < 0:
+        raise B200MError("lengths must be frame counts >= 0")
+    if not 1 <= int(block) <= 8192:
+        raise B200MError("block must be 1..8192 frames")
+    bank = DR14(n, n_channels, rate, dr_mode, device)
+    try:
+        total = int(ln.max())
+        for off in range(0, total, int(block)):
+            nfram = min(int(block), total - off)
+            xb = x(off, nfram) if callable(x) else x[:, off:off + nfram]
+            bank.run(xb, lengths=np.clip(ln - off, 0, nfram))
+        return bank.results()
+    finally:
+        bank.close()

@@ -45,13 +45,17 @@ struct Dr14State {
     const float* cd;                                           // db_to_coeff ((b - 7999) / 100.0) for b = 0..7999, host libm
 };
 
-// dr14_calc_rms_score (:285-352) of the instances whose window closed in this block; one warp per instance
-__global__ void dr14_score_kernel (int n_inst, int nch, float n_sample_cnt_f, Dr14State s, TpkDr dr, int nfram)
+// dr14_calc_rms_score (:285-352) of the instances whose window closed in this block; one warp per instance.
+// RAG: a ragged block, instance i ran over its first rlen[i] frames: its window closed only if the cut lies before that.
+template <bool RAG = false>
+__global__ void dr14_score_kernel (int n_inst, int nch, float n_sample_cnt_f, Dr14State s, TpkDr dr, int nfram, const uint32_t* __restrict__ rlen)
 {
     const int inst = (blockIdx.x * blockDim.x + threadIdx.x) >> 5, lane = threadIdx.x & 31;
     if (inst >= n_inst) return;
     const int ch0 = inst * nch;
-    if (tpk_dr_cut (dr, inst, nfram) < 0) return;             // no window end in this block: emit_* still hold an older window's
+    const int cut = tpk_dr_cut (dr, inst, nfram);
+    if (cut < 0) return;                                       // no window end in this block: emit_* still hold an older window's
+    if (RAG && cut >= (int)rlen[inst]) return;                 // ... or none before the instance's last frame
     if (!s.emit_valid[ch0]) return;                            // silent window: nothing recorded (:287-297)
     unsigned long long nf = 0;
     if (lane == 0) { nf = s.numfrag[inst] + 1; s.numfrag[inst] = nf; }
@@ -97,12 +101,14 @@ __global__ void dr14_score_kernel (int n_inst, int nch, float n_sample_cnt_f, Dr
     }
 }
 
-// read() results -> port values (:418-462); one thread per instance
+// read() results -> port values (:418-462); one thread per instance.  RAG: an instance with rlen 0 did not run (row and hold stay).
+template <bool RAG = false>
 __global__ void dr14_ports_kernel (int n_inst, int nch, int dr_mode, const b200m_tpk_result* __restrict__ res, Dr14State s,
-                                   b200m_dr14_result* __restrict__ out)
+                                   b200m_dr14_result* __restrict__ out, const uint32_t* __restrict__ rlen)
 {
     const int inst = blockIdx.x * blockDim.x + threadIdx.x;
     if (inst >= n_inst) return;
+    if (RAG && rlen[inst] == 0) return;
     b200m_dr14_result o;
     memset (&o, 0, sizeof (o));
     float dr_total = 0.0f; int dr_valid = 0;
@@ -130,6 +136,14 @@ __global__ void dr14_ports_kernel (int n_inst, int nch, int dr_mode, const b200m
     }
     o.block_count = __double2float_rn (__dmul_rn (3.0, (double)s.numfrag[inst]));     // 3.0 * num_fragments
     out[inst] = o;
+}
+
+// a ragged block moves every instance's window clock on by its own length, not by the block's nfram: its phase (the bank time of
+// its last reset, mod w) advances by nfram - rlen[i].  Queued behind the block's process() and scoring kernels, which read the old one.
+__global__ void dr14_ragged_clock_kernel (int n_inst, const uint32_t* __restrict__ rlen, uint32_t nfram, uint32_t w, uint32_t* __restrict__ phase)
+{
+    const int i = blockIdx.x * blockDim.x + threadIdx.x;
+    if (i < n_inst) phase[i] = (phase[i] + (nfram - rlen[i]) % w) % w;
 }
 
 // reset_peaks (:246-262) of the instances inst[0 .. n_sel) (inst == nullptr: instances 0 .. n_sel - 1): their next window
@@ -163,6 +177,11 @@ struct b200m_dr14 {
     float *d_rms_sum = nullptr, *d_peak_cur = nullptr, *d_cd = nullptr;
     Dr14State st{}; b200m_dr14_result* d_out = nullptr;
     cudaStream_t own = nullptr; HostStage stage; bool last_host = false;
+    // a ragged block (b200m_dr14_run_ragged_*): per-instance lengths and K-meter _fall values on the device ([n_inst] each), pinned
+    // staging for their upload (two slots: the copy from one may still be queued while the next block fills the other), and the
+    // _fall of every length met so far (host libm, tpk_km_fall); allocated with the first ragged block
+    uint32_t* d_len = nullptr; uint32_t* h_len[2] = {nullptr, nullptr}; cudaEvent_t ev_len[2] = {nullptr, nullptr}; int len_slot = 0;
+    std::vector<float> fall; std::vector<uint8_t> fall_ok;
 };
 
 // reset_peaks of the instances d_inst[0 .. n_sel) (d_inst == nullptr: every instance), clear: and b200m_tpk_clear of their
@@ -193,8 +212,53 @@ static bool dr14_closes (const b200m_dr14* h, uint32_t nfram)
     return b > h->w && h->phases.begin ()->first < b - h->w;
 }
 
-static int dr14_run (b200m_dr14* h, const float* d_in, size_t stride, uint32_t nfram, cudaStream_t st)
+// 1 if some len[i] differs from nfram, 0 if none does (or len is NULL: the plain call), B200M_E_INVAL if one exceeds nfram
+static int dr14_ragged_check (const b200m_dr14* h, uint32_t nfram, const uint32_t* len)
 {
+    if (!len) return 0;
+    bool rag = false;
+    for (uint32_t i = 0; i < h->n_inst; ++i) {
+        if (len[i] > nfram) return set_err (B200M_E_INVAL, "len[%u] = %u exceeds nfram = %u", i, len[i], nfram);
+        rag |= len[i] != nfram;
+    }
+    return rag ? 1 : 0;
+}
+
+// enqueue the upload of a ragged block's lengths and their K-meter _fall values on `st`
+static int dr14_upload_len (b200m_dr14* h, const uint32_t* len, cudaStream_t st)
+{
+    const size_t n = h->n_inst;
+    cudaError_t e = cudaSuccess;
+    if (!h->d_len) e = cudaMalloc ((void**)&h->d_len, 2 * n * sizeof (uint32_t));
+    for (int s = 0; s < 2; ++s) {
+        if (e == cudaSuccess && !h->h_len[s]) e = cudaHostAlloc ((void**)&h->h_len[s], 2 * n * sizeof (uint32_t), cudaHostAllocDefault);
+        if (e == cudaSuccess && !h->ev_len[s]) e = cudaEventCreateWithFlags (&h->ev_len[s], cudaEventDisableTiming);
+    }
+    if (h->fall.empty ()) { h->fall.assign (B200M_MAX_BLOCK + 1, 0.0f); h->fall_ok.assign (B200M_MAX_BLOCK + 1, 0); }
+    // pinned staging: the copy is truly asynchronous, and the slot's previous copy has run before it is overwritten
+    const int s = h->len_slot; h->len_slot ^= 1;
+    if (e == cudaSuccess) e = cudaEventSynchronize (h->ev_len[s]);
+    if (e != cudaSuccess) return cuda_fail (e, "dr14_upload_len", __FILE__, __LINE__);
+    uint32_t* hl = h->h_len[s];
+    float* hf = reinterpret_cast<float*> (hl + n);
+    memcpy (hl, len, n * sizeof (uint32_t));
+    for (size_t i = 0; i < n; ++i) {
+        const uint32_t L = len[i];
+        if (!h->fall_ok[L]) { h->fall[L] = tpk_km_fall (h->tpk, L); h->fall_ok[L] = 1; }      // once per length
+        hf[i] = h->fall[L];
+    }
+    e = cudaMemcpyAsync (h->d_len, hl, 2 * n * sizeof (uint32_t), cudaMemcpyHostToDevice, st);
+    if (e == cudaSuccess) e = cudaEventRecord (h->ev_len[s], st);
+    if (e != cudaSuccess) return cuda_fail (e, "dr14_upload_len", __FILE__, __LINE__);
+    return 0;
+}
+
+// len (host, every entry <= nfram, some != nfram: dr14_ragged_check): a ragged block, instance i runs over its first len[i] frames;
+// nullptr: every instance runs nfram
+static int dr14_run (b200m_dr14* h, const float* d_in, size_t stride, uint32_t nfram, cudaStream_t st, const uint32_t* len = nullptr)
+{
+    if (len) if (int rc = dr14_upload_len (h, len, st)) return rc;
+    const uint32_t* d_len = len ? h->d_len : nullptr;
     bool closes = false;
     TpkDr dr = {};
     if (h->dr_mode) {
@@ -204,15 +268,26 @@ static int dr14_run (b200m_dr14* h, const float* d_in, size_t stride, uint32_t n
         tpk_set_dr (h->tpk, &dr);
         h->tmod = (uint32_t)((h->tmod + (uint64_t)nfram) % h->w);
     }
-    int rc = b200m_tpk_process_device (h->tpk, d_in, stride, nfram, B200M_TP_MODE_PROCESS, st);
+    int rc = len ? tpk_process_ragged (h->tpk, d_in, stride, nfram, st, d_len, reinterpret_cast<const float*> (d_len + h->n_inst), h->nch)
+                 : b200m_tpk_process_device (h->tpk, d_in, stride, nfram, B200M_TP_MODE_PROCESS, st);
     if (rc) return rc;
+    const unsigned gs = (h->n_inst * 32 + 127) / 128, gp = (h->n_inst + 127) / 128;
     if (closes) {
-        dr14_score_kernel<<<(h->n_inst * 32 + 127) / 128, 128, 0, st>>> ((int)h->n_inst, (int)h->nch, (float)h->n_sample_cnt, h->st, dr, (int)nfram);
+        if (len) dr14_score_kernel<true><<<gs, 128, 0, st>>> ((int)h->n_inst, (int)h->nch, (float)h->n_sample_cnt, h->st, dr, (int)nfram, d_len);
+        else dr14_score_kernel<<<gs, 128, 0, st>>> ((int)h->n_inst, (int)h->nch, (float)h->n_sample_cnt, h->st, dr, (int)nfram, nullptr);
         B200M_LAUNCHED (1);
     }
-    if ((rc = b200m_tpk_read_device (h->tpk, st))) return rc;
-    dr14_ports_kernel<<<(h->n_inst + 127) / 128, 128, 0, st>>> ((int)h->n_inst, (int)h->nch, h->dr_mode, tpk_device_results (h->tpk), h->st, h->d_out);
+    if ((rc = len ? tpk_read_ragged (h->tpk, st, d_len, h->nch) : b200m_tpk_read_device (h->tpk, st))) return rc;
+    if (len) dr14_ports_kernel<true><<<gp, 128, 0, st>>> ((int)h->n_inst, (int)h->nch, h->dr_mode, tpk_device_results (h->tpk), h->st, h->d_out, d_len);
+    else dr14_ports_kernel<<<gp, 128, 0, st>>> ((int)h->n_inst, (int)h->nch, h->dr_mode, tpk_device_results (h->tpk), h->st, h->d_out, nullptr);
     B200M_LAUNCHED (1);
+    if (len && h->dr_mode) {
+        // each instance's clock ran len[i] frames: move the phases on the device and in the host mirror
+        dr14_ragged_clock_kernel<<<gp, 128, 0, st>>> ((int)h->n_inst, d_len, nfram, h->w, h->st.phase);
+        B200M_LAUNCHED (1);
+        for (uint32_t i = 0; i < h->n_inst; ++i)
+            if (len[i] != nfram) dr14_set_phase (h, i, (h->phase[i] + (nfram - len[i]) % h->w) % h->w);
+    }
     B200M_CUDA (cudaGetLastError ());
     return 0;
 }
@@ -276,6 +351,8 @@ int b200m_dr14_destroy (b200m_dr14* h)
     void* ps[] = {h->d_rms_sum, h->d_peak_cur, h->st.emit_rms, h->st.emit_peak, h->st.emit_valid, h->st.peak_hist, h->st.m_rms, h->st.m_peak,
                   h->st.m_dbtp, h->st.numfrag, h->st.phase, h->d_sel, h->st.hist, h->d_cd, h->d_out};
     for (void* p : ps) cudaFree (p);
+    cudaFree (h->d_len);
+    for (int s = 0; s < 2; ++s) { if (h->h_len[s]) cudaFreeHost (h->h_len[s]); if (h->ev_len[s]) cudaEventDestroy (h->ev_len[s]); }
     h->stage.release ();
     if (h->own) cudaStreamDestroy (h->own);
     delete h;
@@ -302,6 +379,33 @@ int b200m_dr14_run_host (b200m_dr14* h, const float* in, size_t stride, uint32_t
                                    cudaMemcpyHostToDevice, h->own));
     h->last_host = true;
     return dr14_run (h, h->stage.d, h->stage.cap, nfram, h->own);
+}
+
+int b200m_dr14_run_ragged_device (b200m_dr14* h, const float* d_in, size_t stride, uint32_t nfram, const uint32_t* len, void* stream)
+{
+    if (int rc = check_block_args (h, d_in, stride, nfram)) return rc;
+    const int rag = dr14_ragged_check (h, nfram, len);
+    if (rag < 0) return rag;
+    if (!rag) return b200m_dr14_run_device (h, d_in, stride, nfram, stream);       // every length is nfram: the plain call
+    DeviceGuard g (h->device);
+    B200M_LEAVE_HOST_PATH (h);
+    return dr14_run (h, d_in, stride, nfram, (cudaStream_t)stream, len);
+}
+
+int b200m_dr14_run_ragged_host (b200m_dr14* h, const float* in, size_t stride, uint32_t nfram, const uint32_t* len)
+{
+    if (int rc = check_block_args (h, in, stride, nfram)) return rc;
+    const int rag = dr14_ragged_check (h, nfram, len);
+    if (rag < 0) return rag;
+    if (!rag) return b200m_dr14_run_host (h, in, stride, nfram);
+    DeviceGuard g (h->device);
+    B200M_ENTER_HOST_PATH (h);
+    const size_t n_ch = (size_t)h->n_inst * h->nch;
+    if (h->stage.ensure (n_ch, nfram)) return set_err (B200M_E_NOMEM, "staging buffer allocation failed");
+    B200M_CUDA (cudaMemcpy2DAsync (h->stage.d, h->stage.cap * sizeof (float), in, stride * sizeof (float), (size_t)nfram * sizeof (float), n_ch,
+                                   cudaMemcpyHostToDevice, h->own));
+    h->last_host = true;
+    return dr14_run (h, h->stage.d, h->stage.cap, nfram, h->own, len);
 }
 
 int b200m_dr14_reset (b200m_dr14* h, void* stream)              // reset_peaks (:241-258), every instance

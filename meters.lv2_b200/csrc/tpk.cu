@@ -415,11 +415,25 @@ B200M_DEV void r128_group_hold (const R128Hold& r, const TpkState& st, float mm,
 // the HOLD instantiation for a launch: 2 (the stereo code) when the launch has no EBUr128 epilogue
 static inline int r128_hold_of (const R128Hold& r) { return !r.tpmax ? 2 : r.lin ? 0 : r.nch; }
 
-template <int CH, int TC, bool TP, bool TPMAX, bool KM, bool IMM, bool DR, bool FMA = false>
+// A ragged process() block (RAG, the DR-14 bank's b200m_dr14_run_ragged_*): row c belongs to instance c / nch, which runs
+// process() over its first len[c / nch] <= nfram frames only; fall[c / nch] is Kmeterdsp's _fall for that length (host libm).
+struct TpkRag {
+    const uint32_t* len; const float* fall; int nch;
+};
+
+// RAG (exact process() with the K-meter, tpk_kernel<16, 64, true, false, true, IMM, DR, false, true>): every row stops at its own
+// length rl.  The FIR phase runs as for a plain block: it is causal, so the outputs before rl never see the unread frames, and
+// unread frames can only make the silence and phase-0 elision guards more conservative (row_absmax propagates NaN, Inf and large
+// values fail phase0_is_delay, a non-zero frame fails the silence vote), never change an output.  The ballistics lanes stay in
+// their loop past rl (its z1 + z2 shuffle needs the whole warp) with their state frozen; the K-meter lanes drop rl mod 4 samples
+// and use rl for _fpp and the hold count; the DR lanes add only samples before rl and close a window only at a cut before rl.
+// A row with rl == 0 did not run: no end-of-block update.  Its next history is the 48 samples before rl (old history first).
+template <int CH, int TC, bool TP, bool TPMAX, bool KM, bool IMM, bool DR, bool FMA = false, bool RAG = false>
 __global__ void __launch_bounds__ (TPK_THREADS)
 tpk_kernel (const float* __restrict__ in, size_t stride, int c_first, int n_chan, int nfram, int aligned, int elide0, TpkParams prm,
-            TpkState st, float* __restrict__ dbg, R128Hold r128, TpkDr dr)
+            TpkState st, float* __restrict__ dbg, R128Hold r128, TpkDr dr, TpkRag rag)
 {
+    static_assert (!RAG || (CH == 16 && TP && !TPMAX && KM && !FMA), "the ragged form is the exact 16-channel process() kernel");
     // processes channels [c_first, n_chan): `n_chan` is the END of the slice (absolute channel index)
     constexpr int XP = TpkGeom<CH, TC, TP && !TPMAX>::XP;   // x row pitch (floats): 16-byte multiple
     constexpr int OP = 4 * TC + 4;                // |out| row pitch
@@ -501,6 +515,8 @@ tpk_kernel (const float* __restrict__ in, size_t stride, int c_first, int n_chan
     const int srow = wbase + (is_tp ? tch : lane);         // tile row of this lane's serial channel
     const int chs = min (c0 + srow, n_chan - 1);
     const bool live = (c0 + srow) < n_chan;
+    int rl = nfram;                                                      // this lane's serial row ends here
+    if constexpr (RAG) rl = (int)rag.len[(unsigned)chs / (unsigned)rag.nch];
     float z = 0, m = 0, p = 0, wf = 0; int res = 0;
     float kz1 = 0, kz2 = 0, kt = 0;
     if (is_tp) {
@@ -523,11 +539,16 @@ tpk_kernel (const float* __restrict__ in, size_t stride, int c_first, int n_chan
     const bool dr_live = dr_warp && lane < 16 && (c0 + drow) < n_chan;
     float drs = 0, drp = 0; int dcut = -1;
     if (dr_warp) { drs = dr.rms_sum[dch]; drp = dr.peak_cur[dch]; dcut = tpk_dr_cut (dr, dch / dr.nch, nfram); }
+    int drl = nfram;
+    if constexpr (RAG) {
+        drl = (int)rag.len[(unsigned)dch / (unsigned)rag.nch];
+        if (dcut >= drl) dcut = -1;                                       // the window ends past this instance's last frame
+    }
     // the first window end of the warp's lanes in this block (each lane's instance has its own); the warp reaches it together, so
     // the silence test's partner exchange is a convergent shuffle
     int wcut = dr_warp ? __reduce_min_sync (0xffffffffu, dcut >= 0 ? dcut : INT_MAX) : INT_MAX;
     float vmax = 0.0f;                                                    // process_max: plain running max (:109-122), per FIR lane
-    const int km_n = (nfram / 4) * 4;                                     // "n /= 4" drops n mod 4 samples (:79)
+    const int km_n = (rl / 4) * 4;                                        // "n /= 4" drops n mod 4 samples (:79)
 
     for (int c = 0; c < nchunks; ++c) {
         const int buf = c & 1;
@@ -539,6 +560,16 @@ tpk_kernel (const float* __restrict__ in, size_t stride, int c_first, int n_chan
         for (int idx = tid; idx < CH * 48; idx += TPK_THREADS) {
             const int r = idx / 48, j = idx % 48;
             xs[buf ^ 1][r][j] = xs[buf][r][len + j];
+        }
+        if constexpr (RAG) {
+            // next history of the rows that end in this chunk (s0 < L <= s0 + len; L == 0: chunk 0, the old history itself).  Every
+            // thread read the old history into xs[0] before the barrier above, so st.hist can be overwritten now.
+            for (int idx = tid; idx < CH * 48; idx += TPK_THREADS) {
+                const int r = idx / 48, j = idx % 48;
+                if (c0 + r >= n_chan) continue;
+                const int L = (int)rag.len[(unsigned)(c0 + r) / (unsigned)rag.nch];
+                if (L > 0 ? (L > s0 && L <= s0 + len) : c == 0) st.hist[(size_t)(c0 + r) * 48 + j] = xs[buf][r][L - s0 + j];
+            }
         }
         load_chunk (c + 1, buf ^ 1);
 
@@ -636,7 +667,16 @@ tpk_kernel (const float* __restrict__ in, size_t stride, int c_first, int n_chan
                 const float t = __fadd_rn (z, __shfl_xor_sync (0xffffffffu, z, 16));    // z1 + z2
                 m = fmaxf (m, t);                           // == `if (t > m) m = t`: m is never NaN, a NaN t leaves it unchanged
             };
-            const int ng = len >> 2;
+            // RAG: input sample j of the chunk counts while j < e; past it the lane (and its partner filter: same row, same e) steps on
+            // frozen, so the warp stays converged on the shuffle.  The warp stops at the last end of its rows in this chunk.
+            int e = len, ew = len;
+            if constexpr (RAG) { e = max (0, min (len, rl - s0)); ew = __reduce_max_sync (0xffffffffu, e); }
+            auto step_rag = [&] (const float4 v4, const int j) {
+                const float z0 = z, p0 = p, m0 = m;
+                step (v4);
+                if (j >= e) { z = z0; p = p0; m = m0; }
+            };
+            const int ng = ew >> 2;
             // two register sets in turn (no copies): group g + 1 is loaded while group g is on the chain
             float4 va[4], vb[4];
 #pragma unroll
@@ -647,15 +687,17 @@ tpk_kernel (const float* __restrict__ in, size_t stride, int c_first, int n_chan
 #pragma unroll
                 for (int i = 0; i < 4; ++i) vb[i] = b4[i * GPC + g1];
 #pragma unroll
-                for (int i = 0; i < 4; ++i) step (va[i]);
+                for (int i = 0; i < 4; ++i) { if constexpr (RAG) step_rag (va[i], 4 * g + i); else step (va[i]); }
                 if (g + 1 < ng) {
 #pragma unroll
                     for (int i = 0; i < 4; ++i) va[i] = b4[i * GPC + g2];
 #pragma unroll
-                    for (int i = 0; i < 4; ++i) step (vb[i]);
+                    for (int i = 0; i < 4; ++i) { if constexpr (RAG) step_rag (vb[i], 4 * g + 4 + i); else step (vb[i]); }
                 }
             }
-            for (int j = 4 * ng; j < len; ++j) step (b4[(j & 3) * GPC + (j >> 2)]);       // a block that does not end on a multiple of 4
+            for (int j = 4 * ng; j < ew; ++j) {                // a block that does not end on a multiple of 4
+                if constexpr (RAG) step_rag (b4[(j & 3) * GPC + (j >> 2)], j); else step (b4[(j & 3) * GPC + (j >> 2)]);
+            }
         }
         if (is_km) {
             // kmeterdsp.cc:80-97: z1 every sample, z2 every 4th; the block's last n%4 samples are ignored
@@ -679,10 +721,17 @@ tpk_kernel (const float* __restrict__ in, size_t stride, int c_first, int n_chan
         }
         if (dr_warp) {
             const float* xr = &xs[buf][drow][48];
-            for (int j = 0; j < len; ++j) {
+            // RAG: samples count below the row's end; the warp walks to the last end of its rows (every valid cut lies before it)
+            int de = len, dew = len;
+            if constexpr (RAG) { de = max (0, min (len, drl - s0)); dew = __reduce_max_sync (0xffffffffu, de); }
+            for (int j = 0; j < dew; ++j) {
                 const float v = xr[j];
-                drs = __fadd_rn (drs, __fmul_rn (v, v));
-                drp = drp > v ? drp : v;                    // MAX (peak_cur, v) on the RAW sample (:408), NaN-transparent like the macro
+                bool on = true;
+                if constexpr (RAG) on = j < de;
+                if (on) {
+                    drs = __fadd_rn (drs, __fmul_rn (v, v));
+                    drp = drp > v ? drp : v;                // MAX (peak_cur, v) on the RAW sample (:408), NaN-transparent like the macro
+                }
                 if (s0 + j == wcut) {                        // warp-uniform: the whole warp exchanges, the lanes whose window ends here close
                     const float other = dr.nch == 2 ? __shfl_xor_sync (0xffffffffu, drs, 1) : drs;
                     if (dcut == wcut) {                      // ++scnt > slmt (:410): this lane's 3 s window closes after this sample
@@ -704,7 +753,7 @@ tpk_kernel (const float* __restrict__ in, size_t stride, int c_first, int n_chan
     if (dr_live) { dr.rms_sum[dch] = drs; dr.peak_cur[dch] = drp; }
 
     // ---- end of block --------------------------------------------------------------------
-    if (TP) {
+    if (TP && !RAG) {                                       // (RAG: written in the chunk loop)
         // new history = the 48 samples that precede the next block (left in xs[nchunks&1][.][0..47])
         const int hb = nchunks & 1;
         for (int idx = tid; idx < CH * 48; idx += TPK_THREADS) {
@@ -749,7 +798,9 @@ tpk_kernel (const float* __restrict__ in, size_t stride, int c_first, int n_chan
             }
         }
     }
-    if (is_tp && live) {
+    bool ran = true;                                        // RAG: rl == 0, the row did not run
+    if constexpr (RAG) ran = rl > 0;
+    if (is_tp && live && ran) {
         if (filt) st.tp_z2[chs] = __fadd_rn (z, 1e-20f);    // :86-87
         else {
             st.tp_z1[chs] = __fadd_rn (z, 1e-20f);
@@ -761,7 +812,7 @@ tpk_kernel (const float* __restrict__ in, size_t stride, int c_first, int n_chan
             }
         }
     }
-    if (is_km && live) {
+    if (is_km && live && ran) {
         if (isnan (kz1)) kz1 = 0;                           // :101-103
         if (isnan (kz2)) kz2 = 0;
         if (!finitef_ (kt)) kt = 0;
@@ -771,12 +822,14 @@ tpk_kernel (const float* __restrict__ in, size_t stride, int c_first, int n_chan
         const float t = __fsqrt_rn (kt);
         if (st.km_flag[chs]) { st.km_rms[chs] = s; st.km_flag[chs] = 0; }
         else if (s > st.km_rms[chs]) st.km_rms[chs] = s;
+        float fall = prm.fall;                              // _fall and _fpp of this row's n (:65-70)
+        if constexpr (RAG) fall = rag.fall[(unsigned)chs / (unsigned)rag.nch];
         float pk = st.km_peak[chs]; int cnt = st.km_cnt[chs];
         if (t >= pk) { pk = t; cnt = prm.hold; }            // :125-139
-        else if (cnt > 0) cnt -= nfram;
-        else { pk = __fmul_rn (pk, prm.fall); pk = __fadd_rn (pk, 1e-10f); }
+        else if (cnt > 0) cnt -= rl;
+        else { pk = __fmul_rn (pk, fall); pk = __fadd_rn (pk, 1e-10f); }
         st.km_peak[chs] = pk; st.km_cnt[chs] = cnt;
-        st.km_fall[chs] = prm.fall; st.km_fpp[chs] = nfram;
+        st.km_fall[chs] = fall; st.km_fpp[chs] = rl;
     }
 }
 
@@ -1999,10 +2052,14 @@ r128_fused_kernel (const __grid_constant__ CUtensorMap tmap, const float* __rest
 // bit-exact but slower: 48 KB of shared memory and 80 registers x 192 threads cut residency to 4 CTAs/SM, and three role
 // bodies (26 KB FIR + ballistics + K-meter) overflow the instruction cache.
 
-__global__ void tpk_read_kernel (int n_chan, uint32_t flags, TpkState st, b200m_tpk_result* __restrict__ out)
+// RAG: after a ragged process() block, channel i belongs to instance i / per; an instance with rlen 0 did not run, so it was not
+// read either (_res, _flag and its result row stay)
+template <bool RAG = false>
+__global__ void tpk_read_kernel (int n_chan, uint32_t flags, TpkState st, b200m_tpk_result* __restrict__ out, const uint32_t* __restrict__ rlen, int per)
 {
     const int i = blockIdx.x * blockDim.x + threadIdx.x;
     if (i >= n_chan) return;
+    if (RAG && rlen[(unsigned)i / (unsigned)per] == 0) return;
     b200m_tpk_result r = out[i];
     if (flags & B200M_TPK_TRUEPEAK) { r.tp_m = st.tp_m[i]; r.tp_p = st.tp_p[i]; st.tp_res[i] = 1; }     // read(m,p) :133-138
     if (flags & B200M_TPK_KMETER)   { r.km_rms = st.km_rms[i]; r.km_peak = st.km_peak[i]; st.km_flag[i] = 1; }  // kmeterdsp.cc:150-155
@@ -2086,6 +2143,8 @@ static void tpk_design (float fsamp, TpkParams& prm, float* ctab)
 
 namespace b200m {
 void tpk_set_dr (b200m_tpk* h, const TpkDr* dr) { h->dr_on = dr != nullptr; if (dr) h->dr = *dr; }
+// Kmeterdsp::process (:65-70): the per-period fallback multiplier of an n-frame call, host libm
+float tpk_km_fall (const b200m_tpk* h, uint32_t n) { return powf (10.0f, -0.05f * 15.0f * ((float)(int)n / h->fsamp)); }
 const b200m_tpk_result* tpk_device_results (b200m_tpk* h) { return h->d_res; }
 int tpk_reset_inst (b200m_tpk* h, const uint32_t* d_inst, uint32_t n_sel, uint32_t per, bool clear, cudaStream_t st)
 {
@@ -2123,7 +2182,7 @@ int tpk_process_sliced (b200m_tpk* h, const float* d_in, size_t stride, uint32_t
     const bool tp = h->flags & B200M_TPK_TRUEPEAK, km = h->flags & B200M_TPK_KMETER;
     TpkParams prm = h->prm;
     // Kmeterdsp::process (:65-70): per-period fallback multiplier, a pure function of n
-    prm.fall = powf (10.0f, -0.05f * 15.0f * ((float)(int)nfram / h->fsamp));
+    prm.fall = tpk_km_fall (h, nfram);
     const int aligned = ((uintptr_t)d_in % 16 == 0) && (stride % 4 == 0);
     dim3 blk (TPK_THREADS);
     bool swap_hist = false;
@@ -2140,9 +2199,9 @@ int tpk_process_sliced (b200m_tpk* h, const float* d_in, size_t stride, uint32_t
         cudaLaunchConfig_t cfg = {};
         cfg.blockDim = blk; cfg.dynamicSmemBytes = 0; cfg.stream = st; cfg.attrs = at; cfg.numAttrs = pdl ? 1 : 0;
 #define TPK_GO(CH, TC, TP, MX, KM, DRM) do { cfg.gridDim = dim3 ((ce - cf + CH - 1) / CH); cfg.dynamicSmemBytes = TpkGeom<CH, TC, (TP) && !(MX)>::BYTES; \
-            if (h->imm && h->fma) B200M_CUDA (cudaLaunchKernelEx (&cfg, tpk_kernel<CH, TC, TP, MX, KM, true, DRM, true>, d_in, stride, cf, ce, (int)nfram, aligned, h->elide0, prm, h->st, h->d_dbg, r128, drp)); \
-            else if (h->imm) B200M_CUDA (cudaLaunchKernelEx (&cfg, tpk_kernel<CH, TC, TP, MX, KM, true, DRM>, d_in, stride, cf, ce, (int)nfram, aligned, h->elide0, prm, h->st, h->d_dbg, r128, drp)); \
-            else B200M_CUDA (cudaLaunchKernelEx (&cfg, tpk_kernel<CH, TC, TP, MX, KM, false, DRM>, d_in, stride, cf, ce, (int)nfram, aligned, h->elide0, prm, h->st, h->d_dbg, r128, drp)); } while (0)
+            if (h->imm && h->fma) B200M_CUDA (cudaLaunchKernelEx (&cfg, tpk_kernel<CH, TC, TP, MX, KM, true, DRM, true>, d_in, stride, cf, ce, (int)nfram, aligned, h->elide0, prm, h->st, h->d_dbg, r128, drp, TpkRag {})); \
+            else if (h->imm) B200M_CUDA (cudaLaunchKernelEx (&cfg, tpk_kernel<CH, TC, TP, MX, KM, true, DRM>, d_in, stride, cf, ce, (int)nfram, aligned, h->elide0, prm, h->st, h->d_dbg, r128, drp, TpkRag {})); \
+            else B200M_CUDA (cudaLaunchKernelEx (&cfg, tpk_kernel<CH, TC, TP, MX, KM, false, DRM>, d_in, stride, cf, ce, (int)nfram, aligned, h->elide0, prm, h->st, h->d_dbg, r128, drp, TpkRag {})); } while (0)
         if (rlen) {
             const int nchunks = ((int)nfram + 255) / 256;
             cfg.gridDim = dim3 ((unsigned)(((ce - cf + 7) / 8) * nchunks));
@@ -2214,7 +2273,7 @@ int tpk_process_sliced (b200m_tpk* h, const float* d_in, size_t stride, uint32_t
             if (km) { if (drp.rms_sum) TPK_GO (64, 32, true, false, true, true); else TPK_GO (64, 32, true, false, true, false); } else TPK_GO (64, 32, true, false, false, false);
         }
         else if (tp) { if (km) { if (drp.rms_sum) TPK_GO (16, 64, true, false, true, true); else TPK_GO (16, 64, true, false, true, false); } else TPK_GO (16, 64, true, false, false, false); }
-        else tpk_kernel<16, 64, false, false, true, false, false><<<(ce - cf + 15) / 16, blk, TpkGeom<16, 64, false>::BYTES, st>>> (d_in, stride, cf, ce, (int)nfram, aligned, h->elide0, prm, h->st, h->d_dbg, r128, drp);
+        else tpk_kernel<16, 64, false, false, true, false, false><<<(ce - cf + 15) / 16, blk, TpkGeom<16, 64, false>::BYTES, st>>> (d_in, stride, cf, ce, (int)nfram, aligned, h->elide0, prm, h->st, h->d_dbg, r128, drp, TpkRag {});
 #undef TPK_GO
         B200M_LAUNCHED (1);
     }
@@ -2228,6 +2287,38 @@ static int tpk_process (b200m_tpk* h, const float* d_in, size_t stride, uint32_t
     const uint32_t bounds[2] = {0, h->n_chan};
     return tpk_process_sliced (h, d_in, stride, nfram, tp_mode, st, 1, bounds, nullptr, R128Hold {}, false, h->dr_on ? &h->dr : nullptr, nullptr);
 }
+
+namespace b200m {
+// A ragged process() block always runs the exact fused kernel in its RAG form, whatever B200M_TPK_SPLIT / B200M_TPK_WIDE /
+// B200M_TPK_DEC would pick for a plain block: only that form stops each row at its own length.
+int tpk_process_ragged (b200m_tpk* h, const float* d_in, size_t stride, uint32_t nfram, cudaStream_t st, const uint32_t* d_len,
+                        const float* d_fall, uint32_t per)
+{
+    if (!(h->flags & B200M_TPK_TRUEPEAK) || !(h->flags & B200M_TPK_KMETER)) return set_err (B200M_E_UNSUPPORTED, "ragged process() needs true peak and the K-meter");
+    if (h->fma) return set_err (B200M_E_UNSUPPORTED, "ragged process() blocks run in exact mode only");
+    const TpkDr drp = h->dr_on ? h->dr : TpkDr {};
+    const TpkRag rag = {d_len, d_fall, (int)per};
+    const int aligned = ((uintptr_t)d_in % 16 == 0) && (stride % 4 == 0);
+    const unsigned grid = (h->n_chan + 15) / 16;
+    const size_t smem = TpkGeom<16, 64, true>::BYTES;
+    const int n = (int)h->n_chan;
+#define TPK_RAG(IMMF, DRF) tpk_kernel<16, 64, true, false, true, IMMF, DRF, false, true><<<grid, TPK_THREADS, smem, st>>> (d_in, stride, 0, n, (int)nfram, aligned, h->elide0, h->prm, h->st, h->d_dbg, R128Hold {}, drp, rag)
+    if (h->imm) { if (drp.rms_sum) TPK_RAG (true, true); else TPK_RAG (true, false); }
+    else { if (drp.rms_sum) TPK_RAG (false, true); else TPK_RAG (false, false); }
+#undef TPK_RAG
+    B200M_LAUNCHED (1);
+    B200M_CUDA (cudaGetLastError ());
+    return 0;
+}
+
+int tpk_read_ragged (b200m_tpk* h, cudaStream_t st, const uint32_t* d_len, uint32_t per)
+{
+    tpk_read_kernel<true><<<(h->n_chan + 255) / 256, 256, 0, st>>> ((int)h->n_chan, h->flags, h->st, h->d_res, d_len, (int)per);
+    B200M_LAUNCHED (1);
+    B200M_CUDA (cudaGetLastError ());
+    return 0;
+}
+}  // namespace b200m
 
 // ---- the EBUr128 cycle's fused K-weighting + true-peak kernel (r128_fused_kernel), launched by the EBU bank in place of K1 (r128.cu)
 // It walks time with one CTA per 128-channel slab, so its cycle costs about the same from a few dozen slabs up to one slab per SM,
@@ -2459,7 +2550,7 @@ int b200m_tpk_read_device (b200m_tpk* h, void* stream)
 {
     if (!h) return set_err (B200M_E_INVAL, "NULL handle");
     DeviceGuard g (h->device);
-    tpk_read_kernel<<<(h->n_chan + 255) / 256, 256, 0, tpk_stream (h, stream)>>> ((int)h->n_chan, h->flags, h->st, h->d_res);
+    tpk_read_kernel<<<(h->n_chan + 255) / 256, 256, 0, tpk_stream (h, stream)>>> ((int)h->n_chan, h->flags, h->st, h->d_res, nullptr, 1);
     B200M_LAUNCHED (1);
     B200M_CUDA (cudaGetLastError ());
     return 0;

@@ -32,5 +32,14 @@ void tpk_set_dr (b200m_tpk* h, const TpkDr* dr);                 // DR accumulat
 const b200m_tpk_result* tpk_device_results (b200m_tpk* h);      // device array filled by b200m_tpk_read_device
 // Kmeterdsp::reset (clear: b200m_tpk_clear) of the channels d_inst[k] * per .. + per - 1, k < n_sel (d_inst == nullptr: every channel)
 int tpk_reset_inst (b200m_tpk* h, const uint32_t* d_inst, uint32_t n_sel, uint32_t per, bool clear, cudaStream_t st);
+// Kmeterdsp's _fall for a process() call of n frames, computed with the host libm as the reference does (kmeterdsp.cc:65-70)
+float tpk_km_fall (const b200m_tpk* h, uint32_t n);
+// A ragged process() block (with the DR accumulation set by tpk_set_dr): channel c belongs to instance c / per, which processes its
+// first d_len[c / per] <= nfram frames; d_fall[c / per] = tpk_km_fall (that length).  Length 0: the channel is not touched.  Exact
+// mode only (B200M_E_UNSUPPORTED in tolerance mode).  Device arrays, read by the kernels queued on `st`.
+int tpk_process_ragged (b200m_tpk* h, const float* d_in, size_t stride, uint32_t nfram, cudaStream_t st, const uint32_t* d_len,
+                        const float* d_fall, uint32_t per);
+// b200m_tpk_read_device after a ragged block: the channels of instances with d_len 0 are not read
+int tpk_read_ragged (b200m_tpk* h, cudaStream_t st, const uint32_t* d_len, uint32_t per);
 
 }  // namespace b200m
