@@ -182,6 +182,19 @@ int b200m_tpk_destroy (b200m_tpk* h);
 /* process() of every enabled meter over one block; tp_mode selects process / process_max */
 int b200m_tpk_process_device (b200m_tpk* h, const float* d_in, size_t stride, uint32_t nfram, uint32_t tp_mode, void* stream);
 int b200m_tpk_process_host (b200m_tpk* h, const float* in, size_t stride, uint32_t nfram, uint32_t tp_mode);
+/* Ragged process() blocks: channel i runs TruePeakdsp::process (:41-99) and Kmeterdsp::process (kmeterdsp.cc:65-140) over the first
+ * len[i] <= nfram frames of its row only, bit-identical to a private meter fed only those frames.  len: host array of n_chan.
+ * - Frames at or after len[i] may hold anything, NaN and Inf included: they reach no state and no reading.
+ * - len[i] == 0: the channel is not called: no process, no end-of-block scrub or bias; b200m_tpk_read_device after this block leaves
+ *   its reading and read latch alone.
+ * - A length above nfram returns B200M_E_INVAL and enqueues nothing.
+ * - NULL, or every len[i] == nfram, is exactly b200m_tpk_process_* (tp_mode process(): same kernels, launches and bits).
+ * - Controls, path switches and streams are ordered between ragged blocks as between plain ones.
+ * A ragged block always runs the exact 16-channel process() kernel, whatever B200M_TPK_SPLIT, B200M_TPK_WIDE, B200M_TPK_DEC or the
+ * precision mode select for plain blocks: in a B200M_PREC_FMA bank its readings are exact for that block.  Ragged process_max blocks:
+ * b200m_r128_run_ragged_*. */
+int b200m_tpk_process_ragged_device (b200m_tpk* h, const float* d_in, size_t stride, uint32_t nfram, const uint32_t* len, void* stream);
+int b200m_tpk_process_ragged_host (b200m_tpk* h, const float* in, size_t stride, uint32_t nfram, const uint32_t* len);
 /* Arithmetic of the 4x polyphase FIR (zita-resampler/resampler.cc:213-230).
  *   B200M_PREC_EXACT (default): the reference's operation order, unfused -- every float bit-identical to the reference build.
  *   B200M_PREC_FMA: fused multiply-add accumulation using the table's symmetry, phase 0 taken as the pure delay it is to
@@ -345,6 +358,17 @@ int b200m_cor_clear (b200m_cor* h, int32_t inst, void* stream);
  * cycles, in both precision modes.  The mask is uploaded only when it differs from the previous call's. */
 int b200m_cor_process_ctl_device (b200m_cor* h, const float* d_in, size_t stride, uint32_t nfram, const uint8_t* run, void* stream);
 int b200m_cor_process_ctl_host (b200m_cor* h, const float* in, size_t stride, uint32_t nfram, const uint8_t* run);
+/* Ragged blocks: pair i runs Stcorrdsp::process (:47-77) over the first len[i] <= nfram frames of its rows only, as a private
+ * Stcorrdsp fed only those frames (bit-identical in B200M_PREC_EXACT, within 1e-5 in B200M_PREC_FMA).  len: host array of n_inst.
+ * - Frames at or after len[i] may hold anything, NaN and Inf included: they reach no state and no reading.
+ * - len[i] == 0: the pair is not called (exactly the hold of b200m_cor_process_ctl_*, which is this call with run[i] ? nfram : 0).
+ * - A length above nfram returns B200M_E_INVAL and enqueues nothing.
+ * - NULL, or every len[i] == nfram, is exactly b200m_cor_process_* (same kernels, launches and bits).
+ * - The lengths are uploaded only when they differ from the previous call's.
+ * - A bank attached to a phasewheel bank (b200m_pw_attach_cor) returns B200M_E_UNSUPPORTED: the phasewheel ring advances bank-wide.
+ *   b200m_pw_attach_cor (pw, NULL) detaches it. */
+int b200m_cor_process_ragged_device (b200m_cor* h, const float* d_in, size_t stride, uint32_t nfram, const uint32_t* len, void* stream);
+int b200m_cor_process_ragged_host (b200m_cor* h, const float* in, size_t stride, uint32_t nfram, const uint32_t* len);
 /* B200M_PREC_EXACT (default): the five recurrences run serially in time, one lane per pair, bit-identical to the reference.
  * B200M_PREC_FMA: time-parallel evaluation -- the recurrences are linear one-pole filters, so a warp owns ONE pair, its lanes take
  * consecutive time segments and an affine warp scan stitches them: 32x more parallelism for small banks (2048 pairs are 64 warps
@@ -375,6 +399,17 @@ int b200m_ppm_set_gain_inst (b200m_ppm* h, int32_t unit, float db_m, float db_s)
 int b200m_ppm_clear (b200m_ppm* h, int32_t unit, void* stream);
 int b200m_ppm_process_device (b200m_ppm* h, const float* d_in, size_t stride, uint32_t nfram, void* stream);
 int b200m_ppm_process_host (b200m_ppm* h, const float* in, size_t stride, uint32_t nfram);
+/* Ragged blocks: unit u (a meter, or for B200M_PPM_MS a stereo pair and its two meters) runs process() (vumeterdsp.cc:45-77,
+ * iec1ppmdsp.cc / iec2ppmdsp.cc :47-80, msppmdsp.cc:50-118) over the first len[u] <= nfram frames of its rows only, bit-identical to a
+ * private meter fed only those frames.  len: host array of n_units.
+ * - Frames at or after len[u] may hold anything, NaN and Inf included: they reach no state and no reading.
+ * - len[u] == 0: the unit is not called: no clamp, scrub or bias, _res unchanged; b200m_ppm_read_device after this block leaves its
+ *   reading and _res alone.  M/S gains set in between (b200m_ppm_set_gain_inst) apply from the unit's next call, as on a private meter.
+ * - A length above nfram returns B200M_E_INVAL and enqueues nothing.
+ * - NULL, or every len[u] == nfram, is exactly b200m_ppm_process_* (same kernels, launches and bits).
+ * - Controls, path switches and streams are ordered between ragged blocks as between plain ones. */
+int b200m_ppm_process_ragged_device (b200m_ppm* h, const float* d_in, size_t stride, uint32_t nfram, const uint32_t* len, void* stream);
+int b200m_ppm_process_ragged_host (b200m_ppm* h, const float* in, size_t stride, uint32_t nfram, const uint32_t* len);
 int b200m_ppm_read_device (b200m_ppm* h, void* stream);                /* read(): _res = true, value = _g * _m */
 int b200m_ppm_results (b200m_ppm* h, float* out, void* stream);        /* one float per meter */
 int b200m_ppm_state (b200m_ppm* h, float* state4, void* stream);       /* per meter: z1 z2 m res */
@@ -448,6 +483,18 @@ int b200m_spec_process_host (b200m_spec* h, const float* in, size_t stride, uint
  * uploaded, on the call's stream. */
 int b200m_spec_process_ctl_device (b200m_spec* h, const float* d_in, size_t stride, uint32_t nfram, const float* ctl, void* stream);
 int b200m_spec_process_ctl_host (b200m_spec* h, const float* in, size_t stride, uint32_t nfram, const float* ctl);
+/* Ragged blocks: instance i runs spectrum_run (src/spectrumlv2.c:159-257) over the first len[i] <= nfram frames of its rows only, with
+ * its controls ctl[i], as a private plugin instance fed only those frames (ports bit-identical in B200M_PREC_EXACT, within +-1e-4 dB
+ * in B200M_PREC_FMA).  len: host array of n_inst; ctl as for b200m_spec_process_ctl_*.
+ * - Frames at or after len[i] may hold anything, NaN and Inf included: they reach no state and no port.
+ * - len[i] == 0: the instance is not run: its ports, filters and speed / reset handshake state stay, its ctl row is ignored.
+ * - Each instance's `ac` dither phase follows its own frame count.
+ * - A length above nfram returns B200M_E_INVAL and enqueues nothing.
+ * - NULL, or every len[i] == nfram, is exactly b200m_spec_process_ctl_* (same kernels, launches and bits).
+ * - Controls, path switches and streams are ordered between ragged blocks as between plain ones. */
+int b200m_spec_process_ragged_device (b200m_spec* h, const float* d_in, size_t stride, uint32_t nfram, const float* ctl, const uint32_t* len,
+                                      void* stream);
+int b200m_spec_process_ragged_host (b200m_spec* h, const float* in, size_t stride, uint32_t nfram, const float* ctl, const uint32_t* len);
 /* instance inst (-1: all) back to what b200m_spec_create gives (spectrum_instantiate, src/spectrumlv2.c:73-121): filter states,
  * val, max and ports zero, rst_h = -4, spd_h = 1, `ac` restarting with the next frame.  Ordered with the bank's runs on the stream
  * it currently runs on. */

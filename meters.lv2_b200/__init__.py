@@ -72,6 +72,8 @@ _PROTOS = {
     "b200m_tpk_process_device": (C.c_int, [_v, _v, C.c_size_t, C.c_uint32, C.c_uint32, _v]),
     "b200m_tpk_process_host": (C.c_int, [_v, _v, C.c_size_t, C.c_uint32, C.c_uint32]),
     "b200m_tpk_read_device": (C.c_int, [_v, _v]),
+    "b200m_tpk_process_ragged_device": (C.c_int, [_v, _v, C.c_size_t, C.c_uint32, _v, _v]),
+    "b200m_tpk_process_ragged_host": (C.c_int, [_v, _v, C.c_size_t, C.c_uint32, _v]),
     "b200m_selftest_log10f": (C.c_int, [C.c_int, C.c_uint32, C.c_uint32, _v, _v]),
     "b200m_lv2_gon_layout": (C.c_int, [_v, C.c_int]),
     "b200m_ebu_clear": (C.c_int, [_v, C.c_int32, _v]),
@@ -133,6 +135,8 @@ _PROTOS = {
     "b200m_cor_process_host": (C.c_int, [_v, _v, C.c_size_t, C.c_uint32]),
     "b200m_cor_process_ctl_device": (C.c_int, [_v, _v, C.c_size_t, C.c_uint32, _v, _v]),
     "b200m_cor_process_ctl_host": (C.c_int, [_v, _v, C.c_size_t, C.c_uint32, _v]),
+    "b200m_cor_process_ragged_device": (C.c_int, [_v, _v, C.c_size_t, C.c_uint32, _v, _v]),
+    "b200m_cor_process_ragged_host": (C.c_int, [_v, _v, C.c_size_t, C.c_uint32, _v]),
     "b200m_cor_results": (C.c_int, [_v, _v, _v]),
     "b200m_cor_state": (C.c_int, [_v, _v, _v]),
     "b200m_cor_coeffs": (C.c_int, [_v, _v]),
@@ -145,6 +149,8 @@ _PROTOS = {
     "b200m_ppm_clear": (C.c_int, [_v, C.c_int32, _v]),
     "b200m_ppm_process_device": (C.c_int, [_v, _v, C.c_size_t, C.c_uint32, _v]),
     "b200m_ppm_process_host": (C.c_int, [_v, _v, C.c_size_t, C.c_uint32]),
+    "b200m_ppm_process_ragged_device": (C.c_int, [_v, _v, C.c_size_t, C.c_uint32, _v, _v]),
+    "b200m_ppm_process_ragged_host": (C.c_int, [_v, _v, C.c_size_t, C.c_uint32, _v]),
     "b200m_ppm_read_device": (C.c_int, [_v, _v]),
     "b200m_ppm_results": (C.c_int, [_v, _v, _v]),
     "b200m_ppm_state": (C.c_int, [_v, _v, _v]),
@@ -175,6 +181,8 @@ _PROTOS = {
     "b200m_spec_process_host": (C.c_int, [_v, _v, C.c_size_t, C.c_uint32, C.c_float, C.c_float]),
     "b200m_spec_process_ctl_device": (C.c_int, [_v, _v, C.c_size_t, C.c_uint32, _v, _v]),
     "b200m_spec_process_ctl_host": (C.c_int, [_v, _v, C.c_size_t, C.c_uint32, _v]),
+    "b200m_spec_process_ragged_device": (C.c_int, [_v, _v, C.c_size_t, C.c_uint32, _v, _v, _v]),
+    "b200m_spec_process_ragged_host": (C.c_int, [_v, _v, C.c_size_t, C.c_uint32, _v, _v]),
     "b200m_spec_clear": (C.c_int, [_v, C.c_int32, _v]),
     "b200m_spec_results": (C.c_int, [_v, _v, _v]),
     "b200m_spec_state": (C.c_int, [_v, C.c_uint32, _v, _v, _v, _v]),
@@ -454,15 +462,26 @@ class TruePeakKmeter(_Bank):
         self.n_chan, self.flags = n_chan, flags
         _ck(lib().b200m_tpk_create(C.byref(self.h), device, n_chan, fsamp, flags))
 
-    def process(self, x, tp_mode=TP_MODE_PROCESS, stream=None):
+    def process(self, x, tp_mode=TP_MODE_PROCESS, stream=None, lengths=None):
+        """lengths: None, or n_chan frame counts <= nfram (tp_mode process() only): channel i runs over the first lengths[i] frames of
+        its row only (0: it is not called, and the next read() leaves it alone), b200m_tpk_process_ragged_*"""
+        if lengths is not None and tp_mode != TP_MODE_PROCESS:
+            raise B200MError("ragged blocks are process() blocks; ragged process_max runs in EBUr128.run(lengths=)")
+        ln = None if lengths is None else _lengths(lengths, self.n_chan)
         if isinstance(x, np.ndarray) or not x.is_cuda:
             p, s, rows, n = _host_planar(x)
             assert rows == self.n_chan
-            _ck(lib().b200m_tpk_process_host(self.h, p, s, n, tp_mode))
+            if ln is None:
+                _ck(lib().b200m_tpk_process_host(self.h, p, s, n, tp_mode))
+            else:
+                _ck(lib().b200m_tpk_process_ragged_host(self.h, p, s, n, _np_ptr(ln)))
         else:
             p, s, rows, n = _dev_ptr(x)
             assert rows == self.n_chan
-            _ck(lib().b200m_tpk_process_device(self.h, p, s, n, tp_mode, _stream_ptr(stream)))
+            if ln is None:
+                _ck(lib().b200m_tpk_process_device(self.h, p, s, n, tp_mode, _stream_ptr(stream)))
+            else:
+                _ck(lib().b200m_tpk_process_ragged_device(self.h, p, s, n, _np_ptr(ln), _stream_ptr(stream)))
 
     def process_ptr(self, ptr, stride, nfram, tp_mode=TP_MODE_PROCESS, stream=None):
         _ck(lib().b200m_tpk_process_device(self.h, C.c_void_p(ptr), stride, nfram, tp_mode, _stream_ptr(stream)))
@@ -520,21 +539,30 @@ class Stcorrdsp(_Bank):
         self.n_inst = n_inst
         _ck(lib().b200m_cor_create(C.byref(self.h), device, n_inst, int(fsamp), flp, tcf))
 
-    def process(self, x, run=None, stream=None):
-        """run: None (every pair) or n_inst flags; a pair whose flag is 0 is held, its state and reading left as they are"""
+    def process(self, x, run=None, stream=None, lengths=None):
+        """run: None (every pair) or n_inst flags; a pair whose flag is 0 is held, its state and reading left as they are.
+        lengths: None, or n_inst frame counts <= nfram: pair i runs over the first lengths[i] frames of its rows only (0: held),
+        b200m_cor_process_ragged_*; not together with run"""
+        if run is not None and lengths is not None:
+            raise B200MError("pass run or lengths, not both")
         mask = None if run is None else np.ascontiguousarray(run, np.uint8)
         assert mask is None or mask.shape == (self.n_inst,)
+        ln = None if lengths is None else _lengths(lengths, self.n_inst)
         if isinstance(x, np.ndarray) or not x.is_cuda:
             p, s, rows, n = _host_planar(x)
             assert rows == 2 * self.n_inst
-            if mask is None:
+            if ln is not None:
+                _ck(lib().b200m_cor_process_ragged_host(self.h, p, s, n, _np_ptr(ln)))
+            elif mask is None:
                 _ck(lib().b200m_cor_process_host(self.h, p, s, n))
             else:
                 _ck(lib().b200m_cor_process_ctl_host(self.h, p, s, n, _np_ptr(mask)))
         else:
             p, s, rows, n = _dev_ptr(x)
             assert rows == 2 * self.n_inst
-            if mask is None:
+            if ln is not None:
+                _ck(lib().b200m_cor_process_ragged_device(self.h, p, s, n, _np_ptr(ln), _stream_ptr(stream)))
+            elif mask is None:
                 _ck(lib().b200m_cor_process_device(self.h, p, s, n, _stream_ptr(stream)))
             else:
                 _ck(lib().b200m_cor_process_ctl_device(self.h, p, s, n, _np_ptr(mask), _stream_ptr(stream)))
@@ -594,15 +622,24 @@ class NeedleMeters(_Bank):
         """unit (-1: all) back to newly constructed meters (M/S: gains -6 / -6 dB)"""
         _ck(lib().b200m_ppm_clear(self.h, unit, _stream_ptr(stream)))
 
-    def process(self, x, stream=None):
+    def process(self, x, stream=None, lengths=None):
+        """lengths: None, or n_units frame counts <= nfram: unit u (a meter, or an M/S pair) runs over the first lengths[u] frames
+        of its rows only (0: it is not called, and the next read() leaves it alone), b200m_ppm_process_ragged_*"""
+        ln = None if lengths is None else _lengths(lengths, self.n_units)
         if isinstance(x, np.ndarray) or not x.is_cuda:
             p, s, rows, n = _host_planar(x)
             assert rows == self.rows
-            _ck(lib().b200m_ppm_process_host(self.h, p, s, n))
+            if ln is None:
+                _ck(lib().b200m_ppm_process_host(self.h, p, s, n))
+            else:
+                _ck(lib().b200m_ppm_process_ragged_host(self.h, p, s, n, _np_ptr(ln)))
         else:
             p, s, rows, n = _dev_ptr(x)
             assert rows == self.rows
-            _ck(lib().b200m_ppm_process_device(self.h, p, s, n, _stream_ptr(stream)))
+            if ln is None:
+                _ck(lib().b200m_ppm_process_device(self.h, p, s, n, _stream_ptr(stream)))
+            else:
+                _ck(lib().b200m_ppm_process_ragged_device(self.h, p, s, n, _np_ptr(ln), _stream_ptr(stream)))
 
     def read(self, stream=None):
         _ck(lib().b200m_ppm_read_device(self.h, _stream_ptr(stream)))
@@ -754,9 +791,24 @@ class Spectr30(_Bank):
         self.n_inst, self.nchan = n_inst, nchan
         _ck(lib().b200m_spec_create(C.byref(self.h), device, n_inst, nchan, rate))
 
-    def process(self, x, speed=1.0, reset=-4.0, stream=None):
-        """speed / reset: ports 60 / 61, one value for every instance or an array of n_inst (each instance its own)"""
+    def process(self, x, speed=1.0, reset=-4.0, stream=None, lengths=None):
+        """speed / reset: ports 60 / 61, one value for every instance or an array of n_inst (each instance its own).
+        lengths: None, or n_inst frame counts <= nfram: instance i runs over the first lengths[i] frames of its rows only (0: it is
+        not run and its controls are ignored), b200m_spec_process_ragged_*"""
         ctl = None
+        if lengths is not None:
+            ln = _lengths(lengths, self.n_inst)
+            ctl = np.empty((self.n_inst, 2), np.float32)
+            ctl[:, 0] = speed; ctl[:, 1] = reset
+            if isinstance(x, np.ndarray) or not x.is_cuda:
+                p, s, rows, n = _host_planar(x)
+                assert rows == self.n_inst * self.nchan
+                _ck(lib().b200m_spec_process_ragged_host(self.h, p, s, n, _np_ptr(ctl), _np_ptr(ln)))
+            else:
+                p, s, rows, n = _dev_ptr(x)
+                assert rows == self.n_inst * self.nchan
+                _ck(lib().b200m_spec_process_ragged_device(self.h, p, s, n, _np_ptr(ctl), _np_ptr(ln), _stream_ptr(stream)))
+            return
         if np.ndim(speed) or np.ndim(reset):
             ctl = np.empty((self.n_inst, 2), np.float32)
             ctl[:, 0] = speed; ctl[:, 1] = reset

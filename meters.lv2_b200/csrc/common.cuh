@@ -51,6 +51,41 @@ struct HostStage {
 
 int check_block_args (const void* h, const void* in, size_t stride, uint32_t nfram);
 
+// A ragged block (b200m_*_ragged_*): len[i] <= nfram frames for each of n meters or instances.  1 if some len[i] differs from
+// nfram, 0 if none does or len is NULL (the plain call), B200M_E_INVAL if one exceeds nfram (nothing is enqueued then).
+int ragged_check (uint32_t n, uint32_t nfram, const uint32_t* len);
+
+// Upload of a ragged block's per-row words (lengths, and whatever a bank derives from them): a device array and two pinned host
+// slots, allocated with the first ragged block.  The copy from one slot may still be queued while the next block fills the other;
+// stage() waits until the slot's previous copy has run, so a pinned copy is truly asynchronous and never sees its source change.
+struct RaggedLen {
+    uint32_t* d = nullptr; uint32_t* h[2] = {nullptr, nullptr}; cudaEvent_t ev[2] = {nullptr, nullptr}; int slot = 0;
+    // the host slot for the next upload (room for `cap` words, the same every call), or nullptr with the CUDA error in *err
+    uint32_t* stage (size_t cap, cudaError_t* err) {
+        cudaError_t e = cudaSuccess;
+        if (!d) e = cudaMalloc ((void**)&d, cap * sizeof (uint32_t));
+        for (int s = 0; s < 2; ++s) {
+            if (e == cudaSuccess && !h[s]) e = cudaHostAlloc ((void**)&h[s], cap * sizeof (uint32_t), cudaHostAllocDefault);
+            if (e == cudaSuccess && !ev[s]) e = cudaEventCreateWithFlags (&ev[s], cudaEventDisableTiming);
+        }
+        if (e == cudaSuccess) e = cudaEventSynchronize (ev[slot]);
+        *err = e;
+        return e == cudaSuccess ? h[slot] : nullptr;
+    }
+    // enqueue the copy of the first `words` words of the slot stage() returned to d, on `st`; the next stage() takes the other slot
+    cudaError_t upload (size_t words, cudaStream_t st) {
+        cudaError_t e = cudaMemcpyAsync (d, h[slot], words * sizeof (uint32_t), cudaMemcpyHostToDevice, st);
+        if (e == cudaSuccess) e = cudaEventRecord (ev[slot], st);
+        slot ^= 1;
+        return e;
+    }
+    void release () {
+        if (d) cudaFree (d);
+        for (int s = 0; s < 2; ++s) { if (h[s]) cudaFreeHost (h[s]); if (ev[s]) cudaEventDestroy (ev[s]); h[s] = nullptr; ev[s] = nullptr; }
+        d = nullptr;
+    }
+};
+
 // A bank switches to its own stream with the first *_host call; whatever the caller queued before that (controls on the
 // streams it passed) must not race with it: one device-wide synchronisation at the transition, nothing afterwards.
 #define B200M_ENTER_HOST_PATH(h) do { if (!(h)->last_host) B200M_CUDA (cudaDeviceSynchronize ()); } while (0)

@@ -14,23 +14,27 @@ namespace b200m {
 
 constexpr int COR_T = 32, COR_P = COR_T + 4, COR_STAGES = 4;
 
-// HOLD (b200m_cor_process_ctl_*): pairs with run[i] == 0 are held -- their rows are never loaded and their state and reading are
-// not written back.  The plain process calls and the phasewheel ring feed are the HOLD = false instantiation.
-template <bool HOLD>
+// RAG (b200m_cor_process_ragged_* and b200m_cor_process_ctl_*): pair i runs process() over its first rlen[i] <= nfram frames only.
+// Each lane stops at its own end; the warp stages tiles up to its longest pair.  A pair with rlen[i] == 0 is not called (held): its
+// rows are never loaded and its state and reading are not written back.  The plain process calls and the phasewheel ring feed are
+// the RAG = false instantiation.
+template <bool RAG>
 __global__ void __launch_bounds__ (32)
 cor_kernel (const float* __restrict__ in, size_t stride, int n_inst, int nfram, int aligned, float w1, float w2,
             float* __restrict__ st /* [5][n_inst] */, float* __restrict__ res, float* __restrict__ ring, int N, int rboff,
-            const uint8_t* __restrict__ run)
+            const uint32_t* __restrict__ rlen)
 {
     __shared__ __align__ (16) float tile[COR_STAGES][2][32 * COR_P];
     const int lane = threadIdx.x;
     const int i0 = blockIdx.x * 32;
     const int inst = min (i0 + lane, n_inst - 1);
     const bool live = (i0 + lane) < n_inst;
-    const int ntiles = (nfram + COR_T - 1) / COR_T;
+    const int rl = RAG ? (int)rlen[inst] : nfram;          // this pair's end
+    const int wend = RAG ? __reduce_max_sync (0xffffffffu, rl) : nfram;
+    const int ntiles = (wend + COR_T - 1) / COR_T;
     // bit p: pair i0 + p is held (lanes past the bank repeat its last pair); a warp of held pairs has nothing to do
-    const unsigned held = HOLD ? __ballot_sync (0xffffffffu, !run[inst]) : 0u;
-    if (HOLD && held == 0xffffffffu) return;
+    const unsigned held = RAG ? __ballot_sync (0xffffffffu, rl == 0) : 0u;
+    if (RAG && held == 0xffffffffu) return;
 
     auto issue = [&] (int t) {
         if (t < ntiles) {
@@ -80,7 +84,7 @@ cor_kernel (const float* __restrict__ in, size_t stride, int n_inst, int nfram, 
         const float* pl = tile[t % COR_STAGES][0] + lane * COR_P;
         const float* pr = tile[t % COR_STAGES][1] + lane * COR_P;
         const int len = min (COR_T, nfram - t * COR_T);
-        if (!HOLD && ring && lane < len) {
+        if (!RAG && ring && lane < len) {
             // fused phasewheel feed (b200m_pw_attach_cor): r_buf[(i + n_off) % n_siz] = data[i] (gui/fft.c:302-305) for the 64 rows
             // of this tile, one 128-byte row segment per store instruction
             int o = rboff + t * COR_T + lane; if (o >= N) o -= N;
@@ -90,13 +94,14 @@ cor_kernel (const float* __restrict__ in, size_t stride, int n_inst, int nfram, 
                 ring[((size_t)(i0 + pr_) * 2 + 1) * N + o] = tile[t % COR_STAGES][1][pr_ * COR_P + lane];
             }
         }
+        const int e = RAG ? max (0, min (COR_T, rl - t * COR_T)) : len;       // this pair's samples in the tile
         int j = 0;
-        for (; j + 4 <= len; j += 4) {
+        for (; j + 4 <= e; j += 4) {
             const float4 a = *reinterpret_cast<const float4*> (pl + j);
             const float4 b = *reinterpret_cast<const float4*> (pr + j);
             step (a.x, b.x); step (a.y, b.y); step (a.z, b.z); step (a.w, b.w);
         }
-        for (; j < len; ++j) step (pl[j], pr[j]);
+        for (; j < e; ++j) step (pl[j], pr[j]);
         __syncwarp ();
         issue (t + COR_STAGES - 1);
     }
@@ -104,7 +109,7 @@ cor_kernel (const float* __restrict__ in, size_t stride, int n_inst, int nfram, 
     // end of process(): non-finite scrub, anti-denormal bias on the three products (:65-75)
     zl = scrub (zl); zr = scrub (zr); zlr = scrub (zlr); zll = scrub (zll); zrr = scrub (zrr);
     zlr = __fadd_rn (zlr, 1e-10f); zll = __fadd_rn (zll, 1e-10f); zrr = __fadd_rn (zrr, 1e-10f);
-    if (live && !((held >> lane) & 1)) {
+    if (live && rl > 0) {
         st[0 * (size_t)n_inst + inst] = zl;  st[1 * (size_t)n_inst + inst] = zr;
         st[2 * (size_t)n_inst + inst] = zlr; st[3 * (size_t)n_inst + inst] = zll; st[4 * (size_t)n_inst + inst] = zrr;
         // Stcorrdsp::read (:79-82)
@@ -143,17 +148,23 @@ B200M_DEV void affine_scan (float& A, float& B, int lane)
     }
 }
 
-template <bool HOLD>
+// RAG: pair inst runs over its first rlen[inst] frames, the warp's block length (warp-uniform: the segment layout is the same as for
+// a plain block of that length); rlen 0: not called.
+template <bool RAG>
 __global__ void __launch_bounds__ (CSC_WARPS * 32)
 cor_scan_kernel (const float* __restrict__ in, size_t stride, int n_inst, int nfram, int aligned, float w1, float w2,
                  float* __restrict__ st /* [5][n_inst] */, float* __restrict__ res, float* __restrict__ ring, int N, int rboff,
-                 const uint8_t* __restrict__ run)
+                 const uint32_t* __restrict__ rlen)
 {
     __shared__ float sm[CSC_WARPS][2][32 * CSC_PITCH];
     const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
     const int inst = blockIdx.x * CSC_WARPS + warp;
-    if (inst >= n_inst || (HOLD && !run[inst])) return;      // warp-uniform; warps never synchronise with each other
-    if (HOLD) ring = nullptr;                                // the phasewheel ring feed never holds: compiled out of this variant
+    if (inst >= n_inst) return;                              // warp-uniform; warps never synchronise with each other
+    if (RAG) {
+        nfram = (int)rlen[inst];
+        if (nfram == 0) return;
+        ring = nullptr;                                      // the phasewheel ring feed is never ragged: compiled out of this variant
+    }
     float* sl = sm[warp][0]; float* sr = sm[warp][1];
     const float* gl = in + (size_t)(2 * inst) * stride; const float* gr = gl + stride;
     float* rl = ring ? ring + (size_t)(2 * inst) * N : nullptr; float* rr = rl ? rl + N : nullptr;
@@ -268,24 +279,27 @@ struct b200m_cor {
     int device; uint32_t n_inst; float w1, w2;
     int scan = 0;                          // B200M_PREC_FMA: time-parallel cor_scan_kernel
     float *d_st = nullptr, *d_res = nullptr;
-    std::vector<uint8_t> run;              // b200m_cor_process_ctl_*: the run mask as last uploaded to d_run (all 1 at create)
-    uint8_t* d_run = nullptr;
+    // ragged blocks (b200m_cor_process_ragged_*, and b200m_cor_process_ctl_* as lengths run[i] ? nfram : 0): the lengths as last
+    // uploaded to rag.d (empty: none yet); a block uploads them only when they differ
+    std::vector<uint32_t> len; RaggedLen rag;
+    std::vector<uint32_t> ctl_len;         // b200m_cor_process_ctl_*: scratch for its lengths
+    int attached = 0;                      // phasewheel banks feeding this one (b200m_pw_attach_cor): ragged calls are refused
     cudaStream_t own = nullptr; HostStage stage; bool last_host = false;
 };
 
 static cudaStream_t cor_stream (b200m_cor* h, void* stream) { return h->last_host ? h->own : (cudaStream_t)stream; }
 
-template <bool HOLD>
+template <bool RAG>
 static int cor_launch (b200m_cor* h, const float* d_in, size_t stride, uint32_t nfram, cudaStream_t st, float* ring, int N, int rboff)
 {
     const int aligned = ((uintptr_t)d_in % 16 == 0) && (stride % 4 == 0);
-    const uint8_t* run = HOLD ? h->d_run : nullptr;
+    const uint32_t* rlen = RAG ? h->rag.d : nullptr;
     if (h->scan)
-        cor_scan_kernel<HOLD><<<(h->n_inst + CSC_WARPS - 1) / CSC_WARPS, CSC_WARPS * 32, 0, st>>> (
-            d_in, stride, (int)h->n_inst, (int)nfram, aligned, h->w1, h->w2, h->d_st, h->d_res, ring, N, rboff, run);
+        cor_scan_kernel<RAG><<<(h->n_inst + CSC_WARPS - 1) / CSC_WARPS, CSC_WARPS * 32, 0, st>>> (
+            d_in, stride, (int)h->n_inst, (int)nfram, aligned, h->w1, h->w2, h->d_st, h->d_res, ring, N, rboff, rlen);
     else
-        cor_kernel<HOLD><<<(h->n_inst + 31) / 32, 32, 0, st>>> (d_in, stride, (int)h->n_inst, (int)nfram, aligned, h->w1, h->w2, h->d_st, h->d_res,
-                                                                ring, N, rboff, run);
+        cor_kernel<RAG><<<(h->n_inst + 31) / 32, 32, 0, st>>> (d_in, stride, (int)h->n_inst, (int)nfram, aligned, h->w1, h->w2, h->d_st, h->d_res,
+                                                               ring, N, rboff, rlen);
     B200M_LAUNCHED (1);
     B200M_CUDA (cudaGetLastError ());
     return 0;
@@ -310,17 +324,30 @@ int cor_follow (b200m_cor* h, bool host)
     return 0;
 }
 cudaStream_t cor_host_stream (const b200m_cor* h, cudaStream_t pw_own) { return h ? h->own : pw_own; }
+void cor_attach (b200m_cor* h, int d) { if (h) h->attached += d; }
 }
 
-// run: NULL (every pair runs) or n_inst flags; the mask is uploaded only when it differs from the last one
-static int cor_process (b200m_cor* h, const float* d_in, size_t stride, uint32_t nfram, const uint8_t* run, cudaStream_t st)
+// len: NULL (every pair runs nfram) or n_inst lengths <= nfram; they are uploaded only when they differ from the last ones
+static int cor_process (b200m_cor* h, const float* d_in, size_t stride, uint32_t nfram, const uint32_t* len, cudaStream_t st)
 {
-    if (!run) return cor_launch<false> (h, d_in, stride, nfram, st, nullptr, 0, 0);
-    if (memcmp (run, h->run.data (), h->n_inst)) {
-        for (uint32_t i = 0; i < h->n_inst; ++i) h->run[i] = run[i] != 0;
-        B200M_CUDA (cudaMemcpyAsync (h->d_run, h->run.data (), h->n_inst, cudaMemcpyHostToDevice, st));
+    if (!len) return cor_launch<false> (h, d_in, stride, nfram, st, nullptr, 0, 0);
+    if (h->len.empty () || memcmp (len, h->len.data (), h->n_inst * sizeof (uint32_t))) {
+        cudaError_t e = cudaSuccess;
+        uint32_t* hl = h->rag.stage (h->n_inst, &e);
+        if (!hl) return cuda_fail (e, "cor_process", __FILE__, __LINE__);
+        memcpy (hl, len, h->n_inst * sizeof (uint32_t));
+        B200M_CUDA (h->rag.upload (h->n_inst, st));
+        h->len.assign (len, len + h->n_inst);
     }
     return cor_launch<true> (h, d_in, stride, nfram, st, nullptr, 0, 0);
+}
+
+// b200m_cor_process_ctl_*: run[i] == 0 holds pair i, a ragged block of lengths run[i] ? nfram : 0 (NULL run: every pair runs)
+static const uint32_t* cor_ctl_len (b200m_cor* h, uint32_t nfram, const uint8_t* run)
+{
+    if (!run) return nullptr;
+    for (uint32_t i = 0; i < h->n_inst; ++i) h->ctl_len[i] = run[i] ? nfram : 0;
+    return h->ctl_len.data ();
 }
 
 extern "C" {
@@ -344,14 +371,12 @@ int b200m_cor_create (b200m_cor** out, int device, uint32_t n_inst, int fsamp, f
     b200m_cor* h = new (std::nothrow) b200m_cor;
     if (!h) return set_err (B200M_E_NOMEM, "host allocation failed");
     h->device = device; h->n_inst = n_inst;
-    h->run.assign (n_inst, 1);
+    h->ctl_len.assign (n_inst, 0);
     { float w[2]; b200m_design_cor (fsamp, flp, tcf, w); h->w1 = w[0]; h->w2 = w[1]; }
     cudaError_t e = cudaMalloc ((void**)&h->d_st, (size_t)5 * n_inst * sizeof (float));
     if (e == cudaSuccess) e = cudaMemset (h->d_st, 0, (size_t)5 * n_inst * sizeof (float));
     if (e == cudaSuccess) e = cudaMalloc ((void**)&h->d_res, n_inst * sizeof (float));
     if (e == cudaSuccess) e = cudaMemset (h->d_res, 0, n_inst * sizeof (float));
-    if (e == cudaSuccess) e = cudaMalloc ((void**)&h->d_run, n_inst);
-    if (e == cudaSuccess) e = cudaMemset (h->d_run, 1, n_inst);
     if (e == cudaSuccess) e = cudaStreamCreateWithFlags (&h->own, cudaStreamNonBlocking);
     if (e != cudaSuccess) { int rc = cuda_fail (e, "cor_create", __FILE__, __LINE__); b200m_cor_destroy (h); return rc; }
     *out = h;
@@ -363,7 +388,7 @@ int b200m_cor_destroy (b200m_cor* h)
     if (!h) return 0;
     DeviceGuard g (h->device);
     cudaDeviceSynchronize ();
-    cudaFree (h->d_st); cudaFree (h->d_res); cudaFree (h->d_run); h->stage.release ();
+    cudaFree (h->d_st); cudaFree (h->d_res); h->rag.release (); h->stage.release ();
     if (h->own) cudaStreamDestroy (h->own);
     delete h;
     return 0;
@@ -374,7 +399,7 @@ int b200m_cor_process_ctl_device (b200m_cor* h, const float* d_in, size_t stride
     if (int rc = check_block_args (h, d_in, stride, nfram)) return rc;
     DeviceGuard g (h->device);
     B200M_LEAVE_HOST_PATH (h);
-    return cor_process (h, d_in, stride, nfram, run, (cudaStream_t)stream);
+    return cor_process (h, d_in, stride, nfram, cor_ctl_len (h, nfram, run), (cudaStream_t)stream);
 }
 
 int b200m_cor_process_device (b200m_cor* h, const float* d_in, size_t stride, uint32_t nfram, void* stream)
@@ -391,12 +416,44 @@ int b200m_cor_process_ctl_host (b200m_cor* h, const float* in, size_t stride, ui
     B200M_CUDA (cudaMemcpy2DAsync (h->stage.d, h->stage.cap * sizeof (float), in, stride * sizeof (float),
                                    (size_t)nfram * sizeof (float), (size_t)2 * h->n_inst, cudaMemcpyHostToDevice, h->own));
     h->last_host = true;
-    return cor_process (h, h->stage.d, h->stage.cap, nfram, run, h->own);
+    return cor_process (h, h->stage.d, h->stage.cap, nfram, cor_ctl_len (h, nfram, run), h->own);
 }
 
 int b200m_cor_process_host (b200m_cor* h, const float* in, size_t stride, uint32_t nfram)
 {
     return b200m_cor_process_ctl_host (h, in, stride, nfram, nullptr);
+}
+
+// the checks of a ragged call: 1 ragged, 0 every length is nfram (the plain call), < 0 an error (nothing enqueued)
+static int cor_ragged_check (const b200m_cor* h, const void* in, size_t stride, uint32_t nfram, const uint32_t* len)
+{
+    if (int rc = check_block_args (h, in, stride, nfram)) return rc;
+    if (h->attached) return set_err (B200M_E_UNSUPPORTED, "ragged blocks: this correlation bank is attached to a phasewheel bank, whose ring advances bank-wide");
+    return ragged_check (h->n_inst, nfram, len);
+}
+
+int b200m_cor_process_ragged_device (b200m_cor* h, const float* d_in, size_t stride, uint32_t nfram, const uint32_t* len, void* stream)
+{
+    const int rag = cor_ragged_check (h, d_in, stride, nfram, len);
+    if (rag < 0) return rag;
+    if (!rag) return b200m_cor_process_device (h, d_in, stride, nfram, stream);       // every length is nfram: the plain call
+    DeviceGuard g (h->device);
+    B200M_LEAVE_HOST_PATH (h);
+    return cor_process (h, d_in, stride, nfram, len, (cudaStream_t)stream);
+}
+
+int b200m_cor_process_ragged_host (b200m_cor* h, const float* in, size_t stride, uint32_t nfram, const uint32_t* len)
+{
+    const int rag = cor_ragged_check (h, in, stride, nfram, len);
+    if (rag < 0) return rag;
+    if (!rag) return b200m_cor_process_host (h, in, stride, nfram);
+    DeviceGuard g (h->device);
+    B200M_ENTER_HOST_PATH (h);
+    if (h->stage.ensure ((size_t)2 * h->n_inst, nfram)) return set_err (B200M_E_NOMEM, "staging buffer allocation failed");
+    B200M_CUDA (cudaMemcpy2DAsync (h->stage.d, h->stage.cap * sizeof (float), in, stride * sizeof (float),
+                                   (size_t)nfram * sizeof (float), (size_t)2 * h->n_inst, cudaMemcpyHostToDevice, h->own));
+    h->last_host = true;
+    return cor_process (h, h->stage.d, h->stage.cap, nfram, len, h->own);
 }
 
 int b200m_cor_set_precision (b200m_cor* h, int mode)

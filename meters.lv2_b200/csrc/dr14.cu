@@ -177,11 +177,6 @@ struct b200m_dr14 {
     float *d_rms_sum = nullptr, *d_peak_cur = nullptr, *d_cd = nullptr;
     Dr14State st{}; b200m_dr14_result* d_out = nullptr;
     cudaStream_t own = nullptr; HostStage stage; bool last_host = false;
-    // a ragged block (b200m_dr14_run_ragged_*): per-instance lengths and K-meter _fall values on the device ([n_inst] each), pinned
-    // staging for their upload (two slots: the copy from one may still be queued while the next block fills the other), and the
-    // _fall of every length met so far (host libm, tpk_km_fall); allocated with the first ragged block
-    uint32_t* d_len = nullptr; uint32_t* h_len[2] = {nullptr, nullptr}; cudaEvent_t ev_len[2] = {nullptr, nullptr}; int len_slot = 0;
-    std::vector<float> fall; std::vector<uint8_t> fall_ok;
 };
 
 // reset_peaks of the instances d_inst[0 .. n_sel) (d_inst == nullptr: every instance), clear: and b200m_tpk_clear of their
@@ -212,53 +207,13 @@ static bool dr14_closes (const b200m_dr14* h, uint32_t nfram)
     return b > h->w && h->phases.begin ()->first < b - h->w;
 }
 
-// 1 if some len[i] differs from nfram, 0 if none does (or len is NULL: the plain call), B200M_E_INVAL if one exceeds nfram
-static int dr14_ragged_check (const b200m_dr14* h, uint32_t nfram, const uint32_t* len)
-{
-    if (!len) return 0;
-    bool rag = false;
-    for (uint32_t i = 0; i < h->n_inst; ++i) {
-        if (len[i] > nfram) return set_err (B200M_E_INVAL, "len[%u] = %u exceeds nfram = %u", i, len[i], nfram);
-        rag |= len[i] != nfram;
-    }
-    return rag ? 1 : 0;
-}
-
-// enqueue the upload of a ragged block's lengths and their K-meter _fall values on `st`
-static int dr14_upload_len (b200m_dr14* h, const uint32_t* len, cudaStream_t st)
-{
-    const size_t n = h->n_inst;
-    cudaError_t e = cudaSuccess;
-    if (!h->d_len) e = cudaMalloc ((void**)&h->d_len, 2 * n * sizeof (uint32_t));
-    for (int s = 0; s < 2; ++s) {
-        if (e == cudaSuccess && !h->h_len[s]) e = cudaHostAlloc ((void**)&h->h_len[s], 2 * n * sizeof (uint32_t), cudaHostAllocDefault);
-        if (e == cudaSuccess && !h->ev_len[s]) e = cudaEventCreateWithFlags (&h->ev_len[s], cudaEventDisableTiming);
-    }
-    if (h->fall.empty ()) { h->fall.assign (B200M_MAX_BLOCK + 1, 0.0f); h->fall_ok.assign (B200M_MAX_BLOCK + 1, 0); }
-    // pinned staging: the copy is truly asynchronous, and the slot's previous copy has run before it is overwritten
-    const int s = h->len_slot; h->len_slot ^= 1;
-    if (e == cudaSuccess) e = cudaEventSynchronize (h->ev_len[s]);
-    if (e != cudaSuccess) return cuda_fail (e, "dr14_upload_len", __FILE__, __LINE__);
-    uint32_t* hl = h->h_len[s];
-    float* hf = reinterpret_cast<float*> (hl + n);
-    memcpy (hl, len, n * sizeof (uint32_t));
-    for (size_t i = 0; i < n; ++i) {
-        const uint32_t L = len[i];
-        if (!h->fall_ok[L]) { h->fall[L] = tpk_km_fall (h->tpk, L); h->fall_ok[L] = 1; }      // once per length
-        hf[i] = h->fall[L];
-    }
-    e = cudaMemcpyAsync (h->d_len, hl, 2 * n * sizeof (uint32_t), cudaMemcpyHostToDevice, st);
-    if (e == cudaSuccess) e = cudaEventRecord (h->ev_len[s], st);
-    if (e != cudaSuccess) return cuda_fail (e, "dr14_upload_len", __FILE__, __LINE__);
-    return 0;
-}
-
-// len (host, every entry <= nfram, some != nfram: dr14_ragged_check): a ragged block, instance i runs over its first len[i] frames;
+// len (host, every entry <= nfram, some != nfram: ragged_check): a ragged block, instance i runs over its first len[i] frames;
 // nullptr: every instance runs nfram
 static int dr14_run (b200m_dr14* h, const float* d_in, size_t stride, uint32_t nfram, cudaStream_t st, const uint32_t* len = nullptr)
 {
-    if (len) if (int rc = dr14_upload_len (h, len, st)) return rc;
-    const uint32_t* d_len = len ? h->d_len : nullptr;
+    // a ragged block: per-instance lengths and K-meter _fall values, uploaded through the true-peak bank's staging and _fall cache
+    const uint32_t* d_len = nullptr; const float* d_fall = nullptr;
+    if (len) if (int rc = tpk_upload_len (h->tpk, len, h->n_inst, st, &d_len, &d_fall)) return rc;
     bool closes = false;
     TpkDr dr = {};
     if (h->dr_mode) {
@@ -268,7 +223,7 @@ static int dr14_run (b200m_dr14* h, const float* d_in, size_t stride, uint32_t n
         tpk_set_dr (h->tpk, &dr);
         h->tmod = (uint32_t)((h->tmod + (uint64_t)nfram) % h->w);
     }
-    int rc = len ? tpk_process_ragged (h->tpk, d_in, stride, nfram, st, d_len, reinterpret_cast<const float*> (d_len + h->n_inst), h->nch)
+    int rc = len ? tpk_process_ragged (h->tpk, d_in, stride, nfram, st, d_len, d_fall, h->nch)
                  : b200m_tpk_process_device (h->tpk, d_in, stride, nfram, B200M_TP_MODE_PROCESS, st);
     if (rc) return rc;
     const unsigned gs = (h->n_inst * 32 + 127) / 128, gp = (h->n_inst + 127) / 128;
@@ -351,8 +306,6 @@ int b200m_dr14_destroy (b200m_dr14* h)
     void* ps[] = {h->d_rms_sum, h->d_peak_cur, h->st.emit_rms, h->st.emit_peak, h->st.emit_valid, h->st.peak_hist, h->st.m_rms, h->st.m_peak,
                   h->st.m_dbtp, h->st.numfrag, h->st.phase, h->d_sel, h->st.hist, h->d_cd, h->d_out};
     for (void* p : ps) cudaFree (p);
-    cudaFree (h->d_len);
-    for (int s = 0; s < 2; ++s) { if (h->h_len[s]) cudaFreeHost (h->h_len[s]); if (h->ev_len[s]) cudaEventDestroy (h->ev_len[s]); }
     h->stage.release ();
     if (h->own) cudaStreamDestroy (h->own);
     delete h;
@@ -384,7 +337,7 @@ int b200m_dr14_run_host (b200m_dr14* h, const float* in, size_t stride, uint32_t
 int b200m_dr14_run_ragged_device (b200m_dr14* h, const float* d_in, size_t stride, uint32_t nfram, const uint32_t* len, void* stream)
 {
     if (int rc = check_block_args (h, d_in, stride, nfram)) return rc;
-    const int rag = dr14_ragged_check (h, nfram, len);
+    const int rag = ragged_check (h->n_inst, nfram, len);
     if (rag < 0) return rag;
     if (!rag) return b200m_dr14_run_device (h, d_in, stride, nfram, stream);       // every length is nfram: the plain call
     DeviceGuard g (h->device);
@@ -395,7 +348,7 @@ int b200m_dr14_run_ragged_device (b200m_dr14* h, const float* d_in, size_t strid
 int b200m_dr14_run_ragged_host (b200m_dr14* h, const float* in, size_t stride, uint32_t nfram, const uint32_t* len)
 {
     if (int rc = check_block_args (h, in, stride, nfram)) return rc;
-    const int rag = dr14_ragged_check (h, nfram, len);
+    const int rag = ragged_check (h->n_inst, nfram, len);
     if (rag < 0) return rag;
     if (!rag) return b200m_dr14_run_host (h, in, stride, nfram);
     DeviceGuard g (h->device);

@@ -38,6 +38,17 @@ int check_block_args (const void* h, const void* in, size_t stride, uint32_t nfr
     return 0;
 }
 
+int ragged_check (uint32_t n, uint32_t nfram, const uint32_t* len)
+{
+    if (!len) return 0;
+    bool rag = false;
+    for (uint32_t i = 0; i < n; ++i) {
+        if (len[i] > nfram) return set_err (B200M_E_INVAL, "len[%u] = %u exceeds nfram = %u", i, len[i], nfram);
+        rag |= len[i] != nfram;
+    }
+    return rag ? 1 : 0;
+}
+
 }  // namespace b200m
 
 using namespace b200m;

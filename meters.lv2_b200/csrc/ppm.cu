@@ -19,10 +19,13 @@ constexpr int PPM_PLANE = 32 * PPM_P;                      // floats of one [32 
 struct PpmParams { float w1, w2, w3; };
 
 // KIND 0: VU   1: IEC I/II PPM   3: M/S PPM (two planes: L and R rows of the pair)
-template <int KIND, bool ALIGNED>
+// RAG (b200m_ppm_process_ragged_*): unit u runs process() over its first rlen[u] <= nfram frames only.  Its lane stops at its own
+// (rlen[u] / 4) * 4; the warp still stages whole [32 x 64] tiles up to its longest row, so frames past a row's end are loaded but never
+// reach its filters.  A unit with rlen[u] == 0 was not called: no clamp, scrub or _res store.
+template <int KIND, bool ALIGNED, bool RAG = false>
 __global__ void __launch_bounds__ (PPM_WARPS * 32)
 ppm_kernel (const float* __restrict__ in, size_t stride, int n_units, int nfram, PpmParams pr, const float2* __restrict__ mv /* M/S: [unit] {mv_m, mv_s} */,
-            float* __restrict__ z1s, float* __restrict__ z2s, float* __restrict__ ms, int* __restrict__ ress)
+            float* __restrict__ z1s, float* __restrict__ z2s, float* __restrict__ ms, int* __restrict__ ress, const uint32_t* __restrict__ rlen)
 {
     constexpr int PLANES = KIND == 3 ? 2 : 1;
     extern __shared__ __align__ (16) float ppm_smem[];
@@ -32,7 +35,12 @@ ppm_kernel (const float* __restrict__ in, size_t stride, int n_units, int nfram,
     float* ring = ppm_smem + warp * (PPM_STAGES * PLANES * PPM_PLANE);
     const int u = min (u0 + lane, n_units - 1);
     const bool live = (u0 + lane) < n_units;
-    const int nproc = (nfram / 4) * 4;                     // "n /= 4": the last n mod 4 samples are ignored
+    int nproc = (nfram / 4) * 4;                           // "n /= 4": the last n mod 4 samples are ignored
+    int rl = nfram, lproc = nproc;                         // RAG: this lane's length and its processed samples
+    if constexpr (RAG) {
+        rl = (int)rlen[u]; lproc = (rl / 4) * 4;
+        nproc = __reduce_max_sync (0xffffffffu, lproc);    // the warp stages up to its longest row
+    }
     const int ntiles = (nproc + PPM_T - 1) / PPM_T;
 
     auto issue = [&] (int t) {
@@ -122,13 +130,16 @@ ppm_kernel (const float* __restrict__ in, size_t stride, int n_units, int nfram,
         const float* base = ring + (t % PPM_STAGES) * (PLANES * PPM_PLANE) + lane * PPM_P;
         const float4* pa = reinterpret_cast<const float4*> (base);
         const float4* pb = reinterpret_cast<const float4*> (base + (PLANES - 1) * PPM_PLANE);
-        const int ng = (min (PPM_T, nproc - t * PPM_T)) / 4;
+        int ng = (min (PPM_T, nproc - t * PPM_T)) / 4;
+        if constexpr (RAG) ng = max (0, min (PPM_T, lproc - t * PPM_T)) / 4;
         for (int q = 0; q < ng; ++q) group (pa[q], pb[q]);
         __syncwarp ();
         issue (t + PPM_STAGES - 1);
     }
     cp_async_wait<0> ();
-    if (live) {
+    bool ran = live;                                       // RAG: a unit with length 0 was not called
+    if constexpr (RAG) ran = live && rl > 0;
+    if (ran) {
 #pragma unroll
         for (int q = 0; q < NM; ++q) {
             const int idx = NM * u + q;
@@ -143,10 +154,14 @@ ppm_kernel (const float* __restrict__ in, size_t stride, int n_units, int nfram,
     }
 }
 
-__global__ void ppm_read_kernel (int nm, float g, const float* __restrict__ ms, int* __restrict__ ress, float* __restrict__ out)
+// RAG: after a ragged block, meter i belongs to unit i / per; a unit with rlen 0 was not called, so it is not read either
+template <bool RAG = false>
+__global__ void ppm_read_kernel (int nm, float g, const float* __restrict__ ms, int* __restrict__ ress, float* __restrict__ out,
+                                 const uint32_t* __restrict__ rlen, int per)
 {
     const int i = blockIdx.x * blockDim.x + threadIdx.x;
     if (i >= nm) return;
+    if (RAG && rlen[(unsigned)i / (unsigned)per] == 0) return;
     out[i] = __fmul_rn (g, ms[i]);                          // read(): _res = true; return _g * _m
     ress[i] = 1;
 }
@@ -169,6 +184,7 @@ struct b200m_ppm {
     std::vector<float2> db, mv;                           // M/S: per unit {M, S} gain in dB and as Msppmdsp::_mv; mv is d_mv's host copy
     float2* d_mv = nullptr; bool mv_dirty = false;        // d_mv is rewritten by the next process call
     float *d_z1 = nullptr, *d_z2 = nullptr, *d_m = nullptr, *d_out = nullptr; int* d_res = nullptr;
+    RaggedLen rag; bool rag_read = false;                 // ragged blocks: lengths per unit; the last block was ragged (read skips length 0)
     cudaStream_t own = nullptr; HostStage stage; bool last_host = false;
 };
 
@@ -181,8 +197,17 @@ static void ppm_design (int kind, float fs, float w[4])
 
 static cudaStream_t ppm_stream (b200m_ppm* h, void* stream) { return h->last_host ? h->own : (cudaStream_t)stream; }
 
-static int ppm_process (b200m_ppm* h, const float* d_in, size_t stride, uint32_t nfram, cudaStream_t st)
+// len (host, every entry <= nfram, some != nfram: ragged_check): unit u runs over its first len[u] frames; nullptr: every unit nfram
+static int ppm_process (b200m_ppm* h, const float* d_in, size_t stride, uint32_t nfram, cudaStream_t st, const uint32_t* len = nullptr)
 {
+    h->rag_read = len != nullptr;
+    if (len) {
+        cudaError_t e = cudaSuccess;
+        uint32_t* hl = h->rag.stage (h->n_units, &e);
+        if (!hl) return cuda_fail (e, "ppm_process", __FILE__, __LINE__);
+        memcpy (hl, len, h->n_units * sizeof (uint32_t));
+        B200M_CUDA (h->rag.upload (h->n_units, st));
+    }
     if (h->mv_dirty) {
         B200M_CUDA (cudaMemcpyAsync (h->d_mv, h->mv.data (), h->n_units * sizeof (float2), cudaMemcpyHostToDevice, st));
         h->mv_dirty = false;
@@ -192,10 +217,16 @@ static int ppm_process (b200m_ppm* h, const float* d_in, size_t stride, uint32_t
     const size_t smem = (size_t)PPM_WARPS * PPM_STAGES * planes * PPM_PLANE * sizeof (float);
     const int nwarps = (h->n_units + 31) / 32;
     dim3 grid ((nwarps + PPM_WARPS - 1) / PPM_WARPS), blk (PPM_WARPS * 32);
-#define PPM_GO(K, A) ppm_kernel<K, A><<<grid, blk, smem, st>>> (d_in, stride, (int)h->n_units, (int)nfram, h->pr, h->d_mv, h->d_z1, h->d_z2, h->d_m, h->d_res)
-    if (h->kind == B200M_PPM_VU) { if (al) PPM_GO (0, true); else PPM_GO (0, false); }
-    else if (h->kind == B200M_PPM_MS) { if (al) PPM_GO (3, true); else PPM_GO (3, false); }
-    else { if (al) PPM_GO (1, true); else PPM_GO (1, false); }
+#define PPM_GO(K, A, R) ppm_kernel<K, A, R><<<grid, blk, smem, st>>> (d_in, stride, (int)h->n_units, (int)nfram, h->pr, h->d_mv, h->d_z1, h->d_z2, h->d_m, h->d_res, \
+                                                                      R ? h->rag.d : nullptr)
+    if (len) {
+        if (h->kind == B200M_PPM_VU) { if (al) PPM_GO (0, true, true); else PPM_GO (0, false, true); }
+        else if (h->kind == B200M_PPM_MS) { if (al) PPM_GO (3, true, true); else PPM_GO (3, false, true); }
+        else { if (al) PPM_GO (1, true, true); else PPM_GO (1, false, true); }
+    }
+    else if (h->kind == B200M_PPM_VU) { if (al) PPM_GO (0, true, false); else PPM_GO (0, false, false); }
+    else if (h->kind == B200M_PPM_MS) { if (al) PPM_GO (3, true, false); else PPM_GO (3, false, false); }
+    else { if (al) PPM_GO (1, true, false); else PPM_GO (1, false, false); }
 #undef PPM_GO
     B200M_LAUNCHED (1);
     B200M_CUDA (cudaGetLastError ());
@@ -235,7 +266,8 @@ int b200m_ppm_create (b200m_ppm** out, int device, uint32_t n_units, float fsamp
     if (kind == B200M_PPM_MS) A ((void**)&h->d_mv, n_units * sizeof (float2));
     if (e == cudaSuccess) e = cudaStreamCreateWithFlags (&h->own, cudaStreamNonBlocking);
     const int smem_max = PPM_WARPS * PPM_STAGES * 2 * PPM_PLANE * (int)sizeof (float);
-#define PPM_ATTR(K, A) if (e == cudaSuccess) e = cudaFuncSetAttribute (ppm_kernel<K, A>, cudaFuncAttributeMaxDynamicSharedMemorySize, smem_max)
+#define PPM_ATTR(K, A) if (e == cudaSuccess) e = cudaFuncSetAttribute (ppm_kernel<K, A>, cudaFuncAttributeMaxDynamicSharedMemorySize, smem_max); \
+                       if (e == cudaSuccess) e = cudaFuncSetAttribute (ppm_kernel<K, A, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, smem_max)
     PPM_ATTR (0, true); PPM_ATTR (0, false); PPM_ATTR (1, true); PPM_ATTR (1, false); PPM_ATTR (3, true); PPM_ATTR (3, false);
 #undef PPM_ATTR
     if (e == cudaSuccess) {
@@ -253,7 +285,7 @@ int b200m_ppm_destroy (b200m_ppm* h)
     if (!h) return 0;
     DeviceGuard g (h->device);
     cudaDeviceSynchronize ();
-    cudaFree (h->d_z1); cudaFree (h->d_z2); cudaFree (h->d_m); cudaFree (h->d_out); cudaFree (h->d_res); cudaFree (h->d_mv); h->stage.release ();
+    cudaFree (h->d_z1); cudaFree (h->d_z2); cudaFree (h->d_m); cudaFree (h->d_out); cudaFree (h->d_res); cudaFree (h->d_mv); h->stage.release (); h->rag.release ();
     if (h->own) cudaStreamDestroy (h->own);
     delete h;
     return 0;
@@ -314,11 +346,42 @@ int b200m_ppm_process_host (b200m_ppm* h, const float* in, size_t stride, uint32
     return ppm_process (h, h->stage.d, h->stage.cap, nfram, h->own);
 }
 
+int b200m_ppm_process_ragged_device (b200m_ppm* h, const float* d_in, size_t stride, uint32_t nfram, const uint32_t* len, void* stream)
+{
+    if (int rc = check_block_args (h, d_in, stride, nfram)) return rc;
+    const int rag = ragged_check (h->n_units, nfram, len);
+    if (rag < 0) return rag;
+    if (!rag) return b200m_ppm_process_device (h, d_in, stride, nfram, stream);       // every length is nfram: the plain call
+    DeviceGuard g (h->device);
+    B200M_LEAVE_HOST_PATH (h);
+    return ppm_process (h, d_in, stride, nfram, (cudaStream_t)stream, len);
+}
+
+int b200m_ppm_process_ragged_host (b200m_ppm* h, const float* in, size_t stride, uint32_t nfram, const uint32_t* len)
+{
+    if (int rc = check_block_args (h, in, stride, nfram)) return rc;
+    const int rag = ragged_check (h->n_units, nfram, len);
+    if (rag < 0) return rag;
+    if (!rag) return b200m_ppm_process_host (h, in, stride, nfram);
+    DeviceGuard g (h->device);
+    B200M_ENTER_HOST_PATH (h);
+    const size_t rows = h->kind == B200M_PPM_MS ? (size_t)2 * h->n_units : h->n_units;
+    if (h->stage.ensure (rows, nfram)) return set_err (B200M_E_NOMEM, "staging buffer allocation failed");
+    B200M_CUDA (cudaMemcpy2DAsync (h->stage.d, h->stage.cap * sizeof (float), in, stride * sizeof (float),
+                                   (size_t)nfram * sizeof (float), rows, cudaMemcpyHostToDevice, h->own));
+    h->last_host = true;
+    return ppm_process (h, h->stage.d, h->stage.cap, nfram, h->own, len);
+}
+
 int b200m_ppm_read_device (b200m_ppm* h, void* stream)
 {
     if (!h) return set_err (B200M_E_INVAL, "NULL handle");
     DeviceGuard g (h->device);
-    ppm_read_kernel<<<(h->n_meters + 255) / 256, 256, 0, ppm_stream (h, stream)>>> ((int)h->n_meters, h->g, h->d_m, h->d_res, h->d_out);
+    const unsigned grid = (h->n_meters + 255) / 256;
+    if (h->rag_read)                                      // after a ragged block: units with length 0 were not called
+        ppm_read_kernel<true><<<grid, 256, 0, ppm_stream (h, stream)>>> ((int)h->n_meters, h->g, h->d_m, h->d_res, h->d_out, h->rag.d,
+                                                                          h->kind == B200M_PPM_MS ? 2 : 1);
+    else ppm_read_kernel<<<grid, 256, 0, ppm_stream (h, stream)>>> ((int)h->n_meters, h->g, h->d_m, h->d_res, h->d_out, nullptr, 1);
     B200M_LAUNCHED (1);
     B200M_CUDA (cudaGetLastError ());
     return 0;

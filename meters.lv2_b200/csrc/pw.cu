@@ -185,6 +185,7 @@ uint32_t cor_instances (const b200m_cor* h);
 // bank first; cor_host_stream is the stream of the host path and of the getters after it
 int cor_follow (b200m_cor* h, bool host);
 cudaStream_t cor_host_stream (const b200m_cor* h, cudaStream_t pw_own);
+void cor_attach (b200m_cor* h, int d);                       // counts the phasewheel banks feeding h (its ragged calls are refused)
 }
 
 struct b200m_pw {
@@ -387,7 +388,9 @@ int b200m_pw_attach_cor (b200m_pw* h, b200m_cor* cor)
     if (cor && cor_instances (cor) != h->n_inst) return set_err (B200M_E_INVAL, "the correlation bank must have as many pairs as the phasewheel bank has instances");
     DeviceGuard g (h->device);
     B200M_CUDA (cudaDeviceSynchronize ());
+    cor_attach (h->cor, -1);
     h->cor = cor;
+    cor_attach (cor, 1);
     return 0;
 }
 

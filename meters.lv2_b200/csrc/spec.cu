@@ -30,16 +30,23 @@ constexpr int SPEC_CLEAR_MAX = 1, SPEC_REINIT_GUI = 2, SPEC_PARITY = 4;   // SPE
 // FMA = B200M_PREC_FMA: the same transposed-DF-II cascade with fused multiply-adds (25 instead of 39 fp64 instructions per frame and
 // band).  Band levels feed no integer result and the filters run in double precision, so the ports move by ~1e-12 dB, far inside the
 // contract's +-1e-4 dB (tests/test_cor_spec_gpu.py::test_spec_fma_mode_within_tolerance).
-template <bool FMA>
+// RAG (b200m_spec_process_ragged_*): instance inst runs over its first rlen[inst] <= nfram frames, the warp's block length (one
+// warp per instance: warp-uniform); rlen 0: the instance is not run at all.  Its `ac` phase is its own (SPEC_PARITY, kept by the host).
+template <bool FMA, bool RAG = false>
 __global__ void __launch_bounds__ (SPEC_WARPS * 32)
 spec_kernel (const float* __restrict__ in, size_t stride, int n_inst, int nfram, SpecRun rp, const SpecCtl* __restrict__ ctl, const double* __restrict__ coef,
-             double* __restrict__ zst /* [inst][12][32] */, float* __restrict__ valf /* [inst][2][32] */, float* __restrict__ ports /* [inst][60] */)
+             double* __restrict__ zst /* [inst][12][32] */, float* __restrict__ valf /* [inst][2][32] */, float* __restrict__ ports /* [inst][60] */,
+             const uint32_t* __restrict__ rlen)
 {
     __shared__ float raw[SPEC_WARPS][2][2][SPEC_TC];      // [warp][stage][channel][frame]
     __shared__ double dd[SPEC_WARPS][SPEC_TC];
     const int lane = threadIdx.x & 31, w = threadIdx.x >> 5;
     const int inst = blockIdx.x * SPEC_WARPS + w;
     if (inst >= n_inst) return;                            // warp-uniform; no block-wide barriers below
+    if constexpr (RAG) {
+        nfram = (int)rlen[inst];
+        if (nfram == 0) return;
+    }
     const int band = min (lane, SPEC_BANDS - 1);
     const bool live = lane < SPEC_BANDS;
     const float* pl = in + (size_t)inst * rp.nchan * stride;
@@ -173,6 +180,7 @@ struct b200m_spec {
     double *d_coef = nullptr, *d_z = nullptr; float *d_val = nullptr, *d_ports = nullptr;
     cudaStream_t own = nullptr; HostStage stage; bool last_host = false;
     int fma = 0;                                          // B200M_PREC_FMA
+    RaggedLen rag;                                        // ragged blocks: lengths per instance
 };
 
 typedef std::complex<double> cplx;
@@ -285,11 +293,22 @@ static void spec_reset_ctl (b200m_spec* h, uint32_t i)
 
 // ctl[i * cstride] = {speed, reset} of instance i; cstride = 0: the same pair for every instance.  Only the instances whose run
 // parameters changed are uploaded (one copy of the changed range, on the call's stream).
-static int spec_process (b200m_spec* h, const float* d_in, size_t stride, uint32_t nfram, const float* ctl, size_t cstride, cudaStream_t st)
+// len (host, every entry <= nfram, some != nfram: ragged_check): instance i runs over its first len[i] frames; len[i] == 0: it is
+// not run, its control state does not advance and its ctl row is ignored.  nullptr: every instance runs nfram.
+static int spec_process (b200m_spec* h, const float* d_in, size_t stride, uint32_t nfram, const float* ctl, size_t cstride, cudaStream_t st,
+                         const uint32_t* len = nullptr)
 {
     for (uint32_t i = 0; i < h->n_inst; ++i) {
+        if (len && len[i] == 0) continue;
         const SpecCtl c = spec_control (h, i, ctl[i * cstride], ctl[i * cstride + 1]);
         if (memcmp (&c, &h->ctl[i], sizeof (c))) { h->ctl[i] = c; spec_mark (h, i, i + 1); }
+    }
+    if (len) {
+        cudaError_t e = cudaSuccess;
+        uint32_t* hl = h->rag.stage (h->n_inst, &e);
+        if (!hl) return cuda_fail (e, "spec_process", __FILE__, __LINE__);
+        memcpy (hl, len, h->n_inst * sizeof (uint32_t));
+        B200M_CUDA (h->rag.upload (h->n_inst, st));
     }
     if (h->ctl_lo < h->ctl_hi) {
         B200M_CUDA (cudaMemcpyAsync (h->d_ctl + h->ctl_lo, h->ctl.data () + h->ctl_lo, (h->ctl_hi - h->ctl_lo) * sizeof (SpecCtl), cudaMemcpyHostToDevice, st));
@@ -298,12 +317,21 @@ static int spec_process (b200m_spec* h, const float* d_in, size_t stride, uint32
     SpecRun rp; rp.nchan = (int)h->nchan;
     rp.ac0 = (int)(h->frames & 1);
     h->frames += nfram;
-    if (h->fma) spec_kernel<true><<<(h->n_inst + SPEC_WARPS - 1) / SPEC_WARPS, SPEC_WARPS * 32, 0, st>>> (
-        d_in, stride, (int)h->n_inst, (int)nfram, rp, h->d_ctl, h->d_coef, h->d_z, h->d_val, h->d_ports);
-    else spec_kernel<false><<<(h->n_inst + SPEC_WARPS - 1) / SPEC_WARPS, SPEC_WARPS * 32, 0, st>>> (
-        d_in, stride, (int)h->n_inst, (int)nfram, rp, h->d_ctl, h->d_coef, h->d_z, h->d_val, h->d_ports);
+    const unsigned grid = (h->n_inst + SPEC_WARPS - 1) / SPEC_WARPS;
+#define SPEC_GO(F, R) spec_kernel<F, R><<<grid, SPEC_WARPS * 32, 0, st>>> (d_in, stride, (int)h->n_inst, (int)nfram, rp, h->d_ctl, h->d_coef, h->d_z, \
+                                                                          h->d_val, h->d_ports, R ? h->rag.d : nullptr)
+    if (len) { if (h->fma) SPEC_GO (true, true); else SPEC_GO (false, true); }
+    else if (h->fma) SPEC_GO (true, false);
+    else SPEC_GO (false, false);
+#undef SPEC_GO
     B200M_LAUNCHED (1);
     B200M_CUDA (cudaGetLastError ());
+    if (len) {
+        // instance i's `ac` toggled len[i] times, the bank's frame count nfram times: its phase against the bank's flips when the
+        // difference is odd.  Uploaded with the next call's control records.
+        for (uint32_t i = 0; i < h->n_inst; ++i)
+            if ((nfram - len[i]) & 1) { h->ctl[i].flags ^= SPEC_PARITY; spec_mark (h, i, i + 1); }
+    }
     return 0;
 }
 
@@ -356,7 +384,7 @@ int b200m_spec_destroy (b200m_spec* h)
     if (!h) return 0;
     DeviceGuard g (h->device);
     cudaDeviceSynchronize ();
-    cudaFree (h->d_coef); cudaFree (h->d_z); cudaFree (h->d_val); cudaFree (h->d_ports); cudaFree (h->d_ctl); h->stage.release ();
+    cudaFree (h->d_coef); cudaFree (h->d_z); cudaFree (h->d_val); cudaFree (h->d_ports); cudaFree (h->d_ctl); h->stage.release (); h->rag.release ();
     if (h->own) cudaStreamDestroy (h->own);
     delete h;
     return 0;
@@ -380,7 +408,8 @@ int b200m_spec_process_device (b200m_spec* h, const float* d_in, size_t stride, 
     return spec_process (h, d_in, stride, nfram, c, 0, (cudaStream_t)stream);
 }
 
-static int spec_process_host (b200m_spec* h, const float* in, size_t stride, uint32_t nfram, const float* ctl, size_t cstride)
+static int spec_process_host (b200m_spec* h, const float* in, size_t stride, uint32_t nfram, const float* ctl, size_t cstride,
+                              const uint32_t* len = nullptr)
 {
     if (int rc = check_block_args (h, in, stride, nfram)) return rc;
     DeviceGuard g (h->device);
@@ -390,7 +419,7 @@ static int spec_process_host (b200m_spec* h, const float* in, size_t stride, uin
     B200M_CUDA (cudaMemcpy2DAsync (h->stage.d, h->stage.cap * sizeof (float), in, stride * sizeof (float),
                                    (size_t)nfram * sizeof (float), nch, cudaMemcpyHostToDevice, h->own));
     h->last_host = true;
-    return spec_process (h, h->stage.d, h->stage.cap, nfram, ctl, cstride, h->own);
+    return spec_process (h, h->stage.d, h->stage.cap, nfram, ctl, cstride, h->own, len);
 }
 
 int b200m_spec_process_ctl_host (b200m_spec* h, const float* in, size_t stride, uint32_t nfram, const float* ctl)
@@ -403,6 +432,29 @@ int b200m_spec_process_host (b200m_spec* h, const float* in, size_t stride, uint
 {
     const float c[2] = {speed, reset};
     return spec_process_host (h, in, stride, nfram, c, 0);
+}
+
+int b200m_spec_process_ragged_device (b200m_spec* h, const float* d_in, size_t stride, uint32_t nfram, const float* ctl, const uint32_t* len,
+                                      void* stream)
+{
+    if (int rc = check_block_args (h, d_in, stride, nfram)) return rc;
+    if (!ctl) return set_err (B200M_E_INVAL, "NULL ctl");
+    const int rag = ragged_check (h->n_inst, nfram, len);
+    if (rag < 0) return rag;
+    if (!rag) return b200m_spec_process_ctl_device (h, d_in, stride, nfram, ctl, stream);     // every length is nfram: the plain call
+    DeviceGuard g (h->device);
+    B200M_LEAVE_HOST_PATH (h);
+    return spec_process (h, d_in, stride, nfram, ctl, 2, (cudaStream_t)stream, len);
+}
+
+int b200m_spec_process_ragged_host (b200m_spec* h, const float* in, size_t stride, uint32_t nfram, const float* ctl, const uint32_t* len)
+{
+    if (int rc = check_block_args (h, in, stride, nfram)) return rc;
+    if (!ctl) return set_err (B200M_E_INVAL, "NULL ctl");
+    const int rag = ragged_check (h->n_inst, nfram, len);
+    if (rag < 0) return rag;
+    if (!rag) return b200m_spec_process_ctl_host (h, in, stride, nfram, ctl);
+    return spec_process_host (h, in, stride, nfram, ctl, 2, len);
 }
 
 int b200m_spec_clear (b200m_spec* h, int32_t inst, void* stream)

@@ -20,6 +20,7 @@
 #include <math.h>
 #include <stdlib.h>
 #include <algorithm>
+#include <vector>
 #include "common.cuh"
 #include "tpk_internal.cuh"
 #include "ebu_kw.cuh"
@@ -415,14 +416,15 @@ B200M_DEV void r128_group_hold (const R128Hold& r, const TpkState& st, float mm,
 // the HOLD instantiation for a launch: 2 (the stereo code) when the launch has no EBUr128 epilogue
 static inline int r128_hold_of (const R128Hold& r) { return !r.tpmax ? 2 : r.lin ? 0 : r.nch; }
 
-// A ragged process() block (RAG, the DR-14 bank's b200m_dr14_run_ragged_*): row c belongs to instance c / nch, which runs
-// process() over its first len[c / nch] <= nfram frames only; fall[c / nch] is Kmeterdsp's _fall for that length (host libm).
+// A ragged process() block (RAG: b200m_tpk_process_ragged_*, nch = 1, and the DR-14 bank's b200m_dr14_run_ragged_*): row c belongs
+// to instance c / nch, which runs process() over its first len[c / nch] <= nfram frames only; fall[c / nch] is Kmeterdsp's _fall
+// for that length (host libm).
 struct TpkRag {
     const uint32_t* len; const float* fall; int nch;
 };
 
-// RAG (exact process() with the K-meter, tpk_kernel<16, 64, true, false, true, IMM, DR, false, true>): every row stops at its own
-// length rl.  The FIR phase runs as for a plain block: it is causal, so the outputs before rl never see the unread frames, and
+// RAG (exact 16-channel process(): tpk_kernel<16, 64, TP, false, KM, IMM, DR, false, true> with true peak, the K-meter or both):
+// every row stops at its own length rl.  The FIR phase runs as for a plain block: it is causal, so the outputs before rl never see the unread frames, and
 // unread frames can only make the silence and phase-0 elision guards more conservative (row_absmax propagates NaN, Inf and large
 // values fail phase0_is_delay, a non-zero frame fails the silence vote), never change an output.  The ballistics lanes stay in
 // their loop past rl (its z1 + z2 shuffle needs the whole warp) with their state frozen; the K-meter lanes drop rl mod 4 samples
@@ -433,7 +435,7 @@ __global__ void __launch_bounds__ (TPK_THREADS)
 tpk_kernel (const float* __restrict__ in, size_t stride, int c_first, int n_chan, int nfram, int aligned, int elide0, TpkParams prm,
             TpkState st, float* __restrict__ dbg, R128Hold r128, TpkDr dr, TpkRag rag)
 {
-    static_assert (!RAG || (CH == 16 && TP && !TPMAX && KM && !FMA), "the ragged form is the exact 16-channel process() kernel");
+    static_assert (!RAG || (CH == 16 && !TPMAX && (TP || KM) && !FMA), "the ragged form is the exact 16-channel process() kernel");
     // processes channels [c_first, n_chan): `n_chan` is the END of the slice (absolute channel index)
     constexpr int XP = TpkGeom<CH, TC, TP && !TPMAX>::XP;   // x row pitch (floats): 16-byte multiple
     constexpr int OP = 4 * TC + 4;                // |out| row pitch
@@ -561,7 +563,7 @@ tpk_kernel (const float* __restrict__ in, size_t stride, int c_first, int n_chan
             const int r = idx / 48, j = idx % 48;
             xs[buf ^ 1][r][j] = xs[buf][r][len + j];
         }
-        if constexpr (RAG) {
+        if constexpr (RAG && TP) {
             // next history of the rows that end in this chunk (s0 < L <= s0 + len; L == 0: chunk 0, the old history itself).  Every
             // thread read the old history into xs[0] before the barrier above, so st.hist can be overwritten now.
             for (int idx = tid; idx < CH * 48; idx += TPK_THREADS) {
@@ -2102,6 +2104,10 @@ struct b200m_tpk {
     int chunked = 1;                        // process_max without K-meter runs as (channel group x time chunk) CTAs (tpmax_kernel); B200M_TPK_CHUNKED=0: one CTA per group
     int fma = 0;                            // B200M_PREC_FMA: tolerance-mode FIR (fir16_fma); needs the literal table (imm)
     TpkDr dr{}; bool dr_on = false;         // DR-14 accumulation of the next process() call (set by dr14.cu)
+    // ragged blocks (tpk_upload_len): [n] lengths then [n] K-meter _fall values per upload, n <= n_chan; the _fall of every length
+    // met so far (host libm, tpk_km_fall), shared by this bank's own ragged calls and the DR-14 bank's
+    RaggedLen rag; std::vector<float> fall; std::vector<uint8_t> fall_ok;
+    bool rag_read = false;                  // the last process() block was a b200m_tpk_process_ragged_* one: read() skips its length-0 rows
     cudaStream_t own = nullptr; HostStage stage; bool last_host = false;
 };
 
@@ -2289,22 +2295,46 @@ static int tpk_process (b200m_tpk* h, const float* d_in, size_t stride, uint32_t
 }
 
 namespace b200m {
-// A ragged process() block always runs the exact fused kernel in its RAG form, whatever B200M_TPK_SPLIT / B200M_TPK_WIDE /
-// B200M_TPK_DEC would pick for a plain block: only that form stops each row at its own length.
+int tpk_upload_len (b200m_tpk* h, const uint32_t* len, uint32_t n, cudaStream_t st, const uint32_t** d_len, const float** d_fall)
+{
+    if (h->fall.empty ()) { h->fall.assign (B200M_MAX_BLOCK + 1, 0.0f); h->fall_ok.assign (B200M_MAX_BLOCK + 1, 0); }
+    cudaError_t e = cudaSuccess;
+    uint32_t* hl = h->rag.stage ((size_t)2 * h->n_chan, &e);
+    if (!hl) return cuda_fail (e, "tpk_upload_len", __FILE__, __LINE__);
+    float* hf = reinterpret_cast<float*> (hl + n);
+    memcpy (hl, len, n * sizeof (uint32_t));
+    for (uint32_t i = 0; i < n; ++i) {
+        const uint32_t L = len[i];
+        if (!h->fall_ok[L]) { h->fall[L] = tpk_km_fall (h, L); h->fall_ok[L] = 1; }      // once per length
+        hf[i] = h->fall[L];
+    }
+    e = h->rag.upload ((size_t)2 * n, st);
+    if (e != cudaSuccess) return cuda_fail (e, "tpk_upload_len", __FILE__, __LINE__);
+    *d_len = h->rag.d; *d_fall = reinterpret_cast<const float*> (h->rag.d + n);
+    return 0;
+}
+
+// A ragged process() block always runs the exact 16-channel kernel in its RAG form, whatever B200M_TPK_SPLIT / B200M_TPK_WIDE /
+// B200M_TPK_DEC or the precision mode would pick for a plain block: only that form stops each row at its own length.
 int tpk_process_ragged (b200m_tpk* h, const float* d_in, size_t stride, uint32_t nfram, cudaStream_t st, const uint32_t* d_len,
                         const float* d_fall, uint32_t per)
 {
-    if (!(h->flags & B200M_TPK_TRUEPEAK) || !(h->flags & B200M_TPK_KMETER)) return set_err (B200M_E_UNSUPPORTED, "ragged process() needs true peak and the K-meter");
-    if (h->fma) return set_err (B200M_E_UNSUPPORTED, "ragged process() blocks run in exact mode only");
-    const TpkDr drp = h->dr_on ? h->dr : TpkDr {};
+    const bool tp = h->flags & B200M_TPK_TRUEPEAK, km = h->flags & B200M_TPK_KMETER;
+    const TpkDr drp = h->dr_on && tp && km ? h->dr : TpkDr {};
     const TpkRag rag = {d_len, d_fall, (int)per};
     const int aligned = ((uintptr_t)d_in % 16 == 0) && (stride % 4 == 0);
     const unsigned grid = (h->n_chan + 15) / 16;
-    const size_t smem = TpkGeom<16, 64, true>::BYTES;
     const int n = (int)h->n_chan;
-#define TPK_RAG(IMMF, DRF) tpk_kernel<16, 64, true, false, true, IMMF, DRF, false, true><<<grid, TPK_THREADS, smem, st>>> (d_in, stride, 0, n, (int)nfram, aligned, h->elide0, h->prm, h->st, h->d_dbg, R128Hold {}, drp, rag)
-    if (h->imm) { if (drp.rms_sum) TPK_RAG (true, true); else TPK_RAG (true, false); }
-    else { if (drp.rms_sum) TPK_RAG (false, true); else TPK_RAG (false, false); }
+#define TPK_RAG(TPF, KMF, IMMF, DRF) tpk_kernel<16, 64, TPF, false, KMF, IMMF, DRF, false, true><<<grid, TPK_THREADS, TpkGeom<16, 64, TPF>::BYTES, st>>> ( \
+        d_in, stride, 0, n, (int)nfram, aligned, h->elide0, h->prm, h->st, h->d_dbg, R128Hold {}, drp, rag)
+    if (tp && km) {
+        if (h->imm) { if (drp.rms_sum) TPK_RAG (true, true, true, true); else TPK_RAG (true, true, true, false); }
+        else { if (drp.rms_sum) TPK_RAG (true, true, false, true); else TPK_RAG (true, true, false, false); }
+    }
+    // true peak alone: the coefficient-table form (the same products in the same order as the immediate form, which spills 8 bytes
+    // in this instantiation)
+    else if (tp) TPK_RAG (true, false, false, false);
+    else TPK_RAG (false, true, false, false);
 #undef TPK_RAG
     B200M_LAUNCHED (1);
     B200M_CUDA (cudaGetLastError ());
@@ -2509,6 +2539,7 @@ int b200m_tpk_destroy (b200m_tpk* h)
     for (void* p : ps) cudaFree (p);
     if (h->sb) cudaStreamDestroy (h->sb);
     for (int i = 0; i < 2; ++i) { if (h->ev_fir[i]) cudaEventDestroy (h->ev_fir[i]); if (h->ev_bal[i]) cudaEventDestroy (h->ev_bal[i]); }
+    h->rag.release ();
     h->stage.release ();
     if (h->own) cudaStreamDestroy (h->own);
     delete h;
@@ -2521,6 +2552,7 @@ int b200m_tpk_process_device (b200m_tpk* h, const float* d_in, size_t stride, ui
     if (tp_mode > 1) return set_err (B200M_E_INVAL, "bad tp_mode %u", tp_mode);
     DeviceGuard g (h->device);
     B200M_LEAVE_HOST_PATH (h);
+    h->rag_read = false;
     return tpk_process (h, d_in, stride, nfram, tp_mode, (cudaStream_t)stream);
 }
 
@@ -2534,7 +2566,43 @@ int b200m_tpk_process_host (b200m_tpk* h, const float* in, size_t stride, uint32
     B200M_CUDA (cudaMemcpy2DAsync (h->stage.d, h->stage.cap * sizeof (float), in, stride * sizeof (float),
                                    (size_t)nfram * sizeof (float), h->n_chan, cudaMemcpyHostToDevice, h->own));
     h->last_host = true;
+    h->rag_read = false;
     return tpk_process (h, h->stage.d, h->stage.cap, nfram, tp_mode, h->own);
+}
+
+// len (host, every entry <= nfram, some != nfram: ragged_check): channel i runs process() over its first len[i] frames
+static int tpk_ragged (b200m_tpk* h, const float* d_in, size_t stride, uint32_t nfram, const uint32_t* len, cudaStream_t st)
+{
+    const uint32_t* d_len = nullptr; const float* d_fall = nullptr;
+    if (int rc = tpk_upload_len (h, len, h->n_chan, st, &d_len, &d_fall)) return rc;
+    h->rag_read = true;
+    return tpk_process_ragged (h, d_in, stride, nfram, st, d_len, d_fall, 1);
+}
+
+int b200m_tpk_process_ragged_device (b200m_tpk* h, const float* d_in, size_t stride, uint32_t nfram, const uint32_t* len, void* stream)
+{
+    if (int rc = check_block_args (h, d_in, stride, nfram)) return rc;
+    const int rag = ragged_check (h->n_chan, nfram, len);
+    if (rag < 0) return rag;
+    if (!rag) return b200m_tpk_process_device (h, d_in, stride, nfram, B200M_TP_MODE_PROCESS, stream);   // every length is nfram
+    DeviceGuard g (h->device);
+    B200M_LEAVE_HOST_PATH (h);
+    return tpk_ragged (h, d_in, stride, nfram, len, (cudaStream_t)stream);
+}
+
+int b200m_tpk_process_ragged_host (b200m_tpk* h, const float* in, size_t stride, uint32_t nfram, const uint32_t* len)
+{
+    if (int rc = check_block_args (h, in, stride, nfram)) return rc;
+    const int rag = ragged_check (h->n_chan, nfram, len);
+    if (rag < 0) return rag;
+    if (!rag) return b200m_tpk_process_host (h, in, stride, nfram, B200M_TP_MODE_PROCESS);
+    DeviceGuard g (h->device);
+    B200M_ENTER_HOST_PATH (h);
+    if (h->stage.ensure (h->n_chan, nfram)) return set_err (B200M_E_NOMEM, "staging buffer allocation failed");
+    B200M_CUDA (cudaMemcpy2DAsync (h->stage.d, h->stage.cap * sizeof (float), in, stride * sizeof (float),
+                                   (size_t)nfram * sizeof (float), h->n_chan, cudaMemcpyHostToDevice, h->own));
+    h->last_host = true;
+    return tpk_ragged (h, h->stage.d, h->stage.cap, nfram, len, h->own);
 }
 
 int b200m_tpk_set_precision (b200m_tpk* h, int mode)
@@ -2550,6 +2618,7 @@ int b200m_tpk_read_device (b200m_tpk* h, void* stream)
 {
     if (!h) return set_err (B200M_E_INVAL, "NULL handle");
     DeviceGuard g (h->device);
+    if (h->rag_read) return tpk_read_ragged (h, tpk_stream (h, stream), h->rag.d, 1);     // rows with length 0 were not called
     tpk_read_kernel<<<(h->n_chan + 255) / 256, 256, 0, tpk_stream (h, stream)>>> ((int)h->n_chan, h->flags, h->st, h->d_res, nullptr, 1);
     B200M_LAUNCHED (1);
     B200M_CUDA (cudaGetLastError ());

@@ -34,9 +34,12 @@ const b200m_tpk_result* tpk_device_results (b200m_tpk* h);      // device array 
 int tpk_reset_inst (b200m_tpk* h, const uint32_t* d_inst, uint32_t n_sel, uint32_t per, bool clear, cudaStream_t st);
 // Kmeterdsp's _fall for a process() call of n frames, computed with the host libm as the reference does (kmeterdsp.cc:65-70)
 float tpk_km_fall (const b200m_tpk* h, uint32_t n);
+// Enqueue on `st` the upload of n <= n_chan lengths and their K-meter _fall values (tpk_km_fall, cached per length) through the
+// bank's pinned staging; *d_len and *d_fall are the device arrays the following kernels on `st` read.
+int tpk_upload_len (b200m_tpk* h, const uint32_t* len, uint32_t n, cudaStream_t st, const uint32_t** d_len, const float** d_fall);
 // A ragged process() block (with the DR accumulation set by tpk_set_dr): channel c belongs to instance c / per, which processes its
-// first d_len[c / per] <= nfram frames; d_fall[c / per] = tpk_km_fall (that length).  Length 0: the channel is not touched.  Exact
-// mode only (B200M_E_UNSUPPORTED in tolerance mode).  Device arrays, read by the kernels queued on `st`.
+// first d_len[c / per] <= nfram frames; d_fall[c / per] = tpk_km_fall (that length).  Length 0: the channel is not touched.  Always
+// the exact kernel, also in tolerance mode.  Device arrays, read by the kernels queued on `st`.
 int tpk_process_ragged (b200m_tpk* h, const float* d_in, size_t stride, uint32_t nfram, cudaStream_t st, const uint32_t* d_len,
                         const float* d_fall, uint32_t per);
 // b200m_tpk_read_device after a ragged block: the channels of instances with d_len 0 are not read
