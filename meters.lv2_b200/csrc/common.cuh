@@ -79,6 +79,12 @@ struct RaggedLen {
         slot ^= 1;
         return e;
     }
+    // stage() + the copy of len[0 .. n) + upload() on `st`: 0 with the lengths in d, or the error (set_err)
+    int put (const uint32_t* len, size_t n, cudaStream_t st) {
+        cudaError_t e = cudaSuccess;
+        if (uint32_t* hl = stage (n, &e)) { memcpy (hl, len, n * sizeof (uint32_t)); e = upload (n, st); }
+        return e == cudaSuccess ? 0 : cuda_fail (e, "RaggedLen::put", __FILE__, __LINE__);
+    }
     void release () {
         if (d) cudaFree (d);
         for (int s = 0; s < 2; ++s) { if (h[s]) cudaFreeHost (h[s]); if (ev[s]) cudaEventDestroy (ev[s]); h[s] = nullptr; ev[s] = nullptr; }
@@ -86,13 +92,51 @@ struct RaggedLen {
     }
 };
 
-// A bank switches to its own stream with the first *_host call; whatever the caller queued before that (controls on the
-// streams it passed) must not race with it: one device-wide synchronisation at the transition, nothing afterwards.
-#define B200M_ENTER_HOST_PATH(h) do { if (!(h)->last_host) B200M_CUDA (cudaDeviceSynchronize ()); } while (0)
-// ... and back: the bank's own stream does not synchronise with the caller's, so the first *_device call after *_host calls waits
-// for the own stream on the host (the host path's copies and kernels have then run); one wait at the transition, nothing afterwards.
-// Every device-path entry point goes through this; it also marks the bank as last driven on the device path.
-#define B200M_LEAVE_HOST_PATH(h) do { if ((h)->last_host) B200M_CUDA (cudaStreamSynchronize ((h)->own)); (h)->last_host = false; } while (0)
+// The host/device path policy of a bank, the one place that keeps the ordering promise of include/b200meters.h (Conventions).
+// A bank switches to its own stream with the first *_host call; whatever the caller queued before that (controls on the streams it
+// passed) must not race with it: one device-wide synchronisation at the transition, nothing afterwards.  And back: the bank's own
+// stream does not synchronise with the caller's, so the first *_device call after *_host calls waits for the own stream on the host
+// (the host path's copies and kernels have then run); one wait at the transition, nothing afterwards.
+struct BankPath {
+    cudaStream_t own = nullptr;          // the host path's copies and kernels
+    HostStage stage;                     // the device copy of a host-path block
+    bool last_host = false;              // the bank was last driven on the host path
+    // the stream of getters and controls: the bank's own after a host-path call, else the caller's
+    cudaStream_t stream (void* caller) const { return last_host ? own : (cudaStream_t)caller; }
+    int enter_device ();                 // every device-path call; waits for own at the switch
+    int enter_host ();                   // every host-path call; synchronises the device at the switch
+    // enter_host, then the copy of a host block (rows x nfram, row pitch stride) into the stage on `st` (normally own):
+    // *d / *dstride are the staged block
+    int stage_block (const float* in, size_t stride, uint32_t nfram, size_t rows, cudaStream_t st, const float** d, size_t* dstride);
+    void release ();                     // frees the stage and destroys own
+};
+
+inline int no_check () { return 0; }
+
+// One block call of a bank: the body of every *_process_* / *_run_* entry point, plain, _ctl_ and ragged, on both paths.  In order:
+// the block arguments; the bank's own check () (0 or an error); the n_len lengths `len` (NULL: every row runs nfram); the device,
+// the path switch and, on the host path, the staging copy of `rows` rows onto own (rows == 0: the bank copies the block itself).
+// Then run (d_in, stride, st, rlen): rlen is len if some length differs from nfram, else nullptr, and the call takes the plain
+// code path.  A refused call enqueues nothing and leaves the bank on its path.  rows and n_len are read from the handle by the
+// caller, which passes 0 for a NULL handle: the handle is dereferenced only after check_block_args.
+template <class Bank, class Check, class Run>
+int bank_call (Bank* h, const float* in, size_t stride, uint32_t nfram, bool host, void* stream, size_t rows, uint32_t n_len,
+               const uint32_t* len, Check check, Run run)
+{
+    if (int rc = check_block_args (h, in, stride, nfram)) return rc;
+    if (int rc = check ()) return rc;
+    const int rag = ragged_check (n_len, nfram, len);
+    if (rag < 0) return rag;
+    DeviceGuard g (h->device);
+    BankPath& p = h->path;
+    const float* d = in; size_t ds = stride; cudaStream_t st = (cudaStream_t)stream;
+    if (!host) { if (int rc = p.enter_device ()) return rc; }
+    else {
+        st = p.own;
+        if (int rc = rows ? p.stage_block (in, stride, nfram, rows, st, &d, &ds) : p.enter_host ()) return rc;
+    }
+    return run (d, ds, st, rag ? len : nullptr);
+}
 
 #ifdef __CUDACC__
 // ---------------------------------------------------------------- device helpers

@@ -284,10 +284,8 @@ struct b200m_cor {
     std::vector<uint32_t> len; RaggedLen rag;
     std::vector<uint32_t> ctl_len;         // b200m_cor_process_ctl_*: scratch for its lengths
     int attached = 0;                      // phasewheel banks feeding this one (b200m_pw_attach_cor): ragged calls are refused
-    cudaStream_t own = nullptr; HostStage stage; bool last_host = false;
+    BankPath path;
 };
-
-static cudaStream_t cor_stream (b200m_cor* h, void* stream) { return h->last_host ? h->own : (cudaStream_t)stream; }
 
 template <bool RAG>
 static int cor_launch (b200m_cor* h, const float* d_in, size_t stride, uint32_t nfram, cudaStream_t st, float* ring, int N, int rboff)
@@ -319,11 +317,9 @@ uint32_t cor_instances (const b200m_cor* h) { return h ? h->n_inst : 0; }
 int cor_follow (b200m_cor* h, bool host)
 {
     if (!h) return 0;
-    if (host) { B200M_ENTER_HOST_PATH (h); h->last_host = true; }
-    else B200M_LEAVE_HOST_PATH (h);
-    return 0;
+    return host ? h->path.enter_host () : h->path.enter_device ();
 }
-cudaStream_t cor_host_stream (const b200m_cor* h, cudaStream_t pw_own) { return h ? h->own : pw_own; }
+cudaStream_t cor_host_stream (const b200m_cor* h, cudaStream_t pw_own) { return h ? h->path.own : pw_own; }
 void cor_attach (b200m_cor* h, int d) { if (h) h->attached += d; }
 }
 
@@ -332,11 +328,7 @@ static int cor_process (b200m_cor* h, const float* d_in, size_t stride, uint32_t
 {
     if (!len) return cor_launch<false> (h, d_in, stride, nfram, st, nullptr, 0, 0);
     if (h->len.empty () || memcmp (len, h->len.data (), h->n_inst * sizeof (uint32_t))) {
-        cudaError_t e = cudaSuccess;
-        uint32_t* hl = h->rag.stage (h->n_inst, &e);
-        if (!hl) return cuda_fail (e, "cor_process", __FILE__, __LINE__);
-        memcpy (hl, len, h->n_inst * sizeof (uint32_t));
-        B200M_CUDA (h->rag.upload (h->n_inst, st));
+        if (int rc = h->rag.put (len, h->n_inst, st)) return rc;
         h->len.assign (len, len + h->n_inst);
     }
     return cor_launch<true> (h, d_in, stride, nfram, st, nullptr, 0, 0);
@@ -377,7 +369,7 @@ int b200m_cor_create (b200m_cor** out, int device, uint32_t n_inst, int fsamp, f
     if (e == cudaSuccess) e = cudaMemset (h->d_st, 0, (size_t)5 * n_inst * sizeof (float));
     if (e == cudaSuccess) e = cudaMalloc ((void**)&h->d_res, n_inst * sizeof (float));
     if (e == cudaSuccess) e = cudaMemset (h->d_res, 0, n_inst * sizeof (float));
-    if (e == cudaSuccess) e = cudaStreamCreateWithFlags (&h->own, cudaStreamNonBlocking);
+    if (e == cudaSuccess) e = cudaStreamCreateWithFlags (&h->path.own, cudaStreamNonBlocking);
     if (e != cudaSuccess) { int rc = cuda_fail (e, "cor_create", __FILE__, __LINE__); b200m_cor_destroy (h); return rc; }
     *out = h;
     return 0;
@@ -388,72 +380,54 @@ int b200m_cor_destroy (b200m_cor* h)
     if (!h) return 0;
     DeviceGuard g (h->device);
     cudaDeviceSynchronize ();
-    cudaFree (h->d_st); cudaFree (h->d_res); h->rag.release (); h->stage.release ();
-    if (h->own) cudaStreamDestroy (h->own);
+    cudaFree (h->d_st); cudaFree (h->d_res); h->rag.release (); h->path.release ();
     delete h;
     return 0;
 }
 
+// every block entry point; run: as b200m_cor_process_ctl_* (NULL: every pair runs); ragged: a b200m_cor_process_ragged_* call with
+// lengths len, refused while a phasewheel bank feeds this one
+static int cor_block (b200m_cor* h, const float* in, size_t stride, uint32_t nfram, const uint8_t* run, bool ragged, bool host, void* stream,
+                      const uint32_t* len)
+{
+    return bank_call (h, in, stride, nfram, host, stream, h ? (size_t)2 * h->n_inst : 0, h ? h->n_inst : 0, len,
+                      [&] {
+                          if (!ragged || !h->attached) return 0;
+                          return set_err (B200M_E_UNSUPPORTED, "ragged blocks: this correlation bank is attached to a phasewheel bank, whose ring advances bank-wide");
+                      },
+                      [&] (const float* d_in, size_t ds, cudaStream_t st, const uint32_t* rlen) {
+                          return cor_process (h, d_in, ds, nfram, rlen ? rlen : cor_ctl_len (h, nfram, run), st);
+                      });
+}
+
 int b200m_cor_process_ctl_device (b200m_cor* h, const float* d_in, size_t stride, uint32_t nfram, const uint8_t* run, void* stream)
 {
-    if (int rc = check_block_args (h, d_in, stride, nfram)) return rc;
-    DeviceGuard g (h->device);
-    B200M_LEAVE_HOST_PATH (h);
-    return cor_process (h, d_in, stride, nfram, cor_ctl_len (h, nfram, run), (cudaStream_t)stream);
+    return cor_block (h, d_in, stride, nfram, run, false, false, stream, nullptr);
 }
 
 int b200m_cor_process_device (b200m_cor* h, const float* d_in, size_t stride, uint32_t nfram, void* stream)
 {
-    return b200m_cor_process_ctl_device (h, d_in, stride, nfram, nullptr, stream);
+    return cor_block (h, d_in, stride, nfram, nullptr, false, false, stream, nullptr);
 }
 
 int b200m_cor_process_ctl_host (b200m_cor* h, const float* in, size_t stride, uint32_t nfram, const uint8_t* run)
 {
-    if (int rc = check_block_args (h, in, stride, nfram)) return rc;
-    DeviceGuard g (h->device);
-    B200M_ENTER_HOST_PATH (h);
-    if (h->stage.ensure ((size_t)2 * h->n_inst, nfram)) return set_err (B200M_E_NOMEM, "staging buffer allocation failed");
-    B200M_CUDA (cudaMemcpy2DAsync (h->stage.d, h->stage.cap * sizeof (float), in, stride * sizeof (float),
-                                   (size_t)nfram * sizeof (float), (size_t)2 * h->n_inst, cudaMemcpyHostToDevice, h->own));
-    h->last_host = true;
-    return cor_process (h, h->stage.d, h->stage.cap, nfram, cor_ctl_len (h, nfram, run), h->own);
+    return cor_block (h, in, stride, nfram, run, false, true, nullptr, nullptr);
 }
 
 int b200m_cor_process_host (b200m_cor* h, const float* in, size_t stride, uint32_t nfram)
 {
-    return b200m_cor_process_ctl_host (h, in, stride, nfram, nullptr);
-}
-
-// the checks of a ragged call: 1 ragged, 0 every length is nfram (the plain call), < 0 an error (nothing enqueued)
-static int cor_ragged_check (const b200m_cor* h, const void* in, size_t stride, uint32_t nfram, const uint32_t* len)
-{
-    if (int rc = check_block_args (h, in, stride, nfram)) return rc;
-    if (h->attached) return set_err (B200M_E_UNSUPPORTED, "ragged blocks: this correlation bank is attached to a phasewheel bank, whose ring advances bank-wide");
-    return ragged_check (h->n_inst, nfram, len);
+    return cor_block (h, in, stride, nfram, nullptr, false, true, nullptr, nullptr);
 }
 
 int b200m_cor_process_ragged_device (b200m_cor* h, const float* d_in, size_t stride, uint32_t nfram, const uint32_t* len, void* stream)
 {
-    const int rag = cor_ragged_check (h, d_in, stride, nfram, len);
-    if (rag < 0) return rag;
-    if (!rag) return b200m_cor_process_device (h, d_in, stride, nfram, stream);       // every length is nfram: the plain call
-    DeviceGuard g (h->device);
-    B200M_LEAVE_HOST_PATH (h);
-    return cor_process (h, d_in, stride, nfram, len, (cudaStream_t)stream);
+    return cor_block (h, d_in, stride, nfram, nullptr, true, false, stream, len);
 }
 
 int b200m_cor_process_ragged_host (b200m_cor* h, const float* in, size_t stride, uint32_t nfram, const uint32_t* len)
 {
-    const int rag = cor_ragged_check (h, in, stride, nfram, len);
-    if (rag < 0) return rag;
-    if (!rag) return b200m_cor_process_host (h, in, stride, nfram);
-    DeviceGuard g (h->device);
-    B200M_ENTER_HOST_PATH (h);
-    if (h->stage.ensure ((size_t)2 * h->n_inst, nfram)) return set_err (B200M_E_NOMEM, "staging buffer allocation failed");
-    B200M_CUDA (cudaMemcpy2DAsync (h->stage.d, h->stage.cap * sizeof (float), in, stride * sizeof (float),
-                                   (size_t)nfram * sizeof (float), (size_t)2 * h->n_inst, cudaMemcpyHostToDevice, h->own));
-    h->last_host = true;
-    return cor_process (h, h->stage.d, h->stage.cap, nfram, len, h->own);
+    return cor_block (h, in, stride, nfram, nullptr, true, true, nullptr, len);
 }
 
 int b200m_cor_set_precision (b200m_cor* h, int mode)
@@ -468,7 +442,7 @@ int b200m_cor_clear (b200m_cor* h, int32_t inst, void* stream)
     if (!h || inst < -1 || inst >= (int32_t)h->n_inst) return set_err (B200M_E_INVAL, "bad argument");
     DeviceGuard g (h->device);
     const int i0 = inst < 0 ? 0 : inst, n = inst < 0 ? (int)h->n_inst : 1;
-    cor_clear_kernel<<<(n + 127) / 128, 128, 0, cor_stream (h, stream)>>> ((int)h->n_inst, i0, n, h->d_st, h->d_res);
+    cor_clear_kernel<<<(n + 127) / 128, 128, 0, h->path.stream (stream)>>> ((int)h->n_inst, i0, n, h->d_st, h->d_res);
     B200M_LAUNCHED (1);
     B200M_CUDA (cudaGetLastError ());
     return 0;
@@ -478,7 +452,7 @@ int b200m_cor_results (b200m_cor* h, float* out, void* stream)
 {
     if (!h || !out) return set_err (B200M_E_INVAL, "NULL argument");
     DeviceGuard g (h->device);
-    cudaStream_t st = cor_stream (h, stream);
+    cudaStream_t st = h->path.stream (stream);
     B200M_CUDA (cudaMemcpyAsync (out, h->d_res, h->n_inst * sizeof (float), cudaMemcpyDeviceToHost, st));
     B200M_CUDA (cudaStreamSynchronize (st));
     return 0;
@@ -488,7 +462,7 @@ int b200m_cor_state (b200m_cor* h, float* state5, void* stream)
 {
     if (!h || !state5) return set_err (B200M_E_INVAL, "NULL argument");
     DeviceGuard g (h->device);
-    cudaStream_t st = cor_stream (h, stream);
+    cudaStream_t st = h->path.stream (stream);
     const size_t n = h->n_inst;
     float* tmp = (float*)malloc (5 * n * sizeof (float));
     if (!tmp) return set_err (B200M_E_NOMEM, "host allocation failed");

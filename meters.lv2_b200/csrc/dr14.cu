@@ -176,7 +176,7 @@ struct b200m_dr14 {
     uint32_t* d_sel = nullptr;                                 // instance list of a control call
     float *d_rms_sum = nullptr, *d_peak_cur = nullptr, *d_cd = nullptr;
     Dr14State st{}; b200m_dr14_result* d_out = nullptr;
-    cudaStream_t own = nullptr; HostStage stage; bool last_host = false;
+    BankPath path;
 };
 
 // reset_peaks of the instances d_inst[0 .. n_sel) (d_inst == nullptr: every instance), clear: and b200m_tpk_clear of their
@@ -286,7 +286,7 @@ int b200m_dr14_create (b200m_dr14** out, int device, uint32_t n_inst, uint32_t n
         }
         h->st.cd = h->d_cd;
     }
-    if (e == cudaSuccess) e = cudaStreamCreateWithFlags (&h->own, cudaStreamNonBlocking);
+    if (e == cudaSuccess) e = cudaStreamCreateWithFlags (&h->path.own, cudaStreamNonBlocking);
     if (e == cudaSuccess) {                                    // instantiate: m_rms = m_peak = -81 (:157-158)
         dr14_reset_kernel<<<(unsigned)((n_ch + 255) / 256), 256>>> (nullptr, n_inst, (int)n_channels, h->dr_mode, 0u, h->d_rms_sum, h->d_peak_cur, h->st);
         B200M_LAUNCHED (1);
@@ -306,59 +306,36 @@ int b200m_dr14_destroy (b200m_dr14* h)
     void* ps[] = {h->d_rms_sum, h->d_peak_cur, h->st.emit_rms, h->st.emit_peak, h->st.emit_valid, h->st.peak_hist, h->st.m_rms, h->st.m_peak,
                   h->st.m_dbtp, h->st.numfrag, h->st.phase, h->d_sel, h->st.hist, h->d_cd, h->d_out};
     for (void* p : ps) cudaFree (p);
-    h->stage.release ();
-    if (h->own) cudaStreamDestroy (h->own);
+    h->path.release ();
     delete h;
     return 0;
 }
 
+// every block entry point: one stream for the copy and every kernel, the true-peak bank driven on its device path on that stream
+static int dr14_block (b200m_dr14* h, const float* in, size_t stride, uint32_t nfram, bool host, void* stream, const uint32_t* len)
+{
+    return bank_call (h, in, stride, nfram, host, stream, h ? (size_t)h->n_inst * h->nch : 0, h ? h->n_inst : 0, len, no_check,
+                      [&] (const float* d_in, size_t ds, cudaStream_t st, const uint32_t* rlen) { return dr14_run (h, d_in, ds, nfram, st, rlen); });
+}
+
 int b200m_dr14_run_device (b200m_dr14* h, const float* d_in, size_t stride, uint32_t nfram, void* stream)
 {
-    if (int rc = check_block_args (h, d_in, stride, nfram)) return rc;
-    DeviceGuard g (h->device);
-    B200M_LEAVE_HOST_PATH (h);
-    return dr14_run (h, d_in, stride, nfram, (cudaStream_t)stream);
+    return dr14_block (h, d_in, stride, nfram, false, stream, nullptr);
 }
 
 int b200m_dr14_run_host (b200m_dr14* h, const float* in, size_t stride, uint32_t nfram)
 {
-    if (int rc = check_block_args (h, in, stride, nfram)) return rc;
-    DeviceGuard g (h->device);
-    B200M_ENTER_HOST_PATH (h);
-    // one stream for the copy and every kernel: stage here, then drive the true-peak bank's device path on it
-    const size_t n_ch = (size_t)h->n_inst * h->nch;
-    if (h->stage.ensure (n_ch, nfram)) return set_err (B200M_E_NOMEM, "staging buffer allocation failed");
-    B200M_CUDA (cudaMemcpy2DAsync (h->stage.d, h->stage.cap * sizeof (float), in, stride * sizeof (float), (size_t)nfram * sizeof (float), n_ch,
-                                   cudaMemcpyHostToDevice, h->own));
-    h->last_host = true;
-    return dr14_run (h, h->stage.d, h->stage.cap, nfram, h->own);
+    return dr14_block (h, in, stride, nfram, true, nullptr, nullptr);
 }
 
 int b200m_dr14_run_ragged_device (b200m_dr14* h, const float* d_in, size_t stride, uint32_t nfram, const uint32_t* len, void* stream)
 {
-    if (int rc = check_block_args (h, d_in, stride, nfram)) return rc;
-    const int rag = ragged_check (h->n_inst, nfram, len);
-    if (rag < 0) return rag;
-    if (!rag) return b200m_dr14_run_device (h, d_in, stride, nfram, stream);       // every length is nfram: the plain call
-    DeviceGuard g (h->device);
-    B200M_LEAVE_HOST_PATH (h);
-    return dr14_run (h, d_in, stride, nfram, (cudaStream_t)stream, len);
+    return dr14_block (h, d_in, stride, nfram, false, stream, len);
 }
 
 int b200m_dr14_run_ragged_host (b200m_dr14* h, const float* in, size_t stride, uint32_t nfram, const uint32_t* len)
 {
-    if (int rc = check_block_args (h, in, stride, nfram)) return rc;
-    const int rag = ragged_check (h->n_inst, nfram, len);
-    if (rag < 0) return rag;
-    if (!rag) return b200m_dr14_run_host (h, in, stride, nfram);
-    DeviceGuard g (h->device);
-    B200M_ENTER_HOST_PATH (h);
-    const size_t n_ch = (size_t)h->n_inst * h->nch;
-    if (h->stage.ensure (n_ch, nfram)) return set_err (B200M_E_NOMEM, "staging buffer allocation failed");
-    B200M_CUDA (cudaMemcpy2DAsync (h->stage.d, h->stage.cap * sizeof (float), in, stride * sizeof (float), (size_t)nfram * sizeof (float), n_ch,
-                                   cudaMemcpyHostToDevice, h->own));
-    h->last_host = true;
-    return dr14_run (h, h->stage.d, h->stage.cap, nfram, h->own, len);
+    return dr14_block (h, in, stride, nfram, true, nullptr, len);
 }
 
 int b200m_dr14_reset (b200m_dr14* h, void* stream)              // reset_peaks (:241-258), every instance
@@ -372,7 +349,7 @@ int b200m_dr14_control (b200m_dr14* h, const uint32_t* inst, uint32_t count, int
     if (cmd != B200M_DR14_RESET && cmd != B200M_DR14_CLEAR) return set_err (B200M_E_INVAL, "unknown control %d", cmd);
     if (!inst && count) return set_err (B200M_E_INVAL, "NULL instance list");
     DeviceGuard g (h->device);
-    cudaStream_t st = h->last_host ? h->own : (cudaStream_t)stream;
+    cudaStream_t st = h->path.stream (stream);
     if (!inst) {
         h->phase.assign (h->n_inst, h->tmod);
         h->phases.clear (); h->phases[h->tmod] = h->n_inst;
@@ -394,7 +371,7 @@ int b200m_dr14_results (b200m_dr14* h, b200m_dr14_result* out, void* stream)
 {
     if (!h || !out) return set_err (B200M_E_INVAL, "NULL argument");
     DeviceGuard g (h->device);
-    cudaStream_t st = h->last_host ? h->own : (cudaStream_t)stream;
+    cudaStream_t st = h->path.stream (stream);
     B200M_CUDA (cudaMemcpyAsync (out, h->d_out, (size_t)h->n_inst * sizeof (b200m_dr14_result), cudaMemcpyDeviceToHost, st));
     B200M_CUDA (cudaStreamSynchronize (st));
     return 0;
@@ -404,7 +381,7 @@ int b200m_dr14_histogram (b200m_dr14* h, uint32_t inst, uint32_t chan, uint32_t*
 {
     if (!h || !hist8000 || inst >= h->n_inst || chan >= h->nch || !h->dr_mode) return set_err (B200M_E_INVAL, "bad argument");
     DeviceGuard g (h->device);
-    cudaStream_t st = h->last_host ? h->own : (cudaStream_t)stream;
+    cudaStream_t st = h->path.stream (stream);
     B200M_CUDA (cudaMemcpyAsync (hist8000, h->st.hist + ((size_t)inst * h->nch + chan) * DR_HISTBINS, DR_HISTBINS * 4, cudaMemcpyDeviceToHost, st));
     B200M_CUDA (cudaStreamSynchronize (st));
     return 0;

@@ -689,7 +689,7 @@ struct b200m_ebu {
     float *d_z = nullptr, *d_frpwr = nullptr, *d_fragpw = nullptr, *d_ring = nullptr, *d_binpow = nullptr, *d_out5 = nullptr;
     EbuCtl* d_ctl = nullptr; b200m_ebu_result* d_res = nullptr;
     int *d_histM = nullptr, *d_histS = nullptr, *d_cnt = nullptr, *d_fph = nullptr;
-    cudaStream_t own = nullptr; HostStage stage; bool last_host = false;
+    BankPath path;
     bool use_tma = false;                // K1 tiles by TMA (opt-in, 16-byte aligned input only) instead of cp.async
     bool split = false;                  // K1 as two warps per 32 channels (ebu_kweight_split), opt-in with B200M_EBU_SPLIT=1: measured slower, see the kernel
     // Host mirror of every instance's S-histogram period (_div2, :234-241), kept in O(1) per fragment and phase class: the
@@ -699,10 +699,9 @@ struct b200m_ebu {
     std::vector<uint8_t> integ, base, frozen; std::vector<int> ph;
     std::map<int, EbuPhase> cls;
     std::vector<int> nf;                 // per class: fragments it completes in the block being launched (scratch)
-    // a ragged block (b200m_ebu_process_ragged_*): its per-instance lengths on the device, pinned staging for their upload (two
-    // slots, each reused only after its previous copy ran), and the instances whose length differs from nfram (scratch: index,
-    // fragments in the block, S-period position div2)
-    uint32_t* d_len = nullptr; uint32_t* h_len[2] = {nullptr, nullptr}; cudaEvent_t ev_len[2] = {nullptr, nullptr}; int len_slot = 0;
+    // a ragged block (b200m_ebu_process_ragged_*, b200m_r128_run_ragged_*): the upload of its per-instance lengths, and the instances
+    // whose length differs from nfram (scratch: index, fragments in the block, S-period position div2)
+    RaggedLen rag;
     struct Rag { uint32_t i; int nf, d2; };
     std::vector<Rag> rg;
     void phase_reset () {
@@ -800,7 +799,7 @@ static int ebu_ctl (b200m_ebu* h, int32_t inst, int cmd, void* stream)
     if (cmd == 3) { if (inst < 0) h->phase_reset (); else h->phase_restart ((uint32_t)inst); }
     else h->phase_ctl (inst, cmd);
     // after process_host the bank runs on its own stream: a control on any other stream would race with the kernels in flight
-    ebu_ctl_kernel<<<(h->n_inst + 127) / 128, 128, 0, h->last_host ? h->own : (cudaStream_t)stream>>> (
+    ebu_ctl_kernel<<<(h->n_inst + 127) / 128, 128, 0, h->path.stream (stream)>>> (
         (int)h->n_inst, inst, cmd, (int)h->nchan, h->d_z, h->d_frpwr, h->d_ring, h->d_ctl, h->d_res, h->d_histM, h->d_histS, h->d_cnt,
         h->d_fph, cmd == 3 ? h->tmod : -1);
     B200M_LAUNCHED (1);
@@ -872,13 +871,8 @@ static int ebu_create (b200m_ebu** out, int device, uint32_t n_inst, uint32_t nc
     A ((void**)&h->d_histS, (size_t)HIST_PITCH * n_inst * sizeof (int));
     A ((void**)&h->d_cnt, (size_t)4 * n_inst * sizeof (int));
     A ((void**)&h->d_fph, n_inst * sizeof (int));
-    A ((void**)&h->d_len, n_inst * sizeof (uint32_t));
-    for (int s = 0; s < 2; ++s) {
-        if (e == cudaSuccess) e = cudaHostAlloc ((void**)&h->h_len[s], n_inst * sizeof (uint32_t), cudaHostAllocDefault);
-        if (e == cudaSuccess) e = cudaEventCreateWithFlags (&h->ev_len[s], cudaEventDisableTiming);
-    }
     if (e == cudaSuccess) e = cudaMemcpy (h->d_binpow, bp, sizeof (bp), cudaMemcpyHostToDevice);
-    if (e == cudaSuccess) e = cudaStreamCreateWithFlags (&h->own, cudaStreamNonBlocking);
+    if (e == cudaSuccess) e = cudaStreamCreateWithFlags (&h->path.own, cudaStreamNonBlocking);
     // K1 carries 102 KB of dynamic shared memory per CTA
     // ... and asks for the largest shared-memory carveout: with the default the driver configures the SM for just what this kernel
     // needs (132 KB), which leaves room for ONE CTA of the true-peak kernel that is meant to share the SM with it (r128.cu)
@@ -963,10 +957,8 @@ int b200m_ebu_destroy (b200m_ebu* h)
     cudaDeviceSynchronize ();
     cudaFree (h->d_z); cudaFree (h->d_frpwr); cudaFree (h->d_fragpw); cudaFree (h->d_ring); cudaFree (h->d_binpow);
     cudaFree (h->d_out5); cudaFree (h->d_ctl); cudaFree (h->d_res); cudaFree (h->d_histM); cudaFree (h->d_histS); cudaFree (h->d_cnt); cudaFree (h->d_fph);
-    cudaFree (h->d_len);
-    for (int s = 0; s < 2; ++s) { if (h->h_len[s]) cudaFreeHost (h->h_len[s]); if (h->ev_len[s]) cudaEventDestroy (h->ev_len[s]); }
-    h->stage.release ();
-    if (h->own) cudaStreamDestroy (h->own);
+    h->rag.release ();
+    h->path.release ();
     delete h;
     return 0;
 }
@@ -984,7 +976,7 @@ int b200m_ebu_clear (b200m_ebu* h, int32_t inst, void* stream)
     if (!h || inst < 0 || inst >= (int32_t)h->n_inst) return set_err (B200M_E_INVAL, "bad argument");
     DeviceGuard g (h->device);
     h->phase_ctl (inst, 0); h->phase_ctl (inst, 2);
-    ebu_ctl_kernel<<<(h->n_inst + 127) / 128, 128, 0, h->last_host ? h->own : (cudaStream_t)stream>>> (
+    ebu_ctl_kernel<<<(h->n_inst + 127) / 128, 128, 0, h->path.stream (stream)>>> (
         (int)h->n_inst, inst, 3, (int)h->nchan, h->d_z, h->d_frpwr, h->d_ring, h->d_ctl, h->d_res, h->d_histM, h->d_histS, h->d_cnt,
         h->d_fph, -1);
     B200M_LAUNCHED (1);
@@ -1024,8 +1016,8 @@ bool ebu_single_k1 (const b200m_ebu* h, uint32_t nfram)
 // fragment/gating kernels run once, after the last slice.
 // `k1_fused`, when given (one slice, a block whose chunk list fits one launch: ebu_single_k1), launches a kernel that does
 // K1's work over the whole bank in its place; `after_k1` is enqueued right behind the first K1 launch.
-// `len` (host) / `d_len` (its copy on the device, ebu_upload_len): a ragged block, instance i processes its first len[i] frames (some
-// len[i] differs from nfram: ebu_ragged_check); nullptr: every instance processes nfram.
+// `len` (host) / `d_len` (its copy on the device, ebu_lens): a ragged block, instance i processes its first len[i] frames (some
+// len[i] differs from nfram: ragged_check); nullptr: every instance processes nfram.
 int ebu_process_sliced (b200m_ebu* h, const float* d_in, size_t stride, uint32_t nfram, cudaStream_t st,
                         int nsl, const uint32_t* bounds, cudaEvent_t* ready, int (*after_k1) (void*), void* after_arg,
                         int (*k1_fused) (void*, const EbuK1Args&), const uint32_t* len, const uint32_t* d_len)
@@ -1132,88 +1124,41 @@ int ebu_process_sliced (b200m_ebu* h, const float* d_in, size_t stride, uint32_t
 static int ebu_process (b200m_ebu* h, const float* d_in, size_t stride, uint32_t nfram, cudaStream_t st, const uint32_t* len = nullptr)
 {
     const uint32_t bounds[2] = {0, h->n_inst};
-    const uint32_t* d_len = len ? ebu_upload_len (h, len, st) : nullptr;
-    if (len && !d_len) return B200M_E_CUDA;
-    return ebu_process_sliced (h, d_in, stride, nfram, st, 1, bounds, nullptr, nullptr, nullptr, nullptr, len, d_len);
+    if (len) if (int rc = h->rag.put (len, h->n_inst, st)) return rc;
+    return ebu_process_sliced (h, d_in, stride, nfram, st, 1, bounds, nullptr, nullptr, nullptr, nullptr, len, len ? h->rag.d : nullptr);
 }
 
-int ebu_ragged_check (const b200m_ebu* h, uint32_t nfram, const uint32_t* len)
+static int ebu_block (b200m_ebu* h, const float* in, size_t stride, uint32_t nfram, bool host, void* stream, const uint32_t* len)
 {
-    if (!len) return 0;
-    bool rag = false;
-    for (uint32_t i = 0; i < h->n_inst; ++i) {
-        if (len[i] > nfram) return set_err (B200M_E_INVAL, "len[%u] = %u exceeds nfram = %u", i, len[i], nfram);
-        rag |= len[i] != nfram;
-    }
-    return rag ? 1 : 0;
-}
-
-const uint32_t* ebu_upload_len (b200m_ebu* h, const uint32_t* len, cudaStream_t st)
-{
-    // pinned staging: the copy is truly asynchronous, and the slot's previous copy has run before it is overwritten
-    const int s = h->len_slot; h->len_slot ^= 1;
-    cudaError_t e = cudaEventSynchronize (h->ev_len[s]);
-    if (e == cudaSuccess) { memcpy (h->h_len[s], len, h->n_inst * sizeof (uint32_t)); e = cudaMemcpyAsync (h->d_len, h->h_len[s], h->n_inst * sizeof (uint32_t), cudaMemcpyHostToDevice, st); }
-    if (e == cudaSuccess) e = cudaEventRecord (h->ev_len[s], st);
-    if (e != cudaSuccess) { cuda_fail (e, "ebu_upload_len", __FILE__, __LINE__); return nullptr; }
-    return h->d_len;
+    return bank_call (h, in, stride, nfram, host, stream, h ? (size_t)h->n_inst * h->nchan : 0, h ? h->n_inst : 0, len, no_check,
+                      [&] (const float* d_in, size_t ds, cudaStream_t st, const uint32_t* rlen) { return ebu_process (h, d_in, ds, nfram, st, rlen); });
 }
 
 int b200m_ebu_process_device (b200m_ebu* h, const float* d_in, size_t stride, uint32_t nfram, void* stream)
 {
-    if (int rc = check_block_args (h, d_in, stride, nfram)) return rc;
-    DeviceGuard g (h->device);
-    B200M_LEAVE_HOST_PATH (h);
-    return ebu_process (h, d_in, stride, nfram, (cudaStream_t)stream);
+    return ebu_block (h, d_in, stride, nfram, false, stream, nullptr);
 }
 
 int b200m_ebu_process_host (b200m_ebu* h, const float* in, size_t stride, uint32_t nfram)
 {
-    if (int rc = check_block_args (h, in, stride, nfram)) return rc;
-    DeviceGuard g (h->device);
-    B200M_ENTER_HOST_PATH (h);
-    const size_t nch = (size_t)h->n_inst * h->nchan;
-    if (h->stage.ensure (nch, nfram)) return set_err (B200M_E_NOMEM, "staging buffer allocation failed");
-    B200M_CUDA (cudaMemcpy2DAsync (h->stage.d, h->stage.cap * sizeof (float), in, stride * sizeof (float),
-                                   (size_t)nfram * sizeof (float), nch, cudaMemcpyHostToDevice, h->own));
-    h->last_host = true;
-    return ebu_process (h, h->stage.d, h->stage.cap, nfram, h->own);
+    return ebu_block (h, in, stride, nfram, true, nullptr, nullptr);
 }
 
 int b200m_ebu_process_ragged_device (b200m_ebu* h, const float* d_in, size_t stride, uint32_t nfram, const uint32_t* len, void* stream)
 {
-    if (int rc = check_block_args (h, d_in, stride, nfram)) return rc;
-    const int rag = ebu_ragged_check (h, nfram, len);
-    if (rag < 0) return rag;
-    if (!rag) return b200m_ebu_process_device (h, d_in, stride, nfram, stream);      // every length is nfram: the plain call
-    DeviceGuard g (h->device);
-    B200M_LEAVE_HOST_PATH (h);
-    return ebu_process (h, d_in, stride, nfram, (cudaStream_t)stream, len);
+    return ebu_block (h, d_in, stride, nfram, false, stream, len);
 }
 
 int b200m_ebu_process_ragged_host (b200m_ebu* h, const float* in, size_t stride, uint32_t nfram, const uint32_t* len)
 {
-    if (int rc = check_block_args (h, in, stride, nfram)) return rc;
-    const int rag = ebu_ragged_check (h, nfram, len);
-    if (rag < 0) return rag;
-    if (!rag) return b200m_ebu_process_host (h, in, stride, nfram);
-    DeviceGuard g (h->device);
-    B200M_ENTER_HOST_PATH (h);
-    const size_t nch = (size_t)h->n_inst * h->nchan;
-    if (h->stage.ensure (nch, nfram)) return set_err (B200M_E_NOMEM, "staging buffer allocation failed");
-    B200M_CUDA (cudaMemcpy2DAsync (h->stage.d, h->stage.cap * sizeof (float), in, stride * sizeof (float),
-                                   (size_t)nfram * sizeof (float), nch, cudaMemcpyHostToDevice, h->own));
-    h->last_host = true;
-    return ebu_process (h, h->stage.d, h->stage.cap, nfram, h->own, len);
+    return ebu_block (h, in, stride, nfram, true, nullptr, len);
 }
-
-static cudaStream_t ebu_stream (b200m_ebu* h, void* stream) { return h->last_host ? h->own : (cudaStream_t)stream; }
 
 int b200m_ebu_results (b200m_ebu* h, b200m_ebu_result* out, void* stream)
 {
     if (!h || !out) return set_err (B200M_E_INVAL, "NULL argument");
     DeviceGuard g (h->device);
-    cudaStream_t st = ebu_stream (h, stream);
+    cudaStream_t st = h->path.stream (stream);
     B200M_CUDA (cudaMemcpyAsync (out, h->d_res, h->n_inst * sizeof (b200m_ebu_result), cudaMemcpyDeviceToHost, st));
     B200M_CUDA (cudaStreamSynchronize (st));
     return 0;
@@ -1223,7 +1168,7 @@ int b200m_ebu_histogram (b200m_ebu* h, uint32_t inst, int32_t* hist_M, int32_t* 
 {
     if (!h || !hist_M || !hist_S || inst >= h->n_inst) return set_err (B200M_E_INVAL, "bad argument");
     DeviceGuard g (h->device);
-    cudaStream_t st = ebu_stream (h, stream);
+    cudaStream_t st = h->path.stream (stream);
     B200M_CUDA (cudaMemcpyAsync (hist_M, h->d_histM + (size_t)inst * HIST_PITCH, 751 * sizeof (int), cudaMemcpyDeviceToHost, st));
     B200M_CUDA (cudaMemcpyAsync (hist_S, h->d_histS + (size_t)inst * HIST_PITCH, 751 * sizeof (int), cudaMemcpyDeviceToHost, st));
     B200M_CUDA (cudaStreamSynchronize (st));
@@ -1267,7 +1212,7 @@ int b200m_ebu_snapshot (b200m_ebu* h, void* buf, size_t bytes, void* stream)
 {
     if (!h || !buf || bytes < b200m_ebu_snapshot_size (h)) return set_err (B200M_E_INVAL, "bad argument / buffer too small");
     DeviceGuard g (h->device);
-    cudaStream_t st = ebu_stream (h, stream);
+    cudaStream_t st = h->path.stream (stream);
     uint8_t* o = (uint8_t*)buf;
     EbuSnapHead hd = {h->weighted ? EBU_SNAP_MAGIC_W : EBU_SNAP_MAGIC, h->n_inst, h->nchan, h->fsamp, h->tmod, {0, 0, 0}};
     memcpy (o, &hd, sizeof (hd)); o += sizeof (hd);
@@ -1292,7 +1237,7 @@ int b200m_ebu_restore (b200m_ebu* h, const void* buf, size_t bytes, void* stream
     if (h->weighted && memcmp ((const uint8_t*)buf + sizeof (hd), h->gw.g, sizeof (h->gw.g)) != 0)
         return set_err (B200M_E_INVAL, "snapshot of a bank with other channel weights");
     DeviceGuard g (h->device);
-    cudaStream_t st = ebu_stream (h, stream);
+    cudaStream_t st = h->path.stream (stream);
     const uint8_t* o = (const uint8_t*)buf + ebu_head_bytes (h);
     const size_t n = h->n_inst;
     h->tmod = hd.tmod;
@@ -1322,7 +1267,7 @@ int b200m_ebu_state (b200m_ebu* h, uint32_t inst, float* z, float* power64, floa
 {
     if (!h || !z || !power64 || !frpwr || !c4 || inst >= h->n_inst) return set_err (B200M_E_INVAL, "bad argument");
     DeviceGuard g (h->device);
-    cudaStream_t st = ebu_stream (h, stream);
+    cudaStream_t st = h->path.stream (stream);
     const size_t nch = (size_t)h->n_inst * h->nchan;
     for (uint32_t c = 0; c < h->nchan; ++c)
         for (int q = 0; q < 4; ++q)
@@ -1340,7 +1285,7 @@ int b200m_ebu_mix_reduce (b200m_ebu* h, int32_t* d_out, void* stream)
 {
     if (!h || !d_out) return set_err (B200M_E_INVAL, "NULL argument");
     DeviceGuard g (h->device);
-    cudaStream_t st = ebu_stream (h, stream);
+    cudaStream_t st = h->path.stream (stream);
     B200M_CUDA (cudaMemsetAsync (d_out, 0, B200M_MIX_WORDS * sizeof (int32_t), st));
     const unsigned slices = (unsigned)std::min<uint32_t> (h->n_inst, 128u);      // ~24 x 128 CTAs: enough loads in flight to stream the histograms
     ebu_mix_reduce_kernel<<<dim3 ((B200M_MIX_WORDS + 63) / 64, slices), 64, 0, st>>> ((int)h->n_inst, h->d_histM, h->d_histS, h->d_cnt, d_out);
@@ -1353,7 +1298,7 @@ int b200m_ebu_mix_finish (b200m_ebu* h, const int32_t* d_mix, float out5[5], voi
 {
     if (!h || !d_mix || !out5) return set_err (B200M_E_INVAL, "NULL argument");
     DeviceGuard g (h->device);
-    cudaStream_t st = ebu_stream (h, stream);
+    cudaStream_t st = h->path.stream (stream);
     ebu_mix_finish_kernel<<<1, 32, 0, st>>> (d_mix, h->d_binpow, h->d_out5);
     B200M_LAUNCHED (1);
     B200M_CUDA (cudaMemcpyAsync (out5, h->d_out5, 5 * sizeof (float), cudaMemcpyDeviceToHost, st));
@@ -1362,3 +1307,5 @@ int b200m_ebu_mix_finish (b200m_ebu* h, const int32_t* d_mix, float out5[5], voi
 }
 
 }  // extern "C"
+
+RaggedLen& ebu_lens (b200m_ebu* h) { return h->rag; }

@@ -240,8 +240,5 @@ extern "C" bool ebu_single_k1 (const b200m_ebu* h, uint32_t nfram);
 extern "C" int ebu_process_sliced (b200m_ebu* h, const float* d_in, size_t stride, uint32_t nfram, cudaStream_t st, int nsl, const uint32_t* bounds,
                                    cudaEvent_t* ready, int (*after_k1) (void*), void* after_arg, int (*k1_fused) (void*, const b200m::EbuK1Args&),
                                    const uint32_t* len = nullptr, const uint32_t* d_len = nullptr);
-// host side, ebu.cu: per-instance lengths of a ragged block (b200m_ebu_process_ragged_*).  ebu_ragged_check: 1 if some len[i] differs
-// from nfram, 0 if none does (or len is NULL: the plain call), B200M_E_INVAL if one exceeds nfram.  ebu_upload_len: enqueue the
-// copy of len[0 .. n_inst) on st into the bank's device array, which it returns (nullptr on a CUDA error, reported by set_err)
-extern "C" int ebu_ragged_check (const b200m_ebu* h, uint32_t nfram, const uint32_t* len);
-extern "C" const uint32_t* ebu_upload_len (b200m_ebu* h, const uint32_t* len, cudaStream_t st);
+// host side, ebu.cu: the upload of a ragged block's per-instance lengths (b200m_ebu_process_ragged_*, and the EBUr128 cycle's)
+b200m::RaggedLen& ebu_lens (b200m_ebu* h);

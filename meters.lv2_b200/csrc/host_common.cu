@@ -49,6 +49,37 @@ int ragged_check (uint32_t n, uint32_t nfram, const uint32_t* len)
     return rag ? 1 : 0;
 }
 
+int BankPath::enter_device ()
+{
+    if (last_host) B200M_CUDA (cudaStreamSynchronize (own));
+    last_host = false;
+    return 0;
+}
+
+int BankPath::enter_host ()
+{
+    if (!last_host) B200M_CUDA (cudaDeviceSynchronize ());
+    last_host = true;
+    return 0;
+}
+
+int BankPath::stage_block (const float* in, size_t stride, uint32_t nfram, size_t rows, cudaStream_t st, const float** d, size_t* dstride)
+{
+    if (int rc = enter_host ()) return rc;
+    if (stage.ensure (rows, nfram)) return set_err (B200M_E_NOMEM, "staging buffer allocation failed");
+    B200M_CUDA (cudaMemcpy2DAsync (stage.d, stage.cap * sizeof (float), in, stride * sizeof (float), (size_t)nfram * sizeof (float), rows,
+                                   cudaMemcpyHostToDevice, st));
+    *d = stage.d; *dstride = stage.cap;
+    return 0;
+}
+
+void BankPath::release ()
+{
+    stage.release ();
+    if (own) cudaStreamDestroy (own);
+    own = nullptr;
+}
+
 }  // namespace b200m
 
 using namespace b200m;

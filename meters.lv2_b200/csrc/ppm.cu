@@ -185,7 +185,7 @@ struct b200m_ppm {
     float2* d_mv = nullptr; bool mv_dirty = false;        // d_mv is rewritten by the next process call
     float *d_z1 = nullptr, *d_z2 = nullptr, *d_m = nullptr, *d_out = nullptr; int* d_res = nullptr;
     RaggedLen rag; bool rag_read = false;                 // ragged blocks: lengths per unit; the last block was ragged (read skips length 0)
-    cudaStream_t own = nullptr; HostStage stage; bool last_host = false;
+    BankPath path;
 };
 
 static void ppm_design (int kind, float fs, float w[4])
@@ -195,19 +195,11 @@ static void ppm_design (int kind, float fs, float w[4])
     else                             { w[0] = 200.0f / fs; w[1] = 860.0f / fs;  w[2] = 1.0f - 4.0f / fs; w[3] = 0.5141f; }            // iec2ppmdsp.cc:93-99, msppmdsp.cc:127-133
 }
 
-static cudaStream_t ppm_stream (b200m_ppm* h, void* stream) { return h->last_host ? h->own : (cudaStream_t)stream; }
-
 // len (host, every entry <= nfram, some != nfram: ragged_check): unit u runs over its first len[u] frames; nullptr: every unit nfram
 static int ppm_process (b200m_ppm* h, const float* d_in, size_t stride, uint32_t nfram, cudaStream_t st, const uint32_t* len = nullptr)
 {
     h->rag_read = len != nullptr;
-    if (len) {
-        cudaError_t e = cudaSuccess;
-        uint32_t* hl = h->rag.stage (h->n_units, &e);
-        if (!hl) return cuda_fail (e, "ppm_process", __FILE__, __LINE__);
-        memcpy (hl, len, h->n_units * sizeof (uint32_t));
-        B200M_CUDA (h->rag.upload (h->n_units, st));
-    }
+    if (len) if (int rc = h->rag.put (len, h->n_units, st)) return rc;
     if (h->mv_dirty) {
         B200M_CUDA (cudaMemcpyAsync (h->d_mv, h->mv.data (), h->n_units * sizeof (float2), cudaMemcpyHostToDevice, st));
         h->mv_dirty = false;
@@ -264,7 +256,7 @@ int b200m_ppm_create (b200m_ppm** out, int device, uint32_t n_units, float fsamp
     const size_t nm = h->n_meters;
     A ((void**)&h->d_z1, nm * 4); A ((void**)&h->d_z2, nm * 4); A ((void**)&h->d_m, nm * 4); A ((void**)&h->d_out, nm * 4); A ((void**)&h->d_res, nm * 4);
     if (kind == B200M_PPM_MS) A ((void**)&h->d_mv, n_units * sizeof (float2));
-    if (e == cudaSuccess) e = cudaStreamCreateWithFlags (&h->own, cudaStreamNonBlocking);
+    if (e == cudaSuccess) e = cudaStreamCreateWithFlags (&h->path.own, cudaStreamNonBlocking);
     const int smem_max = PPM_WARPS * PPM_STAGES * 2 * PPM_PLANE * (int)sizeof (float);
 #define PPM_ATTR(K, A) if (e == cudaSuccess) e = cudaFuncSetAttribute (ppm_kernel<K, A>, cudaFuncAttributeMaxDynamicSharedMemorySize, smem_max); \
                        if (e == cudaSuccess) e = cudaFuncSetAttribute (ppm_kernel<K, A, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, smem_max)
@@ -285,8 +277,7 @@ int b200m_ppm_destroy (b200m_ppm* h)
     if (!h) return 0;
     DeviceGuard g (h->device);
     cudaDeviceSynchronize ();
-    cudaFree (h->d_z1); cudaFree (h->d_z2); cudaFree (h->d_m); cudaFree (h->d_out); cudaFree (h->d_res); cudaFree (h->d_mv); h->stage.release (); h->rag.release ();
-    if (h->own) cudaStreamDestroy (h->own);
+    cudaFree (h->d_z1); cudaFree (h->d_z2); cudaFree (h->d_m); cudaFree (h->d_out); cudaFree (h->d_res); cudaFree (h->d_mv); h->rag.release (); h->path.release ();
     delete h;
     return 0;
 }
@@ -314,7 +305,7 @@ int b200m_ppm_clear (b200m_ppm* h, int32_t unit, void* stream)
     DeviceGuard g (h->device);
     const int per = h->kind == B200M_PPM_MS ? 2 : 1;
     const int m0 = unit < 0 ? 0 : per * unit, nm = unit < 0 ? (int)h->n_meters : per;
-    ppm_clear_kernel<<<(nm + 255) / 256, 256, 0, ppm_stream (h, stream)>>> (m0, nm, h->d_z1, h->d_z2, h->d_m, h->d_out, h->d_res);
+    ppm_clear_kernel<<<(nm + 255) / 256, 256, 0, h->path.stream (stream)>>> (m0, nm, h->d_z1, h->d_z2, h->d_m, h->d_out, h->d_res);
     B200M_LAUNCHED (1);
     B200M_CUDA (cudaGetLastError ());
     if (h->kind == B200M_PPM_MS) {                         // the constructor's gains: a fresh Msppmdsp (-6) pair
@@ -325,52 +316,30 @@ int b200m_ppm_clear (b200m_ppm* h, int32_t unit, void* stream)
     return 0;
 }
 
+static int ppm_block (b200m_ppm* h, const float* in, size_t stride, uint32_t nfram, bool host, void* stream, const uint32_t* len)
+{
+    return bank_call (h, in, stride, nfram, host, stream, h ? h->n_meters : 0, h ? h->n_units : 0, len, no_check,
+                      [&] (const float* d_in, size_t ds, cudaStream_t st, const uint32_t* rlen) { return ppm_process (h, d_in, ds, nfram, st, rlen); });
+}
+
 int b200m_ppm_process_device (b200m_ppm* h, const float* d_in, size_t stride, uint32_t nfram, void* stream)
 {
-    if (int rc = check_block_args (h, d_in, stride, nfram)) return rc;
-    DeviceGuard g (h->device);
-    B200M_LEAVE_HOST_PATH (h);
-    return ppm_process (h, d_in, stride, nfram, (cudaStream_t)stream);
+    return ppm_block (h, d_in, stride, nfram, false, stream, nullptr);
 }
 
 int b200m_ppm_process_host (b200m_ppm* h, const float* in, size_t stride, uint32_t nfram)
 {
-    if (int rc = check_block_args (h, in, stride, nfram)) return rc;
-    DeviceGuard g (h->device);
-    B200M_ENTER_HOST_PATH (h);
-    const size_t rows = h->kind == B200M_PPM_MS ? (size_t)2 * h->n_units : h->n_units;
-    if (h->stage.ensure (rows, nfram)) return set_err (B200M_E_NOMEM, "staging buffer allocation failed");
-    B200M_CUDA (cudaMemcpy2DAsync (h->stage.d, h->stage.cap * sizeof (float), in, stride * sizeof (float),
-                                   (size_t)nfram * sizeof (float), rows, cudaMemcpyHostToDevice, h->own));
-    h->last_host = true;
-    return ppm_process (h, h->stage.d, h->stage.cap, nfram, h->own);
+    return ppm_block (h, in, stride, nfram, true, nullptr, nullptr);
 }
 
 int b200m_ppm_process_ragged_device (b200m_ppm* h, const float* d_in, size_t stride, uint32_t nfram, const uint32_t* len, void* stream)
 {
-    if (int rc = check_block_args (h, d_in, stride, nfram)) return rc;
-    const int rag = ragged_check (h->n_units, nfram, len);
-    if (rag < 0) return rag;
-    if (!rag) return b200m_ppm_process_device (h, d_in, stride, nfram, stream);       // every length is nfram: the plain call
-    DeviceGuard g (h->device);
-    B200M_LEAVE_HOST_PATH (h);
-    return ppm_process (h, d_in, stride, nfram, (cudaStream_t)stream, len);
+    return ppm_block (h, d_in, stride, nfram, false, stream, len);
 }
 
 int b200m_ppm_process_ragged_host (b200m_ppm* h, const float* in, size_t stride, uint32_t nfram, const uint32_t* len)
 {
-    if (int rc = check_block_args (h, in, stride, nfram)) return rc;
-    const int rag = ragged_check (h->n_units, nfram, len);
-    if (rag < 0) return rag;
-    if (!rag) return b200m_ppm_process_host (h, in, stride, nfram);
-    DeviceGuard g (h->device);
-    B200M_ENTER_HOST_PATH (h);
-    const size_t rows = h->kind == B200M_PPM_MS ? (size_t)2 * h->n_units : h->n_units;
-    if (h->stage.ensure (rows, nfram)) return set_err (B200M_E_NOMEM, "staging buffer allocation failed");
-    B200M_CUDA (cudaMemcpy2DAsync (h->stage.d, h->stage.cap * sizeof (float), in, stride * sizeof (float),
-                                   (size_t)nfram * sizeof (float), rows, cudaMemcpyHostToDevice, h->own));
-    h->last_host = true;
-    return ppm_process (h, h->stage.d, h->stage.cap, nfram, h->own, len);
+    return ppm_block (h, in, stride, nfram, true, nullptr, len);
 }
 
 int b200m_ppm_read_device (b200m_ppm* h, void* stream)
@@ -379,9 +348,9 @@ int b200m_ppm_read_device (b200m_ppm* h, void* stream)
     DeviceGuard g (h->device);
     const unsigned grid = (h->n_meters + 255) / 256;
     if (h->rag_read)                                      // after a ragged block: units with length 0 were not called
-        ppm_read_kernel<true><<<grid, 256, 0, ppm_stream (h, stream)>>> ((int)h->n_meters, h->g, h->d_m, h->d_res, h->d_out, h->rag.d,
+        ppm_read_kernel<true><<<grid, 256, 0, h->path.stream (stream)>>> ((int)h->n_meters, h->g, h->d_m, h->d_res, h->d_out, h->rag.d,
                                                                           h->kind == B200M_PPM_MS ? 2 : 1);
-    else ppm_read_kernel<<<grid, 256, 0, ppm_stream (h, stream)>>> ((int)h->n_meters, h->g, h->d_m, h->d_res, h->d_out, nullptr, 1);
+    else ppm_read_kernel<<<grid, 256, 0, h->path.stream (stream)>>> ((int)h->n_meters, h->g, h->d_m, h->d_res, h->d_out, nullptr, 1);
     B200M_LAUNCHED (1);
     B200M_CUDA (cudaGetLastError ());
     return 0;
@@ -391,7 +360,7 @@ int b200m_ppm_results (b200m_ppm* h, float* out, void* stream)
 {
     if (!h || !out) return set_err (B200M_E_INVAL, "NULL argument");
     DeviceGuard g (h->device);
-    cudaStream_t st = ppm_stream (h, stream);
+    cudaStream_t st = h->path.stream (stream);
     B200M_CUDA (cudaMemcpyAsync (out, h->d_out, h->n_meters * sizeof (float), cudaMemcpyDeviceToHost, st));
     B200M_CUDA (cudaStreamSynchronize (st));
     return 0;
@@ -401,7 +370,7 @@ int b200m_ppm_state (b200m_ppm* h, float* state4, void* stream)
 {
     if (!h || !state4) return set_err (B200M_E_INVAL, "NULL argument");
     DeviceGuard g (h->device);
-    cudaStream_t st = ppm_stream (h, stream);
+    cudaStream_t st = h->path.stream (stream);
     const size_t nm = h->n_meters;
     float* tmp = (float*)malloc (4 * nm * sizeof (float));
     if (!tmp) return set_err (B200M_E_NOMEM, "host allocation failed");

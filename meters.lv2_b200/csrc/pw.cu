@@ -195,10 +195,11 @@ struct b200m_pw {
     float *d_ring = nullptr, *d_win = nullptr, *d_raw = nullptr, *d_phase = nullptr, *d_level = nullptr, *d_peak = nullptr;
     float2* d_tw = nullptr;
     b200m_cor* cor = nullptr;                              // attached correlation bank (fused feed), not owned
-    cudaStream_t own = nullptr; HostStage stage; bool last_host = false;
+    BankPath path;
 };
 
-static cudaStream_t pw_stream (b200m_pw* h, void* stream) { return h->last_host ? cor_host_stream (h->cor, h->own) : (cudaStream_t)stream; }
+// the host path of a phasewheel bank runs on its attached correlation bank's own stream, if it has one (cor_host_stream)
+static cudaStream_t pw_stream (b200m_pw* h, void* stream) { return h->path.last_host ? cor_host_stream (h->cor, h->path.own) : (cudaStream_t)stream; }
 static size_t pw_smem_bytes (uint32_t N) { return (size_t)12 * N; }   // 2 x N/2 float2 + 2 x N/2 float
 
 static int pw_process (b200m_pw* h, const float* d_in, size_t stride, uint32_t nfram, float db_thresh, int* fired, cudaStream_t st)
@@ -291,7 +292,7 @@ int b200m_pw_create (b200m_pw** out, int device, uint32_t n_inst, uint32_t fft_b
     if (e == cudaSuccess) e = cudaMemcpy (h->d_tw, tw, N * sizeof (float2), cudaMemcpyHostToDevice);
     free (win); free (tw);
     if (e == cudaSuccess) e = cudaFuncSetAttribute (pw_analyze_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)pw_smem_bytes (16384));
-    if (e == cudaSuccess) e = cudaStreamCreateWithFlags (&h->own, cudaStreamNonBlocking);
+    if (e == cudaSuccess) e = cudaStreamCreateWithFlags (&h->path.own, cudaStreamNonBlocking);
     if (e == cudaSuccess) {
         const size_t n = (size_t)n_inst * fft_bins;       // ui->level[i] = -100, ui->phase[i] = 0 (phasewheel.c:199-202)
         pw_init_kernel<<<(unsigned)((n + 255) / 256), 256>>> (n, h->d_level, h->d_phase, 0.0f);
@@ -309,8 +310,7 @@ int b200m_pw_destroy (b200m_pw* h)
     DeviceGuard g (h->device);
     cudaDeviceSynchronize ();
     cudaFree (h->d_ring); cudaFree (h->d_win); cudaFree (h->d_tw); cudaFree (h->d_raw); cudaFree (h->d_phase); cudaFree (h->d_level); cudaFree (h->d_peak);
-    h->stage.release ();
-    if (h->own) cudaStreamDestroy (h->own);
+    h->path.release ();
     delete h;
     return 0;
 }
@@ -336,7 +336,7 @@ int b200m_pw_process_device (b200m_pw* h, const float* d_in, size_t stride, uint
     if (int rc = check_block_args (h, d_in, stride, nfram)) return rc;
     DeviceGuard g (h->device);
     if (int rc = cor_follow (h->cor, false)) return rc;
-    B200M_LEAVE_HOST_PATH (h);      // while a correlation bank is attached h->own is idle: its host-path calls ran on cor_host_stream
+    if (int rc = h->path.enter_device ()) return rc;      // while a correlation bank is attached own is idle: its host-path calls ran on cor_host_stream
     return pw_process (h, d_in, stride, nfram, db_thresh, fired, (cudaStream_t)stream);
 }
 
@@ -344,14 +344,12 @@ int b200m_pw_process_host (b200m_pw* h, const float* in, size_t stride, uint32_t
 {
     if (int rc = check_block_args (h, in, stride, nfram)) return rc;
     DeviceGuard g (h->device);
-    B200M_ENTER_HOST_PATH (h);
+    if (int rc = h->path.enter_host ()) return rc;
     if (int rc = cor_follow (h->cor, true)) return rc;
-    if (h->stage.ensure ((size_t)2 * h->n_inst, nfram)) return set_err (B200M_E_NOMEM, "staging buffer allocation failed");
-    const cudaStream_t own = cor_host_stream (h->cor, h->own);
-    B200M_CUDA (cudaMemcpy2DAsync (h->stage.d, h->stage.cap * sizeof (float), in, stride * sizeof (float),
-                                   (size_t)nfram * sizeof (float), (size_t)2 * h->n_inst, cudaMemcpyHostToDevice, own));
-    h->last_host = true;
-    return pw_process (h, h->stage.d, h->stage.cap, nfram, db_thresh, fired, own);
+    const cudaStream_t st = cor_host_stream (h->cor, h->path.own);
+    const float* d_in; size_t ds;
+    if (int rc = h->path.stage_block (in, stride, nfram, (size_t)2 * h->n_inst, st, &d_in, &ds)) return rc;
+    return pw_process (h, d_in, ds, nfram, db_thresh, fired, st);
 }
 
 int b200m_pw_results (b200m_pw* h, float* phase, float* level, float* peak, void* stream)

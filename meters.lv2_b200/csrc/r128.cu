@@ -93,11 +93,11 @@ struct b200m_r128 {
     float* d_tpmax = nullptr;
     float* d_tplin = nullptr;            // 3 or 5 channels, weighted banks: every channel's read() of the cycle, folded by r128_hold_kernel
     R128Hold hold () const { return {d_tpmax, d_tplin, (int)nchan}; }
-    // own: EBU kernels + joins (host path);  side: true-peak kernels (run concurrently with the latency-bound EBU
+    // path.own: EBU kernels + joins (host path);  side: true-peak kernels (run concurrently with the latency-bound EBU
     // kernel);  copy: host->device slices, so that the copy of slice s+1 overlaps the kernels of slice s
-    cudaStream_t own = nullptr, side = nullptr, copy = nullptr;
+    BankPath path; cudaStream_t side = nullptr, copy = nullptr;
     cudaEvent_t ev_tp = nullptr, ev_done = nullptr, ev_pre = nullptr, ev_ready[R128_SLICES] = {nullptr};
-    HostStage stage; bool last_host = false; int concurrent = 1, slices = R128_SLICES;
+    int concurrent = 1, slices = R128_SLICES;
 };
 
 static int env_int (const char* name, int dflt) { const char* v = getenv (name); return v ? atoi (v) : dflt; }
@@ -142,7 +142,10 @@ static int r128_run (b200m_r128* h, const float* d_in, size_t stride, uint32_t n
     // A ragged block: one upload of the lengths, read by the K-weighting, fragment and true-peak kernels.  The true-peak FIR is
     // tpmax_kernel in both precision modes (tpk_process_sliced): no fused kernel.
     const uint32_t* d_len = nullptr;
-    if (len && !(d_len = ebu_upload_len (h->ebu, len, st))) return B200M_E_CUDA;
+    if (len) {
+        if (int rc = ebu_lens (h->ebu).put (len, h->n_inst, st)) return rc;
+        d_len = ebu_lens (h->ebu).d;
+    }
     const bool mixed = h->n_off && h->n_off < h->n_inst;
     if (mixed) {
         // the first mixed cycle after a change: device mask, then the frozen histories of the disabled instances.  Until now every
@@ -233,7 +236,7 @@ static int r128_create (b200m_r128** out, int device, uint32_t n_inst, uint32_t 
         if (e == cudaSuccess) e = cudaMalloc ((void**)&h->d_off, n_inst);
         if (e == cudaSuccess) e = cudaMalloc ((void**)&h->d_stash, (size_t)n_inst * nchan * 48 * sizeof (float));
         if (e == cudaSuccess && (nchan == 3 || nchan == 5 || gains)) e = cudaMalloc ((void**)&h->d_tplin, (size_t)n_inst * nchan * sizeof (float));
-        for (cudaStream_t* sp : {&h->own, &h->side, &h->copy}) if (e == cudaSuccess) e = cudaStreamCreateWithFlags (sp, cudaStreamNonBlocking);
+        for (cudaStream_t* sp : {&h->path.own, &h->side, &h->copy}) if (e == cudaSuccess) e = cudaStreamCreateWithFlags (sp, cudaStreamNonBlocking);
         for (cudaEvent_t* ep : {&h->ev_tp, &h->ev_done, &h->ev_pre}) if (e == cudaSuccess) e = cudaEventCreateWithFlags (ep, cudaEventDisableTiming);
         for (int s = 0; s < R128_SLICES; ++s) if (e == cudaSuccess) e = cudaEventCreateWithFlags (&h->ev_ready[s], cudaEventDisableTiming);
         if (e == cudaSuccess) {
@@ -273,8 +276,8 @@ int b200m_r128_destroy (b200m_r128* h)
     b200m_ebu_destroy (h->ebu); b200m_tpk_destroy (h->tpk);
     DeviceGuard g (h->device);
     cudaDeviceSynchronize ();
-    cudaFree (h->d_tpmax); cudaFree (h->d_off); cudaFree (h->d_stash); cudaFree (h->d_tplin); h->stage.release ();
-    for (cudaStream_t sp : {h->own, h->side, h->copy}) if (sp) cudaStreamDestroy (sp);
+    cudaFree (h->d_tpmax); cudaFree (h->d_off); cudaFree (h->d_stash); cudaFree (h->d_tplin); h->path.release ();
+    for (cudaStream_t sp : {h->side, h->copy}) if (sp) cudaStreamDestroy (sp);
     for (cudaEvent_t ep : {h->ev_tp, h->ev_done, h->ev_pre}) if (ep) cudaEventDestroy (ep);
     for (int s = 0; s < R128_SLICES; ++s) if (h->ev_ready[s]) cudaEventDestroy (h->ev_ready[s]);
     delete h;
@@ -284,7 +287,7 @@ int b200m_r128_destroy (b200m_r128* h)
 int b200m_r128_control (b200m_r128* h, int32_t inst, int cmd, void* stream)
 {
     if (!h) return set_err (B200M_E_INVAL, "NULL handle");
-    void* st = h->last_host ? (void*)h->own : stream;
+    void* st = h->path.stream (stream);
     switch (cmd) {
     case B200M_R128_START: return b200m_ebu_integr_start (h->ebu, inst, st);
     case B200M_R128_PAUSE: return b200m_ebu_integr_pause (h->ebu, inst, st);
@@ -315,77 +318,71 @@ int b200m_r128_control (b200m_r128* h, int32_t inst, int cmd, void* stream)
     }
 }
 
+}  // extern "C"
+
+// the sliced host path: the copy of each instance slice on the copy stream, each slice's kernels behind its copy
+static int r128_run_host (b200m_r128* h, const float* in, size_t stride, uint32_t nfram, const uint32_t* len)
+{
+    HostStage& sg = h->path.stage;
+    const size_t nch = (size_t)h->nchan * h->n_inst;
+    if (sg.ensure (nch, nfram)) return set_err (B200M_E_NOMEM, "staging buffer allocation failed");
+    // the staging buffer is single: the next copy may only start when the previous cycle's kernels have read it (after device-path
+    // calls a no-op: ev_done was recorded on own, which enter_device has waited for)
+    B200M_CUDA (cudaStreamWaitEvent (h->copy, h->ev_done, 0));
+    const int nsl = h->n_inst >= 64 ? h->slices : 1;
+    for (int s = 0; s < nsl; ++s) {
+        const size_t r0 = h->nchan * ((uint64_t)h->n_inst * s / nsl), r1 = h->nchan * ((uint64_t)h->n_inst * (s + 1) / nsl);
+        if (stride == nfram && sg.cap == nfram)                // both sides dense: one contiguous DMA per slice (faster than 4 KB rows)
+            B200M_CUDA (cudaMemcpyAsync (sg.d + r0 * sg.cap, in + r0 * stride, (r1 - r0) * (size_t)nfram * sizeof (float), cudaMemcpyHostToDevice, h->copy));
+        else
+            B200M_CUDA (cudaMemcpy2DAsync (sg.d + r0 * sg.cap, sg.cap * sizeof (float), in + r0 * stride, stride * sizeof (float),
+                                           (size_t)nfram * sizeof (float), r1 - r0, cudaMemcpyHostToDevice, h->copy));
+        B200M_CUDA (cudaEventRecord (h->ev_ready[s], h->copy));
+    }
+    // own ends every cycle: the EBU kernels wait for each slice's copy event (ebu_process_sliced), and own waits for the side
+    // stream's true-peak kernels (ev_tp) whenever they run there.  So a wait for own (enter_device, *_results) covers all
+    // three streams, with dBTP on, off or mixed.
+    if (int rc = r128_run (h, sg.d, sg.cap, nfram, h->path.own, nsl, h->ev_ready, len)) return rc;
+    B200M_CUDA (cudaEventRecord (h->ev_done, h->path.own));
+    return 0;
+}
+
+// every block entry point; the host path copies the block itself (r128_run_host)
+static int r128_block (b200m_r128* h, const float* in, size_t stride, uint32_t nfram, bool host, void* stream, const uint32_t* len)
+{
+    return bank_call (h, in, stride, nfram, host, stream, 0, h ? h->n_inst : 0, len, no_check,
+                      [&] (const float* d_in, size_t ds, cudaStream_t st, const uint32_t* rlen) {
+                          return host ? r128_run_host (h, in, stride, nfram, rlen) : r128_run (h, d_in, ds, nfram, st, 1, nullptr, rlen);
+                      });
+}
+
+extern "C" {
+
 int b200m_r128_run_device (b200m_r128* h, const float* d_in, size_t stride, uint32_t nfram, void* stream)
 {
-    if (int rc = check_block_args (h, d_in, stride, nfram)) return rc;
-    DeviceGuard g (h->device);
-    B200M_LEAVE_HOST_PATH (h);      // own covers the host path's copy and side streams: see r128_run_host
-    return r128_run (h, d_in, stride, nfram, (cudaStream_t)stream, 1, nullptr);
+    return r128_block (h, d_in, stride, nfram, false, stream, nullptr);
 }
 
 int b200m_r128_run_ragged_device (b200m_r128* h, const float* d_in, size_t stride, uint32_t nfram, const uint32_t* len, void* stream)
 {
-    if (int rc = check_block_args (h, d_in, stride, nfram)) return rc;
-    const int rag = ebu_ragged_check (h->ebu, nfram, len);
-    if (rag < 0) return rag;
-    if (!rag) return b200m_r128_run_device (h, d_in, stride, nfram, stream);        // every length is nfram: the plain call
-    DeviceGuard g (h->device);
-    B200M_LEAVE_HOST_PATH (h);
-    return r128_run (h, d_in, stride, nfram, (cudaStream_t)stream, 1, nullptr, len);
+    return r128_block (h, d_in, stride, nfram, false, stream, len);
 }
-
-static int r128_run_host (b200m_r128* h, const float* in, size_t stride, uint32_t nfram, const uint32_t* len);
 
 int b200m_r128_run_host (b200m_r128* h, const float* in, size_t stride, uint32_t nfram)
 {
-    return r128_run_host (h, in, stride, nfram, nullptr);
+    return r128_block (h, in, stride, nfram, true, nullptr, nullptr);
 }
 
 int b200m_r128_run_ragged_host (b200m_r128* h, const float* in, size_t stride, uint32_t nfram, const uint32_t* len)
 {
-    if (int rc = check_block_args (h, in, stride, nfram)) return rc;
-    const int rag = ebu_ragged_check (h->ebu, nfram, len);
-    if (rag < 0) return rag;
-    return r128_run_host (h, in, stride, nfram, rag ? len : nullptr);
+    return r128_block (h, in, stride, nfram, true, nullptr, len);
 }
-
-}  // extern "C"
-
-static int r128_run_host (b200m_r128* h, const float* in, size_t stride, uint32_t nfram, const uint32_t* len)
-{
-    if (int rc = check_block_args (h, in, stride, nfram)) return rc;
-    DeviceGuard g (h->device);
-    B200M_ENTER_HOST_PATH (h);
-    const size_t nch = (size_t)h->nchan * h->n_inst;
-    if (h->stage.ensure (nch, nfram)) return set_err (B200M_E_NOMEM, "staging buffer allocation failed");
-    // the staging buffer is single: the next copy may only start when the previous cycle's kernels have read it
-    if (h->last_host) B200M_CUDA (cudaStreamWaitEvent (h->copy, h->ev_done, 0));
-    const int nsl = h->n_inst >= 64 ? h->slices : 1;
-    for (int s = 0; s < nsl; ++s) {
-        const size_t r0 = h->nchan * ((uint64_t)h->n_inst * s / nsl), r1 = h->nchan * ((uint64_t)h->n_inst * (s + 1) / nsl);
-        if (stride == nfram && h->stage.cap == nfram)          // both sides dense: one contiguous DMA per slice (faster than 4 KB rows)
-            B200M_CUDA (cudaMemcpyAsync (h->stage.d + r0 * h->stage.cap, in + r0 * stride, (r1 - r0) * (size_t)nfram * sizeof (float), cudaMemcpyHostToDevice, h->copy));
-        else
-            B200M_CUDA (cudaMemcpy2DAsync (h->stage.d + r0 * h->stage.cap, h->stage.cap * sizeof (float), in + r0 * stride, stride * sizeof (float),
-                                           (size_t)nfram * sizeof (float), r1 - r0, cudaMemcpyHostToDevice, h->copy));
-        B200M_CUDA (cudaEventRecord (h->ev_ready[s], h->copy));
-    }
-    h->last_host = true;
-    // own ends every cycle: the EBU kernels wait for each slice's copy event (ebu_process_sliced), and own waits for the side
-    // stream's true-peak kernels (ev_tp) whenever they run there.  So a wait for own (B200M_LEAVE_HOST_PATH, *_results) covers all
-    // three streams, with dBTP on, off or mixed.
-    if (int rc = r128_run (h, h->stage.d, h->stage.cap, nfram, h->own, nsl, h->ev_ready, len)) return rc;
-    B200M_CUDA (cudaEventRecord (h->ev_done, h->own));
-    return 0;
-}
-
-extern "C" {
 
 int b200m_r128_results (b200m_r128* h, b200m_ebu_result* ebu_out, float* tp_max_db, void* stream)
 {
     if (!h) return set_err (B200M_E_INVAL, "NULL handle");
     DeviceGuard g (h->device);
-    cudaStream_t st = h->last_host ? h->own : (cudaStream_t)stream;
+    cudaStream_t st = h->path.stream (stream);
     if (tp_max_db) B200M_CUDA (cudaMemcpyAsync (tp_max_db, h->d_tpmax, h->n_inst * sizeof (float), cudaMemcpyDeviceToHost, st));
     if (ebu_out) return b200m_ebu_results (h->ebu, ebu_out, st);
     B200M_CUDA (cudaStreamSynchronize (st));
@@ -411,7 +408,7 @@ int b200m_r128_set_precision (b200m_r128* h, int mode)
 int b200m_r128_histogram (b200m_r128* h, uint32_t inst, int32_t* hist_M, int32_t* hist_S, void* stream)
 {
     if (!h) return set_err (B200M_E_INVAL, "NULL handle");
-    return b200m_ebu_histogram (h->ebu, inst, hist_M, hist_S, h->last_host ? (void*)h->own : stream);
+    return b200m_ebu_histogram (h->ebu, inst, hist_M, hist_S, h->path.stream (stream));
 }
 
 // snapshot = [u64 ebu bytes][u64 tpk bytes][ebu blob][tpk blob][tp_max floats][16 bytes of flags][per-instance dBTP off bytes].
@@ -428,7 +425,7 @@ int b200m_r128_snapshot (b200m_r128* h, void* buf, size_t bytes, void* stream)
 {
     if (!h || !buf || bytes < b200m_r128_snapshot_size (h)) return set_err (B200M_E_INVAL, "bad argument / buffer too small");
     DeviceGuard g (h->device);
-    void* st = h->last_host ? (void*)h->own : stream;
+    void* st = h->path.stream (stream);
     const uint64_t eb = b200m_ebu_snapshot_size (h->ebu), tb = b200m_tpk_snapshot_size (h->tpk);
     uint8_t* o = (uint8_t*)buf;
     memcpy (o, &eb, 8); memcpy (o + 8, &tb, 8); o += 16;
@@ -449,7 +446,7 @@ int b200m_r128_restore (b200m_r128* h, const void* buf, size_t bytes, void* stre
 {
     if (!h || !buf || bytes < b200m_r128_snapshot_size (h)) return set_err (B200M_E_INVAL, "bad argument / buffer too small");
     DeviceGuard g (h->device);
-    void* st = h->last_host ? (void*)h->own : stream;
+    void* st = h->path.stream (stream);
     uint64_t eb, tb;
     const uint8_t* o = (const uint8_t*)buf;
     memcpy (&eb, o, 8); memcpy (&tb, o + 8, 8); o += 16;

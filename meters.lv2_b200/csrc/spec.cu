@@ -178,7 +178,7 @@ struct b200m_spec {
     SpecCtl* d_ctl = nullptr; uint32_t ctl_lo = 0, ctl_hi = 0;
     double W[30][6][6];                                   // a0 a1 a2 b0 b1 b2 per stage, as the reference stores them
     double *d_coef = nullptr, *d_z = nullptr; float *d_val = nullptr, *d_ports = nullptr;
-    cudaStream_t own = nullptr; HostStage stage; bool last_host = false;
+    BankPath path;
     int fma = 0;                                          // B200M_PREC_FMA
     RaggedLen rag;                                        // ragged blocks: lengths per instance
 };
@@ -255,8 +255,6 @@ static float spec_omega (float speed, double rate)
     return 1.0f - expf (-2.0 * M_PI * speed / rate);
 }
 
-static cudaStream_t spec_stream (b200m_spec* h, void* stream) { return h->last_host ? h->own : (cudaStream_t)stream; }
-
 // control-port handling at the top of spectrum_run (:170-205) for one instance: updates its state, returns its run parameters
 static SpecCtl spec_control (b200m_spec* h, uint32_t i, float speed, float reset)
 {
@@ -303,13 +301,7 @@ static int spec_process (b200m_spec* h, const float* d_in, size_t stride, uint32
         const SpecCtl c = spec_control (h, i, ctl[i * cstride], ctl[i * cstride + 1]);
         if (memcmp (&c, &h->ctl[i], sizeof (c))) { h->ctl[i] = c; spec_mark (h, i, i + 1); }
     }
-    if (len) {
-        cudaError_t e = cudaSuccess;
-        uint32_t* hl = h->rag.stage (h->n_inst, &e);
-        if (!hl) return cuda_fail (e, "spec_process", __FILE__, __LINE__);
-        memcpy (hl, len, h->n_inst * sizeof (uint32_t));
-        B200M_CUDA (h->rag.upload (h->n_inst, st));
-    }
+    if (len) if (int rc = h->rag.put (len, h->n_inst, st)) return rc;
     if (h->ctl_lo < h->ctl_hi) {
         B200M_CUDA (cudaMemcpyAsync (h->d_ctl + h->ctl_lo, h->ctl.data () + h->ctl_lo, (h->ctl_hi - h->ctl_lo) * sizeof (SpecCtl), cudaMemcpyHostToDevice, st));
         h->ctl_lo = h->ctl_hi = 0;
@@ -373,7 +365,7 @@ int b200m_spec_create (b200m_spec** out, int device, uint32_t n_inst, uint32_t n
     A ((void**)&h->d_ctl, (size_t)n_inst * sizeof (SpecCtl));
     if (e == cudaSuccess) e = cudaMemcpy (h->d_coef, coef, sizeof (coef), cudaMemcpyHostToDevice);
     if (e == cudaSuccess) e = cudaMemcpy (h->d_ctl, h->ctl.data (), (size_t)n_inst * sizeof (SpecCtl), cudaMemcpyHostToDevice);
-    if (e == cudaSuccess) e = cudaStreamCreateWithFlags (&h->own, cudaStreamNonBlocking);
+    if (e == cudaSuccess) e = cudaStreamCreateWithFlags (&h->path.own, cudaStreamNonBlocking);
     if (e != cudaSuccess) { int rc = cuda_fail (e, "spec_create", __FILE__, __LINE__); b200m_spec_destroy (h); return rc; }
     *out = h;
     return 0;
@@ -384,84 +376,60 @@ int b200m_spec_destroy (b200m_spec* h)
     if (!h) return 0;
     DeviceGuard g (h->device);
     cudaDeviceSynchronize ();
-    cudaFree (h->d_coef); cudaFree (h->d_z); cudaFree (h->d_val); cudaFree (h->d_ports); cudaFree (h->d_ctl); h->stage.release (); h->rag.release ();
-    if (h->own) cudaStreamDestroy (h->own);
+    cudaFree (h->d_coef); cudaFree (h->d_z); cudaFree (h->d_val); cudaFree (h->d_ports); cudaFree (h->d_ctl); h->rag.release (); h->path.release ();
     delete h;
     return 0;
 }
 
+// every block entry point; ctl: the control pairs (NULL: refused), cstride as in spec_process
+static int spec_block (b200m_spec* h, const float* in, size_t stride, uint32_t nfram, const float* ctl, size_t cstride, bool host, void* stream,
+                       const uint32_t* len)
+{
+    return bank_call (h, in, stride, nfram, host, stream, h ? (size_t)h->n_inst * h->nchan : 0, h ? h->n_inst : 0, len,
+                      [&] { return ctl ? 0 : set_err (B200M_E_INVAL, "NULL ctl"); },
+                      [&] (const float* d_in, size_t ds, cudaStream_t st, const uint32_t* rlen) {
+                          return spec_process (h, d_in, ds, nfram, ctl, cstride, st, rlen);
+                      });
+}
+
 int b200m_spec_process_ctl_device (b200m_spec* h, const float* d_in, size_t stride, uint32_t nfram, const float* ctl, void* stream)
 {
-    if (int rc = check_block_args (h, d_in, stride, nfram)) return rc;
-    if (!ctl) return set_err (B200M_E_INVAL, "NULL ctl");
-    DeviceGuard g (h->device);
-    B200M_LEAVE_HOST_PATH (h);
-    return spec_process (h, d_in, stride, nfram, ctl, 2, (cudaStream_t)stream);
+    return spec_block (h, d_in, stride, nfram, ctl, 2, false, stream, nullptr);
 }
 
 int b200m_spec_process_device (b200m_spec* h, const float* d_in, size_t stride, uint32_t nfram, float speed, float reset, void* stream)
 {
-    if (int rc = check_block_args (h, d_in, stride, nfram)) return rc;
-    DeviceGuard g (h->device);
-    B200M_LEAVE_HOST_PATH (h);
     const float c[2] = {speed, reset};
-    return spec_process (h, d_in, stride, nfram, c, 0, (cudaStream_t)stream);
-}
-
-static int spec_process_host (b200m_spec* h, const float* in, size_t stride, uint32_t nfram, const float* ctl, size_t cstride,
-                              const uint32_t* len = nullptr)
-{
-    if (int rc = check_block_args (h, in, stride, nfram)) return rc;
-    DeviceGuard g (h->device);
-    B200M_ENTER_HOST_PATH (h);
-    const size_t nch = (size_t)h->n_inst * h->nchan;
-    if (h->stage.ensure (nch, nfram)) return set_err (B200M_E_NOMEM, "staging buffer allocation failed");
-    B200M_CUDA (cudaMemcpy2DAsync (h->stage.d, h->stage.cap * sizeof (float), in, stride * sizeof (float),
-                                   (size_t)nfram * sizeof (float), nch, cudaMemcpyHostToDevice, h->own));
-    h->last_host = true;
-    return spec_process (h, h->stage.d, h->stage.cap, nfram, ctl, cstride, h->own, len);
+    return spec_block (h, d_in, stride, nfram, c, 0, false, stream, nullptr);
 }
 
 int b200m_spec_process_ctl_host (b200m_spec* h, const float* in, size_t stride, uint32_t nfram, const float* ctl)
 {
-    if (!ctl) return set_err (B200M_E_INVAL, "NULL ctl");
-    return spec_process_host (h, in, stride, nfram, ctl, 2);
+    return spec_block (h, in, stride, nfram, ctl, 2, true, nullptr, nullptr);
 }
 
 int b200m_spec_process_host (b200m_spec* h, const float* in, size_t stride, uint32_t nfram, float speed, float reset)
 {
     const float c[2] = {speed, reset};
-    return spec_process_host (h, in, stride, nfram, c, 0);
+    return spec_block (h, in, stride, nfram, c, 0, true, nullptr, nullptr);
 }
 
 int b200m_spec_process_ragged_device (b200m_spec* h, const float* d_in, size_t stride, uint32_t nfram, const float* ctl, const uint32_t* len,
                                       void* stream)
 {
-    if (int rc = check_block_args (h, d_in, stride, nfram)) return rc;
-    if (!ctl) return set_err (B200M_E_INVAL, "NULL ctl");
-    const int rag = ragged_check (h->n_inst, nfram, len);
-    if (rag < 0) return rag;
-    if (!rag) return b200m_spec_process_ctl_device (h, d_in, stride, nfram, ctl, stream);     // every length is nfram: the plain call
-    DeviceGuard g (h->device);
-    B200M_LEAVE_HOST_PATH (h);
-    return spec_process (h, d_in, stride, nfram, ctl, 2, (cudaStream_t)stream, len);
+    return spec_block (h, d_in, stride, nfram, ctl, 2, false, stream, len);
 }
 
 int b200m_spec_process_ragged_host (b200m_spec* h, const float* in, size_t stride, uint32_t nfram, const float* ctl, const uint32_t* len)
 {
-    if (int rc = check_block_args (h, in, stride, nfram)) return rc;
-    if (!ctl) return set_err (B200M_E_INVAL, "NULL ctl");
-    const int rag = ragged_check (h->n_inst, nfram, len);
-    if (rag < 0) return rag;
-    if (!rag) return b200m_spec_process_ctl_host (h, in, stride, nfram, ctl);
-    return spec_process_host (h, in, stride, nfram, ctl, 2, len);
+    return spec_block (h, in, stride, nfram, ctl, 2, true, nullptr, len);
 }
 
 int b200m_spec_clear (b200m_spec* h, int32_t inst, void* stream)
 {
     if (!h || inst < -1 || inst >= (int32_t)h->n_inst) return set_err (B200M_E_INVAL, "bad argument");
     DeviceGuard g (h->device);
-    cudaStream_t st = spec_stream (h, stream);
+    cudaStream_t st = h->path.stream (stream);
     const uint32_t i0 = inst < 0 ? 0 : (uint32_t)inst, n = inst < 0 ? h->n_inst : 1;
     // filter states, val / max and the ports as b200m_spec_create zeroes them
     B200M_CUDA (cudaMemsetAsync (h->d_z + (size_t)i0 * 12 * 32, 0, (size_t)n * 12 * 32 * sizeof (double), st));
@@ -483,7 +451,7 @@ int b200m_spec_results (b200m_spec* h, float* out60, void* stream)
 {
     if (!h || !out60) return set_err (B200M_E_INVAL, "NULL argument");
     DeviceGuard g (h->device);
-    cudaStream_t st = spec_stream (h, stream);
+    cudaStream_t st = h->path.stream (stream);
     B200M_CUDA (cudaMemcpyAsync (out60, h->d_ports, (size_t)h->n_inst * 60 * sizeof (float), cudaMemcpyDeviceToHost, st));
     B200M_CUDA (cudaStreamSynchronize (st));
     return 0;
@@ -493,7 +461,7 @@ int b200m_spec_state (b200m_spec* h, uint32_t inst, double* z360, float* val30, 
 {
     if (!h || !z360 || !val30 || !max30 || inst >= h->n_inst) return set_err (B200M_E_INVAL, "bad argument");
     DeviceGuard g (h->device);
-    cudaStream_t st = spec_stream (h, stream);
+    cudaStream_t st = h->path.stream (stream);
     double zt[12 * 32]; float vt[64];
     B200M_CUDA (cudaMemcpyAsync (zt, h->d_z + (size_t)inst * 12 * 32, sizeof (zt), cudaMemcpyDeviceToHost, st));
     B200M_CUDA (cudaMemcpyAsync (vt, h->d_val + (size_t)inst * 64, sizeof (vt), cudaMemcpyDeviceToHost, st));

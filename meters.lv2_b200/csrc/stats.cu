@@ -266,12 +266,12 @@ struct b200m_bim {
     // the statistics as they stood when an instance's last ~5 fps window closed, i.e. what bim_run publishes before bim_clear (:267-326)
     int32_t *d_pub_hist = nullptr, *d_pub_cnt = nullptr; float* d_pub_mm = nullptr; int64_t* d_pub_itime = nullptr;
     int resync = 0; bool window_closed = false;                // the window clock of a bank driven only bank-wide (b200m_bim_window_closed)
-    cudaStream_t own = nullptr; HostStage stage; bool last_host = false;
+    BankPath path;
 };
 struct b200m_sdh {
     int device; uint32_t n_inst; double rate;
     int32_t *d_hist = nullptr, *d_ip = nullptr, *d_integ = nullptr; double* d_dp = nullptr; int64_t* d_itime = nullptr;
-    cudaStream_t own = nullptr; HostStage stage; bool last_host = false;
+    BankPath path;
 };
 
 static int bim_control (b200m_bim* h, int32_t inst, int cmd, cudaStream_t st)
@@ -344,7 +344,7 @@ int b200m_bim_create (b200m_bim** out, int device, uint32_t n_inst, double rate)
     A ((void**)&h->d_st, (size_t)n_inst * 4 * 4); A ((void**)&h->d_itime, (size_t)n_inst * 8);
     A ((void**)&h->d_pub_hist, (size_t)n_inst * BIM_LEN * 4); A ((void**)&h->d_pub_cnt, (size_t)n_inst * 8 * 4); A ((void**)&h->d_pub_mm, (size_t)n_inst * 2 * 4);
     A ((void**)&h->d_pub_itime, (size_t)n_inst * 8);
-    if (e == cudaSuccess) e = cudaStreamCreateWithFlags (&h->own, cudaStreamNonBlocking);
+    if (e == cudaSuccess) e = cudaStreamCreateWithFlags (&h->path.own, cudaStreamNonBlocking);
     if (e == cudaSuccess) { bim_control (h, -1, B200M_CTL_CLEAR, nullptr); e = cudaDeviceSynchronize (); }      // bim_instantiate (:146-158)
     if (e != cudaSuccess) { int rc = cuda_fail (e, "bim_create", __FILE__, __LINE__); b200m_bim_destroy (h); return rc; }
     *out = h;
@@ -356,8 +356,7 @@ int b200m_bim_destroy (b200m_bim* h)
     DeviceGuard g (h->device);
     cudaDeviceSynchronize ();
     cudaFree (h->d_hist); cudaFree (h->d_cnt); cudaFree (h->d_mm); cudaFree (h->d_st); cudaFree (h->d_itime);
-    cudaFree (h->d_pub_hist); cudaFree (h->d_pub_cnt); cudaFree (h->d_pub_mm); cudaFree (h->d_pub_itime); h->stage.release ();
-    if (h->own) cudaStreamDestroy (h->own);
+    cudaFree (h->d_pub_hist); cudaFree (h->d_pub_cnt); cudaFree (h->d_pub_mm); cudaFree (h->d_pub_itime); h->path.release ();
     delete h;
     return 0;
 }
@@ -366,25 +365,15 @@ int b200m_bim_control_inst (b200m_bim* h, int32_t inst, int cmd, void* stream)
 {
     if (!h) return set_err (B200M_E_INVAL, "NULL handle");
     DeviceGuard g (h->device);
-    return bim_control (h, inst, cmd, h->last_host ? h->own : (cudaStream_t)stream);   // CTL_* handling of bim_run (:207-231)
+    return bim_control (h, inst, cmd, h->path.stream (stream));   // CTL_* handling of bim_run (:207-231)
 }
-int b200m_bim_run_device (b200m_bim* h, const float* d_in, size_t stride, uint32_t nfram, void* stream)
+static int bim_block (b200m_bim* h, const float* in, size_t stride, uint32_t nfram, bool host, void* stream)
 {
-    if (int rc = check_block_args (h, d_in, stride, nfram)) return rc;
-    DeviceGuard g (h->device);
-    B200M_LEAVE_HOST_PATH (h);
-    return bim_run (h, d_in, stride, nfram, (cudaStream_t)stream);
+    return bank_call (h, in, stride, nfram, host, stream, h ? h->n_inst : 0, 0, nullptr, no_check,
+                      [&] (const float* d_in, size_t ds, cudaStream_t st, const uint32_t*) { return bim_run (h, d_in, ds, nfram, st); });
 }
-int b200m_bim_run_host (b200m_bim* h, const float* in, size_t stride, uint32_t nfram)
-{
-    if (int rc = check_block_args (h, in, stride, nfram)) return rc;
-    DeviceGuard g (h->device);
-    B200M_ENTER_HOST_PATH (h);
-    if (h->stage.ensure (h->n_inst, nfram)) return set_err (B200M_E_NOMEM, "staging buffer allocation failed");
-    B200M_CUDA (cudaMemcpy2DAsync (h->stage.d, h->stage.cap * sizeof (float), in, stride * sizeof (float), (size_t)nfram * sizeof (float), h->n_inst, cudaMemcpyHostToDevice, h->own));
-    h->last_host = true;
-    return bim_run (h, h->stage.d, h->stage.cap, nfram, h->own);
-}
+int b200m_bim_run_device (b200m_bim* h, const float* d_in, size_t stride, uint32_t nfram, void* stream) { return bim_block (h, d_in, stride, nfram, false, stream); }
+int b200m_bim_run_host (b200m_bim* h, const float* in, size_t stride, uint32_t nfram) { return bim_block (h, in, stride, nfram, true, nullptr); }
 // one row of statistics (hist, counters, min/max, integration time), live or published, of instances [i0, i0 + n)
 static int bim_copy_rows (b200m_bim* h, bool pub, uint32_t i0, uint32_t n, int32_t* hist, int32_t* cnt5, float* mm2, int64_t* itime, cudaStream_t st)
 {
@@ -400,7 +389,7 @@ int b200m_bim_results (b200m_bim* h, uint32_t inst, int32_t* hist584, int32_t* c
 {
     if (!h || inst >= h->n_inst) return set_err (B200M_E_INVAL, "bad argument");
     DeviceGuard g (h->device);
-    cudaStream_t st = h->last_host ? h->own : (cudaStream_t)stream;
+    cudaStream_t st = h->path.stream (stream);
     if (int rc = bim_copy_rows (h, false, inst, 1, hist584, cnt5, minmax2, integration_time, st)) return rc;
     B200M_CUDA (cudaStreamSynchronize (st));
     return 0;
@@ -410,7 +399,7 @@ int b200m_bim_published (b200m_bim* h, uint32_t inst, int32_t* hist584, int32_t*
 {
     if (!h || inst >= h->n_inst) return set_err (B200M_E_INVAL, "bad argument");
     DeviceGuard g (h->device);
-    cudaStream_t st = h->last_host ? h->own : (cudaStream_t)stream;
+    cudaStream_t st = h->path.stream (stream);
     if (int rc = bim_copy_rows (h, true, inst, 1, hist584, cnt5, minmax2, integration_time, st)) return rc;
     B200M_CUDA (cudaStreamSynchronize (st));
     return 0;
@@ -420,7 +409,7 @@ int b200m_bim_results_all (b200m_bim* h, int32_t* hist, int32_t* cnt5, float* mi
 {
     if (!h) return set_err (B200M_E_INVAL, "NULL handle");
     DeviceGuard g (h->device);
-    cudaStream_t st = h->last_host ? h->own : (cudaStream_t)stream;
+    cudaStream_t st = h->path.stream (stream);
     if (int rc = bim_copy_rows (h, false, 0, h->n_inst, hist, cnt5, minmax2, integration_time, st)) return rc;
     if (int rc = bim_copy_rows (h, true, 0, h->n_inst, pub_hist, pub_cnt5, pub_minmax2, pub_integration_time, st)) return rc;
     if (closed) B200M_CUDA (cudaMemcpy2DAsync (closed, 4, h->d_st + 3, 4 * 4, 4, h->n_inst, cudaMemcpyDeviceToHost, st));
@@ -444,7 +433,7 @@ int b200m_sdh_create (b200m_sdh** out, int device, uint32_t n_inst, double rate)
     auto A = [&] (void** p, size_t bytes) { if (e == cudaSuccess) { e = cudaMalloc (p, bytes); if (e == cudaSuccess) e = cudaMemset (*p, 0, bytes); } };
     A ((void**)&h->d_hist, (size_t)n_inst * SDH_BINS * 4); A ((void**)&h->d_ip, (size_t)n_inst * 2 * 4); A ((void**)&h->d_dp, (size_t)n_inst * 3 * 8);
     A ((void**)&h->d_integ, (size_t)n_inst * 4); A ((void**)&h->d_itime, (size_t)n_inst * 8);
-    if (e == cudaSuccess) e = cudaStreamCreateWithFlags (&h->own, cudaStreamNonBlocking);
+    if (e == cudaSuccess) e = cudaStreamCreateWithFlags (&h->path.own, cudaStreamNonBlocking);
     if (e == cudaSuccess) e = cudaFuncSetAttribute (sdh_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, SDH_SMEM);
     if (e == cudaSuccess) { sdh_control (h, -1, B200M_CTL_CLEAR, nullptr); e = cudaDeviceSynchronize (); }        // sdh_instantiate (:141-150)
     if (e != cudaSuccess) { int rc = cuda_fail (e, "sdh_create", __FILE__, __LINE__); b200m_sdh_destroy (h); return rc; }
@@ -456,8 +445,7 @@ int b200m_sdh_destroy (b200m_sdh* h)
     if (!h) return 0;
     DeviceGuard g (h->device);
     cudaDeviceSynchronize ();
-    cudaFree (h->d_hist); cudaFree (h->d_ip); cudaFree (h->d_dp); cudaFree (h->d_integ); cudaFree (h->d_itime); h->stage.release ();
-    if (h->own) cudaStreamDestroy (h->own);
+    cudaFree (h->d_hist); cudaFree (h->d_ip); cudaFree (h->d_dp); cudaFree (h->d_integ); cudaFree (h->d_itime); h->path.release ();
     delete h;
     return 0;
 }
@@ -466,25 +454,15 @@ int b200m_sdh_control_inst (b200m_sdh* h, int32_t inst, int cmd, void* stream)
 {
     if (!h) return set_err (B200M_E_INVAL, "NULL handle");
     DeviceGuard g (h->device);
-    return sdh_control (h, inst, cmd, h->last_host ? h->own : (cudaStream_t)stream);   // sdh_integrate / sdh_reset (:233-241)
+    return sdh_control (h, inst, cmd, h->path.stream (stream));   // sdh_integrate / sdh_reset (:233-241)
 }
-int b200m_sdh_run_device (b200m_sdh* h, const float* d_in, size_t stride, uint32_t nfram, void* stream)
+static int sdh_block (b200m_sdh* h, const float* in, size_t stride, uint32_t nfram, bool host, void* stream)
 {
-    if (int rc = check_block_args (h, d_in, stride, nfram)) return rc;
-    DeviceGuard g (h->device);
-    B200M_LEAVE_HOST_PATH (h);
-    return sdh_run (h, d_in, stride, nfram, (cudaStream_t)stream);
+    return bank_call (h, in, stride, nfram, host, stream, h ? h->n_inst : 0, 0, nullptr, no_check,
+                      [&] (const float* d_in, size_t ds, cudaStream_t st, const uint32_t*) { return sdh_run (h, d_in, ds, nfram, st); });
 }
-int b200m_sdh_run_host (b200m_sdh* h, const float* in, size_t stride, uint32_t nfram)
-{
-    if (int rc = check_block_args (h, in, stride, nfram)) return rc;
-    DeviceGuard g (h->device);
-    B200M_ENTER_HOST_PATH (h);
-    if (h->stage.ensure (h->n_inst, nfram)) return set_err (B200M_E_NOMEM, "staging buffer allocation failed");
-    B200M_CUDA (cudaMemcpy2DAsync (h->stage.d, h->stage.cap * sizeof (float), in, stride * sizeof (float), (size_t)nfram * sizeof (float), h->n_inst, cudaMemcpyHostToDevice, h->own));
-    h->last_host = true;
-    return sdh_run (h, h->stage.d, h->stage.cap, nfram, h->own);
-}
+int b200m_sdh_run_device (b200m_sdh* h, const float* d_in, size_t stride, uint32_t nfram, void* stream) { return sdh_block (h, d_in, stride, nfram, false, stream); }
+int b200m_sdh_run_host (b200m_sdh* h, const float* in, size_t stride, uint32_t nfram) { return sdh_block (h, in, stride, nfram, true, nullptr); }
 static int sdh_copy_rows (b200m_sdh* h, uint32_t i0, uint32_t n, int32_t* hist, int32_t* mp2, double* atv3, int64_t* itime, cudaStream_t st)
 {
     if (hist) B200M_CUDA (cudaMemcpyAsync (hist, h->d_hist + (size_t)i0 * SDH_BINS, (size_t)n * SDH_BINS * 4, cudaMemcpyDeviceToHost, st));
@@ -497,7 +475,7 @@ int b200m_sdh_results (b200m_sdh* h, uint32_t inst, int32_t* hist361, int32_t* m
 {
     if (!h || inst >= h->n_inst) return set_err (B200M_E_INVAL, "bad argument");
     DeviceGuard g (h->device);
-    cudaStream_t st = h->last_host ? h->own : (cudaStream_t)stream;
+    cudaStream_t st = h->path.stream (stream);
     if (int rc = sdh_copy_rows (h, inst, 1, hist361, max_peak2, avg_tmp_var3, integration_time, st)) return rc;
     B200M_CUDA (cudaStreamSynchronize (st));
     return 0;
@@ -506,7 +484,7 @@ int b200m_sdh_results_all (b200m_sdh* h, int32_t* hist, int32_t* max_peak2, doub
 {
     if (!h) return set_err (B200M_E_INVAL, "NULL handle");
     DeviceGuard g (h->device);
-    cudaStream_t st = h->last_host ? h->own : (cudaStream_t)stream;
+    cudaStream_t st = h->path.stream (stream);
     if (int rc = sdh_copy_rows (h, 0, h->n_inst, hist, max_peak2, avg_tmp_var3, integration_time, st)) return rc;
     B200M_CUDA (cudaStreamSynchronize (st));
     return 0;

@@ -2108,7 +2108,7 @@ struct b200m_tpk {
     // met so far (host libm, tpk_km_fall), shared by this bank's own ragged calls and the DR-14 bank's
     RaggedLen rag; std::vector<float> fall; std::vector<uint8_t> fall_ok;
     bool rag_read = false;                  // the last process() block was a b200m_tpk_process_ragged_* one: read() skips its length-0 rows
-    cudaStream_t own = nullptr; HostStage stage; bool last_host = false;
+    BankPath path;
 };
 
 // zita-resampler table for (fr = 1.0, hl = 24, np = 4); restates Resampler_table's constructor
@@ -2161,8 +2161,6 @@ int tpk_reset_inst (b200m_tpk* h, const uint32_t* d_inst, uint32_t n_sel, uint32
     return 0;
 }
 }
-
-static cudaStream_t tpk_stream (b200m_tpk* h, void* stream) { return h->last_host ? h->own : (cudaStream_t)stream; }
 
 // the instantiations of the EBUr128 epilogue's HOLD (r128_group_hold)
 template <bool IMM, bool FMA, bool RAG = false> static decltype (&tpmax_kernel<IMM, FMA, 2, RAG>) tpmax_kernel_for (int hold)
@@ -2516,7 +2514,7 @@ int b200m_tpk_create (b200m_tpk** out, int device, uint32_t n_chan, float fsamp,
     if (e == cudaSuccess) e = cudaFuncSetAttribute (tpk_kernel<64, 32, true, false, true, false, true, false>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)TpkGeom<64, 32, true>::BYTES);
     if (e == cudaSuccess) e = cudaFuncSetAttribute (tpk_kernel<64, 32, true, false, true, false, false, false>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)TpkGeom<64, 32, true>::BYTES);
     if (e == cudaSuccess) e = cudaFuncSetAttribute (tpk_kernel<64, 32, true, false, false, false, false, false>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)TpkGeom<64, 32, true>::BYTES);
-    if (e == cudaSuccess) e = cudaStreamCreateWithFlags (&h->own, cudaStreamNonBlocking);
+    if (e == cudaSuccess) e = cudaStreamCreateWithFlags (&h->path.own, cudaStreamNonBlocking);
     if (e == cudaSuccess) {
         // constructors: TruePeakdsp _res(true) (:29); Kmeterdsp _flag(false), all zero (kmeterdsp.cc:30-40);
         // the 8192-zero pre-roll (:159-168) leaves an all-zero history, which the memset above provides
@@ -2540,69 +2538,44 @@ int b200m_tpk_destroy (b200m_tpk* h)
     if (h->sb) cudaStreamDestroy (h->sb);
     for (int i = 0; i < 2; ++i) { if (h->ev_fir[i]) cudaEventDestroy (h->ev_fir[i]); if (h->ev_bal[i]) cudaEventDestroy (h->ev_bal[i]); }
     h->rag.release ();
-    h->stage.release ();
-    if (h->own) cudaStreamDestroy (h->own);
+    h->path.release ();
     delete h;
     return 0;
 }
 
+// every block entry point; len: a ragged block, channel i runs process() over its first len[i] frames
+static int tpk_block (b200m_tpk* h, const float* in, size_t stride, uint32_t nfram, uint32_t tp_mode, bool host, void* stream, const uint32_t* len)
+{
+    const uint32_t n = h ? h->n_chan : 0;
+    return bank_call (h, in, stride, nfram, host, stream, n, n, len,
+                      [&] { return tp_mode > 1 ? set_err (B200M_E_INVAL, "bad tp_mode %u", tp_mode) : 0; },
+                      [&] (const float* d_in, size_t ds, cudaStream_t st, const uint32_t* rlen) {
+                          if (!rlen) { h->rag_read = false; return tpk_process (h, d_in, ds, nfram, tp_mode, st); }
+                          const uint32_t* d_len = nullptr; const float* d_fall = nullptr;
+                          if (int rc = tpk_upload_len (h, rlen, h->n_chan, st, &d_len, &d_fall)) return rc;
+                          h->rag_read = true;
+                          return tpk_process_ragged (h, d_in, ds, nfram, st, d_len, d_fall, 1);
+                      });
+}
+
 int b200m_tpk_process_device (b200m_tpk* h, const float* d_in, size_t stride, uint32_t nfram, uint32_t tp_mode, void* stream)
 {
-    if (int rc = check_block_args (h, d_in, stride, nfram)) return rc;
-    if (tp_mode > 1) return set_err (B200M_E_INVAL, "bad tp_mode %u", tp_mode);
-    DeviceGuard g (h->device);
-    B200M_LEAVE_HOST_PATH (h);
-    h->rag_read = false;
-    return tpk_process (h, d_in, stride, nfram, tp_mode, (cudaStream_t)stream);
+    return tpk_block (h, d_in, stride, nfram, tp_mode, false, stream, nullptr);
 }
 
 int b200m_tpk_process_host (b200m_tpk* h, const float* in, size_t stride, uint32_t nfram, uint32_t tp_mode)
 {
-    if (int rc = check_block_args (h, in, stride, nfram)) return rc;
-    if (tp_mode > 1) return set_err (B200M_E_INVAL, "bad tp_mode %u", tp_mode);
-    DeviceGuard g (h->device);
-    B200M_ENTER_HOST_PATH (h);
-    if (h->stage.ensure (h->n_chan, nfram)) return set_err (B200M_E_NOMEM, "staging buffer allocation failed");
-    B200M_CUDA (cudaMemcpy2DAsync (h->stage.d, h->stage.cap * sizeof (float), in, stride * sizeof (float),
-                                   (size_t)nfram * sizeof (float), h->n_chan, cudaMemcpyHostToDevice, h->own));
-    h->last_host = true;
-    h->rag_read = false;
-    return tpk_process (h, h->stage.d, h->stage.cap, nfram, tp_mode, h->own);
-}
-
-// len (host, every entry <= nfram, some != nfram: ragged_check): channel i runs process() over its first len[i] frames
-static int tpk_ragged (b200m_tpk* h, const float* d_in, size_t stride, uint32_t nfram, const uint32_t* len, cudaStream_t st)
-{
-    const uint32_t* d_len = nullptr; const float* d_fall = nullptr;
-    if (int rc = tpk_upload_len (h, len, h->n_chan, st, &d_len, &d_fall)) return rc;
-    h->rag_read = true;
-    return tpk_process_ragged (h, d_in, stride, nfram, st, d_len, d_fall, 1);
+    return tpk_block (h, in, stride, nfram, tp_mode, true, nullptr, nullptr);
 }
 
 int b200m_tpk_process_ragged_device (b200m_tpk* h, const float* d_in, size_t stride, uint32_t nfram, const uint32_t* len, void* stream)
 {
-    if (int rc = check_block_args (h, d_in, stride, nfram)) return rc;
-    const int rag = ragged_check (h->n_chan, nfram, len);
-    if (rag < 0) return rag;
-    if (!rag) return b200m_tpk_process_device (h, d_in, stride, nfram, B200M_TP_MODE_PROCESS, stream);   // every length is nfram
-    DeviceGuard g (h->device);
-    B200M_LEAVE_HOST_PATH (h);
-    return tpk_ragged (h, d_in, stride, nfram, len, (cudaStream_t)stream);
+    return tpk_block (h, d_in, stride, nfram, B200M_TP_MODE_PROCESS, false, stream, len);
 }
 
 int b200m_tpk_process_ragged_host (b200m_tpk* h, const float* in, size_t stride, uint32_t nfram, const uint32_t* len)
 {
-    if (int rc = check_block_args (h, in, stride, nfram)) return rc;
-    const int rag = ragged_check (h->n_chan, nfram, len);
-    if (rag < 0) return rag;
-    if (!rag) return b200m_tpk_process_host (h, in, stride, nfram, B200M_TP_MODE_PROCESS);
-    DeviceGuard g (h->device);
-    B200M_ENTER_HOST_PATH (h);
-    if (h->stage.ensure (h->n_chan, nfram)) return set_err (B200M_E_NOMEM, "staging buffer allocation failed");
-    B200M_CUDA (cudaMemcpy2DAsync (h->stage.d, h->stage.cap * sizeof (float), in, stride * sizeof (float),
-                                   (size_t)nfram * sizeof (float), h->n_chan, cudaMemcpyHostToDevice, h->own));
-    h->last_host = true;
-    return tpk_ragged (h, h->stage.d, h->stage.cap, nfram, len, h->own);
+    return tpk_block (h, in, stride, nfram, B200M_TP_MODE_PROCESS, true, nullptr, len);
 }
 
 int b200m_tpk_set_precision (b200m_tpk* h, int mode)
@@ -2618,8 +2591,8 @@ int b200m_tpk_read_device (b200m_tpk* h, void* stream)
 {
     if (!h) return set_err (B200M_E_INVAL, "NULL handle");
     DeviceGuard g (h->device);
-    if (h->rag_read) return tpk_read_ragged (h, tpk_stream (h, stream), h->rag.d, 1);     // rows with length 0 were not called
-    tpk_read_kernel<<<(h->n_chan + 255) / 256, 256, 0, tpk_stream (h, stream)>>> ((int)h->n_chan, h->flags, h->st, h->d_res, nullptr, 1);
+    if (h->rag_read) return tpk_read_ragged (h, h->path.stream (stream), h->rag.d, 1);     // rows with length 0 were not called
+    tpk_read_kernel<<<(h->n_chan + 255) / 256, 256, 0, h->path.stream (stream)>>> ((int)h->n_chan, h->flags, h->st, h->d_res, nullptr, 1);
     B200M_LAUNCHED (1);
     B200M_CUDA (cudaGetLastError ());
     return 0;
@@ -2629,7 +2602,7 @@ int b200m_tpk_results (b200m_tpk* h, b200m_tpk_result* out, void* stream)
 {
     if (!h || !out) return set_err (B200M_E_INVAL, "NULL argument");
     DeviceGuard g (h->device);
-    cudaStream_t st = tpk_stream (h, stream);
+    cudaStream_t st = h->path.stream (stream);
     B200M_CUDA (cudaMemcpyAsync (out, h->d_res, h->n_chan * sizeof (b200m_tpk_result), cudaMemcpyDeviceToHost, st));
     B200M_CUDA (cudaStreamSynchronize (st));
     return 0;
@@ -2639,7 +2612,7 @@ int b200m_tpk_reset (b200m_tpk* h, int32_t chan, void* stream)
 {
     if (!h || chan >= (int32_t)h->n_chan) return set_err (B200M_E_INVAL, "bad argument");
     DeviceGuard g (h->device);
-    tpk_reset_kernel<<<(h->n_chan + 127) / 128, 128, 0, tpk_stream (h, stream)>>> ((int)h->n_chan, chan, h->flags, h->st, nullptr, 0, 1);
+    tpk_reset_kernel<<<(h->n_chan + 127) / 128, 128, 0, h->path.stream (stream)>>> ((int)h->n_chan, chan, h->flags, h->st, nullptr, 0, 1);
     B200M_LAUNCHED (1);
     B200M_CUDA (cudaGetLastError ());
     return 0;
@@ -2651,7 +2624,7 @@ int b200m_tpk_clear (b200m_tpk* h, int32_t chan, void* stream)
     // TruePeakdsp::init's pre-roll, truepeakdsp.cc:159-168).  For slot reuse in shared banks.
     if (!h || chan >= (int32_t)h->n_chan) return set_err (B200M_E_INVAL, "bad argument");
     DeviceGuard g (h->device);
-    tpk_reset_kernel<<<(h->n_chan + 127) / 128, 128, 0, tpk_stream (h, stream)>>> ((int)h->n_chan, chan, h->flags | 4u, h->st, nullptr, 0, 1);
+    tpk_reset_kernel<<<(h->n_chan + 127) / 128, 128, 0, h->path.stream (stream)>>> ((int)h->n_chan, chan, h->flags | 4u, h->st, nullptr, 0, 1);
     B200M_LAUNCHED (1);
     B200M_CUDA (cudaGetLastError ());
     return 0;
@@ -2662,7 +2635,7 @@ int b200m_tpk_reset_kmeter (b200m_tpk* h, void* stream)
     // reset_peaks of the TPnRMS/DR14 plugin resets only its K-meters (src/dr14.c:241-258)
     if (!h) return set_err (B200M_E_INVAL, "NULL handle");
     DeviceGuard g (h->device);
-    tpk_reset_kernel<<<(h->n_chan + 127) / 128, 128, 0, tpk_stream (h, stream)>>> ((int)h->n_chan, -1, h->flags & B200M_TPK_KMETER, h->st, nullptr, 0, 1);
+    tpk_reset_kernel<<<(h->n_chan + 127) / 128, 128, 0, h->path.stream (stream)>>> ((int)h->n_chan, -1, h->flags & B200M_TPK_KMETER, h->st, nullptr, 0, 1);
     B200M_LAUNCHED (1);
     B200M_CUDA (cudaGetLastError ());
     return 0;
@@ -2696,7 +2669,7 @@ int b200m_tpk_snapshot (b200m_tpk* h, void* buf, size_t bytes, void* stream)
 {
     if (!h || !buf || bytes < b200m_tpk_snapshot_size (h)) return set_err (B200M_E_INVAL, "bad argument / buffer too small");
     DeviceGuard g (h->device);
-    cudaStream_t st = tpk_stream (h, stream);
+    cudaStream_t st = h->path.stream (stream);
     const TpkSnapHead hd = {TPK_SNAP_MAGIC, h->n_chan, h->flags, h->fsamp};
     memcpy (buf, &hd, sizeof (hd));
     uint8_t* o = (uint8_t*)buf + 16;
@@ -2713,7 +2686,7 @@ int b200m_tpk_restore (b200m_tpk* h, const void* buf, size_t bytes, void* stream
     if (hd.magic != TPK_SNAP_MAGIC || hd.n_chan != h->n_chan || hd.flags != h->flags || hd.fsamp != h->fsamp)
         return set_err (B200M_E_INVAL, "snapshot does not match this bank (channels / meters / sample rate)");
     DeviceGuard g (h->device);
-    cudaStream_t st = tpk_stream (h, stream);
+    cudaStream_t st = h->path.stream (stream);
     const uint8_t* o = (const uint8_t*)buf + 16;
     void* p[15]; size_t b[15]; const int k = tpk_segments (h, p, b);
     for (int i = 0; i < k; ++i) { B200M_CUDA (cudaMemcpyAsync (p[i], o, b[i], cudaMemcpyHostToDevice, st)); o += (b[i] + 15) & ~size_t (15); }
@@ -2734,7 +2707,7 @@ int b200m_tpk_state (b200m_tpk* h, float* tp_m, float* tp_p, float* tp_z1, float
 {
     if (!h) return set_err (B200M_E_INVAL, "NULL handle");
     DeviceGuard g (h->device);
-    cudaStream_t st = tpk_stream (h, stream);
+    cudaStream_t st = h->path.stream (stream);
     const size_t n = h->n_chan, b = n * 4;
     if (tp_m)  B200M_CUDA (cudaMemcpyAsync (tp_m, h->st.tp_m, b, cudaMemcpyDeviceToHost, st));
     if (tp_p)  B200M_CUDA (cudaMemcpyAsync (tp_p, h->st.tp_p, b, cudaMemcpyDeviceToHost, st));
@@ -2783,7 +2756,7 @@ int b200m_tpk_debug_upsampled (b200m_tpk* h, uint32_t chan, float* out, uint32_t
     if (!h || !out || chan >= h->n_chan || n_out > 4 * B200M_MAX_BLOCK) return set_err (B200M_E_INVAL, "bad argument");
     if (!h->d_dbg) return set_err (B200M_E_INVAL, "debug capture not enabled");
     DeviceGuard g (h->device);
-    cudaStream_t st = tpk_stream (h, stream);
+    cudaStream_t st = h->path.stream (stream);
     B200M_CUDA (cudaMemcpyAsync (out, h->d_dbg + (size_t)chan * 4 * B200M_MAX_BLOCK, (size_t)n_out * 4, cudaMemcpyDeviceToHost, st));
     B200M_CUDA (cudaStreamSynchronize (st));
     return 0;
