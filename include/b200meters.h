@@ -443,7 +443,8 @@ int b200m_bim_results (b200m_bim* h, uint32_t inst, int32_t* hist584, int32_t* c
  * as they stood at that moment -- what bim_run publishes in its bim_stats message before the windowed-mode bim_clear
  * (:269-291,323-325) -- stay readable through b200m_bim_published until the next window closes.
  * b200m_bim_window_closed follows a bank-wide window clock: it is exact for a bank whose instances were only cleared together
- * (b200m_bim_control, or b200m_bim_control_inst with inst = -1).  The closed flag of each instance's own clock is returned by
+ * (b200m_bim_control, or b200m_bim_control_inst with inst = -1) and driven only with plain blocks.  A ragged block (below) does not
+ * advance that clock, and b200m_bim_window_closed reads 0 after one.  The closed flag of each instance's own clock is returned by
  * b200m_bim_results_all. */
 int b200m_bim_window_closed (const b200m_bim* h);
 int b200m_bim_published (b200m_bim* h, uint32_t inst, int32_t* hist584, int32_t* cnt5, float* minmax2, int64_t* integration_time, void* stream);
@@ -452,7 +453,7 @@ int b200m_bim_published (b200m_bim* h, uint32_t inst, int32_t* hist584, int32_t*
  *   cnt5 [n][5]         zero, pos, nan, inf, den
  *   minmax2 [n][2]      min, max of |sample| over normal numbers
  *   integration_time [n]
- *   closed [n]          1 if the last run closed that instance's window
+ *   closed [n]          1 if the last run closed that instance's window (0 after a ragged block with len[i] == 0)
  *   pub_* [n][...]      the same rows for the snapshot published when that instance's window last closed */
 int b200m_bim_results_all (b200m_bim* h, int32_t* hist, int32_t* cnt5, float* minmax2, int64_t* integration_time, int32_t* closed,
                            int32_t* pub_hist, int32_t* pub_cnt5, float* pub_minmax2, int64_t* pub_integration_time, void* stream);
@@ -466,6 +467,22 @@ int b200m_sdh_results (b200m_sdh* h, uint32_t inst, int32_t* hist361, int32_t* m
 /* every instance in ONE synchronisation; any pointer may be NULL.  Rows: hist [n][361], max_peak2 [n][2] = max count, peak bin;
  * avg_tmp_var3 [n][3] = sum, running mean, running variance accumulator; integration_time [n] */
 int b200m_sdh_results_all (b200m_sdh* h, int32_t* hist, int32_t* max_peak2, double* avg_tmp_var3, int64_t* integration_time, void* stream);
+/* Ragged blocks: instance i runs bim_run (src/bitmeter.c:248-327) / sdh_run (src/sigdistlv2.c:287-327) over the first len[i] <= nfram
+ * frames of its row only, bit-identical to a private plugin instance fed only those frames: histograms, counters, min / max, the fp64
+ * accumulators and the integration time (its 2^31-sample cap tested against len[i]).  len: host array of n_inst.
+ * - Frames at or after len[i] may hold anything, NaN, Inf and denormals included: they reach no counter, bin or statistic.
+ * - The bit-meter's ~5 fps window limit is that of a run of len[i] frames, len[i] * ceil (rate / (5 * len[i])) (:264), and its window
+ *   clock advances by len[i].
+ * - len[i] == 0: the instance is not run: nothing is acquired, its window clock stands still, no result changes -- except the
+ *   bit-meter's closed flag of that instance in b200m_bim_results_all, which reads 0 (its window did not close in this block).
+ * - A ragged bit-meter block leaves the bank-wide clock of b200m_bim_window_closed alone; that function reads 0 after it.
+ * - A length above nfram returns B200M_E_INVAL and enqueues nothing.
+ * - NULL, or every len[i] == nfram, is exactly b200m_bim_run_* / b200m_sdh_run_* (same kernels, launches and bits).
+ * - Controls, path switches and streams are ordered between ragged blocks as between plain ones. */
+int b200m_bim_run_ragged_device (b200m_bim* h, const float* d_in, size_t stride, uint32_t nfram, const uint32_t* len, void* stream);
+int b200m_bim_run_ragged_host (b200m_bim* h, const float* in, size_t stride, uint32_t nfram, const uint32_t* len);
+int b200m_sdh_run_ragged_device (b200m_sdh* h, const float* d_in, size_t stride, uint32_t nfram, const uint32_t* len, void* stream);
+int b200m_sdh_run_ragged_host (b200m_sdh* h, const float* in, size_t stride, uint32_t nfram, const uint32_t* len);
 
 /* ======================================================================================
  * 30-band 1/3-octave spectrum bank — replaces spectrum_instantiate / spectrum_run
@@ -523,6 +540,23 @@ int b200m_pw_set_mode (b200m_pw* h, int mode);
 /* returns (via *fired) whether this call completed an analysis (fftx_run()==0) */
 int b200m_pw_process_device (b200m_pw* h, const float* d_in, size_t stride, uint32_t nfram, float db_thresh, int* fired, void* stream);
 int b200m_pw_process_host (b200m_pw* h, const float* in, size_t stride, uint32_t nfram, float db_thresh, int* fired);
+/* Ragged blocks: stereo instance i (rows 2i, 2i+1) runs fftx_run on both channels (gui/fft.c:296-361) and then process_audio over the
+ * first len[i] <= nfram frames of its rows only, with its own ring offset and 25 Hz analysis clock, bit-identical to a private bank of
+ * one fed only those frames: phase, level, peak and the b200m_pw_raw spectra.  len: host array of n_inst.  *fired is 1 if any instance
+ * completed an analysis in this call.
+ * - Frames at or after len[i] may hold anything, NaN and Inf included: they reach no ring, spectrum or output.
+ * - len[i] == 0: the instance is not called: its ring and clock do not advance and its outputs stay.
+ * - A length above nfram returns B200M_E_INVAL and enqueues nothing.
+ * - NULL, or every len[i] == nfram, is exactly b200m_pw_process_* (same kernels, launches and bits) while the instances share one
+ *   ring offset and clock.  Once ragged blocks have moved them apart, plain blocks run the per-instance form with every length nfram
+ *   (unfused from an attached correlation bank), until the offsets and clocks agree again.
+ * - An attached correlation bank (b200m_pw_attach_cor) runs each pair over the same len[i] frames (b200m_cor_process_ragged_*), once
+ *   per call; b200m_cor_process_ragged_* on that bank itself stays refused.
+ * - Controls, path switches and streams are ordered between ragged blocks as between plain ones. */
+int b200m_pw_process_ragged_device (b200m_pw* h, const float* d_in, size_t stride, uint32_t nfram, const uint32_t* len,
+                                    float db_thresh, int* fired, void* stream);
+int b200m_pw_process_ragged_host (b200m_pw* h, const float* in, size_t stride, uint32_t nfram, const uint32_t* len,
+                                  float db_thresh, int* fired);
 /* phase[n_inst][fft_bins], level[n_inst][fft_bins], peak[n_inst] (ui->phase/level/peak) */
 int b200m_pw_results (b200m_pw* h, float* phase, float* level, float* peak, void* stream);
 /* ft->power / ft->phase of both channels of the last analysis (gui/fft.c:163-180), kept only while b200m_pw_debug_capture is on */

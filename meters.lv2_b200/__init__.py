@@ -162,6 +162,8 @@ _PROTOS = {
     "b200m_bim_control_inst": (C.c_int, [_v, C.c_int32, C.c_int, _v]),
     "b200m_bim_run_device": (C.c_int, [_v, _v, C.c_size_t, C.c_uint32, _v]),
     "b200m_bim_run_host": (C.c_int, [_v, _v, C.c_size_t, C.c_uint32]),
+    "b200m_bim_run_ragged_device": (C.c_int, [_v, _v, C.c_size_t, C.c_uint32, _v, _v]),
+    "b200m_bim_run_ragged_host": (C.c_int, [_v, _v, C.c_size_t, C.c_uint32, _v]),
     "b200m_bim_results": (C.c_int, [_v, C.c_uint32, _v, _v, _v, _v, _v]),
     "b200m_bim_window_closed": (C.c_int, [_v]),
     "b200m_bim_published": (C.c_int, [_v, C.c_uint32, _v, _v, _v, _v, _v]),
@@ -172,6 +174,8 @@ _PROTOS = {
     "b200m_sdh_control_inst": (C.c_int, [_v, C.c_int32, C.c_int, _v]),
     "b200m_sdh_run_device": (C.c_int, [_v, _v, C.c_size_t, C.c_uint32, _v]),
     "b200m_sdh_run_host": (C.c_int, [_v, _v, C.c_size_t, C.c_uint32]),
+    "b200m_sdh_run_ragged_device": (C.c_int, [_v, _v, C.c_size_t, C.c_uint32, _v, _v]),
+    "b200m_sdh_run_ragged_host": (C.c_int, [_v, _v, C.c_size_t, C.c_uint32, _v]),
     "b200m_sdh_results": (C.c_int, [_v, C.c_uint32, _v, _v, _v, _v, _v]),
     "b200m_sdh_results_all": (C.c_int, [_v, _v, _v, _v, _v, _v]),
     # spectr30
@@ -193,6 +197,8 @@ _PROTOS = {
     "b200m_pw_destroy": (C.c_int, [_v]),
     "b200m_pw_process_device": (C.c_int, [_v, _v, C.c_size_t, C.c_uint32, C.c_float, C.POINTER(C.c_int), _v]),
     "b200m_pw_process_host": (C.c_int, [_v, _v, C.c_size_t, C.c_uint32, C.c_float, C.POINTER(C.c_int)]),
+    "b200m_pw_process_ragged_device": (C.c_int, [_v, _v, C.c_size_t, C.c_uint32, _v, C.c_float, C.POINTER(C.c_int), _v]),
+    "b200m_pw_process_ragged_host": (C.c_int, [_v, _v, C.c_size_t, C.c_uint32, _v, C.c_float, C.POINTER(C.c_int)]),
     "b200m_pw_results": (C.c_int, [_v, _v, _v, _v, _v]),
     "b200m_pw_raw": (C.c_int, [_v, C.c_uint32, _v, _v, _v, _v, _v]),
     "b200m_pw_device_results": (C.c_int, [_v, C.POINTER(_v), C.POINTER(_v), C.POINTER(_v)]),
@@ -668,15 +674,25 @@ class _StatBank(_Bank):
         """CTL_* on one instance, or on every instance with inst = -1"""
         _ck(getattr(lib(), self._pfx + "control_inst")(self.h, inst, cmd, _stream_ptr(stream)))
 
-    def run(self, x, stream=None):
+    def run(self, x, stream=None, lengths=None):
+        """one run of every instance over x [n_inst, nfram] (CUDA tensor: device path; numpy / CPU tensor: host path).
+        lengths: None, or n_inst frame counts <= nfram: instance i runs over its first lengths[i] frames only (0: it is not run,
+        its window clock stands still), b200m_*_run_ragged_*."""
+        ln = None if lengths is None else _lengths(lengths, self.n_inst)
         if isinstance(x, np.ndarray) or not x.is_cuda:
             p, s, rows, n = _host_planar(x)
             assert rows == self.n_inst
-            _ck(getattr(lib(), self._pfx + "run_host")(self.h, p, s, n))
+            if ln is None:
+                _ck(getattr(lib(), self._pfx + "run_host")(self.h, p, s, n))
+            else:
+                _ck(getattr(lib(), self._pfx + "run_ragged_host")(self.h, p, s, n, _np_ptr(ln)))
         else:
             p, s, rows, n = _dev_ptr(x)
             assert rows == self.n_inst
-            _ck(getattr(lib(), self._pfx + "run_device")(self.h, p, s, n, _stream_ptr(stream)))
+            if ln is None:
+                _ck(getattr(lib(), self._pfx + "run_device")(self.h, p, s, n, _stream_ptr(stream)))
+            else:
+                _ck(getattr(lib(), self._pfx + "run_ragged_device")(self.h, p, s, n, _np_ptr(ln), _stream_ptr(stream)))
 
     def run_ptr(self, ptr, stride, nfram, stream=None):
         _ck(getattr(lib(), self._pfx + "run_device")(self.h, C.c_void_p(ptr), stride, nfram, _stream_ptr(stream)))
@@ -863,16 +879,26 @@ class Phasewheel(_Bank):
         self.n_inst, self.bins = n_inst, fft_bins
         _ck(lib().b200m_pw_create(C.byref(self.h), device, n_inst, fft_bins, rate))
 
-    def process(self, x, db_thresh=1e-6, stream=None):
+    def process(self, x, db_thresh=1e-6, stream=None, lengths=None):
+        """one block of every instance over x [2 n_inst, nfram]; returns 1 if an analysis completed.
+        lengths: None, or n_inst frame counts <= nfram: instance i runs over the first lengths[i] frames of its rows only, with its own
+        ring offset and analysis clock (0: it is not called), b200m_pw_process_ragged_*"""
         fired = C.c_int(0)
+        ln = None if lengths is None else _lengths(lengths, self.n_inst)
         if isinstance(x, np.ndarray) or not x.is_cuda:
             p, s, rows, n = _host_planar(x)
             assert rows == 2 * self.n_inst
-            _ck(lib().b200m_pw_process_host(self.h, p, s, n, db_thresh, C.byref(fired)))
+            if ln is None:
+                _ck(lib().b200m_pw_process_host(self.h, p, s, n, db_thresh, C.byref(fired)))
+            else:
+                _ck(lib().b200m_pw_process_ragged_host(self.h, p, s, n, _np_ptr(ln), db_thresh, C.byref(fired)))
         else:
             p, s, rows, n = _dev_ptr(x)
             assert rows == 2 * self.n_inst
-            _ck(lib().b200m_pw_process_device(self.h, p, s, n, db_thresh, C.byref(fired), _stream_ptr(stream)))
+            if ln is None:
+                _ck(lib().b200m_pw_process_device(self.h, p, s, n, db_thresh, C.byref(fired), _stream_ptr(stream)))
+            else:
+                _ck(lib().b200m_pw_process_ragged_device(self.h, p, s, n, _np_ptr(ln), db_thresh, C.byref(fired), _stream_ptr(stream)))
         return fired.value
 
     def process_ptr(self, ptr, stride, nfram, db_thresh=1e-6, stream=None):
@@ -1068,3 +1094,48 @@ def programme_dr14(x, lengths, rate=48000.0, n_channels=2, dr_mode=True, block=1
         return bank.results()
     finally:
         bank.close()
+
+
+def programme_stats(x, lengths, rate=48000.0, block=1024, device=0):
+    """Whole-clip bit-meter and signal-distribution statistics of N mono clips of different lengths (file QC: the bit depth actually
+    used, NaN / Inf / denormal counts, the sample distribution), in one bit-meter bank (averaging mode, integrating) and one
+    SigDistHist bank (integrating).
+
+    x: row i = clip i, valid for its first lengths[i] frames: a [N, >= max(lengths)] float32 numpy array / CPU tensor (host path) or
+    CUDA tensor (device path), or a callable f(offset, nfram) that returns frames offset .. offset + nfram - 1 of every row as such an
+    array.  Frames past a clip's length are never read into a result.  The clips are fed in blocks of `block` frames with clip i's
+    length in block k clamp(lengths[i] - k * block, 0, block) (Bitmeter.run / SigDistHist.run with lengths), so clip i's rows are
+    bit-identical to a bitmeter (averaging) and a SigDistHist plugin instance fed the whole clip.
+    Returns a dict of arrays of N rows, each clip's statistics after its last frame:
+      bim_hist [N, 584] int32, bim_cnt [N, 5] int32 (zero, pos, nan, inf, den), bim_minmax [N, 2] float32, bim_itime [N] int64;
+      sdh_hist [N, 361] int32, sdh_max_peak [N, 2] int32, sdh_avg_tmp_var [N, 3] float64 (sum, running mean, running variance
+      accumulator), sdh_itime [N] int64.
+    An empty clip reads what a freshly instantiated plugin reads: zero counts and sums, bit-meter minimum +inf, peak bin -1."""
+    ln = np.asarray(lengths, np.int64).ravel()
+    n = ln.size
+    if n == 0:
+        raise B200MError("no clips")
+    if ln.min() < 0:
+        raise B200MError("lengths must be frame counts >= 0")
+    if not 1 <= int(block) <= 8192:
+        raise B200MError("block must be 1..8192 frames")
+    bim, sdh = Bitmeter(n, rate, device), None
+    try:
+        sdh = SigDistHist(n, rate, device)
+        bim.control(CTL_AVERAGE)
+        sdh.control(CTL_START)
+        total = int(ln.max())
+        for off in range(0, total, int(block)):
+            nfram = min(int(block), total - off)
+            xb = x(off, nfram) if callable(x) else x[:, off:off + nfram]
+            lb = np.clip(ln - off, 0, nfram)
+            bim.run(xb, lengths=lb)
+            sdh.run(xb, lengths=lb)
+        b = bim.results_all()
+        h, mp, av, it = sdh.results_all()
+    finally:
+        bim.close()
+        if sdh is not None:
+            sdh.close()
+    return dict(bim_hist=b["hist"], bim_cnt=b["cnt"], bim_minmax=b["minmax"], bim_itime=b["itime"],
+                sdh_hist=h, sdh_max_peak=mp, sdh_avg_tmp_var=av, sdh_itime=it)

@@ -334,6 +334,15 @@ static int cor_process (b200m_cor* h, const float* d_in, size_t stride, uint32_t
     return cor_launch<true> (h, d_in, stride, nfram, st, nullptr, 0, 0);
 }
 
+namespace b200m {
+// a ragged block of the phasewheel bank this one is attached to (b200m_pw_process_ragged_*): pair i runs over its first len[i] frames,
+// unfused, exactly as b200m_cor_process_ragged_* would run it
+int cor_feed_ragged (b200m_cor* h, const float* d_in, size_t stride, uint32_t nfram, const uint32_t* len, cudaStream_t st)
+{
+    return cor_process (h, d_in, stride, nfram, len, st);
+}
+}
+
 // b200m_cor_process_ctl_*: run[i] == 0 holds pair i, a ragged block of lengths run[i] ? nfram : 0 (NULL run: every pair runs)
 static const uint32_t* cor_ctl_len (b200m_cor* h, uint32_t nfram, const uint8_t* run)
 {

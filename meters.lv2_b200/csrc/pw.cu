@@ -9,13 +9,16 @@
 // Every size the reference GUI offers is provided: fft_bins 64 .. 8192 and 6144 (N = 128 .. 16384 and 12288 = 3 * 4096,
 // gui/phasewheel.c:1108-1116).
 //
-// Design: the ring buffers of all instances advance in lock step, so the host tracks the write
-// offset and the 25 Hz analysis clock; one CTA per instance runs, per channel, an N/2-point complex autosort
+// Design: while the ring buffers of all instances advance in lock step, the host tracks one write offset and one 25 Hz analysis
+// clock; ragged blocks (b200m_pw_process_ragged_*) give each instance its own, mirrored on the host, which then decides per step of
+// the block which instances' analyses to launch.  One CTA per instance runs, per channel, an N/2-point complex autosort
 // (Stockham) FFT in shared memory (radix-3 pass when 3 | N, radix-4 passes, one radix-2 pass when needed), splits it
 // into the real spectrum, and writes phase difference / level bins with coalesced stores.  The block append can be
 // fused with the stereo-correlation bank (b200m_pw_attach_cor): the input is then read from HBM once for both meters.
 #include <math.h>
 #include <stdlib.h>
+#include <algorithm>
+#include <vector>
 #include "common.cuh"
 
 namespace b200m {
@@ -31,6 +34,20 @@ __global__ void pw_append_kernel (const float* __restrict__ in, size_t stride, i
     const int row = (int)(idx / nfram), j = (int)(idx % nfram);
     int o = rboff + j; if (o >= N) o -= N;                                    // nfram <= N, rboff < N
     ring[(size_t)row * N + o] = in[(size_t)row * stride + j];
+}
+
+// Step s of a ragged block (b200m_pw_process_ragged_*, frames [s0, s0 + cmax), s0 = s N): instance i appends its frames
+// [s0, min (len[i], s0 + N)) to its own ring at its own offset rb[i].  Every whole step advances a ring by N frames, so the offset at
+// the start of each step is the one at the start of the call.
+__global__ void pw_ragged_append_kernel (const float* __restrict__ in, size_t stride, int n_inst, int cmax, int s0, int N,
+                                         const uint32_t* __restrict__ rb, const uint32_t* __restrict__ len, float* __restrict__ ring)
+{
+    const size_t idx = (size_t)blockIdx.x * blockDim.x + threadIdx.x;
+    if (idx >= (size_t)n_inst * 2 * cmax) return;
+    const int row = (int)(idx / cmax), j = (int)(idx % cmax), i = row >> 1;
+    if (s0 + j >= (int)len[i]) return;
+    int o = (int)rb[i] + j; if (o >= N) o -= N;                               // cmax <= N, rb[i] < N
+    ring[(size_t)row * N + o] = in[(size_t)row * stride + s0 + j];
 }
 
 B200M_DEV float2 cmul (float2 a, float2 b) { return make_float2 (fmaf (a.x, b.x, -a.y * b.y), fmaf (a.x, b.y, a.y * b.x)); }
@@ -88,17 +105,21 @@ B200M_DEV void stockham_pass (const float2* __restrict__ X, float2* __restrict__
 // z[n] = x[2n] + i x[2n+1] followed by the usual split  X[k] = E[k] + W_N^k O[k]  (E, O: transforms of the even / odd samples):
 // half the shared memory of packing L + iR into one N-point transform, which is what lets N = 16384 (gui/phasewheel.c:1116)
 // fit: 2 x M complex ping-pong buffers + the left channel's power / phase = 12 N bytes.
+// RAG (ragged blocks): CTA b analyses instance fire[2 b] with the oldest sample at fire[2 b + 1], its own ring offset when it fired.
+template <bool RAG>
 __global__ void __launch_bounds__ (PW_THREADS)
 pw_analyze_kernel (const float* __restrict__ ring, int N, int f3, int f4, int f2, int start, const float* __restrict__ window,
                    const float2* __restrict__ tw, float db_thresh, float* __restrict__ rawp /* [inst][4][bins] or NULL */,
-                   float* __restrict__ phase, float* __restrict__ level, float* __restrict__ peak, int mode)
+                   float* __restrict__ phase, float* __restrict__ level, float* __restrict__ peak, int mode,
+                   const uint32_t* __restrict__ fire)
 {
     extern __shared__ __align__ (16) float2 sm[];          // X, Y: M complex each; then powL[bins], phL[bins]
     __shared__ float red[PW_THREADS / 32];
     const int M = N / 2, bins = N / 2;
     float2* bufA = sm; float2* bufB = sm + M;
     float* sPL = reinterpret_cast<float*> (sm + 2 * M); float* sFL = sPL + bins;
-    const int inst = blockIdx.x, tid = threadIdx.x;
+    const int inst = RAG ? (int)fire[2 * blockIdx.x] : blockIdx.x, tid = threadIdx.x;
+    if (RAG) start = (int)fire[2 * blockIdx.x + 1];
     float pk = 0.0f;
     for (int ch = 0; ch < 2; ++ch) {
         const float* rg = ring + ((size_t)inst * 2 + ch) * N;
@@ -180,6 +201,8 @@ namespace b200m {
 // cor.cu: one Stcorrdsp::process block for every pair of the bank; when `ring` is given the block is also appended to the
 // phasewheel ring [pair][2][N] at offset rboff (fused feed: the input is read once)
 int cor_feed (b200m_cor* h, const float* d_in, size_t stride, uint32_t nfram, cudaStream_t st, float* ring, int N, int rboff);
+// cor.cu: the same block with pair i over its first len[i] frames (cor_kernel<true> / cor_scan_kernel<true>), no ring
+int cor_feed_ragged (b200m_cor* h, const float* d_in, size_t stride, uint32_t nfram, const uint32_t* len, cudaStream_t st);
 uint32_t cor_instances (const b200m_cor* h);
 // the ordering of a phasewheel bank and its attached correlation bank (nullptr: none): a call enters its path on the correlation
 // bank first; cor_host_stream is the stream of the host path and of the getters after it
@@ -191,6 +214,12 @@ void cor_attach (b200m_cor* h, int d);                       // counts the phase
 struct b200m_pw {
     int device; uint32_t n_inst, bins, N; int f3, f4, f2; double rate;
     uint32_t rboff, smps, sps, step;                       // shared ring offset + 25 Hz analysis clock (gui/fft.c:43-64)
+    // each instance's ring offset and clock once ragged blocks have moved them apart; empty while every instance agrees (rboff, smps)
+    std::vector<uint32_t> rb, sm;
+    // ragged-block scratch: every length nfram (a plain block once the clocks differ), each instance's last firing step, the
+    // firing instances per step; and the upload of rb[n] | len[n] | (instance, ring start) of the firing instances by step
+    std::vector<uint32_t> full, off; std::vector<int> fire;
+    RaggedLen rag;
     int mode = 0;                                          // 0: phasewheel process_audio, 1: stereoscope process_audio
     float *d_ring = nullptr, *d_win = nullptr, *d_raw = nullptr, *d_phase = nullptr, *d_level = nullptr, *d_peak = nullptr;
     float2* d_tw = nullptr;
@@ -202,7 +231,8 @@ struct b200m_pw {
 static cudaStream_t pw_stream (b200m_pw* h, void* stream) { return h->path.last_host ? cor_host_stream (h->cor, h->path.own) : (cudaStream_t)stream; }
 static size_t pw_smem_bytes (uint32_t N) { return (size_t)12 * N; }   // 2 x N/2 float2 + 2 x N/2 float
 
-static int pw_process (b200m_pw* h, const float* d_in, size_t stride, uint32_t nfram, float db_thresh, int* fired, cudaStream_t st)
+// a plain block while every instance shares one ring offset and clock
+static int pw_lockstep (b200m_pw* h, const float* d_in, size_t stride, uint32_t nfram, float db_thresh, int* fired, cudaStream_t st)
 {
     // fftx_run walks the block in steps of at most window_size (gui/fft.c:346-360) and process_audio runs ONCE
     // after both channels' fftx_run (gui/phasewheel.c:1310-1313): when several analyses fire inside one call only
@@ -233,8 +263,9 @@ static int pw_process (b200m_pw* h, const float* d_in, size_t stride, uint32_t n
         if (h->smps >= h->sps) {                            // :308-313
             h->step = h->smps; h->smps = 0;
             if (step == last_fire) {
-                pw_analyze_kernel<<<h->n_inst, PW_THREADS, pw_smem_bytes (h->N), st>>> (
-                    h->d_ring, (int)h->N, h->f3, h->f4, h->f2, (int)h->rboff, h->d_win, h->d_tw, db_thresh, h->d_raw, h->d_phase, h->d_level, h->d_peak, h->mode);
+                pw_analyze_kernel<false><<<h->n_inst, PW_THREADS, pw_smem_bytes (h->N), st>>> (
+                    h->d_ring, (int)h->N, h->f3, h->f4, h->f2, (int)h->rboff, h->d_win, h->d_tw, db_thresh, h->d_raw, h->d_phase, h->d_level, h->d_peak, h->mode,
+                    nullptr);
                 B200M_LAUNCHED (1);
             }
             any = 1;
@@ -244,6 +275,104 @@ static int pw_process (b200m_pw* h, const float* d_in, size_t stride, uint32_t n
     if (fired) *fired = any;
     B200M_CUDA (cudaGetLastError ());
     return 0;
+}
+
+// Instance i over its first len[i] frames, with its own ring offset rb[i] and clock sm[i]: the per-instance form of pw_lockstep.
+// plain: a plain block (every length nfram) of a bank whose clocks differ; an attached correlation bank then runs the plain kernel.
+// Each instance's block is walked in steps of N frames as fftx_run walks it (gui/fft.c:346-360): step s covers its frames
+// [s N, min (len[i], (s + 1) N)).  Per step, one append kernel, then one analysis of the instances whose LAST firing in this call
+// falls in that step (process_audio runs once per call, after fftx_run: gui/phasewheel.c:1310-1313); stream order gives each
+// analysis its ring as it stood when that instance fired.
+static int pw_ragged (b200m_pw* h, const float* d_in, size_t stride, uint32_t nfram, const uint32_t* len, bool plain, float db_thresh,
+                      int* fired, cudaStream_t st)
+{
+    const uint32_t n = h->n_inst, N = h->N;
+    if (h->rb.empty ()) { h->rb.assign (n, h->rboff); h->sm.assign (n, h->smps); }
+    uint32_t maxlen = 0, nfire = 0;
+    h->fire.assign (n, -1);
+    for (uint32_t i = 0; i < n; ++i) {                     // the host mirror of _fftx_run's clock (gui/fft.c:308-313)
+        uint32_t smps = h->sm[i], s = 0;
+        for (uint32_t d = 0; d < len[i]; d += N, ++s) {
+            smps += std::min (N, len[i] - d);
+            if (smps >= h->sps) { smps = 0; h->fire[i] = (int)s; }
+        }
+        h->sm[i] = smps;
+        maxlen = std::max (maxlen, len[i]);
+        nfire += h->fire[i] >= 0;
+    }
+    const uint32_t nsteps = (maxlen + N - 1) / N;
+    // upload rb[n] | len[n] | (instance, ring start at its firing) pairs, grouped by firing step (counting sort)
+    cudaError_t e = cudaSuccess;
+    uint32_t* w = h->rag.stage ((size_t)4 * n, &e);
+    if (!w) return cuda_fail (e, "pw_ragged", __FILE__, __LINE__);
+    memcpy (w, h->rb.data (), n * sizeof (uint32_t));
+    memcpy (w + n, len, n * sizeof (uint32_t));
+    h->off.assign (nsteps + 1, 0);
+    for (uint32_t i = 0; i < n; ++i) if (h->fire[i] >= 0) ++h->off[h->fire[i] + 1];
+    for (uint32_t s = 0; s < nsteps; ++s) h->off[s + 1] += h->off[s];
+    {
+        std::vector<uint32_t> cur (h->off.begin (), h->off.end () - 1);
+        for (uint32_t i = 0; i < n; ++i) {
+            if (h->fire[i] < 0) continue;
+            const uint32_t f = (uint32_t)h->fire[i], k = cur[f]++;
+            w[2 * n + 2 * k] = i;
+            w[2 * n + 2 * k + 1] = (h->rb[i] + std::min (N, len[i] - f * N)) % N;          // its ring offset after step f
+        }
+    }
+    B200M_CUDA (h->rag.upload ((size_t)2 * n + 2 * nfire, st));
+    // Stcorrdsp::process sees the call as ONE block per pair (its scrub and bias act per call): unfused, ahead of the steps
+    if (h->cor) {
+        const int rc = plain ? cor_feed (h->cor, d_in, stride, nfram, st, nullptr, 0, 0) : cor_feed_ragged (h->cor, d_in, stride, nfram, len, st);
+        if (rc) return rc;
+    }
+    for (uint32_t s = 0; s < nsteps; ++s) {
+        const uint32_t cmax = std::min (N, maxlen - s * N);
+        const size_t total = (size_t)n * 2 * cmax;
+        pw_ragged_append_kernel<<<(unsigned)((total + 255) / 256), 256, 0, st>>> (d_in, stride, (int)n, (int)cmax, (int)(s * N), (int)N, h->rag.d,
+                                                                                   h->rag.d + n, h->d_ring);
+        B200M_LAUNCHED (1);
+        if (const uint32_t c = h->off[s + 1] - h->off[s]) {
+            pw_analyze_kernel<true><<<c, PW_THREADS, pw_smem_bytes (N), st>>> (
+                h->d_ring, (int)N, h->f3, h->f4, h->f2, 0, h->d_win, h->d_tw, db_thresh, h->d_raw, h->d_phase, h->d_level, h->d_peak, h->mode,
+                h->rag.d + 2 * n + 2 * h->off[s]);
+            B200M_LAUNCHED (1);
+        }
+    }
+    bool agree = true;
+    for (uint32_t i = 0; i < n; ++i) {
+        h->rb[i] = (h->rb[i] + len[i]) % N;
+        agree = agree && h->rb[i] == h->rb[0] && h->sm[i] == h->sm[0];
+    }
+    if (agree) { h->rboff = h->rb[0]; h->smps = h->sm[0]; h->rb.clear (); h->sm.clear (); }   // back to the lock-step path
+    if (fired) *fired = nfire > 0;
+    B200M_CUDA (cudaGetLastError ());
+    return 0;
+}
+
+// rlen: NULL (a plain block) or the host array of n_inst lengths, some below nfram
+static int pw_process (b200m_pw* h, const float* d_in, size_t stride, uint32_t nfram, const uint32_t* rlen, float db_thresh, int* fired,
+                       cudaStream_t st)
+{
+    if (!rlen && h->rb.empty ()) return pw_lockstep (h, d_in, stride, nfram, db_thresh, fired, st);
+    if (rlen) return pw_ragged (h, d_in, stride, nfram, rlen, false, db_thresh, fired, st);
+    h->full.assign (h->n_inst, nfram);
+    return pw_ragged (h, d_in, stride, nfram, h->full.data (), true, db_thresh, fired, st);
+}
+
+// every block entry point.  A call first enters its path on the attached correlation bank (cor_follow); the host path stages the
+// block on that bank's own stream, if one is attached (cor_host_stream), else on the phasewheel bank's own.
+static int pw_block (b200m_pw* h, const float* in, size_t stride, uint32_t nfram, const uint32_t* len, float db_thresh, int* fired, bool host,
+                     void* stream)
+{
+    return bank_call (h, in, stride, nfram, host, stream, 0, h ? h->n_inst : 0, len, no_check,
+                      [&] (const float* d_in, size_t ds, cudaStream_t st, const uint32_t* rlen) {
+                          if (int rc = cor_follow (h->cor, host)) return rc;
+                          if (host) {
+                              st = cor_host_stream (h->cor, h->path.own);
+                              if (int rc = h->path.stage_block (in, stride, nfram, (size_t)2 * h->n_inst, st, &d_in, &ds)) return rc;
+                          }
+                          return pw_process (h, d_in, ds, nfram, rlen, db_thresh, fired, st);
+                      });
 }
 
 extern "C" {
@@ -291,7 +420,8 @@ int b200m_pw_create (b200m_pw** out, int device, uint32_t n_inst, uint32_t fft_b
     if (e == cudaSuccess) e = cudaMemcpy (h->d_win, win, N * sizeof (float), cudaMemcpyHostToDevice);
     if (e == cudaSuccess) e = cudaMemcpy (h->d_tw, tw, N * sizeof (float2), cudaMemcpyHostToDevice);
     free (win); free (tw);
-    if (e == cudaSuccess) e = cudaFuncSetAttribute (pw_analyze_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)pw_smem_bytes (16384));
+    if (e == cudaSuccess) e = cudaFuncSetAttribute (pw_analyze_kernel<false>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)pw_smem_bytes (16384));
+    if (e == cudaSuccess) e = cudaFuncSetAttribute (pw_analyze_kernel<true>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)pw_smem_bytes (16384));
     if (e == cudaSuccess) e = cudaStreamCreateWithFlags (&h->path.own, cudaStreamNonBlocking);
     if (e == cudaSuccess) {
         const size_t n = (size_t)n_inst * fft_bins;       // ui->level[i] = -100, ui->phase[i] = 0 (phasewheel.c:199-202)
@@ -310,7 +440,7 @@ int b200m_pw_destroy (b200m_pw* h)
     DeviceGuard g (h->device);
     cudaDeviceSynchronize ();
     cudaFree (h->d_ring); cudaFree (h->d_win); cudaFree (h->d_tw); cudaFree (h->d_raw); cudaFree (h->d_phase); cudaFree (h->d_level); cudaFree (h->d_peak);
-    h->path.release ();
+    h->rag.release (); h->path.release ();
     delete h;
     return 0;
 }
@@ -331,25 +461,26 @@ int b200m_pw_set_mode (b200m_pw* h, int mode)
     return 0;
 }
 
+// while a correlation bank is attached the phasewheel bank's own stream is idle: its host-path calls run on cor_host_stream
 int b200m_pw_process_device (b200m_pw* h, const float* d_in, size_t stride, uint32_t nfram, float db_thresh, int* fired, void* stream)
 {
-    if (int rc = check_block_args (h, d_in, stride, nfram)) return rc;
-    DeviceGuard g (h->device);
-    if (int rc = cor_follow (h->cor, false)) return rc;
-    if (int rc = h->path.enter_device ()) return rc;      // while a correlation bank is attached own is idle: its host-path calls ran on cor_host_stream
-    return pw_process (h, d_in, stride, nfram, db_thresh, fired, (cudaStream_t)stream);
+    return pw_block (h, d_in, stride, nfram, nullptr, db_thresh, fired, false, stream);
 }
 
 int b200m_pw_process_host (b200m_pw* h, const float* in, size_t stride, uint32_t nfram, float db_thresh, int* fired)
 {
-    if (int rc = check_block_args (h, in, stride, nfram)) return rc;
-    DeviceGuard g (h->device);
-    if (int rc = h->path.enter_host ()) return rc;
-    if (int rc = cor_follow (h->cor, true)) return rc;
-    const cudaStream_t st = cor_host_stream (h->cor, h->path.own);
-    const float* d_in; size_t ds;
-    if (int rc = h->path.stage_block (in, stride, nfram, (size_t)2 * h->n_inst, st, &d_in, &ds)) return rc;
-    return pw_process (h, d_in, ds, nfram, db_thresh, fired, st);
+    return pw_block (h, in, stride, nfram, nullptr, db_thresh, fired, true, nullptr);
+}
+
+int b200m_pw_process_ragged_device (b200m_pw* h, const float* d_in, size_t stride, uint32_t nfram, const uint32_t* len, float db_thresh, int* fired,
+                                    void* stream)
+{
+    return pw_block (h, d_in, stride, nfram, len, db_thresh, fired, false, stream);
+}
+
+int b200m_pw_process_ragged_host (b200m_pw* h, const float* in, size_t stride, uint32_t nfram, const uint32_t* len, float db_thresh, int* fired)
+{
+    return pw_block (h, in, stride, nfram, len, db_thresh, fired, true, nullptr);
 }
 
 int b200m_pw_results (b200m_pw* h, float* phase, float* level, float* peak, void* stream)

@@ -24,15 +24,25 @@ constexpr int BIM_WARPS = 4;
 // the snapshot published when the ~5 fps window closes: pub_hist[584], pub_cnt[8], pub_mm[2], pub_itime.
 // One run of bim_run (src/bitmeter.c:248-327) per instance: acquisition (skipped while paused or at the 2^31 cap), then the
 // window clock; a closing window publishes the warp's shared-memory histogram and, in windowed mode, clears the statistics.
-__global__ void __launch_bounds__ (BIM_WARPS * 32, 16)
+// RAG (b200m_bim_run_ragged_*): instance inst runs bim_run over its first rlen[inst] frames, with the window limit of that run
+// length, fps_tab[rlen[inst]] (:264, the host's fps_limit of every block length); rlen 0: not run, only its closed flag reads 0.
+// The run length then sits in a register, not in the parameter bank: 12 CTAs per SM (40 registers) instead of 16 keep it unspilled.
+template <bool RAG>
+__global__ void __launch_bounds__ (BIM_WARPS * 32, RAG ? 12 : 16)
 bim_kernel (const float* __restrict__ in, size_t stride, int n_inst, int nfram, int fps_limit, int32_t* __restrict__ hist,
             int32_t* __restrict__ cnt, float* __restrict__ minmax, int32_t* __restrict__ st, int64_t* __restrict__ itime,
-            int32_t* __restrict__ pub_hist, int32_t* __restrict__ pub_cnt, float* __restrict__ pub_mm, int64_t* __restrict__ pub_itime)
+            int32_t* __restrict__ pub_hist, int32_t* __restrict__ pub_cnt, float* __restrict__ pub_mm, int64_t* __restrict__ pub_itime,
+            const uint32_t* __restrict__ rlen, const int32_t* __restrict__ fps_tab)
 {
     __shared__ int32_t sh[BIM_WARPS][BIM_LEN];
     const int lane = threadIdx.x & 31, w = threadIdx.x >> 5;
     const int inst = blockIdx.x * BIM_WARPS + w;
     if (inst >= n_inst) return;
+    if (RAG) {                                               // one warp per instance: the length is warp-uniform
+        nfram = (int)rlen[inst];
+        if (nfram == 0) { if (lane == 0) st[4 * inst + 3] = 0; return; }
+        fps_limit = fps_tab[nfram];
+    }
     const int integrating = st[4 * inst], average = st[4 * inst + 1];
     int64_t it = itime[inst];
     bool acc = false;
@@ -161,9 +171,13 @@ constexpr int SDH_SMEM = (SDH_BINS * SDH_BP + 3 + SDH_STAGES * 32 * SDH_P) * 4; 
 
 // per instance: hist[361] (layout [n][361]), ip[2] = max count, peak bin; dp[3] = avg, var_m, var_s; integrating, itime.
 // A lane whose instance is paused or at the 2^31-sample cap (src/sigdistlv2.c:287) scans nothing; a CTA with no such lane exits.
+// RAG (b200m_sdh_run_ragged_*): lane's instance runs sdh_run over its first rlen[inst] frames (0: not run); the warp stages tiles
+// up to its longest running length.
+template <bool RAG>
 __global__ void __launch_bounds__ (32)
 sdh_kernel (const float* __restrict__ in, size_t stride, int n_inst, int nfram, int aligned, const int32_t* __restrict__ integrating,
-            int64_t* __restrict__ itime, int32_t* __restrict__ hist, int32_t* __restrict__ ip, double* __restrict__ dp)
+            int64_t* __restrict__ itime, int32_t* __restrict__ hist, int32_t* __restrict__ ip, double* __restrict__ dp,
+            const uint32_t* __restrict__ rlen)
 {
     extern __shared__ __align__ (16) int32_t sdh_smem[];
     int32_t* sb = sdh_smem;                                  // [361][33]
@@ -171,19 +185,21 @@ sdh_kernel (const float* __restrict__ in, size_t stride, int n_inst, int nfram, 
     const int lane = threadIdx.x, i0 = blockIdx.x * 32;
     const int inst = min (i0 + lane, n_inst - 1);
     const bool live = (i0 + lane) < n_inst;
+    const int rl = RAG ? (live ? (int)rlen[inst] : 0) : nfram;                 // this instance's run length
     int64_t it = itime[inst];
-    bool run = live && integrating[inst] && it < 2147483647;
-    if (run && it > 2147483647 - nfram) { it = 2147483647; run = false; }
+    bool run = live && (!RAG || rl > 0) && integrating[inst] && it < 2147483647;
+    if (run && it > 2147483647 - rl) { it = 2147483647; run = false; }
     if (!__any_sync (0xffffffffu, run)) { if (live) itime[inst] = it; return; }
+    const int wend = RAG ? __reduce_max_sync (0xffffffffu, run ? rl : 0) : nfram;   // frames the warp stages
     const double itime0 = (double)it;
-    const int ntiles = (nfram + SDH_T - 1) / SDH_T;
+    const int ntiles = (wend + SDH_T - 1) / SDH_T;
     auto issue = [&] (int t) {
         if (t < ntiles) {
             float* dst = tile + (t % SDH_STAGES) * (32 * SDH_P);
             const int s0 = t * SDH_T;
             if (aligned) {
                 const int c4 = (lane & 15) * 4;
-                const int left = (nfram - (s0 + c4)) * 4;
+                const int left = (wend - (s0 + c4)) * 4;
                 const int nb = left >= 16 ? 16 : (left > 0 ? left : 0);
 #pragma unroll
                 for (int i = 0; i < 16; ++i) {
@@ -196,7 +212,7 @@ sdh_kernel (const float* __restrict__ in, size_t stride, int n_inst, int nfram, 
                     const int ir = min (i0 + r, n_inst - 1);
 #pragma unroll
                     for (int hh = 0; hh < 2; ++hh) {
-                        const int c = lane + 32 * hh; const bool ok = (s0 + c) < nfram;
+                        const int c = lane + 32 * hh; const bool ok = (s0 + c) < wend;
                         cp_async4 (dst + r * SDH_P + c, ok ? in + (size_t)ir * stride + s0 + c : in, ok ? 4 : 0);
                     }
                 }
@@ -218,7 +234,7 @@ sdh_kernel (const float* __restrict__ in, size_t stride, int n_inst, int nfram, 
         cp_async_wait<1> ();
         __syncwarp ();
         const float* row = tile + (t % SDH_STAGES) * (32 * SDH_P) + lane * SDH_P;
-        const int len = run ? min (SDH_T, nfram - t * SDH_T) : 0;
+        const int len = run ? min (SDH_T, rl - t * SDH_T) : 0;
         for (int j = 0; j < len; ++j) {                      // src/sigdistlv2.c:303-318
             const float val = row[j];
             const float r = rintf (__fadd_rn (180.f, __fmul_rn (val, 150.f)));
@@ -239,7 +255,7 @@ sdh_kernel (const float* __restrict__ in, size_t stride, int n_inst, int nfram, 
         if (i0 + r >= n_inst) break;
         for (int b = lane; b < SDH_BINS; b += 32) hist[(size_t)(i0 + r) * SDH_BINS + b] = sb[b * SDH_BP + r];
     }
-    if (run) { ip[2 * inst] = peak_cnt; ip[2 * inst + 1] = peak_bin; dp[3 * inst] = avg; dp[3 * inst + 1] = vm; dp[3 * inst + 2] = vs; it += nfram; }
+    if (run) { ip[2 * inst] = peak_cnt; ip[2 * inst + 1] = peak_bin; dp[3 * inst] = avg; dp[3 * inst + 1] = vm; dp[3 * inst + 2] = vs; it += rl; }
     if (live) itime[inst] = it;
 }
 
@@ -266,11 +282,14 @@ struct b200m_bim {
     // the statistics as they stood when an instance's last ~5 fps window closed, i.e. what bim_run publishes before bim_clear (:267-326)
     int32_t *d_pub_hist = nullptr, *d_pub_cnt = nullptr; float* d_pub_mm = nullptr; int64_t* d_pub_itime = nullptr;
     int resync = 0; bool window_closed = false;                // the window clock of a bank driven only bank-wide (b200m_bim_window_closed)
+    RaggedLen rag;                                             // the lengths of a ragged block
+    int32_t* d_fps = nullptr;                                  // fps_limit of every block length 0 .. B200M_MAX_BLOCK (ragged blocks)
     BankPath path;
 };
 struct b200m_sdh {
     int device; uint32_t n_inst; double rate;
     int32_t *d_hist = nullptr, *d_ip = nullptr, *d_integ = nullptr; double* d_dp = nullptr; int64_t* d_itime = nullptr;
+    RaggedLen rag;
     BankPath path;
 };
 
@@ -288,12 +307,27 @@ static int bim_control (b200m_bim* h, int32_t inst, int cmd, cudaStream_t st)
     return 0;
 }
 
-static int bim_run (b200m_bim* h, const float* d_in, size_t stride, uint32_t n, cudaStream_t st)
+// rlen: NULL, or the host array of n_inst lengths of a ragged block (bank_call passes it only when some length differs from n)
+// the ~5 fps window limit of a block of n frames (:264)
+static int bim_fps_limit (double rate, uint32_t n) { return n * ceil (rate / (5.f * n)); }
+
+static int bim_run (b200m_bim* h, const float* d_in, size_t stride, uint32_t n, const uint32_t* rlen, cudaStream_t st)
 {
     // bim_run (:248-327) for every instance: acquisition, the ~5 fps window clock, publish + windowed-mode clear
-    const int fps_limit = n * ceil (h->rate / (5.f * n));
-    bim_kernel<<<(h->n_inst + BIM_WARPS - 1) / BIM_WARPS, BIM_WARPS * 32, 0, st>>> (d_in, stride, (int)h->n_inst, (int)n, fps_limit, h->d_hist, h->d_cnt, h->d_mm,
-                                                                                   h->d_st, h->d_itime, h->d_pub_hist, h->d_pub_cnt, h->d_pub_mm, h->d_pub_itime);
+    const int fps_limit = bim_fps_limit (h->rate, n);
+    const unsigned grid = (h->n_inst + BIM_WARPS - 1) / BIM_WARPS;
+    if (rlen) {
+        // each instance's window limit follows its own run length; the bank-wide clock stands still and reads "not closed"
+        if (int rc = h->rag.put (rlen, h->n_inst, st)) return rc;
+        bim_kernel<true><<<grid, BIM_WARPS * 32, 0, st>>> (d_in, stride, (int)h->n_inst, (int)n, fps_limit, h->d_hist, h->d_cnt, h->d_mm, h->d_st,
+                                                           h->d_itime, h->d_pub_hist, h->d_pub_cnt, h->d_pub_mm, h->d_pub_itime, h->rag.d, h->d_fps);
+        B200M_LAUNCHED (1);
+        h->window_closed = false;
+        B200M_CUDA (cudaGetLastError ());
+        return 0;
+    }
+    bim_kernel<false><<<grid, BIM_WARPS * 32, 0, st>>> (d_in, stride, (int)h->n_inst, (int)n, fps_limit, h->d_hist, h->d_cnt, h->d_mm,
+                                                        h->d_st, h->d_itime, h->d_pub_hist, h->d_pub_cnt, h->d_pub_mm, h->d_pub_itime, nullptr, nullptr);
     B200M_LAUNCHED (1);
     h->resync += n;
     h->window_closed = h->resync >= fps_limit;
@@ -315,10 +349,18 @@ static int sdh_control (b200m_sdh* h, int32_t inst, int cmd, cudaStream_t st)
     return 0;
 }
 
-static int sdh_run (b200m_sdh* h, const float* d_in, size_t stride, uint32_t n, cudaStream_t st)
+static int sdh_run (b200m_sdh* h, const float* d_in, size_t stride, uint32_t n, const uint32_t* rlen, cudaStream_t st)
 {
     const int aligned = ((uintptr_t)d_in % 16 == 0) && (stride % 4 == 0);
-    sdh_kernel<<<(h->n_inst + 31) / 32, 32, SDH_SMEM, st>>> (d_in, stride, (int)h->n_inst, (int)n, aligned, h->d_integ, h->d_itime, h->d_hist, h->d_ip, h->d_dp);
+    const unsigned grid = (h->n_inst + 31) / 32;
+    if (rlen) {
+        if (int rc = h->rag.put (rlen, h->n_inst, st)) return rc;
+        sdh_kernel<true><<<grid, 32, SDH_SMEM, st>>> (d_in, stride, (int)h->n_inst, (int)n, aligned, h->d_integ, h->d_itime, h->d_hist, h->d_ip, h->d_dp,
+                                                      h->rag.d);
+    } else {
+        sdh_kernel<false><<<grid, 32, SDH_SMEM, st>>> (d_in, stride, (int)h->n_inst, (int)n, aligned, h->d_integ, h->d_itime, h->d_hist, h->d_ip, h->d_dp,
+                                                       nullptr);
+    }
     B200M_LAUNCHED (1);
     B200M_CUDA (cudaGetLastError ());
     return 0;
@@ -343,7 +385,13 @@ int b200m_bim_create (b200m_bim** out, int device, uint32_t n_inst, double rate)
     A ((void**)&h->d_hist, (size_t)n_inst * BIM_LEN * 4); A ((void**)&h->d_cnt, (size_t)n_inst * 8 * 4); A ((void**)&h->d_mm, (size_t)n_inst * 2 * 4);
     A ((void**)&h->d_st, (size_t)n_inst * 4 * 4); A ((void**)&h->d_itime, (size_t)n_inst * 8);
     A ((void**)&h->d_pub_hist, (size_t)n_inst * BIM_LEN * 4); A ((void**)&h->d_pub_cnt, (size_t)n_inst * 8 * 4); A ((void**)&h->d_pub_mm, (size_t)n_inst * 2 * 4);
-    A ((void**)&h->d_pub_itime, (size_t)n_inst * 8);
+    A ((void**)&h->d_pub_itime, (size_t)n_inst * 8); A ((void**)&h->d_fps, (B200M_MAX_BLOCK + 1) * 4);
+    if (e == cudaSuccess) {
+        static_assert (B200M_MAX_BLOCK <= 8192, "fps table on the stack");
+        int32_t fps[B200M_MAX_BLOCK + 1] = {0};
+        for (uint32_t n = 1; n <= B200M_MAX_BLOCK; ++n) fps[n] = bim_fps_limit (rate, n);
+        e = cudaMemcpy (h->d_fps, fps, sizeof (fps), cudaMemcpyHostToDevice);
+    }
     if (e == cudaSuccess) e = cudaStreamCreateWithFlags (&h->path.own, cudaStreamNonBlocking);
     if (e == cudaSuccess) { bim_control (h, -1, B200M_CTL_CLEAR, nullptr); e = cudaDeviceSynchronize (); }      // bim_instantiate (:146-158)
     if (e != cudaSuccess) { int rc = cuda_fail (e, "bim_create", __FILE__, __LINE__); b200m_bim_destroy (h); return rc; }
@@ -356,7 +404,8 @@ int b200m_bim_destroy (b200m_bim* h)
     DeviceGuard g (h->device);
     cudaDeviceSynchronize ();
     cudaFree (h->d_hist); cudaFree (h->d_cnt); cudaFree (h->d_mm); cudaFree (h->d_st); cudaFree (h->d_itime);
-    cudaFree (h->d_pub_hist); cudaFree (h->d_pub_cnt); cudaFree (h->d_pub_mm); cudaFree (h->d_pub_itime); h->path.release ();
+    cudaFree (h->d_pub_hist); cudaFree (h->d_pub_cnt); cudaFree (h->d_pub_mm); cudaFree (h->d_pub_itime); cudaFree (h->d_fps); h->rag.release ();
+    h->path.release ();
     delete h;
     return 0;
 }
@@ -367,13 +416,21 @@ int b200m_bim_control_inst (b200m_bim* h, int32_t inst, int cmd, void* stream)
     DeviceGuard g (h->device);
     return bim_control (h, inst, cmd, h->path.stream (stream));   // CTL_* handling of bim_run (:207-231)
 }
-static int bim_block (b200m_bim* h, const float* in, size_t stride, uint32_t nfram, bool host, void* stream)
+static int bim_block (b200m_bim* h, const float* in, size_t stride, uint32_t nfram, const uint32_t* len, bool host, void* stream)
 {
-    return bank_call (h, in, stride, nfram, host, stream, h ? h->n_inst : 0, 0, nullptr, no_check,
-                      [&] (const float* d_in, size_t ds, cudaStream_t st, const uint32_t*) { return bim_run (h, d_in, ds, nfram, st); });
+    return bank_call (h, in, stride, nfram, host, stream, h ? h->n_inst : 0, h ? h->n_inst : 0, len, no_check,
+                      [&] (const float* d_in, size_t ds, cudaStream_t st, const uint32_t* rlen) { return bim_run (h, d_in, ds, nfram, rlen, st); });
 }
-int b200m_bim_run_device (b200m_bim* h, const float* d_in, size_t stride, uint32_t nfram, void* stream) { return bim_block (h, d_in, stride, nfram, false, stream); }
-int b200m_bim_run_host (b200m_bim* h, const float* in, size_t stride, uint32_t nfram) { return bim_block (h, in, stride, nfram, true, nullptr); }
+int b200m_bim_run_device (b200m_bim* h, const float* d_in, size_t stride, uint32_t nfram, void* stream) { return bim_block (h, d_in, stride, nfram, nullptr, false, stream); }
+int b200m_bim_run_host (b200m_bim* h, const float* in, size_t stride, uint32_t nfram) { return bim_block (h, in, stride, nfram, nullptr, true, nullptr); }
+int b200m_bim_run_ragged_device (b200m_bim* h, const float* d_in, size_t stride, uint32_t nfram, const uint32_t* len, void* stream)
+{
+    return bim_block (h, d_in, stride, nfram, len, false, stream);
+}
+int b200m_bim_run_ragged_host (b200m_bim* h, const float* in, size_t stride, uint32_t nfram, const uint32_t* len)
+{
+    return bim_block (h, in, stride, nfram, len, true, nullptr);
+}
 // one row of statistics (hist, counters, min/max, integration time), live or published, of instances [i0, i0 + n)
 static int bim_copy_rows (b200m_bim* h, bool pub, uint32_t i0, uint32_t n, int32_t* hist, int32_t* cnt5, float* mm2, int64_t* itime, cudaStream_t st)
 {
@@ -434,7 +491,8 @@ int b200m_sdh_create (b200m_sdh** out, int device, uint32_t n_inst, double rate)
     A ((void**)&h->d_hist, (size_t)n_inst * SDH_BINS * 4); A ((void**)&h->d_ip, (size_t)n_inst * 2 * 4); A ((void**)&h->d_dp, (size_t)n_inst * 3 * 8);
     A ((void**)&h->d_integ, (size_t)n_inst * 4); A ((void**)&h->d_itime, (size_t)n_inst * 8);
     if (e == cudaSuccess) e = cudaStreamCreateWithFlags (&h->path.own, cudaStreamNonBlocking);
-    if (e == cudaSuccess) e = cudaFuncSetAttribute (sdh_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, SDH_SMEM);
+    if (e == cudaSuccess) e = cudaFuncSetAttribute (sdh_kernel<false>, cudaFuncAttributeMaxDynamicSharedMemorySize, SDH_SMEM);
+    if (e == cudaSuccess) e = cudaFuncSetAttribute (sdh_kernel<true>, cudaFuncAttributeMaxDynamicSharedMemorySize, SDH_SMEM);
     if (e == cudaSuccess) { sdh_control (h, -1, B200M_CTL_CLEAR, nullptr); e = cudaDeviceSynchronize (); }        // sdh_instantiate (:141-150)
     if (e != cudaSuccess) { int rc = cuda_fail (e, "sdh_create", __FILE__, __LINE__); b200m_sdh_destroy (h); return rc; }
     *out = h;
@@ -445,7 +503,7 @@ int b200m_sdh_destroy (b200m_sdh* h)
     if (!h) return 0;
     DeviceGuard g (h->device);
     cudaDeviceSynchronize ();
-    cudaFree (h->d_hist); cudaFree (h->d_ip); cudaFree (h->d_dp); cudaFree (h->d_integ); cudaFree (h->d_itime); h->path.release ();
+    cudaFree (h->d_hist); cudaFree (h->d_ip); cudaFree (h->d_dp); cudaFree (h->d_integ); cudaFree (h->d_itime); h->rag.release (); h->path.release ();
     delete h;
     return 0;
 }
@@ -456,13 +514,21 @@ int b200m_sdh_control_inst (b200m_sdh* h, int32_t inst, int cmd, void* stream)
     DeviceGuard g (h->device);
     return sdh_control (h, inst, cmd, h->path.stream (stream));   // sdh_integrate / sdh_reset (:233-241)
 }
-static int sdh_block (b200m_sdh* h, const float* in, size_t stride, uint32_t nfram, bool host, void* stream)
+static int sdh_block (b200m_sdh* h, const float* in, size_t stride, uint32_t nfram, const uint32_t* len, bool host, void* stream)
 {
-    return bank_call (h, in, stride, nfram, host, stream, h ? h->n_inst : 0, 0, nullptr, no_check,
-                      [&] (const float* d_in, size_t ds, cudaStream_t st, const uint32_t*) { return sdh_run (h, d_in, ds, nfram, st); });
+    return bank_call (h, in, stride, nfram, host, stream, h ? h->n_inst : 0, h ? h->n_inst : 0, len, no_check,
+                      [&] (const float* d_in, size_t ds, cudaStream_t st, const uint32_t* rlen) { return sdh_run (h, d_in, ds, nfram, rlen, st); });
 }
-int b200m_sdh_run_device (b200m_sdh* h, const float* d_in, size_t stride, uint32_t nfram, void* stream) { return sdh_block (h, d_in, stride, nfram, false, stream); }
-int b200m_sdh_run_host (b200m_sdh* h, const float* in, size_t stride, uint32_t nfram) { return sdh_block (h, in, stride, nfram, true, nullptr); }
+int b200m_sdh_run_device (b200m_sdh* h, const float* d_in, size_t stride, uint32_t nfram, void* stream) { return sdh_block (h, d_in, stride, nfram, nullptr, false, stream); }
+int b200m_sdh_run_host (b200m_sdh* h, const float* in, size_t stride, uint32_t nfram) { return sdh_block (h, in, stride, nfram, nullptr, true, nullptr); }
+int b200m_sdh_run_ragged_device (b200m_sdh* h, const float* d_in, size_t stride, uint32_t nfram, const uint32_t* len, void* stream)
+{
+    return sdh_block (h, d_in, stride, nfram, len, false, stream);
+}
+int b200m_sdh_run_ragged_host (b200m_sdh* h, const float* in, size_t stride, uint32_t nfram, const uint32_t* len)
+{
+    return sdh_block (h, in, stride, nfram, len, true, nullptr);
+}
 static int sdh_copy_rows (b200m_sdh* h, uint32_t i0, uint32_t n, int32_t* hist, int32_t* mp2, double* atv3, int64_t* itime, cudaStream_t st)
 {
     if (hist) B200M_CUDA (cudaMemcpyAsync (hist, h->d_hist + (size_t)i0 * SDH_BINS, (size_t)n * SDH_BINS * 4, cudaMemcpyDeviceToHost, st));
