@@ -140,6 +140,20 @@ int b200m_ebu_process_ragged_host (b200m_ebu* h, const float* in, size_t stride,
 /* getters -> host array of n_inst results.  stream = the stream last used for processing
  * (ignored after process_host, which uses the bank's stream). */
 int b200m_ebu_results (b200m_ebu* h, b200m_ebu_result* out, void* stream);
+/* Loudness log (an extension; the reference keeps only the latest values): one point per completed 50 ms fragment of an instance
+ * (every pass through process()'s _frcnt == 0 branch, :217-243), holding exactly what b200m_ebu_results would return right after
+ * that fragment, its gating included.  Points are written whether integration runs or not; controls write none and leave the log
+ * alone, snapshots neither save nor restore it.  Each instance keeps its last `capacity` points in a ring on the device. */
+typedef struct b200m_ebu_point { float loudness_M, loudness_S, integrated, range_min, range_max; } b200m_ebu_point;
+/* capacity points per instance; 0 turns the log off and frees it; (re)enabling empties it.  B200M_E_NOMEM (the log off) if the
+ * device cannot hold 2 x capacity x n_inst points. */
+int b200m_ebu_log_enable (b200m_ebu* h, uint32_t capacity, void* stream);
+/* the capacity the log was enabled with: the row length of b200m_ebu_log_drain's `out`; 0 while the log is off or h is NULL */
+uint32_t b200m_ebu_log_capacity (const b200m_ebu* h);
+/* host out [n_inst][capacity], count [n_inst], lost [n_inst]: instance i's points since the previous drain, oldest first, in
+ * out[i][0 .. count[i]) (NaN after them); lost[i] older unread points were overwritten.  Ordered after the work on `stream` like
+ * b200m_ebu_results (synchronises it).  B200M_E_INVAL with the log off. */
+int b200m_ebu_log_drain (b200m_ebu* h, b200m_ebu_point* out, uint32_t* count, uint64_t* lost, void* stream);
 /* histogram_M()/histogram_S() (:91-92) of one instance: 751 + 751 int32 */
 int b200m_ebu_histogram (b200m_ebu* h, uint32_t inst, int32_t* hist_M, int32_t* hist_S, void* stream);
 /* K-weighting coefficients as designed on the host (detect_init, :263-293): a0 a1 a2 b1 b2 c3 c4 */
@@ -292,6 +306,8 @@ size_t b200m_r128_snapshot_size (b200m_r128* h);
 int b200m_r128_snapshot (b200m_r128* h, void* buf, size_t bytes, void* stream);
 int b200m_r128_restore (b200m_r128* h, const void* buf, size_t bytes, void* stream);
 b200m_ebu* b200m_r128_ebu (b200m_r128* h);     /* the underlying banks (histograms, state, coefficients) */
+/* the EBU bank of an EBUr128 bank follows that bank's path: after a b200m_r128_run_host* call its getters, controls and log calls
+ * (b200m_ebu_log_enable / _drain) run on the EBUr128 bank's own stream, after a device-path call on the stream they are given */
 b200m_tpk* b200m_r128_tpk (b200m_r128* h);
 
 /* ======================================================================================

@@ -33,6 +33,8 @@ class EbuResult(C.Structure):
 EBU_RESULT_DTYPE = np.dtype([(n, "<f4") for n in ("loudness_M", "maxloudn_M", "loudness_S", "maxloudn_S", "integrated",
                                                     "integ_thr", "range_min", "range_max", "range_thr")] +
                             [("hist_M_count", "<i4"), ("hist_S_count", "<i4"), ("frag_power", "<f4")])
+# one point of the loudness log (b200m_ebu_point): the values after one completed 50 ms fragment of an instance
+EBU_POINT_DTYPE = np.dtype([(n, "<f4") for n in ("loudness_M", "loudness_S", "integrated", "range_min", "range_max")])
 TPK_RESULT_DTYPE = np.dtype([("tp_m", "<f4"), ("tp_p", "<f4"), ("km_rms", "<f4"), ("km_peak", "<f4")])
 
 _PROTOS = {
@@ -62,6 +64,9 @@ _PROTOS = {
     "b200m_ebu_process_ragged_host": (C.c_int, [_v, _v, C.c_size_t, C.c_uint32, _v]),
     "b200m_ebu_results": (C.c_int, [_v, _v, _v]),
     "b200m_ebu_histogram": (C.c_int, [_v, C.c_uint32, _v, _v, _v]),
+    "b200m_ebu_log_enable": (C.c_int, [_v, C.c_uint32, _v]),
+    "b200m_ebu_log_drain": (C.c_int, [_v, _v, _v, _v, _v]),
+    "b200m_ebu_log_capacity": (C.c_uint32, [_v]),
     "b200m_ebu_coeffs": (C.c_int, [_v, _v]),
     "b200m_ebu_state": (C.c_int, [_v, C.c_uint32, _v, _v, _v, _v, _v]),
     "b200m_ebu_mix_reduce": (C.c_int, [_v, _v, _v]),
@@ -426,6 +431,20 @@ class Ebu_r128_proc(_Bank):
         out = np.empty(self.n_inst, EBU_RESULT_DTYPE)
         _ck(lib().b200m_ebu_results(self.h, _np_ptr(out), _stream_ptr(stream)))
         return out
+
+    def log_enable(self, capacity, stream=None):
+        """keep the last `capacity` loudness points of every instance on the device, one per completed 50 ms fragment
+        (b200m_ebu_log_enable); 0 turns the log off, (re)enabling empties it"""
+        _ck(lib().b200m_ebu_log_enable(self.h, int(capacity), _stream_ptr(stream)))
+
+    def log_drain(self, stream=None):
+        """the points logged since the last drain (b200m_ebu_log_drain): (points [n_inst, capacity] EBU_POINT_DTYPE, oldest first,
+        NaN past count; count uint32 [n_inst]; lost uint64 [n_inst], older points overwritten before they were drained)"""
+        cap = int(lib().b200m_ebu_log_capacity(self.h))          # the bank's, whoever enabled the log
+        pts = np.empty((self.n_inst, max(cap, 1)), EBU_POINT_DTYPE)
+        cnt = np.empty(self.n_inst, np.uint32); lost = np.empty(self.n_inst, np.uint64)
+        _ck(lib().b200m_ebu_log_drain(self.h, _np_ptr(pts), _np_ptr(cnt), _np_ptr(lost), _stream_ptr(stream)))
+        return pts, cnt, lost
 
     def histogram(self, inst, stream=None):
         hm = np.empty(HIST_LEN, np.int32); hs = np.empty(HIST_LEN, np.int32)
@@ -1017,11 +1036,23 @@ class EBUr128(_Bank):
         _ck(lib().b200m_r128_histogram(self.h, int(inst), _np_ptr(m), _np_ptr(s), _stream_ptr(stream)))
         return m, s
 
+    def log_enable(self, capacity, stream=None):
+        """the loudness log of the cycle's EBU R128 bank: Ebu_r128_proc.log_enable"""
+        self.ebu.log_enable(capacity, stream)
+
+    def log_drain(self, stream=None):
+        """Ebu_r128_proc.log_drain of the cycle's EBU R128 bank"""
+        return self.ebu.log_drain(stream)
+
 
 PROGRAMME_FIELDS = ("integrated", "integ_thr", "range_min", "range_max", "maxloudn_M", "maxloudn_S")
+CURVE_FIELDS = (("curve_M", "loudness_M"), ("curve_S", "loudness_S"), ("curve_I", "integrated"), ("curve_range_min", "range_min"),
+                ("curve_range_max", "range_max"))
+CURVE_LOG_POINTS = 1200        # the loudness log's capacity in programme_loudness: 60 s of fragments at 48 kHz
 
 
-def programme_loudness(x, lengths, fsamp=48000.0, nchan=2, gains=None, block=1024, dbtp=True, precision=PREC_EXACT, device=0):
+def programme_loudness(x, lengths, fsamp=48000.0, nchan=2, gains=None, block=1024, dbtp=True, precision=PREC_EXACT, device=0,
+                       curves=False):
     """Whole-programme EBU R128 loudness and true peak of N clips of different lengths, in one bank.
 
     x: rows i * nchan + c of clip i (nchan channels, or len(gains) with per-channel weights as in EBUr128), clip i valid for its
@@ -1034,7 +1065,12 @@ def programme_loudness(x, lengths, fsamp=48000.0, nchan=2, gains=None, block=102
     clip in blocks of `block` frames with a short last block -- the reference's results depend on where blocks are cut
     (ebu_r128_proc.cc:212-216).  No padding is metered: a short clip's loudness, maxima, histograms and range stop at its end.
     Returns a dict of float32 arrays of N: integrated, integ_thr, range_min, range_max, maxloudn_M, maxloudn_S (LUFS / LU, -200
-    where the reference reports nothing) and tp_max (dBTP, -inf when dbtp is False or the clip is empty)."""
+    where the reference reports nothing) and tp_max (dBTP, -inf when dbtp is False or the clip is empty).
+    curves=True adds each clip's loudness curve, one point per 50 ms fragment (fragm = int(fsamp) // 20 frames), point k ending at
+    frame (k + 1) * fragm of the clip: n_points (int64 [N], lengths // fragm) and curve_M, curve_S, curve_I, curve_range_min,
+    curve_range_max (float32 [N, max(n_points)], NaN past a clip's n_points), each point what the clip's reading was right after
+    that fragment.  The bank's loudness log holds CURVE_LOG_POINTS points per clip and is drained before it can overflow, so the
+    device memory does not grow with the programme; the other fields are the same as with curves=False."""
     ln = np.asarray(lengths, np.int64).ravel()
     n = ln.size
     if n == 0:
@@ -1050,15 +1086,40 @@ def programme_loudness(x, lengths, fsamp=48000.0, nchan=2, gains=None, block=102
         bank.set_precision(precision)
         bank.control(EBUr128.START)
         total = int(ln.max())
-        for off in range(0, total, int(block)):
+        if curves:
+            fragm = int(fsamp) // 20
+            n_points = ln // fragm
+            cv = {k: np.full((n, int(n_points.max())), np.nan, np.float32) for k, _ in CURVE_FIELDS}
+            pos = np.zeros(n, np.int64)
+            bank.log_enable(CURVE_LOG_POINTS)
+            per_block = int(block) // fragm + 1                 # the most fragments one block completes for an instance
+            drain_every = CURVE_LOG_POINTS // per_block
+
+            def drain():
+                # a drain copies every instance's whole [CURVE_LOG_POINTS] row (NaN past its count), however few points are new
+                pts, cnt, lost = bank.log_drain()
+                if lost.any():
+                    raise B200MError("loudness log overflow: %d points lost" % int(lost.sum()))
+                i, j = np.nonzero(np.arange(pts.shape[1]) < cnt[:, None].astype(np.int64))
+                for k, f in CURVE_FIELDS:
+                    cv[k][i, pos[i] + j] = pts[f][i, j]
+                pos[:] += cnt
+        for b, off in enumerate(range(0, total, int(block))):
             nfram = min(int(block), total - off)
             xb = x(off, nfram) if callable(x) else x[:, off:off + nfram]
             bank.run(xb, lengths=np.clip(ln - off, 0, nfram))
+            if curves and (b + 1) % drain_every == 0:
+                drain()
+        if curves:
+            drain()
         r, tp = bank.results()
     finally:
         bank.close()
     out = {k: np.ascontiguousarray(r[k], np.float32) for k in PROGRAMME_FIELDS}
     out["tp_max"] = tp
+    if curves:
+        out["n_points"] = n_points
+        out.update(cv)
     return out
 
 

@@ -473,6 +473,13 @@ B200M_DEV void hist_calc_range (const int* row, int count, const float* bp, int 
     v1 = __fdiv_rn ((float)(j - 699), 10.0f);
 }
 
+// The loudness log (b200m_ebu_log_enable): one point {M, S, I, range_min, range_max} per completed fragment of an instance, `cap`
+// points per instance.  Field f of point slot s of instance i is pts[(f * cap + s) * n_inst + i] (planes [5][cap][n_inst]: lane =
+// instance stores coalesce, like the power ring); written[i] counts the instance's points, the next goes to slot written[i] % cap.
+// pts == nullptr: the log is off.
+struct EbuLog { float* pts; unsigned long long* written; uint32_t cap; };
+constexpr int EBU_LOG_FIELDS = 5;
+
 // K2a: one THREAD per instance, one completed 50 ms fragment (process :217-243 minus the gated statistics).
 // ring layout [64][n_inst] so that lane = instance accesses coalesce; each thread parks its 64-slot ring column
 // in shared memory (column private to the thread: no barrier needed) for the two ordered sums.
@@ -484,7 +491,7 @@ constexpr int K2A_THREADS = 128;
 __global__ void __launch_bounds__ (K2A_THREADS)
 ebu_fragment_kernel (int n_inst, int frag, const int* __restrict__ fph, int tmod, int fragm, int nfram, const float* __restrict__ fragpw,
                      float* __restrict__ ring, EbuCtl* __restrict__ ctl, b200m_ebu_result* __restrict__ res, int* __restrict__ histM,
-                     int* __restrict__ histS, int* __restrict__ cnt, const uint32_t* __restrict__ rlen)
+                     int* __restrict__ histS, int* __restrict__ cnt, const uint32_t* __restrict__ rlen, EbuLog lg)
 {
     __shared__ float sring[64][K2A_THREADS];
     const int tid = threadIdx.x;
@@ -545,6 +552,13 @@ ebu_fragment_kernel (int n_inst, int frag, const int* __restrict__ fph, int tmod
         }
     }
     ctl[i] = c; res[i] = r;
+    if (lg.pts) {                                           // the values before this fragment's gating: K2b rewrites I and the range
+        const unsigned long long w = lg.written[i];
+        const size_t pl = (size_t)lg.cap * n_inst;
+        float* p = lg.pts + (size_t)(w % lg.cap) * n_inst + i;
+        p[0] = lm; p[pl] = ls; p[2 * pl] = r.integrated; p[3 * pl] = r.range_min; p[4 * pl] = r.range_max;
+        lg.written[i] = w + 1;
+    }
 }
 
 // K2b: one WARP per instance, only launched when the host's phase book-keeping says that some instance
@@ -553,7 +567,7 @@ constexpr int K2B_WARPS = 4;
 
 __global__ void __launch_bounds__ (K2B_WARPS * 32)
 ebu_gate_kernel (int n_inst, EbuCtl* __restrict__ ctl, b200m_ebu_result* __restrict__ res, const int* histM,
-                 const int* histS, const int* __restrict__ cnt, const float* __restrict__ bin_power)
+                 const int* histS, const int* __restrict__ cnt, const float* __restrict__ bin_power, EbuLog lg)
 {
     __shared__ float sbp[100];
     for (int q = threadIdx.x; q < 100; q += blockDim.x) sbp[q] = bin_power[q];
@@ -570,7 +584,64 @@ ebu_gate_kernel (int n_inst, EbuCtl* __restrict__ ctl, b200m_ebu_result* __restr
         res[inst].integrated = vi; res[inst].integ_thr = th;
         res[inst].range_min = v0; res[inst].range_max = v1; res[inst].range_thr = rt;
         ctl[inst].calc = 0;
+        // the K2a launch in front of this one set calc and wrote the instance's latest point
+        const unsigned long long w = lg.pts ? lg.written[inst] : 0ull;
+        if (w) {
+            const size_t pl = (size_t)lg.cap * n_inst;
+            float* p = lg.pts + (size_t)((w - 1) % lg.cap) * n_inst + inst;
+            p[2 * pl] = vi; p[3 * pl] = v0; p[4 * pl] = v1;
+        }
     }
+}
+
+// Drain of the loudness log: per instance the points written since the last drain, oldest first, at most cap of them, into
+// out[n_inst][cap][5] (NaN past the instance's count), with count[i] and lost[i] (unread points overwritten before this drain);
+// then the read cursor moves to written[i].  A CTA owns 32 instances and walks their points in tiles of 32: lane = instance reads
+// the planes, a shared-memory transpose makes the stores of the [cap][5] rows coalesce.
+constexpr int LOG_DRAIN_ROWS = 8;
+
+__global__ void __launch_bounds__ (32 * LOG_DRAIN_ROWS)
+ebu_log_drain_kernel (int n_inst, EbuLog lg, unsigned long long* __restrict__ rd, float* __restrict__ out, uint32_t* __restrict__ count,
+                      unsigned long long* __restrict__ lost)
+{
+    __shared__ float tile[32][32 * EBU_LOG_FIELDS + 1];
+    const int tx = threadIdx.x & 31, ty = threadIdx.x >> 5;
+    const int i0 = blockIdx.x * 32, i = i0 + tx;
+    const uint32_t cap = lg.cap;
+    const size_t pl = (size_t)cap * n_inst;
+    unsigned long long w = 0, start = 0;
+    uint32_t cnt = 0;
+    if (i < n_inst) {
+        w = lg.written[i];
+        const unsigned long long unread = w - rd[i];
+        cnt = unread < cap ? (uint32_t)unread : cap;
+        start = w - cnt;
+        if (ty == 0) { count[i] = cnt; lost[i] = unread - cnt; }
+    }
+    for (uint32_t j0 = 0; j0 < cap; j0 += 32) {
+        for (int jl = ty; jl < 32; jl += LOG_DRAIN_ROWS) {
+            const uint32_t j = j0 + jl;
+            float v[EBU_LOG_FIELDS];
+            if (i < n_inst && j < cnt) {
+                const float* p = lg.pts + (size_t)((start + j) % cap) * n_inst + i;
+#pragma unroll
+                for (int f = 0; f < EBU_LOG_FIELDS; ++f) v[f] = p[f * pl];
+            } else {
+#pragma unroll
+                for (int f = 0; f < EBU_LOG_FIELDS; ++f) v[f] = __int_as_float (0x7fc00000);
+            }
+#pragma unroll
+            for (int f = 0; f < EBU_LOG_FIELDS; ++f) tile[tx][jl * EBU_LOG_FIELDS + f] = v[f];
+        }
+        __syncthreads ();
+        const int nq = (int)min (32u, cap - j0) * EBU_LOG_FIELDS;        // the tile's floats of one instance's row, contiguous in out
+        for (int il = ty; il < 32 && i0 + il < n_inst; il += LOG_DRAIN_ROWS) {
+            float* o = out + ((size_t)(i0 + il) * cap + j0) * EBU_LOG_FIELDS;
+            for (int q = tx; q < nq; q += 32) o[q] = tile[il][q];
+        }
+        __syncthreads ();
+    }
+    if (i < n_inst && ty == 0) rd[i] = w;
 }
 
 // a ragged block moves every instance's clock on by its own length, not by the block's nfram: its phase (the bank time at which
@@ -689,7 +760,19 @@ struct b200m_ebu {
     float *d_z = nullptr, *d_frpwr = nullptr, *d_fragpw = nullptr, *d_ring = nullptr, *d_binpow = nullptr, *d_out5 = nullptr;
     EbuCtl* d_ctl = nullptr; b200m_ebu_result* d_res = nullptr;
     int *d_histM = nullptr, *d_histS = nullptr, *d_cnt = nullptr, *d_fph = nullptr;
+    // the loudness log (b200m_ebu_log_enable), off while log.pts is null: the planes and written counters K2a / K2b update, the read
+    // cursors, and the drain's device output (points, counts, lost counts)
+    EbuLog log = {nullptr, nullptr, 0};
+    unsigned long long *d_log_rd = nullptr, *d_log_lost = nullptr; float* d_log_out = nullptr; uint32_t* d_log_cnt = nullptr;
+    void log_free () {
+        cudaFree (log.pts); cudaFree (log.written); cudaFree (d_log_rd); cudaFree (d_log_lost); cudaFree (d_log_out); cudaFree (d_log_cnt);
+        log = {nullptr, nullptr, 0}; d_log_rd = d_log_lost = nullptr; d_log_out = nullptr; d_log_cnt = nullptr;
+    }
     BankPath path;
+    // the path of the EBUr128 bank this bank belongs to (ebu_follow), nullptr for a bank of its own: that bank drives this one's
+    // kernels on its streams, so this bank's getters, controls and log calls resolve their stream through its path
+    const BankPath* owner = nullptr;
+    cudaStream_t stream (void* caller) const { return (owner ? owner : &path)->stream (caller); }
     bool use_tma = false;                // K1 tiles by TMA (opt-in, 16-byte aligned input only) instead of cp.async
     bool split = false;                  // K1 as two warps per 32 channels (ebu_kweight_split), opt-in with B200M_EBU_SPLIT=1: measured slower, see the kernel
     // Host mirror of every instance's S-histogram period (_div2, :234-241), kept in O(1) per fragment and phase class: the
@@ -799,7 +882,7 @@ static int ebu_ctl (b200m_ebu* h, int32_t inst, int cmd, void* stream)
     if (cmd == 3) { if (inst < 0) h->phase_reset (); else h->phase_restart ((uint32_t)inst); }
     else h->phase_ctl (inst, cmd);
     // after process_host the bank runs on its own stream: a control on any other stream would race with the kernels in flight
-    ebu_ctl_kernel<<<(h->n_inst + 127) / 128, 128, 0, h->path.stream (stream)>>> (
+    ebu_ctl_kernel<<<(h->n_inst + 127) / 128, 128, 0, h->stream (stream)>>> (
         (int)h->n_inst, inst, cmd, (int)h->nchan, h->d_z, h->d_frpwr, h->d_ring, h->d_ctl, h->d_res, h->d_histM, h->d_histS, h->d_cnt,
         h->d_fph, cmd == 3 ? h->tmod : -1);
     B200M_LAUNCHED (1);
@@ -957,6 +1040,7 @@ int b200m_ebu_destroy (b200m_ebu* h)
     cudaDeviceSynchronize ();
     cudaFree (h->d_z); cudaFree (h->d_frpwr); cudaFree (h->d_fragpw); cudaFree (h->d_ring); cudaFree (h->d_binpow);
     cudaFree (h->d_out5); cudaFree (h->d_ctl); cudaFree (h->d_res); cudaFree (h->d_histM); cudaFree (h->d_histS); cudaFree (h->d_cnt); cudaFree (h->d_fph);
+    h->log_free ();
     h->rag.release ();
     h->path.release ();
     delete h;
@@ -976,7 +1060,7 @@ int b200m_ebu_clear (b200m_ebu* h, int32_t inst, void* stream)
     if (!h || inst < 0 || inst >= (int32_t)h->n_inst) return set_err (B200M_E_INVAL, "bad argument");
     DeviceGuard g (h->device);
     h->phase_ctl (inst, 0); h->phase_ctl (inst, 2);
-    ebu_ctl_kernel<<<(h->n_inst + 127) / 128, 128, 0, h->path.stream (stream)>>> (
+    ebu_ctl_kernel<<<(h->n_inst + 127) / 128, 128, 0, h->stream (stream)>>> (
         (int)h->n_inst, inst, 3, (int)h->nchan, h->d_z, h->d_frpwr, h->d_ring, h->d_ctl, h->d_res, h->d_histM, h->d_histS, h->d_cnt,
         h->d_fph, -1);
     B200M_LAUNCHED (1);
@@ -1092,7 +1176,7 @@ int ebu_process_sliced (b200m_ebu* h, const float* d_in, size_t stride, uint32_t
         if (after_k1 && done == 0) { if (int rc = after_k1 (after_arg)) return rc; }      // work to enqueue right behind the first K1
         for (int f = 0; f < nfrag; ++f) {                    // fragments complete in order; each may trigger gating
             ebu_fragment_kernel<<<(h->n_inst + K2A_THREADS - 1) / K2A_THREADS, K2A_THREADS, 0, st>>> (
-                (int)h->n_inst, f, ck.fph, h->tmod, h->fragm, (int)nfram, h->d_fragpw, h->d_ring, h->d_ctl, h->d_res, h->d_histM, h->d_histS, h->d_cnt, d_len);
+                (int)h->n_inst, f, ck.fph, h->tmod, h->fragm, (int)nfram, h->d_fragpw, h->d_ring, h->d_ctl, h->d_res, h->d_histM, h->d_histS, h->d_cnt, d_len, h->log);
             B200M_LAUNCHED (1);
             // K2b behind fragment f only if some class completing its fragment f has an integrating member whose S period wraps
             // there: a later addpoint in the same block would otherwise be gated into the statistics
@@ -1105,7 +1189,7 @@ int ebu_process_sliced (b200m_ebu* h, const float* d_in, size_t stride, uint32_t
             if (d_len) wrap |= h->ragged_tick (f);
             if (wrap) {
                 ebu_gate_kernel<<<(h->n_inst + K2B_WARPS - 1) / K2B_WARPS, K2B_WARPS * 32, 0, st>>> (
-                    (int)h->n_inst, h->d_ctl, h->d_res, h->d_histM, h->d_histS, h->d_cnt, h->d_binpow);
+                    (int)h->n_inst, h->d_ctl, h->d_res, h->d_histM, h->d_histS, h->d_cnt, h->d_binpow, h->log);
                 B200M_LAUNCHED (1);
             }
         }
@@ -1158,8 +1242,60 @@ int b200m_ebu_results (b200m_ebu* h, b200m_ebu_result* out, void* stream)
 {
     if (!h || !out) return set_err (B200M_E_INVAL, "NULL argument");
     DeviceGuard g (h->device);
-    cudaStream_t st = h->path.stream (stream);
+    cudaStream_t st = h->stream (stream);
     B200M_CUDA (cudaMemcpyAsync (out, h->d_res, h->n_inst * sizeof (b200m_ebu_result), cudaMemcpyDeviceToHost, st));
+    B200M_CUDA (cudaStreamSynchronize (st));
+    return 0;
+}
+
+int b200m_ebu_log_enable (b200m_ebu* h, uint32_t capacity, void* stream)
+{
+    if (!h) return set_err (B200M_E_INVAL, "NULL handle");
+    DeviceGuard g (h->device);
+    cudaStream_t st = h->stream (stream);
+    if (h->log.pts) {                                        // kernels in flight may still write the old log
+        B200M_CUDA (cudaStreamSynchronize (st));
+        h->log_free ();
+    }
+    if (capacity == 0) return 0;
+    const size_t n = h->n_inst, pts = (size_t)capacity * n * EBU_LOG_FIELDS * sizeof (float);
+    EbuLog lg = {nullptr, nullptr, capacity};
+    cudaError_t e = cudaMalloc ((void**)&lg.pts, pts);
+    if (e == cudaSuccess) e = cudaMalloc ((void**)&lg.written, n * sizeof (unsigned long long));
+    h->log = lg;                                             // log_free releases whatever was allocated
+    if (e == cudaSuccess) e = cudaMalloc ((void**)&h->d_log_rd, n * sizeof (unsigned long long));
+    if (e == cudaSuccess) e = cudaMalloc ((void**)&h->d_log_lost, n * sizeof (unsigned long long));
+    if (e == cudaSuccess) e = cudaMalloc ((void**)&h->d_log_cnt, n * sizeof (uint32_t));
+    if (e == cudaSuccess) e = cudaMalloc ((void**)&h->d_log_out, pts);
+    if (e == cudaSuccess) e = cudaMemsetAsync (h->log.written, 0, n * sizeof (unsigned long long), st);
+    if (e == cudaSuccess) e = cudaMemsetAsync (h->d_log_rd, 0, n * sizeof (unsigned long long), st);
+    if (e != cudaSuccess) {
+        h->log_free ();
+        cudaGetLastError ();                                 // a failed allocation is not sticky: later calls must not see it
+        if (e == cudaErrorMemoryAllocation) return set_err (B200M_E_NOMEM, "loudness log of %u points x %u instances: out of device memory", capacity, h->n_inst);
+        return cuda_fail (e, "b200m_ebu_log_enable", __FILE__, __LINE__);
+    }
+    return 0;
+}
+
+uint32_t b200m_ebu_log_capacity (const b200m_ebu* h)
+{
+    return h ? h->log.cap : 0;
+}
+
+int b200m_ebu_log_drain (b200m_ebu* h, b200m_ebu_point* out, uint32_t* count, uint64_t* lost, void* stream)
+{
+    if (!h || !out || !count || !lost) return set_err (B200M_E_INVAL, "NULL argument");
+    if (!h->log.pts) return set_err (B200M_E_INVAL, "the loudness log is off (b200m_ebu_log_enable)");
+    DeviceGuard g (h->device);
+    cudaStream_t st = h->stream (stream);
+    const size_t n = h->n_inst;
+    ebu_log_drain_kernel<<<(unsigned)((n + 31) / 32), 32 * LOG_DRAIN_ROWS, 0, st>>> ((int)n, h->log, h->d_log_rd, h->d_log_out, h->d_log_cnt, h->d_log_lost);
+    B200M_LAUNCHED (1);
+    B200M_CUDA (cudaGetLastError ());
+    B200M_CUDA (cudaMemcpyAsync (out, h->d_log_out, n * h->log.cap * sizeof (b200m_ebu_point), cudaMemcpyDeviceToHost, st));
+    B200M_CUDA (cudaMemcpyAsync (count, h->d_log_cnt, n * sizeof (uint32_t), cudaMemcpyDeviceToHost, st));
+    B200M_CUDA (cudaMemcpyAsync (lost, h->d_log_lost, n * sizeof (uint64_t), cudaMemcpyDeviceToHost, st));
     B200M_CUDA (cudaStreamSynchronize (st));
     return 0;
 }
@@ -1168,7 +1304,7 @@ int b200m_ebu_histogram (b200m_ebu* h, uint32_t inst, int32_t* hist_M, int32_t* 
 {
     if (!h || !hist_M || !hist_S || inst >= h->n_inst) return set_err (B200M_E_INVAL, "bad argument");
     DeviceGuard g (h->device);
-    cudaStream_t st = h->path.stream (stream);
+    cudaStream_t st = h->stream (stream);
     B200M_CUDA (cudaMemcpyAsync (hist_M, h->d_histM + (size_t)inst * HIST_PITCH, 751 * sizeof (int), cudaMemcpyDeviceToHost, st));
     B200M_CUDA (cudaMemcpyAsync (hist_S, h->d_histS + (size_t)inst * HIST_PITCH, 751 * sizeof (int), cudaMemcpyDeviceToHost, st));
     B200M_CUDA (cudaStreamSynchronize (st));
@@ -1212,7 +1348,7 @@ int b200m_ebu_snapshot (b200m_ebu* h, void* buf, size_t bytes, void* stream)
 {
     if (!h || !buf || bytes < b200m_ebu_snapshot_size (h)) return set_err (B200M_E_INVAL, "bad argument / buffer too small");
     DeviceGuard g (h->device);
-    cudaStream_t st = h->path.stream (stream);
+    cudaStream_t st = h->stream (stream);
     uint8_t* o = (uint8_t*)buf;
     EbuSnapHead hd = {h->weighted ? EBU_SNAP_MAGIC_W : EBU_SNAP_MAGIC, h->n_inst, h->nchan, h->fsamp, h->tmod, {0, 0, 0}};
     memcpy (o, &hd, sizeof (hd)); o += sizeof (hd);
@@ -1237,7 +1373,7 @@ int b200m_ebu_restore (b200m_ebu* h, const void* buf, size_t bytes, void* stream
     if (h->weighted && memcmp ((const uint8_t*)buf + sizeof (hd), h->gw.g, sizeof (h->gw.g)) != 0)
         return set_err (B200M_E_INVAL, "snapshot of a bank with other channel weights");
     DeviceGuard g (h->device);
-    cudaStream_t st = h->path.stream (stream);
+    cudaStream_t st = h->stream (stream);
     const uint8_t* o = (const uint8_t*)buf + ebu_head_bytes (h);
     const size_t n = h->n_inst;
     h->tmod = hd.tmod;
@@ -1267,7 +1403,7 @@ int b200m_ebu_state (b200m_ebu* h, uint32_t inst, float* z, float* power64, floa
 {
     if (!h || !z || !power64 || !frpwr || !c4 || inst >= h->n_inst) return set_err (B200M_E_INVAL, "bad argument");
     DeviceGuard g (h->device);
-    cudaStream_t st = h->path.stream (stream);
+    cudaStream_t st = h->stream (stream);
     const size_t nch = (size_t)h->n_inst * h->nchan;
     for (uint32_t c = 0; c < h->nchan; ++c)
         for (int q = 0; q < 4; ++q)
@@ -1285,7 +1421,7 @@ int b200m_ebu_mix_reduce (b200m_ebu* h, int32_t* d_out, void* stream)
 {
     if (!h || !d_out) return set_err (B200M_E_INVAL, "NULL argument");
     DeviceGuard g (h->device);
-    cudaStream_t st = h->path.stream (stream);
+    cudaStream_t st = h->stream (stream);
     B200M_CUDA (cudaMemsetAsync (d_out, 0, B200M_MIX_WORDS * sizeof (int32_t), st));
     const unsigned slices = (unsigned)std::min<uint32_t> (h->n_inst, 128u);      // ~24 x 128 CTAs: enough loads in flight to stream the histograms
     ebu_mix_reduce_kernel<<<dim3 ((B200M_MIX_WORDS + 63) / 64, slices), 64, 0, st>>> ((int)h->n_inst, h->d_histM, h->d_histS, h->d_cnt, d_out);
@@ -1298,7 +1434,7 @@ int b200m_ebu_mix_finish (b200m_ebu* h, const int32_t* d_mix, float out5[5], voi
 {
     if (!h || !d_mix || !out5) return set_err (B200M_E_INVAL, "NULL argument");
     DeviceGuard g (h->device);
-    cudaStream_t st = h->path.stream (stream);
+    cudaStream_t st = h->stream (stream);
     ebu_mix_finish_kernel<<<1, 32, 0, st>>> (d_mix, h->d_binpow, h->d_out5);
     B200M_LAUNCHED (1);
     B200M_CUDA (cudaMemcpyAsync (out5, h->d_out5, 5 * sizeof (float), cudaMemcpyDeviceToHost, st));
@@ -1309,3 +1445,4 @@ int b200m_ebu_mix_finish (b200m_ebu* h, const int32_t* d_mix, float out5[5], voi
 }  // extern "C"
 
 RaggedLen& ebu_lens (b200m_ebu* h) { return h->rag; }
+void ebu_follow (b200m_ebu* h, const BankPath* owner) { h->owner = owner; }

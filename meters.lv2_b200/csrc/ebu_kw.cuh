@@ -242,3 +242,6 @@ extern "C" int ebu_process_sliced (b200m_ebu* h, const float* d_in, size_t strid
                                    const uint32_t* len = nullptr, const uint32_t* d_len = nullptr);
 // host side, ebu.cu: the upload of a ragged block's per-instance lengths (b200m_ebu_process_ragged_*, and the EBUr128 cycle's)
 b200m::RaggedLen& ebu_lens (b200m_ebu* h);
+// host side, ebu.cu: the bank is driven by an EBUr128 bank whose path is `owner` (b200m_r128_create*): from now on its getters,
+// controls and log calls resolve their stream through that path, so after the EBUr128 bank's host-path calls they run on its own stream
+void ebu_follow (b200m_ebu* h, const b200m::BankPath* owner);

@@ -229,6 +229,7 @@ static int r128_create (b200m_r128** out, int device, uint32_t n_inst, uint32_t 
     if (h->slices > R128_SLICES) h->slices = R128_SLICES;
     int rc = gains ? b200m_ebu_create_weighted (&h->ebu, device, n_inst, nchan, gains, fsamp)
                    : b200m_ebu_create (&h->ebu, device, n_inst, nchan, fsamp);                // ebu->init (nchan, rate), src/ebulv2.cc:190
+    if (!rc) ebu_follow (h->ebu, &h->path);       // b200m_r128_ebu (h)'s getters and log calls are ordered after this bank's calls
     if (!rc) rc = b200m_tpk_create (&h->tpk, device, nchan * n_inst, fsamp, B200M_TPK_TRUEPEAK);   // nchan x TruePeakdsp, :192-196
     if (!rc) {
         DeviceGuard g (device);
