@@ -305,6 +305,27 @@ int b200m_r128_histogram (b200m_r128* h, uint32_t inst, int32_t* hist_M, int32_t
 size_t b200m_r128_snapshot_size (b200m_r128* h);
 int b200m_r128_snapshot (b200m_r128* h, void* buf, size_t bytes, void* stream);
 int b200m_r128_restore (b200m_r128* h, const void* buf, size_t bytes, void* stream);
+/* True-peak curves (an extension, like the loudness log): the loudness log of b200m_r128_ebu (h) with a sixth field per point, the
+ * dBTP of its fragment: coef_to_db (:227-230) of the largest |4x oversampled| output that TruePeakdsp::process_max computes, over
+ * all the instance's channels (zero-weight ones included, as in the tp_max hold) and the input frames of that fragment that ran
+ * with the instance's dBTP on (b200m_r128_set_dbtp_inst; in a ragged block its first len[i] frames).  -inf when that maximum is 0 or
+ * no frame of the fragment ran with dBTP on.  The fragment is the one the loudness fields describe: the frames between two edges of
+ * the instance's 50 ms clock, across blocks.
+ * - The frames of the fragment left open by a control that restarts or clears the instance's clock (NEW, CLEAR, b200m_ebu_reset /
+ *   b200m_ebu_clear of the member) or by a restore do not count: the first point after it covers only the frames metered since.
+ *   RESET and CLEAR_TPMAX leave the fragment alone.
+ * - While the plane is on, the cycle's true-peak maximum runs on the chunk-parallel kernel in either precision mode, never on the
+ *   tensor-core or fused kernels (its tolerance-mode readings are those of a B200M_TPK_TC=0 bank); B200M_TPK_CHUNKED=0 does not apply.
+ *   With the plane off nothing changes. */
+typedef struct b200m_r128_point { float loudness_M, loudness_S, integrated, range_min, range_max, dbtp; } b200m_r128_point;
+/* the loudness log with the dBTP plane, as b200m_ebu_log_enable (b200m_r128_ebu (h), capacity, stream) otherwise: 0 turns both off,
+ * (re)enabling empties the log (the first point's dBTP then covers the frames metered from here on), B200M_E_NOMEM leaves it off.
+ * B200M_E_UNSUPPORTED below 5120 Hz (fragments of < 256 frames).
+ * b200m_ebu_log_enable on the member bank turns the plane off. */
+int b200m_r128_log_enable (b200m_r128* h, uint32_t capacity, void* stream);
+/* b200m_ebu_log_drain of the member bank with the sixth field: out [n_inst][capacity] (b200m_ebu_log_capacity), the same read
+ * cursor, ordering and NaN past count.  B200M_E_INVAL while the plane is off (b200m_ebu_log_drain still drains five fields then). */
+int b200m_r128_log_drain (b200m_r128* h, b200m_r128_point* out, uint32_t* count, uint64_t* lost, void* stream);
 b200m_ebu* b200m_r128_ebu (b200m_r128* h);     /* the underlying banks (histograms, state, coefficients) */
 /* the EBU bank of an EBUr128 bank follows that bank's path: after a b200m_r128_run_host* call its getters, controls and log calls
  * (b200m_ebu_log_enable / _drain) run on the EBUr128 bank's own stream, after a device-path call on the stream they are given */

@@ -35,6 +35,7 @@ EBU_RESULT_DTYPE = np.dtype([(n, "<f4") for n in ("loudness_M", "maxloudn_M", "l
                             [("hist_M_count", "<i4"), ("hist_S_count", "<i4"), ("frag_power", "<f4")])
 # one point of the loudness log (b200m_ebu_point): the values after one completed 50 ms fragment of an instance
 EBU_POINT_DTYPE = np.dtype([(n, "<f4") for n in ("loudness_M", "loudness_S", "integrated", "range_min", "range_max")])
+R128_POINT_DTYPE = np.dtype([(n, "<f4") for n in ("loudness_M", "loudness_S", "integrated", "range_min", "range_max", "dbtp")])
 TPK_RESULT_DTYPE = np.dtype([("tp_m", "<f4"), ("tp_p", "<f4"), ("km_rms", "<f4"), ("km_peak", "<f4")])
 
 _PROTOS = {
@@ -121,6 +122,8 @@ _PROTOS = {
     "b200m_tpk_snapshot_size": (C.c_size_t, [_v]),
     "b200m_tpk_snapshot": (C.c_int, [_v, _v, C.c_size_t, _v]),
     "b200m_tpk_restore": (C.c_int, [_v, _v, C.c_size_t, _v]),
+    "b200m_r128_log_enable": (C.c_int, [_v, C.c_uint32, _v]),
+    "b200m_r128_log_drain": (C.c_int, [_v, _v, _v, _v, _v]),
     "b200m_r128_ebu": (_v, [_v]),
     "b200m_r128_tpk": (_v, [_v]),
     # Stcorr
@@ -1036,19 +1039,32 @@ class EBUr128(_Bank):
         _ck(lib().b200m_r128_histogram(self.h, int(inst), _np_ptr(m), _np_ptr(s), _stream_ptr(stream)))
         return m, s
 
-    def log_enable(self, capacity, stream=None):
-        """the loudness log of the cycle's EBU R128 bank: Ebu_r128_proc.log_enable"""
-        self.ebu.log_enable(capacity, stream)
+    def log_enable(self, capacity, stream=None, dbtp=False):
+        """the loudness log of the cycle's EBU R128 bank: Ebu_r128_proc.log_enable.  dbtp=True adds each point's dBTP, the true peak
+        of its fragment (b200m_r128_log_enable); log_drain then returns R128_POINT_DTYPE"""
+        if dbtp:
+            _ck(lib().b200m_r128_log_enable(self.h, int(capacity), _stream_ptr(stream)))
+        else:
+            self.ebu.log_enable(capacity, stream)
+        self._tplog = bool(dbtp) and int(capacity) > 0
 
     def log_drain(self, stream=None):
-        """Ebu_r128_proc.log_drain of the cycle's EBU R128 bank"""
-        return self.ebu.log_drain(stream)
+        """Ebu_r128_proc.log_drain of the cycle's EBU R128 bank; with the dBTP plane on (log_enable(..., dbtp=True)) the points are
+        R128_POINT_DTYPE (b200m_r128_log_drain)"""
+        if not getattr(self, "_tplog", False):
+            return self.ebu.log_drain(stream)
+        cap = int(lib().b200m_ebu_log_capacity(self.ebu.h))
+        pts = np.empty((self.n_inst, max(cap, 1)), R128_POINT_DTYPE)
+        cnt = np.empty(self.n_inst, np.uint32); lost = np.empty(self.n_inst, np.uint64)
+        _ck(lib().b200m_r128_log_drain(self.h, _np_ptr(pts), _np_ptr(cnt), _np_ptr(lost), _stream_ptr(stream)))
+        return pts, cnt, lost
 
 
 PROGRAMME_FIELDS = ("integrated", "integ_thr", "range_min", "range_max", "maxloudn_M", "maxloudn_S")
 CURVE_FIELDS = (("curve_M", "loudness_M"), ("curve_S", "loudness_S"), ("curve_I", "integrated"), ("curve_range_min", "range_min"),
-                ("curve_range_max", "range_max"))
+                ("curve_range_max", "range_max"), ("curve_TP", "dbtp"))
 CURVE_LOG_POINTS = 1200        # the loudness log's capacity in programme_loudness: 60 s of fragments at 48 kHz
+TPLOG_MIN_FRAGM = 256          # the log's dBTP plane needs fragments of >= 256 frames (b200m_r128_log_enable): fsamp >= 5120 Hz
 
 
 def programme_loudness(x, lengths, fsamp=48000.0, nchan=2, gains=None, block=1024, dbtp=True, precision=PREC_EXACT, device=0,
@@ -1069,8 +1085,10 @@ def programme_loudness(x, lengths, fsamp=48000.0, nchan=2, gains=None, block=102
     curves=True adds each clip's loudness curve, one point per 50 ms fragment (fragm = int(fsamp) // 20 frames), point k ending at
     frame (k + 1) * fragm of the clip: n_points (int64 [N], lengths // fragm) and curve_M, curve_S, curve_I, curve_range_min,
     curve_range_max (float32 [N, max(n_points)], NaN past a clip's n_points), each point what the clip's reading was right after
-    that fragment.  The bank's loudness log holds CURVE_LOG_POINTS points per clip and is drained before it can overflow, so the
-    device memory does not grow with the programme; the other fields are the same as with curves=False."""
+    that fragment, and curve_TP (float32 [N, max(n_points)]): the dBTP of each fragment's true peak over the clip's channels (-inf
+    when dbtp is False; NaN below 5120 Hz, where the log has no dBTP plane).  The bank's loudness log holds CURVE_LOG_POINTS points per clip and is drained before it can overflow, so
+    the device memory does not grow with the programme; the other fields are the same as with curves=False (in tolerance mode tp_max
+    is then always the chunk-parallel FIR's, b200m_r128_log_enable)."""
     ln = np.asarray(lengths, np.int64).ravel()
     n = ln.size
     if n == 0:
@@ -1091,7 +1109,7 @@ def programme_loudness(x, lengths, fsamp=48000.0, nchan=2, gains=None, block=102
             n_points = ln // fragm
             cv = {k: np.full((n, int(n_points.max())), np.nan, np.float32) for k, _ in CURVE_FIELDS}
             pos = np.zeros(n, np.int64)
-            bank.log_enable(CURVE_LOG_POINTS)
+            bank.log_enable(CURVE_LOG_POINTS, dbtp=fragm >= TPLOG_MIN_FRAGM)
             per_block = int(block) // fragm + 1                 # the most fragments one block completes for an instance
             drain_every = CURVE_LOG_POINTS // per_block
 
@@ -1102,7 +1120,8 @@ def programme_loudness(x, lengths, fsamp=48000.0, nchan=2, gains=None, block=102
                     raise B200MError("loudness log overflow: %d points lost" % int(lost.sum()))
                 i, j = np.nonzero(np.arange(pts.shape[1]) < cnt[:, None].astype(np.int64))
                 for k, f in CURVE_FIELDS:
-                    cv[k][i, pos[i] + j] = pts[f][i, j]
+                    if f in pts.dtype.names:
+                        cv[k][i, pos[i] + j] = pts[f][i, j]
                 pos[:] += cnt
         for b, off in enumerate(range(0, total, int(block))):
             nfram = min(int(block), total - off)

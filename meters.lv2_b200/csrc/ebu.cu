@@ -473,12 +473,7 @@ B200M_DEV void hist_calc_range (const int* row, int count, const float* bp, int 
     v1 = __fdiv_rn ((float)(j - 699), 10.0f);
 }
 
-// The loudness log (b200m_ebu_log_enable): one point {M, S, I, range_min, range_max} per completed fragment of an instance, `cap`
-// points per instance.  Field f of point slot s of instance i is pts[(f * cap + s) * n_inst + i] (planes [5][cap][n_inst]: lane =
-// instance stores coalesce, like the power ring); written[i] counts the instance's points, the next goes to slot written[i] % cap.
-// pts == nullptr: the log is off.
-struct EbuLog { float* pts; unsigned long long* written; uint32_t cap; };
-constexpr int EBU_LOG_FIELDS = 5;
+// The loudness log (EbuLog, ebu_kw.cuh): K2a writes a point's five loudness fields, K2b rewrites three of them after it gates.
 
 // K2a: one THREAD per instance, one completed 50 ms fragment (process :217-243 minus the gated statistics).
 // ring layout [64][n_inst] so that lane = instance accesses coalesce; each thread parks its 64-slot ring column
@@ -595,16 +590,18 @@ ebu_gate_kernel (int n_inst, EbuCtl* __restrict__ ctl, b200m_ebu_result* __restr
 }
 
 // Drain of the loudness log: per instance the points written since the last drain, oldest first, at most cap of them, into
-// out[n_inst][cap][5] (NaN past the instance's count), with count[i] and lost[i] (unread points overwritten before this drain);
+// out[n_inst][cap][NF] (NaN past the instance's count), with count[i] and lost[i] (unread points overwritten before this drain);
 // then the read cursor moves to written[i].  A CTA owns 32 instances and walks their points in tiles of 32: lane = instance reads
-// the planes, a shared-memory transpose makes the stores of the [cap][5] rows coalesce.
+// the planes, a shared-memory transpose makes the stores of the [cap][NF] rows coalesce.  NF = 5: the loudness fields; 6: the
+// dBTP plane too.
 constexpr int LOG_DRAIN_ROWS = 8;
 
+template <int NF>
 __global__ void __launch_bounds__ (32 * LOG_DRAIN_ROWS)
 ebu_log_drain_kernel (int n_inst, EbuLog lg, unsigned long long* __restrict__ rd, float* __restrict__ out, uint32_t* __restrict__ count,
                       unsigned long long* __restrict__ lost)
 {
-    __shared__ float tile[32][32 * EBU_LOG_FIELDS + 1];
+    __shared__ float tile[32][32 * NF + 1];
     const int tx = threadIdx.x & 31, ty = threadIdx.x >> 5;
     const int i0 = blockIdx.x * 32, i = i0 + tx;
     const uint32_t cap = lg.cap;
@@ -621,22 +618,22 @@ ebu_log_drain_kernel (int n_inst, EbuLog lg, unsigned long long* __restrict__ rd
     for (uint32_t j0 = 0; j0 < cap; j0 += 32) {
         for (int jl = ty; jl < 32; jl += LOG_DRAIN_ROWS) {
             const uint32_t j = j0 + jl;
-            float v[EBU_LOG_FIELDS];
+            float v[NF];
             if (i < n_inst && j < cnt) {
                 const float* p = lg.pts + (size_t)((start + j) % cap) * n_inst + i;
 #pragma unroll
-                for (int f = 0; f < EBU_LOG_FIELDS; ++f) v[f] = p[f * pl];
+                for (int f = 0; f < NF; ++f) v[f] = p[f * pl];
             } else {
 #pragma unroll
-                for (int f = 0; f < EBU_LOG_FIELDS; ++f) v[f] = __int_as_float (0x7fc00000);
+                for (int f = 0; f < NF; ++f) v[f] = __int_as_float (0x7fc00000);
             }
 #pragma unroll
-            for (int f = 0; f < EBU_LOG_FIELDS; ++f) tile[tx][jl * EBU_LOG_FIELDS + f] = v[f];
+            for (int f = 0; f < NF; ++f) tile[tx][jl * NF + f] = v[f];
         }
         __syncthreads ();
-        const int nq = (int)min (32u, cap - j0) * EBU_LOG_FIELDS;        // the tile's floats of one instance's row, contiguous in out
+        const int nq = (int)min (32u, cap - j0) * NF;        // the tile's floats of one instance's row, contiguous in out
         for (int il = ty; il < 32 && i0 + il < n_inst; il += LOG_DRAIN_ROWS) {
-            float* o = out + ((size_t)(i0 + il) * cap + j0) * EBU_LOG_FIELDS;
+            float* o = out + ((size_t)(i0 + il) * cap + j0) * NF;
             for (int q = tx; q < nq; q += 32) o[q] = tile[il][q];
         }
         __syncthreads ();
@@ -654,9 +651,10 @@ __global__ void ebu_ragged_clock_kernel (int n_inst, const uint32_t* __restrict_
 }
 
 // reset / integration control, one thread per instance.  tph >= 0 (cmd 3 only): the instance's clock restarts at bank time tph --
-// fragment phase and ring write index -- as in reset(); tph = -1 keeps both (b200m_ebu_clear)
+// fragment phase and ring write index -- as in reset(); tph = -1 keeps both (b200m_ebu_clear).  tp_open (the log's dBTP plane is on):
+// cmd 3 also drops the true-peak maximum of the instance's open fragment, whose frames the restarted instance no longer meters.
 __global__ void ebu_ctl_kernel (int n_inst, int inst_sel, int cmd, int nchan, float* zst, float* frpwr, float* ring,
-                                EbuCtl* ctl, b200m_ebu_result* res, int* histM, int* histS, int* cnt, int* fph, int tph)
+                                EbuCtl* ctl, b200m_ebu_result* res, int* histM, int* histS, int* cnt, int* fph, int tph, float* tp_open)
 {
     const int i = blockIdx.x * blockDim.x + threadIdx.x;
     if (i >= n_inst || (inst_sel >= 0 && i != inst_sel)) return;
@@ -678,6 +676,7 @@ __global__ void ebu_ctl_kernel (int n_inst, int inst_sel, int cmd, int nchan, fl
         const size_t nch = (size_t)n_inst * nchan;
         for (int c = 0; c < nchan; ++c) for (int z = 0; z < 4; ++z) zst[z * nch + (size_t)i * nchan + c] = 0.0f;
         if (tph >= 0) { fph[i] = tph; ctl[i].wrind = 0; }
+        if (tp_open) tp_open[i] = 0.0f;
     }
     res[i] = r;
 }
@@ -764,9 +763,13 @@ struct b200m_ebu {
     // cursors, and the drain's device output (points, counts, lost counts)
     EbuLog log = {nullptr, nullptr, 0};
     unsigned long long *d_log_rd = nullptr, *d_log_lost = nullptr; float* d_log_out = nullptr; uint32_t* d_log_cnt = nullptr;
+    // the log's dBTP plane (b200m_r128_log_enable), off while tp.fmax is null
+    EbuTpPlane tp = {};
     void log_free () {
         cudaFree (log.pts); cudaFree (log.written); cudaFree (d_log_rd); cudaFree (d_log_lost); cudaFree (d_log_out); cudaFree (d_log_cnt);
         log = {nullptr, nullptr, 0}; d_log_rd = d_log_lost = nullptr; d_log_out = nullptr; d_log_cnt = nullptr;
+        cudaFree (tp.fmax); cudaFree (tp.fph0); cudaFree (tp.open); cudaFree (tp.filled);
+        tp = {};
     }
     BankPath path;
     // the path of the EBUr128 bank this bank belongs to (ebu_follow), nullptr for a bank of its own: that bank drives this one's
@@ -884,7 +887,7 @@ static int ebu_ctl (b200m_ebu* h, int32_t inst, int cmd, void* stream)
     // after process_host the bank runs on its own stream: a control on any other stream would race with the kernels in flight
     ebu_ctl_kernel<<<(h->n_inst + 127) / 128, 128, 0, h->stream (stream)>>> (
         (int)h->n_inst, inst, cmd, (int)h->nchan, h->d_z, h->d_frpwr, h->d_ring, h->d_ctl, h->d_res, h->d_histM, h->d_histS, h->d_cnt,
-        h->d_fph, cmd == 3 ? h->tmod : -1);
+        h->d_fph, cmd == 3 ? h->tmod : -1, h->tp.open);
     B200M_LAUNCHED (1);
     B200M_CUDA (cudaGetLastError ());
     return 0;
@@ -1062,7 +1065,7 @@ int b200m_ebu_clear (b200m_ebu* h, int32_t inst, void* stream)
     h->phase_ctl (inst, 0); h->phase_ctl (inst, 2);
     ebu_ctl_kernel<<<(h->n_inst + 127) / 128, 128, 0, h->stream (stream)>>> (
         (int)h->n_inst, inst, 3, (int)h->nchan, h->d_z, h->d_frpwr, h->d_ring, h->d_ctl, h->d_res, h->d_histM, h->d_histS, h->d_cnt,
-        h->d_fph, -1);
+        h->d_fph, -1, h->tp.open);
     B200M_LAUNCHED (1);
     B200M_CUDA (cudaGetLastError ());
     return 0;
@@ -1250,32 +1253,7 @@ int b200m_ebu_results (b200m_ebu* h, b200m_ebu_result* out, void* stream)
 
 int b200m_ebu_log_enable (b200m_ebu* h, uint32_t capacity, void* stream)
 {
-    if (!h) return set_err (B200M_E_INVAL, "NULL handle");
-    DeviceGuard g (h->device);
-    cudaStream_t st = h->stream (stream);
-    if (h->log.pts) {                                        // kernels in flight may still write the old log
-        B200M_CUDA (cudaStreamSynchronize (st));
-        h->log_free ();
-    }
-    if (capacity == 0) return 0;
-    const size_t n = h->n_inst, pts = (size_t)capacity * n * EBU_LOG_FIELDS * sizeof (float);
-    EbuLog lg = {nullptr, nullptr, capacity};
-    cudaError_t e = cudaMalloc ((void**)&lg.pts, pts);
-    if (e == cudaSuccess) e = cudaMalloc ((void**)&lg.written, n * sizeof (unsigned long long));
-    h->log = lg;                                             // log_free releases whatever was allocated
-    if (e == cudaSuccess) e = cudaMalloc ((void**)&h->d_log_rd, n * sizeof (unsigned long long));
-    if (e == cudaSuccess) e = cudaMalloc ((void**)&h->d_log_lost, n * sizeof (unsigned long long));
-    if (e == cudaSuccess) e = cudaMalloc ((void**)&h->d_log_cnt, n * sizeof (uint32_t));
-    if (e == cudaSuccess) e = cudaMalloc ((void**)&h->d_log_out, pts);
-    if (e == cudaSuccess) e = cudaMemsetAsync (h->log.written, 0, n * sizeof (unsigned long long), st);
-    if (e == cudaSuccess) e = cudaMemsetAsync (h->d_log_rd, 0, n * sizeof (unsigned long long), st);
-    if (e != cudaSuccess) {
-        h->log_free ();
-        cudaGetLastError ();                                 // a failed allocation is not sticky: later calls must not see it
-        if (e == cudaErrorMemoryAllocation) return set_err (B200M_E_NOMEM, "loudness log of %u points x %u instances: out of device memory", capacity, h->n_inst);
-        return cuda_fail (e, "b200m_ebu_log_enable", __FILE__, __LINE__);
-    }
-    return 0;
+    return ebu_log_enable (h, capacity, false, stream);
 }
 
 uint32_t b200m_ebu_log_capacity (const b200m_ebu* h)
@@ -1285,19 +1263,7 @@ uint32_t b200m_ebu_log_capacity (const b200m_ebu* h)
 
 int b200m_ebu_log_drain (b200m_ebu* h, b200m_ebu_point* out, uint32_t* count, uint64_t* lost, void* stream)
 {
-    if (!h || !out || !count || !lost) return set_err (B200M_E_INVAL, "NULL argument");
-    if (!h->log.pts) return set_err (B200M_E_INVAL, "the loudness log is off (b200m_ebu_log_enable)");
-    DeviceGuard g (h->device);
-    cudaStream_t st = h->stream (stream);
-    const size_t n = h->n_inst;
-    ebu_log_drain_kernel<<<(unsigned)((n + 31) / 32), 32 * LOG_DRAIN_ROWS, 0, st>>> ((int)n, h->log, h->d_log_rd, h->d_log_out, h->d_log_cnt, h->d_log_lost);
-    B200M_LAUNCHED (1);
-    B200M_CUDA (cudaGetLastError ());
-    B200M_CUDA (cudaMemcpyAsync (out, h->d_log_out, n * h->log.cap * sizeof (b200m_ebu_point), cudaMemcpyDeviceToHost, st));
-    B200M_CUDA (cudaMemcpyAsync (count, h->d_log_cnt, n * sizeof (uint32_t), cudaMemcpyDeviceToHost, st));
-    B200M_CUDA (cudaMemcpyAsync (lost, h->d_log_lost, n * sizeof (uint64_t), cudaMemcpyDeviceToHost, st));
-    B200M_CUDA (cudaStreamSynchronize (st));
-    return 0;
+    return ebu_log_drain (h, (float*)out, count, lost, stream, false);
 }
 
 int b200m_ebu_histogram (b200m_ebu* h, uint32_t inst, int32_t* hist_M, int32_t* hist_S, void* stream)
@@ -1388,6 +1354,8 @@ int b200m_ebu_restore (b200m_ebu* h, const void* buf, size_t bytes, void* stream
     o = (const uint8_t*)buf + ((ebu_head_bytes (h) + EBU_SNAP_HOST_PER_INST * n + 15) & ~size_t (15));
     EbuSeg seg[9]; const int k = ebu_segments (h, seg);
     for (int i = 0; i < k; ++i) { B200M_CUDA (cudaMemcpyAsync (seg[i].p, o, seg[i].bytes, cudaMemcpyHostToDevice, st)); o += (seg[i].bytes + 15) & ~size_t (15); }
+    // the log's dBTP plane: the open fragments' true-peak maxima belong to the bank before the restore, the snapshot has none
+    if (h->tp.open) B200M_CUDA (cudaMemsetAsync (h->tp.open, 0, n * sizeof (float), st));
     B200M_CUDA (cudaStreamSynchronize (st));
     return 0;
 }
@@ -1443,6 +1411,78 @@ int b200m_ebu_mix_finish (b200m_ebu* h, const int32_t* d_mix, float out5[5], voi
 }
 
 }  // extern "C"
+
+int ebu_log_enable (b200m_ebu* h, uint32_t capacity, bool dbtp, void* stream)
+{
+    if (!h) return set_err (B200M_E_INVAL, "NULL handle");
+    if (dbtp && capacity && h->fragm < TPLOG_MIN_FRAGM)
+        return set_err (B200M_E_UNSUPPORTED, "the dBTP plane needs fragments of >= %d frames (a sample rate of >= %d Hz)", TPLOG_MIN_FRAGM, 20 * TPLOG_MIN_FRAGM);
+    DeviceGuard g (h->device);
+    cudaStream_t st = h->stream (stream);
+    if (h->log.pts) {                                        // kernels in flight may still write the old log
+        B200M_CUDA (cudaStreamSynchronize (st));
+        h->log_free ();
+    }
+    if (capacity == 0) return 0;
+    const size_t n = h->n_inst, pts = (size_t)capacity * n * (EBU_LOG_FIELDS + (dbtp ? 1 : 0)) * sizeof (float);
+    EbuLog lg = {nullptr, nullptr, capacity};
+    cudaError_t e = cudaMalloc ((void**)&lg.pts, pts);
+    if (e == cudaSuccess) e = cudaMalloc ((void**)&lg.written, n * sizeof (unsigned long long));
+    h->log = lg;                                             // log_free releases whatever was allocated
+    if (e == cudaSuccess) e = cudaMalloc ((void**)&h->d_log_rd, n * sizeof (unsigned long long));
+    if (e == cudaSuccess) e = cudaMalloc ((void**)&h->d_log_lost, n * sizeof (unsigned long long));
+    if (e == cudaSuccess) e = cudaMalloc ((void**)&h->d_log_cnt, n * sizeof (uint32_t));
+    if (e == cudaSuccess) e = cudaMalloc ((void**)&h->d_log_out, pts);
+    if (e == cudaSuccess) e = cudaMemsetAsync (h->log.written, 0, n * sizeof (unsigned long long), st);
+    if (e == cudaSuccess) e = cudaMemsetAsync (h->d_log_rd, 0, n * sizeof (unsigned long long), st);
+    if (dbtp) {
+        EbuTpPlane tp = {};
+        tp.E = (int)(B200M_MAX_BLOCK / (uint32_t)h->fragm) + 2;
+        const size_t fm = (size_t)tp.E * n * h->nchan * sizeof (unsigned);
+        if (e == cudaSuccess) e = cudaMalloc ((void**)&tp.fmax, fm);
+        h->tp = tp;                                          // log_free releases whatever was allocated
+        if (e == cudaSuccess) e = cudaMalloc ((void**)&h->tp.fph0, n * sizeof (int));
+        if (e == cudaSuccess) e = cudaMalloc ((void**)&h->tp.open, n * sizeof (float));
+        if (e == cudaSuccess) e = cudaMalloc ((void**)&h->tp.filled, n * sizeof (unsigned long long));
+        if (e == cudaSuccess) e = cudaMemsetAsync (h->tp.fmax, 0, fm, st);
+        if (e == cudaSuccess) e = cudaMemsetAsync (h->tp.open, 0, n * sizeof (float), st);
+        if (e == cudaSuccess) e = cudaMemsetAsync (h->tp.filled, 0, n * sizeof (unsigned long long), st);
+    }
+    if (e != cudaSuccess) {
+        h->log_free ();
+        cudaGetLastError ();                                 // a failed allocation is not sticky: later calls must not see it
+        if (e == cudaErrorMemoryAllocation) return set_err (B200M_E_NOMEM, "loudness log of %u points x %u instances: out of device memory", capacity, h->n_inst);
+        return cuda_fail (e, "b200m_ebu_log_enable", __FILE__, __LINE__);
+    }
+    return 0;
+}
+
+int ebu_log_drain (b200m_ebu* h, float* out, uint32_t* count, uint64_t* lost, void* stream, bool dbtp)
+{
+    if (!h || !out || !count || !lost) return set_err (B200M_E_INVAL, "NULL argument");
+    if (!h->log.pts) return set_err (B200M_E_INVAL, "the loudness log is off (b200m_ebu_log_enable)");
+    if (dbtp && !h->tp.fmax) return set_err (B200M_E_INVAL, "the loudness log has no dBTP plane (b200m_r128_log_enable)");
+    DeviceGuard g (h->device);
+    cudaStream_t st = h->stream (stream);
+    const size_t n = h->n_inst, nf = EBU_LOG_FIELDS + (dbtp ? 1 : 0);
+    const unsigned grid = (unsigned)((n + 31) / 32);
+    if (dbtp) ebu_log_drain_kernel<EBU_LOG_FIELDS + 1><<<grid, 32 * LOG_DRAIN_ROWS, 0, st>>> ((int)n, h->log, h->d_log_rd, h->d_log_out, h->d_log_cnt, h->d_log_lost);
+    else ebu_log_drain_kernel<EBU_LOG_FIELDS><<<grid, 32 * LOG_DRAIN_ROWS, 0, st>>> ((int)n, h->log, h->d_log_rd, h->d_log_out, h->d_log_cnt, h->d_log_lost);
+    B200M_LAUNCHED (1);
+    B200M_CUDA (cudaGetLastError ());
+    B200M_CUDA (cudaMemcpyAsync (out, h->d_log_out, n * h->log.cap * nf * sizeof (float), cudaMemcpyDeviceToHost, st));
+    B200M_CUDA (cudaMemcpyAsync (count, h->d_log_cnt, n * sizeof (uint32_t), cudaMemcpyDeviceToHost, st));
+    B200M_CUDA (cudaMemcpyAsync (lost, h->d_log_lost, n * sizeof (uint64_t), cudaMemcpyDeviceToHost, st));
+    B200M_CUDA (cudaStreamSynchronize (st));
+    return 0;
+}
+
+bool ebu_tp_view (b200m_ebu* h, EbuTpView* v)
+{
+    if (!h->tp.fmax) return false;
+    *v = {h->log, h->tp, h->d_fph, h->tmod, h->fragm};
+    return true;
+}
 
 RaggedLen& ebu_lens (b200m_ebu* h) { return h->rag; }
 void ebu_follow (b200m_ebu* h, const BankPath* owner) { h->owner = owner; }

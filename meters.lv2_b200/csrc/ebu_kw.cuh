@@ -58,12 +58,44 @@ struct EbuK1Args {
 // r128_hold_kernel folds them.
 struct R128Hold { float* tpmax; float* lin; int nch; };
 
-// coef_to_db (src/ebulv2.cc:227-230) of the larger read() t, then tp_max = max (tp_max, tp)
+// coef_to_db (src/ebulv2.cc:227-230)
+B200M_DEV float r128_db (float t)
+{
+    return (t == 0) ? -INFINITY : __double2float_rn (__dmul_rn (20.0, (double)log10f_glibc (t)));
+}
+
+// coef_to_db of the larger read() t, then tp_max = max (tp_max, tp)
 B200M_DEV void r128_hold (float* tpmax, float t)
 {
-    const float tp = (t == 0) ? -INFINITY : __double2float_rn (__dmul_rn (20.0, (double)log10f_glibc (t)));
+    const float tp = r128_db (t);
     if (tp > *tpmax) *tpmax = tp;
 }
+
+// The loudness log (b200m_ebu_log_enable, ebu.cu): one point {M, S, I, range_min, range_max} per completed fragment of an instance,
+// `cap` points per instance.  Field f of point slot s of instance i is pts[(f * cap + s) * n_inst + i] (planes [5][cap][n_inst], or
+// [6][cap][n_inst] with the dBTP plane: lane = instance stores coalesce, like the power ring); written[i] counts the instance's
+// points, the next goes to slot written[i] % cap.  pts == nullptr: the log is off.
+struct EbuLog { float* pts; unsigned long long* written; uint32_t cap; };
+constexpr int EBU_LOG_FIELDS = 5;
+
+// The log's dBTP plane (b200m_r128_log_enable): field 5 of a point is the dBTP of the true-peak maximum over the instance's
+// channels and the frames of that fragment.  The EBUr128 cycle's true-peak kernel splits each channel's maximum at the instance's
+// fragment edges into fmax, and r128_tplog_fold_kernel (r128.cu) folds those into the points K2a wrote in the block.
+// fmax == nullptr: the plane is off.
+constexpr int TPLOG_MIN_FRAGM = 256;      // a 256-frame true-peak chunk then holds at most one edge of a row: fsamp >= 5120 Hz
+struct EbuTpPlane {
+    unsigned* fmax;                       // [E][n_chan] float bits, atomicMax: interval 0 = the fragment the block found open, interval j
+                                          // starts at the instance's j-th edge in the block; zeroed again by the fold
+    int* fph0;                            // [n_inst] the fragment phases at the block's start, for the true-peak kernel (see r128_run)
+    float* open;                          // [n_inst] the maximum of the instance's open fragment over the blocks before (0: nothing)
+    unsigned long long* filled;           // [n_inst] the points whose field 5 the fold has written (it trails written[] by one block)
+    int E;                                // B200M_MAX_BLOCK / fragm + 2: the most intervals a block can have
+};
+
+// What the true-peak kernel needs to split its maxima (tpk.cu, tpmax_kernel<..., SPLIT = true>): channel c belongs to instance
+// c / R128Hold::nch, whose fragment clock last started at bank time fph[i] (mod fragm); the block starts at bank time tmod.
+// fmax == nullptr: no split.
+struct TpSplit { unsigned* fmax; const int* fph; int tmod, fragm, pitch; };
 
 // ---- K1: K-weighting recurrence + per-chunk power sums ------------------------------------
 // One warp = 32 consecutive mono channels (lane = channel).  Tiles of [32 ch x 64 samples] are
@@ -245,3 +277,11 @@ b200m::RaggedLen& ebu_lens (b200m_ebu* h);
 // host side, ebu.cu: the bank is driven by an EBUr128 bank whose path is `owner` (b200m_r128_create*): from now on its getters,
 // controls and log calls resolve their stream through that path, so after the EBUr128 bank's host-path calls they run on its own stream
 void ebu_follow (b200m_ebu* h, const b200m::BankPath* owner);
+// host side, ebu.cu: the loudness log with (dbtp) or without the dBTP plane, enabled on the bank's path (b200m_ebu_log_enable is
+// dbtp = false; B200M_E_UNSUPPORTED for the plane below TPLOG_MIN_FRAGM frames per fragment), and its drain of 5 or 6 fields per point
+int ebu_log_enable (b200m_ebu* h, uint32_t capacity, bool dbtp, void* stream);
+int ebu_log_drain (b200m_ebu* h, float* out, uint32_t* count, uint64_t* lost, void* stream, bool dbtp);
+// host side, ebu.cu: the EBUr128 cycle's view of the log while its dBTP plane is on (false otherwise): the log, the plane's buffers,
+// the bank's phases on the device and its clock at the start of the next block
+struct EbuTpView { b200m::EbuLog lg; b200m::EbuTpPlane tp; int* fph; int tmod, fragm; };
+bool ebu_tp_view (b200m_ebu* h, EbuTpView* v);

@@ -68,11 +68,42 @@ __global__ void r128_dbtp_fix_kernel (int n_inst, int nh, const uint8_t* __restr
     if (t % nh == 0 && !(rlen && rlen[i] == 0)) tpmax[i] = -INFINITY;
 }
 
+// The log's dBTP plane (EbuTpPlane, ebu_kw.cuh), one thread per instance behind the block's true-peak and fragment kernels.  The
+// points K2a wrote in this block are filled[i] .. written[i] - 1, one per fragment edge of the instance, in order: point k takes the
+// maximum over the instance's channels of interval k (k = 0: with the open fragment's maximum of the blocks before) and holds its
+// coef_to_db; the interval after the last edge stays open.  Every interval read is zeroed for the next block.  on == 0 (no instance
+// has dBTP on) or off[i] (a disabled instance of a mixed bank): the instance's frames ran no true-peak meter and add nothing.
+__global__ void r128_tplog_fold_kernel (int n_inst, int nch, EbuLog lg, EbuTpPlane tp, const uint8_t* __restrict__ off, int on)
+{
+    const int i = blockIdx.x * blockDim.x + threadIdx.x;
+    if (i >= n_inst) return;
+    const unsigned long long w = lg.written[i], f = tp.filled[i];
+    const int n = (int)(w - f);                           // <= E - 1: the edges of one block
+    const size_t pitch = (size_t)n_inst * nch, pl = (size_t)lg.cap * n_inst;
+    const bool use = on && !(off && off[i]);
+    float m = tp.open[i];
+    for (int j = 0; j <= n && j < tp.E; ++j) {
+        float v = 0.0f;
+        for (int c = 0; c < nch; ++c) {
+            unsigned* q = tp.fmax + j * pitch + (size_t)i * nch + c;
+            v = fmaxf (v, __uint_as_float (*q));
+            *q = 0u;
+        }
+        if (use) m = fmaxf (m, v);
+        if (j < n) {
+            lg.pts[EBU_LOG_FIELDS * pl + (size_t)((f + j) % lg.cap) * n_inst + i] = r128_db (m);
+            m = 0.0f;
+        }
+    }
+    tp.open[i] = m;
+    tp.filled[i] = w;
+}
+
 }  // namespace b200m
 
 // sliced process entry point of the true-peak bank and the fused K-weighting + true-peak kernel (tpk.cu); the EBU bank's: ebu_kw.cuh
 int tpk_process_sliced (b200m_tpk* h, const float* d_in, size_t stride, uint32_t nfram, uint32_t tp_mode, cudaStream_t st, int nsl, const uint32_t* bounds, cudaEvent_t* ready,
-                        b200m::R128Hold r128, bool pdl, const void* dr, const uint32_t* rlen);
+                        b200m::R128Hold r128, bool pdl, const void* dr, const uint32_t* rlen, b200m::TpSplit sp);
 bool tpk_r128_fused_ok (const b200m_tpk* h, const float* d_in, size_t stride, uint32_t nfram);
 float* tpk_hist (b200m_tpk* h);
 int tpk_r128_fused (b200m_tpk* h, const b200m::EbuK1Args& a, float* r128_tpmax, cudaStream_t st);
@@ -102,14 +133,14 @@ struct b200m_r128 {
 
 static int env_int (const char* name, int dflt) { const char* v = getenv (name); return v ? atoi (v) : dflt; }
 
-struct R128Step { b200m_r128* h; const float* d_in; size_t stride; uint32_t nfram; cudaStream_t st; const uint32_t* bc; const uint32_t* d_len; };
+struct R128Step { b200m_r128* h; const float* d_in; size_t stride; uint32_t nfram; cudaStream_t st; const uint32_t* bc; const uint32_t* d_len; TpSplit sp; };
 
 // device path: the true-peak kernel goes onto the caller's stream right behind the first K-weighting launch, with
 // programmatic dependent launch, so that the two kernels share the SMs (see r128_run)
 static int r128_tp_behind_k1 (void* p)
 {
     R128Step* a = (R128Step*)p;
-    return tpk_process_sliced (a->h->tpk, a->d_in, a->stride, a->nfram, B200M_TP_MODE_MAX, a->st, 1, a->bc, nullptr, a->h->hold (), true, nullptr, a->d_len);
+    return tpk_process_sliced (a->h->tpk, a->d_in, a->stride, a->nfram, B200M_TP_MODE_MAX, a->st, 1, a->bc, nullptr, a->h->hold (), true, nullptr, a->d_len, a->sp);
 }
 
 // device path, fused: one kernel does K1's work and the true-peak maximum over one shared-memory copy of the block (tpk.cu)
@@ -146,6 +177,12 @@ static int r128_run (b200m_r128* h, const float* d_in, size_t stride, uint32_t n
         if (int rc = ebu_lens (h->ebu).put (len, h->n_inst, st)) return rc;
         d_len = ebu_lens (h->ebu).d;
     }
+    // the log's dBTP plane: the true-peak kernel splits its maxima at the fragment edges of this block (the bank clock before the EBU
+    // bank moves it), r128_tplog_fold_kernel folds them into the points behind it
+    EbuTpView tv;
+    const bool plane = ebu_tp_view (h->ebu, &tv);
+    TpSplit sp = {};
+    if (plane && h->dbtp) sp = {tv.tp.fmax, tv.fph, tv.tmod, tv.fragm, (int)(h->n_inst * h->nchan)};
     const bool mixed = h->n_off && h->n_off < h->n_inst;
     if (mixed) {
         // the first mixed cycle after a change: device mask, then the frozen histories of the disabled instances.  Until now every
@@ -160,18 +197,26 @@ static int r128_run (b200m_r128* h, const float* d_in, size_t stride, uint32_t n
         }
     }
     // weighted banks have no fused form: they keep the two-kernel cycle (K1 + the true-peak kernel behind it), see DESIGN.md §3
-    const bool fused = !ready && !d_len && h->dbtp && !h->weighted && tpk_r128_fused_ok (h->tpk, d_in, stride, nfram) && ebu_single_k1 (h->ebu, nfram);
+    // ... nor does the split of the dBTP plane: it needs the chunk-parallel true-peak kernel (tpk_process_sliced)
+    const bool fused = !ready && !d_len && !plane && h->dbtp && !h->weighted && tpk_r128_fused_ok (h->tpk, d_in, stride, nfram) && ebu_single_k1 (h->ebu, nfram);
     const bool pdl = !fused && h->dbtp && h->concurrent >= 2 && !ready;
     const bool conc = h->dbtp && h->concurrent >= 1 && ready;
-    // the side stream's true-peak kernels read the history that the stash / fix-up kernels on st touch
-    if (conc && (mixed || h->fixed || d_len)) { B200M_CUDA (cudaEventRecord (h->ev_pre, st)); B200M_CUDA (cudaStreamWaitEvent (h->side, h->ev_pre, 0)); }
+    // A ragged block's ebu_ragged_clock_kernel rewrites the phases behind the fragment kernels on st, so a split kernel that does not
+    // run ahead of them on st (the device path's PDL launch does) reads the phases the block began with from a copy
+    if (sp.fmax && d_len && !pdl) {
+        B200M_CUDA (cudaMemcpyAsync (tv.tp.fph0, tv.fph, h->n_inst * sizeof (int), cudaMemcpyDeviceToDevice, st));
+        sp.fph = tv.tp.fph0;
+    }
+    // the side stream's true-peak kernels read the history that the stash / fix-up kernels on st touch, and the split kernel the phases
+    // that controls on st write
+    if (conc && (mixed || h->fixed || d_len || sp.fmax)) { B200M_CUDA (cudaEventRecord (h->ev_pre, st)); B200M_CUDA (cudaStreamWaitEvent (h->side, h->ev_pre, 0)); }
     h->fixed = mixed && h->dbtp;
-    R128Step step = {h, d_in, stride, nfram, st, bc, d_len};
+    R128Step step = {h, d_in, stride, nfram, st, bc, d_len, sp};
     if (int rc = ebu_process_sliced (h->ebu, d_in, stride, nfram, st, nsl, bi, ready, pdl ? r128_tp_behind_k1 : nullptr, &step,
                                      fused ? r128_fused_k1 : nullptr, len, d_len)) return rc;
     if (h->dbtp) {
         if (!pdl && !fused) {
-            if (int rc = tpk_process_sliced (h->tpk, d_in, stride, nfram, B200M_TP_MODE_MAX, conc ? h->side : st, nsl, bc, conc ? ready : nullptr, h->hold (), false, nullptr, d_len)) return rc;
+            if (int rc = tpk_process_sliced (h->tpk, d_in, stride, nfram, B200M_TP_MODE_MAX, conc ? h->side : st, nsl, bc, conc ? ready : nullptr, h->hold (), false, nullptr, d_len, sp)) return rc;
             if (conc) { B200M_CUDA (cudaEventRecord (h->ev_tp, h->side)); B200M_CUDA (cudaStreamWaitEvent (st, h->ev_tp, 0)); }
         }
         if (h->d_tplin && !fused) {                        // behind every slice's true-peak kernel, before the fix-up clears holds
@@ -189,6 +234,10 @@ static int r128_run (b200m_r128* h, const float* d_in, size_t stride, uint32_t n
     } else {
         if (d_len) r128_fill_ran_kernel<<<(h->n_inst + 255) / 256, 256, 0, st>>> ((int)h->n_inst, h->d_tpmax, -INFINITY, d_len);
         else r128_fill_kernel<<<(h->n_inst + 255) / 256, 256, 0, st>>> ((int)h->n_inst, h->d_tpmax, -INFINITY);   // :365-366
+        B200M_LAUNCHED (1);
+    }
+    if (plane) {                                           // behind the true-peak kernels (st waited for the side stream) and K2a
+        r128_tplog_fold_kernel<<<(h->n_inst + 255) / 256, 256, 0, st>>> ((int)h->n_inst, (int)h->nchan, tv.lg, tv.tp, mixed ? h->d_off : nullptr, h->dbtp);
         B200M_LAUNCHED (1);
     }
     B200M_CUDA (cudaGetLastError ());
@@ -465,6 +514,18 @@ int b200m_r128_restore (b200m_r128* h, const void* buf, size_t bytes, void* stre
     h->dbtp = h->n_off < h->n_inst;
     h->off_dirty = true; h->stash_ok = false;
     return 0;
+}
+
+int b200m_r128_log_enable (b200m_r128* h, uint32_t capacity, void* stream)
+{
+    if (!h) return set_err (B200M_E_INVAL, "NULL handle");
+    return ebu_log_enable (h->ebu, capacity, true, stream);
+}
+
+int b200m_r128_log_drain (b200m_r128* h, b200m_r128_point* out, uint32_t* count, uint64_t* lost, void* stream)
+{
+    if (!h) return set_err (B200M_E_INVAL, "NULL handle");
+    return ebu_log_drain (h->ebu, (float*)out, count, lost, stream, true);
 }
 
 b200m_ebu* b200m_r128_ebu (b200m_r128* h) { return h ? h->ebu : nullptr; }

@@ -344,6 +344,20 @@ B200M_DEV void fir16_fma_max (const float (&w)[52], int nvalid, float& va, float
     for (int r = 0; r < 4; ++r)
         if (r < nvalid) { va = max3_abs (va, w[r + 24], R[r]); vb = fmaxf (vb, __fadd_rn (fabsf (P[r]), fabsf (Q[r]))); }
 }
+
+// the same with the 4 positions cut at `ns`: positions r < ns into (va, vb), the others into (va2, vb2) (a fragment edge of the row)
+template <bool IMM>
+B200M_DEV void fir16_fma_max_split (const float (&w)[52], int nvalid, int ns, float& va, float& vb, float& va2, float& vb2)
+{
+    float P[4], Q[4], R[4];
+    fir_pqr<IMM> (w, P, Q, R);
+#pragma unroll
+    for (int r = 0; r < 4; ++r)
+        if (r < nvalid) {
+            const float a = max3_abs (0.0f, w[r + 24], R[r]), b = __fadd_rn (fabsf (P[r]), fabsf (Q[r]));
+            if (r < ns) { va = fmaxf (va, a); vb = fmaxf (vb, b); } else { va2 = fmaxf (va2, a); vb2 = fmaxf (vb2, b); }
+        }
+}
 #endif
 
 template <bool IMM>
@@ -848,16 +862,22 @@ tpk_kernel (const float* __restrict__ in, size_t stride, int c_first, int n_chan
 // whose chunk holds the row's end writes the row's next history from xs (its 48-sample prefix covers lengths < 48; length 0: chunk 0
 // copies the current history, which the host swap would otherwise lose); the epilogue leaves tp_m, tp_res and the hold of a
 // length-0 instance untouched (the plugin did not run).
-template <bool IMM, bool FMA, int HOLD, bool RAG = false>
+// SPLIT: the EBUr128 cycle with the loudness log's dBTP plane on (TpSplit, ebu_kw.cuh).  Besides all of the above, each row's maximum
+// is also cut at its instance's fragment edges: the 4 outputs of input frame s belong to s's fragment, and fragm >= 256 puts at most
+// one edge inside a 256-frame chunk, so a thread keeps one maximum before the edge and one after it.  The two go to the row's
+// intervals ja and ja + 1 of sp.fmax.
+template <bool IMM, bool FMA, int HOLD, bool RAG = false, bool SPLIT = false>
 __global__ void __launch_bounds__ (TPK_THREADS)
 tpmax_kernel (const float* __restrict__ in, size_t stride, int c_first, int n_chan, int nfram, int nchunks, int aligned, int elide0,
-              TpkState st, float* __restrict__ dbg, R128Hold r128, const uint32_t* __restrict__ rlen)
+              TpkState st, float* __restrict__ dbg, R128Hold r128, const uint32_t* __restrict__ rlen, TpSplit sp)
 {
     constexpr int CH = 8, TC = 256;
     constexpr int XP = 48 + TC + 4;
     constexpr int GPC = TC / 4, LPR = TPK_THREADS / CH;
     __shared__ __align__ (16) float xs[CH][XP];
     __shared__ float s_rowmax[CH];
+    __shared__ float s_rowa[SPLIT ? CH : 1], s_rowb[SPLIT ? CH : 1];     // SPLIT: the row's maxima before and after its edge
+    __shared__ int s_ja[SPLIT ? CH : 1];
     const int tid = threadIdx.x, lane = tid & 31;
     const int grp = blockIdx.x / nchunks, chunk = blockIdx.x - grp * nchunks;
     const int c0 = c_first + grp * CH;
@@ -904,6 +924,16 @@ tpmax_kernel (const float* __restrict__ in, size_t stride, int c_first, int n_ch
     // positions of this thread's row that count in this chunk
     const int rl = RAG ? max (0, min (len, (int)rlen[(unsigned)min (c0 + r, n_chan - 1) / (unsigned)r128.nch] - s0)) : len;
     float vmax = 0.0f, vmax2 = 0.0f;                        // vmax2: max (|P| + |Q|) = 2 max (|ph1|, |ph3|), tolerance mode
+    // SPLIT: positions >= eb of the chunk lie after the row's next fragment edge (interval ja + 1) and go to vb / vb2
+    int eb = 0x7fffffff, ja = 0;
+    float vb = 0.0f, vb2 = 0.0f;
+    if constexpr (SPLIT) {
+        const int inst = (int)((unsigned)min (c0 + r, n_chan - 1) / (unsigned)r128.nch);
+        int el = (sp.tmod - sp.fph[inst]) % sp.fragm; if (el < 0) el += sp.fragm;
+        const int e0 = sp.fragm - el;                       // the instance's first edge in the block, 1 .. fragm
+        ja = s0 >= e0 ? 1 + (s0 - e0) / sp.fragm : 0;      // edges at or before frame s0
+        eb = e0 + ja * sp.fragm - s0;
+    }
     {
         float M = 0.0f;
         if (elide0) M = row_absmax<LPR, 12 + GPC> (reinterpret_cast<const float4*> (&xs[r][0]), lane);
@@ -930,7 +960,10 @@ tpmax_kernel (const float* __restrict__ in, size_t stride, int c_first, int n_ch
 #pragma unroll
                 for (int i = 0; i < 13; ++i) { const float4 v = xr[i]; w[4 * i] = v.x; w[4 * i + 1] = v.y; w[4 * i + 2] = v.z; w[4 * i + 3] = v.w; }
 #if B200M_TPK_SYM
-                if (FMA && !dbg) { fir16_fma_max<IMM> (w, min (4, rl - 4 * q), vmax, vmax2); continue; }      // maxima only (dbg: warp-uniform)
+                if constexpr (SPLIT) {
+                    if (FMA && !dbg) { fir16_fma_max_split<IMM> (w, min (4, rl - 4 * q), eb - 4 * q, vmax, vmax2, vb, vb2); continue; }
+                }
+                else if (FMA && !dbg) { fir16_fma_max<IMM> (w, min (4, rl - 4 * q), vmax, vmax2); continue; }      // maxima only (dbg: warp-uniform)
 #endif
                 float o[16];
                 if (FMA) fir16_fma<IMM> (w, o); else fir16<IMM> (w, &xs[r][4 * q], o, full0);
@@ -942,14 +975,27 @@ tpmax_kernel (const float* __restrict__ in, size_t stride, int c_first, int n_ch
                 // positions beyond len inside the last group come from zero-filled input: exclude them
 #pragma unroll
                 for (int i = 0; i < 4; ++i)
-                    if (4 * q + i < rl)
-                        vmax = fmaxf (fmaxf (vmax, fmaxf (fabsf (o[4 * i]), fabsf (o[4 * i + 1]))), fmaxf (fabsf (o[4 * i + 2]), fabsf (o[4 * i + 3])));
+                    if (4 * q + i < rl) {
+                        if constexpr (SPLIT) {
+                            const float m = fmaxf (fmaxf (fabsf (o[4 * i]), fabsf (o[4 * i + 1])), fmaxf (fabsf (o[4 * i + 2]), fabsf (o[4 * i + 3])));
+                            if (4 * q + i < eb) vmax = fmaxf (vmax, m); else vb = fmaxf (vb, m);
+                        }
+                        else vmax = fmaxf (fmaxf (vmax, fmaxf (fabsf (o[4 * i]), fabsf (o[4 * i + 1]))), fmaxf (fabsf (o[4 * i + 2]), fabsf (o[4 * i + 3])));
+                    }
             }
         }
     }
     vmax = fmaxf (vmax, __fmul_rn (0.5f, vmax2));
 #pragma unroll
     for (int o = LPR / 2; o; o >>= 1) vmax = fmaxf (vmax, __shfl_xor_sync (0xffffffffu, vmax, o));
+    if constexpr (SPLIT) {
+        // the maximum is exact and order-free: s_rowmax is the value the plain kernel finds
+        vb = fmaxf (vb, __fmul_rn (0.5f, vb2));
+#pragma unroll
+        for (int o = LPR / 2; o; o >>= 1) vb = fmaxf (vb, __shfl_xor_sync (0xffffffffu, vb, o));
+        if (ql == 0) { s_rowa[r] = vmax; s_rowb[r] = vb; s_ja[r] = ja; }
+        vmax = fmaxf (vmax, vb);
+    }
     if (ql == 0) s_rowmax[r] = vmax;
 
     // history of the next block = the 48 samples that end this one (the last chunk holds them: prefix + chunk >= 48 samples)
@@ -973,6 +1019,10 @@ tpmax_kernel (const float* __restrict__ in, size_t stride, int c_first, int n_ch
     bool own = lane < CH && cc < n_chan;
     if constexpr (RAG) own = own && rlen[(unsigned)cc / (unsigned)r128.nch] != 0;
     if (own && s_rowmax[lane] > 0.0f) atomicMax (st.blk_max + cc, __float_as_uint (s_rowmax[lane]));
+    if constexpr (SPLIT) {
+        if (own && s_rowa[lane] > 0.0f) atomicMax (sp.fmax + (size_t)s_ja[lane] * sp.pitch + cc, __float_as_uint (s_rowa[lane]));
+        if (own && s_rowb[lane] > 0.0f) atomicMax (sp.fmax + (size_t)(s_ja[lane] + 1) * sp.pitch + cc, __float_as_uint (s_rowb[lane]));
+    }
     __threadfence ();                                       // the maxima are visible before this CTA's arrival is
     unsigned prev = 0;
     if (lane == 0) prev = atomicAdd (st.grp_cnt + c0, 1u);
@@ -2163,10 +2213,16 @@ int tpk_reset_inst (b200m_tpk* h, const uint32_t* d_inst, uint32_t n_sel, uint32
 }
 
 // the instantiations of the EBUr128 epilogue's HOLD (r128_group_hold)
-template <bool IMM, bool FMA, bool RAG = false> static decltype (&tpmax_kernel<IMM, FMA, 2, RAG>) tpmax_kernel_for (int hold)
+template <bool IMM, bool FMA, bool RAG = false, bool SPLIT = false> static decltype (&tpmax_kernel<IMM, FMA, 2, RAG, SPLIT>) tpmax_kernel_for (int hold)
 {
-    return hold == 0 ? tpmax_kernel<IMM, FMA, 0, RAG> : hold == 1 ? tpmax_kernel<IMM, FMA, 1, RAG> : hold == 4 ? tpmax_kernel<IMM, FMA, 4, RAG>
-                                                                                                       : tpmax_kernel<IMM, FMA, 2, RAG>;
+    return hold == 0 ? tpmax_kernel<IMM, FMA, 0, RAG, SPLIT> : hold == 1 ? tpmax_kernel<IMM, FMA, 1, RAG, SPLIT>
+         : hold == 4 ? tpmax_kernel<IMM, FMA, 4, RAG, SPLIT> : tpmax_kernel<IMM, FMA, 2, RAG, SPLIT>;
+}
+// ... by precision mode: exact with the coefficient table or the immediates, FMA (immediates only)
+template <bool RAG, bool SPLIT> static decltype (&tpmax_kernel<true, true, 2, RAG, SPLIT>) tpmax_kernel_mode (const b200m_tpk* h, int hold)
+{
+    return h->imm && h->fma ? tpmax_kernel_for<true, true, RAG, SPLIT> (hold) : h->imm ? tpmax_kernel_for<true, false, RAG, SPLIT> (hold)
+                                                                                          : tpmax_kernel_for<false, false, RAG, SPLIT> (hold);
 }
 static decltype (&tpmax_tc_kernel<2>) tpmax_tc_kernel_for (int hold)
 {
@@ -2179,8 +2235,12 @@ static const int R128_HOLDS[4] = {0, 1, 2, 4};
 // rlen (device, one length per EBUr128 instance, r128.nch channels each): a ragged block of the EBUr128 cycle.  It always runs
 // tpmax_kernel, exact or FMA: the tensor-core and fused kernels walk whole 8-channel groups through every chunk of the block with
 // no per-row end, so only the chunk-parallel kernel has the per-row mask and the per-row history hand-over.
+// sp.fmax (the EBUr128 cycle with the loudness log's dBTP plane on): the true-peak maximum is also split at fragment edges, which
+// only tpmax_kernel<..., SPLIT> does; like a ragged block it therefore always runs that kernel, exact or FMA, whatever the tensor-core
+// path or B200M_TPK_CHUNKED would select.
 int tpk_process_sliced (b200m_tpk* h, const float* d_in, size_t stride, uint32_t nfram, uint32_t tp_mode, cudaStream_t st,
-                        int nsl, const uint32_t* bounds, cudaEvent_t* ready, R128Hold r128, bool pdl, const void* dr_v, const uint32_t* rlen)
+                        int nsl, const uint32_t* bounds, cudaEvent_t* ready, R128Hold r128, bool pdl, const void* dr_v, const uint32_t* rlen,
+                        TpSplit sp)
 {
     const TpkDr* dr = (const TpkDr*)dr_v;
     const bool tp = h->flags & B200M_TPK_TRUEPEAK, km = h->flags & B200M_TPK_KMETER;
@@ -2206,13 +2266,13 @@ int tpk_process_sliced (b200m_tpk* h, const float* d_in, size_t stride, uint32_t
             if (h->imm && h->fma) B200M_CUDA (cudaLaunchKernelEx (&cfg, tpk_kernel<CH, TC, TP, MX, KM, true, DRM, true>, d_in, stride, cf, ce, (int)nfram, aligned, h->elide0, prm, h->st, h->d_dbg, r128, drp, TpkRag {})); \
             else if (h->imm) B200M_CUDA (cudaLaunchKernelEx (&cfg, tpk_kernel<CH, TC, TP, MX, KM, true, DRM>, d_in, stride, cf, ce, (int)nfram, aligned, h->elide0, prm, h->st, h->d_dbg, r128, drp, TpkRag {})); \
             else B200M_CUDA (cudaLaunchKernelEx (&cfg, tpk_kernel<CH, TC, TP, MX, KM, false, DRM>, d_in, stride, cf, ce, (int)nfram, aligned, h->elide0, prm, h->st, h->d_dbg, r128, drp, TpkRag {})); } while (0)
-        if (rlen) {
+        if (rlen || sp.fmax) {
             const int nchunks = ((int)nfram + 255) / 256;
             cfg.gridDim = dim3 ((unsigned)(((ce - cf + 7) / 8) * nchunks));
             const int hold = r128_hold_of (r128);
-            const auto k = h->imm && h->fma ? tpmax_kernel_for<true, true, true> (hold) : h->imm ? tpmax_kernel_for<true, false, true> (hold)
-                                                                                                 : tpmax_kernel_for<false, false, true> (hold);
-            B200M_CUDA (cudaLaunchKernelEx (&cfg, k, d_in, stride, cf, ce, (int)nfram, nchunks, aligned, h->elide0, h->st, h->d_dbg, r128, rlen));
+            const auto k = rlen ? (sp.fmax ? tpmax_kernel_mode<true, true> (h, hold) : tpmax_kernel_mode<true, false> (h, hold))
+                                : tpmax_kernel_mode<false, true> (h, hold);
+            B200M_CUDA (cudaLaunchKernelEx (&cfg, k, d_in, stride, cf, ce, (int)nfram, nchunks, aligned, h->elide0, h->st, h->d_dbg, r128, rlen, sp));
             swap_hist = true;
         }
         else if (tp && tp_mode == B200M_TP_MODE_MAX && !km && h->chunked && h->tc && h->fma && h->imm && h->d_btc && aligned && nfram % 4 == 0 && !h->d_dbg
@@ -2230,7 +2290,7 @@ int tpk_process_sliced (b200m_tpk* h, const float* d_in, size_t stride, uint32_t
             cfg.gridDim = dim3 ((unsigned)(((ce - cf + 7) / 8) * nchunks));
             const int hold = r128_hold_of (r128);
             const auto k = h->imm && h->fma ? tpmax_kernel_for<true, true> (hold) : h->imm ? tpmax_kernel_for<true, false> (hold) : tpmax_kernel_for<false, false> (hold);
-            B200M_CUDA (cudaLaunchKernelEx (&cfg, k, d_in, stride, cf, ce, (int)nfram, nchunks, aligned, h->elide0, h->st, h->d_dbg, r128, (const uint32_t*)nullptr));
+            B200M_CUDA (cudaLaunchKernelEx (&cfg, k, d_in, stride, cf, ce, (int)nfram, nchunks, aligned, h->elide0, h->st, h->d_dbg, r128, (const uint32_t*)nullptr, TpSplit {}));
             swap_hist = true;
         }
         else if (tp && tp_mode == B200M_TP_MODE_MAX) { if (km) TPK_GO (8, 256, true, true, true, false); else TPK_GO (8, 256, true, true, false, false); }
@@ -2289,7 +2349,7 @@ int tpk_process_sliced (b200m_tpk* h, const float* d_in, size_t stride, uint32_t
 static int tpk_process (b200m_tpk* h, const float* d_in, size_t stride, uint32_t nfram, uint32_t tp_mode, cudaStream_t st)
 {
     const uint32_t bounds[2] = {0, h->n_chan};
-    return tpk_process_sliced (h, d_in, stride, nfram, tp_mode, st, 1, bounds, nullptr, R128Hold {}, false, h->dr_on ? &h->dr : nullptr, nullptr);
+    return tpk_process_sliced (h, d_in, stride, nfram, tp_mode, st, 1, bounds, nullptr, R128Hold {}, false, h->dr_on ? &h->dr : nullptr, nullptr, TpSplit {});
 }
 
 namespace b200m {
@@ -2434,7 +2494,10 @@ int b200m_tpk_create (b200m_tpk** out, int device, uint32_t n_chan, float fsamp,
     if (e == cudaSuccess) e = cudaFuncSetAttribute (tpdec_kernel<false, false>, cudaFuncAttributePreferredSharedMemoryCarveout, cudaSharedmemCarveoutMaxShared);
     for (const int hold : R128_HOLDS)
         for (const auto k : {tpmax_kernel_for<true, true> (hold), tpmax_kernel_for<true, false> (hold), tpmax_kernel_for<false, false> (hold),
-                             tpmax_kernel_for<true, true, true> (hold), tpmax_kernel_for<true, false, true> (hold), tpmax_kernel_for<false, false, true> (hold)})
+                             tpmax_kernel_for<true, true, true> (hold), tpmax_kernel_for<true, false, true> (hold), tpmax_kernel_for<false, false, true> (hold),
+                             tpmax_kernel_for<true, true, false, true> (hold), tpmax_kernel_for<true, false, false, true> (hold),
+                             tpmax_kernel_for<false, false, false, true> (hold), tpmax_kernel_for<true, true, true, true> (hold),
+                             tpmax_kernel_for<true, false, true, true> (hold), tpmax_kernel_for<false, false, true, true> (hold)})
             if (e == cudaSuccess) e = cudaFuncSetAttribute (k, cudaFuncAttributePreferredSharedMemoryCarveout, cudaSharedmemCarveoutMaxShared);
     auto A = [&] (void** p, size_t bytes) { if (e == cudaSuccess) { e = cudaMalloc (p, bytes); if (e == cudaSuccess) e = cudaMemset (*p, 0, bytes); } };
     const size_t n = n_chan;
