@@ -6,10 +6,26 @@
 #include <string.h>
 #include <atomic>
 #include <new>
+#include <type_traits>
 
 #include "../../include/b200meters.h"
 
 namespace b200m {
+
+// Run-time choices handed to a template as compile-time ones, for the host code that picks a kernel instantiation.
+// with_bools (f, b...) calls f (std::bool_constant<b> {}...); f is instantiated for every combination.
+template <class F> auto with_bools (F f) { return f (); }
+template <class F, class... B> auto with_bools (F f, bool b, B... bs)
+{
+    auto g = [&] (auto c) { return with_bools ([&] (auto... cs) { return f (c, cs...); }, bs...); };
+    return b ? g (std::true_type {}) : g (std::false_type {});
+}
+// with_int<V...> (v, f) calls f (std::integral_constant<int, v> {}) if v is one of V..., else with the last of them
+template <int V, int... Vs, class F> auto with_int (int v, F f)
+{
+    if constexpr (sizeof... (Vs) == 0) return f (std::integral_constant<int, V> {});
+    else return v == V ? f (std::integral_constant<int, V> {}) : with_int<Vs...> (v, f);
+}
 
 // ---------------------------------------------------------------- host-side plumbing
 extern thread_local char g_err[512];

@@ -926,6 +926,27 @@ int ebu_check_gains (uint32_t nchan, const float* gains)
 }
 
 // gains == nullptr: the default weights of a 1..5-channel bank (the compile-time K1 instantiations); otherwise a weighted bank
+// K1 selectors: the launch in ebu_process_sliced and ebu_create's attributes both go through them.  With several fragment phases
+// or a ragged block (PHASES, RAG) every lane cuts at its own instance's fragment edges; a ragged block always has phases.
+// ebu_kweight_frag of an unweighted bank (1..5 channels per instance)
+static auto ebu_k1_for (int nchan, bool al, bool phases, bool rag)
+{
+    return with_int<1, 2, 3, 4, 5> (nchan, [&] (auto NC) {
+        return with_bools ([&] (auto AL, auto PH, auto RG) { return ebu_kweight_frag<NC, AL, PH || RG, RG>; }, al, phases, rag);
+    });
+}
+// ebu_kweight_frag_w of a weighted bank (the run-time channel count)
+static auto ebu_k1w_for (bool al, bool phases, bool rag)
+{
+    return with_bools ([] (auto AL, auto PH, auto RG) { return ebu_kweight_frag_w<AL, PH || RG, RG>; }, al, phases, rag);
+}
+// the opt-in variants of 1..2 channels per instance, one phase class: TMA staging and split K-weighting roles
+static auto ebu_k1t_for (int nchan) { return with_int<1, 2> (nchan, [] (auto NC) { return ebu_kweight_tma<NC>; }); }
+static auto ebu_k1s_for (int nchan, bool al)
+{
+    return with_int<1, 2> (nchan, [&] (auto NC) { return with_bools ([&] (auto AL) { return ebu_kweight_split<NC, AL>; }, al); });
+}
+
 static int ebu_create (b200m_ebu** out, int device, uint32_t n_inst, uint32_t nchan, float fsamp, const float* gains)
 {
     if (n_inst == 0 || !(fsamp >= 1000.0f)) return set_err (B200M_E_INVAL, "bad n_inst/fsamp");
@@ -962,33 +983,23 @@ static int ebu_create (b200m_ebu** out, int device, uint32_t n_inst, uint32_t nc
     // K1 carries 102 KB of dynamic shared memory per CTA
     // ... and asks for the largest shared-memory carveout: with the default the driver configures the SM for just what this kernel
     // needs (132 KB), which leaves room for ONE CTA of the true-peak kernel that is meant to share the SM with it (r128.cu)
-#define EBU_ATTR1(NC, AL, PH) if (e == cudaSuccess) e = cudaFuncSetAttribute (ebu_kweight_frag<NC, AL, PH>, cudaFuncAttributeMaxDynamicSharedMemorySize, EBU_SMEM_BYTES); \
-    if (e == cudaSuccess) e = cudaFuncSetAttribute (ebu_kweight_frag<NC, AL, PH>, cudaFuncAttributePreferredSharedMemoryCarveout, cudaSharedmemCarveoutMaxShared)
-#define EBU_ATTR2(NC, AL) if (e == cudaSuccess) e = cudaFuncSetAttribute (ebu_kweight_frag<NC, AL, true, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, EBU_SMEM_BYTES); \
-    if (e == cudaSuccess) e = cudaFuncSetAttribute (ebu_kweight_frag<NC, AL, true, true>, cudaFuncAttributePreferredSharedMemoryCarveout, cudaSharedmemCarveoutMaxShared)
-#define EBU_ATTR(NC, AL) EBU_ATTR1 (NC, AL, false); EBU_ATTR1 (NC, AL, true); EBU_ATTR2 (NC, AL)
-    EBU_ATTR (1, true); EBU_ATTR (1, false); EBU_ATTR (2, true); EBU_ATTR (2, false);
-    EBU_ATTR (3, true); EBU_ATTR (3, false); EBU_ATTR (4, true); EBU_ATTR (4, false); EBU_ATTR (5, true); EBU_ATTR (5, false);
-#undef EBU_ATTR
-#undef EBU_ATTR1
-#undef EBU_ATTR2
-    if (gains)
-        for (const auto k : {ebu_kweight_frag_w<true, false>, ebu_kweight_frag_w<true, true>, ebu_kweight_frag_w<false, false>, ebu_kweight_frag_w<false, true>,
-                             ebu_kweight_frag_w<true, true, true>, ebu_kweight_frag_w<false, true, true>}) {
-            if (e == cudaSuccess) e = cudaFuncSetAttribute (k, cudaFuncAttributeMaxDynamicSharedMemorySize, EBU_SMEM_BYTES);
-            if (e == cudaSuccess) e = cudaFuncSetAttribute (k, cudaFuncAttributePreferredSharedMemoryCarveout, cudaSharedmemCarveoutMaxShared);
-        }
-    if (e == cudaSuccess) e = cudaFuncSetAttribute (ebu_kweight_tma<1>, cudaFuncAttributeMaxDynamicSharedMemorySize, EBU_TMA_SMEM);
-    if (e == cudaSuccess) e = cudaFuncSetAttribute (ebu_kweight_tma<2>, cudaFuncAttributeMaxDynamicSharedMemorySize, EBU_TMA_SMEM);
-    if (e == cudaSuccess) e = cudaFuncSetAttribute (ebu_kweight_tma<1>, cudaFuncAttributePreferredSharedMemoryCarveout, cudaSharedmemCarveoutMaxShared);
-    if (e == cudaSuccess) e = cudaFuncSetAttribute (ebu_kweight_tma<2>, cudaFuncAttributePreferredSharedMemoryCarveout, cudaSharedmemCarveoutMaxShared);
+    auto attrs = [&] (auto k, int smem) {
+        if (e == cudaSuccess) e = cudaFuncSetAttribute (k, cudaFuncAttributeMaxDynamicSharedMemorySize, smem);
+        if (e == cudaSuccess) e = cudaFuncSetAttribute (k, cudaFuncAttributePreferredSharedMemoryCarveout, cudaSharedmemCarveoutMaxShared);
+    };
+    for (const bool al : {false, true})
+        for (const bool ph : {false, true})
+            for (const bool rag : {false, true}) {
+                for (int nc = 1; nc <= 5; ++nc) attrs (ebu_k1_for (nc, al, ph, rag), EBU_SMEM_BYTES);
+                if (gains) attrs (ebu_k1w_for (al, ph, rag), EBU_SMEM_BYTES);
+            }
     // TMA staging is bit-identical and removes ~120 address instructions per tile, but is no faster standalone and slower inside the
     // EBUr128 cycle (the mbarrier try_wait spin takes issue slots from the co-running true-peak kernel, a scoreboard wait does not):
     // opt-in with B200M_EBU_TMA=1
-#define EBU_SATTR(NC, AL) if (e == cudaSuccess) e = cudaFuncSetAttribute (ebu_kweight_split<NC, AL>, cudaFuncAttributeMaxDynamicSharedMemorySize, EBU_SPLIT_SMEM); \
-    if (e == cudaSuccess) e = cudaFuncSetAttribute (ebu_kweight_split<NC, AL>, cudaFuncAttributePreferredSharedMemoryCarveout, cudaSharedmemCarveoutMaxShared)
-    EBU_SATTR (1, true); EBU_SATTR (1, false); EBU_SATTR (2, true); EBU_SATTR (2, false);
-#undef EBU_SATTR
+    for (int nc = 1; nc <= 2; ++nc) {
+        attrs (ebu_k1t_for (nc), EBU_TMA_SMEM);
+        for (const bool al : {false, true}) attrs (ebu_k1s_for (nc, al), EBU_SPLIT_SMEM);
+    }
     if (const char* v = getenv ("B200M_EBU_SPLIT")) h->split = atoi (v) != 0;
     h->use_tma = false;
     if (const char* v = getenv ("B200M_EBU_TMA")) h->use_tma = atoi (v) != 0 && tma_encoder () != nullptr;
@@ -1144,36 +1155,16 @@ int ebu_process_sliced (b200m_ebu* h, const float* d_in, size_t stride, uint32_t
             const int cpw = (32 / (int)h->nchan) * (int)h->nchan;          // a warp takes whole instances only
             const int nwarps = (ke - kf + cpw - 1) / cpw;
             dim3 grid ((nwarps + EBU_WARPS - 1) / EBU_WARPS), blk (EBU_WARPS * 32);
-#define EBU_K1P(NC, AL, PH, RG) ebu_kweight_frag<NC, AL, PH, RG><<<grid, blk, EBU_SMEM_BYTES, st>>> (src, stride, nch, kf, ke, (int)pos, h->cf, ck, (float)h->fragm, h->d_z, h->d_frpwr, h->d_fragpw, (int)h->n_inst, (after_k1 && done == 0) ? 1 : 0, d_len)
-#define EBU_K1(NC, AL) do { if (d_len) EBU_K1P (NC, AL, true, true); else if (multi) EBU_K1P (NC, AL, true, false); else EBU_K1P (NC, AL, false, false); } while (0)
-#define EBU_K1T(NC) ebu_kweight_tma<NC><<<grid, blk, EBU_TMA_SMEM, st>>> (tmap, nch, kf, ke, (int)pos, h->cf, ck, (float)h->fragm, h->d_z, h->d_frpwr, h->d_fragpw, (int)h->n_inst, (after_k1 && done == 0) ? 1 : 0)
-            if (h->weighted) {                                   // weighted banks: the run-time channel count, lanes grouped per instance
-                const int pt = (after_k1 && done == 0) ? 1 : 0;
-#define EBU_K1W(AL, PH, RG) ebu_kweight_frag_w<AL, PH, RG><<<grid, blk, EBU_SMEM_BYTES, st>>> (src, stride, nch, kf, ke, (int)pos, h->cf, ck, (float)h->fragm, h->d_z, h->d_frpwr, h->d_fragpw, (int)h->n_inst, pt, h->gw, d_len)
-                if (al) { if (d_len) EBU_K1W (true, true, true); else if (multi) EBU_K1W (true, true, false); else EBU_K1W (true, false, false); }
-                else    { if (d_len) EBU_K1W (false, true, true); else if (multi) EBU_K1W (false, true, false); else EBU_K1W (false, false, false); }
-#undef EBU_K1W
-            }
-            else if (h->nchan > 2) {                             // surround banks (3..5 channels): the one-warp kernel, lanes grouped per instance
-                switch (h->nchan * 2 + (al ? 1 : 0)) {
-                case 7: EBU_K1 (3, true); break; case 6: EBU_K1 (3, false); break;
-                case 9: EBU_K1 (4, true); break; case 8: EBU_K1 (4, false); break;
-                case 11: EBU_K1 (5, true); break; default: EBU_K1 (5, false); break;
-                }
-            }
-            else if (h->split && !tma && !multi) {           // the opt-in variants know the chunk list only
+            const int pt = (after_k1 && done == 0) ? 1 : 0;
+            if (h->weighted)                                     // weighted banks: the run-time channel count, lanes grouped per instance
+                ebu_k1w_for (al, multi, d_len)<<<grid, blk, EBU_SMEM_BYTES, st>>> (src, stride, nch, kf, ke, (int)pos, h->cf, ck, (float)h->fragm, h->d_z, h->d_frpwr, h->d_fragpw, (int)h->n_inst, pt, h->gw, d_len);
+            else if (h->nchan <= 2 && h->split && !tma && !multi) {       // the opt-in variants know the chunk list only
                 dim3 sgrid ((nwarps + EBU_SPLIT_PAIRS - 1) / EBU_SPLIT_PAIRS), sblk (2 * EBU_SPLIT_PAIRS * 32);
-#define EBU_K1S(NC, AL) ebu_kweight_split<NC, AL><<<sgrid, sblk, EBU_SPLIT_SMEM, st>>> (src, stride, nch, kf, ke, (int)pos, h->cf, ck, (float)h->fragm, h->d_z, h->d_frpwr, h->d_fragpw, (int)h->n_inst, (after_k1 && done == 0) ? 1 : 0)
-                if (h->nchan == 1) { if (al) EBU_K1S (1, true); else EBU_K1S (1, false); }
-                else               { if (al) EBU_K1S (2, true); else EBU_K1S (2, false); }
-#undef EBU_K1S
+                ebu_k1s_for (h->nchan, al)<<<sgrid, sblk, EBU_SPLIT_SMEM, st>>> (src, stride, nch, kf, ke, (int)pos, h->cf, ck, (float)h->fragm, h->d_z, h->d_frpwr, h->d_fragpw, (int)h->n_inst, pt);
             }
-            else if (tma) { if (h->nchan == 1) EBU_K1T (1); else EBU_K1T (2); }
-            else if (h->nchan == 1) { if (al) EBU_K1 (1, true); else EBU_K1 (1, false); }
-            else               { if (al) EBU_K1 (2, true); else EBU_K1 (2, false); }
-#undef EBU_K1
-#undef EBU_K1P
-#undef EBU_K1T
+            else if (tma) ebu_k1t_for (h->nchan)<<<grid, blk, EBU_TMA_SMEM, st>>> (tmap, nch, kf, ke, (int)pos, h->cf, ck, (float)h->fragm, h->d_z, h->d_frpwr, h->d_fragpw, (int)h->n_inst, pt);
+            // 1..5 channels; surround banks (3..5) with the lanes grouped per instance
+            else ebu_k1_for (h->nchan, al, multi, d_len)<<<grid, blk, EBU_SMEM_BYTES, st>>> (src, stride, nch, kf, ke, (int)pos, h->cf, ck, (float)h->fragm, h->d_z, h->d_frpwr, h->d_fragpw, (int)h->n_inst, pt, d_len);
             B200M_LAUNCHED (1);
         }
         if (after_k1 && done == 0) { if (int rc = after_k1 (after_arg)) return rc; }      // work to enqueue right behind the first K1

@@ -195,6 +195,14 @@ static void ppm_design (int kind, float fs, float w[4])
     else                             { w[0] = 200.0f / fs; w[1] = 860.0f / fs;  w[2] = 1.0f - 4.0f / fs; w[3] = 0.5141f; }            // iec2ppmdsp.cc:93-99, msppmdsp.cc:127-133
 }
 
+// ppm_kernel of a meter kind (both IEC kinds run KIND 1), an aligned block and a ragged one
+static auto ppm_kernel_for (int kind, bool al, bool rag)
+{
+    return with_int<B200M_PPM_VU, B200M_PPM_MS, 1> (kind, [&] (auto K) {
+        return with_bools ([&] (auto AL, auto RAG) { return ppm_kernel<K, AL, RAG>; }, al, rag);
+    });
+}
+
 // len (host, every entry <= nfram, some != nfram: ragged_check): unit u runs over its first len[u] frames; nullptr: every unit nfram
 static int ppm_process (b200m_ppm* h, const float* d_in, size_t stride, uint32_t nfram, cudaStream_t st, const uint32_t* len = nullptr)
 {
@@ -209,17 +217,8 @@ static int ppm_process (b200m_ppm* h, const float* d_in, size_t stride, uint32_t
     const size_t smem = (size_t)PPM_WARPS * PPM_STAGES * planes * PPM_PLANE * sizeof (float);
     const int nwarps = (h->n_units + 31) / 32;
     dim3 grid ((nwarps + PPM_WARPS - 1) / PPM_WARPS), blk (PPM_WARPS * 32);
-#define PPM_GO(K, A, R) ppm_kernel<K, A, R><<<grid, blk, smem, st>>> (d_in, stride, (int)h->n_units, (int)nfram, h->pr, h->d_mv, h->d_z1, h->d_z2, h->d_m, h->d_res, \
-                                                                      R ? h->rag.d : nullptr)
-    if (len) {
-        if (h->kind == B200M_PPM_VU) { if (al) PPM_GO (0, true, true); else PPM_GO (0, false, true); }
-        else if (h->kind == B200M_PPM_MS) { if (al) PPM_GO (3, true, true); else PPM_GO (3, false, true); }
-        else { if (al) PPM_GO (1, true, true); else PPM_GO (1, false, true); }
-    }
-    else if (h->kind == B200M_PPM_VU) { if (al) PPM_GO (0, true, false); else PPM_GO (0, false, false); }
-    else if (h->kind == B200M_PPM_MS) { if (al) PPM_GO (3, true, false); else PPM_GO (3, false, false); }
-    else { if (al) PPM_GO (1, true, false); else PPM_GO (1, false, false); }
-#undef PPM_GO
+    ppm_kernel_for (h->kind, al, len)<<<grid, blk, smem, st>>> (d_in, stride, (int)h->n_units, (int)nfram, h->pr, h->d_mv, h->d_z1, h->d_z2, h->d_m,
+                                                            h->d_res, len ? h->rag.d : nullptr);
     B200M_LAUNCHED (1);
     B200M_CUDA (cudaGetLastError ());
     return 0;
@@ -258,10 +257,10 @@ int b200m_ppm_create (b200m_ppm** out, int device, uint32_t n_units, float fsamp
     if (kind == B200M_PPM_MS) A ((void**)&h->d_mv, n_units * sizeof (float2));
     if (e == cudaSuccess) e = cudaStreamCreateWithFlags (&h->path.own, cudaStreamNonBlocking);
     const int smem_max = PPM_WARPS * PPM_STAGES * 2 * PPM_PLANE * (int)sizeof (float);
-#define PPM_ATTR(K, A) if (e == cudaSuccess) e = cudaFuncSetAttribute (ppm_kernel<K, A>, cudaFuncAttributeMaxDynamicSharedMemorySize, smem_max); \
-                       if (e == cudaSuccess) e = cudaFuncSetAttribute (ppm_kernel<K, A, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, smem_max)
-    PPM_ATTR (0, true); PPM_ATTR (0, false); PPM_ATTR (1, true); PPM_ATTR (1, false); PPM_ATTR (3, true); PPM_ATTR (3, false);
-#undef PPM_ATTR
+    for (int k = B200M_PPM_VU; k <= B200M_PPM_MS; ++k)
+        for (const bool al : {false, true})
+            for (const bool rag : {false, true})
+                if (e == cudaSuccess) e = cudaFuncSetAttribute (ppm_kernel_for (k, al, rag), cudaFuncAttributeMaxDynamicSharedMemorySize, smem_max);
     if (e == cudaSuccess) {
         ppm_init_kernel<<<(unsigned)((nm + 255) / 256), 256>>> ((int)nm, h->d_res);    // constructors: _res (true)
         B200M_LAUNCHED (1);

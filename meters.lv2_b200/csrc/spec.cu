@@ -310,12 +310,9 @@ static int spec_process (b200m_spec* h, const float* d_in, size_t stride, uint32
     rp.ac0 = (int)(h->frames & 1);
     h->frames += nfram;
     const unsigned grid = (h->n_inst + SPEC_WARPS - 1) / SPEC_WARPS;
-#define SPEC_GO(F, R) spec_kernel<F, R><<<grid, SPEC_WARPS * 32, 0, st>>> (d_in, stride, (int)h->n_inst, (int)nfram, rp, h->d_ctl, h->d_coef, h->d_z, \
-                                                                          h->d_val, h->d_ports, R ? h->rag.d : nullptr)
-    if (len) { if (h->fma) SPEC_GO (true, true); else SPEC_GO (false, true); }
-    else if (h->fma) SPEC_GO (true, false);
-    else SPEC_GO (false, false);
-#undef SPEC_GO
+    const auto k = with_bools ([] (auto FMA, auto RAG) { return spec_kernel<FMA, RAG>; }, h->fma, len);
+    k<<<grid, SPEC_WARPS * 32, 0, st>>> (d_in, stride, (int)h->n_inst, (int)nfram, rp, h->d_ctl, h->d_coef, h->d_z, h->d_val, h->d_ports,
+                                         len ? h->rag.d : nullptr);
     B200M_LAUNCHED (1);
     B200M_CUDA (cudaGetLastError ());
     if (len) {

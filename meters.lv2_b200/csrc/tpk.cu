@@ -2212,23 +2212,68 @@ int tpk_reset_inst (b200m_tpk* h, const uint32_t* d_inst, uint32_t n_sel, uint32
 }
 }
 
-// the instantiations of the EBUr128 epilogue's HOLD (r128_group_hold)
-template <bool IMM, bool FMA, bool RAG = false, bool SPLIT = false> static decltype (&tpmax_kernel<IMM, FMA, 2, RAG, SPLIT>) tpmax_kernel_for (int hold)
+// ---- kernel selectors: each maps a bank's run-time choices to one instantiation of a kernel family.  The launch paths and
+// b200m_tpk_create's attributes both go through them, so every form a path can launch is a form that gets its attributes.
+
+// The FIR form of a bank: exact with the coefficient table or with immediate coefficients, or tolerance mode (FMA, immediates only)
+enum class TpkFir { TAB, IMM, FMA };
+static constexpr TpkFir TPK_FIRS[] = {TpkFir::TAB, TpkFir::IMM, TpkFir::FMA};
+static TpkFir tpk_mode (const b200m_tpk* h) { return h->imm && h->fma ? TpkFir::FMA : h->imm ? TpkFir::IMM : TpkFir::TAB; }
+// f (IMM, FMA) of a FIR form, as compile-time flags
+template <class F> static auto with_fir (TpkFir m, F f)
 {
-    return hold == 0 ? tpmax_kernel<IMM, FMA, 0, RAG, SPLIT> : hold == 1 ? tpmax_kernel<IMM, FMA, 1, RAG, SPLIT>
-         : hold == 4 ? tpmax_kernel<IMM, FMA, 4, RAG, SPLIT> : tpmax_kernel<IMM, FMA, 2, RAG, SPLIT>;
+    return m == TpkFir::FMA ? f (std::true_type {}, std::true_type {}) : m == TpkFir::IMM ? f (std::true_type {}, std::false_type {})
+                                                                     : f (std::false_type {}, std::false_type {});
 }
-// ... by precision mode: exact with the coefficient table or the immediates, FMA (immediates only)
-template <bool RAG, bool SPLIT> static decltype (&tpmax_kernel<true, true, 2, RAG, SPLIT>) tpmax_kernel_mode (const b200m_tpk* h, int hold)
+// the EBUr128 epilogue's HOLD (r128_hold_of)
+static constexpr int R128_HOLDS[] = {0, 1, 2, 4};
+template <class F> static auto with_hold (int hold, F f) { return with_int<0, 1, 4, 2> (hold, f); }
+
+// Named before any other kernel of this file, so that tcf_smem is the module's first extern __shared__ array: where ptxas starts the
+// dynamic shared memory of tpk_kernel depends on that order, and with this one it is 128-byte aligned, as that kernel was tuned
+using TpmaxTcKernel = decltype (&tpmax_tc_kernel<2>);
+static TpmaxTcKernel tpmax_tc_kernel_for (int hold) { return with_hold (hold, [] (auto HOLD) { return tpmax_tc_kernel<HOLD>; }); }
+// tpk_kernel<CH, TC, TP, MX, ...> of a FIR form, the K-meter and the DR-14 sums.  Choices that mean nothing for a form collapse, so
+// that only launchable forms are instantiated: without true peak there is no FIR and the bank is a K-meter; the DR-14 sums ride on
+// process() with both meters; a ragged block runs the exact kernel, with the immediates only beside the K-meter (the true-peak-only
+// immediate form spills 8 bytes).
+using TpkKernel = decltype (&tpk_kernel<16, 64, true, false, true, false, false>);
+template <int CH, int TC, bool TP, bool MX, bool RAG = false> static TpkKernel tpk_kernel_for (TpkFir m, bool km, bool dr)
 {
-    return h->imm && h->fma ? tpmax_kernel_for<true, true, RAG, SPLIT> (hold) : h->imm ? tpmax_kernel_for<true, false, RAG, SPLIT> (hold)
-                                                                                          : tpmax_kernel_for<false, false, RAG, SPLIT> (hold);
+    return with_fir (m, [&] (auto IMM, auto FMA) {
+        return with_bools ([&] (auto KM, auto DR) {
+            return tpk_kernel<CH, TC, TP, MX, KM || !TP, IMM && TP && (KM || !RAG), DR && KM && TP && !MX, FMA && TP && !RAG, RAG>;
+        }, km, dr);
+    });
 }
-static decltype (&tpmax_tc_kernel<2>) tpmax_tc_kernel_for (int hold)
+// tpmax_kernel of a FIR form, a hold, a ragged block and the dBTP plane's fragment split
+using TpmaxKernel = decltype (&tpmax_kernel<true, true, 2>);
+static TpmaxKernel tpmax_kernel_for (TpkFir m, int hold, bool rag, bool split)
 {
-    return hold == 0 ? tpmax_tc_kernel<0> : hold == 1 ? tpmax_tc_kernel<1> : hold == 4 ? tpmax_tc_kernel<4> : tpmax_tc_kernel<2>;
+    return with_fir (m, [&] (auto IMM, auto FMA) {
+        return with_hold (hold, [&] (auto HOLD) {
+            return with_bools ([&] (auto RAG, auto SPLIT) { return tpmax_kernel<IMM, FMA, HOLD, RAG, SPLIT>; }, rag, split);
+        });
+    });
 }
-static const int R128_HOLDS[4] = {0, 1, 2, 4};
+// tpdec_kernel runs the immediates only: m is IMM or FMA
+using TpdecKernel = decltype (&tpdec_kernel<true, true>);
+static TpdecKernel tpdec_kernel_for (TpkFir m, bool km) { return with_bools ([] (auto KM, auto FMA) { return tpdec_kernel<KM, FMA>; }, km, m == TpkFir::FMA); }
+static auto tpfir_kernel_for (TpkFir m) { return with_fir (m, [] (auto IMM, auto FMA) { return tpfir_kernel<IMM, FMA>; }); }
+static auto tpbal_kernel_for (bool km, bool dr) { return with_bools ([] (auto KM, auto DR) { return tpbal_kernel<KM, DR && KM>; }, km, dr); }
+// r128_fused_kernel of 1..5 channels per instance, with or without per-instance fragment phases
+static auto r128_fused_kernel_for (int nchan, bool phases)
+{
+    return with_int<1, 2, 3, 4, 5> (nchan, [&] (auto N) { return with_bools ([&] (auto PH) { return r128_fused_kernel<N, PH>; }, phases); });
+}
+
+// The tensor-core true-peak kernels (tpmax_tc_kernel, r128_fused_kernel) can run this bank's process_max: true peak alone, tolerance
+// mode, the chunk-parallel and tensor-core paths on, no debug tap, and a 16-byte-aligned block of whole float4 rows
+static bool tpk_tc_ok (const b200m_tpk* h, bool aligned, uint32_t nfram)
+{
+    return (h->flags & B200M_TPK_TRUEPEAK) && !(h->flags & B200M_TPK_KMETER) && h->chunked && h->tc && h->fma && h->imm && h->d_btc && !h->d_dbg
+        && aligned && nfram % 4 == 0;
+}
 
 // process()/process_max() of every meter; channel slices [bounds[s], bounds[s+1]) are launched separately, slice s
 // after event ready[s] when `ready` is given (see ebu_process_sliced).
@@ -2248,7 +2293,8 @@ int tpk_process_sliced (b200m_tpk* h, const float* d_in, size_t stride, uint32_t
     // Kmeterdsp::process (:65-70): per-period fallback multiplier, a pure function of n
     prm.fall = tpk_km_fall (h, nfram);
     const int aligned = ((uintptr_t)d_in % 16 == 0) && (stride % 4 == 0);
-    dim3 blk (TPK_THREADS);
+    const TpkFir m = tpk_mode (h);
+    const int hold = r128_hold_of (r128), nchunks = ((int)nfram + 255) / 256;
     bool swap_hist = false;
     for (int sl = 0; sl < nsl; ++sl) {
         const int cf = (int)bounds[sl], ce = (int)bounds[sl + 1];
@@ -2261,58 +2307,36 @@ int tpk_process_sliced (b200m_tpk* h, const float* d_in, size_t stride, uint32_t
         cudaLaunchAttribute at[1];
         at[0].id = cudaLaunchAttributeProgrammaticStreamSerialization; at[0].val.programmaticStreamSerializationAllowed = 1;
         cudaLaunchConfig_t cfg = {};
-        cfg.blockDim = blk; cfg.dynamicSmemBytes = 0; cfg.stream = st; cfg.attrs = at; cfg.numAttrs = pdl ? 1 : 0;
-#define TPK_GO(CH, TC, TP, MX, KM, DRM) do { cfg.gridDim = dim3 ((ce - cf + CH - 1) / CH); cfg.dynamicSmemBytes = TpkGeom<CH, TC, (TP) && !(MX)>::BYTES; \
-            if (h->imm && h->fma) B200M_CUDA (cudaLaunchKernelEx (&cfg, tpk_kernel<CH, TC, TP, MX, KM, true, DRM, true>, d_in, stride, cf, ce, (int)nfram, aligned, h->elide0, prm, h->st, h->d_dbg, r128, drp, TpkRag {})); \
-            else if (h->imm) B200M_CUDA (cudaLaunchKernelEx (&cfg, tpk_kernel<CH, TC, TP, MX, KM, true, DRM>, d_in, stride, cf, ce, (int)nfram, aligned, h->elide0, prm, h->st, h->d_dbg, r128, drp, TpkRag {})); \
-            else B200M_CUDA (cudaLaunchKernelEx (&cfg, tpk_kernel<CH, TC, TP, MX, KM, false, DRM>, d_in, stride, cf, ce, (int)nfram, aligned, h->elide0, prm, h->st, h->d_dbg, r128, drp, TpkRag {})); } while (0)
-        if (rlen || sp.fmax) {
-            const int nchunks = ((int)nfram + 255) / 256;
-            cfg.gridDim = dim3 ((unsigned)(((ce - cf + 7) / 8) * nchunks));
-            const int hold = r128_hold_of (r128);
-            const auto k = rlen ? (sp.fmax ? tpmax_kernel_mode<true, true> (h, hold) : tpmax_kernel_mode<true, false> (h, hold))
-                                : tpmax_kernel_mode<false, true> (h, hold);
-            B200M_CUDA (cudaLaunchKernelEx (&cfg, k, d_in, stride, cf, ce, (int)nfram, nchunks, aligned, h->elide0, h->st, h->d_dbg, r128, rlen, sp));
-            swap_hist = true;
-        }
-        else if (tp && tp_mode == B200M_TP_MODE_MAX && !km && h->chunked && h->tc && h->fma && h->imm && h->d_btc && aligned && nfram % 4 == 0 && !h->d_dbg
-            && (ce - cf + 7) / 8 >= h->n_sm) {
+        cfg.blockDim = dim3 (TPK_THREADS); cfg.dynamicSmemBytes = 0; cfg.stream = st; cfg.attrs = at; cfg.numAttrs = pdl ? 1 : 0;
+        // choose one kernel and its launch shape (the slab pipeline launches its own), then launch it
+        TpmaxKernel mk = nullptr; TpmaxTcKernel ck = nullptr; TpkKernel tk = nullptr; TpdecKernel dk = nullptr;
+        auto tpk = [&] (TpkKernel k, int ch, size_t smem) { tk = k; cfg.gridDim = dim3 ((ce - cf + ch - 1) / ch); cfg.dynamicSmemBytes = smem; };
+        if (rlen || sp.fmax) mk = tpmax_kernel_for (m, hold, rlen, sp.fmax);
+        else if (tp_mode == B200M_TP_MODE_MAX && tpk_tc_ok (h, aligned, nfram) && (ce - cf + 7) / 8 >= h->n_sm) {
             // tensor-core path: persistent CTAs, each takes whole 8-channel groups (a bank too small to give every SM a group runs tpmax_kernel)
-            const int nchunks = ((int)nfram + 255) / 256;
+            ck = tpmax_tc_kernel_for (hold);
             cfg.blockDim = dim3 (TCF_THREADS); cfg.gridDim = dim3 ((unsigned)std::min ((ce - cf + 7) / 8, h->n_sm)); cfg.dynamicSmemBytes = TCF_SMEM;
-            B200M_CUDA (cudaLaunchKernelEx (&cfg, tpmax_tc_kernel_for (r128_hold_of (r128)), d_in, stride, cf, ce, (int)nfram, nchunks, (const float*)h->d_btc, h->st, r128));
-            cfg.blockDim = blk;
-            swap_hist = true;
         }
-        else if (tp && tp_mode == B200M_TP_MODE_MAX && !km && h->chunked) {
-            // chunk-parallel process_max (tpmax_kernel): the EBUr128 epilogue's groups need c_first to be a multiple of r128.nch (r128.cu)
-            const int nchunks = ((int)nfram + 255) / 256;
-            cfg.gridDim = dim3 ((unsigned)(((ce - cf + 7) / 8) * nchunks));
-            const int hold = r128_hold_of (r128);
-            const auto k = h->imm && h->fma ? tpmax_kernel_for<true, true> (hold) : h->imm ? tpmax_kernel_for<true, false> (hold) : tpmax_kernel_for<false, false> (hold);
-            B200M_CUDA (cudaLaunchKernelEx (&cfg, k, d_in, stride, cf, ce, (int)nfram, nchunks, aligned, h->elide0, h->st, h->d_dbg, r128, (const uint32_t*)nullptr, TpSplit {}));
-            swap_hist = true;
-        }
-        else if (tp && tp_mode == B200M_TP_MODE_MAX) { if (km) TPK_GO (8, 256, true, true, true, false); else TPK_GO (8, 256, true, true, false, false); }
+        // chunk-parallel process_max (tpmax_kernel): the EBUr128 epilogue's groups need c_first to be a multiple of r128.nch (r128.cu)
+        else if (tp && tp_mode == B200M_TP_MODE_MAX && !km && h->chunked) mk = tpmax_kernel_for (m, hold, false, false);
+        else if (tp && tp_mode == B200M_TP_MODE_MAX) tpk (tpk_kernel_for<8, 256, true, true> (m, km, false), 8, TpkGeom<8, 256, false>::BYTES);
         else if (tp && h->split && h->d_scr) {
             // FIR / ballistics slab pipeline: FIR kernels on `st`, ballistics kernels on the bank's second stream, one slab behind
             const int nslab = ((int)nfram + (int)h->slab - 1) / (int)h->slab;
             const int ngrp = (ce - cf + TPF_CH - 1) / TPF_CH, nb16 = (ce - cf + 15) / 16;
+            const auto fk = tpfir_kernel_for (m);
+            const auto bk = tpbal_kernel_for (km, drp.rms_sum);
             // the ballistics stream must not start before everything queued on `st` so far (previous block's state, controls)
             for (int sidx = 0; sidx < nslab; ++sidx) {
                 const int sb0 = sidx * (int)h->slab, sl_len = std::min ((int)h->slab, (int)nfram - sb0), b = sidx & 1;
                 float4* scr = h->d_scr + (size_t)b * h->n_chan * h->slab + (size_t)cf * h->slab;
                 if (sidx >= 2) B200M_CUDA (cudaStreamWaitEvent (st, h->ev_bal[b], 0));          // the slab buffer is free again
                 const int nch = (sl_len + TPF_TC - 1) / TPF_TC;
-                if (h->imm && h->fma) tpfir_kernel<true, true><<<ngrp * nch, blk, 0, st>>> (d_in, stride, cf, ce, (int)nfram, sb0, sl_len, aligned, h->elide0, h->st, scr, (int)h->slab, h->d_dbg, h->d_tl, h->tl_next);
-                else if (h->imm) tpfir_kernel<true, false><<<ngrp * nch, blk, 0, st>>> (d_in, stride, cf, ce, (int)nfram, sb0, sl_len, aligned, h->elide0, h->st, scr, (int)h->slab, h->d_dbg, h->d_tl, h->tl_next);
-                else tpfir_kernel<false, false><<<ngrp * nch, blk, 0, st>>> (d_in, stride, cf, ce, (int)nfram, sb0, sl_len, aligned, h->elide0, h->st, scr, (int)h->slab, h->d_dbg, h->d_tl, h->tl_next);
+                fk<<<ngrp * nch, TPK_THREADS, 0, st>>> (d_in, stride, cf, ce, (int)nfram, sb0, sl_len, aligned, h->elide0, h->st, scr, (int)h->slab, h->d_dbg, h->d_tl, h->tl_next);
                 B200M_CUDA (cudaEventRecord (h->ev_fir[b], st));
                 B200M_CUDA (cudaStreamWaitEvent (h->sb, h->ev_fir[b], 0));
                 const int first = sidx == 0, last = sidx == nslab - 1;
-                if (km && drp.rms_sum) tpbal_kernel<true, true><<<nb16, 64, 0, h->sb>>> (scr, (int)h->slab, d_in, stride, cf, ce, (int)h->n_chan, (int)nfram, sb0, sl_len, first, last, aligned, 1, prm, h->st, drp, h->d_tl, h->tl_next + 1);
-                else if (km) tpbal_kernel<true, false><<<nb16, 64, 0, h->sb>>> (scr, (int)h->slab, d_in, stride, cf, ce, (int)h->n_chan, (int)nfram, sb0, sl_len, first, last, aligned, 1, prm, h->st, drp, h->d_tl, h->tl_next + 1);
-                else tpbal_kernel<false, false><<<nb16, 64, 0, h->sb>>> (scr, (int)h->slab, d_in, stride, cf, ce, (int)h->n_chan, (int)nfram, sb0, sl_len, first, last, aligned, 1, prm, h->st, drp, h->d_tl, h->tl_next + 1);
+                bk<<<nb16, 64, 0, h->sb>>> (scr, (int)h->slab, d_in, stride, cf, ce, (int)h->n_chan, (int)nfram, sb0, sl_len, first, last, aligned, 1, prm, h->st, drp, h->d_tl, h->tl_next + 1);
                 B200M_CUDA (cudaEventRecord (h->ev_bal[b], h->sb));
                 B200M_LAUNCHED (2);
                 if (h->d_tl) h->tl_next = (h->tl_next + 2) % 4096;
@@ -2322,23 +2346,23 @@ int tpk_process_sliced (b200m_tpk* h, const float* d_in, size_t stride, uint32_t
             swap_hist = true;
             continue;
         }
-        else if (tp && h->dec && h->imm && !h->d_dbg && !drp.rms_sum) {
-            const unsigned grid = (unsigned)((ce - cf + TPD_CH - 1) / TPD_CH);
-            if (h->fma) {
-                if (km) tpdec_kernel<true, true><<<grid, blk, 0, st>>> (d_in, stride, cf, ce, (int)nfram, aligned, h->elide0, prm, h->st);
-                else tpdec_kernel<false, true><<<grid, blk, 0, st>>> (d_in, stride, cf, ce, (int)nfram, aligned, h->elide0, prm, h->st);
-            } else {
-                if (km) tpdec_kernel<true, false><<<grid, blk, 0, st>>> (d_in, stride, cf, ce, (int)nfram, aligned, h->elide0, prm, h->st);
-                else tpdec_kernel<false, false><<<grid, blk, 0, st>>> (d_in, stride, cf, ce, (int)nfram, aligned, h->elide0, prm, h->st);
-            }
+        else if (tp && h->dec && h->imm && !h->d_dbg && !drp.rms_sum) { dk = tpdec_kernel_for (m, km); cfg.gridDim = dim3 ((unsigned)((ce - cf + TPD_CH - 1) / TPD_CH)); }
+        // wide CTAs (64 channels x 32-sample chunks): every warp has ballistics lanes, so none idles through the serial phase
+        else if (tp && h->wide && (ce - cf) >= h->wide_min) tpk (tpk_kernel_for<64, 32, true, false> (m, km, drp.rms_sum), 64, TpkGeom<64, 32, true>::BYTES);
+        else if (tp) tpk (tpk_kernel_for<16, 64, true, false> (m, km, drp.rms_sum), 16, TpkGeom<16, 64, true>::BYTES);
+        else tpk (tpk_kernel_for<16, 64, false, false> (m, km, false), 16, TpkGeom<16, 64, false>::BYTES);
+        // (pdl comes with the EBUr128 cycle's process_max only, which never picks tpdec_kernel)
+        if (ck) {
+            B200M_CUDA (cudaLaunchKernelEx (&cfg, ck, d_in, stride, cf, ce, (int)nfram, nchunks, (const float*)h->d_btc, h->st, r128));
+            swap_hist = true;
         }
-        else if (tp && h->wide && (ce - cf) >= h->wide_min) {
-            // wide CTAs (64 channels x 32-sample chunks): every warp has ballistics lanes, so none idles through the serial phase
-            if (km) { if (drp.rms_sum) TPK_GO (64, 32, true, false, true, true); else TPK_GO (64, 32, true, false, true, false); } else TPK_GO (64, 32, true, false, false, false);
+        if (mk) {
+            cfg.gridDim = dim3 ((unsigned)(((ce - cf + 7) / 8) * nchunks));
+            B200M_CUDA (cudaLaunchKernelEx (&cfg, mk, d_in, stride, cf, ce, (int)nfram, nchunks, aligned, h->elide0, h->st, h->d_dbg, r128, rlen, sp));
+            swap_hist = true;
         }
-        else if (tp) { if (km) { if (drp.rms_sum) TPK_GO (16, 64, true, false, true, true); else TPK_GO (16, 64, true, false, true, false); } else TPK_GO (16, 64, true, false, false, false); }
-        else tpk_kernel<16, 64, false, false, true, false, false><<<(ce - cf + 15) / 16, blk, TpkGeom<16, 64, false>::BYTES, st>>> (d_in, stride, cf, ce, (int)nfram, aligned, h->elide0, prm, h->st, h->d_dbg, r128, drp, TpkRag {});
-#undef TPK_GO
+        if (tk) B200M_CUDA (cudaLaunchKernelEx (&cfg, tk, d_in, stride, cf, ce, (int)nfram, aligned, h->elide0, prm, h->st, h->d_dbg, r128, drp, TpkRag {}));
+        if (dk) B200M_CUDA (cudaLaunchKernelEx (&cfg, dk, d_in, stride, cf, ce, (int)nfram, aligned, h->elide0, prm, h->st));
         B200M_LAUNCHED (1);
     }
     if (swap_hist) { float* t = h->st.hist; h->st.hist = h->st.hist_alt; h->st.hist_alt = t; }     // every slice wrote the alternate buffer
@@ -2382,18 +2406,10 @@ int tpk_process_ragged (b200m_tpk* h, const float* d_in, size_t stride, uint32_t
     const TpkRag rag = {d_len, d_fall, (int)per};
     const int aligned = ((uintptr_t)d_in % 16 == 0) && (stride % 4 == 0);
     const unsigned grid = (h->n_chan + 15) / 16;
-    const int n = (int)h->n_chan;
-#define TPK_RAG(TPF, KMF, IMMF, DRF) tpk_kernel<16, 64, TPF, false, KMF, IMMF, DRF, false, true><<<grid, TPK_THREADS, TpkGeom<16, 64, TPF>::BYTES, st>>> ( \
-        d_in, stride, 0, n, (int)nfram, aligned, h->elide0, h->prm, h->st, h->d_dbg, R128Hold {}, drp, rag)
-    if (tp && km) {
-        if (h->imm) { if (drp.rms_sum) TPK_RAG (true, true, true, true); else TPK_RAG (true, true, true, false); }
-        else { if (drp.rms_sum) TPK_RAG (true, true, false, true); else TPK_RAG (true, true, false, false); }
-    }
-    // true peak alone: the coefficient-table form (the same products in the same order as the immediate form, which spills 8 bytes
-    // in this instantiation)
-    else if (tp) TPK_RAG (true, false, false, false);
-    else TPK_RAG (false, true, false, false);
-#undef TPK_RAG
+    const TpkKernel k = tp ? tpk_kernel_for<16, 64, true, false, true> (tpk_mode (h), km, drp.rms_sum)
+                           : tpk_kernel_for<16, 64, false, false, true> (tpk_mode (h), km, false);
+    k<<<grid, TPK_THREADS, tp ? TpkGeom<16, 64, true>::BYTES : TpkGeom<16, 64, false>::BYTES, st>>> (
+        d_in, stride, 0, (int)h->n_chan, (int)nfram, aligned, h->elide0, h->prm, h->st, h->d_dbg, R128Hold {}, drp, rag);
     B200M_LAUNCHED (1);
     B200M_CUDA (cudaGetLastError ());
     return 0;
@@ -2421,14 +2437,8 @@ float* tpk_hist (b200m_tpk* h) { return h->st.hist; }
 
 bool tpk_r128_fused_ok (const b200m_tpk* h, const float* d_in, size_t stride, uint32_t nfram)
 {
-    return (h->flags & B200M_TPK_TRUEPEAK) && !(h->flags & B200M_TPK_KMETER) && h->chunked && h->tc && h->fma && h->imm && h->d_btc && !h->d_dbg
-        && (uintptr_t)d_in % 16 == 0 && stride % 4 == 0 && nfram % 4 == 0 && h->n_chan >= R128F_MIN_CH;
+    return tpk_tc_ok (h, (uintptr_t)d_in % 16 == 0 && stride % 4 == 0, nfram) && h->n_chan >= R128F_MIN_CH;
 }
-
-// r128_fused_kernel<nchan, PHASES> as r128f_kernels[nchan - 1][PHASES]
-#define R128F_K(N) {r128_fused_kernel<N, false>, r128_fused_kernel<N, true>}
-static const decltype (&r128_fused_kernel<2, false>) r128f_kernels[5][2] = {R128F_K (1), R128F_K (2), R128F_K (3), R128F_K (4), R128F_K (5)};
-#undef R128F_K
 
 int tpk_r128_fused (b200m_tpk* h, const EbuK1Args& a, float* r128_tpmax, cudaStream_t st)
 {
@@ -2439,7 +2449,7 @@ int tpk_r128_fused (b200m_tpk* h, const EbuK1Args& a, float* r128_tpmax, cudaStr
     if (!ebu_tma_map (&tm, a.in, a.stride, h->n_chan, (uint32_t)a.nfram, R128F_PITCH, R128F_CH, false))
         return set_err (B200M_E_CUDA, "r128: the driver rejected the input block's tensor map");
     const int slab = 4 * (32 / nchan) * nchan, nslabs = ((int)h->n_chan + slab - 1) / slab;         // r128_fused_kernel's SLAB
-    r128f_kernels[nchan - 1][a.ck.fph ? 1 : 0]<<<std::min (nslabs, h->n_sm), R128F_WARPS * 32, R128F_SMEM, st>>> (
+    r128_fused_kernel_for (nchan, a.ck.fph)<<<std::min (nslabs, h->n_sm), R128F_WARPS * 32, R128F_SMEM, st>>> (
         tm, a.in, a.stride, (int)h->n_chan, a.nfram, h->d_btc, h->st, r128_tpmax, a.cf, a.ck, a.fragm_f, a.zst, a.frpwr, a.fragpw, a.n_inst);
     B200M_LAUNCHED (1);
     B200M_CUDA (cudaGetLastError ());
@@ -2482,23 +2492,19 @@ int b200m_tpk_create (b200m_tpk** out, int device, uint32_t n_chan, float fsamp,
     if (const char* v = getenv ("B200M_TPK_ELIDE0")) h->elide0 = h->elide0 && atoi (v);      // 0: always evaluate phase 0 (tests, worst-case timing)
     if (const char* v = getenv ("B200M_TPK_PRECISION")) h->fma = (strcmp (v, "fma") == 0) && h->imm && h->ctab[23] == 1.0f;
     cudaError_t e = cudaMemcpyToSymbol (c_tp_tab, h->ctab, sizeof (h->ctab));
-    // the process_max kernels share SMs with the K-weighting kernel in the EBUr128 cycle: same (maximum) carveout, so that the SM
-    // need not be reconfigured between the two
-    if (e == cudaSuccess) e = cudaFuncSetAttribute (tpk_kernel<8, 256, true, true, false, true, false, true>, cudaFuncAttributePreferredSharedMemoryCarveout, cudaSharedmemCarveoutMaxShared);
-    if (e == cudaSuccess) e = cudaFuncSetAttribute (tpk_kernel<8, 256, true, true, false, true, false, false>, cudaFuncAttributePreferredSharedMemoryCarveout, cudaSharedmemCarveoutMaxShared);
-    if (e == cudaSuccess) e = cudaFuncSetAttribute (tpk_kernel<8, 256, true, true, false, false, false, false>, cudaFuncAttributePreferredSharedMemoryCarveout, cudaSharedmemCarveoutMaxShared);
-    // seven CTAs x 24 KB per SM: without the hint the driver may pick a carveout that fits four
-    if (e == cudaSuccess) e = cudaFuncSetAttribute (tpdec_kernel<true, true>, cudaFuncAttributePreferredSharedMemoryCarveout, cudaSharedmemCarveoutMaxShared);
-    if (e == cudaSuccess) e = cudaFuncSetAttribute (tpdec_kernel<false, true>, cudaFuncAttributePreferredSharedMemoryCarveout, cudaSharedmemCarveoutMaxShared);
-    if (e == cudaSuccess) e = cudaFuncSetAttribute (tpdec_kernel<true, false>, cudaFuncAttributePreferredSharedMemoryCarveout, cudaSharedmemCarveoutMaxShared);
-    if (e == cudaSuccess) e = cudaFuncSetAttribute (tpdec_kernel<false, false>, cudaFuncAttributePreferredSharedMemoryCarveout, cudaSharedmemCarveoutMaxShared);
-    for (const int hold : R128_HOLDS)
-        for (const auto k : {tpmax_kernel_for<true, true> (hold), tpmax_kernel_for<true, false> (hold), tpmax_kernel_for<false, false> (hold),
-                             tpmax_kernel_for<true, true, true> (hold), tpmax_kernel_for<true, false, true> (hold), tpmax_kernel_for<false, false, true> (hold),
-                             tpmax_kernel_for<true, true, false, true> (hold), tpmax_kernel_for<true, false, false, true> (hold),
-                             tpmax_kernel_for<false, false, false, true> (hold), tpmax_kernel_for<true, true, true, true> (hold),
-                             tpmax_kernel_for<true, false, true, true> (hold), tpmax_kernel_for<false, false, true, true> (hold)})
-            if (e == cudaSuccess) e = cudaFuncSetAttribute (k, cudaFuncAttributePreferredSharedMemoryCarveout, cudaSharedmemCarveoutMaxShared);
+    auto carveout = [&] (auto k) { if (e == cudaSuccess) e = cudaFuncSetAttribute (k, cudaFuncAttributePreferredSharedMemoryCarveout, cudaSharedmemCarveoutMaxShared); };
+    auto smem = [&] (auto k, int bytes) { if (e == cudaSuccess) e = cudaFuncSetAttribute (k, cudaFuncAttributeMaxDynamicSharedMemorySize, bytes); };
+    const bool NO_YES[] = {false, true};
+    for (const TpkFir m : TPK_FIRS) {
+        // the process_max kernels share SMs with the K-weighting kernel in the EBUr128 cycle: same (maximum) carveout, so that the SM
+        // need not be reconfigured between the two (with the K-meter, the 8-channel kernel keeps the default)
+        carveout (tpk_kernel_for<8, 256, true, true> (m, false, false));
+        for (const int hold : R128_HOLDS) for (const bool rag : NO_YES) for (const bool split : NO_YES) carveout (tpmax_kernel_for (m, hold, rag, split));
+        // seven CTAs x 24 KB per SM: without the hint the driver may pick a carveout that fits four
+        if (m != TpkFir::TAB) for (const bool km : NO_YES) carveout (tpdec_kernel_for (m, km));
+        // the wide process() kernels need 87 KB of dynamic shared memory
+        for (const bool km : NO_YES) for (const bool dr : NO_YES) smem (tpk_kernel_for<64, 32, true, false> (m, km, dr), (int)TpkGeom<64, 32, true>::BYTES);
+    }
     auto A = [&] (void** p, size_t bytes) { if (e == cudaSuccess) { e = cudaMalloc (p, bytes); if (e == cudaSuccess) e = cudaMemset (*p, 0, bytes); } };
     const size_t n = n_chan;
     A ((void**)&h->st.hist, n * 48 * sizeof (float));
@@ -2530,12 +2536,8 @@ int b200m_tpk_create (b200m_tpk** out, int device, uint32_t n_chan, float fsamp,
             delete[] hb;
         }
         // it shares SMs with the K-weighting kernel in the EBUr128 cycle (106 KB + 104 KB): same (maximum) carveout as that one
-        for (const int hold : R128_HOLDS) {
-            if (e == cudaSuccess) e = cudaFuncSetAttribute (tpmax_tc_kernel_for (hold), cudaFuncAttributeMaxDynamicSharedMemorySize, TCF_SMEM);
-            if (e == cudaSuccess) e = cudaFuncSetAttribute (tpmax_tc_kernel_for (hold), cudaFuncAttributePreferredSharedMemoryCarveout, cudaSharedmemCarveoutMaxShared);
-        }
-        for (const auto& kp : r128f_kernels)
-            for (const auto k : kp) if (e == cudaSuccess) e = cudaFuncSetAttribute (k, cudaFuncAttributeMaxDynamicSharedMemorySize, R128F_SMEM);
+        for (const int hold : R128_HOLDS) { smem (tpmax_tc_kernel_for (hold), TCF_SMEM); carveout (tpmax_tc_kernel_for (hold)); }
+        for (int nchan = 1; nchan <= 5; ++nchan) for (const bool ph : NO_YES) smem (r128_fused_kernel_for (nchan, ph), R128F_SMEM);
         if (e == cudaSuccess) e = cudaDeviceGetAttribute (&h->n_sm, cudaDevAttrMultiProcessorCount, device);
     }
     if (const char* v = getenv ("B200M_TPK_DEC")) h->dec = atoi (v) != 0;
@@ -2570,13 +2572,6 @@ int b200m_tpk_create (b200m_tpk** out, int device, uint32_t n_chan, float fsamp,
         if (w > 1) h->wide_min = w;
         else if (e == cudaSuccess) { int nsm = 0; e = cudaDeviceGetAttribute (&nsm, cudaDevAttrMultiProcessorCount, device); h->wide_min = 64 * nsm; }
     }
-    // the wide process() kernels need 87 KB of dynamic shared memory
-#define TPK_WATTR(KMF, DRF, FMAF) if (e == cudaSuccess) e = cudaFuncSetAttribute (tpk_kernel<64, 32, true, false, KMF, true, DRF, FMAF>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)TpkGeom<64, 32, true>::BYTES)
-    TPK_WATTR (true, true, true); TPK_WATTR (true, true, false); TPK_WATTR (true, false, true); TPK_WATTR (true, false, false); TPK_WATTR (false, false, true); TPK_WATTR (false, false, false);
-#undef TPK_WATTR
-    if (e == cudaSuccess) e = cudaFuncSetAttribute (tpk_kernel<64, 32, true, false, true, false, true, false>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)TpkGeom<64, 32, true>::BYTES);
-    if (e == cudaSuccess) e = cudaFuncSetAttribute (tpk_kernel<64, 32, true, false, true, false, false, false>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)TpkGeom<64, 32, true>::BYTES);
-    if (e == cudaSuccess) e = cudaFuncSetAttribute (tpk_kernel<64, 32, true, false, false, false, false, false>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)TpkGeom<64, 32, true>::BYTES);
     if (e == cudaSuccess) e = cudaStreamCreateWithFlags (&h->path.own, cudaStreamNonBlocking);
     if (e == cudaSuccess) {
         // constructors: TruePeakdsp _res(true) (:29); Kmeterdsp _flag(false), all zero (kmeterdsp.cc:30-40);
