@@ -373,6 +373,36 @@ enum { B200M_DR14_RESET = 1, B200M_DR14_CLEAR = 2 };
 int b200m_dr14_control (b200m_dr14* h, const uint32_t* inst, uint32_t count, int cmd, void* stream);
 int b200m_dr14_results (b200m_dr14* h, b200m_dr14_result* out, void* stream);
 int b200m_dr14_histogram (b200m_dr14* h, uint32_t inst, uint32_t chan, uint32_t* hist8000, void* stream);   /* hist[c] (:46,309-311) */
+/* Window log (an extension; the reference keeps only the latest values), DR mode: one point per completed 3 s window of an
+ * instance (every dr14_calc_rms_score call, :285-352), silent windows included.  All fields float, in dB unless noted:
+ * - window: the windows this instance completed since its last RESET / CLEAR / creation, this one included (1, 2, ...); window k
+ *   ends after frame k * (n_sample_cnt + 1) of the instance's own frames.  Exact up to 2^24 windows.
+ * - silent: 1 if the silence gate skipped the window (:287-298): no histogram entry, the running fields unchanged; else 0.
+ * - rms: the window's RMS as the reference bins it, coeff_to_db (sqrt (2 rms_sum / n_sample_cnt)) (:306,310).  -80 for a silent
+ *   window, which is also what that formula gives for it (a window whose sum is NaN is silent too).
+ * - peak: coeff_to_db (peak_cur) handed to the second-peak pair (:338-344): the largest sample (signed maximum, as the reference)
+ *   since the previous scored window or reset.  NaN for a silent window, whose samples count towards the next scored one's peak.
+ * - m_rms, dr, dr_total, block_count: the b200m_dr14_results fields after this window, bit for bit (a window is longer than any
+ *   block, so at most one closes per block).  peak2: coeff_to_db of the second-highest window peak after this window, -81 before
+ *   3 scored windows (not the m_peak port, which is the true-peak hold).
+ * - A mono bank's channel-1 fields and dr_total are NaN.
+ * A ragged block logs a window only if it closes within the instance's len[i] frames, as it is scored.  RESET / CLEAR drop the open
+ * window (no point for it; window restarts at 1) and leave the points already logged; no control writes a point. */
+typedef struct b200m_dr14_point {
+    float window, silent;
+    float rms[2], peak[2];
+    float m_rms[2], peak2[2];
+    float dr[2], dr_total, block_count;
+} b200m_dr14_point;
+/* capacity points per instance, kept in a ring on the device; 0 turns the log off and frees it; (re)enabling empties it.
+ * B200M_E_NOMEM (the log off) if the device cannot hold 2 x capacity x n_inst points; B200M_E_UNSUPPORTED in TPnRMS mode. */
+int b200m_dr14_log_enable (b200m_dr14* h, uint32_t capacity, void* stream);
+/* the capacity the log was enabled with: the row length of b200m_dr14_log_drain's `out`; 0 while the log is off or h is NULL */
+uint32_t b200m_dr14_log_capacity (const b200m_dr14* h);
+/* host out [n_inst][capacity], count [n_inst], lost [n_inst]: instance i's points since the previous drain, oldest first, in
+ * out[i][0 .. count[i]) (NaN after them); lost[i] older unread points were overwritten.  Ordered after the work on `stream` like
+ * b200m_dr14_results (synchronises it).  B200M_E_INVAL with the log off. */
+int b200m_dr14_log_drain (b200m_dr14* h, b200m_dr14_point* out, uint32_t* count, uint64_t* lost, void* stream);
 
 /* ======================================================================================
  * Stereo correlation bank — replaces LV2M::Stcorrdsp (jmeters/stcorrdsp.h:27-55) as driven by

@@ -137,6 +137,9 @@ _PROTOS = {
     "b200m_dr14_control": (C.c_int, [_v, _v, C.c_uint32, C.c_int, _v]),
     "b200m_dr14_results": (C.c_int, [_v, _v, _v]),
     "b200m_dr14_histogram": (C.c_int, [_v, C.c_uint32, C.c_uint32, _v, _v]),
+    "b200m_dr14_log_enable": (C.c_int, [_v, C.c_uint32, _v]),
+    "b200m_dr14_log_drain": (C.c_int, [_v, _v, _v, _v, _v]),
+    "b200m_dr14_log_capacity": (C.c_uint32, [_v]),
     "b200m_cor_create": (C.c_int, [C.POINTER(_v), C.c_int, C.c_uint32, C.c_int, C.c_float, C.c_float]),
     "b200m_cor_destroy": (C.c_int, [_v]),
     "b200m_cor_process_device": (C.c_int, [_v, _v, C.c_size_t, C.c_uint32, _v]),
@@ -760,6 +763,9 @@ class SigDistHist(_StatBank):
 
 DR14_RESULT_DTYPE = np.dtype([("v_rms", "<f4", 2), ("v_peak", "<f4", 2), ("m_peak", "<f4", 2), ("m_rms", "<f4", 2), ("dr", "<f4", 2),
                               ("dr_total", "<f4"), ("block_count", "<f4")])
+# one point of the DR-14 window log (b200m_dr14_point): one completed 3 s window of an instance and the readings after it
+DR14_POINT_DTYPE = np.dtype([("window", "<f4"), ("silent", "<f4"), ("rms", "<f4", 2), ("peak", "<f4", 2), ("m_rms", "<f4", 2),
+                             ("peak2", "<f4", 2), ("dr", "<f4", 2), ("dr_total", "<f4"), ("block_count", "<f4")])
 
 
 DR14_RESET, DR14_CLEAR = 1, 2
@@ -818,6 +824,20 @@ class DR14(_Bank):
         h = np.empty(8000, np.uint32)
         _ck(lib().b200m_dr14_histogram(self.h, inst, chan, _np_ptr(h), _stream_ptr(stream)))
         return h
+
+    def log_enable(self, capacity, stream=None):
+        """keep the last `capacity` window points of every instance on the device, one per completed 3 s window, silent ones
+        included (b200m_dr14_log_enable, DR mode only); 0 turns the log off, (re)enabling empties it"""
+        _ck(lib().b200m_dr14_log_enable(self.h, int(capacity), _stream_ptr(stream)))
+
+    def log_drain(self, stream=None):
+        """the points logged since the last drain (b200m_dr14_log_drain): (points [n_inst, capacity] DR14_POINT_DTYPE, oldest first,
+        NaN past count; count uint32 [n_inst]; lost uint64 [n_inst], older points overwritten before they were drained)"""
+        cap = int(lib().b200m_dr14_log_capacity(self.h))
+        pts = np.empty((self.n_inst, max(cap, 1)), DR14_POINT_DTYPE)
+        cnt = np.empty(self.n_inst, np.uint32); lost = np.empty(self.n_inst, np.uint64)
+        _ck(lib().b200m_dr14_log_drain(self.h, _np_ptr(pts), _np_ptr(cnt), _np_ptr(lost), _stream_ptr(stream)))
+        return pts, cnt, lost
 
 
 class Spectr30(_Bank):
@@ -1142,7 +1162,12 @@ def programme_loudness(x, lengths, fsamp=48000.0, nchan=2, gains=None, block=102
     return out
 
 
-def programme_dr14(x, lengths, rate=48000.0, n_channels=2, dr_mode=True, block=1024, device=0):
+DR_CURVE_FIELDS = (("window_rms", "rms"), ("window_peak", "peak"), ("m_rms", "m_rms"), ("peak2", "peak2"), ("dr", "dr"),
+                   ("dr_total", "dr_total"), ("block_count", "block_count"))
+DR_CURVE_LOG_POINTS = 16       # the window log's capacity in programme_dr14: 48 s of windows
+
+
+def programme_dr14(x, lengths, rate=48000.0, n_channels=2, dr_mode=True, block=1024, device=0, curves=False):
     """DR-14 (dr_mode=True) or TPnRMS meter readings of N whole tracks of different lengths, in one bank.
 
     x: rows i * n_channels + c of track i, track i valid for its first lengths[i] frames: a [N * n_channels, >= max(lengths)]
@@ -1155,7 +1180,14 @@ def programme_dr14(x, lengths, rate=48000.0, n_channels=2, dr_mode=True, block=1
     window is never scored, and a track shorter than three windows reads dr 21 ("not valid").  dr_mode needs rate >= 2731 Hz
     (b200m_dr14_create: a window longer than the largest block).
     Returns a DR14_RESULT_DTYPE array of N: each track's b200m_dr14_result after its last frame (all zero for an empty track,
-    which never runs)."""
+    which never runs).
+    curves=True (DR mode only) returns (that array, curves): each track's DR curve, one point per whole 3 s window, silent ones
+    included, point k (index k - 1) ending at frame k * w of the track (w = rintf (3 * rate) + 1 frames).  curves holds n_windows
+    (int64 [N], lengths // w); window_rms, window_peak (each window's own RMS and peak), m_rms, peak2 (second-highest window peak)
+    and dr (float32 [N, W, n_channels]); dr_total and block_count (float32 [N, W]); silent (bool [N, W]), with W = max(n_windows),
+    NaN (silent False) past a track's n_windows: the b200m_dr14_point fields.  The bank's window log holds DR_CURVE_LOG_POINTS
+    points per track and is drained before it can overflow, so the device memory does not grow with the tracks; the result array
+    is the same as with curves=False."""
     ln = np.asarray(lengths, np.int64).ravel()
     n = ln.size
     if n == 0:
@@ -1164,13 +1196,44 @@ def programme_dr14(x, lengths, rate=48000.0, n_channels=2, dr_mode=True, block=1
         raise B200MError("lengths must be frame counts >= 0")
     if not 1 <= int(block) <= 8192:
         raise B200MError("block must be 1..8192 frames")
+    if curves and not dr_mode:
+        raise B200MError("DR curves need dr_mode (a TPnRMS bank has no 3 s windows)")
     bank = DR14(n, n_channels, rate, dr_mode, device)
     try:
         total = int(ln.max())
-        for off in range(0, total, int(block)):
+        if curves:
+            w = int(np.rint(np.float32(rate * 3.0))) + 1
+            n_windows = ln // w
+            nw = int(n_windows.max())
+            cv = {k: np.full((n, nw, n_channels), np.nan, np.float32) for k, _ in DR_CURVE_FIELDS[:5]}
+            cv.update({k: np.full((n, nw), np.nan, np.float32) for k, _ in DR_CURVE_FIELDS[5:]})
+            silent = np.zeros((n, nw), bool)
+            bank.log_enable(DR_CURVE_LOG_POINTS)
+            # k blocks of `block` frames close at most (k * block - 1) // w + 1 windows of a track: no more than the log holds
+            # while k * block <= DR_CURVE_LOG_POINTS * w
+            drain_every = DR_CURVE_LOG_POINTS * w // int(block)
+
+            def drain():
+                pts, cnt, lost = bank.log_drain()
+                if lost.any():
+                    raise B200MError("window log overflow: %d points lost" % int(lost.sum()))
+                i, j = np.nonzero(np.arange(pts.shape[1]) < cnt[:, None].astype(np.int64))
+                k = pts["window"][i, j].astype(np.int64) - 1
+                for name, f in DR_CURVE_FIELDS:
+                    v = pts[f][i, j]
+                    cv[name][i, k] = v[:, :n_channels] if v.ndim == 2 else v
+                silent[i, k] = pts["silent"][i, j] != 0
+        for b, off in enumerate(range(0, total, int(block))):
             nfram = min(int(block), total - off)
             xb = x(off, nfram) if callable(x) else x[:, off:off + nfram]
             bank.run(xb, lengths=np.clip(ln - off, 0, nfram))
+            if curves and (b + 1) % drain_every == 0:
+                drain()
+        if curves:
+            drain()
+            cv["n_windows"] = n_windows
+            cv["silent"] = silent
+            return bank.results(), cv
         return bank.results()
     finally:
         bank.close()

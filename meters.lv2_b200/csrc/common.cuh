@@ -129,6 +129,38 @@ struct BankPath {
 
 inline int no_check () { return 0; }
 
+// The point log of a bank (the EBU R128 loudness log, the DR-14 window log): one point of NF floats per completed fragment or window
+// of an instance, `cap` points per instance in a ring on the device.  Field f of point slot s of instance i is
+// pts[(f * cap + s) * n_inst + i] (planes [NF][cap][n_inst]: lane = instance stores coalesce); written[i] counts the instance's
+// points, the next goes to slot written[i] % cap.  pts == nullptr: the log is off.
+struct PointLog { float* pts; unsigned long long* written; uint32_t cap; };
+
+// The host side of a point log: the planes and counters the bank's kernels update, the read cursors, and the drain's device output
+// (points, counts, lost counts).
+struct PointRing {
+    PointLog log = {nullptr, nullptr, 0};
+    unsigned long long *rd = nullptr, *lost = nullptr; float* out = nullptr; uint32_t* cnt = nullptr;
+    // an empty log of cap points of nf floats for each of n instances, emptied on st; on an error nothing stays allocated
+    cudaError_t alloc (size_t n, uint32_t cap, size_t nf, cudaStream_t st) {
+        const size_t pts = (size_t)cap * n * nf * sizeof (float);
+        log.cap = cap;
+        cudaError_t e = cudaMalloc ((void**)&log.pts, pts);
+        if (e == cudaSuccess) e = cudaMalloc ((void**)&log.written, n * sizeof (unsigned long long));
+        if (e == cudaSuccess) e = cudaMalloc ((void**)&rd, n * sizeof (unsigned long long));
+        if (e == cudaSuccess) e = cudaMalloc ((void**)&lost, n * sizeof (unsigned long long));
+        if (e == cudaSuccess) e = cudaMalloc ((void**)&cnt, n * sizeof (uint32_t));
+        if (e == cudaSuccess) e = cudaMalloc ((void**)&out, pts);
+        if (e == cudaSuccess) e = cudaMemsetAsync (log.written, 0, n * sizeof (unsigned long long), st);
+        if (e == cudaSuccess) e = cudaMemsetAsync (rd, 0, n * sizeof (unsigned long long), st);
+        if (e != cudaSuccess) release ();
+        return e;
+    }
+    void release () {
+        cudaFree (log.pts); cudaFree (log.written); cudaFree (rd); cudaFree (lost); cudaFree (out); cudaFree (cnt);
+        log = {nullptr, nullptr, 0}; rd = lost = nullptr; out = nullptr; cnt = nullptr;
+    }
+};
+
 // One block call of a bank: the body of every *_process_* / *_run_* entry point, plain, _ctl_ and ragged, on both paths.  In order:
 // the block arguments; the bank's own check () (0 or an error); the n_len lengths `len` (NULL: every row runs nfram); the device,
 // the path switch and, on the host path, the staging copy of `rows` rows onto own (rows == 0: the bank copies the block itself).
@@ -230,6 +262,74 @@ B200M_DEV float log10f_glibc (float x)
     float y = (float)(k + i);
     float z = __fadd_rn (__fmul_rn (y, log10_2lo), __fmul_rn (ivln10, logf_glibc_normal (__int_as_float (hx))));
     return __fadd_rn (z, __fmul_rn (y, log10_2hi));
+}
+
+// ---- drain of a point log (PointLog) ---------------------------------------------------
+// Per instance the points written since the last drain, oldest first, at most cap of them, into out[n_inst][cap][NF] (NaN past the
+// instance's count), with count[i] and lost[i] (unread points overwritten before this drain); then the read cursor moves to
+// written[i].  A CTA owns 32 instances and walks their points in tiles of PTS: lane = instance reads the planes, a shared-memory
+// transpose makes the stores of the [cap][NF] rows coalesce.  The static tile is 32 x (PTS * NF + 1) floats, under 48 KB: PTS = 32
+// up to NF = 11, PTS = 16 up to NF = 23.
+constexpr int LOG_DRAIN_ROWS = 8;
+
+template <int NF, int PTS>
+__global__ void __launch_bounds__ (32 * LOG_DRAIN_ROWS)
+log_drain_kernel (int n_inst, PointLog lg, unsigned long long* __restrict__ rd, float* __restrict__ out, uint32_t* __restrict__ count,
+                  unsigned long long* __restrict__ lost)
+{
+    __shared__ float tile[32][PTS * NF + 1];
+    const int tx = threadIdx.x & 31, ty = threadIdx.x >> 5;
+    const int i0 = blockIdx.x * 32, i = i0 + tx;
+    const uint32_t cap = lg.cap;
+    const size_t pl = (size_t)cap * n_inst;
+    unsigned long long w = 0, start = 0;
+    uint32_t cnt = 0;
+    if (i < n_inst) {
+        w = lg.written[i];
+        const unsigned long long unread = w - rd[i];
+        cnt = unread < cap ? (uint32_t)unread : cap;
+        start = w - cnt;
+        if (ty == 0) { count[i] = cnt; lost[i] = unread - cnt; }
+    }
+    for (uint32_t j0 = 0; j0 < cap; j0 += PTS) {
+        for (int jl = ty; jl < PTS; jl += LOG_DRAIN_ROWS) {
+            const uint32_t j = j0 + jl;
+            float v[NF];
+            if (i < n_inst && j < cnt) {
+                const float* p = lg.pts + (size_t)((start + j) % cap) * n_inst + i;
+#pragma unroll
+                for (int f = 0; f < NF; ++f) v[f] = p[f * pl];
+            } else {
+#pragma unroll
+                for (int f = 0; f < NF; ++f) v[f] = __int_as_float (0x7fc00000);
+            }
+#pragma unroll
+            for (int f = 0; f < NF; ++f) tile[tx][jl * NF + f] = v[f];
+        }
+        __syncthreads ();
+        const int nq = (int)min ((uint32_t)PTS, cap - j0) * NF;      // the tile's floats of one instance's row, contiguous in out
+        for (int il = ty; il < 32 && i0 + il < n_inst; il += LOG_DRAIN_ROWS) {
+            float* o = out + ((size_t)(i0 + il) * cap + j0) * NF;
+            for (int q = tx; q < nq; q += 32) o[q] = tile[il][q];
+        }
+        __syncthreads ();
+    }
+    if (i < n_inst && ty == 0) rd[i] = w;
+}
+
+// b200m_*_log_drain of n instances on st: the drain kernel, the copies of its output into the host arrays out [n][cap][NF],
+// count [n] and lost [n], and the wait for them
+template <int NF, int PTS>
+int log_drain (PointRing& r, size_t n, float* out, uint32_t* count, uint64_t* lost, cudaStream_t st)
+{
+    log_drain_kernel<NF, PTS><<<(unsigned)((n + 31) / 32), 32 * LOG_DRAIN_ROWS, 0, st>>> ((int)n, r.log, r.rd, r.out, r.cnt, r.lost);
+    B200M_LAUNCHED (1);
+    B200M_CUDA (cudaGetLastError ());
+    B200M_CUDA (cudaMemcpyAsync (out, r.out, n * r.log.cap * NF * sizeof (float), cudaMemcpyDeviceToHost, st));
+    B200M_CUDA (cudaMemcpyAsync (count, r.cnt, n * sizeof (uint32_t), cudaMemcpyDeviceToHost, st));
+    B200M_CUDA (cudaMemcpyAsync (lost, r.lost, n * sizeof (uint64_t), cudaMemcpyDeviceToHost, st));
+    B200M_CUDA (cudaStreamSynchronize (st));
+    return 0;
 }
 #endif  // __CUDACC__
 

@@ -41,14 +41,70 @@ struct Dr14State {
     float *peak_hist, *m_rms, *m_peak, *m_dbtp;                // per channel (peak_hist: 2 per channel)
     unsigned long long* numfrag;                               // per instance
     uint32_t* phase;                                           // per instance: bank time of its last reset_peaks, mod the window length
+    uint32_t* nwin;                                            // per instance: windows completed since its last reset_peaks (the window log's count)
     uint32_t* hist;                                            // [n_ch][8000]
     const float* cd;                                           // db_to_coeff ((b - 7999) / 100.0) for b = 0..7999, host libm
 };
 
-// dr14_calc_rms_score (:285-352) of the instances whose window closed in this block; one warp per instance.
+// The DR ports (:436-458) of an instance from its channels' top-20 % RMS scores m_rms and second-highest window peaks m_peak (dB):
+// dr[c] = MIN (0, m_peak) - m_rms clamped to 1..20 (21: not yet valid), dr_total their average over the valid channels, clamped
+// alike (21: none valid).  dr[1] is not written for a mono instance.
+struct DrPorts { float dr[2], dr_total; };
+
+B200M_DEV DrPorts dr_ports (const float* m_rms, const float* m_peak, int nch)
+{
+    DrPorts o;
+    float dr_total = 0.0f; int dr_valid = 0;
+#pragma unroll
+    for (int c = 0; c < 2 && c < nch; ++c) {                  // unrolled: o stays in registers
+        const float rdb = m_rms[c], pdb = m_peak[c];
+        const float dr = __fsub_rn (0.0f < pdb ? 0.0f : pdb, rdb);                     // MIN (0, pdb) - rdb
+        const bool ok = rdb > -80.0f && pdb > -80.0f;
+        if (ok) { dr_total = __fadd_rn (dr_total, dr); ++dr_valid; }
+        const float lo = 20.0f < dr ? 20.0f : dr;                                       // MAX (1, MIN (20, dr))
+        o.dr[c] = ok ? (1.0f > lo ? 1.0f : lo) : 21.0f;
+    }
+    if (dr_valid > 0) { const float a = __fdiv_rn (dr_total, (float)dr_valid); const float lo = 20.0f < a ? 20.0f : a; o.dr_total = 1.0f > lo ? 1.0f : lo; }
+    else o.dr_total = 21.0f;
+    return o;
+}
+
+B200M_DEV float dr_block_count (unsigned long long num_fragments)      // 3.0 * num_fragments (:460)
+{
+    return __double2float_rn (__dmul_rn (3.0, (double)num_fragments));
+}
+
+// The window log (b200m_dr14_log_enable): a PointLog (common.cuh) of one b200m_dr14_point per completed 3 s window of an instance,
+// planes [14][cap][n_inst] in the struct's field order.
+constexpr int DR_LOG_FIELDS = 14;
+static_assert (sizeof (b200m_dr14_point) == DR_LOG_FIELDS * sizeof (float), "b200m_dr14_point is 14 floats");
+
+// Append instance inst's point for its window number win: rms / peak that window's own values per channel (dB), every other field
+// from the instance's state after the window.  A mono instance's channel-1 fields and dr_total are NaN.
+B200M_DEV void dr14_log_point (const PointLog& lg, int n_inst, int inst, int nch, const Dr14State& s, uint32_t win, bool silent,
+                               float rms0, float rms1, float peak0, float peak1)
+{
+    const float nan = __int_as_float (0x7fc00000);
+    const int ch0 = inst * nch;
+    const DrPorts d = dr_ports (s.m_rms + ch0, s.m_peak + ch0, nch);
+    const unsigned long long w = lg.written[inst];
+    const size_t pl = (size_t)lg.cap * n_inst;
+    float* p = lg.pts + (size_t)(w % lg.cap) * n_inst + inst;
+    p[0] = (float)win;                                         // exact up to 2^24 windows
+    p[pl] = silent ? 1.0f : 0.0f;
+    p[2 * pl] = rms0; p[4 * pl] = peak0; p[6 * pl] = s.m_rms[ch0]; p[8 * pl] = s.m_peak[ch0]; p[10 * pl] = d.dr[0];
+    if (nch > 1) { p[3 * pl] = rms1; p[5 * pl] = peak1; p[7 * pl] = s.m_rms[ch0 + 1]; p[9 * pl] = s.m_peak[ch0 + 1]; p[11 * pl] = d.dr[1]; p[12 * pl] = d.dr_total; }
+    else { p[3 * pl] = nan; p[5 * pl] = nan; p[7 * pl] = nan; p[9 * pl] = nan; p[11 * pl] = nan; p[12 * pl] = nan; }
+    p[13 * pl] = dr_block_count (s.numfrag[inst]);
+    lg.written[inst] = w + 1;
+}
+
+// dr14_calc_rms_score (:285-352) of the instances whose window closed in this block; one warp per instance.  With the window log
+// on (lg.pts), lane 0 also appends the window's point.
 // RAG: a ragged block, instance i ran over its first rlen[i] frames: its window closed only if the cut lies before that.
 template <bool RAG = false>
-__global__ void dr14_score_kernel (int n_inst, int nch, float n_sample_cnt_f, Dr14State s, TpkDr dr, int nfram, const uint32_t* __restrict__ rlen)
+__global__ void dr14_score_kernel (int n_inst, int nch, float n_sample_cnt_f, Dr14State s, TpkDr dr, int nfram, const uint32_t* __restrict__ rlen,
+                                   PointLog lg)
 {
     const int inst = (blockIdx.x * blockDim.x + threadIdx.x) >> 5, lane = threadIdx.x & 31;
     if (inst >= n_inst) return;
@@ -56,19 +112,30 @@ __global__ void dr14_score_kernel (int n_inst, int nch, float n_sample_cnt_f, Dr
     const int cut = tpk_dr_cut (dr, inst, nfram);
     if (cut < 0) return;                                       // no window end in this block: emit_* still hold an older window's
     if (RAG && cut >= (int)rlen[inst]) return;                 // ... or none before the instance's last frame
-    if (!s.emit_valid[ch0]) return;                            // silent window: nothing recorded (:287-297)
+    uint32_t win = 0;                                          // counted with the log off too: a log enabled later numbers windows alike
+    if (lane == 0) { win = s.nwin[inst] + 1; s.nwin[inst] = win; }
+    const float nan = __int_as_float (0x7fc00000);
+    if (!s.emit_valid[ch0]) {                                  // silent window: nothing recorded (:287-297)
+        // its RMS is logged as -80: what coeff_to_db gives for the RMS below 1e-4 that a sum <= 1e-9 n_sample_cnt means, and the
+        // value for a window gated because its sum is NaN too.  Its peak is NaN: peak_cur carries on into the next window (:293-296).
+        if (lg.pts && lane == 0) dr14_log_point (lg, n_inst, inst, nch, s, win, true, -80.0f, -80.0f, nan, nan);
+        return;
+    }
     unsigned long long nf = 0;
     if (lane == 0) { nf = s.numfrag[inst] + 1; s.numfrag[inst] = nf; }
     nf = __shfl_sync (0xffffffffu, nf, 0);
     const float mc = floorf (__double2float_rn (__ddiv_rn ((double)nf, 5.0)));      // MAX (1, floorf (num_fragments / 5.0)) (:301)
     const uint32_t m_cut = (uint32_t)(1.0f > mc ? 1.0f : mc);
+    float wrms[2] = {nan, nan}, wpeak[2] = {nan, nan};         // lane 0: the window's own RMS and peak per channel, for the log
     for (int c = 0; c < nch; ++c) {
         const int ch = ch0 + c;
         uint32_t* hist = s.hist + (size_t)ch * DR_HISTBINS;
         if (lane == 0) {
             const float q = __fdiv_rn (__fmul_rn (2.0f, s.emit_rms[ch]), n_sample_cnt_f);
             const float rms = __double2float_rn (__dsqrt_rn ((double)q));                   // sqrt () in double (:304)
-            int bin = dr_f2i (__fsub_rn (rintf (__fmul_rn (100.0f, __fadd_rn (80.0f, dr_coeff_to_db (rms)))), 1.0f));   // (int)(rintf (..) - 1): float subtraction (:308)
+            const float rdb = dr_coeff_to_db (rms);
+            if (c == 0) wrms[0] = rdb; else wrms[1] = rdb;
+            int bin = dr_f2i (__fsub_rn (rintf (__fmul_rn (100.0f, __fadd_rn (80.0f, rdb))), 1.0f));   // (int)(rintf (..) - 1): float subtraction (:308)
             if (bin >= DR_HISTBINS) bin = DR_HISTBINS - 1;
             if (bin > 0) hist[bin] += 1;
         }
@@ -92,6 +159,7 @@ __global__ void dr14_score_kernel (int n_inst, int nch, float n_sample_cnt_f, Dr
         if (lane == 0) {
             s.m_rms[ch] = n_cut > 0 ? dr_coeff_to_db (__fsqrt_rn (__fdiv_rn (rms_score, (float)n_cut))) : -81.0f;
             const float pc = s.emit_peak[ch];                  // second highest window peak (:339-351)
+            if (c == 0) wpeak[0] = pc; else wpeak[1] = pc;
             float h0 = s.peak_hist[2 * ch], h1 = s.peak_hist[2 * ch + 1];
             if (pc >= h0) { h1 = h0; h0 = pc; } else if (pc > h1) h1 = pc;
             s.peak_hist[2 * ch] = h0; s.peak_hist[2 * ch + 1] = h1;
@@ -99,6 +167,8 @@ __global__ void dr14_score_kernel (int n_inst, int nch, float n_sample_cnt_f, Dr
         }
         __syncwarp ();
     }
+    if (lg.pts && lane == 0)
+        dr14_log_point (lg, n_inst, inst, nch, s, win, false, wrms[0], wrms[1], dr_coeff_to_db (wpeak[0]), nch > 1 ? dr_coeff_to_db (wpeak[1]) : nan);
 }
 
 // read() results -> port values (:418-462); one thread per instance.  RAG: an instance with rlen 0 did not run (row and hold stay).
@@ -111,7 +181,6 @@ __global__ void dr14_ports_kernel (int n_inst, int nch, int dr_mode, const b200m
     if (RAG && rlen[inst] == 0) return;
     b200m_dr14_result o;
     memset (&o, 0, sizeof (o));
-    float dr_total = 0.0f; int dr_valid = 0;
     for (int c = 0; c < nch; ++c) {
         const int ch = inst * nch + c;
         const b200m_tpk_result r = res[ch];
@@ -120,21 +189,14 @@ __global__ void dr14_ports_kernel (int n_inst, int nch, int dr_mode, const b200m
         o.v_rms[c] = dr_coeff_to_db (r.km_rms);
         o.v_peak[c] = dr_coeff_to_db (r.tp_m);
         o.m_peak[c] = dr_coeff_to_db (hold);
-        if (dr_mode) {
-            const float rdb = s.m_rms[ch], pdb = s.m_peak[ch];
-            const float dr = __fsub_rn (0.0f < pdb ? 0.0f : pdb, rdb);                 // MIN (0, pdb) - rdb
-            const bool ok = rdb > -80.0f && pdb > -80.0f;
-            if (ok) { dr_total = __fadd_rn (dr_total, dr); ++dr_valid; }
-            const float lo = 20.0f < dr ? 20.0f : dr;                                   // MAX (1, MIN (20, dr))
-            o.dr[c] = ok ? (1.0f > lo ? 1.0f : lo) : 21.0f;
-            o.m_rms[c] = rdb;
-        } else o.m_rms[c] = dr_coeff_to_db (r.km_peak);
+        o.m_rms[c] = dr_mode ? s.m_rms[ch] : dr_coeff_to_db (r.km_peak);
     }
-    if (nch > 1 && dr_mode) {
-        if (dr_valid > 0) { const float a = __fdiv_rn (dr_total, (float)dr_valid); const float lo = 20.0f < a ? 20.0f : a; o.dr_total = 1.0f > lo ? 1.0f : lo; }
-        else o.dr_total = 21.0f;
+    if (dr_mode) {
+        const DrPorts d = dr_ports (s.m_rms + inst * nch, s.m_peak + inst * nch, nch);
+        o.dr[0] = d.dr[0];
+        if (nch > 1) { o.dr[1] = d.dr[1]; o.dr_total = d.dr_total; }
     }
-    o.block_count = __double2float_rn (__dmul_rn (3.0, (double)s.numfrag[inst]));     // 3.0 * num_fragments
+    o.block_count = dr_block_count (s.numfrag[inst]);
     out[inst] = o;
 }
 
@@ -153,7 +215,7 @@ __global__ void dr14_reset_kernel (const uint32_t* inst, size_t n_sel, int nch, 
     const size_t t = (size_t)blockIdx.x * blockDim.x + threadIdx.x, n_ch = n_sel * nch;
     auto chan = [&] (size_t k) { return inst ? (size_t)inst[k / nch] * nch + k % nch : k; };
     if (t < n_ch) { const size_t i = chan (t); s.m_peak[i] = -81.0f; s.m_rms[i] = -81.0f; s.m_dbtp[i] = 0.0f; rms_sum[i] = 0.0f; peak_cur[i] = 0.0f; s.peak_hist[2 * i] = 0.0f; s.peak_hist[2 * i + 1] = 0.0f; s.emit_valid[i] = 0; }
-    if (t < n_sel) { const size_t j = inst ? inst[t] : t; s.numfrag[j] = 0; s.phase[j] = tmod; }
+    if (t < n_sel) { const size_t j = inst ? inst[t] : t; s.numfrag[j] = 0; s.nwin[j] = 0; s.phase[j] = tmod; }
     if (dr_mode)
         for (size_t k = t; k < n_ch * DR_HISTBINS; k += (size_t)gridDim.x * blockDim.x) {
             if (!inst) { s.hist[k] = 0; continue; }
@@ -176,6 +238,7 @@ struct b200m_dr14 {
     uint32_t* d_sel = nullptr;                                 // instance list of a control call
     float *d_rms_sum = nullptr, *d_peak_cur = nullptr, *d_cd = nullptr;
     Dr14State st{}; b200m_dr14_result* d_out = nullptr;
+    PointRing ring;                                            // the window log (b200m_dr14_log_enable), off while ring.log.pts is null
     BankPath path;
 };
 
@@ -228,8 +291,8 @@ static int dr14_run (b200m_dr14* h, const float* d_in, size_t stride, uint32_t n
     if (rc) return rc;
     const unsigned gs = (h->n_inst * 32 + 127) / 128, gp = (h->n_inst + 127) / 128;
     if (closes) {
-        if (len) dr14_score_kernel<true><<<gs, 128, 0, st>>> ((int)h->n_inst, (int)h->nch, (float)h->n_sample_cnt, h->st, dr, (int)nfram, d_len);
-        else dr14_score_kernel<<<gs, 128, 0, st>>> ((int)h->n_inst, (int)h->nch, (float)h->n_sample_cnt, h->st, dr, (int)nfram, nullptr);
+        if (len) dr14_score_kernel<true><<<gs, 128, 0, st>>> ((int)h->n_inst, (int)h->nch, (float)h->n_sample_cnt, h->st, dr, (int)nfram, d_len, h->ring.log);
+        else dr14_score_kernel<<<gs, 128, 0, st>>> ((int)h->n_inst, (int)h->nch, (float)h->n_sample_cnt, h->st, dr, (int)nfram, nullptr, h->ring.log);
         B200M_LAUNCHED (1);
     }
     if ((rc = len ? tpk_read_ragged (h->tpk, st, d_len, h->nch) : b200m_tpk_read_device (h->tpk, st))) return rc;
@@ -272,7 +335,7 @@ int b200m_dr14_create (b200m_dr14** out, int device, uint32_t n_inst, uint32_t n
     A ((void**)&h->d_rms_sum, n_ch * 4); A ((void**)&h->d_peak_cur, n_ch * 4);
     A ((void**)&h->st.emit_rms, n_ch * 4); A ((void**)&h->st.emit_peak, n_ch * 4); A ((void**)&h->st.emit_valid, n_ch * 4);
     A ((void**)&h->st.peak_hist, n_ch * 8); A ((void**)&h->st.m_rms, n_ch * 4); A ((void**)&h->st.m_peak, n_ch * 4); A ((void**)&h->st.m_dbtp, n_ch * 4);
-    A ((void**)&h->st.numfrag, (size_t)n_inst * 8); A ((void**)&h->st.phase, (size_t)n_inst * 4); A ((void**)&h->d_sel, (size_t)n_inst * 4);
+    A ((void**)&h->st.numfrag, (size_t)n_inst * 8); A ((void**)&h->st.phase, (size_t)n_inst * 4); A ((void**)&h->st.nwin, (size_t)n_inst * 4); A ((void**)&h->d_sel, (size_t)n_inst * 4);
     if (h->dr_mode) A ((void**)&h->st.hist, n_ch * DR_HISTBINS * 4);
     A ((void**)&h->d_cd, DR_HISTBINS * 4); A ((void**)&h->d_out, (size_t)n_inst * sizeof (b200m_dr14_result));
     if (e == cudaSuccess) {
@@ -304,8 +367,9 @@ int b200m_dr14_destroy (b200m_dr14* h)
     DeviceGuard g (h->device);
     cudaDeviceSynchronize ();
     void* ps[] = {h->d_rms_sum, h->d_peak_cur, h->st.emit_rms, h->st.emit_peak, h->st.emit_valid, h->st.peak_hist, h->st.m_rms, h->st.m_peak,
-                  h->st.m_dbtp, h->st.numfrag, h->st.phase, h->d_sel, h->st.hist, h->d_cd, h->d_out};
+                  h->st.m_dbtp, h->st.numfrag, h->st.phase, h->st.nwin, h->d_sel, h->st.hist, h->d_cd, h->d_out};
     for (void* p : ps) cudaFree (p);
+    h->ring.release ();
     h->path.release ();
     delete h;
     return 0;
@@ -385,6 +449,40 @@ int b200m_dr14_histogram (b200m_dr14* h, uint32_t inst, uint32_t chan, uint32_t*
     B200M_CUDA (cudaMemcpyAsync (hist8000, h->st.hist + ((size_t)inst * h->nch + chan) * DR_HISTBINS, DR_HISTBINS * 4, cudaMemcpyDeviceToHost, st));
     B200M_CUDA (cudaStreamSynchronize (st));
     return 0;
+}
+
+int b200m_dr14_log_enable (b200m_dr14* h, uint32_t capacity, void* stream)
+{
+    if (!h) return set_err (B200M_E_INVAL, "NULL handle");
+    if (!h->dr_mode) return set_err (B200M_E_UNSUPPORTED, "a TPnRMS bank has no 3 s windows to log");
+    DeviceGuard g (h->device);
+    cudaStream_t st = h->path.stream (stream);
+    if (h->ring.log.pts) {                                     // kernels in flight may still write the old log
+        B200M_CUDA (cudaStreamSynchronize (st));
+        h->ring.release ();
+    }
+    if (capacity == 0) return 0;
+    const cudaError_t e = h->ring.alloc (h->n_inst, capacity, DR_LOG_FIELDS, st);
+    if (e != cudaSuccess) {
+        cudaGetLastError ();                                   // a failed allocation is not sticky: later calls must not see it
+        if (e == cudaErrorMemoryAllocation) return set_err (B200M_E_NOMEM, "window log of %u points x %u instances: out of device memory", capacity, h->n_inst);
+        return cuda_fail (e, "b200m_dr14_log_enable", __FILE__, __LINE__);
+    }
+    return 0;
+}
+
+uint32_t b200m_dr14_log_capacity (const b200m_dr14* h)
+{
+    return h ? h->ring.log.cap : 0;
+}
+
+int b200m_dr14_log_drain (b200m_dr14* h, b200m_dr14_point* out, uint32_t* count, uint64_t* lost, void* stream)
+{
+    if (!h || !out || !count || !lost) return set_err (B200M_E_INVAL, "NULL argument");
+    if (!h->ring.log.pts) return set_err (B200M_E_INVAL, "the window log is off (b200m_dr14_log_enable)");
+    DeviceGuard g (h->device);
+    // 16 points per tile: the drain's static tile of 32 x (16 x 14 + 1) floats stays under 48 KB
+    return log_drain<DR_LOG_FIELDS, 16> (h->ring, h->n_inst, (float*)out, count, lost, h->path.stream (stream));
 }
 
 }  // extern "C"

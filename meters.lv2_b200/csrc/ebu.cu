@@ -473,7 +473,7 @@ B200M_DEV void hist_calc_range (const int* row, int count, const float* bp, int 
     v1 = __fdiv_rn ((float)(j - 699), 10.0f);
 }
 
-// The loudness log (EbuLog, ebu_kw.cuh): K2a writes a point's five loudness fields, K2b rewrites three of them after it gates.
+// The loudness log (a PointLog, common.cuh): K2a writes a point's five loudness fields, K2b rewrites three of them after it gates.
 
 // K2a: one THREAD per instance, one completed 50 ms fragment (process :217-243 minus the gated statistics).
 // ring layout [64][n_inst] so that lane = instance accesses coalesce; each thread parks its 64-slot ring column
@@ -486,7 +486,7 @@ constexpr int K2A_THREADS = 128;
 __global__ void __launch_bounds__ (K2A_THREADS)
 ebu_fragment_kernel (int n_inst, int frag, const int* __restrict__ fph, int tmod, int fragm, int nfram, const float* __restrict__ fragpw,
                      float* __restrict__ ring, EbuCtl* __restrict__ ctl, b200m_ebu_result* __restrict__ res, int* __restrict__ histM,
-                     int* __restrict__ histS, int* __restrict__ cnt, const uint32_t* __restrict__ rlen, EbuLog lg)
+                     int* __restrict__ histS, int* __restrict__ cnt, const uint32_t* __restrict__ rlen, PointLog lg)
 {
     __shared__ float sring[64][K2A_THREADS];
     const int tid = threadIdx.x;
@@ -562,7 +562,7 @@ constexpr int K2B_WARPS = 4;
 
 __global__ void __launch_bounds__ (K2B_WARPS * 32)
 ebu_gate_kernel (int n_inst, EbuCtl* __restrict__ ctl, b200m_ebu_result* __restrict__ res, const int* histM,
-                 const int* histS, const int* __restrict__ cnt, const float* __restrict__ bin_power, EbuLog lg)
+                 const int* histS, const int* __restrict__ cnt, const float* __restrict__ bin_power, PointLog lg)
 {
     __shared__ float sbp[100];
     for (int q = threadIdx.x; q < 100; q += blockDim.x) sbp[q] = bin_power[q];
@@ -587,58 +587,6 @@ ebu_gate_kernel (int n_inst, EbuCtl* __restrict__ ctl, b200m_ebu_result* __restr
             p[2 * pl] = vi; p[3 * pl] = v0; p[4 * pl] = v1;
         }
     }
-}
-
-// Drain of the loudness log: per instance the points written since the last drain, oldest first, at most cap of them, into
-// out[n_inst][cap][NF] (NaN past the instance's count), with count[i] and lost[i] (unread points overwritten before this drain);
-// then the read cursor moves to written[i].  A CTA owns 32 instances and walks their points in tiles of 32: lane = instance reads
-// the planes, a shared-memory transpose makes the stores of the [cap][NF] rows coalesce.  NF = 5: the loudness fields; 6: the
-// dBTP plane too.
-constexpr int LOG_DRAIN_ROWS = 8;
-
-template <int NF>
-__global__ void __launch_bounds__ (32 * LOG_DRAIN_ROWS)
-ebu_log_drain_kernel (int n_inst, EbuLog lg, unsigned long long* __restrict__ rd, float* __restrict__ out, uint32_t* __restrict__ count,
-                      unsigned long long* __restrict__ lost)
-{
-    __shared__ float tile[32][32 * NF + 1];
-    const int tx = threadIdx.x & 31, ty = threadIdx.x >> 5;
-    const int i0 = blockIdx.x * 32, i = i0 + tx;
-    const uint32_t cap = lg.cap;
-    const size_t pl = (size_t)cap * n_inst;
-    unsigned long long w = 0, start = 0;
-    uint32_t cnt = 0;
-    if (i < n_inst) {
-        w = lg.written[i];
-        const unsigned long long unread = w - rd[i];
-        cnt = unread < cap ? (uint32_t)unread : cap;
-        start = w - cnt;
-        if (ty == 0) { count[i] = cnt; lost[i] = unread - cnt; }
-    }
-    for (uint32_t j0 = 0; j0 < cap; j0 += 32) {
-        for (int jl = ty; jl < 32; jl += LOG_DRAIN_ROWS) {
-            const uint32_t j = j0 + jl;
-            float v[NF];
-            if (i < n_inst && j < cnt) {
-                const float* p = lg.pts + (size_t)((start + j) % cap) * n_inst + i;
-#pragma unroll
-                for (int f = 0; f < NF; ++f) v[f] = p[f * pl];
-            } else {
-#pragma unroll
-                for (int f = 0; f < NF; ++f) v[f] = __int_as_float (0x7fc00000);
-            }
-#pragma unroll
-            for (int f = 0; f < NF; ++f) tile[tx][jl * NF + f] = v[f];
-        }
-        __syncthreads ();
-        const int nq = (int)min (32u, cap - j0) * NF;        // the tile's floats of one instance's row, contiguous in out
-        for (int il = ty; il < 32 && i0 + il < n_inst; il += LOG_DRAIN_ROWS) {
-            float* o = out + ((size_t)(i0 + il) * cap + j0) * NF;
-            for (int q = tx; q < nq; q += 32) o[q] = tile[il][q];
-        }
-        __syncthreads ();
-    }
-    if (i < n_inst && ty == 0) rd[i] = w;
 }
 
 // a ragged block moves every instance's clock on by its own length, not by the block's nfram: its phase (the bank time at which
@@ -759,15 +707,12 @@ struct b200m_ebu {
     float *d_z = nullptr, *d_frpwr = nullptr, *d_fragpw = nullptr, *d_ring = nullptr, *d_binpow = nullptr, *d_out5 = nullptr;
     EbuCtl* d_ctl = nullptr; b200m_ebu_result* d_res = nullptr;
     int *d_histM = nullptr, *d_histS = nullptr, *d_cnt = nullptr, *d_fph = nullptr;
-    // the loudness log (b200m_ebu_log_enable), off while log.pts is null: the planes and written counters K2a / K2b update, the read
-    // cursors, and the drain's device output (points, counts, lost counts)
-    EbuLog log = {nullptr, nullptr, 0};
-    unsigned long long *d_log_rd = nullptr, *d_log_lost = nullptr; float* d_log_out = nullptr; uint32_t* d_log_cnt = nullptr;
+    // the loudness log (b200m_ebu_log_enable), off while ring.log.pts is null: the planes and written counters K2a / K2b update
+    PointRing ring;
     // the log's dBTP plane (b200m_r128_log_enable), off while tp.fmax is null
     EbuTpPlane tp = {};
     void log_free () {
-        cudaFree (log.pts); cudaFree (log.written); cudaFree (d_log_rd); cudaFree (d_log_lost); cudaFree (d_log_out); cudaFree (d_log_cnt);
-        log = {nullptr, nullptr, 0}; d_log_rd = d_log_lost = nullptr; d_log_out = nullptr; d_log_cnt = nullptr;
+        ring.release ();
         cudaFree (tp.fmax); cudaFree (tp.fph0); cudaFree (tp.open); cudaFree (tp.filled);
         tp = {};
     }
@@ -1170,7 +1115,7 @@ int ebu_process_sliced (b200m_ebu* h, const float* d_in, size_t stride, uint32_t
         if (after_k1 && done == 0) { if (int rc = after_k1 (after_arg)) return rc; }      // work to enqueue right behind the first K1
         for (int f = 0; f < nfrag; ++f) {                    // fragments complete in order; each may trigger gating
             ebu_fragment_kernel<<<(h->n_inst + K2A_THREADS - 1) / K2A_THREADS, K2A_THREADS, 0, st>>> (
-                (int)h->n_inst, f, ck.fph, h->tmod, h->fragm, (int)nfram, h->d_fragpw, h->d_ring, h->d_ctl, h->d_res, h->d_histM, h->d_histS, h->d_cnt, d_len, h->log);
+                (int)h->n_inst, f, ck.fph, h->tmod, h->fragm, (int)nfram, h->d_fragpw, h->d_ring, h->d_ctl, h->d_res, h->d_histM, h->d_histS, h->d_cnt, d_len, h->ring.log);
             B200M_LAUNCHED (1);
             // K2b behind fragment f only if some class completing its fragment f has an integrating member whose S period wraps
             // there: a later addpoint in the same block would otherwise be gated into the statistics
@@ -1183,7 +1128,7 @@ int ebu_process_sliced (b200m_ebu* h, const float* d_in, size_t stride, uint32_t
             if (d_len) wrap |= h->ragged_tick (f);
             if (wrap) {
                 ebu_gate_kernel<<<(h->n_inst + K2B_WARPS - 1) / K2B_WARPS, K2B_WARPS * 32, 0, st>>> (
-                    (int)h->n_inst, h->d_ctl, h->d_res, h->d_histM, h->d_histS, h->d_cnt, h->d_binpow, h->log);
+                    (int)h->n_inst, h->d_ctl, h->d_res, h->d_histM, h->d_histS, h->d_cnt, h->d_binpow, h->ring.log);
                 B200M_LAUNCHED (1);
             }
         }
@@ -1249,7 +1194,7 @@ int b200m_ebu_log_enable (b200m_ebu* h, uint32_t capacity, void* stream)
 
 uint32_t b200m_ebu_log_capacity (const b200m_ebu* h)
 {
-    return h ? h->log.cap : 0;
+    return h ? h->ring.log.cap : 0;
 }
 
 int b200m_ebu_log_drain (b200m_ebu* h, b200m_ebu_point* out, uint32_t* count, uint64_t* lost, void* stream)
@@ -1410,22 +1355,13 @@ int ebu_log_enable (b200m_ebu* h, uint32_t capacity, bool dbtp, void* stream)
         return set_err (B200M_E_UNSUPPORTED, "the dBTP plane needs fragments of >= %d frames (a sample rate of >= %d Hz)", TPLOG_MIN_FRAGM, 20 * TPLOG_MIN_FRAGM);
     DeviceGuard g (h->device);
     cudaStream_t st = h->stream (stream);
-    if (h->log.pts) {                                        // kernels in flight may still write the old log
+    if (h->ring.log.pts) {                                   // kernels in flight may still write the old log
         B200M_CUDA (cudaStreamSynchronize (st));
         h->log_free ();
     }
     if (capacity == 0) return 0;
-    const size_t n = h->n_inst, pts = (size_t)capacity * n * (EBU_LOG_FIELDS + (dbtp ? 1 : 0)) * sizeof (float);
-    EbuLog lg = {nullptr, nullptr, capacity};
-    cudaError_t e = cudaMalloc ((void**)&lg.pts, pts);
-    if (e == cudaSuccess) e = cudaMalloc ((void**)&lg.written, n * sizeof (unsigned long long));
-    h->log = lg;                                             // log_free releases whatever was allocated
-    if (e == cudaSuccess) e = cudaMalloc ((void**)&h->d_log_rd, n * sizeof (unsigned long long));
-    if (e == cudaSuccess) e = cudaMalloc ((void**)&h->d_log_lost, n * sizeof (unsigned long long));
-    if (e == cudaSuccess) e = cudaMalloc ((void**)&h->d_log_cnt, n * sizeof (uint32_t));
-    if (e == cudaSuccess) e = cudaMalloc ((void**)&h->d_log_out, pts);
-    if (e == cudaSuccess) e = cudaMemsetAsync (h->log.written, 0, n * sizeof (unsigned long long), st);
-    if (e == cudaSuccess) e = cudaMemsetAsync (h->d_log_rd, 0, n * sizeof (unsigned long long), st);
+    const size_t n = h->n_inst;
+    cudaError_t e = h->ring.alloc (n, capacity, EBU_LOG_FIELDS + (dbtp ? 1 : 0), st);
     if (dbtp) {
         EbuTpPlane tp = {};
         tp.E = (int)(B200M_MAX_BLOCK / (uint32_t)h->fragm) + 2;
@@ -1451,27 +1387,18 @@ int ebu_log_enable (b200m_ebu* h, uint32_t capacity, bool dbtp, void* stream)
 int ebu_log_drain (b200m_ebu* h, float* out, uint32_t* count, uint64_t* lost, void* stream, bool dbtp)
 {
     if (!h || !out || !count || !lost) return set_err (B200M_E_INVAL, "NULL argument");
-    if (!h->log.pts) return set_err (B200M_E_INVAL, "the loudness log is off (b200m_ebu_log_enable)");
+    if (!h->ring.log.pts) return set_err (B200M_E_INVAL, "the loudness log is off (b200m_ebu_log_enable)");
     if (dbtp && !h->tp.fmax) return set_err (B200M_E_INVAL, "the loudness log has no dBTP plane (b200m_r128_log_enable)");
     DeviceGuard g (h->device);
     cudaStream_t st = h->stream (stream);
-    const size_t n = h->n_inst, nf = EBU_LOG_FIELDS + (dbtp ? 1 : 0);
-    const unsigned grid = (unsigned)((n + 31) / 32);
-    if (dbtp) ebu_log_drain_kernel<EBU_LOG_FIELDS + 1><<<grid, 32 * LOG_DRAIN_ROWS, 0, st>>> ((int)n, h->log, h->d_log_rd, h->d_log_out, h->d_log_cnt, h->d_log_lost);
-    else ebu_log_drain_kernel<EBU_LOG_FIELDS><<<grid, 32 * LOG_DRAIN_ROWS, 0, st>>> ((int)n, h->log, h->d_log_rd, h->d_log_out, h->d_log_cnt, h->d_log_lost);
-    B200M_LAUNCHED (1);
-    B200M_CUDA (cudaGetLastError ());
-    B200M_CUDA (cudaMemcpyAsync (out, h->d_log_out, n * h->log.cap * nf * sizeof (float), cudaMemcpyDeviceToHost, st));
-    B200M_CUDA (cudaMemcpyAsync (count, h->d_log_cnt, n * sizeof (uint32_t), cudaMemcpyDeviceToHost, st));
-    B200M_CUDA (cudaMemcpyAsync (lost, h->d_log_lost, n * sizeof (uint64_t), cudaMemcpyDeviceToHost, st));
-    B200M_CUDA (cudaStreamSynchronize (st));
-    return 0;
+    if (dbtp) return log_drain<EBU_LOG_FIELDS + 1, 32> (h->ring, h->n_inst, out, count, lost, st);
+    return log_drain<EBU_LOG_FIELDS, 32> (h->ring, h->n_inst, out, count, lost, st);
 }
 
 bool ebu_tp_view (b200m_ebu* h, EbuTpView* v)
 {
     if (!h->tp.fmax) return false;
-    *v = {h->log, h->tp, h->d_fph, h->tmod, h->fragm};
+    *v = {h->ring.log, h->tp, h->d_fph, h->tmod, h->fragm};
     return true;
 }
 

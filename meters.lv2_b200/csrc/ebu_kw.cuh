@@ -71,11 +71,8 @@ B200M_DEV void r128_hold (float* tpmax, float t)
     if (tp > *tpmax) *tpmax = tp;
 }
 
-// The loudness log (b200m_ebu_log_enable, ebu.cu): one point {M, S, I, range_min, range_max} per completed fragment of an instance,
-// `cap` points per instance.  Field f of point slot s of instance i is pts[(f * cap + s) * n_inst + i] (planes [5][cap][n_inst], or
-// [6][cap][n_inst] with the dBTP plane: lane = instance stores coalesce, like the power ring); written[i] counts the instance's
-// points, the next goes to slot written[i] % cap.  pts == nullptr: the log is off.
-struct EbuLog { float* pts; unsigned long long* written; uint32_t cap; };
+// The loudness log (b200m_ebu_log_enable, ebu.cu): a PointLog (common.cuh) of one point {M, S, I, range_min, range_max} per
+// completed fragment of an instance: planes [5][cap][n_inst], or [6][cap][n_inst] with the dBTP plane.
 constexpr int EBU_LOG_FIELDS = 5;
 
 // The log's dBTP plane (b200m_r128_log_enable): field 5 of a point is the dBTP of the true-peak maximum over the instance's
@@ -283,5 +280,5 @@ int ebu_log_enable (b200m_ebu* h, uint32_t capacity, bool dbtp, void* stream);
 int ebu_log_drain (b200m_ebu* h, float* out, uint32_t* count, uint64_t* lost, void* stream, bool dbtp);
 // host side, ebu.cu: the EBUr128 cycle's view of the log while its dBTP plane is on (false otherwise): the log, the plane's buffers,
 // the bank's phases on the device and its clock at the start of the next block
-struct EbuTpView { b200m::EbuLog lg; b200m::EbuTpPlane tp; int* fph; int tmod, fragm; };
+struct EbuTpView { b200m::PointLog lg; b200m::EbuTpPlane tp; int* fph; int tmod, fragm; };
 bool ebu_tp_view (b200m_ebu* h, EbuTpView* v);

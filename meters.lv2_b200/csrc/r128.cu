@@ -73,7 +73,7 @@ __global__ void r128_dbtp_fix_kernel (int n_inst, int nh, const uint8_t* __restr
 // maximum over the instance's channels of interval k (k = 0: with the open fragment's maximum of the blocks before) and holds its
 // coef_to_db; the interval after the last edge stays open.  Every interval read is zeroed for the next block.  on == 0 (no instance
 // has dBTP on) or off[i] (a disabled instance of a mixed bank): the instance's frames ran no true-peak meter and add nothing.
-__global__ void r128_tplog_fold_kernel (int n_inst, int nch, EbuLog lg, EbuTpPlane tp, const uint8_t* __restrict__ off, int on)
+__global__ void r128_tplog_fold_kernel (int n_inst, int nch, PointLog lg, EbuTpPlane tp, const uint8_t* __restrict__ off, int on)
 {
     const int i = blockIdx.x * blockDim.x + threadIdx.x;
     if (i >= n_inst) return;
