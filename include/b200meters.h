@@ -172,6 +172,26 @@ int b200m_ebu_mix_reduce (b200m_ebu* h, int32_t* d_out, void* stream);
 /* calc_integ + calc_range (:105-150) on a summed histogram vector (device pointer);
  * out5 (host) = integrated, integ_thr, range_min, range_max, range_thr */
 int b200m_ebu_mix_finish (b200m_ebu* h, const int32_t* d_mix, float out5[5], void* stream);
+/* Album loudness (an extension; the reference has no album concept): the whole-mix quantity for many groups of instances at once,
+ * e.g. the albums, playlists or segmented episodes of a library metered clip by clip.  An album's histograms are the sum of its
+ * members' histograms, i.e. the union of their 400 ms and 3 s measurement blocks (no block spans two clips, so this is not the
+ * loudness of the clips played back to back; it is libebur128's loudness_global_multiple).
+ * b200m_ebu_group_reduce: group (host, n_inst entries) maps instance i to album group[i] in 0 .. n_groups - 1, or to
+ * B200M_NO_GROUP (counted in no album).  d_out (device) receives n_groups rows of B200M_MIX_WORDS int32, each in the layout of
+ * b200m_ebu_mix_reduce's vector; an album without members gets a zero row.  n_groups does not depend on n_inst: shards of one
+ * library reduce into the same shape, which may be all-reduced across GPUs (int32 sums) and handed to b200m_ebu_group_finish.
+ * The member list is uploaded again only when group differs from the previous call's.
+ * b200m_ebu_group_finish: calc_integ + calc_range (:105-150) on each of the n_groups rows of d_groups (device); out5 (host,
+ * n_groups x 5) = integrated, integ_thr, range_min, range_max, range_thr of each row, -200 where the reference reports nothing (an
+ * empty album among them).  One device-to-host copy and one synchronisation per call.
+ * Both are ordered like the getters (an EBU bank of an EBUr128 bank follows that bank's path) and write nothing the bank's
+ * processing reads.  B200M_E_INVAL, with nothing enqueued, for a NULL argument, n_groups == 0,
+ * n_groups > B200M_MAX_GROUPS, or a group[i] >= n_groups other than B200M_NO_GROUP.  The sums are exact while each album's block
+ * counts fit in int32, as for b200m_ebu_mix_reduce. */
+#define B200M_NO_GROUP   0xFFFFFFFFu
+#define B200M_MAX_GROUPS 65536u     /* 395 MB of d_out */
+int b200m_ebu_group_reduce (b200m_ebu* h, const uint32_t* group, uint32_t n_groups, int32_t* d_out, void* stream);
+int b200m_ebu_group_finish (b200m_ebu* h, const int32_t* d_groups, uint32_t n_groups, float* out5, void* stream);
 
 /* ======================================================================================
  * True-peak + K-meter bank — replaces LV2M::TruePeakdsp (jmeters/truepeakdsp.h:28-61) and

@@ -15,6 +15,8 @@ _HERE = os.path.dirname(os.path.abspath(__file__))
 LIB_PATH = os.path.join(_HERE, "libb200meters.so")
 HIST_LEN = 751
 MIX_WORDS = 1508
+MAX_GROUPS = 65536          # B200M_MAX_GROUPS: albums per group_reduce / group_finish call
+NO_GROUP = 0xFFFFFFFF       # B200M_NO_GROUP: an instance counted in no album (-1 in the Python interface)
 MAX_BLOCK = 8192
 _v = C.c_void_p
 _lib = None
@@ -72,6 +74,8 @@ _PROTOS = {
     "b200m_ebu_state": (C.c_int, [_v, C.c_uint32, _v, _v, _v, _v, _v]),
     "b200m_ebu_mix_reduce": (C.c_int, [_v, _v, _v]),
     "b200m_ebu_mix_finish": (C.c_int, [_v, _v, _v, _v]),
+    "b200m_ebu_group_reduce": (C.c_int, [_v, _v, C.c_uint32, _v, _v]),
+    "b200m_ebu_group_finish": (C.c_int, [_v, _v, C.c_uint32, _v, _v]),
     # True peak + K-meter
     "b200m_tpk_create": (C.c_int, [C.POINTER(_v), C.c_int, C.c_uint32, C.c_float, C.c_uint32]),
     "b200m_tpk_destroy": (C.c_int, [_v]),
@@ -335,6 +339,24 @@ def _lengths(lengths, n_inst):
     return np.ascontiguousarray(a, np.uint32)
 
 
+def _groups(groups, n):
+    """album ids (>= 0, or -1 for no album) of n instances or clips as an int64 array (the C side checks them against n_groups)"""
+    a = np.asarray(groups).ravel()
+    if a.size != n:
+        raise B200MError("%d album ids for %d instances" % (a.size, n))
+    if a.size and (not np.issubdtype(a.dtype, np.integer) or a.min() < -1 or a.max() >= NO_GROUP):
+        raise B200MError("album ids must be integers >= 0, or -1 for no album")
+    return a.astype(np.int64)
+
+
+def _group_rows(d, what):
+    """(pointer, G) of an int32 CUDA tensor [G, MIX_WORDS]"""
+    import torch
+    if not (d.is_cuda and d.dtype == torch.int32 and d.dim() == 2 and d.shape[1] == MIX_WORDS and d.is_contiguous()):
+        raise B200MError("%s must be a contiguous int32 CUDA tensor [G, %d]" % (what, MIX_WORDS))
+    return C.c_void_p(d.data_ptr()), d.shape[0]
+
+
 def host_alloc(rows, cols):
     """[rows, cols] float32 numpy array in pinned host memory from b200m_host_alloc (placed on the GPU-local NUMA node);
     freed with b200m_host_free when the array is garbage-collected."""
@@ -486,6 +508,22 @@ class Ebu_r128_proc(_Bank):
     def mix_finish(self, d_mix, stream=None):
         out = np.empty(5, np.float32)
         _ck(lib().b200m_ebu_mix_finish(self.h, C.c_void_p(d_mix.data_ptr()), _np_ptr(out), _stream_ptr(stream)))
+        return out
+
+    def group_reduce(self, groups, d_out, stream=None):
+        """album histogram sums (b200m_ebu_group_reduce): groups holds n_inst album ids, 0 .. G - 1 or -1 (no album); d_out, an
+        int32 CUDA tensor [G, MIX_WORDS], receives each album's mix_reduce vector.  Ordered like the getters: after a host-path
+        call it runs on the bank's own stream, which group_finish synchronises."""
+        p, n_groups = _group_rows(d_out, "d_out")
+        g = np.ascontiguousarray(_groups(groups, self.n_inst).astype(np.uint32))     # -1 wraps to B200M_NO_GROUP
+        _ck(lib().b200m_ebu_group_reduce(self.h, _np_ptr(g), n_groups, p, _stream_ptr(stream)))
+
+    def group_finish(self, d_groups, stream=None):
+        """mix_finish of every row of d_groups (int32 CUDA tensor [G, MIX_WORDS], b200m_ebu_group_finish): float32 [G, 5] of
+        integrated, integ_thr, range_min, range_max, range_thr"""
+        p, n_groups = _group_rows(d_groups, "d_groups")
+        out = np.empty((n_groups, 5), np.float32)
+        _ck(lib().b200m_ebu_group_finish(self.h, p, n_groups, _np_ptr(out), _stream_ptr(stream)))
         return out
 
 
@@ -1018,8 +1056,11 @@ CURVE_LOG_POINTS = 1200        # the loudness log's capacity in programme_loudne
 TPLOG_MIN_FRAGM = 256          # the log's dBTP plane needs fragments of >= 256 frames (b200m_r128_log_enable): fsamp >= 5120 Hz
 
 
+ALBUM_FIELDS = ("integrated", "integ_thr", "range_min", "range_max")      # the first four of group_finish's five
+
+
 def programme_loudness(x, lengths, fsamp=48000.0, nchan=2, gains=None, block=1024, dbtp=True, precision=PREC_EXACT, device=0,
-                       curves=False):
+                       curves=False, groups=None):
     """Whole-programme EBU R128 loudness and true peak of N clips of different lengths, in one bank.
 
     x: rows i * nchan + c of clip i (nchan channels, or len(gains) with per-channel weights as in EBUr128), clip i valid for its
@@ -1039,9 +1080,15 @@ def programme_loudness(x, lengths, fsamp=48000.0, nchan=2, gains=None, block=102
     that fragment, and curve_TP (float32 [N, max(n_points)]): the dBTP of each fragment's true peak over the clip's channels (-inf
     when dbtp is False; NaN below 5120 Hz, where the log has no dBTP plane).  The bank's loudness log holds CURVE_LOG_POINTS points per clip and is drained before it can overflow, so
     the device memory does not grow with the programme; the other fields are the same as with curves=False (in tolerance mode tp_max
-    is then always the chunk-parallel FIR's, b200m_r128_log_enable)."""
+    is then always the chunk-parallel FIR's, b200m_r128_log_enable).
+    groups: None, or N album ids (>= 0, or -1 for a clip in no album) for album loudness: the result then also holds, for each of
+    G = max(groups) + 1 albums, album_integrated, album_integ_thr, album_range_min, album_range_max (the gated statistics of the
+    sum of the member clips' histograms, Ebu_r128_proc.group_reduce / group_finish after the last block), album_maxloudn_M,
+    album_maxloudn_S and album_tp_max (the largest of the member clips' values) and album_n_clips (int64).  An album without
+    members reads -200 and tp_max -inf.  Every other field is the same as without groups."""
     ln, blocks = _programme_blocks(x, lengths, block, "no clips")
     n = ln.size
+    grp = None if groups is None else _groups(groups, n)
     if gains is not None:
         nchan = np.asarray(gains).size
     bank = EBUr128(n, fsamp, dbtp, device, nchan=nchan, gains=gains)
@@ -1071,6 +1118,13 @@ def programme_loudness(x, lengths, fsamp=48000.0, nchan=2, gains=None, block=102
         if curves:
             drain()
         r, tp = bank.results()
+        n_albums = 0 if grp is None else int(grp.max()) + 1
+        if n_albums:
+            import torch
+            d = torch.empty((n_albums, MIX_WORDS), dtype=torch.int32, device="cuda:%d" % device)
+            torch.cuda.synchronize(device)          # after host input the bank's own stream writes d: no other work may still use it
+            bank.ebu.group_reduce(grp, d)
+            album5 = bank.ebu.group_finish(d)
     finally:
         bank.close()
     out = {k: np.ascontiguousarray(r[k], np.float32) for k in PROGRAMME_FIELDS}
@@ -1078,6 +1132,15 @@ def programme_loudness(x, lengths, fsamp=48000.0, nchan=2, gains=None, block=102
     if curves:
         out["n_points"] = n_points
         out.update(cv)
+    if grp is not None:
+        member = grp >= 0
+        for j, k in enumerate(ALBUM_FIELDS):
+            out["album_" + k] = album5[:, j].copy() if n_albums else np.empty(0, np.float32)
+        for k, v, empty in (("maxloudn_M", out["maxloudn_M"], -200.0), ("maxloudn_S", out["maxloudn_S"], -200.0), ("tp_max", tp, -np.inf)):
+            a = np.full(n_albums, empty, np.float32)
+            np.maximum.at(a, grp[member], v[member])
+            out["album_" + k] = a
+        out["album_n_clips"] = np.bincount(grp[member], minlength=n_albums).astype(np.int64)
     return out
 
 

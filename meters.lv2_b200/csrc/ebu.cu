@@ -660,6 +660,80 @@ __global__ void ebu_mix_finish_kernel (const int* __restrict__ mix, const float*
     if (lane == 0) { out5[0] = vi; out5[1] = th; out5[2] = v0; out5[3] = v1; out5[4] = rt; }
 }
 
+// Album histogram sums (b200m_ebu_group_reduce).  The host sorts the instances by album into a member list (with each member's album
+// beside it) and a CTA takes GRP_CHUNK consecutive members of that list, whatever the album sizes: one album of the whole bank and
+// one album per instance both give n / GRP_CHUNK CTAs.  A CTA streams its members' rows (6032 bytes each, one column per thread:
+// coalesced) and merges each album's partial sums into the album's zeroed row with integer atomicAdd, skipping zero sums:
+// order-independent, hence exact.  Its members are sorted by album, so it flushes once per album it meets.
+constexpr int GRP_THREADS = 256, GRP_CHUNK = 16, GRP_BATCH = 4;
+constexpr int GRP_COLS = (B200M_MIX_WORDS + GRP_THREADS - 1) / GRP_THREADS;     // columns per thread
+
+__global__ void __launch_bounds__ (GRP_THREADS)
+ebu_group_reduce_kernel (const int* __restrict__ histM, const int* __restrict__ histS, const int* __restrict__ cnt,
+                         const uint32_t* __restrict__ members, const uint32_t* __restrict__ album, int n_members, int* __restrict__ out)
+{
+    __shared__ uint32_t mem[GRP_CHUNK], alb[GRP_CHUNK];
+    const int first = blockIdx.x * GRP_CHUNK, n = min (GRP_CHUNK, n_members - first);
+    if (threadIdx.x < n) { mem[threadIdx.x] = members[first + threadIdx.x]; alb[threadIdx.x] = album[first + threadIdx.x]; }
+    __syncthreads ();
+    const int* src[GRP_COLS]; int pitch[GRP_COLS]; int acc[GRP_COLS];
+#pragma unroll
+    for (int j = 0; j < GRP_COLS; ++j) {
+        const int col = threadIdx.x + j * GRP_THREADS;
+        if (col < 752) { src[j] = histM + col; pitch[j] = HIST_PITCH; }
+        else if (col < 1504) { src[j] = histS + (col - 752); pitch[j] = HIST_PITCH; }
+        else { src[j] = cnt + (col - 1504); pitch[j] = 4; }
+        acc[j] = 0;
+    }
+    auto flush = [&] (uint32_t a) {
+        int* row = out + (size_t)a * B200M_MIX_WORDS;
+#pragma unroll
+        for (int j = 0; j < GRP_COLS; ++j) {
+            const int col = threadIdx.x + j * GRP_THREADS;
+            if (col < B200M_MIX_WORDS && acc[j]) atomicAdd (row + col, acc[j]);
+            acc[j] = 0;
+        }
+    };
+    // GRP_BATCH members' loads in flight before their sums (a flush between them must not hold back the loads)
+    uint32_t cur = alb[0];
+    for (int k0 = 0; k0 < n; k0 += GRP_BATCH) {
+        int v[GRP_BATCH][GRP_COLS];
+#pragma unroll
+        for (int q = 0; q < GRP_BATCH; ++q) {
+            const size_t m = mem[min (k0 + q, n - 1)];
+#pragma unroll
+            for (int j = 0; j < GRP_COLS; ++j)
+                v[q][j] = (k0 + q < n && threadIdx.x + j * GRP_THREADS < B200M_MIX_WORDS) ? src[j][m * pitch[j]] : 0;
+        }
+#pragma unroll
+        for (int q = 0; q < GRP_BATCH; ++q) {
+            if (k0 + q < n && alb[k0 + q] != cur) { flush (cur); cur = alb[k0 + q]; }        // uniform across the CTA
+#pragma unroll
+            for (int j = 0; j < GRP_COLS; ++j) acc[j] += v[q][j];
+        }
+    }
+    flush (cur);
+}
+
+// b200m_ebu_group_finish: one warp per album row, the whole-mix finish of each (rows is not __restrict__: with it ptxas spills)
+constexpr int GRP_FIN_WARPS = 4;
+
+__global__ void __launch_bounds__ (GRP_FIN_WARPS * 32)
+ebu_group_finish_kernel (int n_groups, const int* rows, const float* __restrict__ bin_power, float* __restrict__ out5)
+{
+    __shared__ float sbp[100];
+    for (int q = threadIdx.x; q < 100; q += blockDim.x) sbp[q] = bin_power[q];
+    __syncthreads ();
+    const int lane = threadIdx.x & 31;
+    const int g = blockIdx.x * GRP_FIN_WARPS + (threadIdx.x >> 5);
+    if (g >= n_groups) return;
+    const int* row = rows + (size_t)g * B200M_MIX_WORDS;
+    float vi = -200.0f, th = -200.0f, v0 = -200.0f, v1 = -200.0f, rt = -200.0f;
+    hist_calc_integ (row, row[1504], sbp, lane, vi, th);
+    hist_calc_range (row + 752, row[1505], sbp, lane, v0, v1, rt);
+    if (lane == 0) { float* o = out5 + (size_t)g * 5; o[0] = vi; o[1] = th; o[2] = v0; o[3] = v1; o[4] = rt; }
+}
+
 }  // namespace b200m
 
 using namespace b200m;
@@ -733,6 +807,10 @@ struct b200m_ebu {
     // a ragged block (b200m_ebu_process_ragged_*, b200m_r128_run_ragged_*): the upload of its per-instance lengths, and the instances
     // whose length differs from nfram (scratch: index, fragments in the block, S-period position div2)
     RaggedLen rag;
+    // album reduce (b200m_ebu_group_reduce): the assignment as last uploaded (empty: none yet) and its upload to grp.d, the member
+    // list (grp_members instances sorted by album) followed by each member's album; the finish's device output, grown on demand
+    std::vector<uint32_t> grp_of; RaggedLen grp; uint32_t grp_members = 0;
+    float* d_grp5 = nullptr; uint32_t grp5_cap = 0;
     struct Rag { uint32_t i; int nf, d2; };
     std::vector<Rag> rg;
     void phase_reset () {
@@ -1001,6 +1079,7 @@ int b200m_ebu_destroy (b200m_ebu* h)
     cudaFree (h->d_out5); cudaFree (h->d_ctl); cudaFree (h->d_res); cudaFree (h->d_histM); cudaFree (h->d_histS); cudaFree (h->d_cnt); cudaFree (h->d_fph);
     h->log_free ();
     h->rag.release ();
+    h->grp.release (); cudaFree (h->d_grp5);
     h->path.release ();
     delete h;
     return 0;
@@ -1342,6 +1421,63 @@ int b200m_ebu_mix_finish (b200m_ebu* h, const int32_t* d_mix, float out5[5], voi
     ebu_mix_finish_kernel<<<1, 32, 0, st>>> (d_mix, h->d_binpow, h->d_out5);
     B200M_LAUNCHED (1);
     B200M_CUDA (cudaMemcpyAsync (out5, h->d_out5, 5 * sizeof (float), cudaMemcpyDeviceToHost, st));
+    B200M_CUDA (cudaStreamSynchronize (st));
+    return 0;
+}
+
+int b200m_ebu_group_reduce (b200m_ebu* h, const uint32_t* group, uint32_t n_groups, int32_t* d_out, void* stream)
+{
+    if (!h || !group || !d_out) return set_err (B200M_E_INVAL, "NULL argument");
+    if (n_groups == 0 || n_groups > B200M_MAX_GROUPS) return set_err (B200M_E_INVAL, "n_groups %u outside 1..%u", n_groups, B200M_MAX_GROUPS);
+    const uint32_t n = h->n_inst;
+    for (uint32_t i = 0; i < n; ++i)
+        if (group[i] >= n_groups && group[i] != B200M_NO_GROUP)
+            return set_err (B200M_E_INVAL, "group[%u] = %u is neither < n_groups = %u nor B200M_NO_GROUP", i, group[i], n_groups);
+    DeviceGuard g (h->device);
+    cudaStream_t st = h->stream (stream);
+    if (h->grp_of.empty () || memcmp (group, h->grp_of.data (), n * sizeof (uint32_t))) {
+        // counting sort of the instances by album, each album's members in instance order, and the album of each member
+        cudaError_t e = cudaSuccess;
+        uint32_t* w = h->grp.stage (2 * (size_t)n, &e);
+        if (!w) return cuda_fail (e, "b200m_ebu_group_reduce", __FILE__, __LINE__);
+        std::vector<uint32_t> off (n_groups + 1, 0);
+        for (uint32_t i = 0; i < n; ++i) if (group[i] != B200M_NO_GROUP) off[group[i] + 1]++;
+        for (uint32_t a = 0; a < n_groups; ++a) off[a + 1] += off[a];
+        const uint32_t nm = off[n_groups];
+        for (uint32_t i = 0; i < n; ++i)
+            if (group[i] != B200M_NO_GROUP) { const uint32_t p = off[group[i]]++; w[p] = i; w[nm + p] = group[i]; }
+        B200M_CUDA (h->grp.upload (2 * (size_t)nm, st));
+        h->grp_of.assign (group, group + n); h->grp_members = nm;
+    }
+    const uint32_t nm = h->grp_members;
+    B200M_CUDA (cudaMemsetAsync (d_out, 0, (size_t)n_groups * B200M_MIX_WORDS * sizeof (int32_t), st));
+    if (nm) {
+        ebu_group_reduce_kernel<<<(nm + GRP_CHUNK - 1) / GRP_CHUNK, GRP_THREADS, 0, st>>> (h->d_histM, h->d_histS, h->d_cnt, h->grp.d,
+                                                                                         h->grp.d + nm, (int)nm, d_out);
+        B200M_LAUNCHED (1);
+    }
+    B200M_CUDA (cudaGetLastError ());
+    return 0;
+}
+
+int b200m_ebu_group_finish (b200m_ebu* h, const int32_t* d_groups, uint32_t n_groups, float* out5, void* stream)
+{
+    if (!h || !d_groups || !out5) return set_err (B200M_E_INVAL, "NULL argument");
+    if (n_groups == 0 || n_groups > B200M_MAX_GROUPS) return set_err (B200M_E_INVAL, "n_groups %u outside 1..%u", n_groups, B200M_MAX_GROUPS);
+    DeviceGuard g (h->device);
+    cudaStream_t st = h->stream (stream);
+    if (n_groups > h->grp5_cap) {                           // the previous call synchronised: nothing in flight uses the old buffer
+        cudaFree (h->d_grp5); h->d_grp5 = nullptr; h->grp5_cap = 0;
+        if (cudaMalloc ((void**)&h->d_grp5, (size_t)n_groups * 5 * sizeof (float)) != cudaSuccess) {
+            cudaGetLastError ();
+            return set_err (B200M_E_NOMEM, "album results of %u groups: out of device memory", n_groups);
+        }
+        h->grp5_cap = n_groups;
+    }
+    ebu_group_finish_kernel<<<(n_groups + GRP_FIN_WARPS - 1) / GRP_FIN_WARPS, GRP_FIN_WARPS * 32, 0, st>>> ((int)n_groups, d_groups, h->d_binpow, h->d_grp5);
+    B200M_LAUNCHED (1);
+    B200M_CUDA (cudaGetLastError ());
+    B200M_CUDA (cudaMemcpyAsync (out5, h->d_grp5, (size_t)n_groups * 5 * sizeof (float), cudaMemcpyDeviceToHost, st));
     B200M_CUDA (cudaStreamSynchronize (st));
     return 0;
 }

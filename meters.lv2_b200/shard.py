@@ -4,7 +4,8 @@ Every metering instance is self-contained (SURVEY.md §8e), so N GPUs simply own
 rank r of W processes instances  [r*n/W, (r+1)*n/W).  The only cross-instance quantity is the whole-mix gated
 loudness: the int32 sum of all instances' hist_M / hist_S (+ counts), reduced per GPU by
 b200m_ebu_mix_reduce and across GPUs by ONE all-reduce of B200M_MIX_WORDS int32 (NCCL on GPUs, gloo in CPU
-tests); integer sums are order independent, hence bit-exact for any GPU count.
+tests); integer sums are order independent, hence bit-exact for any GPU count.  Album loudness works the same way with
+one row per album (b200m_ebu_group_reduce): the clips of one album may sit on different GPUs.
 """
 MIX_WORDS = 1508
 
@@ -25,11 +26,12 @@ def shard_rows(n_total, nchan, rank, world):
 
 
 def allreduce_mix(mix, group=None):
-    """sum the per-rank whole-mix histogram vector (int32[MIX_WORDS]) over all ranks, in place."""
+    """sum the per-rank whole-mix histogram vector (int32[MIX_WORDS]), or the album rows of Ebu_r128_proc.group_reduce
+    (int32[G, MIX_WORDS], the same G on every rank), over all ranks, in place."""
     import torch
     import torch.distributed as dist
-    if mix.dtype != torch.int32 or mix.numel() != MIX_WORDS:
-        raise ValueError("mix must be int32[%d]" % MIX_WORDS)
+    if mix.dtype != torch.int32 or not (mix.numel() == MIX_WORDS or (mix.dim() == 2 and mix.shape[1] == MIX_WORDS)):
+        raise ValueError("mix must be int32[%d] or int32[G, %d]" % (MIX_WORDS, MIX_WORDS))
     if dist.is_available() and dist.is_initialized() and dist.get_world_size(group) > 1:
         dist.all_reduce(mix, op=dist.ReduceOp.SUM, group=group)
     return mix
