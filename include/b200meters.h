@@ -446,7 +446,8 @@ int b200m_cor_clear (b200m_cor* h, int32_t inst, void* stream);
 int b200m_cor_process_ctl_device (b200m_cor* h, const float* d_in, size_t stride, uint32_t nfram, const uint8_t* run, void* stream);
 int b200m_cor_process_ctl_host (b200m_cor* h, const float* in, size_t stride, uint32_t nfram, const uint8_t* run);
 /* Ragged blocks: pair i runs Stcorrdsp::process (:47-77) over the first len[i] <= nfram frames of its rows only, as a private
- * Stcorrdsp fed only those frames (bit-identical in B200M_PREC_EXACT, within 1e-5 in B200M_PREC_FMA).  len: host array of n_inst.
+ * Stcorrdsp fed only those frames (bit-identical in B200M_PREC_EXACT, within 1e-5 in B200M_PREC_FMA, bit-identical there too when
+ * tcf * fsamp > 21600: see b200m_cor_set_precision).  len: host array of n_inst.
  * - Frames at or after len[i] may hold anything, NaN and Inf included: they reach no state and no reading.
  * - len[i] == 0: the pair is not called (exactly the hold of b200m_cor_process_ctl_*, which is this call with run[i] ? nfram : 0).
  * - A length above nfram returns B200M_E_INVAL and enqueues nothing.
@@ -459,7 +460,10 @@ int b200m_cor_process_ragged_host (b200m_cor* h, const float* in, size_t stride,
 /* B200M_PREC_EXACT (default): the five recurrences run serially in time, one lane per pair, bit-identical to the reference.
  * B200M_PREC_FMA: time-parallel evaluation -- the recurrences are linear one-pole filters, so a warp owns ONE pair, its lanes take
  * consecutive time segments and an affine warp scan stitches them: 32x more parallelism for small banks (2048 pairs are 64 warps
- * in exact mode); the correlation stays within 1e-5 of the reference. */
+ * in exact mode); the correlation stays within 1e-5 of the reference.  The reference's own fp32 rounding noise grows with the product
+ * filters' memory tcf * fsamp, and no more accurate evaluation can follow it: a bank whose memory exceeds 21600 samples (tcf 0.3 s
+ * above 72 kHz, i.e. at 88.2-192 kHz; tcf above 0.45 s at 48 kHz) runs the exact kernel in this mode too, bit-identical to the
+ * reference.  The bound is fixed at creation, whatever the block. */
 int b200m_cor_set_precision (b200m_cor* h, int mode);
 int b200m_cor_state (b200m_cor* h, float* state5, void* stream);          /* [n][5] zl zr zlr zll zrr */
 int b200m_cor_coeffs (const b200m_cor* h, float w[2]);

@@ -277,7 +277,7 @@ using namespace b200m;
 
 struct b200m_cor {
     int device; uint32_t n_inst; float w1, w2;
-    int scan = 0;                          // B200M_PREC_FMA: time-parallel cor_scan_kernel
+    int scan = 0;                          // B200M_PREC_FMA: time-parallel cor_scan_kernel (when 1 / w2 <= COR_SCAN_MAX_MEMORY)
     float *d_st = nullptr, *d_res = nullptr;
     // ragged blocks (b200m_cor_process_ragged_*, and b200m_cor_process_ctl_* as lengths run[i] ? nfram : 0): the lengths as last
     // uploaded to rag.d (empty: none yet); a block uploads them only when they differ
@@ -287,12 +287,18 @@ struct b200m_cor {
     BankPath path;
 };
 
+// The tolerance mode's promise is 1e-5 of the reference, and the reference's own fp32 rounding noise grows with the product filters'
+// memory 1 / w2 = tcf * fs: the scan, ~1e-6 from float64 arithmetic, cannot track it beyond this many samples.  Measured on an H100
+// (60 s per rate, tests/test_tolerance_rates_gpu.py): worst |scan - reference| <= 5.8e-6 up to 21600 samples (0.3 s up to 72 kHz,
+// 0.45 s at 48 kHz), 8.3e-6 at 26460 (88.2 kHz), 1.5e-5 at 52920 (176.4 kHz).  A longer memory runs cor_kernel, bit-identical.
+constexpr float COR_SCAN_MAX_MEMORY = 21600.0f;
+
 template <bool RAG>
 static int cor_launch (b200m_cor* h, const float* d_in, size_t stride, uint32_t nfram, cudaStream_t st, float* ring, int N, int rboff)
 {
     const int aligned = ((uintptr_t)d_in % 16 == 0) && (stride % 4 == 0);
     const uint32_t* rlen = RAG ? h->rag.d : nullptr;
-    if (h->scan)
+    if (h->scan && h->w2 >= 1.0f / COR_SCAN_MAX_MEMORY)
         cor_scan_kernel<RAG><<<(h->n_inst + CSC_WARPS - 1) / CSC_WARPS, CSC_WARPS * 32, 0, st>>> (
             d_in, stride, (int)h->n_inst, (int)nfram, aligned, h->w1, h->w2, h->d_st, h->d_res, ring, N, rboff, rlen);
     else
