@@ -423,6 +423,44 @@ uint32_t b200m_dr14_log_capacity (const b200m_dr14* h);
  * out[i][0 .. count[i]) (NaN after them); lost[i] older unread points were overwritten.  Ordered after the work on `stream` like
  * b200m_dr14_results (synchronises it).  B200M_E_INVAL with the log off. */
 int b200m_dr14_log_drain (b200m_dr14* h, b200m_dr14_point* out, uint32_t* count, uint64_t* lost, void* stream);
+/* Album DR (an extension; the reference has no album concept), DR mode: the DR score of many groups of instances at once, e.g. the
+ * albums of a library metered track by track, bit-identical to one private dr14 instance fed every member track back to back when
+ * each track holds whole 3 s windows and ends in a scored one.  dr14_calc_rms_score (:285-352) depends only on the 8000-bin RMS
+ * histogram, the count of scored windows and the two highest window peaks, so an album's state is the sum of its members'
+ * histograms and window counts and the two largest of their top-two peak pairs.
+ * b200m_dr14_group_reduce: group (host, n_inst entries) maps instance i to album group[i] in 0 .. n_groups - 1, or to
+ * B200M_NO_GROUP, as for b200m_ebu_group_reduce.  d_rows (device) receives n_groups rows of B200M_DR14_GROUP_WORDS (nch) int32:
+ * the channel-0 histogram, then the channel-1 histogram (bins in the order of b200m_dr14_histogram), the number of windows scored
+ * (the sum of the members' num_fragments) and the number of members.  The rows are zeroed and summed into with integer atomics,
+ * so the rows of shards of one library may be all-reduced with SUM across GPUs.  d_peaks (device) receives [n_groups][nch][3]
+ * floats of linear values: the album's highest and second-highest window peak (the top two of the members' peak_hist pairs by
+ * value; NaN never enters a pair) and its true-peak hold (m_dbtp, the m_peak port before coeff_to_db): the largest member hold
+ * that is not NaN, NaN only if every member's hold is NaN (MAX written as `>` makes a hold NaN after a block whose true peak is, :430).  Peaks cannot be
+ * summed: shards all-gather theirs and hand every part to the finish.  An album without members gets zeros everywhere, which is
+ * what a freshly instantiated plugin holds.
+ * b200m_dr14_group_finish: d_peaks (device) holds n_parts consecutive [n_groups][nch][3] blocks (one per shard after an
+ * all-gather; n_parts = 1 on one GPU).  Per album the finish merges the parts' top-two pairs by value and takes their largest
+ * non-NaN hold (an empty part holds 0), then scores each channel's row as dr14_calc_rms_score does: m_cut = MAX (1, floorf (nf /
+ * 5.0)), the walk from the top bin down in the reference's bin order, nothing before nf > 2 windows, coeff_to_db; then the port
+ * arithmetic (:436-460).  out (host, n_groups entries): m_rms, dr, dr_total, block_count as in b200m_dr14_result; peak2 as in
+ * b200m_dr14_point; m_peak = coeff_to_db (hold); windows and members as floats (exact up to 2^24).  A mono bank's channel-1
+ * fields and dr_total are NaN.  An empty album reads like a fresh plugin: m_rms = peak2 = -81, dr = dr_total = 21,
+ * block_count 0, m_peak -80.  One device-to-host copy and one synchronisation per call.
+ * Both are ordered like the getters and write nothing the bank's processing reads.  B200M_E_INVAL, with nothing enqueued, for a
+ * NULL argument, n_groups == 0, n_groups > B200M_DR14_MAX_GROUPS, n_parts == 0, or a group[i] >= n_groups other than
+ * B200M_NO_GROUP; B200M_E_UNSUPPORTED on a TPnRMS bank.  The sums are exact while each album's window counts fit in int32. */
+#define B200M_DR14_MAX_GROUPS 16384u                          /* 1.05 GB of d_rows for a stereo bank */
+#define B200M_DR14_GROUP_WORDS(nch) ((nch) * 8000u + 2u)      /* int32 words per album row */
+typedef struct b200m_dr14_album {
+    float m_rms[2], peak2[2];        /* top-20 % RMS score and second-highest window peak (dB, -81 before 3 windows) */
+    float dr[2], dr_total;           /* clamped to 1..20; 21 = not valid */
+    float block_count;               /* 3.0 * windows */
+    float m_peak[2];                 /* coeff_to_db of the largest member true-peak hold */
+    float windows, members;
+} b200m_dr14_album;
+int b200m_dr14_group_reduce (b200m_dr14* h, const uint32_t* group, uint32_t n_groups, int32_t* d_rows, float* d_peaks, void* stream);
+int b200m_dr14_group_finish (b200m_dr14* h, const int32_t* d_rows, const float* d_peaks, uint32_t n_parts, uint32_t n_groups,
+                             b200m_dr14_album* out, void* stream);
 
 /* ======================================================================================
  * Stereo correlation bank — replaces LV2M::Stcorrdsp (jmeters/stcorrdsp.h:27-55) as driven by

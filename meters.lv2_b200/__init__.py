@@ -144,6 +144,8 @@ _PROTOS = {
     "b200m_dr14_log_enable": (C.c_int, [_v, C.c_uint32, _v]),
     "b200m_dr14_log_drain": (C.c_int, [_v, _v, _v, _v, _v]),
     "b200m_dr14_log_capacity": (C.c_uint32, [_v]),
+    "b200m_dr14_group_reduce": (C.c_int, [_v, _v, C.c_uint32, _v, _v, _v]),
+    "b200m_dr14_group_finish": (C.c_int, [_v, _v, _v, C.c_uint32, C.c_uint32, _v, _v]),
     "b200m_cor_create": (C.c_int, [C.POINTER(_v), C.c_int, C.c_uint32, C.c_int, C.c_float, C.c_float]),
     "b200m_cor_destroy": (C.c_int, [_v]),
     "b200m_cor_process_device": (C.c_int, [_v, _v, C.c_size_t, C.c_uint32, _v]),
@@ -349,11 +351,11 @@ def _groups(groups, n):
     return a.astype(np.int64)
 
 
-def _group_rows(d, what):
-    """(pointer, G) of an int32 CUDA tensor [G, MIX_WORDS]"""
+def _group_rows(d, what, words=MIX_WORDS):
+    """(pointer, G) of an int32 CUDA tensor [G, words]"""
     import torch
-    if not (d.is_cuda and d.dtype == torch.int32 and d.dim() == 2 and d.shape[1] == MIX_WORDS and d.is_contiguous()):
-        raise B200MError("%s must be a contiguous int32 CUDA tensor [G, %d]" % (what, MIX_WORDS))
+    if not (d.is_cuda and d.dtype == torch.int32 and d.dim() == 2 and d.shape[1] == words and d.is_contiguous()):
+        raise B200MError("%s must be a contiguous int32 CUDA tensor [G, %d]" % (what, words))
     return C.c_void_p(d.data_ptr()), d.shape[0]
 
 
@@ -770,6 +772,16 @@ DR14_POINT_DTYPE = np.dtype([("window", "<f4"), ("silent", "<f4"), ("rms", "<f4"
 
 
 DR14_RESET, DR14_CLEAR = 1, 2
+DR14_MAX_GROUPS = 16384     # B200M_DR14_MAX_GROUPS: albums per DR14.group_reduce / group_finish call
+# one album's DR (b200m_dr14_album): m_rms, dr, dr_total, block_count as in DR14_RESULT_DTYPE, peak2 as in DR14_POINT_DTYPE, m_peak
+# the largest member true-peak hold (dB); channel 1 and dr_total NaN in a mono bank
+DR14_ALBUM_DTYPE = np.dtype([("m_rms", "<f4", 2), ("peak2", "<f4", 2), ("dr", "<f4", 2), ("dr_total", "<f4"), ("block_count", "<f4"),
+                             ("m_peak", "<f4", 2), ("windows", "<f4"), ("members", "<f4")])
+
+
+def dr14_group_words(n_channels):
+    """B200M_DR14_GROUP_WORDS: int32 words of one album row of DR14.group_reduce (histograms, window count, member count)"""
+    return n_channels * 8000 + 2
 
 
 class DR14(_Bank):
@@ -823,6 +835,34 @@ class DR14(_Bank):
         """the points logged since the last drain (b200m_dr14_log_drain): (points [n_inst, capacity] DR14_POINT_DTYPE, oldest first,
         NaN past count; count uint32 [n_inst]; lost uint64 [n_inst], older points overwritten before they were drained)"""
         return self._drain(lib().b200m_dr14_log_drain, lib().b200m_dr14_log_capacity(self.h), DR14_POINT_DTYPE, stream)
+
+    def _peaks(self, d, n_groups, parts):
+        """(pointer, n_parts) of a float32 CUDA tensor [G, nchan, 3], or with parts also [P, G, nchan, 3]"""
+        import torch
+        shape = tuple(d.shape)
+        ok = d.is_cuda and d.dtype == torch.float32 and d.is_contiguous() and shape[-3:] == (n_groups, self.nchan, 3)
+        if not (ok and (d.dim() == 3 or (parts and d.dim() == 4))):
+            raise B200MError("d_peaks must be a contiguous float32 CUDA tensor [%s%d, %d, 3]" % ("P, " if parts else "", n_groups, self.nchan))
+        return C.c_void_p(d.data_ptr()), (shape[0] if d.dim() == 4 else 1)
+
+    def group_reduce(self, groups, d_rows, d_peaks, stream=None):
+        """album DR state (b200m_dr14_group_reduce, DR mode): groups holds n_inst album ids, 0 .. G - 1 or -1 (no album); d_rows, an
+        int32 CUDA tensor [G, dr14_group_words(nchan)], receives each album's summed histograms, window count and member count;
+        d_peaks, a float32 CUDA tensor [G, nchan, 3], its top two window peaks and true-peak hold (linear).  Ordered like the getters:
+        after a host-path call it runs on the bank's own stream, which group_finish synchronises."""
+        p, n_groups = _group_rows(d_rows, "d_rows", dr14_group_words(self.nchan))
+        q, _ = self._peaks(d_peaks, n_groups, False)
+        g = np.ascontiguousarray(_groups(groups, self.n_inst).astype(np.uint32))     # -1 wraps to B200M_NO_GROUP
+        _ck(lib().b200m_dr14_group_reduce(self.h, _np_ptr(g), n_groups, p, q, _stream_ptr(stream)))
+
+    def group_finish(self, d_rows, d_peaks, stream=None):
+        """the DR of every album (b200m_dr14_group_finish): d_rows as group_reduce fills it (summed over shards), d_peaks [G, nchan, 3]
+        or the [P, G, nchan, 3] parts of P shards (shard.allreduce_dr14_groups); a DR14_ALBUM_DTYPE array of G"""
+        p, n_groups = _group_rows(d_rows, "d_rows", dr14_group_words(self.nchan))
+        q, n_parts = self._peaks(d_peaks, n_groups, True)
+        out = np.empty(n_groups, DR14_ALBUM_DTYPE)
+        _ck(lib().b200m_dr14_group_finish(self.h, p, q, n_parts, n_groups, _np_ptr(out), _stream_ptr(stream)))
+        return out
 
 
 class Spectr30(_Bank):
@@ -1149,7 +1189,7 @@ DR_CURVE_FIELDS = (("window_rms", "rms"), ("window_peak", "peak"), ("m_rms", "m_
 DR_CURVE_LOG_POINTS = 16       # the window log's capacity in programme_dr14: 48 s of windows
 
 
-def programme_dr14(x, lengths, rate=48000.0, n_channels=2, dr_mode=True, block=1024, device=0, curves=False):
+def programme_dr14(x, lengths, rate=48000.0, n_channels=2, dr_mode=True, block=1024, device=0, curves=False, groups=None):
     """DR-14 (dr_mode=True) or TPnRMS meter readings of N whole tracks of different lengths, in one bank.
 
     x: rows i * n_channels + c of track i, track i valid for its first lengths[i] frames: a [N * n_channels, >= max(lengths)]
@@ -1169,11 +1209,20 @@ def programme_dr14(x, lengths, rate=48000.0, n_channels=2, dr_mode=True, block=1
     and dr (float32 [N, W, n_channels]); dr_total and block_count (float32 [N, W]); silent (bool [N, W]), with W = max(n_windows),
     NaN (silent False) past a track's n_windows: the b200m_dr14_point fields.  The bank's window log holds DR_CURVE_LOG_POINTS
     points per track and is drained before it can overflow, so the device memory does not grow with the tracks; the result array
-    is the same as with curves=False."""
+    is the same as with curves=False.
+    groups: None, or N album ids (>= 0, or -1 for a track in no album) for album DR (DR mode only).  One more trailing element is
+    then returned, albums: a dict for G = max(groups) + 1 albums of m_rms, peak2, dr, m_peak (float32 [G, n_channels]), dr_total,
+    block_count (float32 [G]) (DR14.group_reduce / group_finish after the last block: the DR of one dr14 instance that scored every
+    window of every member track), n_windows and n_tracks (int64 [G]), and dr_mean (float64 [G]): the arithmetic mean of the
+    member tracks' valid (1 .. 20) dr_total (dr[0] for mono), NaN if none is valid.  An album without members reads like a fresh
+    plugin (m_rms and peak2 -81, dr and dr_total 21, m_peak -80).  Every other returned value is the same as without groups."""
     ln, blocks = _programme_blocks(x, lengths, block, "no tracks")
     n = ln.size
     if curves and not dr_mode:
         raise B200MError("DR curves need dr_mode (a TPnRMS bank has no 3 s windows)")
+    grp = None if groups is None else _groups(groups, n)
+    if grp is not None and not dr_mode:
+        raise B200MError("album DR needs dr_mode (a TPnRMS bank has no 3 s windows)")
     bank = DR14(n, n_channels, rate, dr_mode, device)
     try:
         if curves:
@@ -1203,10 +1252,38 @@ def programme_dr14(x, lengths, rate=48000.0, n_channels=2, dr_mode=True, block=1
             drain()
             cv["n_windows"] = n_windows
             cv["silent"] = silent
-            return bank.results(), cv
-        return bank.results()
+        res = bank.results()
+        out = (res, cv) if curves else (res,)
+        if grp is not None:
+            out += (_dr14_albums(bank, grp, res, device),)
+        return out if len(out) > 1 else res
     finally:
         bank.close()
+
+
+def _dr14_albums(bank, grp, res, device):
+    """programme_dr14's albums dict (see there) of the tracks of `bank` after their last block, res their results"""
+    import torch
+    nch, g = bank.nchan, int(grp.max()) + 1 if grp.size else 0
+    if g > 0:
+        rows = torch.empty((g, dr14_group_words(nch)), dtype=torch.int32, device="cuda:%d" % device)
+        peaks = torch.empty((g, nch, 3), dtype=torch.float32, device="cuda:%d" % device)
+        torch.cuda.synchronize(device)          # after host input the bank's own stream writes rows: no other work may still use them
+        bank.group_reduce(grp, rows, peaks)
+        alb = bank.group_finish(rows, peaks)
+        tail = rows[:, -2:].cpu().numpy().astype(np.int64)
+    else:
+        alb, tail = np.empty(0, DR14_ALBUM_DTYPE), np.empty((0, 2), np.int64)
+    out = {k: np.ascontiguousarray(alb[k][:, :nch]) for k in ("m_rms", "peak2", "dr", "m_peak")}
+    out.update(dr_total=alb["dr_total"].copy(), block_count=alb["block_count"].copy(), n_windows=tail[:, 0].copy(),
+               n_tracks=tail[:, 1].copy())
+    v = (res["dr_total"] if nch > 1 else res["dr"][:, 0]).astype(np.float64)
+    ok = (grp >= 0) & (v >= 1) & (v <= 20)                      # 21: not valid; 0: an empty track, which never ran
+    s, c = np.zeros(g), np.zeros(g)
+    np.add.at(s, grp[ok], v[ok]); np.add.at(c, grp[ok], 1)
+    with np.errstate(invalid="ignore", divide="ignore"):
+        out["dr_mean"] = np.where(c > 0, s / np.maximum(c, 1), np.nan)
+    return out
 
 
 def programme_stats(x, lengths, rate=48000.0, block=1024, device=0):

@@ -7,6 +7,7 @@
 #include <atomic>
 #include <new>
 #include <type_traits>
+#include <vector>
 
 #include "../../include/b200meters.h"
 
@@ -106,6 +107,26 @@ struct RaggedLen {
         for (int s = 0; s < 2; ++s) { if (h[s]) cudaFreeHost (h[s]); if (ev[s]) cudaEventDestroy (ev[s]); h[s] = nullptr; ev[s] = nullptr; }
         d = nullptr;
     }
+};
+
+// The album member list of b200m_ebu_group_reduce and b200m_dr14_group_reduce.  group (host, n entries) maps instance i to an
+// album 0 .. n_groups - 1 or to B200M_NO_GROUP.  group_check refuses n_groups outside 1 .. max_groups or an album id out of range
+// (B200M_E_INVAL; the caller has checked its pointers).  assign sorts the instances by album (a counting sort, each album's
+// members in instance order) and uploads in one copy the member list, each member's album, and each album's offset into the list
+// (n_groups + 1 words: album a's members are members[off[a] .. off[a + 1])).  It uploads nothing when group and n_groups are the
+// previous call's.
+int group_check (const uint32_t* group, uint32_t n, uint32_t n_groups, uint32_t max_groups);
+
+struct GroupList {
+    std::vector<uint32_t> of;                // the assignment as last uploaded (empty: none yet)
+    uint32_t n_groups = 0, members = 0;      // its album count and number of members
+    RaggedLen up;                            // up.d: members [members], album [members], off [n_groups + 1]
+    const uint32_t* d_members () const { return up.d; }
+    const uint32_t* d_album () const { return up.d + members; }
+    const uint32_t* d_off () const { return up.d + 2 * (size_t)members; }
+    // max_groups: the bank's cap on n_groups, the same every call (it sizes the upload buffers)
+    int assign (const uint32_t* group, uint32_t n, uint32_t n_groups, uint32_t max_groups, cudaStream_t st);
+    void release () { up.release (); of.clear (); }
 };
 
 // The host/device path policy of a bank, the one place that keeps the ordering promise of include/b200meters.h (Conventions).

@@ -99,6 +99,29 @@ B200M_DEV void dr14_log_point (const PointLog& lg, int n_inst, int inst, int nch
     lg.written[inst] = w + 1;
 }
 
+// The mean of the loudest 20 % of the windows (:316-324): the bins of hist from the top down, 32 at a time by ballot, added in exactly
+// the reference's bin order until m_cut windows are counted.  Called by the whole warp; the bins are read from L2 (__ldcg).  Returns
+// the sum of cd^2 * count over the bins walked and their count in n_cut, the same in every lane.
+B200M_DEV float dr_walk (const uint32_t* hist, const float* cd, uint32_t m_cut, int lane, uint32_t& n_cut)
+{
+    float rms_score = 0.0f;
+    n_cut = 0;
+    for (int base = DR_HISTBINS - 32; base >= 0 && n_cut < m_cut; base -= 32) {
+        const int b = base + lane;
+        const uint32_t bc = b > 0 ? __ldcg (&hist[b]) : 0u;
+        unsigned mask = __ballot_sync (0xffffffffu, bc != 0);
+        while (mask && n_cut < m_cut) {
+            const int l = 31 - __clz (mask);
+            const uint32_t bcl = __shfl_sync (0xffffffffu, bc, l);
+            const float c = cd[base + l];
+            rms_score = __fadd_rn (rms_score, __fmul_rn (__fmul_rn (c, c), (float)bcl));
+            n_cut += bcl;
+            mask &= ~(1u << l);
+        }
+    }
+    return rms_score;
+}
+
 // dr14_calc_rms_score (:285-352) of the instances whose window closed in this block; one warp per instance.  With the window log
 // on (lg.pts), lane 0 also appends the window's point.
 // RAG: a ragged block, instance i ran over its first rlen[i] frames: its window closed only if the cut lies before that.
@@ -141,21 +164,7 @@ __global__ void dr14_score_kernel (int n_inst, int nch, float n_sample_cnt_f, Dr
         }
         __syncwarp ();
         uint32_t n_cut = 0; float rms_score = 0.0f;
-        if (nf > 2) {                                          // mean of the loudest 20 % (:316-324), bins in descending order
-            for (int base = DR_HISTBINS - 32; base >= 0 && n_cut < m_cut; base -= 32) {
-                const int b = base + lane;
-                const uint32_t bc = b > 0 ? __ldcg (&hist[b]) : 0u;      // L2 read: lane 0 has just incremented one bin
-                unsigned mask = __ballot_sync (0xffffffffu, bc != 0);
-                while (mask && n_cut < m_cut) {
-                    const int l = 31 - __clz (mask);
-                    const uint32_t bcl = __shfl_sync (0xffffffffu, bc, l);
-                    const float cd = s.cd[base + l];
-                    rms_score = __fadd_rn (rms_score, __fmul_rn (__fmul_rn (cd, cd), (float)bcl));
-                    n_cut += bcl;
-                    mask &= ~(1u << l);
-                }
-            }
-        }
+        if (nf > 2) rms_score = dr_walk (hist, s.cd, m_cut, lane, n_cut);      // L2 reads: lane 0 has just incremented one bin
         if (lane == 0) {
             s.m_rms[ch] = n_cut > 0 ? dr_coeff_to_db (__fsqrt_rn (__fdiv_rn (rms_score, (float)n_cut))) : -81.0f;
             const float pc = s.emit_peak[ch];                  // second highest window peak (:339-351)
@@ -224,6 +233,172 @@ __global__ void dr14_reset_kernel (const uint32_t* inst, size_t n_sel, int nch, 
         }
 }
 
+// Album DR (b200m_dr14_group_reduce / _finish).  The member list is the EBU bank's (GroupList, common.cuh): instances sorted by album,
+// each member's album beside it, and each album's slice of the list.
+//
+// dr14_group_reduce_kernel: a 2-D grid of member chunks x column tiles.  CTA (x, y) takes DRG_CHUNK consecutive members of the list
+// and DRG_TILE words of their histogram rows (an instance's nch x 8000 bins are contiguous: 16 B loads, coalesced); each thread keeps
+// one uint4 of partial sums, DRG_BATCH members' loads in flight before their sums, and adds its non-zero sums into the album's
+// zeroed row with integer atomicAdd when the album changes: order-independent, hence exact.  The histograms are sparse (a track
+// fills a few dozen bins per channel), so the cost is the read.
+constexpr int DRG_THREADS = 256, DRG_CHUNK = 16, DRG_BATCH = 4;
+constexpr int DRG_TILE = DRG_THREADS * 4;                       // histogram words per column tile
+
+__global__ void __launch_bounds__ (DRG_THREADS)
+dr14_group_reduce_kernel (const uint32_t* __restrict__ hist, int row_words, const uint32_t* __restrict__ members,
+                          const uint32_t* __restrict__ album, int n_members, int* __restrict__ rows)
+{
+    __shared__ uint32_t mem[DRG_CHUNK], alb[DRG_CHUNK];
+    const int first = blockIdx.x * DRG_CHUNK, n = min (DRG_CHUNK, n_members - first);
+    if (threadIdx.x < n) { mem[threadIdx.x] = members[first + threadIdx.x]; alb[threadIdx.x] = album[first + threadIdx.x]; }
+    __syncthreads ();
+    const int col = blockIdx.y * DRG_TILE + threadIdx.x * 4;
+    if (col >= row_words) return;                               // row_words is a multiple of 4: a thread's 4 columns are all in
+    const uint4* src = reinterpret_cast<const uint4*> (hist + col);
+    const size_t pitch = (size_t)row_words / 4;
+    uint4 acc = make_uint4 (0, 0, 0, 0);
+    auto flush = [&] (uint32_t a) {
+        int* row = rows + (size_t)a * (row_words + 2) + col;
+        if (acc.x) atomicAdd (row, (int)acc.x);
+        if (acc.y) atomicAdd (row + 1, (int)acc.y);
+        if (acc.z) atomicAdd (row + 2, (int)acc.z);
+        if (acc.w) atomicAdd (row + 3, (int)acc.w);
+        acc = make_uint4 (0, 0, 0, 0);
+    };
+    uint32_t cur = alb[0];
+    for (int k0 = 0; k0 < n; k0 += DRG_BATCH) {
+        uint4 v[DRG_BATCH];
+#pragma unroll
+        for (int q = 0; q < DRG_BATCH; ++q)
+            v[q] = k0 + q < n ? __ldcs (src + mem[k0 + q] * pitch) : make_uint4 (0, 0, 0, 0);      // read once: streaming loads
+#pragma unroll
+        for (int q = 0; q < DRG_BATCH; ++q) {
+            if (k0 + q < n && alb[k0 + q] != cur) { flush (cur); cur = alb[k0 + q]; }           // uniform across the CTA
+            acc.x += v[q].x; acc.y += v[q].y; acc.z += v[q].z; acc.w += v[q].w;
+        }
+    }
+    flush (cur);
+}
+
+// The two largest of two top-two pairs (h0 >= h1, never NaN): the two largest of their union
+struct Top2 { float h0, h1; };
+B200M_DEV Top2 top2_merge (const Top2 a, const Top2 b)
+{
+    const bool ab = a.h0 >= b.h0;
+    const float lo = ab ? b.h0 : a.h0, h1 = a.h1 >= b.h1 ? a.h1 : b.h1;
+    return {ab ? a.h0 : b.h0, lo >= h1 ? lo : h1};
+}
+
+B200M_DEV Top2 top2_shfl_xor (const Top2 t, int o)
+{
+    return {__shfl_xor_sync (0xffffffffu, t.h0, o), __shfl_xor_sync (0xffffffffu, t.h1, o)};
+}
+
+// dr14_group_peaks_kernel: one warp per album walks its slice of the member list: the top two of the members' peak_hist pairs and
+// the largest non-NaN m_dbtp per channel (fmaxf ignores NaN; an album without members holds 0), and the album's window and member
+// counts, written into the last two words of its row.
+constexpr int DRG_PEAK_WARPS = 8;
+
+__global__ void __launch_bounds__ (DRG_PEAK_WARPS * 32)
+dr14_group_peaks_kernel (int n_groups, int nch, const uint32_t* __restrict__ members, const uint32_t* __restrict__ off,
+                         const float* __restrict__ peak_hist, const float* __restrict__ m_dbtp,
+                         const unsigned long long* __restrict__ numfrag, int row_words, int* __restrict__ rows, float* __restrict__ peaks)
+{
+    const int lane = threadIdx.x & 31, g = blockIdx.x * DRG_PEAK_WARPS + (threadIdx.x >> 5);
+    if (g >= n_groups) return;
+    const uint32_t a = off[g], b = off[g + 1];
+    const float nan = __int_as_float (0x7fc00000);
+    Top2 t[2] = {{0.0f, 0.0f}, {0.0f, 0.0f}};
+    float hold[2] = {nan, nan};
+    unsigned long long nf = 0;
+    for (uint32_t k = a + lane; k < b; k += 32) {
+        const size_t m = members[k];
+        nf += numfrag[m];
+#pragma unroll
+        for (int c = 0; c < 2; ++c)
+            if (c < nch) {
+                const size_t ch = m * nch + c;
+                t[c] = top2_merge (t[c], {peak_hist[2 * ch], peak_hist[2 * ch + 1]});
+                hold[c] = fmaxf (hold[c], m_dbtp[ch]);
+            }
+    }
+#pragma unroll
+    for (int o = 16; o; o >>= 1) {
+        nf += __shfl_xor_sync (0xffffffffu, nf, o);
+#pragma unroll
+        for (int c = 0; c < 2; ++c) {
+            t[c] = top2_merge (t[c], top2_shfl_xor (t[c], o));
+            hold[c] = fmaxf (hold[c], __shfl_xor_sync (0xffffffffu, hold[c], o));
+        }
+    }
+    if (lane == 0) {
+        int* tail = rows + (size_t)g * (row_words + 2) + row_words;
+        tail[0] = (int)nf; tail[1] = (int)(b - a);
+        for (int c = 0; c < nch; ++c) {
+            float* p = peaks + ((size_t)g * nch + c) * 3;
+            p[0] = t[c].h0; p[1] = t[c].h1; p[2] = b > a ? hold[c] : 0.0f;
+        }
+    }
+}
+
+// dr14_group_finish_kernel: one warp per (album, channel), DRG_FIN_ALBUMS albums per CTA.  The warp merges the n_parts peak blocks,
+// then scores the channel's row as dr14_score_kernel scores an instance (dr_walk); lane 0 of an album's channel-0 warp applies the
+// port arithmetic (dr_ports) to both channels.
+constexpr int DRG_FIN_ALBUMS = 4;
+
+__global__ void __launch_bounds__ (DRG_FIN_ALBUMS * 64)
+dr14_group_finish_kernel (int n_groups, int nch, uint32_t n_parts, const int* rows, const float* __restrict__ peaks,
+                          const float* __restrict__ cd, b200m_dr14_album* __restrict__ out)
+{
+    __shared__ float s_rms[DRG_FIN_ALBUMS][2], s_p2[DRG_FIN_ALBUMS][2], s_hold[DRG_FIN_ALBUMS][2];
+    const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
+    const int ga = warp / nch, c = warp % nch, g = blockIdx.x * DRG_FIN_ALBUMS + ga;
+    const int row_words = nch * DR_HISTBINS;
+    uint32_t nf = 0;
+    if (g < n_groups) {
+        const int* row = rows + (size_t)g * (row_words + 2);
+        nf = (uint32_t)row[row_words];
+        Top2 t = {0.0f, 0.0f};
+        float hold = __int_as_float (0x7fc00000);
+        for (uint32_t p = lane; p < n_parts; p += 32) {
+            const float* q = peaks + (((size_t)p * n_groups + g) * nch + c) * 3;
+            t = top2_merge (t, {q[0], q[1]});
+            hold = fmaxf (hold, q[2]);
+        }
+#pragma unroll
+        for (int o = 16; o; o >>= 1) {
+            t = top2_merge (t, top2_shfl_xor (t, o));
+            hold = fmaxf (hold, __shfl_xor_sync (0xffffffffu, hold, o));
+        }
+        const float mc = floorf (__double2float_rn (__ddiv_rn ((double)nf, 5.0)));      // MAX (1, floorf (num_fragments / 5.0)) (:301)
+        const uint32_t m_cut = (uint32_t)(1.0f > mc ? 1.0f : mc);
+        uint32_t n_cut = 0; float rms_score = 0.0f;
+        if (nf > 2) rms_score = dr_walk (reinterpret_cast<const uint32_t*> (row) + c * DR_HISTBINS, cd, m_cut, lane, n_cut);
+        if (lane == 0) {
+            s_rms[ga][c] = n_cut > 0 ? dr_coeff_to_db (__fsqrt_rn (__fdiv_rn (rms_score, (float)n_cut))) : -81.0f;
+            s_p2[ga][c] = nf > 2 ? dr_coeff_to_db (t.h1) : -81.0f;
+            s_hold[ga][c] = dr_coeff_to_db (hold);
+        }
+    }
+    __syncthreads ();
+    if (g >= n_groups || c != 0 || lane != 0) return;
+    const float nan = __int_as_float (0x7fc00000);
+    const DrPorts d = dr_ports (s_rms[ga], s_p2[ga], nch);
+    b200m_dr14_album o;
+    for (int k = 0; k < 2; ++k) {
+        const bool on = k < nch;
+        o.m_rms[k] = on ? s_rms[ga][k] : nan;
+        o.peak2[k] = on ? s_p2[ga][k] : nan;
+        o.dr[k] = on ? d.dr[k] : nan;
+        o.m_peak[k] = on ? s_hold[ga][k] : nan;
+    }
+    o.dr_total = nch > 1 ? d.dr_total : nan;
+    o.block_count = dr_block_count (nf);
+    const int* tail = rows + (size_t)g * (row_words + 2) + row_words;
+    o.windows = (float)nf; o.members = (float)(uint32_t)tail[1];
+    out[g] = o;
+}
+
 }  // namespace b200m
 
 using namespace b200m;
@@ -239,6 +414,8 @@ struct b200m_dr14 {
     float *d_rms_sum = nullptr, *d_peak_cur = nullptr, *d_cd = nullptr;
     Dr14State st{}; b200m_dr14_result* d_out = nullptr;
     PointRing ring;                                            // the window log (b200m_dr14_log_enable), off while ring.log.pts is null
+    GroupList grp;                                             // album DR (b200m_dr14_group_reduce): the member list
+    b200m_dr14_album* d_alb = nullptr; uint32_t alb_cap = 0;   // the finish's device output, grown on demand
     BankPath path;
 };
 
@@ -370,6 +547,7 @@ int b200m_dr14_destroy (b200m_dr14* h)
                   h->st.m_dbtp, h->st.numfrag, h->st.phase, h->st.nwin, h->d_sel, h->st.hist, h->d_cd, h->d_out};
     for (void* p : ps) cudaFree (p);
     h->ring.release ();
+    h->grp.release (); cudaFree (h->d_alb);
     h->path.release ();
     delete h;
     return 0;
@@ -483,6 +661,54 @@ int b200m_dr14_log_drain (b200m_dr14* h, b200m_dr14_point* out, uint32_t* count,
     DeviceGuard g (h->device);
     // 16 points per tile: the drain's static tile of 32 x (16 x 14 + 1) floats stays under 48 KB
     return log_drain<DR_LOG_FIELDS, 16> (h->ring, h->n_inst, (float*)out, count, lost, h->path.stream (stream));
+}
+
+int b200m_dr14_group_reduce (b200m_dr14* h, const uint32_t* group, uint32_t n_groups, int32_t* d_rows, float* d_peaks, void* stream)
+{
+    if (!h || !group || !d_rows || !d_peaks) return set_err (B200M_E_INVAL, "NULL argument");
+    if (!h->dr_mode) return set_err (B200M_E_UNSUPPORTED, "a TPnRMS bank has no window histograms to pool");
+    if (int rc = group_check (group, h->n_inst, n_groups, B200M_DR14_MAX_GROUPS)) return rc;
+    DeviceGuard g (h->device);
+    cudaStream_t st = h->path.stream (stream);
+    if (int rc = h->grp.assign (group, h->n_inst, n_groups, B200M_DR14_MAX_GROUPS, st)) return rc;
+    const uint32_t nm = h->grp.members, rw = h->nch * DR_HISTBINS;
+    B200M_CUDA (cudaMemsetAsync (d_rows, 0, (size_t)n_groups * (rw + 2) * sizeof (int32_t), st));
+    if (nm) {
+        const dim3 grid ((nm + DRG_CHUNK - 1) / DRG_CHUNK, (rw + DRG_TILE - 1) / DRG_TILE);
+        dr14_group_reduce_kernel<<<grid, DRG_THREADS, 0, st>>> (h->st.hist, (int)rw, h->grp.d_members (), h->grp.d_album (), (int)nm, d_rows);
+        B200M_LAUNCHED (1);
+    }
+    dr14_group_peaks_kernel<<<(n_groups + DRG_PEAK_WARPS - 1) / DRG_PEAK_WARPS, DRG_PEAK_WARPS * 32, 0, st>>> (
+        (int)n_groups, (int)h->nch, h->grp.d_members (), h->grp.d_off (), h->st.peak_hist, h->st.m_dbtp, h->st.numfrag, (int)rw, d_rows, d_peaks);
+    B200M_LAUNCHED (1);
+    B200M_CUDA (cudaGetLastError ());
+    return 0;
+}
+
+int b200m_dr14_group_finish (b200m_dr14* h, const int32_t* d_rows, const float* d_peaks, uint32_t n_parts, uint32_t n_groups,
+                             b200m_dr14_album* out, void* stream)
+{
+    if (!h || !d_rows || !d_peaks || !out) return set_err (B200M_E_INVAL, "NULL argument");
+    if (!h->dr_mode) return set_err (B200M_E_UNSUPPORTED, "a TPnRMS bank has no window histograms to pool");
+    if (n_groups == 0 || n_groups > B200M_DR14_MAX_GROUPS) return set_err (B200M_E_INVAL, "n_groups %u outside 1..%u", n_groups, B200M_DR14_MAX_GROUPS);
+    if (n_parts == 0) return set_err (B200M_E_INVAL, "n_parts is 0");
+    DeviceGuard g (h->device);
+    cudaStream_t st = h->path.stream (stream);
+    if (n_groups > h->alb_cap) {                               // the previous call synchronised: nothing in flight uses the old buffer
+        cudaFree (h->d_alb); h->d_alb = nullptr; h->alb_cap = 0;
+        if (cudaMalloc ((void**)&h->d_alb, (size_t)n_groups * sizeof (b200m_dr14_album)) != cudaSuccess) {
+            cudaGetLastError ();
+            return set_err (B200M_E_NOMEM, "album results of %u groups: out of device memory", n_groups);
+        }
+        h->alb_cap = n_groups;
+    }
+    dr14_group_finish_kernel<<<(n_groups + DRG_FIN_ALBUMS - 1) / DRG_FIN_ALBUMS, DRG_FIN_ALBUMS * 32 * h->nch, 0, st>>> (
+        (int)n_groups, (int)h->nch, n_parts, d_rows, d_peaks, h->d_cd, h->d_alb);
+    B200M_LAUNCHED (1);
+    B200M_CUDA (cudaGetLastError ());
+    B200M_CUDA (cudaMemcpyAsync (out, h->d_alb, (size_t)n_groups * sizeof (b200m_dr14_album), cudaMemcpyDeviceToHost, st));
+    B200M_CUDA (cudaStreamSynchronize (st));
+    return 0;
 }
 
 }  // extern "C"

@@ -807,9 +807,8 @@ struct b200m_ebu {
     // a ragged block (b200m_ebu_process_ragged_*, b200m_r128_run_ragged_*): the upload of its per-instance lengths, and the instances
     // whose length differs from nfram (scratch: index, fragments in the block, S-period position div2)
     RaggedLen rag;
-    // album reduce (b200m_ebu_group_reduce): the assignment as last uploaded (empty: none yet) and its upload to grp.d, the member
-    // list (grp_members instances sorted by album) followed by each member's album; the finish's device output, grown on demand
-    std::vector<uint32_t> grp_of; RaggedLen grp; uint32_t grp_members = 0;
+    // album reduce (b200m_ebu_group_reduce): the member list (GroupList, common.cuh); the finish's device output, grown on demand
+    GroupList grp;
     float* d_grp5 = nullptr; uint32_t grp5_cap = 0;
     struct Rag { uint32_t i; int nf, d2; };
     std::vector<Rag> rg;
@@ -1428,32 +1427,15 @@ int b200m_ebu_mix_finish (b200m_ebu* h, const int32_t* d_mix, float out5[5], voi
 int b200m_ebu_group_reduce (b200m_ebu* h, const uint32_t* group, uint32_t n_groups, int32_t* d_out, void* stream)
 {
     if (!h || !group || !d_out) return set_err (B200M_E_INVAL, "NULL argument");
-    if (n_groups == 0 || n_groups > B200M_MAX_GROUPS) return set_err (B200M_E_INVAL, "n_groups %u outside 1..%u", n_groups, B200M_MAX_GROUPS);
-    const uint32_t n = h->n_inst;
-    for (uint32_t i = 0; i < n; ++i)
-        if (group[i] >= n_groups && group[i] != B200M_NO_GROUP)
-            return set_err (B200M_E_INVAL, "group[%u] = %u is neither < n_groups = %u nor B200M_NO_GROUP", i, group[i], n_groups);
+    if (int rc = group_check (group, h->n_inst, n_groups, B200M_MAX_GROUPS)) return rc;
     DeviceGuard g (h->device);
     cudaStream_t st = h->stream (stream);
-    if (h->grp_of.empty () || memcmp (group, h->grp_of.data (), n * sizeof (uint32_t))) {
-        // counting sort of the instances by album, each album's members in instance order, and the album of each member
-        cudaError_t e = cudaSuccess;
-        uint32_t* w = h->grp.stage (2 * (size_t)n, &e);
-        if (!w) return cuda_fail (e, "b200m_ebu_group_reduce", __FILE__, __LINE__);
-        std::vector<uint32_t> off (n_groups + 1, 0);
-        for (uint32_t i = 0; i < n; ++i) if (group[i] != B200M_NO_GROUP) off[group[i] + 1]++;
-        for (uint32_t a = 0; a < n_groups; ++a) off[a + 1] += off[a];
-        const uint32_t nm = off[n_groups];
-        for (uint32_t i = 0; i < n; ++i)
-            if (group[i] != B200M_NO_GROUP) { const uint32_t p = off[group[i]]++; w[p] = i; w[nm + p] = group[i]; }
-        B200M_CUDA (h->grp.upload (2 * (size_t)nm, st));
-        h->grp_of.assign (group, group + n); h->grp_members = nm;
-    }
-    const uint32_t nm = h->grp_members;
+    if (int rc = h->grp.assign (group, h->n_inst, n_groups, B200M_MAX_GROUPS, st)) return rc;
+    const uint32_t nm = h->grp.members;
     B200M_CUDA (cudaMemsetAsync (d_out, 0, (size_t)n_groups * B200M_MIX_WORDS * sizeof (int32_t), st));
     if (nm) {
-        ebu_group_reduce_kernel<<<(nm + GRP_CHUNK - 1) / GRP_CHUNK, GRP_THREADS, 0, st>>> (h->d_histM, h->d_histS, h->d_cnt, h->grp.d,
-                                                                                         h->grp.d + nm, (int)nm, d_out);
+        ebu_group_reduce_kernel<<<(nm + GRP_CHUNK - 1) / GRP_CHUNK, GRP_THREADS, 0, st>>> (h->d_histM, h->d_histS, h->d_cnt, h->grp.d_members (),
+                                                                                         h->grp.d_album (), (int)nm, d_out);
         B200M_LAUNCHED (1);
     }
     B200M_CUDA (cudaGetLastError ());

@@ -49,6 +49,33 @@ int ragged_check (uint32_t n, uint32_t nfram, const uint32_t* len)
     return rag ? 1 : 0;
 }
 
+int group_check (const uint32_t* group, uint32_t n, uint32_t n_groups, uint32_t max_groups)
+{
+    if (n_groups == 0 || n_groups > max_groups) return set_err (B200M_E_INVAL, "n_groups %u outside 1..%u", n_groups, max_groups);
+    for (uint32_t i = 0; i < n; ++i)
+        if (group[i] >= n_groups && group[i] != B200M_NO_GROUP)
+            return set_err (B200M_E_INVAL, "group[%u] = %u is neither < n_groups = %u nor B200M_NO_GROUP", i, group[i], n_groups);
+    return 0;
+}
+
+int GroupList::assign (const uint32_t* group, uint32_t n, uint32_t ng, uint32_t max_groups, cudaStream_t st)
+{
+    if (!of.empty () && ng == n_groups && !memcmp (group, of.data (), n * sizeof (uint32_t))) return 0;
+    cudaError_t e = cudaSuccess;
+    uint32_t* w = up.stage (2 * (size_t)n + max_groups + 1, &e);
+    if (!w) return cuda_fail (e, "GroupList::assign", __FILE__, __LINE__);
+    std::vector<uint32_t> off (ng + 1, 0);
+    for (uint32_t i = 0; i < n; ++i) if (group[i] != B200M_NO_GROUP) off[group[i] + 1]++;
+    for (uint32_t a = 0; a < ng; ++a) off[a + 1] += off[a];
+    const uint32_t nm = off[ng];
+    memcpy (w + 2 * (size_t)nm, off.data (), (ng + 1) * sizeof (uint32_t));
+    for (uint32_t i = 0; i < n; ++i)
+        if (group[i] != B200M_NO_GROUP) { const uint32_t p = off[group[i]]++; w[p] = i; w[nm + p] = group[i]; }
+    B200M_CUDA (up.upload (2 * (size_t)nm + ng + 1, st));
+    of.assign (group, group + n); n_groups = ng; members = nm;
+    return 0;
+}
+
 int BankPath::enter_device ()
 {
     if (last_host) B200M_CUDA (cudaStreamSynchronize (own));

@@ -1,4 +1,4 @@
-"""Multi-GPU plumbing: channel-instance sharding (no data-path collective) and the one optional exchange.
+"""Multi-GPU plumbing: channel-instance sharding (no data-path collective) and two optional exchanges.
 
 Every metering instance is self-contained (SURVEY.md §8e), so N GPUs simply own contiguous instance ranges:
 rank r of W processes instances  [r*n/W, (r+1)*n/W).  The only cross-instance quantity is the whole-mix gated
@@ -6,8 +6,12 @@ loudness: the int32 sum of all instances' hist_M / hist_S (+ counts), reduced pe
 b200m_ebu_mix_reduce and across GPUs by ONE all-reduce of B200M_MIX_WORDS int32 (NCCL on GPUs, gloo in CPU
 tests); integer sums are order independent, hence bit-exact for any GPU count.  Album loudness works the same way with
 one row per album (b200m_ebu_group_reduce): the clips of one album may sit on different GPUs.
+The second exchange is album DR (b200m_dr14_group_reduce): each album's int32 row of summed window histograms and counts is
+all-reduced the same way, but its window peaks cannot be summed (an album's second-highest window peak is the second largest over
+all its tracks), so every rank's [G, nch, 3] peaks are all-gathered and b200m_dr14_group_finish merges the W parts by value.
 """
 MIX_WORDS = 1508
+DR14_HISTBINS = 8000
 
 
 def shard_range(n_total, rank, world):
@@ -35,6 +39,27 @@ def allreduce_mix(mix, group=None):
     if dist.is_available() and dist.is_initialized() and dist.get_world_size(group) > 1:
         dist.all_reduce(mix, op=dist.ReduceOp.SUM, group=group)
     return mix
+
+
+def allreduce_dr14_groups(rows, peaks, group=None):
+    """album DR across ranks: sum the rows of DR14.group_reduce (int32[G, nch * 8000 + 2], the same G on every rank) in place, and
+    all-gather its peaks (float32[G, nch, 3]).  Returns the [W, G, nch, 3] stack of every rank's peaks in rank order (W = 1 without
+    a process group), which DR14.group_finish takes with the summed rows."""
+    import torch
+    import torch.distributed as dist
+    if rows.dtype != torch.int32 or rows.dim() != 2:
+        raise ValueError("rows must be int32[G, nch * %d + 2]" % DR14_HISTBINS)
+    g, words = rows.shape
+    if peaks.dtype != torch.float32 or peaks.dim() != 3 or peaks.shape[0] != g or peaks.shape[2] != 3 \
+            or words != peaks.shape[1] * DR14_HISTBINS + 2:
+        raise ValueError("peaks must be float32[G, nch, 3] matching rows int32[G, nch * %d + 2]" % DR14_HISTBINS)
+    if dist.is_available() and dist.is_initialized() and dist.get_world_size(group) > 1:
+        dist.all_reduce(rows, op=dist.ReduceOp.SUM, group=group)
+        p = peaks.contiguous()
+        parts = [torch.empty_like(p) for _ in range(dist.get_world_size(group))]
+        dist.all_gather(parts, p, group=group)
+        return torch.stack(parts)
+    return peaks.unsqueeze(0).contiguous()
 
 
 def gather_results(local, group=None):
