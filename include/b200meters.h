@@ -652,6 +652,19 @@ int b200m_spec_set_precision (b200m_spec* h, int mode);
 int b200m_spec_results (b200m_spec* h, float* out60, void* stream);
 int b200m_spec_state (b200m_spec* h, uint32_t inst, double* z360, float* val30, float* max30, void* stream);
 int b200m_spec_coeffs (const b200m_spec* h, double* W1080);              /* [30][6][6] a0 a1 a2 b0 b1 b2 */
+/* Long-term average spectrum (an extension; the reference keeps only the smoothed level and its peak hold): with the plane on, every
+ * band of every instance adds its per-frame power s = v * v (the value spectrum_run smooths, src/spectrumlv2.c:221-226, after
+ * bandpass_process, src/spectr.c:79-87) to a double sum, sum = sum + (double) s frame by frame in frame order, and counts the frames
+ * it added.  A frame whose s is not finite adds nothing and is not counted (non-finite input leaves the filters NaN until the
+ * end-of-run scrub, :229-236).  Ragged blocks add an instance's own len[i] frames only; B200M_PREC_FMA adds its own v.  Ports and
+ * b200m_spec_state are bit-identical with the plane on or off; with it off the bank runs exactly the kernel it runs without it.
+ * enable != 0: allocates the plane on first use (B200M_E_NOMEM if the device cannot hold 16 x 32 bytes per instance) and zeroes every
+ * instance's sums and counts, also when it was on already; 0: turns it off.  While it is on, b200m_spec_clear also zeroes the
+ * cleared instances' sums and counts.  Ordered like the getters. */
+int b200m_spec_ltas_enable (b200m_spec* h, int enable, void* stream);
+/* host sums [n_inst][30] and counts [n_inst][30] of every instance, in one copy and one synchronisation of the stream, ordered like
+ * b200m_spec_results; the band's long-term average power is sums / counts.  B200M_E_INVAL while the plane is off. */
+int b200m_spec_ltas_read (b200m_spec* h, double* sums, uint64_t* counts, void* stream);
 
 /* ======================================================================================
  * Phasewheel FFT analysis bank — replaces fftx_init / fftx_run / ft_analyze (gui/fft.c:208-361)

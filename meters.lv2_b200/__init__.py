@@ -208,6 +208,8 @@ _PROTOS = {
     "b200m_spec_results": (C.c_int, [_v, _v, _v]),
     "b200m_spec_state": (C.c_int, [_v, C.c_uint32, _v, _v, _v, _v]),
     "b200m_spec_coeffs": (C.c_int, [_v, _v]),
+    "b200m_spec_ltas_enable": (C.c_int, [_v, C.c_int, _v]),
+    "b200m_spec_ltas_read": (C.c_int, [_v, _v, _v, _v]),
     # phasewheel
     "b200m_pw_create": (C.c_int, [C.POINTER(_v), C.c_int, C.c_uint32, C.c_uint32, C.c_double]),
     "b200m_pw_set_mode": (C.c_int, [_v, C.c_int]),
@@ -865,6 +867,10 @@ class DR14(_Bank):
         return out
 
 
+# the 30 bands' nominal centre frequencies in Hz, 1000 * 2^((i - 16) / 3) (src/spectrumlv2.c:100-118): 24.8 Hz .. 20.2 kHz
+SPEC_BAND_HZ = 1000.0 * 2.0 ** ((np.arange(30) - 16) / 3.0)
+
+
 class Spectr30(_Bank):
     """N x the spectr30 plugin (src/spectrumlv2.c:73-257): ports 0..59 per instance."""
     _pfx = "spec"
@@ -915,6 +921,18 @@ class Spectr30(_Bank):
         W = np.empty((30, 6, 6), np.float64)
         _ck(lib().b200m_spec_coeffs(self.h, _np_ptr(W)))
         return W
+
+    def ltas_enable(self, on=True, stream=None):
+        """the long-term average spectrum plane (b200m_spec_ltas_enable): on, every band of every instance adds up its per-frame
+        power v * v and counts the finite frames it added; (re)enabling zeroes every instance's sums and counts"""
+        _ck(lib().b200m_spec_ltas_enable(self.h, int(bool(on)), _stream_ptr(stream)))
+
+    def ltas(self, stream=None):
+        """(sums float64 [n_inst, 30], counts int64 [n_inst, 30]) of the LTAS plane (b200m_spec_ltas_read): the band's average power
+        is sums / counts; raises while the plane is off"""
+        s = np.empty((self.n_inst, 30), np.float64); c = np.empty((self.n_inst, 30), np.uint64)
+        _ck(lib().b200m_spec_ltas_read(self.h, _np_ptr(s), _np_ptr(c), _stream_ptr(stream)))
+        return s, c.astype(np.int64)
 
 
 class Phasewheel(_Bank):
@@ -1319,3 +1337,88 @@ def programme_stats(x, lengths, rate=48000.0, block=1024, device=0):
             sdh.close()
     return dict(bim_hist=b["hist"], bim_cnt=b["cnt"], bim_minmax=b["minmax"], bim_itime=b["itime"],
                 sdh_hist=h, sdh_max_peak=mp, sdh_avg_tmp_var=av, sdh_itime=it)
+
+
+def _ltas_db(p):
+    """10 log10 (2 p) of average band powers p, -100 where sqrt (2 p) <= 1e-5 or p is NaN: the scale and floor of the spectrum's
+    level ports (src/spectrumlv2.c:240-247), so a settled steady tone reads the same here and in its band's port"""
+    with np.errstate(invalid="ignore", divide="ignore"):
+        return np.where(np.sqrt(2.0 * p) > 1e-5, 10.0 * np.log10(2.0 * p), -100.0)
+
+
+def _ltas(sums, counts):
+    """sums / counts, NaN where the count is 0"""
+    with np.errstate(invalid="ignore", divide="ignore"):
+        return np.where(counts > 0, sums / np.maximum(counts, 1), np.nan)
+
+
+def spectrum_albums(sums, counts, peak_db, groups):
+    """Album long-term average spectra from per-clip rows: programme_spectrum's sums, counts and peak_db, or those of several banks
+    (shards on several GPUs) concatenated in clip order, e.g. with shard.gather_results.  groups: N album ids (>= 0, or -1 for a clip
+    in no album).  An album's sums are its members' sums added in ascending clip index and its counts the sum of theirs, so the
+    result does not depend on how the clips were split between banks.  Returns a dict for G = max(groups) + 1 albums: album_ltas
+    (float64 [G, 30], summed sums / summed counts), album_ltas_db (float64 [G, 30], on the level ports' scale), album_peak_db
+    (float32 [G, 30], the largest member peak_db) and album_n_clips (int64 [G]).  An album without members reads NaN, -100, -100
+    and 0."""
+    sums = np.asarray(sums, np.float64); counts = np.asarray(counts, np.int64); peak_db = np.asarray(peak_db, np.float32)
+    n = sums.shape[0] if sums.ndim == 2 else -1
+    if n < 0 or sums.shape != (n, 30) or counts.shape != (n, 30) or peak_db.shape != (n, 30):
+        raise B200MError("sums, counts and peak_db must be [N, 30] rows of the same N clips")
+    grp = _groups(groups, n)
+    g = int(grp.max()) + 1 if n else 0
+    s, c = np.zeros((g, 30)), np.zeros((g, 30), np.int64)
+    pk = np.full((g, 30), -100.0, np.float32)
+    for i in np.flatnonzero(grp >= 0):                 # one clip at a time, in ascending index: a fixed order of the fp64 sums
+        a = grp[i]
+        s[a] += sums[i]
+        c[a] += counts[i]
+        np.maximum(pk[a], peak_db[i], out=pk[a])
+    ltas = _ltas(s, c)
+    return dict(album_ltas=ltas, album_ltas_db=_ltas_db(ltas), album_peak_db=pk,
+                album_n_clips=np.bincount(grp[grp >= 0], minlength=g).astype(np.int64))
+
+
+def programme_spectrum(x, lengths, rate=48000.0, nchan=2, speed=1.0, block=1024, precision=PREC_EXACT, device=0, groups=None):
+    """Long-term average spectrum (LTAS) of N clips of different lengths in 30 1/3-octave bands (SPEC_BAND_HZ), in one spectrum bank.
+
+    x: rows i * nchan + c of clip i (nchan 1 or 2; the bands analyse (L + R) / 2 of a stereo clip), clip i valid for its first
+    lengths[i] frames: a [N * nchan, >= max(lengths)] float32 numpy array / CPU tensor (host path) or CUDA tensor (device path), or a
+    callable f(offset, nfram) that returns frames offset .. offset + nfram - 1 of every row as such an array.  Frames past a clip's
+    length are never read into a result.  The clips are fed in blocks of `block` frames with clip i's length in block k
+    clamp(lengths[i] - k * block, 0, block) (Spectr30.process with lengths), so clip i's numbers are bit-identical (exact mode) to one
+    spectr30 instance fed only that clip in blocks of `block` frames, with the speed port at `speed` and the LTAS plane on
+    (Spectr30.ltas_enable).  precision=PREC_FMA runs the tolerance-mode filters (ltas_db within 1e-4 dB of exact mode).
+    Returns a dict of arrays of N rows of 30 bands:
+      sums (float64) and counts (int64): the LTAS plane after the clip's last frame (Spectr30.ltas): the sum of the band's per-frame
+        power v * v over the clip's frames where it is finite, and the number of those frames;
+      ltas (float64): sums / counts, the band's mean power, NaN where the count is 0;
+      ltas_db (float64): 10 log10 (2 ltas), -100 where sqrt (2 ltas) <= 1e-5 or ltas is NaN: the level ports' scale and floor, so a
+        settled steady tone reads the same as its band's level port;
+      peak_db (float32): ports 30..59 after the clip's last block, the peak hold of the level smoothed at `speed` over the whole clip
+        (never reset: the reset port is held at the value the instance's handshake state already has), -100 for an empty clip.
+    groups: None, or N album ids (>= 0, or -1 for a clip in no album): the dict then also holds spectrum_albums(sums, counts,
+    peak_db, groups)."""
+    ln, blocks = _programme_blocks(x, lengths, block, "no clips")
+    n = ln.size
+    grp = None if groups is None else _groups(groups, n)
+    bank = Spectr30(n, nchan, rate, device)
+    try:
+        bank.set_precision(precision)
+        bank.ltas_enable()
+        spd = np.full(n, speed, np.float32)
+        # a speed other than the initial 1 sets rst_h = 0 on the first run (src/spectrumlv2.c:170-177), else rst_h stays -4: a reset
+        # port equal to rst_h never starts the peak-reset handshake, whose max ports read -500
+        rst = np.full(n, -4.0 if spd[0] == 1.0 else 0.0, np.float32)
+        for _, xb, lb in blocks:
+            bank.process(xb, speed=spd, reset=rst, lengths=lb)
+        sums, counts = bank.ltas()
+        ports = bank.read()
+    finally:
+        bank.close()
+    peak_db = np.ascontiguousarray(ports[:, 30:])
+    peak_db[ln == 0] = -100.0
+    ltas = _ltas(sums, counts)
+    out = dict(sums=sums, counts=counts, ltas=ltas, ltas_db=_ltas_db(ltas), peak_db=peak_db)
+    if grp is not None:
+        out.update(spectrum_albums(sums, counts, peak_db, grp))
+    return out

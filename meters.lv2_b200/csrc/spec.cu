@@ -32,11 +32,14 @@ constexpr int SPEC_CLEAR_MAX = 1, SPEC_REINIT_GUI = 2, SPEC_PARITY = 4;   // SPE
 // contract's +-1e-4 dB (tests/test_cor_spec_gpu.py::test_spec_fma_mode_within_tolerance).
 // RAG (b200m_spec_process_ragged_*): instance inst runs over its first rlen[inst] <= nfram frames, the warp's block length (one
 // warp per instance: warp-uniform); rlen 0: the instance is not run at all.  Its `ac` phase is its own (SPEC_PARITY, kept by the host).
-template <bool FMA, bool RAG = false>
+// LTAS (b200m_spec_ltas_enable): each band also adds its per-frame power sq = v * v (the value the level smooths, src/spectrumlv2.c:
+// 221-226) to an fp64 sum, frame by frame in frame order, and counts the frames it added; a non-finite sq adds nothing and is not
+// counted.  Sum and count stay in registers across the block, so nothing the ports read changes.
+template <bool FMA, bool RAG = false, bool LTAS = false>
 __global__ void __launch_bounds__ (SPEC_WARPS * 32)
 spec_kernel (const float* __restrict__ in, size_t stride, int n_inst, int nfram, SpecRun rp, const SpecCtl* __restrict__ ctl, const double* __restrict__ coef,
              double* __restrict__ zst /* [inst][12][32] */, float* __restrict__ valf /* [inst][2][32] */, float* __restrict__ ports /* [inst][60] */,
-             const uint32_t* __restrict__ rlen)
+             const uint32_t* __restrict__ rlen, double* __restrict__ lsum /* [inst][32] */, unsigned long long* __restrict__ lcnt /* [inst][32] */)
 {
     __shared__ float raw[SPEC_WARPS][2][2][SPEC_TC];      // [warp][stage][channel][frame]
     __shared__ double dd[SPEC_WARPS][SPEC_TC];
@@ -82,6 +85,8 @@ spec_kernel (const float* __restrict__ in, size_t stride, int n_inst, int nfram,
     if (cp.flags & SPEC_CLEAR_MAX) mx = 0.0f;              // peak-hold reset (src/spectrumlv2.c:192-203)
     const float omega = cp.omega;
     const int ac0 = rp.ac0 ^ ((cp.flags & SPEC_PARITY) ? 1 : 0);
+    double psum = 0.0; unsigned long long pcnt = 0; uint32_t added = 0;
+    if constexpr (LTAS) { psum = lsum[(size_t)inst * 32 + lane]; pcnt = lcnt[(size_t)inst * 32 + lane]; }
 
     for (int c = 0; c < nchunks; ++c) {
         const int s0 = c * SPEC_TC;
@@ -139,6 +144,9 @@ spec_kernel (const float* __restrict__ in, size_t stride, int n_inst, int nfram,
             const float sq = __fmul_rn (v, v);
             val = __fadd_rn (val, __fmul_rn (omega, __fsub_rn (sq, val)));
             if (val > mx) mx = val;
+            if constexpr (LTAS) {
+                if (finitef_ (sq)) { psum = __dadd_rn (psum, (double)sq); ++added; }
+            }
         }
         __syncwarp ();
     }
@@ -156,6 +164,7 @@ spec_kernel (const float* __restrict__ in, size_t stride, int n_inst, int nfram,
         for (int s = 0; s < 6; ++s) { zp[(2 * s) * 32] = z1[s]; zp[(2 * s + 1) * 32] = z2[s]; }
         valf[(size_t)inst * 64 + lane] = __fadd_rn (val, 1e-20f);
         valf[(size_t)inst * 64 + 32 + lane] = mx;
+        if constexpr (LTAS) { lsum[(size_t)inst * 32 + lane] = psum; lcnt[(size_t)inst * 32 + lane] = pcnt + added; }
         const float vs = __fsqrt_rn (__double2float_rn (__dmul_rn (2.0, (double)val)));
         const float ms = __fsqrt_rn (__double2float_rn (__dmul_rn (2.0, (double)mx)));
         ports[(size_t)inst * 60 + lane] = vs > .00001f ? __double2float_rn (__dmul_rn (20.0, (double)log10f_glibc (vs))) : -100.0f;
@@ -181,6 +190,12 @@ struct b200m_spec {
     BankPath path;
     int fma = 0;                                          // B200M_PREC_FMA
     RaggedLen rag;                                        // ragged blocks: lengths per instance
+    // the LTAS plane (b200m_spec_ltas_enable): [n_inst][32] fp64 sums, then [n_inst][32] frame counts, in one allocation so that a
+    // read is one copy; allocated on first use, kept until destroy
+    void* d_ltas = nullptr;
+    bool ltas = false;
+    double* ltas_sum () const { return (double*)d_ltas; }
+    unsigned long long* ltas_cnt () const { return (unsigned long long*)((double*)d_ltas + (size_t)n_inst * 32); }
 };
 
 typedef std::complex<double> cplx;
@@ -310,9 +325,9 @@ static int spec_process (b200m_spec* h, const float* d_in, size_t stride, uint32
     rp.ac0 = (int)(h->frames & 1);
     h->frames += nfram;
     const unsigned grid = (h->n_inst + SPEC_WARPS - 1) / SPEC_WARPS;
-    const auto k = with_bools ([] (auto FMA, auto RAG) { return spec_kernel<FMA, RAG>; }, h->fma, len);
+    const auto k = with_bools ([] (auto FMA, auto RAG, auto LTAS) { return spec_kernel<FMA, RAG, LTAS>; }, h->fma, len, h->ltas);
     k<<<grid, SPEC_WARPS * 32, 0, st>>> (d_in, stride, (int)h->n_inst, (int)nfram, rp, h->d_ctl, h->d_coef, h->d_z, h->d_val, h->d_ports,
-                                         len ? h->rag.d : nullptr);
+                                         len ? h->rag.d : nullptr, h->ltas ? h->ltas_sum () : nullptr, h->ltas ? h->ltas_cnt () : nullptr);
     B200M_LAUNCHED (1);
     B200M_CUDA (cudaGetLastError ());
     if (len) {
@@ -373,7 +388,8 @@ int b200m_spec_destroy (b200m_spec* h)
     if (!h) return 0;
     DeviceGuard g (h->device);
     cudaDeviceSynchronize ();
-    cudaFree (h->d_coef); cudaFree (h->d_z); cudaFree (h->d_val); cudaFree (h->d_ports); cudaFree (h->d_ctl); h->rag.release (); h->path.release ();
+    cudaFree (h->d_coef); cudaFree (h->d_z); cudaFree (h->d_val); cudaFree (h->d_ports); cudaFree (h->d_ctl); cudaFree (h->d_ltas);
+    h->rag.release (); h->path.release ();
     delete h;
     return 0;
 }
@@ -432,6 +448,10 @@ int b200m_spec_clear (b200m_spec* h, int32_t inst, void* stream)
     B200M_CUDA (cudaMemsetAsync (h->d_z + (size_t)i0 * 12 * 32, 0, (size_t)n * 12 * 32 * sizeof (double), st));
     B200M_CUDA (cudaMemsetAsync (h->d_val + (size_t)i0 * 64, 0, (size_t)n * 64 * sizeof (float), st));
     B200M_CUDA (cudaMemsetAsync (h->d_ports + (size_t)i0 * 60, 0, (size_t)n * 60 * sizeof (float), st));
+    if (h->ltas) {                                         // a cleared slot is a fresh instance for the LTAS too
+        B200M_CUDA (cudaMemsetAsync (h->ltas_sum () + (size_t)i0 * 32, 0, (size_t)n * 32 * sizeof (double), st));
+        B200M_CUDA (cudaMemsetAsync (h->ltas_cnt () + (size_t)i0 * 32, 0, (size_t)n * 32 * sizeof (unsigned long long), st));
+    }
     for (uint32_t i = i0; i < i0 + n; ++i) spec_reset_ctl (h, i);
     spec_mark (h, i0, i0 + n);                             // uploaded by the next process call, on its stream
     return 0;
@@ -466,6 +486,45 @@ int b200m_spec_state (b200m_spec* h, uint32_t inst, double* z360, float* val30, 
     for (int b = 0; b < 30; ++b) {
         for (int s = 0; s < 6; ++s) { z360[(b * 6 + s) * 2] = zt[(2 * s) * 32 + b]; z360[(b * 6 + s) * 2 + 1] = zt[(2 * s + 1) * 32 + b]; }
         val30[b] = vt[b]; max30[b] = vt[32 + b];
+    }
+    return 0;
+}
+
+int b200m_spec_ltas_enable (b200m_spec* h, int enable, void* stream)
+{
+    if (!h) return set_err (B200M_E_INVAL, "NULL handle");
+    DeviceGuard g (h->device);
+    if (!enable) { h->ltas = false; return 0; }           // the plane's memory stays for the next enable
+    cudaStream_t st = h->path.stream (stream);
+    const size_t bytes = (size_t)h->n_inst * 32 * (sizeof (double) + sizeof (unsigned long long));
+    if (!h->d_ltas) {
+        const cudaError_t e = cudaMalloc (&h->d_ltas, bytes);
+        if (e != cudaSuccess) {
+            cudaGetLastError ();                               // a failed allocation is not sticky: later calls must not see it
+            h->d_ltas = nullptr;
+            if (e == cudaErrorMemoryAllocation) return set_err (B200M_E_NOMEM, "LTAS plane of %u instances: out of device memory", h->n_inst);
+            return cuda_fail (e, "b200m_spec_ltas_enable", __FILE__, __LINE__);
+        }
+    }
+    B200M_CUDA (cudaMemsetAsync (h->d_ltas, 0, bytes, st));
+    h->ltas = true;
+    return 0;
+}
+
+int b200m_spec_ltas_read (b200m_spec* h, double* sums, uint64_t* counts, void* stream)
+{
+    if (!h || !sums || !counts) return set_err (B200M_E_INVAL, "NULL argument");
+    if (!h->ltas) return set_err (B200M_E_INVAL, "the LTAS plane is off (b200m_spec_ltas_enable)");
+    DeviceGuard g (h->device);
+    cudaStream_t st = h->path.stream (stream);
+    const size_t n32 = (size_t)h->n_inst * 32;
+    std::vector<double> buf (2 * n32);                    // sums, then the counts' bits
+    B200M_CUDA (cudaMemcpyAsync (buf.data (), h->d_ltas, buf.size () * sizeof (double), cudaMemcpyDeviceToHost, st));
+    B200M_CUDA (cudaStreamSynchronize (st));
+    const uint64_t* cnt = reinterpret_cast<const uint64_t*> (buf.data () + n32);
+    for (size_t i = 0; i < h->n_inst; ++i) {
+        memcpy (sums + i * SPEC_BANDS, buf.data () + i * 32, SPEC_BANDS * sizeof (double));
+        memcpy (counts + i * SPEC_BANDS, cnt + i * 32, SPEC_BANDS * sizeof (uint64_t));
     }
     return 0;
 }

@@ -9,6 +9,8 @@ one row per album (b200m_ebu_group_reduce): the clips of one album may sit on di
 The second exchange is album DR (b200m_dr14_group_reduce): each album's int32 row of summed window histograms and counts is
 all-reduced the same way, but its window peaks cannot be summed (an album's second-highest window peak is the second largest over
 all its tracks), so every rank's [G, nch, 3] peaks are all-gathered and b200m_dr14_group_finish merges the W parts by value.
+Album spectra need no exchange of their own: gather_results collects each rank's per-clip sums, counts and peak_db of
+programme_spectrum in clip order, and spectrum_albums pools them on the host exactly as it pools the rows of one bank.
 """
 MIX_WORDS = 1508
 DR14_HISTBINS = 8000
