@@ -225,21 +225,26 @@ _PROTOS = {
 EXPORTS = tuple(_PROTOS)
 
 
+def load_lib(path):
+    """Load a build of libb200meters.so, this tree's or another (to compare two builds), with the prototypes of _PROTOS."""
+    L = C.CDLL(os.path.abspath(path))
+    for name, (res, args) in _PROTOS.items():
+        try:
+            fn = getattr(L, name)
+        except AttributeError:      # an export this build lacks: missing_exports() reports it, calling it raises AttributeError
+            continue
+        fn.restype, fn.argtypes = res, args
+    return L
+
+
 def lib():
-    """Load libb200meters.so (fails loudly if it has not been built: there is no fallback)."""
+    """Load this tree's libb200meters.so (fails loudly if it has not been built: there is no fallback)."""
     global _lib
     if _lib is None:
         if not os.path.exists(LIB_PATH):
             raise B200MError("%s is missing: run `python meters.lv2_b200/build.py` "
                              "(or __graft_entry__.build()); there is no CPU fallback" % LIB_PATH)
-        L = C.CDLL(LIB_PATH)
-        for name, (res, args) in _PROTOS.items():
-            try:
-                fn = getattr(L, name)
-            except AttributeError:      # reported by missing_exports(); calling it raises AttributeError
-                continue
-            fn.restype, fn.argtypes = res, args
-        _lib = L
+        _lib = load_lib(LIB_PATH)
     return _lib
 
 

@@ -459,8 +459,8 @@ tpk_kernel (const float* __restrict__ in, size_t stride, int c_first, int n_chan
     // K-meter / DR roles or idle during the serial phase), a 64-channel CTA ("wide") keeps ALL four warps busy in the serial phase.
     // 87 KB of shared memory per CTA leave two CTAs = eight warps per SM, too few to hide the FIR's latencies (the 16-channel form
     // keeps seven CTAs resident and lets other CTAs' FIR phases run under a CTA's serial phase; its DR form takes 94 registers and
-    // keeps five, measured faster than the same code bounded to seven, meters.lv2_b200/host/dr14_run_cost.py).  Kept opt-in,
-    // bit-identical, tested.
+    // keeps five, measured faster than the same code bounded to seven, meters.lv2_b200/host/phase_cost.py --banks dr14).  Kept
+    // opt-in, bit-identical, tested.
     static_assert (!BAL || CH == 16 || CH == 64, "split ballistics lanes assume 16 channels per warp");
     constexpr bool ALLW = BAL && CH == 64;
     constexpr int LPR = TPK_THREADS / CH;         // lanes that share one channel row in the FIR phase (an aligned lane group)

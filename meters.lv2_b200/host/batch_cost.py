@@ -7,29 +7,27 @@ mode and library.  The GPU's name and power limit are read at the start and prin
     python meters.lv2_b200/host/batch_cost.py [--lib meters.lv2_b200/libb200meters.so ...] [--uri COR ...] [--runs 3] [--instances 512]
                                               [--ui 1]
 """
-import argparse
 import json
 import os
 import subprocess
 import sys
 
+import _cost
+from _cost import B
+
 HERE = os.path.dirname(os.path.abspath(__file__))
 
 
 def main():
-    ap = argparse.ArgumentParser()
-    ap.add_argument("--lib", action="append")
+    ap = _cost.parser(__doc__, lib=True, instances=512, nframes=1024, runs=3)
     ap.add_argument("--uri", action="append")
-    ap.add_argument("--runs", type=int, default=3)
-    ap.add_argument("--instances", type=int, default=512)
     ap.add_argument("--cycles", type=int, default=100)
-    ap.add_argument("--nframes", type=int, default=1024)
     ap.add_argument("--batch", type=int, default=64)
     ap.add_argument("--ui", type=int, default=0)                 # 1: a GUI is attached to every instance (lv2_host --ui)
     a = ap.parse_args()
-    libs = a.lib or [os.path.join(HERE, "..", "libb200meters.so")]
+    libs = a.lib or [B.LIB_PATH]
     uris = a.uri or ["spectr30stereo", "BBCM6", "surround5", "COR", "phasewheel", "goniometer"]
-    gpu = subprocess.run(["nvidia-smi", "--query-gpu=name,power.limit", "--format=csv,noheader"], capture_output=True, text=True).stdout.strip()
+    gpu = _cost.gpu()
     print(json.dumps({"gpu": gpu}), flush=True)
     res = {}
     for r in range(a.runs):

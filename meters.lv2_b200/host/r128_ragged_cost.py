@@ -9,18 +9,14 @@ name and power limit are read in the same call and printed with the results (one
 
     python meters.lv2_b200/host/r128_ragged_cost.py [--instances 8192] [--nframes 1024] [--iters 300] [--runs 3]
 """
-import argparse
 import json
-import os
-import subprocess
-import sys
 import time
 
 import numpy as np
 import torch
 
-sys.path.insert(0, os.path.join(os.path.dirname(os.path.abspath(__file__)), "..", ".."))
-import meters_lv2_b200 as B  # noqa: E402
+import _cost
+from _cost import B
 
 PREC = {"tolerance": B.PREC_FMA, "exact": B.PREC_EXACT}
 
@@ -32,36 +28,18 @@ def _bank(n, mode):
     return bk
 
 
-def _events(fn, iters):
-    for _ in range(20):
-        fn()
-    torch.cuda.synchronize()
-    a, b = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
-    a.record()
-    for _ in range(iters):
-        fn()
-    b.record()
-    torch.cuda.synchronize()
-    return round(a.elapsed_time(b) / iters * 1e3, 2)
-
-
 def _one(x, n, nf, mode, iters, rng):
     out = {}
-    full = np.full(n, nf, np.uint32)
     bk = _bank(n, mode)
-    out["a plain"] = _events(lambda: bk.run(x), iters)
-    out["a ragged all nfram"] = _events(lambda: bk.run(x, lengths=full), iters)
-    for pct in (1, 50):
-        lens = full.copy()
-        idx = rng.choice(n, size=n * pct // 100, replace=False)
-        lens[idx] = rng.integers(0, nf, size=idx.size)
-        out[f"b {pct}% end early"] = _events(lambda: bk.run(x, lengths=lens), iters)
+    for k, lens in _cost.ragged_forms(n, nf, rng, ab=True).items():
+        out[k] = _cost.events(lambda: bk.run(x, lengths=lens), iters, 20)
     bk.close()
     bk = _bank(n, mode)
+    full = np.full(n, nf, np.uint32)
     for k in range(64):                        # 64 blocks in which one instance in 64 is one frame short: >= 64 phase classes
         lens = full.copy(); lens[k::64] = nf - 1 - k
         bk.run(x, lengths=lens)
-    out["c plain after scatter"] = _events(lambda: bk.run(x), iters)
+    out["c plain after scatter"] = _cost.events(lambda: bk.run(x), iters, 20)
     bk.close()
     return out
 
@@ -76,20 +54,14 @@ def _programme(x, n, nf, lengths):
 
 
 def main():
-    ap = argparse.ArgumentParser()
-    ap.add_argument("--runs", type=int, default=3)
-    ap.add_argument("--instances", type=int, default=8192)
-    ap.add_argument("--nframes", type=int, default=1024)
-    ap.add_argument("--iters", type=int, default=300)
-    a = ap.parse_args()
-    gpu = subprocess.run(["nvidia-smi", "--query-gpu=name,power.limit", "--format=csv,noheader"], capture_output=True, text=True).stdout.strip()
-    torch.manual_seed(0)
+    a = _cost.parser(__doc__, instances=8192, nframes=1024, iters=300, runs=3).parse_args()
+    gpu = _cost.gpu()
     n, nf = a.instances, a.nframes
-    x = (torch.rand(2 * n, nf, device="cuda") * 2 - 1) * 0.5
+    x = _cost.noise(2 * n, nf)
     rng = np.random.default_rng(0)
     res = {}
     for r in range(a.runs):
-        for mode in (PREC if r % 2 == 0 else list(PREC)[::-1]):
+        for mode in _cost.alternate(PREC, r):
             for k, v in _one(x, n, nf, mode, a.iters, rng).items():
                 res.setdefault(f"{mode} {k}", []).append(v)
     mixed = rng.integers(20 * 48000, 60 * 48000, size=n)

@@ -4,44 +4,19 @@ off against plane on.  Each figure is the CUDA-event time per block over --iters
 --runs times, off and on alternating and swapping order each run.  The GPU's name and power limit are read in the same call and
 printed with the results (one JSON line).
 
-    python meters.lv2_b200/host/spec_ltas_cost.py [--n-inst 4096] [--nframes 1024] [--iters 300] [--runs 3]
+    python meters.lv2_b200/host/spec_ltas_cost.py [--instances 4096] [--nframes 1024] [--iters 300] [--runs 3]
 """
-import argparse
 import json
-import os
-import subprocess
-import sys
 
-import torch
-
-sys.path.insert(0, os.path.join(os.path.dirname(os.path.abspath(__file__)), "..", ".."))
-import meters_lv2_b200 as B  # noqa: E402
-
-
-def _time(fn, iters):
-    for _ in range(20):
-        B._ck(fn())
-    torch.cuda.synchronize()
-    a, b = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
-    a.record()
-    for _ in range(iters):
-        fn()
-    b.record()
-    torch.cuda.synchronize()
-    return round(a.elapsed_time(b) / iters * 1e3, 2)
+import _cost
+from _cost import B
 
 
 def main():
-    ap = argparse.ArgumentParser()
-    ap.add_argument("--n-inst", type=int, default=4096)
-    ap.add_argument("--nframes", type=int, default=1024)
-    ap.add_argument("--iters", type=int, default=300)
-    ap.add_argument("--runs", type=int, default=3)
-    a = ap.parse_args()
-    gpu = subprocess.run(["nvidia-smi", "--query-gpu=name,power.limit", "--format=csv,noheader"], capture_output=True, text=True).stdout.strip()
-    torch.manual_seed(0)
-    n, nf = a.n_inst, a.nframes
-    x = (torch.rand(2 * n, nf, device="cuda") * 2 - 1) * 0.5
+    a = _cost.parser(__doc__, instances=4096, nframes=1024, iters=300, runs=3).parse_args()
+    gpu = _cost.gpu()
+    n, nf = a.instances, a.nframes
+    x = _cost.noise(2 * n, nf)
     p, s, _, _ = B._dev_ptr(x)
     st = B._stream_ptr(None)
     L = B.lib()
@@ -49,12 +24,12 @@ def main():
     for mode, prec in (("exact", B.PREC_EXACT), ("tolerance", B.PREC_FMA)):
         res = {"off": [], "on": []}
         for r in range(a.runs):
-            for plane in (("off", "on") if r % 2 == 0 else ("on", "off")):
+            for plane in _cost.alternate(("off", "on"), r):
                 g = B.Spectr30(n, 2)
                 g.set_precision(prec)
                 if plane == "on":
                     g.ltas_enable()
-                res[plane].append(_time(lambda: L.b200m_spec_process_device(g.h, p, s, nf, 1.0, -4.0, st), a.iters))
+                res[plane].append(_cost.events(lambda: L.b200m_spec_process_device(g.h, p, s, nf, 1.0, -4.0, st), a.iters, 20))
                 g.close()
         out["us_per_block"][mode] = res
     print(json.dumps(out))
