@@ -473,8 +473,8 @@ int b200m_cor_process_device (b200m_cor* h, const float* d_in, size_t stride, ui
 int b200m_cor_process_host (b200m_cor* h, const float* in, size_t stride, uint32_t nfram);
 int b200m_cor_results (b200m_cor* h, float* out, void* stream);           /* Stcorrdsp::read (:79-82) */
 /* pair inst (-1: all) back to a newly constructed Stcorrdsp (stcorrdsp.cc:33-37): the five filter states and the reading zero, in
- * both precision modes.  Ordered with the bank's runs on the stream it currently runs on.  A phasewheel ring fed from this bank
- * (b200m_pw_attach_cor) is not touched. */
+ * both precision modes, and, while the histogram plane is on (b200m_cor_hist_enable), its counts and sum.  Ordered with the bank's
+ * runs on the stream it currently runs on.  A phasewheel ring fed from this bank (b200m_pw_attach_cor) is not touched. */
 int b200m_cor_clear (b200m_cor* h, int32_t inst, void* stream);
 /* b200m_cor_process_* with a per-pair hold: run = n_inst flags, NULL = every pair runs (exactly b200m_cor_process_*).  A pair
  * with run[i] == 0 is left as if the call had not been made for it: its five filter states and its reading stay bit-identical,
@@ -501,10 +501,32 @@ int b200m_cor_process_ragged_host (b200m_cor* h, const float* in, size_t stride,
  * in exact mode); the correlation stays within 1e-5 of the reference.  The reference's own fp32 rounding noise grows with the product
  * filters' memory tcf * fsamp, and no more accurate evaluation can follow it: a bank whose memory exceeds 21600 samples (tcf 0.3 s
  * above 72 kHz, i.e. at 88.2-192 kHz; tcf above 0.45 s at 48 kHz) runs the exact kernel in this mode too, bit-identical to the
- * reference.  The bound is fixed at creation, whatever the block. */
+ * reference.  The bound is fixed at creation, whatever the block.  While the correlation histogram plane is on
+ * (b200m_cor_hist_enable) this mode also runs the exact kernel: the plane has one form, and the plane, the states and the readings
+ * are then bit-identical to B200M_PREC_EXACT. */
 int b200m_cor_set_precision (b200m_cor* h, int mode);
 int b200m_cor_state (b200m_cor* h, float* state5, void* stream);          /* [n][5] zl zr zlr zll zrr */
 int b200m_cor_coeffs (const b200m_cor* h, float w[2]);
+/* Correlation histogram (an extension; the reference keeps only the state its read() reports at block end): with the plane on,
+ * after each frame's five updates of Stcorrdsp::process (stcorrdsp.cc:58-62) every pair forms the frame's reading
+ * r = zlr / sqrtf (zll * zrr + 1e-10f) (the read() formula, :79-82, on the in-loop state; fp32, no contraction).  The frame counts
+ * if zll + zrr >= thr (fp32) and r is finite, with thr = (float) (2 * 10^(gate_db / 10)) computed in double.  A counted frame adds
+ * 1 to bin clamp ((int) floorf ((r + 1.0f) * 100.0f), 0, 199) of the pair's B200M_COR_HIST_BINS bins of width 0.01 over [-1, 1]
+ * (r = 1 falls in bin 199; readings past +-1 are clamped), and adds (double) r to the pair's double sum in frame order.  The
+ * end-of-process scrub and bias (:65-75) apply at block end only, as without the plane.  Ragged blocks and held pairs of
+ * b200m_cor_process_ctl_* add only the frames the pair runs; a phasewheel bank's feed (b200m_pw_attach_cor) counts like a call of
+ * this bank.  Ports and b200m_cor_state are bit-identical with the plane on or off; with it off the bank runs exactly the kernels it
+ * runs without it.
+ * enable != 0: allocates the plane on first use (B200M_E_NOMEM if the device cannot hold 1608 bytes per pair), zeroes every pair's
+ * counts and sum, also when it was on already, and sets the gate; 0: stops counting and keeps the memory.  gate_db = -INFINITY
+ * gives thr = 0 (every frame with a finite reading counts); NaN or +INFINITY returns B200M_E_INVAL.  While the plane is on,
+ * b200m_cor_clear also zeroes the cleared pairs' counts and sums.  Ordered like the getters. */
+#define B200M_COR_HIST_BINS 200
+int b200m_cor_hist_enable (b200m_cor* h, int enable, float gate_db, void* stream);
+/* host counts [n_inst][B200M_COR_HIST_BINS] and sums [n_inst] of every pair, in one copy and one synchronisation of the stream,
+ * ordered like b200m_cor_results; the mean reading of the counted frames is sums / (the row's total count).  B200M_E_INVAL while
+ * the plane is off. */
+int b200m_cor_hist_read (b200m_cor* h, uint64_t* counts, double* sums, void* stream);
 
 /* ======================================================================================
  * Needle-meter ballistics bank (SURVEY §8f rank 3) — replaces LV2M::Vumeterdsp (jmeters/vumeterdsp.cc:45-93),

@@ -158,6 +158,8 @@ _PROTOS = {
     "b200m_cor_state": (C.c_int, [_v, _v, _v]),
     "b200m_cor_coeffs": (C.c_int, [_v, _v]),
     "b200m_cor_clear": (C.c_int, [_v, C.c_int32, _v]),
+    "b200m_cor_hist_enable": (C.c_int, [_v, C.c_int, C.c_float, _v]),
+    "b200m_cor_hist_read": (C.c_int, [_v, _v, _v, _v]),
     # needle-meter ballistics
     "b200m_ppm_create": (C.c_int, [C.POINTER(_v), C.c_int, C.c_uint32, C.c_float, C.c_int]),
     "b200m_ppm_destroy": (C.c_int, [_v]),
@@ -608,6 +610,12 @@ class TruePeakKmeter(_Bank):
         return out
 
 
+COR_HIST_BINS = 200           # B200M_COR_HIST_BINS
+# the correlation histogram's 201 bin edges, -1 .. 1 in steps of 0.01: bin k holds readings r with floorf ((r + 1) * 100) == k
+# (fp32), readings past +-1 clamped to bins 0 and 199
+COR_HIST_EDGES = (np.arange(COR_HIST_BINS + 1) - 100) / 100.0
+
+
 class Stcorrdsp(_Bank):
     """N x LV2M::Stcorrdsp (jmeters/stcorrdsp.h:27-55); channels 2i, 2i+1 = L, R of pair i."""
     _pfx = "cor"
@@ -655,8 +663,21 @@ class Stcorrdsp(_Bank):
         return w
 
     def clear(self, inst=-1, stream=None):
-        """pair inst (-1: all) back to a newly constructed Stcorrdsp; an attached phasewheel ring is not touched"""
+        """pair inst (-1: all) back to a newly constructed Stcorrdsp, its histogram row too while the plane is on; an attached
+        phasewheel ring is not touched"""
         _ck(lib().b200m_cor_clear(self.h, inst, _stream_ptr(stream)))
+
+    def hist_enable(self, on=True, gate_db=-70.0, stream=None):
+        """the correlation histogram plane (b200m_cor_hist_enable): on, every pair counts each frame's reading r in
+        COR_HIST_EDGES's 200 bins and adds it to a float64 sum, if zll + zrr >= 2 * 10^(gate_db / 10) and r is finite; (re)enabling
+        zeroes every pair's row and sets the gate (-inf: no gate); off, the bank stops counting and runs its plain kernels"""
+        _ck(lib().b200m_cor_hist_enable(self.h, int(bool(on)), float(gate_db), _stream_ptr(stream)))
+
+    def hist(self, stream=None):
+        """(counts int64 [n_inst, 200], sums float64 [n_inst]) of the histogram plane (b200m_cor_hist_read); raises while it is off"""
+        c = np.empty((self.n_inst, COR_HIST_BINS), np.uint64); s = np.empty(self.n_inst, np.float64)
+        _ck(lib().b200m_cor_hist_read(self.h, _np_ptr(c), _np_ptr(s), _stream_ptr(stream)))
+        return c.astype(np.int64), s
 
 
 PPM_VU, PPM_IEC1, PPM_IEC2, PPM_MS = 0, 1, 2, 3
@@ -1426,4 +1447,84 @@ def programme_spectrum(x, lengths, rate=48000.0, nchan=2, speed=1.0, block=1024,
     out = dict(sums=sums, counts=counts, ltas=ltas, ltas_db=_ltas_db(ltas), peak_db=peak_db)
     if grp is not None:
         out.update(spectrum_albums(sums, counts, peak_db, grp))
+    return out
+
+
+def _cor_dist(hist, sums):
+    """the derived fields of correlation histogram rows (int64 [N, 200], float64 [N]): frames (the row total), mean (sums / frames),
+    below0 (the fraction of frames in bins 0..99, readings with (r + 1) * 100 < 100), p1 and p5 (the lower edge of the first bin
+    where the cumulative count reaches 1 % / 5 % of frames); the float fields are NaN where frames is 0"""
+    frames = hist.sum(axis=1)
+    live = frames > 0
+    cum = np.cumsum(hist, axis=1)
+
+    def edge(den):                                      # first k with cum[k] / frames >= 1 / den, in integers
+        k = np.argmax(cum * den >= frames[:, None], axis=1)
+        return np.where(live, COR_HIST_EDGES[k], np.nan)
+    with np.errstate(invalid="ignore", divide="ignore"):
+        mean = np.where(live, sums / np.maximum(frames, 1), np.nan)
+        below0 = np.where(live, cum[:, 99] / np.maximum(frames, 1), np.nan)
+    return dict(frames=frames, mean=mean, below0=below0, p1=edge(100), p5=edge(20))
+
+
+def correlation_albums(hist, sums, groups):
+    """Album correlation distributions from per-clip rows: programme_correlation's hist and sums, or those of several banks (shards
+    on several GPUs) concatenated in clip order, e.g. with shard.gather_results.  groups: N album ids (>= 0, or -1 for a clip in no
+    album).  An album's counts are the sum of its members' and its sum their sums added in ascending clip index, so the result does
+    not depend on how the clips were split between banks.  Returns a dict for G = max(groups) + 1 albums: album_hist (int64 [G, 200]),
+    album_frames (int64 [G]), album_sums (float64 [G]), album_mean, album_below0, album_p1, album_p5 (float64 [G], as
+    programme_correlation's clip fields) and album_n_clips (int64 [G]).  An album without counted frames reads NaN."""
+    hist = np.asarray(hist, np.int64); sums = np.asarray(sums, np.float64)
+    n = hist.shape[0] if hist.ndim == 2 else -1
+    if n < 0 or hist.shape != (n, COR_HIST_BINS) or sums.shape != (n,):
+        raise B200MError("hist and sums must be [N, 200] and [N] rows of the same N clips")
+    grp = _groups(groups, n)
+    g = int(grp.max()) + 1 if n else 0
+    h, s = np.zeros((g, COR_HIST_BINS), np.int64), np.zeros(g)
+    for i in np.flatnonzero(grp >= 0):                 # one clip at a time, in ascending index: a fixed order of the fp64 sums
+        a = grp[i]
+        h[a] += hist[i]
+        s[a] += sums[i]
+    d = _cor_dist(h, s)
+    return dict(album_hist=h, album_frames=d["frames"], album_sums=s, album_mean=d["mean"], album_below0=d["below0"],
+                album_p1=d["p1"], album_p5=d["p5"], album_n_clips=np.bincount(grp[grp >= 0], minlength=g).astype(np.int64))
+
+
+def programme_correlation(x, lengths, rate=48000.0, flp=2e3, tcf=0.3, gate_db=-70.0, block=1024, device=0, groups=None):
+    """Phase-correlation distribution of N stereo clips of different lengths, in one correlation bank.
+
+    x: rows 2i, 2i + 1 = L, R of clip i, clip i valid for its first lengths[i] frames: a [2N, >= max(lengths)] float32 numpy array /
+    CPU tensor (host path) or CUDA tensor (device path), or a callable f(offset, nfram) that returns frames offset .. offset +
+    nfram - 1 of every row as such an array.  Frames past a clip's length are never read into a result.  The clips are fed in blocks
+    of `block` frames with clip i's length in block k clamp(lengths[i] - k * block, 0, block) (Stcorrdsp.process with lengths), so
+    clip i's numbers are bit-identical to one Stcorrdsp(rate, flp, tcf) fed only that clip in blocks of `block` frames with the
+    histogram plane on (Stcorrdsp.hist_enable(gate_db=gate_db)).  The plane always runs exact.
+    Returns a dict of N rows:
+      hist (int64 [N, 200]): the counted frames' readings in the bins of COR_HIST_EDGES; a frame counts if the correlation filters'
+        power zll + zrr >= 2 * 10^(gate_db / 10) and its reading is finite;
+      frames (int64): counted frames; sums (float64): the sum of their readings in frame order;
+      mean (float64): sums / frames;
+      below0 (float64): the fraction of counted frames in bins 0..99, readings below 0 (anti-phase);
+      p1, p5 (float64): the lower edge of the bin where the cumulative count first reaches 1 % / 5 % of frames, the lowest
+        correlation the clip holds for at least 1 % / 5 % of its gated time;
+      reading (float32): the port reading (Stcorrdsp::read) after the clip's last block, 0 for an empty clip.
+    mean, below0, p1 and p5 are NaN where frames is 0.
+    groups: None, or N album ids (>= 0, or -1 for a clip in no album): the dict then also holds correlation_albums(hist, sums,
+    groups)."""
+    ln, blocks = _programme_blocks(x, lengths, block, "no clips")
+    n = ln.size
+    grp = None if groups is None else _groups(groups, n)
+    bank = Stcorrdsp(n, rate, flp, tcf, device)
+    try:
+        bank.hist_enable(gate_db=gate_db)
+        for _, xb, lb in blocks:
+            bank.process(xb, lengths=lb)
+        hist, sums = bank.hist()
+        reading = bank.read()
+    finally:
+        bank.close()
+    out = dict(hist=hist, sums=sums, reading=reading)
+    out.update(_cor_dist(hist, sums))
+    if grp is not None:
+        out.update(correlation_albums(hist, sums, grp))
     return out

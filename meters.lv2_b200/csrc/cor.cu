@@ -18,11 +18,18 @@ constexpr int COR_T = 32, COR_P = COR_T + 4, COR_STAGES = 4;
 // Each lane stops at its own end; the warp stages tiles up to its longest pair.  A pair with rlen[i] == 0 is not called (held): its
 // rows are never loaded and its state and reading are not written back.  The plain process calls and the phasewheel ring feed are
 // the RAG = false instantiation.
-template <bool RAG>
+// HIST (b200m_cor_hist_enable): after each frame's five updates the lane also forms the frame's reading r (Stcorrdsp::read, :79-82,
+// on the in-loop state) and, if zll + zrr >= thr and r is finite, adds (double) r to the pair's fp64 sum in frame order and counts
+// the frame in bin clamp (floor ((r + 1) * 100), 0, 199).  The counts are run-length coded in registers: the reading moves slowly
+// (its filters smooth over tcf * fsamp frames), so a lane holds (bin, run) and adds the run to its own row of hcnt with one
+// fire-and-forget atomic (RED) only when the bin changes and at kernel end.  The recurrences, states and readings are the same bits
+// as without the plane; the per-frame reading's cost is in DESIGN.md §3.
+template <bool RAG, bool HIST = false>
 __global__ void __launch_bounds__ (32)
 cor_kernel (const float* __restrict__ in, size_t stride, int n_inst, int nfram, int aligned, float w1, float w2,
             float* __restrict__ st /* [5][n_inst] */, float* __restrict__ res, float* __restrict__ ring, int N, int rboff,
-            const uint32_t* __restrict__ rlen)
+            const uint32_t* __restrict__ rlen, unsigned long long* __restrict__ hcnt /* [n_inst][200] */,
+            double* __restrict__ hsum /* [n_inst] */, float thr)
 {
     __shared__ __align__ (16) float tile[COR_STAGES][2][32 * COR_P];
     const int lane = threadIdx.x;
@@ -76,6 +83,21 @@ cor_kernel (const float* __restrict__ in, size_t stride, int n_inst, int nfram, 
         zrr = __fadd_rn (zrr, __fmul_rn (w2, __fsub_rn (__fmul_rn (zr, zr), zrr)));
     };
 
+    double hs = 0.0; int hbin = 0; uint32_t hrun = 0;            // HIST: the pair's sum, and the open run of frames in bin hbin
+    if constexpr (HIST) hs = hsum[inst];
+    auto flush = [&] () {                                        // lanes past the bank repeat its last pair: they add nothing
+        if (live && hrun) atomicAdd (hcnt + (size_t)inst * B200M_COR_HIST_BINS + hbin, (unsigned long long)hrun);
+    };
+    auto tally = [&] () {
+        const float r = __fdiv_rn (zlr, __fsqrt_rn (__fadd_rn (__fmul_rn (zll, zrr), 1e-10f)));
+        if (__fadd_rn (zll, zrr) >= thr && finitef_ (r)) {
+            const int k = (int)fminf (fmaxf (floorf (__fmul_rn (__fadd_rn (r, 1.0f), 100.0f)), 0.0f), (float)(B200M_COR_HIST_BINS - 1));
+            hs = __dadd_rn (hs, (double)r);
+            if (k != hbin) { flush (); hbin = k; hrun = 0; }
+            ++hrun;
+        }
+    };
+
 #pragma unroll
     for (int t = 0; t < COR_STAGES - 1; ++t) issue (t);
     for (int t = 0; t < ntiles; ++t) {
@@ -96,16 +118,21 @@ cor_kernel (const float* __restrict__ in, size_t stride, int n_inst, int nfram, 
         }
         const int e = RAG ? max (0, min (COR_T, rl - t * COR_T)) : len;       // this pair's samples in the tile
         int j = 0;
+        auto frame = [&] (float l, float r) {
+            step (l, r);
+            if constexpr (HIST) tally ();
+        };
         for (; j + 4 <= e; j += 4) {
             const float4 a = *reinterpret_cast<const float4*> (pl + j);
             const float4 b = *reinterpret_cast<const float4*> (pr + j);
-            step (a.x, b.x); step (a.y, b.y); step (a.z, b.z); step (a.w, b.w);
+            frame (a.x, b.x); frame (a.y, b.y); frame (a.z, b.z); frame (a.w, b.w);
         }
-        for (; j < e; ++j) step (pl[j], pr[j]);
+        for (; j < e; ++j) frame (pl[j], pr[j]);
         __syncwarp ();
         issue (t + COR_STAGES - 1);
     }
     cp_async_wait<0> ();
+    if constexpr (HIST) flush ();
     // end of process(): non-finite scrub, anti-denormal bias on the three products (:65-75)
     zl = scrub (zl); zr = scrub (zr); zlr = scrub (zlr); zll = scrub (zll); zrr = scrub (zrr);
     zlr = __fadd_rn (zlr, 1e-10f); zll = __fadd_rn (zll, 1e-10f); zrr = __fadd_rn (zrr, 1e-10f);
@@ -114,6 +141,7 @@ cor_kernel (const float* __restrict__ in, size_t stride, int n_inst, int nfram, 
         st[2 * (size_t)n_inst + inst] = zlr; st[3 * (size_t)n_inst + inst] = zll; st[4 * (size_t)n_inst + inst] = zrr;
         // Stcorrdsp::read (:79-82)
         res[inst] = __fdiv_rn (zlr, __fsqrt_rn (__fadd_rn (__fmul_rn (zll, zrr), 1e-10f)));
+        if constexpr (HIST) hsum[inst] = hs;
     }
 }
 
@@ -285,6 +313,14 @@ struct b200m_cor {
     std::vector<uint32_t> ctl_len;         // b200m_cor_process_ctl_*: scratch for its lengths
     int attached = 0;                      // phasewheel banks feeding this one (b200m_pw_attach_cor): ragged calls are refused
     BankPath path;
+    // the correlation histogram plane (b200m_cor_hist_enable): [n_inst][200] uint64 counts, then [n_inst] fp64 sums, in one allocation
+    // so that a read is one copy; allocated on first use, kept until destroy
+    void* d_hist = nullptr;
+    bool hist = false;
+    float hist_thr = 0.0f;                 // the gate on zll + zrr
+    unsigned long long* hist_cnt () const { return (unsigned long long*)d_hist; }
+    double* hist_sum () const { return (double*)(hist_cnt () + (size_t)n_inst * B200M_COR_HIST_BINS); }
+    size_t hist_bytes () const { return (size_t)n_inst * (B200M_COR_HIST_BINS * sizeof (unsigned long long) + sizeof (double)); }
 };
 
 // The tolerance mode's promise is 1e-5 of the reference, and the reference's own fp32 rounding noise grows with the product filters'
@@ -298,12 +334,17 @@ static int cor_launch (b200m_cor* h, const float* d_in, size_t stride, uint32_t 
 {
     const int aligned = ((uintptr_t)d_in % 16 == 0) && (stride % 4 == 0);
     const uint32_t* rlen = RAG ? h->rag.d : nullptr;
-    if (h->scan && h->w2 >= 1.0f / COR_SCAN_MAX_MEMORY)
+    // the histogram plane has one form, in cor_kernel: with it on, tolerance mode runs the exact kernel (bit-identical plane, state
+    // and reading), as a memory beyond COR_SCAN_MAX_MEMORY does
+    if (h->scan && !h->hist && h->w2 >= 1.0f / COR_SCAN_MAX_MEMORY)
         cor_scan_kernel<RAG><<<(h->n_inst + CSC_WARPS - 1) / CSC_WARPS, CSC_WARPS * 32, 0, st>>> (
             d_in, stride, (int)h->n_inst, (int)nfram, aligned, h->w1, h->w2, h->d_st, h->d_res, ring, N, rboff, rlen);
+    else if (h->hist)
+        cor_kernel<RAG, true><<<(h->n_inst + 31) / 32, 32, 0, st>>> (d_in, stride, (int)h->n_inst, (int)nfram, aligned, h->w1, h->w2, h->d_st,
+                                                                     h->d_res, ring, N, rboff, rlen, h->hist_cnt (), h->hist_sum (), h->hist_thr);
     else
         cor_kernel<RAG><<<(h->n_inst + 31) / 32, 32, 0, st>>> (d_in, stride, (int)h->n_inst, (int)nfram, aligned, h->w1, h->w2, h->d_st, h->d_res,
-                                                               ring, N, rboff, rlen);
+                                                               ring, N, rboff, rlen, nullptr, nullptr, 0.0f);
     B200M_LAUNCHED (1);
     B200M_CUDA (cudaGetLastError ());
     return 0;
@@ -395,7 +436,7 @@ int b200m_cor_destroy (b200m_cor* h)
     if (!h) return 0;
     DeviceGuard g (h->device);
     cudaDeviceSynchronize ();
-    cudaFree (h->d_st); cudaFree (h->d_res); h->rag.release (); h->path.release ();
+    cudaFree (h->d_st); cudaFree (h->d_res); cudaFree (h->d_hist); h->rag.release (); h->path.release ();
     delete h;
     return 0;
 }
@@ -457,9 +498,52 @@ int b200m_cor_clear (b200m_cor* h, int32_t inst, void* stream)
     if (!h || inst < -1 || inst >= (int32_t)h->n_inst) return set_err (B200M_E_INVAL, "bad argument");
     DeviceGuard g (h->device);
     const int i0 = inst < 0 ? 0 : inst, n = inst < 0 ? (int)h->n_inst : 1;
-    cor_clear_kernel<<<(n + 127) / 128, 128, 0, h->path.stream (stream)>>> ((int)h->n_inst, i0, n, h->d_st, h->d_res);
+    cudaStream_t st = h->path.stream (stream);
+    cor_clear_kernel<<<(n + 127) / 128, 128, 0, st>>> ((int)h->n_inst, i0, n, h->d_st, h->d_res);
     B200M_LAUNCHED (1);
     B200M_CUDA (cudaGetLastError ());
+    if (h->hist) {                                         // a cleared slot is a fresh instance for the histogram too
+        B200M_CUDA (cudaMemsetAsync (h->hist_cnt () + (size_t)i0 * B200M_COR_HIST_BINS, 0,
+                                     (size_t)n * B200M_COR_HIST_BINS * sizeof (unsigned long long), st));
+        B200M_CUDA (cudaMemsetAsync (h->hist_sum () + i0, 0, (size_t)n * sizeof (double), st));
+    }
+    return 0;
+}
+
+int b200m_cor_hist_enable (b200m_cor* h, int enable, float gate_db, void* stream)
+{
+    if (!h) return set_err (B200M_E_INVAL, "NULL handle");
+    if (isnan (gate_db) || gate_db == INFINITY) return set_err (B200M_E_INVAL, "gate_db must be a number or -inf");
+    DeviceGuard g (h->device);
+    if (!enable) { h->hist = false; return 0; }           // the plane's memory stays for the next enable
+    cudaStream_t st = h->path.stream (stream);
+    if (!h->d_hist) {
+        const cudaError_t e = cudaMalloc (&h->d_hist, h->hist_bytes ());
+        if (e != cudaSuccess) {
+            cudaGetLastError ();                               // a failed allocation is not sticky: later calls must not see it
+            h->d_hist = nullptr;
+            if (e == cudaErrorMemoryAllocation) return set_err (B200M_E_NOMEM, "correlation histogram of %u pairs: out of device memory", h->n_inst);
+            return cuda_fail (e, "b200m_cor_hist_enable", __FILE__, __LINE__);
+        }
+    }
+    B200M_CUDA (cudaMemsetAsync (h->d_hist, 0, h->hist_bytes (), st));
+    h->hist_thr = (float)(2.0 * pow (10.0, (double)gate_db / 10.0));   // -inf dB: 0, every frame with a finite reading counts
+    h->hist = true;
+    return 0;
+}
+
+int b200m_cor_hist_read (b200m_cor* h, uint64_t* counts, double* sums, void* stream)
+{
+    if (!h || !counts || !sums) return set_err (B200M_E_INVAL, "NULL argument");
+    if (!h->hist) return set_err (B200M_E_INVAL, "the correlation histogram plane is off (b200m_cor_hist_enable)");
+    DeviceGuard g (h->device);
+    cudaStream_t st = h->path.stream (stream);
+    std::vector<unsigned char> buf (h->hist_bytes ());
+    B200M_CUDA (cudaMemcpyAsync (buf.data (), h->d_hist, buf.size (), cudaMemcpyDeviceToHost, st));
+    B200M_CUDA (cudaStreamSynchronize (st));
+    const size_t nc = (size_t)h->n_inst * B200M_COR_HIST_BINS * sizeof (uint64_t);
+    memcpy (counts, buf.data (), nc);
+    memcpy (sums, buf.data () + nc, (size_t)h->n_inst * sizeof (double));
     return 0;
 }
 

@@ -11,6 +11,8 @@ all-reduced the same way, but its window peaks cannot be summed (an album's seco
 all its tracks), so every rank's [G, nch, 3] peaks are all-gathered and b200m_dr14_group_finish merges the W parts by value.
 Album spectra need no exchange of their own: gather_results collects each rank's per-clip sums, counts and peak_db of
 programme_spectrum in clip order, and spectrum_albums pools them on the host exactly as it pools the rows of one bank.
+Album correlation distributions likewise: gather_results collects each rank's per-clip hist and sums of programme_correlation,
+and correlation_albums pools them on the host.
 """
 MIX_WORDS = 1508
 DR14_HISTBINS = 8000
