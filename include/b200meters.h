@@ -545,7 +545,8 @@ int b200m_ppm_set_gain (b200m_ppm* h, float db_m, float db_s);       /* Msppmdsp
  * on that call's stream. */
 int b200m_ppm_set_gain_inst (b200m_ppm* h, int32_t unit, float db_m, float db_s);
 /* unit (-1: all) back to newly constructed meters (vumeterdsp.cc / iec1ppmdsp.cc / iec2ppmdsp.cc / msppmdsp.cc constructors):
- * z1 z2 m = 0, _res = true, both meters of an M/S pair, whose gains return to -6 / -6 dB.  Ordered with the bank's runs on the
+ * z1 z2 m = 0, _res = true, both meters of an M/S pair, whose gains return to -6 / -6 dB, and, while the histogram plane is on
+ * (b200m_ppm_hist_enable), the unit's counts and statistics (both rows of an M/S pair).  Ordered with the bank's runs on the
  * stream it currently runs on. */
 int b200m_ppm_clear (b200m_ppm* h, int32_t unit, void* stream);
 int b200m_ppm_process_device (b200m_ppm* h, const float* d_in, size_t stride, uint32_t nfram, void* stream);
@@ -565,6 +566,37 @@ int b200m_ppm_read_device (b200m_ppm* h, void* stream);                /* read()
 int b200m_ppm_results (b200m_ppm* h, float* out, void* stream);        /* one float per meter */
 int b200m_ppm_state (b200m_ppm* h, float* state4, void* stream);       /* per meter: z1 z2 m res */
 int b200m_design_ppm (int kind, float fsamp, float w[4]);              /* w1 w2 w3 g (VU: w 0 0 g) */
+/* Needle histogram (an extension; read() keeps only the highest needle since the last read): process() meters a call in groups of
+ * 4 frames ("n /= 4": a call's last nfram mod 4 frames are not metered).  With the plane on, after each group's updates every meter
+ * takes the needle value s the reference compares with m (VU: z2 after its update, vumeterdsp.cc:57-68; IEC I / IEC II and both
+ * meters of an M/S pair: t = z1 + z2, iec1ppmdsp.cc / iec2ppmdsp.cc / msppmdsp.cc) and forms the group's reading v = _g * s (fp32,
+ * no contraction): the value read() would return if that group alone had set _m.  Per meter the plane keeps:
+ * - counts [B200M_PPM_HIST_BINS] (uint64): a finite v goes to bin #{k : v >= e[k]}, with the 241 edges
+ *   e[k] = (float) pow (10.0, (-80.0 + 0.5 * k) / 20.0) (double, k = 0..240, b200m_ppm_hist_edges).  Bin 0 holds readings below
+ *   -80 dB (v <= 0 included: a VU needle can swing negative), bins 1..240 are 0.5 dB wide, bin 241 is +40 dB and above;
+ * - nonfinite: groups whose v is not finite (IEC on Inf input, VU on NaN or Inf input); they go to no bin;
+ * - peak: the largest finite v, -INFINITY before the first;
+ * - overs of the bank's limit L = (float) pow (10.0, limit_db / 20.0) (double): over_groups counts finite v >= L, overs the runs of
+ *   such readings, longest_over the most over readings in one run (the open run included) and run the open run's length (0 if the
+ *   last finite reading was not over).  A non-finite reading neither starts, extends nor ends a run; a run continues across calls,
+ *   ragged zero-length holds and unmetered tails, as on a private meter fed the clip in pieces.
+ * Ragged blocks count only each unit's own groups; a unit with length 0 adds nothing.  Ports and b200m_ppm_state are bit-identical
+ * with the plane on or off; with it off the bank runs exactly the kernels it runs without it. */
+#define B200M_PPM_HIST_BINS 242
+typedef struct {
+    uint64_t nonfinite, over_groups, overs, longest_over, run;
+    float peak;
+    uint32_t pad;
+} b200m_ppm_hist_stats;
+/* enable != 0: allocates the plane on first use (B200M_E_NOMEM if the device cannot hold 1984 bytes per meter), zeroes every
+ * meter's counts and statistics (peak -INFINITY), also when it was on already, and sets L; 0: stops counting and keeps the memory.
+ * limit_db NaN returns B200M_E_INVAL; +INFINITY (no reading is over) and -INFINITY (L = 0) are allowed.  Ordered like the getters. */
+int b200m_ppm_hist_enable (b200m_ppm* h, int enable, float limit_db, void* stream);
+/* host counts [n_meters][B200M_PPM_HIST_BINS] and stats [n_meters], in one copy and one synchronisation of the stream, ordered like
+ * b200m_ppm_results.  B200M_E_INVAL while the plane is off. */
+int b200m_ppm_hist_read (b200m_ppm* h, uint64_t* counts, b200m_ppm_hist_stats* stats, void* stream);
+/* the library's 241 bin edges e[k] (host only: needs no device), so that callers bin with the same floats */
+int b200m_ppm_hist_edges (float* edges);
 
 /* ======================================================================================
  * Bit-meter and signal-distribution-histogram banks (SURVEY §8f rank 1), N mono instances each.

@@ -173,6 +173,9 @@ _PROTOS = {
     "b200m_ppm_read_device": (C.c_int, [_v, _v]),
     "b200m_ppm_results": (C.c_int, [_v, _v, _v]),
     "b200m_ppm_state": (C.c_int, [_v, _v, _v]),
+    "b200m_ppm_hist_enable": (C.c_int, [_v, C.c_int, C.c_float, _v]),
+    "b200m_ppm_hist_read": (C.c_int, [_v, _v, _v, _v]),
+    "b200m_ppm_hist_edges": (C.c_int, [_v]),
     "b200m_design_ppm": (C.c_int, [C.c_int, C.c_float, _v]),
     # bit-meter, signal distribution histogram
     "b200m_bim_create": (C.c_int, [C.POINTER(_v), C.c_int, C.c_uint32, C.c_double]),
@@ -689,6 +692,30 @@ def design_ppm(kind, fsamp):
     return w
 
 
+PPM_HIST_BINS = 242           # B200M_PPM_HIST_BINS
+# b200m_ppm_hist_stats
+PPM_HIST_STATS_DTYPE = np.dtype([("nonfinite", "<u8"), ("over_groups", "<u8"), ("overs", "<u8"), ("longest_over", "<u8"),
+                                 ("run", "<u8"), ("peak", "<f4"), ("pad", "<u4")])
+# the dB value of each of the needle histogram's 241 edges: bin 0 lies below -80 dB, bin k (1..240) from edge k - 1 up to edge k,
+# bin 241 at +40 dB and above
+PPM_HIST_EDGES_DB = -80.0 + 0.5 * np.arange(PPM_HIST_BINS - 1)
+_ppm_edges = None
+
+
+def __getattr__(name):
+    # PPM_HIST_EDGES, the library's float32 edges (b200m_ppm_hist_edges), is read from the library on first use, so that importing
+    # the package does not need it
+    global _ppm_edges
+    if name == "PPM_HIST_EDGES":
+        if _ppm_edges is None:
+            e = np.empty(PPM_HIST_BINS - 1, np.float32)
+            _ck(lib().b200m_ppm_hist_edges(_np_ptr(e)))
+            e.flags.writeable = False
+            _ppm_edges = e
+        return _ppm_edges
+    raise AttributeError("module %r has no attribute %r" % (__name__, name))
+
+
 class NeedleMeters(_Bank):
     """N x Vumeterdsp / Iec1ppmdsp / Iec2ppmdsp, or N stereo pairs x (Msppmdsp M, Msppmdsp S) (jmeters/*.cc)."""
     _pfx = "ppm"
@@ -705,8 +732,21 @@ class NeedleMeters(_Bank):
         _ck(lib().b200m_ppm_set_gain_inst(self.h, unit, db_m, db_s))
 
     def clear(self, unit=-1, stream=None):
-        """unit (-1: all) back to newly constructed meters (M/S: gains -6 / -6 dB)"""
+        """unit (-1: all) back to newly constructed meters (M/S: gains -6 / -6 dB), its histogram rows too while the plane is on"""
         _ck(lib().b200m_ppm_clear(self.h, unit, _stream_ptr(stream)))
+
+    def hist_enable(self, on=True, limit_db=0.0, stream=None):
+        """the needle histogram plane (b200m_ppm_hist_enable): on, every meter counts each group of 4 frames' reading v = g * s in
+        the 242 bins of PPM_HIST_EDGES and keeps PPM_HIST_STATS_DTYPE's statistics, overs against 10^(limit_db / 20); (re)enabling
+        zeroes every row and sets the limit; off, the bank stops counting and runs its plain kernels"""
+        _ck(lib().b200m_ppm_hist_enable(self.h, int(bool(on)), float(limit_db), _stream_ptr(stream)))
+
+    def hist(self, stream=None):
+        """(counts int64 [n_meters, 242], stats PPM_HIST_STATS_DTYPE [n_meters]) of the histogram plane (b200m_ppm_hist_read);
+        raises while it is off"""
+        c = np.empty((self.n_meters, PPM_HIST_BINS), np.uint64); st = np.empty(self.n_meters, PPM_HIST_STATS_DTYPE)
+        _ck(lib().b200m_ppm_hist_read(self.h, _np_ptr(c), _np_ptr(st), _stream_ptr(stream)))
+        return c.astype(np.int64), st
 
     def process(self, x, stream=None, lengths=None):
         """lengths: None, or n_units frame counts <= nfram: unit u (a meter, or an M/S pair) runs over the first lengths[u] frames
@@ -1527,4 +1567,121 @@ def programme_correlation(x, lengths, rate=48000.0, flp=2e3, tcf=0.3, gate_db=-7
     out.update(_cor_dist(hist, sums))
     if grp is not None:
         out.update(correlation_albums(hist, sums, grp))
+    return out
+
+
+def _needle_dist(hist):
+    """groups (the row total: finite readings) and p95_db / p99_db of needle histogram rows (int64 [..., 242]): the lower edge, in dB,
+    of the first bin where the cumulative count reaches 95 % / 99 % of groups, compared in integers; -inf for bin 0, NaN where
+    groups is 0"""
+    groups = hist.sum(axis=-1)
+    cum = np.cumsum(hist, axis=-1)
+    lower = np.concatenate([[-np.inf], PPM_HIST_EDGES_DB])   # bin k's lower edge
+
+    def edge(pct):
+        k = np.argmax(cum * 100 >= pct * groups[..., None], axis=-1)
+        return np.where(groups > 0, lower[k], np.nan)
+    return groups, edge(95), edge(99)
+
+
+def _peak_db(peak):
+    """20 log10 of float32 readings, -inf where the reading is not above 0 (no finite reading: peak is -inf)"""
+    p = np.asarray(peak, np.float64)
+    with np.errstate(divide="ignore", invalid="ignore"):
+        return np.where(p > 0, 20.0 * np.log10(np.where(p > 0, p, 1.0)), -np.inf)
+
+
+def needle_albums(hist, stats, groups):
+    """Album needle distributions from per-clip rows: programme_needle's hist and stats, or those of several banks (shards on several
+    GPUs) concatenated in clip order, e.g. with shard.gather_results.  groups: N album ids (>= 0, or -1 for a clip in no album).
+    Pooling is per meter position (channel, or M and S): an album's counts, nonfinite, over_groups and overs are the sums of its
+    members', its longest_over and peak their maxima.  All are integer sums or maxima, so the result does not depend on how the clips
+    were split between banks.  Returns a dict for G = max(groups) + 1 albums of M meters: album_hist (int64 [G, M, 242]), album_groups,
+    album_nonfinite, album_over_groups, album_overs, album_longest_over (int64 [G, M]), album_peak (float32 [G, M], -inf without a
+    finite reading), album_peak_db, album_p95_db, album_p99_db (float64 [G, M], as programme_needle's clip fields) and album_n_clips
+    (int64 [G]).  An album without members reads 0 counts, -inf peak and NaN percentiles.  An over run that ends one clip and one
+    that starts the next are counted as two overs, and the longest run is the longest within one clip."""
+    hist = np.asarray(hist, np.int64); stats = np.asarray(stats)
+    n = hist.shape[0] if hist.ndim == 3 else -1
+    if n < 0 or hist.shape[2:] != (PPM_HIST_BINS,) or stats.dtype != PPM_HIST_STATS_DTYPE or stats.shape != hist.shape[:2]:
+        raise B200MError("hist and stats must be [N, M, 242] and [N, M] (PPM_HIST_STATS_DTYPE) rows of the same N clips")
+    m = hist.shape[1]
+    grp = _groups(groups, n)
+    g = int(grp.max()) + 1 if n else 0
+    h = np.zeros((g, m, PPM_HIST_BINS), np.int64)
+    tot = {k: np.zeros((g, m), np.int64) for k in ("nonfinite", "over_groups", "overs", "longest_over")}
+    pk = np.full((g, m), -np.inf, np.float32)
+    for i in np.flatnonzero(grp >= 0):
+        a = grp[i]
+        h[a] += hist[i]
+        for k in ("nonfinite", "over_groups", "overs"):
+            tot[k][a] += stats[k][i].astype(np.int64)
+        np.maximum(tot["longest_over"][a], stats["longest_over"][i].astype(np.int64), out=tot["longest_over"][a])
+        np.maximum(pk[a], stats["peak"][i], out=pk[a])
+    ng, p95, p99 = _needle_dist(h)
+    out = dict(album_hist=h, album_groups=ng)
+    out.update({"album_" + k: v for k, v in tot.items()})
+    out.update(album_peak=pk, album_peak_db=_peak_db(pk), album_p95_db=p95, album_p99_db=p99,
+               album_n_clips=np.bincount(grp[grp >= 0], minlength=g).astype(np.int64))
+    return out
+
+
+def programme_needle(x, lengths, kind, rate=48000.0, nchan=2, limit_db=0.0, ms_gain_db=(-6.0, -6.0), block=1024, device=0,
+                     groups=None):
+    """Needle-meter distribution of N clips of different lengths, in one needle-meter bank of `kind` (PPM_VU, PPM_IEC1, PPM_IEC2 or
+    PPM_MS).
+
+    x: VU / IEC: rows i * nchan + c of clip i, one meter per channel; M/S: rows 2i, 2i + 1 = L, R of clip i, one M/S pair (meters M
+    and S, gains ms_gain_db), nchan ignored.  Clip i is valid for its first lengths[i] frames: a [rows, >= max(lengths)] float32 numpy
+    array / CPU tensor (host path) or CUDA tensor (device path), or a callable f(offset, nfram) that returns frames offset .. offset +
+    nfram - 1 of every row as such an array.  Frames past a clip's length are never read into a result.  The clips are fed in blocks
+    of `block` frames with clip i's length in block k clamp(lengths[i] - k * block, 0, block) (NeedleMeters.process with lengths), so
+    clip i's numbers are bit-identical to one NeedleMeters fed only that clip in blocks of `block` frames with the histogram plane on
+    (NeedleMeters.hist_enable(limit_db=limit_db)); a block's last nfram mod 4 frames are not metered, as in the reference.
+    Returns a dict of [N, M] rows, M = nchan (M/S: 2, M then S):
+      hist (int64 [N, M, 242]): every finite group reading v = g * s in the bins of PPM_HIST_EDGES;
+      stats (PPM_HIST_STATS_DTYPE): the plane's statistics, for needle_albums;
+      groups (int64): finite readings; seconds (float64): 4 * groups / rate; nonfinite (int64): readings that were not finite;
+      peak (float32): the largest finite reading, -inf without one; peak_db (float64): 20 log10 peak, -inf where peak <= 0;
+      p95_db, p99_db (float64): the lower edge of the bin where the cumulative count first reaches 95 % / 99 % of groups: the level
+        the needle stays under for 95 % / 99 % of the metered time (-inf: bin 0, below -80 dB; NaN: no reading);
+      over_groups (int64) and over_seconds (float64): readings at or above 10^(limit_db / 20) and their time; overs (int64): the
+        separate runs of such readings; longest_over_s (float64): the longest run's time;
+      reading (float32): the read() port value after the clip's last block, the highest needle of the whole clip on the level
+        port's scale (0 for an empty clip).
+    groups: None, or N album ids (>= 0, or -1 for a clip in no album): the dict then also holds needle_albums(hist, stats, groups)."""
+    ln, blocks = _programme_blocks(x, lengths, block, "no clips")
+    n = ln.size
+    grp = None if groups is None else _groups(groups, n)
+    ms = kind == PPM_MS
+    if not ms and int(nchan) < 1:
+        raise B200MError("nchan must be >= 1")
+    per = 2 if ms else int(nchan)
+    units = n if ms else n * per
+    bank = NeedleMeters(units, kind, rate, device)
+    try:
+        if ms:
+            bank.set_gain(*ms_gain_db)
+        bank.hist_enable(limit_db=limit_db)
+        for _, xb, lb in blocks:
+            bank.process(xb, lengths=lb if ms else np.repeat(lb, per))     # each meter of a clip runs the clip's frames
+        hist, stats = bank.hist()
+        st = bank.state()
+    finally:
+        bank.close()
+    # read() is _g * _m, and _m holds the highest needle since the clip's first block (never read in between): formed here with the
+    # same fp32 multiply, because the bank's read() skips units whose clip ended before the last block
+    g = np.float32(design_ppm(kind, rate)[3])
+    reading = (g * st[:, 2].astype(np.float32)).astype(np.float32)
+    hist = hist.reshape(n, per, PPM_HIST_BINS); stats = stats.reshape(n, per); reading = reading.reshape(n, per)
+    ng, p95, p99 = _needle_dist(hist)
+
+    def sec(groups):                                      # 4 frames per group
+        return groups.astype(np.float64) * 4.0 / float(rate)
+    out = dict(hist=hist, stats=stats, groups=ng, seconds=sec(ng), nonfinite=stats["nonfinite"].astype(np.int64),
+               peak=stats["peak"].copy(), peak_db=_peak_db(stats["peak"]), p95_db=p95, p99_db=p99,
+               over_groups=stats["over_groups"].astype(np.int64), over_seconds=sec(stats["over_groups"]),
+               overs=stats["overs"].astype(np.int64), longest_over_s=sec(stats["longest_over"]), reading=reading)
+    if grp is not None:
+        out.update(needle_albums(hist, stats, grp))
     return out

@@ -18,17 +18,41 @@ constexpr int PPM_PLANE = 32 * PPM_P;                      // floats of one [32 
 
 struct PpmParams { float w1, w2, w3; };
 
+constexpr int PPM_EDGES = B200M_PPM_HIST_BINS - 1;
+
+// the needle histogram plane (b200m_ppm_hist_enable), one allocation: counts, then stats, then the edge table
+struct PpmHist {
+    unsigned long long* cnt;                               // [n_meters][B200M_PPM_HIST_BINS]
+    b200m_ppm_hist_stats* st;                              // [n_meters]
+    const float* edges;                                    // [PPM_EDGES]
+    float lim;                                             // L
+};
+
 // KIND 0: VU   1: IEC I/II PPM   3: M/S PPM (two planes: L and R rows of the pair)
 // RAG (b200m_ppm_process_ragged_*): unit u runs process() over its first rlen[u] <= nfram frames only.  Its lane stops at its own
 // (rlen[u] / 4) * 4; the warp still stages whole [32 x 64] tiles up to its longest row, so frames past a row's end are loaded but never
 // reach its filters.  A unit with rlen[u] == 0 was not called: no clamp, scrub or _res store.
-template <int KIND, bool ALIGNED, bool RAG = false>
+// HIST (b200m_ppm_hist_enable): after each group of 4 frames every meter forms the reading v = g * s of the needle value s the
+// reference compares with m, and counts it (include/b200meters.h).  The needle moves slowly against the 0.5 dB bins, so a lane holds
+// each meter's (bin, run) with the bin's two edges in registers and adds the run to the meter's own row with one fire-and-forget
+// atomic (RED) only when the bin changes and at kernel end; the edge table sits in shared memory for the search.  The meter's
+// statistics are loaded at kernel start and stored at kernel end: the lane owns its meters.  The recurrences, states and ports are
+// the same bits as without the plane.
+template <int KIND, bool ALIGNED, bool RAG = false, bool HIST = false>
 __global__ void __launch_bounds__ (PPM_WARPS * 32)
 ppm_kernel (const float* __restrict__ in, size_t stride, int n_units, int nfram, PpmParams pr, const float2* __restrict__ mv /* M/S: [unit] {mv_m, mv_s} */,
-            float* __restrict__ z1s, float* __restrict__ z2s, float* __restrict__ ms, int* __restrict__ ress, const uint32_t* __restrict__ rlen)
+            float* __restrict__ z1s, float* __restrict__ z2s, float* __restrict__ ms, int* __restrict__ ress, const uint32_t* __restrict__ rlen,
+            float gr /* read()'s _g */, PpmHist hp)
 {
     constexpr int PLANES = KIND == 3 ? 2 : 1;
     extern __shared__ __align__ (16) float ppm_smem[];
+    const float* E = nullptr;                              // HIST: the edge table
+    if constexpr (HIST) {
+        __shared__ float ppm_edges[PPM_EDGES];
+        for (int i = threadIdx.x; i < PPM_EDGES; i += blockDim.x) ppm_edges[i] = hp.edges[i];
+        __syncthreads ();                                  // before any warp leaves
+        E = ppm_edges;
+    }
     const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
     const int u0 = (blockIdx.x * PPM_WARPS + warp) * 32;    // first unit (meter, or stereo pair) of this warp
     if (u0 >= n_units) return;
@@ -91,6 +115,39 @@ ppm_kernel (const float* __restrict__ in, size_t stride, int n_units, int nfram,
     const float w4 = __fmul_rn (4.0f, pr.w1);
     const float2 g = KIND == 3 ? mv[u] : make_float2 (1.0f, 1.0f);
 
+    // HIST, per meter: the open run hr of readings in bin hb, whose edges are [hlo, hhi), and the statistics of b200m_ppm_hist_stats
+    int hb[NM] = {}; uint32_t hr[NM] = {}; float hlo[NM] = {}, hhi[NM] = {}, pk[NM] = {};
+    unsigned long long nnf[NM] = {}, nov[NM] = {}, novs[NM] = {}, nlong[NM] = {}, nrun[NM] = {};
+    if constexpr (HIST) {
+#pragma unroll
+        for (int q = 0; q < NM; ++q) {
+            const b200m_ppm_hist_stats& a = hp.st[NM * u + q];
+            nnf[q] = a.nonfinite; nov[q] = a.over_groups; novs[q] = a.overs; nlong[q] = a.longest_over; nrun[q] = a.run; pk[q] = a.peak;
+            hlo[q] = INFINITY; hhi[q] = -INFINITY;         // an empty range: the first reading searches
+        }
+    }
+    auto flush = [&] (int q) {                             // lanes past the bank repeat its last unit: they add nothing
+        if (live && hr[q]) atomicAdd (hp.cnt + (size_t)(NM * u + q) * B200M_PPM_HIST_BINS + hb[q], (unsigned long long)hr[q]);
+    };
+    auto tally = [&] (int q, float s) {
+        const float v = __fmul_rn (gr, s);
+        if (!finitef_ (v)) { ++nnf[q]; return; }           // no bin, and the over run stands
+        if (v > pk[q]) pk[q] = v;
+        if (v >= hp.lim) { ++nov[q]; novs[q] += nrun[q] == 0; ++nrun[q]; if (nrun[q] > nlong[q]) nlong[q] = nrun[q]; }
+        else nrun[q] = 0;
+        if (v >= hlo[q] && v < hhi[q]) { ++hr[q]; return; }
+        flush (q);
+        // bin = #{k : v >= E[k]}: an estimate from 40 log10 v + 161, corrected against the table, which alone defines the bins
+        int k = 0;
+        if (v >= E[0]) {
+            k = (int)fminf (fmaxf (__fadd_rn (__fmul_rn (__log2f (v), 12.0411998f), 161.0f), 1.0f), (float)PPM_EDGES);
+            while (k > 1 && v < E[k - 1]) --k;
+            while (k < PPM_EDGES && v >= E[k]) ++k;
+        }
+        hb[q] = k; hr[q] = 1;
+        hlo[q] = k > 0 ? E[k - 1] : -INFINITY; hhi[q] = k < PPM_EDGES ? E[k] : INFINITY;
+    };
+
     auto group = [&] (const float4 a, const float4 b) {
         const float xa[4] = {a.x, a.y, a.z, a.w}, xb[4] = {b.x, b.y, b.z, b.w};
         if (KIND == 0) {                                   // vumeterdsp.cc:57-68
@@ -102,6 +159,7 @@ ppm_kernel (const float* __restrict__ in, size_t stride, int n_units, int nfram,
             }
             z2[0] = __fadd_rn (z2[0], __fmul_rn (w4, __fsub_rn (z1[0], z2[0])));
             if (z2[0] > m[0]) m[0] = z2[0];
+            if constexpr (HIST) tally (0, z2[0]);
         } else {
 #pragma unroll
             for (int q = 0; q < NM; ++q) { z1[q] = __fmul_rn (z1[q], pr.w3); z2[q] = __fmul_rn (z2[q], pr.w3); }   // iec1ppmdsp.cc:59-60
@@ -118,7 +176,11 @@ ppm_kernel (const float* __restrict__ in, size_t stride, int n_units, int nfram,
                 }
             }
 #pragma unroll
-            for (int q = 0; q < NM; ++q) { const float s = __fadd_rn (z1[q], z2[q]); if (s > m[q]) m[q] = s; }
+            for (int q = 0; q < NM; ++q) {
+                const float s = __fadd_rn (z1[q], z2[q]);
+                if (s > m[q]) m[q] = s;
+                if constexpr (HIST) tally (q, s);
+            }
         }
     };
 
@@ -137,6 +199,16 @@ ppm_kernel (const float* __restrict__ in, size_t stride, int n_units, int nfram,
         issue (t + PPM_STAGES - 1);
     }
     cp_async_wait<0> ();
+    if constexpr (HIST) {
+#pragma unroll
+        for (int q = 0; q < NM; ++q) {
+            flush (q);
+            if (live) {
+                b200m_ppm_hist_stats& a = hp.st[NM * u + q];
+                a.nonfinite = nnf[q]; a.over_groups = nov[q]; a.overs = novs[q]; a.longest_over = nlong[q]; a.run = nrun[q]; a.peak = pk[q];
+            }
+        }
+    }
     bool ran = live;                                       // RAG: a unit with length 0 was not called
     if constexpr (RAG) ran = live && rl > 0;
     if (ran) {
@@ -174,6 +246,14 @@ __global__ void ppm_clear_kernel (int m0, int nm, float* z1s, float* z2s, float*
     z1s[m0 + i] = 0; z2s[m0 + i] = 0; ms[m0 + i] = 0; out[m0 + i] = 0; ress[m0 + i] = 1;
 }
 
+// the histogram rows of meters [m0, m0 + nm) back to an empty plane: counts and statistics zero, peak -INFINITY
+__global__ void ppm_hist_clear_kernel (int m0, int nm, unsigned long long* __restrict__ cnt, b200m_ppm_hist_stats* __restrict__ st)
+{
+    const size_t i = blockIdx.x * (size_t)blockDim.x + threadIdx.x;
+    if (i < (size_t)nm * B200M_PPM_HIST_BINS) cnt[(size_t)m0 * B200M_PPM_HIST_BINS + i] = 0;
+    if (i < (size_t)nm) st[m0 + i] = b200m_ppm_hist_stats {0, 0, 0, 0, 0, -INFINITY, 0};
+}
+
 }  // namespace b200m
 
 using namespace b200m;
@@ -186,7 +266,27 @@ struct b200m_ppm {
     float *d_z1 = nullptr, *d_z2 = nullptr, *d_m = nullptr, *d_out = nullptr; int* d_res = nullptr;
     RaggedLen rag; bool rag_read = false;                 // ragged blocks: lengths per unit; the last block was ragged (read skips length 0)
     BankPath path;
+    // the needle histogram plane (b200m_ppm_hist_enable): [n_meters][242] uint64 counts, then [n_meters] statistics, then the edge
+    // table, in one allocation so that a read is one copy; allocated on first use, kept until destroy
+    void* d_hist = nullptr;
+    bool hist = false;
+    float hist_lim = 0.0f;                                // L
+    unsigned long long* hist_cnt () const { return (unsigned long long*)d_hist; }
+    b200m_ppm_hist_stats* hist_st () const { return (b200m_ppm_hist_stats*)(hist_cnt () + (size_t)n_meters * B200M_PPM_HIST_BINS); }
+    float* hist_edges () const { return (float*)(hist_st () + n_meters); }
+    size_t hist_read_bytes () const { return (size_t)n_meters * (B200M_PPM_HIST_BINS * sizeof (uint64_t) + sizeof (b200m_ppm_hist_stats)); }
 };
+
+// the bin edges e[k] = (float) 10^((-80 + 0.5 k) / 20), computed in double once
+static const float* ppm_hist_table ()
+{
+    static const std::vector<float> e = [] {
+        std::vector<float> t (PPM_EDGES);
+        for (int k = 0; k < PPM_EDGES; ++k) t[k] = (float)pow (10.0, (-80.0 + 0.5 * k) / 20.0);
+        return t;
+    } ();
+    return e.data ();
+}
 
 static void ppm_design (int kind, float fs, float w[4])
 {
@@ -195,11 +295,11 @@ static void ppm_design (int kind, float fs, float w[4])
     else                             { w[0] = 200.0f / fs; w[1] = 860.0f / fs;  w[2] = 1.0f - 4.0f / fs; w[3] = 0.5141f; }            // iec2ppmdsp.cc:93-99, msppmdsp.cc:127-133
 }
 
-// ppm_kernel of a meter kind (both IEC kinds run KIND 1), an aligned block and a ragged one
-static auto ppm_kernel_for (int kind, bool al, bool rag)
+// ppm_kernel of a meter kind (both IEC kinds run KIND 1), an aligned block, a ragged one and the histogram plane
+static auto ppm_kernel_for (int kind, bool al, bool rag, bool hist)
 {
     return with_int<B200M_PPM_VU, B200M_PPM_MS, 1> (kind, [&] (auto K) {
-        return with_bools ([&] (auto AL, auto RAG) { return ppm_kernel<K, AL, RAG>; }, al, rag);
+        return with_bools ([&] (auto AL, auto RAG, auto HIST) { return ppm_kernel<K, AL, RAG, HIST>; }, al, rag, hist);
     });
 }
 
@@ -217,8 +317,18 @@ static int ppm_process (b200m_ppm* h, const float* d_in, size_t stride, uint32_t
     const size_t smem = (size_t)PPM_WARPS * PPM_STAGES * planes * PPM_PLANE * sizeof (float);
     const int nwarps = (h->n_units + 31) / 32;
     dim3 grid ((nwarps + PPM_WARPS - 1) / PPM_WARPS), blk (PPM_WARPS * 32);
-    ppm_kernel_for (h->kind, al, len)<<<grid, blk, smem, st>>> (d_in, stride, (int)h->n_units, (int)nfram, h->pr, h->d_mv, h->d_z1, h->d_z2, h->d_m,
-                                                            h->d_res, len ? h->rag.d : nullptr);
+    const PpmHist hp = h->hist ? PpmHist {h->hist_cnt (), h->hist_st (), h->hist_edges (), h->hist_lim} : PpmHist {};
+    ppm_kernel_for (h->kind, al, len, h->hist)<<<grid, blk, smem, st>>> (d_in, stride, (int)h->n_units, (int)nfram, h->pr, h->d_mv, h->d_z1, h->d_z2,
+                                                                     h->d_m, h->d_res, len ? h->rag.d : nullptr, h->g, hp);
+    B200M_LAUNCHED (1);
+    B200M_CUDA (cudaGetLastError ());
+    return 0;
+}
+
+static int ppm_hist_clear (b200m_ppm* h, int m0, int nm, cudaStream_t st)
+{
+    const size_t n = (size_t)nm * B200M_PPM_HIST_BINS;
+    ppm_hist_clear_kernel<<<(unsigned)((n + 255) / 256), 256, 0, st>>> (m0, nm, h->hist_cnt (), h->hist_st ());
     B200M_LAUNCHED (1);
     B200M_CUDA (cudaGetLastError ());
     return 0;
@@ -260,7 +370,8 @@ int b200m_ppm_create (b200m_ppm** out, int device, uint32_t n_units, float fsamp
     for (int k = B200M_PPM_VU; k <= B200M_PPM_MS; ++k)
         for (const bool al : {false, true})
             for (const bool rag : {false, true})
-                if (e == cudaSuccess) e = cudaFuncSetAttribute (ppm_kernel_for (k, al, rag), cudaFuncAttributeMaxDynamicSharedMemorySize, smem_max);
+                for (const bool hist : {false, true})
+                    if (e == cudaSuccess) e = cudaFuncSetAttribute (ppm_kernel_for (k, al, rag, hist), cudaFuncAttributeMaxDynamicSharedMemorySize, smem_max);
     if (e == cudaSuccess) {
         ppm_init_kernel<<<(unsigned)((nm + 255) / 256), 256>>> ((int)nm, h->d_res);    // constructors: _res (true)
         B200M_LAUNCHED (1);
@@ -276,7 +387,7 @@ int b200m_ppm_destroy (b200m_ppm* h)
     if (!h) return 0;
     DeviceGuard g (h->device);
     cudaDeviceSynchronize ();
-    cudaFree (h->d_z1); cudaFree (h->d_z2); cudaFree (h->d_m); cudaFree (h->d_out); cudaFree (h->d_res); cudaFree (h->d_mv); h->rag.release (); h->path.release ();
+    cudaFree (h->d_z1); cudaFree (h->d_z2); cudaFree (h->d_m); cudaFree (h->d_out); cudaFree (h->d_res); cudaFree (h->d_mv); cudaFree (h->d_hist); h->rag.release (); h->path.release ();
     delete h;
     return 0;
 }
@@ -304,9 +415,12 @@ int b200m_ppm_clear (b200m_ppm* h, int32_t unit, void* stream)
     DeviceGuard g (h->device);
     const int per = h->kind == B200M_PPM_MS ? 2 : 1;
     const int m0 = unit < 0 ? 0 : per * unit, nm = unit < 0 ? (int)h->n_meters : per;
-    ppm_clear_kernel<<<(nm + 255) / 256, 256, 0, h->path.stream (stream)>>> (m0, nm, h->d_z1, h->d_z2, h->d_m, h->d_out, h->d_res);
+    cudaStream_t st = h->path.stream (stream);
+    ppm_clear_kernel<<<(nm + 255) / 256, 256, 0, st>>> (m0, nm, h->d_z1, h->d_z2, h->d_m, h->d_out, h->d_res);
     B200M_LAUNCHED (1);
     B200M_CUDA (cudaGetLastError ());
+    if (h->hist)                                           // a cleared unit is a fresh meter for the histogram too
+        if (int rc = ppm_hist_clear (h, m0, nm, st)) return rc;
     if (h->kind == B200M_PPM_MS) {                         // the constructor's gains: a fresh Msppmdsp (-6) pair
         const uint32_t u0 = unit < 0 ? 0 : (uint32_t)unit, u1 = unit < 0 ? h->n_units : u0 + 1;
         for (uint32_t u = u0; u < u1; ++u) { h->db[u] = make_float2 (0, 0); h->mv[u] = make_float2 (1, 1); }
@@ -383,6 +497,51 @@ int b200m_ppm_state (b200m_ppm* h, float* state4, void* stream)
         state4[4 * i + 3] = (float)((const int*)(tmp + 3 * nm))[i];
     }
     free (tmp);
+    return 0;
+}
+
+int b200m_ppm_hist_enable (b200m_ppm* h, int enable, float limit_db, void* stream)
+{
+    if (!h) return set_err (B200M_E_INVAL, "NULL handle");
+    if (isnan (limit_db)) return set_err (B200M_E_INVAL, "limit_db must not be NaN");
+    DeviceGuard g (h->device);
+    if (!enable) { h->hist = false; return 0; }           // the plane's memory stays for the next enable
+    cudaStream_t st = h->path.stream (stream);
+    if (!h->d_hist) {
+        const cudaError_t e = cudaMalloc (&h->d_hist, h->hist_read_bytes () + PPM_EDGES * sizeof (float));
+        if (e != cudaSuccess) {
+            cudaGetLastError ();                               // a failed allocation is not sticky: later calls must not see it
+            h->d_hist = nullptr;
+            if (e == cudaErrorMemoryAllocation) return set_err (B200M_E_NOMEM, "needle histogram of %u meters: out of device memory", h->n_meters);
+            return cuda_fail (e, "b200m_ppm_hist_enable", __FILE__, __LINE__);
+        }
+        B200M_CUDA (cudaMemcpyAsync (h->hist_edges (), ppm_hist_table (), PPM_EDGES * sizeof (float), cudaMemcpyHostToDevice, st));
+    }
+    if (int rc = ppm_hist_clear (h, 0, (int)h->n_meters, st)) return rc;
+    h->hist_lim = (float)pow (10.0, (double)limit_db / 20.0);     // +inf dB: no reading is over; -inf dB: L = 0
+    h->hist = true;
+    return 0;
+}
+
+int b200m_ppm_hist_read (b200m_ppm* h, uint64_t* counts, b200m_ppm_hist_stats* stats, void* stream)
+{
+    if (!h || !counts || !stats) return set_err (B200M_E_INVAL, "NULL argument");
+    if (!h->hist) return set_err (B200M_E_INVAL, "the needle histogram plane is off (b200m_ppm_hist_enable)");
+    DeviceGuard g (h->device);
+    cudaStream_t st = h->path.stream (stream);
+    std::vector<unsigned char> buf (h->hist_read_bytes ());
+    B200M_CUDA (cudaMemcpyAsync (buf.data (), h->d_hist, buf.size (), cudaMemcpyDeviceToHost, st));
+    B200M_CUDA (cudaStreamSynchronize (st));
+    const size_t nc = (size_t)h->n_meters * B200M_PPM_HIST_BINS * sizeof (uint64_t);
+    memcpy (counts, buf.data (), nc);
+    memcpy (stats, buf.data () + nc, (size_t)h->n_meters * sizeof (b200m_ppm_hist_stats));
+    return 0;
+}
+
+int b200m_ppm_hist_edges (float* edges)
+{
+    if (!edges) return set_err (B200M_E_INVAL, "NULL argument");
+    memcpy (edges, ppm_hist_table (), PPM_EDGES * sizeof (float));
     return 0;
 }
 

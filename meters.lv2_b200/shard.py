@@ -13,6 +13,8 @@ Album spectra need no exchange of their own: gather_results collects each rank's
 programme_spectrum in clip order, and spectrum_albums pools them on the host exactly as it pools the rows of one bank.
 Album correlation distributions likewise: gather_results collects each rank's per-clip hist and sums of programme_correlation,
 and correlation_albums pools them on the host.
+Album needle distributions too: gather_results collects each rank's per-clip hist and stats of programme_needle, and needle_albums
+pools them on the host; every album value is an integer sum or a maximum, so any split of the clips gives the same result.
 """
 MIX_WORDS = 1508
 DR14_HISTBINS = 8000
