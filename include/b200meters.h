@@ -598,6 +598,38 @@ int b200m_ppm_hist_read (b200m_ppm* h, uint64_t* counts, b200m_ppm_hist_stats* s
 /* the library's 241 bin edges e[k] (host only: needs no device), so that callers bin with the same floats */
 int b200m_ppm_hist_edges (float* edges);
 
+/* True-peak / K-meter histogram (an extension of the b200m_tpk bank above; read() keeps only the highest value since the last read).
+ * With the plane on, every channel keeps a TP row (with B200M_TPK_TRUEPEAK) and a KM row (with B200M_TPK_KMETER): counts
+ * [B200M_PPM_HIST_BINS] (uint64) and a b200m_ppm_hist_stats, with the needle plane's edges e[k] (b200m_ppm_hist_edges) and rules: a
+ * finite reading u goes to bin #{k : u >= e[k]}; nonfinite counts the others; peak is the largest finite u (-INFINITY before the
+ * first); over_groups counts readings u >= L, overs their runs, longest_over the longest run (the open run included) and run the open
+ * run.  A non-finite reading neither starts, extends nor ends a run; runs continue across calls, ragged zero-length holds and the
+ * K-meter's unmetered nfram mod 4 tails.
+ * - TP: one reading per frame of TruePeakdsp::process (truepeakdsp.cc:57-84): u = the largest of the frame's four |out|, the values
+ *   the reference compares in "if (v > p) p = v"; a frame with a non-finite |out| is nonfinite.  With a read() after every block,
+ *   the finite frames' maximum in a block is that block's tp_p; a clip with no non-finite frame has peak = the _p of a meter never
+ *   read over it.
+ * - KM: one reading per group of 4 frames of Kmeterdsp::process (kmeterdsp.cc:80-98): after the group's z2 update, u = sqrtf (2 * z2)
+ *   (fp32, correctly rounded, no contraction), the rms the block end would form (:109) had the block ended there; a NaN z2 (which the
+ *   block end scrubs to 0) or a non-finite u is nonfinite.  L_km is dBFS RMS on the port's sine-calibrated scale.
+ * - L_tp = (float) pow (10.0, tp_limit_db / 20.0), L_km likewise from km_limit_db (double), per bank.
+ * Only process() blocks count, plain and ragged: a ragged row counts its own first len[i] frames, length 0 adds nothing.  While the
+ * plane is on every process() block runs the exact 16-channel kernel, whatever B200M_TPK_SPLIT, B200M_TPK_WIDE, B200M_TPK_DEC or
+ * the precision mode select: in a B200M_PREC_FMA bank the plane, the states and the readings are exact for those blocks.  Ports and
+ * b200m_tpk_state are bit-identical with the plane on or off; with it off the bank runs exactly the kernels it runs without it.
+ * process_max with the plane on returns B200M_E_UNSUPPORTED and enqueues nothing.  b200m_tpk_clear also zeroes the cleared
+ * channels' rows; b200m_tpk_reset, b200m_tpk_reset_kmeter and b200m_tpk_read_device leave the plane alone.  The plane is not part of
+ * b200m_tpk_snapshot, and b200m_tpk_restore leaves its rows as they are. */
+/* enable != 0: allocates the plane on first use (B200M_E_NOMEM if the device cannot hold it: 1984 bytes per channel and meter),
+ * zeroes every row (peak -INFINITY), also when it was on already, and sets both limits; 0: stops counting and keeps the memory.  A
+ * NaN limit returns B200M_E_INVAL; +-INFINITY is allowed.  The true-peak bank of an EBUr128 bank (b200m_r128_tpk) returns
+ * B200M_E_UNSUPPORTED.  Ordered like the getters. */
+int b200m_tpk_hist_enable (b200m_tpk* h, int enable, float tp_limit_db, float km_limit_db, void* stream);
+/* host counts [n_chan][B200M_PPM_HIST_BINS] and stats [n_chan] of each meter the bank has, in one copy and one synchronisation of
+ * the stream; the pointers of a meter the bank lacks must be NULL.  B200M_E_INVAL while the plane is off. */
+int b200m_tpk_hist_read (b200m_tpk* h, uint64_t* tp_counts, b200m_ppm_hist_stats* tp_stats, uint64_t* km_counts,
+                         b200m_ppm_hist_stats* km_stats, void* stream);
+
 /* ======================================================================================
  * Bit-meter and signal-distribution-histogram banks (SURVEY §8f rank 1), N mono instances each.
  * bit-meter: float_stats + the acquisition / ~5 fps window logic of bim_run (src/bitmeter.c:63-105,248-327);

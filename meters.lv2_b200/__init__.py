@@ -102,6 +102,8 @@ _PROTOS = {
     "b200m_tpk_debug_capture": (C.c_int, [_v, C.c_int]),
     "b200m_tpk_debug_timeline": (C.c_int, [_v, _v, C.c_int]),
     "b200m_tpk_debug_upsampled": (C.c_int, [_v, C.c_uint32, _v, C.c_uint32, _v]),
+    "b200m_tpk_hist_enable": (C.c_int, [_v, C.c_int, C.c_float, C.c_float, _v]),
+    "b200m_tpk_hist_read": (C.c_int, [_v, _v, _v, _v, _v, _v]),
     # EBUr128 plugin cycle
     "b200m_r128_create": (C.c_int, [C.POINTER(_v), C.c_int, C.c_uint32, C.c_float, C.c_int]),
     "b200m_r128_create_nch": (C.c_int, [C.POINTER(_v), C.c_int, C.c_uint32, C.c_uint32, C.c_float, C.c_int]),
@@ -591,6 +593,31 @@ class TruePeakKmeter(_Bank):
 
     def reset(self, chan=-1, stream=None):
         _ck(lib().b200m_tpk_reset(self.h, chan, _stream_ptr(stream)))
+
+    def clear(self, chan=-1, stream=None):
+        """chan (-1: all) back to a newly constructed meter (b200m_tpk_clear), its histogram rows too while the plane is on"""
+        _ck(lib().b200m_tpk_clear(self.h, chan, _stream_ptr(stream)))
+
+    def hist_enable(self, on=True, tp_limit_db=-1.0, km_limit_db=-10.0, stream=None):
+        """the histogram plane (b200m_tpk_hist_enable): on, every channel counts each process() frame's true-peak reading (the
+        largest of its four |out|) and each group of 4 frames' K-meter reading sqrtf(2 z2) in the 242 bins of PPM_HIST_EDGES, with
+        PPM_HIST_STATS_DTYPE's statistics, overs against 10^(tp_limit_db / 20) and 10^(km_limit_db / 20); (re)enabling zeroes every
+        row and sets the limits; off, the bank stops counting and runs its plain kernels.  process_max raises while it is on."""
+        _ck(lib().b200m_tpk_hist_enable(self.h, int(bool(on)), float(tp_limit_db), float(km_limit_db), _stream_ptr(stream)))
+
+    def hist(self, stream=None):
+        """(tp_counts, tp_stats, km_counts, km_stats) of the histogram plane (b200m_tpk_hist_read): counts int64 [n_chan, 242] and
+        stats PPM_HIST_STATS_DTYPE [n_chan] of each meter, None for a meter the bank lacks; raises while the plane is off"""
+        rows = []
+        for flag in (TPK_TRUEPEAK, TPK_KMETER):
+            if self.flags & flag:
+                rows.append((np.empty((self.n_chan, PPM_HIST_BINS), np.uint64), np.empty(self.n_chan, PPM_HIST_STATS_DTYPE)))
+            else:
+                rows.append((None, None))
+        ptrs = [_np_ptr(a) if a is not None else None for r in rows for a in r]
+        _ck(lib().b200m_tpk_hist_read(self.h, *ptrs, _stream_ptr(stream)))
+        (tc, ts), (kc, ks) = rows
+        return (None if tc is None else tc.astype(np.int64), ts, None if kc is None else kc.astype(np.int64), ks)
 
     def coeffs(self):
         w = np.empty(4, np.float32); t = np.empty(120, np.float32); k = np.empty(2, np.float32)
@@ -1684,4 +1711,86 @@ def programme_needle(x, lengths, kind, rate=48000.0, nchan=2, limit_db=0.0, ms_g
                overs=stats["overs"].astype(np.int64), longest_over_s=sec(stats["longest_over"]), reading=reading)
     if grp is not None:
         out.update(needle_albums(hist, stats, grp))
+    return out
+
+
+def _truepeak_fields(pfx, cnt, stats, rate, grp=None):
+    """programme_truepeak's fields of one meter ("tp": a reading per frame, "km": per 4 frames) from its rows, cnt int64 [N, M, 242]
+    and stats PPM_HIST_STATS_DTYPE [N, M]; grp: album ids for needle_albums, or None"""
+    fpr = 1 if pfx == "tp" else 4
+    unit, what = ("_dbtp", "frames") if pfx == "tp" else ("_db", "groups")
+
+    def sec(readings):
+        return readings.astype(np.float64) * fpr / float(rate)
+    ng, p95, p99 = _needle_dist(cnt)
+    out = {pfx + "_hist": cnt, pfx + "_stats": stats, pfx + "_" + what: ng, pfx + "_nonfinite": stats["nonfinite"].astype(np.int64),
+           pfx + "_peak": stats["peak"].copy(), pfx + "_peak" + unit: _peak_db(stats["peak"]), pfx + "_p95" + unit: p95,
+           pfx + "_p99" + unit: p99, pfx + "_over_" + what: stats["over_groups"].astype(np.int64),
+           pfx + "_over_seconds": sec(stats["over_groups"]), pfx + "_overs": stats["overs"].astype(np.int64),
+           pfx + "_longest_over_s": sec(stats["longest_over"])}
+    if grp is not None:
+        out.update({pfx + "_" + k: v for k, v in needle_albums(cnt, stats, grp).items()})
+    return out
+
+
+def programme_truepeak(x, lengths, rate=48000.0, nchan=2, flags=TPK_TRUEPEAK | TPK_KMETER, tp_limit_db=-1.0, km_limit_db=-10.0,
+                       block=1024, device=0, groups=None):
+    """True-peak and K-meter distributions of N clips of different lengths, in one TruePeakKmeter bank with the histogram plane on.
+
+    x: rows i * nchan + c of clip i, one true-peak meter and one K-meter per channel, clip i valid for its first lengths[i] frames: a
+    [N * nchan, >= max(lengths)] float32 numpy array / CPU tensor (host path) or CUDA tensor (device path), or a callable f(offset,
+    nfram) that returns frames offset .. offset + nfram - 1 of every row as such an array.  Frames past a clip's length are never
+    read into a result.  The clips are fed in process() blocks of `block` frames with clip i's length in block k clamp(lengths[i] -
+    k * block, 0, block) (TruePeakKmeter.process with lengths, repeated per channel), so clip i's numbers are bit-identical to one
+    TruePeakKmeter fed only that clip in blocks of `block` frames with the plane on (hist_enable(tp_limit_db=..., km_limit_db=...)).
+    flags: the meters to run (TPK_TRUEPEAK, TPK_KMETER or both); the fields of a meter the bank lacks are absent.
+    Returns a dict of [N, nchan] rows.  True peak, one reading per frame (the largest of its four 4x-oversampled |out|):
+      tp_hist (int64 [N, nchan, 242]): the finite readings in the bins of PPM_HIST_EDGES; tp_stats (PPM_HIST_STATS_DTYPE), for
+        needle_albums; tp_frames (int64): finite readings; tp_nonfinite (int64): frames with a non-finite |out|;
+      tp_peak (float32): the largest finite reading, -inf without one; tp_peak_dbtp (float64): 20 log10 tp_peak;
+      tp_p95_dbtp, tp_p99_dbtp (float64): the lower edge of the bin where the cumulative count first reaches 95 % / 99 % of tp_frames
+        (-inf: below -80 dB; NaN: no reading); a p99 within a dB of tp_peak_dbtp marks an over-limited master;
+      tp_over_frames (int64) and tp_over_seconds (float64): frames at or above 10^(tp_limit_db / 20), e.g. the -1 dBTP ceiling of EBU
+        R128; tp_overs (int64): their separate runs; tp_longest_over_s (float64): the longest run's time;
+      tp_max_dbtp (float64 [N]): the largest tp_peak_dbtp over the clip's channels.
+    K-meter, one reading per group of 4 frames (sqrtf(2 z2), the rms port's value had a block ended after that group; a block's last
+    nfram mod 4 frames are not metered, as in the reference): km_hist, km_stats, km_groups, km_nonfinite, km_peak, km_peak_db,
+      km_p95_db, km_p99_db, km_over_groups, km_over_seconds, km_overs, km_longest_over_s likewise, 4 frames per reading.
+      km_limit_db is dBFS RMS on the port's sine-calibrated scale: -10 dBFS is +4 on a K-14 scale, so the default counts the time
+      spent above the K-14 meter's +4 zone.
+    Final readings of the clip's last block, as read() would return them with no read in between: tp_m and tp_p (true peak), km_rms
+    and km_peak (K-meter) (float32 [N, nchan]; 0 for an empty clip).
+    groups: None, or N album ids (>= 0, or -1 for a clip in no album): the dict then also holds needle_albums of each meter's rows
+    under the keys tp_album_* and km_album_* (album_hist, album_groups, album_peak_db, album_p95_db, album_overs, ...)."""
+    ln, blocks = _programme_blocks(x, lengths, block, "no clips")
+    n = ln.size
+    grp = None if groups is None else _groups(groups, n)
+    flags = int(flags)
+    if flags not in (TPK_TRUEPEAK, TPK_KMETER, TPK_TRUEPEAK | TPK_KMETER):
+        raise B200MError("flags must be TPK_TRUEPEAK, TPK_KMETER or both")
+    per = int(nchan)
+    if per < 1:
+        raise B200MError("nchan must be >= 1")
+    bank = TruePeakKmeter(n * per, rate, flags, device)
+    try:
+        bank.hist_enable(tp_limit_db=tp_limit_db, km_limit_db=km_limit_db)
+        for _, xb, lb in blocks:
+            bank.process(xb, lengths=np.repeat(lb, per))        # each meter of a clip runs the clip's frames
+        tc, ts, kc, ks = bank.hist()
+        st = bank.state()
+    finally:
+        bank.close()
+    out = {}
+    for pfx, cnt, stats in (("tp", tc, ts), ("km", kc, ks)):
+        if cnt is not None:
+            out.update(_truepeak_fields(pfx, cnt.reshape(n, per, PPM_HIST_BINS), stats.reshape(n, per), rate, grp))
+    if tc is not None:
+        out["tp_max_dbtp"] = out["tp_peak_dbtp"].max(axis=1)
+        # read() returns _m and _p; no read happens in between, so they hold the whole clip's values (0 for an empty clip: _res)
+        res = st["res"].astype(bool)
+        out["tp_m"] = np.where(res, np.float32(0), st["m"]).astype(np.float32).reshape(n, per)
+        out["tp_p"] = np.where(res, np.float32(0), st["p"]).astype(np.float32).reshape(n, per)
+    if kc is not None:
+        out["km_rms"] = st["km"][:, 2].astype(np.float32).reshape(n, per)
+        out["km_peak"] = st["km"][:, 3].astype(np.float32).reshape(n, per)
     return out

@@ -106,6 +106,7 @@ int tpk_process_sliced (b200m_tpk* h, const float* d_in, size_t stride, uint32_t
                         b200m::R128Hold r128, bool pdl, const void* dr, const uint32_t* rlen, b200m::TpSplit sp);
 bool tpk_r128_fused_ok (const b200m_tpk* h, const float* d_in, size_t stride, uint32_t nfram);
 float* tpk_hist (b200m_tpk* h);
+void tpk_set_r128_owned (b200m_tpk* h);                            // b200m_tpk_hist_enable on it returns B200M_E_UNSUPPORTED
 int tpk_r128_fused (b200m_tpk* h, const b200m::EbuK1Args& a, float* r128_tpmax, cudaStream_t st);
 
 using namespace b200m;
@@ -280,6 +281,7 @@ static int r128_create (b200m_r128** out, int device, uint32_t n_inst, uint32_t 
                    : b200m_ebu_create (&h->ebu, device, n_inst, nchan, fsamp);                // ebu->init (nchan, rate), src/ebulv2.cc:190
     if (!rc) ebu_follow (h->ebu, &h->path);       // b200m_r128_ebu (h)'s getters and log calls are ordered after this bank's calls
     if (!rc) rc = b200m_tpk_create (&h->tpk, device, nchan * n_inst, fsamp, B200M_TPK_TRUEPEAK);   // nchan x TruePeakdsp, :192-196
+    if (!rc) tpk_set_r128_owned (h->tpk);
     if (!rc) {
         DeviceGuard g (device);
         cudaError_t e = cudaMalloc ((void**)&h->d_tpmax, n_inst * sizeof (float));

@@ -437,6 +437,45 @@ struct TpkRag {
     const uint32_t* len; const float* fall; int nch;
 };
 
+constexpr int TPK_HIST_BINS = B200M_PPM_HIST_BINS, TPK_HIST_EDGES = B200M_PPM_HIST_BINS - 1;
+
+// The programme plane (b200m_tpk_hist_enable): per channel a row of the true-peak frames' readings and one of the K-meter groups'
+// readings, each 242 uint64 counts and a b200m_ppm_hist_stats.  A meter the bank lacks has null rows.
+struct TpkHistPlane {
+    unsigned long long *tp_cnt, *km_cnt;                   // [n_chan][242]
+    b200m_ppm_hist_stats *tp_st, *km_st;                   // [n_chan]
+    const float* edges;                                    // [241] e[k], the needle plane's edges
+    const float* kthr;                                     // [241] the least float t with sqrtf (t) >= e[k]
+    float tp_lim;                                          // L_tp
+    float km_thr;                                          // the least float t with sqrtf (t) >= L_km
+};
+// dynamic shared memory of the plane's per-CTA true-peak counts: 16 rows x 242 uint16 (a block has at most 8192 frames)
+constexpr size_t TPK_HIST_SMEM = (size_t)16 * TPK_HIST_BINS * sizeof (unsigned short);
+
+// bin #{k : v >= t[k]} of a table t of 241 ascending floats, for a v >= t[0]: an estimate from est = 40 log10 of the reading + 161,
+// corrected against the table (read through L1), which alone defines the bins
+B200M_DEV int tpk_hist_bin (const float* __restrict__ t, float v, float est)
+{
+    int k = (int)fminf (fmaxf (est, 1.0f), (float)TPK_HIST_EDGES);
+    while (k > 1 && v < __ldg (t + k - 1)) --k;
+    while (k < TPK_HIST_EDGES && v >= __ldg (t + k)) ++k;
+    return k;
+}
+
+// a row's statistics in registers while its lane counts one chunk: loaded before the chunk, stored after it, so that none of them is
+// live through the FIR phase (that would cost the FIR its registers)
+struct TpkHistStats {
+    unsigned long long nnf, nov, novs, nlong, nrun; float pk;
+    B200M_DEV void load (const b200m_ppm_hist_stats& a) { nnf = a.nonfinite; nov = a.over_groups; novs = a.overs; nlong = a.longest_over; nrun = a.run; pk = a.peak; }
+    B200M_DEV void store (b200m_ppm_hist_stats& a) const { a.nonfinite = nnf; a.over_groups = nov; a.overs = novs; a.longest_over = nlong; a.run = nrun; a.peak = pk; }
+    // a finite reading against the limit: over runs continue across chunks and calls
+    B200M_DEV void over (bool o)
+    {
+        if (o) { ++nov; novs += nrun == 0; ++nrun; if (nrun > nlong) nlong = nrun; }
+        else nrun = 0;
+    }
+};
+
 // RAG (exact 16-channel process(): tpk_kernel<16, 64, TP, false, KM, IMM, DR, false, true> with true peak, the K-meter or both):
 // every row stops at its own length rl.  The FIR phase runs as for a plain block: it is causal, so the outputs before rl never see the unread frames, and
 // unread frames can only make the silence and phase-0 elision guards more conservative (row_absmax propagates NaN, Inf and large
@@ -444,12 +483,22 @@ struct TpkRag {
 // their loop past rl (its z1 + z2 shuffle needs the whole warp) with their state frozen; the K-meter lanes drop rl mod 4 samples
 // and use rl for _fpp and the hold count; the DR lanes add only samples before rl and close a window only at a cut before rl.
 // A row with rl == 0 did not run: no end-of-block update.  Its next history is the 48 samples before rl (old history first).
-template <int CH, int TC, bool TP, bool TPMAX, bool KM, bool IMM, bool DR, bool FMA = false, bool RAG = false>
+// HIST (b200m_tpk_hist_enable; exact 16-channel process(), plain or ragged): the programme plane (include/b200meters.h) on lanes
+// that no recurrence uses.  True peak: a lane of warp role 2 (idle without DR-14 sums) per channel walks the |out| tile `ob` the
+// ballistics lanes walk, after the same barrier, and takes each frame's reading u = max of its four |out| (all finite, else the
+// frame is non-finite).  The reading has no smoothing and changes bin almost every frame, so the counts go to a per-CTA uint16 row in
+// shared memory (a block has at most 8192 frames), added to the channel's uint64 row at kernel end, and only the last bin's edges are
+// kept in registers.  K-meter: the K-meter lane takes y = 2 z2 after each group's z2 update and bins it against the thresholds
+// kthr[k] (sqrtf is monotone, so y >= kthr[k] <=> sqrtf (y) >= e[k]); the reading moves slowly, so (bin, run) and the bin's two
+// thresholds stay in registers and a run goes to the channel's row with a fire-and-forget atomic (RED) when the bin changes.  The
+// statistics are loaded at kernel start and stored at kernel end: the lane owns its channel.  No recurrence changes a bit.
+template <int CH, int TC, bool TP, bool TPMAX, bool KM, bool IMM, bool DR, bool FMA = false, bool RAG = false, bool HIST = false>
 __global__ void __launch_bounds__ (TPK_THREADS)
 tpk_kernel (const float* __restrict__ in, size_t stride, int c_first, int n_chan, int nfram, int aligned, int elide0, TpkParams prm,
-            TpkState st, float* __restrict__ dbg, R128Hold r128, TpkDr dr, TpkRag rag)
+            TpkState st, float* __restrict__ dbg, R128Hold r128, TpkDr dr, TpkRag rag, TpkHistPlane hp)
 {
     static_assert (!RAG || (CH == 16 && !TPMAX && (TP || KM) && !FMA), "the ragged form is the exact 16-channel process() kernel");
+    static_assert (!HIST || (CH == 16 && !TPMAX && !DR && !FMA), "the histogram plane runs in the exact 16-channel process() kernel");
     // processes channels [c_first, n_chan): `n_chan` is the END of the slice (absolute channel index)
     constexpr int XP = TpkGeom<CH, TC, TP && !TPMAX>::XP;   // x row pitch (floats): 16-byte multiple
     constexpr int OP = 4 * TC + 4;                // |out| row pitch
@@ -468,6 +517,11 @@ tpk_kernel (const float* __restrict__ in, size_t stride, int c_first, int n_chan
     extern __shared__ __align__ (16) float tpk_smem[];        // xs[2][CH][XP], then ob[BAL ? CH : 1][BAL ? OP : 4]
     float (*xs)[CH][XP] = reinterpret_cast<float (*)[CH][XP]> (tpk_smem);
     float (*ob)[BAL ? OP : 4] = reinterpret_cast<float (*)[BAL ? OP : 4]> (tpk_smem + 2 * CH * XP);
+    constexpr bool THIST = HIST && BAL;           // the true-peak plane's counts, after ob: [CH][242] uint16
+    unsigned short (*th)[TPK_HIST_BINS] = reinterpret_cast<unsigned short (*)[TPK_HIST_BINS]> (tpk_smem + 2 * CH * XP + (BAL ? CH * OP : 4));
+    if constexpr (THIST) {
+        for (int i = threadIdx.x; i < CH * TPK_HIST_BINS / 2; i += TPK_THREADS) reinterpret_cast<unsigned*> (&th[0][0])[i] = 0u;
+    }
     const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
     const int c0 = c_first + blockIdx.x * CH;
     // Chunk schedule.  Co-resident CTAs of process() start together and would run their FIR phases (issue-bound, every warp busy) and
@@ -548,6 +602,9 @@ tpk_kernel (const float* __restrict__ in, size_t stride, int c_first, int n_chan
         kz1 = a > 50 ? 50 : (a < 0 ? 0 : a);
         kz2 = b > 50 ? 50 : (b < 0 ? 0 : b);
     }
+    // HIST: role 2 counts the true-peak frames, lane = channel (no DR-14 sums here); the K-meter lanes count their groups.  Only the
+    // lanes of the bank's channels count (the others would repeat its last channel).
+    const bool is_th = THIST && wrole == 2 && lane < CH && live;
     // role 2 (idle otherwise while the serial lanes run): DR-14 sums, lane = channel
     const bool dr_warp = DR && BAL && KM && dr.rms_sum != nullptr && (ALLW || wrole == 2);
     const int drow = wbase + (lane & 15);
@@ -715,11 +772,52 @@ tpk_kernel (const float* __restrict__ in, size_t stride, int c_first, int n_chan
                 if constexpr (RAG) step_rag (b4[(j & 3) * GPC + (j >> 2)], j); else step (b4[(j & 3) * GPC + (j >> 2)]);
             }
         }
+        if (is_th) {
+            // HIST: the frames of this row's chunk (RAG: before its end), the same float4 slots the ballistics lanes read.  u = the largest
+            // of a frame's four |out| (>= +0, or NaN) when all are finite; the last bin and its edges [lo, hi) save most table reads.
+            const float4* b4 = reinterpret_cast<const float4*> (&ob[BAL ? lane : 0][0]);
+            unsigned short* row = th[lane];
+            int e = len;
+            if constexpr (RAG) e = max (0, min (len, rl - s0));
+            TpkHistStats a; a.load (hp.tp_st[chs]);
+            int hb = 0; float lo = INFINITY, hi = -INFINITY;
+#pragma unroll 1
+            for (int j = 0; j < e; ++j) {
+                const float4 v = b4[(j & 3) * GPC + (j >> 2)];
+                if (!(v.x < INFINITY && v.y < INFINITY && v.z < INFINITY && v.w < INFINITY)) { ++a.nnf; continue; }   // no bin, the run stands
+                const float u = fmaxf (fmaxf (v.x, v.y), fmaxf (v.z, v.w));
+                if (u > a.pk) a.pk = u;
+                a.over (u >= hp.tp_lim);
+                if (!(u >= lo && u < hi)) {
+                    hb = u >= __ldg (hp.edges) ? tpk_hist_bin (hp.edges, u, __fadd_rn (__fmul_rn (__log2f (u), 12.0411998f), 161.0f)) : 0;
+                    lo = hb > 0 ? __ldg (hp.edges + hb - 1) : -INFINITY; hi = hb < TPK_HIST_EDGES ? __ldg (hp.edges + hb) : INFINITY;
+                }
+                ++row[hb];
+            }
+            a.store (hp.tp_st[chs]);
+        }
         if (is_km) {
             // kmeterdsp.cc:80-97: z1 every sample, z2 every 4th; the block's last n%4 samples are ignored
             const int e = min (len, km_n - s0);
             const float4* x4 = reinterpret_cast<const float4*> (&xs[buf][wbase + lane][48]);
             const float om4 = __fmul_rn (4.0f, prm.omega);
+            // HIST: the open run hr of readings in bin hb, whose thresholds are [lo, hi), goes to the row with one RED when the bin
+            // changes and at the chunk's end; ymax: the largest finite y of the chunk (its root is taken once)
+            TpkHistStats a; int hb = 0; uint32_t hr = 0; float lo = INFINITY, hi = -INFINITY, ymax = -INFINITY;
+            if constexpr (HIST) a.load (hp.km_st[chs]);
+            auto flush = [&] { if (live && hr) atomicAdd (hp.km_cnt + (size_t)chs * TPK_HIST_BINS + hb, (unsigned long long)hr); };
+            // a group's y = 2 z2 (fp32): the reading is sqrtf (y), non-finite where y is NaN, negative or +Inf
+            auto tally = [&] (const float y) {
+                if (!(y >= 0.0f && y < INFINITY)) { ++a.nnf; return; }    // no bin, and the over run stands
+                if (y > ymax) ymax = y;
+                a.over (y >= hp.km_thr);
+                if (y >= lo && y < hi) { ++hr; return; }
+                flush ();
+                // 20 log10 y + 161 = 40 log10 sqrtf (y) + 161
+                hb = y >= __ldg (hp.kthr) ? tpk_hist_bin (hp.kthr, y, __fadd_rn (__fmul_rn (__log2f (y), 6.02059991f), 161.0f)) : 0;
+                hr = 1;
+                lo = hb > 0 ? __ldg (hp.kthr + hb - 1) : -INFINITY; hi = hb < TPK_HIST_EDGES ? __ldg (hp.kthr + hb) : INFINITY;
+            };
             for (int j = 0; j + 4 <= e; j += 4) {
                 const float4 v4 = x4[j >> 2];
                 const float vv[4] = {v4.x, v4.y, v4.z, v4.w};
@@ -733,6 +831,12 @@ tpk_kernel (const float* __restrict__ in, size_t stride, int c_first, int n_chan
                 }
                 if (FMA) kz2 = fmaf (om4, __fsub_rn (kz1, kz2), kz2);
                 else kz2 = __fadd_rn (kz2, __fmul_rn (om4, __fsub_rn (kz1, kz2)));
+                if constexpr (HIST) tally (__fmul_rn (2.0f, kz2));
+            }
+            if constexpr (HIST) {
+                flush ();
+                if (ymax >= 0.0f) { const float u = __fsqrt_rn (ymax); if (u > a.pk) a.pk = u; }     // sqrtf is monotone
+                if (live) a.store (hp.km_st[chs]);
             }
         }
         if (dr_warp) {
@@ -767,6 +871,15 @@ tpk_kernel (const float* __restrict__ in, size_t stride, int c_first, int n_chan
     }
     cp_async_wait<0> ();
     if (dr_live) { dr.rms_sum[dch] = drs; dr.peak_cur[dch] = drp; }
+    if constexpr (THIST) {
+        __syncthreads ();                                   // every count of the block is in th (also when the block had no chunk)
+        // this CTA alone runs its channels: plain adds, non-zero bins only
+        for (int i = tid; i < CH * TPK_HIST_BINS; i += TPK_THREADS) {
+            const int r = i / TPK_HIST_BINS, k = i - r * TPK_HIST_BINS;
+            const unsigned v = th[r][k];
+            if (v && c0 + r < n_chan) hp.tp_cnt[(size_t)(c0 + r) * TPK_HIST_BINS + k] += v;
+        }
+    }
 
     // ---- end of block --------------------------------------------------------------------
     if (TP && !RAG) {                                       // (RAG: written in the chunk loop)
@@ -2132,6 +2245,15 @@ __global__ void tpk_reset_kernel (int n_chan, int sel, uint32_t flags, TpkState 
     }
 }
 
+// the histogram rows of channels [c0, c0 + nc) of the nm present meters back to an empty plane: counts and statistics zero, peak
+// -INFINITY
+__global__ void tpk_hist_clear_kernel (int n_chan, int nm, int c0, int nc, unsigned long long* __restrict__ cnt, b200m_ppm_hist_stats* __restrict__ st)
+{
+    const size_t i = blockIdx.x * (size_t)blockDim.x + threadIdx.x, per = (size_t)nc * TPK_HIST_BINS;
+    if (i < (size_t)nm * per) cnt[(i / per) * n_chan * TPK_HIST_BINS + (size_t)c0 * TPK_HIST_BINS + i % per] = 0;
+    if (i < (size_t)nm * nc) st[(i / nc) * n_chan + c0 + i % nc] = b200m_ppm_hist_stats {0, 0, 0, 0, 0, -INFINITY, 0};
+}
+
 }  // namespace b200m
 
 using namespace b200m;
@@ -2159,6 +2281,25 @@ struct b200m_tpk {
     RaggedLen rag; std::vector<float> fall; std::vector<uint8_t> fall_ok;
     bool rag_read = false;                  // the last process() block was a b200m_tpk_process_ragged_* one: read() skips its length-0 rows
     BankPath path;
+    bool r128_owned = false;                // the true-peak bank of an EBUr128 bank (b200m_r128_tpk): process_max only, no histogram plane
+    // the histogram plane (b200m_tpk_hist_enable): [nm][n_chan][242] uint64 counts, then [nm][n_chan] statistics (nm present meters,
+    // true peak first), then the edges and the K-meter thresholds, in one allocation so that a read is one copy; allocated on first
+    // use, kept until destroy
+    void* d_hist = nullptr;
+    bool hist = false;
+    float hist_tp_lim = 0.0f, hist_km_thr = 0.0f;
+    int hist_nm () const { return ((flags & B200M_TPK_TRUEPEAK) ? 1 : 0) + ((flags & B200M_TPK_KMETER) ? 1 : 0); }
+    unsigned long long* hist_cnt (int q) const { return (unsigned long long*)d_hist + (size_t)q * n_chan * TPK_HIST_BINS; }
+    b200m_ppm_hist_stats* hist_st (int q) const { return (b200m_ppm_hist_stats*)hist_cnt (hist_nm ()) + (size_t)q * n_chan; }
+    float* hist_tab () const { return (float*)hist_st (hist_nm ()); }       // edges [241], then the K-meter thresholds [241]
+    size_t hist_read_bytes () const { return (size_t)hist_nm () * n_chan * (TPK_HIST_BINS * sizeof (uint64_t) + sizeof (b200m_ppm_hist_stats)); }
+    TpkHistPlane hist_plane () const
+    {
+        const int qk = (flags & B200M_TPK_TRUEPEAK) ? 1 : 0;
+        const bool tp = flags & B200M_TPK_TRUEPEAK, km = flags & B200M_TPK_KMETER;
+        return TpkHistPlane {tp ? hist_cnt (0) : nullptr, km ? hist_cnt (qk) : nullptr, tp ? hist_st (0) : nullptr, km ? hist_st (qk) : nullptr,
+                             hist_tab (), hist_tab () + TPK_HIST_EDGES, hist_tp_lim, hist_km_thr};
+    }
 };
 
 // zita-resampler table for (fr = 1.0, hl = 24, np = 4); restates Resampler_table's constructor
@@ -2236,13 +2377,13 @@ static TpmaxTcKernel tpmax_tc_kernel_for (int hold) { return with_hold (hold, []
 // tpk_kernel<CH, TC, TP, MX, ...> of a FIR form, the K-meter and the DR-14 sums.  Choices that mean nothing for a form collapse, so
 // that only launchable forms are instantiated: without true peak there is no FIR and the bank is a K-meter; the DR-14 sums ride on
 // process() with both meters; a ragged block runs the exact kernel, with the immediates only beside the K-meter (the true-peak-only
-// immediate form spills 8 bytes).
+// immediate form spills 8 bytes).  The histogram plane (HIST) runs the exact kernel without DR-14 sums, as a ragged block does.
 using TpkKernel = decltype (&tpk_kernel<16, 64, true, false, true, false, false>);
-template <int CH, int TC, bool TP, bool MX, bool RAG = false> static TpkKernel tpk_kernel_for (TpkFir m, bool km, bool dr)
+template <int CH, int TC, bool TP, bool MX, bool RAG = false, bool HIST = false> static TpkKernel tpk_kernel_for (TpkFir m, bool km, bool dr)
 {
     return with_fir (m, [&] (auto IMM, auto FMA) {
         return with_bools ([&] (auto KM, auto DR) {
-            return tpk_kernel<CH, TC, TP, MX, KM || !TP, IMM && TP && (KM || !RAG), DR && KM && TP && !MX, FMA && TP && !RAG, RAG>;
+            return tpk_kernel<CH, TC, TP, MX, KM || !TP, IMM && TP && (KM || !(RAG || HIST)), DR && KM && TP && !MX && !HIST, FMA && TP && !RAG && !HIST, RAG, HIST>;
         }, km, dr);
     });
 }
@@ -2312,6 +2453,10 @@ int tpk_process_sliced (b200m_tpk* h, const float* d_in, size_t stride, uint32_t
         TpmaxKernel mk = nullptr; TpmaxTcKernel ck = nullptr; TpkKernel tk = nullptr; TpdecKernel dk = nullptr;
         auto tpk = [&] (TpkKernel k, int ch, size_t smem) { tk = k; cfg.gridDim = dim3 ((ce - cf + ch - 1) / ch); cfg.dynamicSmemBytes = smem; };
         if (rlen || sp.fmax) mk = tpmax_kernel_for (m, hold, rlen, sp.fmax);
+        // the histogram plane (process() only: b200m_tpk_block refuses process_max while it is on) counts in the exact 16-channel
+        // kernel, whatever the slab pipeline, the decoupled kernel, the wide form or the precision mode would pick
+        else if (h->hist && tp) tpk (tpk_kernel_for<16, 64, true, false, false, true> (m, km, false), 16, TpkGeom<16, 64, true>::BYTES + TPK_HIST_SMEM);
+        else if (h->hist) tpk (tpk_kernel_for<16, 64, false, false, false, true> (m, km, false), 16, TpkGeom<16, 64, false>::BYTES);
         else if (tp_mode == B200M_TP_MODE_MAX && tpk_tc_ok (h, aligned, nfram) && (ce - cf + 7) / 8 >= h->n_sm) {
             // tensor-core path: persistent CTAs, each takes whole 8-channel groups (a bank too small to give every SM a group runs tpmax_kernel)
             ck = tpmax_tc_kernel_for (hold);
@@ -2361,7 +2506,8 @@ int tpk_process_sliced (b200m_tpk* h, const float* d_in, size_t stride, uint32_t
             B200M_CUDA (cudaLaunchKernelEx (&cfg, mk, d_in, stride, cf, ce, (int)nfram, nchunks, aligned, h->elide0, h->st, h->d_dbg, r128, rlen, sp));
             swap_hist = true;
         }
-        if (tk) B200M_CUDA (cudaLaunchKernelEx (&cfg, tk, d_in, stride, cf, ce, (int)nfram, aligned, h->elide0, prm, h->st, h->d_dbg, r128, drp, TpkRag {}));
+        if (tk) B200M_CUDA (cudaLaunchKernelEx (&cfg, tk, d_in, stride, cf, ce, (int)nfram, aligned, h->elide0, prm, h->st, h->d_dbg, r128, drp, TpkRag {},
+                                                h->hist ? h->hist_plane () : TpkHistPlane {}));
         if (dk) B200M_CUDA (cudaLaunchKernelEx (&cfg, dk, d_in, stride, cf, ce, (int)nfram, aligned, h->elide0, prm, h->st));
         B200M_LAUNCHED (1);
     }
@@ -2374,6 +2520,25 @@ static int tpk_process (b200m_tpk* h, const float* d_in, size_t stride, uint32_t
 {
     const uint32_t bounds[2] = {0, h->n_chan};
     return tpk_process_sliced (h, d_in, stride, nfram, tp_mode, st, 1, bounds, nullptr, R128Hold {}, false, h->dr_on ? &h->dr : nullptr, nullptr, TpSplit {});
+}
+
+static int tpk_hist_clear (b200m_tpk* h, int c0, int nc, cudaStream_t st)
+{
+    const size_t n = (size_t)h->hist_nm () * nc * TPK_HIST_BINS;
+    tpk_hist_clear_kernel<<<(unsigned)((n + 255) / 256), 256, 0, st>>> ((int)h->n_chan, h->hist_nm (), c0, nc, h->hist_cnt (0), h->hist_st (0));
+    B200M_LAUNCHED (1);
+    B200M_CUDA (cudaGetLastError ());
+    return 0;
+}
+
+// the least float t with sqrtf (t) >= e (host sqrtf, correctly rounded like the device's __fsqrt_rn): y >= t <=> sqrtf (y) >= e for
+// every float y, so the K-meter's readings are binned without a root.  e = 0: t = 0; e = +INFINITY: t = +INFINITY.
+static float tpk_sqrt_threshold (float e)
+{
+    float t = (float)((double)e * (double)e);
+    while (sqrtf (t) < e) t = nextafterf (t, INFINITY);
+    for (float d = nextafterf (t, -INFINITY); sqrtf (d) >= e; d = nextafterf (t, -INFINITY)) t = d;
+    return t;
 }
 
 namespace b200m {
@@ -2406,10 +2571,13 @@ int tpk_process_ragged (b200m_tpk* h, const float* d_in, size_t stride, uint32_t
     const TpkRag rag = {d_len, d_fall, (int)per};
     const int aligned = ((uintptr_t)d_in % 16 == 0) && (stride % 4 == 0);
     const unsigned grid = (h->n_chan + 15) / 16;
-    const TpkKernel k = tp ? tpk_kernel_for<16, 64, true, false, true> (tpk_mode (h), km, drp.rms_sum)
+    const TpkKernel k = h->hist ? (tp ? tpk_kernel_for<16, 64, true, false, true, true> (tpk_mode (h), km, false)
+                                      : tpk_kernel_for<16, 64, false, false, true, true> (tpk_mode (h), km, false))
+                      : tp ? tpk_kernel_for<16, 64, true, false, true> (tpk_mode (h), km, drp.rms_sum)
                            : tpk_kernel_for<16, 64, false, false, true> (tpk_mode (h), km, false);
-    k<<<grid, TPK_THREADS, tp ? TpkGeom<16, 64, true>::BYTES : TpkGeom<16, 64, false>::BYTES, st>>> (
-        d_in, stride, 0, (int)h->n_chan, (int)nfram, aligned, h->elide0, h->prm, h->st, h->d_dbg, R128Hold {}, drp, rag);
+    const size_t smem = tp ? TpkGeom<16, 64, true>::BYTES + (h->hist ? TPK_HIST_SMEM : 0) : TpkGeom<16, 64, false>::BYTES;
+    k<<<grid, TPK_THREADS, smem, st>>> (d_in, stride, 0, (int)h->n_chan, (int)nfram, aligned, h->elide0, h->prm, h->st, h->d_dbg, R128Hold {}, drp, rag,
+                                        h->hist ? h->hist_plane () : TpkHistPlane {});
     B200M_LAUNCHED (1);
     B200M_CUDA (cudaGetLastError ());
     return 0;
@@ -2434,6 +2602,7 @@ constexpr uint32_t R128F_MIN_CH = 10240;
 
 // the history the next block reads (48 floats per channel): after a block, the buffer its kernels left current
 float* tpk_hist (b200m_tpk* h) { return h->st.hist; }
+void tpk_set_r128_owned (b200m_tpk* h) { h->r128_owned = true; }
 
 bool tpk_r128_fused_ok (const b200m_tpk* h, const float* d_in, size_t stride, uint32_t nfram)
 {
@@ -2591,7 +2760,8 @@ int b200m_tpk_destroy (b200m_tpk* h)
     DeviceGuard g (h->device);
     cudaDeviceSynchronize ();
     void* ps[] = {h->st.hist, h->st.tp_z1, h->st.tp_z2, h->st.tp_m, h->st.tp_p, h->st.tp_res, h->st.km_z1, h->st.km_z2, h->st.km_rms,
-                  h->st.km_peak, h->st.km_fall, h->st.km_cnt, h->st.km_fpp, h->st.km_flag, h->d_res, h->d_dbg, h->st.done_cnt, h->st.hist_alt, h->st.blk_max, h->st.grp_cnt, h->st.tmp, h->d_scr, h->st.sm_arr, h->d_tl, h->d_btc};
+                  h->st.km_peak, h->st.km_fall, h->st.km_cnt, h->st.km_fpp, h->st.km_flag, h->d_res, h->d_dbg, h->st.done_cnt, h->st.hist_alt, h->st.blk_max, h->st.grp_cnt, h->st.tmp, h->d_scr, h->st.sm_arr, h->d_tl, h->d_btc,
+                  h->d_hist};
     for (void* p : ps) cudaFree (p);
     if (h->sb) cudaStreamDestroy (h->sb);
     for (int i = 0; i < 2; ++i) { if (h->ev_fir[i]) cudaEventDestroy (h->ev_fir[i]); if (h->ev_bal[i]) cudaEventDestroy (h->ev_bal[i]); }
@@ -2606,7 +2776,12 @@ static int tpk_block (b200m_tpk* h, const float* in, size_t stride, uint32_t nfr
 {
     const uint32_t n = h ? h->n_chan : 0;
     return bank_call (h, in, stride, nfram, host, stream, n, n, len,
-                      [&] { return tp_mode > 1 ? set_err (B200M_E_INVAL, "bad tp_mode %u", tp_mode) : 0; },
+                      [&] {
+                          if (tp_mode > 1) return set_err (B200M_E_INVAL, "bad tp_mode %u", tp_mode);
+                          if (h->hist && tp_mode == B200M_TP_MODE_MAX)
+                              return set_err (B200M_E_UNSUPPORTED, "process_max does not count in the histogram plane (b200m_tpk_hist_enable)");
+                          return 0;
+                      },
                       [&] (const float* d_in, size_t ds, cudaStream_t st, const uint32_t* rlen) {
                           if (!rlen) { h->rag_read = false; return tpk_process (h, d_in, ds, nfram, tp_mode, st); }
                           const uint32_t* d_len = nullptr; const float* d_fall = nullptr;
@@ -2682,9 +2857,12 @@ int b200m_tpk_clear (b200m_tpk* h, int32_t chan, void* stream)
     // TruePeakdsp::init's pre-roll, truepeakdsp.cc:159-168).  For slot reuse in shared banks.
     if (!h || chan >= (int32_t)h->n_chan) return set_err (B200M_E_INVAL, "bad argument");
     DeviceGuard g (h->device);
-    tpk_reset_kernel<<<(h->n_chan + 127) / 128, 128, 0, h->path.stream (stream)>>> ((int)h->n_chan, chan, h->flags | 4u, h->st, nullptr, 0, 1);
+    cudaStream_t st = h->path.stream (stream);
+    tpk_reset_kernel<<<(h->n_chan + 127) / 128, 128, 0, st>>> ((int)h->n_chan, chan, h->flags | 4u, h->st, nullptr, 0, 1);
     B200M_LAUNCHED (1);
     B200M_CUDA (cudaGetLastError ());
+    if (h->hist)                                           // a cleared channel is a fresh meter for the histogram plane too
+        return tpk_hist_clear (h, chan < 0 ? 0 : chan, chan < 0 ? (int)h->n_chan : 1, st);
     return 0;
 }
 
@@ -2786,6 +2964,57 @@ int b200m_tpk_state (b200m_tpk* h, float* tp_m, float* tp_p, float* tp_z1, float
         free (tmp);
     }
     B200M_CUDA (cudaStreamSynchronize (st));
+    return 0;
+}
+
+int b200m_tpk_hist_enable (b200m_tpk* h, int enable, float tp_limit_db, float km_limit_db, void* stream)
+{
+    if (!h) return set_err (B200M_E_INVAL, "NULL handle");
+    if (isnan (tp_limit_db) || isnan (km_limit_db)) return set_err (B200M_E_INVAL, "the limits must not be NaN");
+    if (h->r128_owned) return set_err (B200M_E_UNSUPPORTED, "the true-peak bank of an EBUr128 bank runs process_max only: no histogram plane");
+    DeviceGuard g (h->device);
+    if (!enable) { h->hist = false; return 0; }           // the plane's memory stays for the next enable
+    cudaStream_t st = h->path.stream (stream);
+    if (!h->d_hist) {
+        const size_t tab = 2 * TPK_HIST_EDGES * sizeof (float);
+        const cudaError_t e = cudaMalloc (&h->d_hist, h->hist_read_bytes () + tab);
+        if (e != cudaSuccess) {
+            cudaGetLastError ();                               // a failed allocation is not sticky: later calls must not see it
+            h->d_hist = nullptr;
+            if (e == cudaErrorMemoryAllocation) return set_err (B200M_E_NOMEM, "true-peak / K-meter histogram of %u channels: out of device memory", h->n_chan);
+            return cuda_fail (e, "b200m_tpk_hist_enable", __FILE__, __LINE__);
+        }
+        // the needle plane's edges, and for the K-meter the least y = 2 z2 whose sqrtf reaches each edge (pageable: copied before return)
+        std::vector<float> t (2 * TPK_HIST_EDGES);
+        b200m_ppm_hist_edges (t.data ());
+        for (int k = 0; k < TPK_HIST_EDGES; ++k) t[TPK_HIST_EDGES + k] = tpk_sqrt_threshold (t[k]);
+        B200M_CUDA (cudaMemcpyAsync (h->hist_tab (), t.data (), tab, cudaMemcpyHostToDevice, st));
+    }
+    if (int rc = tpk_hist_clear (h, 0, (int)h->n_chan, st)) return rc;
+    h->hist_tp_lim = (float)pow (10.0, (double)tp_limit_db / 20.0);                    // +inf dB: no reading is over; -inf dB: L = 0
+    h->hist_km_thr = tpk_sqrt_threshold ((float)pow (10.0, (double)km_limit_db / 20.0));
+    h->hist = true;
+    return 0;
+}
+
+int b200m_tpk_hist_read (b200m_tpk* h, uint64_t* tp_counts, b200m_ppm_hist_stats* tp_stats, uint64_t* km_counts, b200m_ppm_hist_stats* km_stats,
+                         void* stream)
+{
+    if (!h) return set_err (B200M_E_INVAL, "NULL handle");
+    const bool tp = h->flags & B200M_TPK_TRUEPEAK, km = h->flags & B200M_TPK_KMETER;
+    if (tp != (tp_counts && tp_stats) || (!tp && (tp_counts || tp_stats)) || km != (km_counts && km_stats) || (!km && (km_counts || km_stats)))
+        return set_err (B200M_E_INVAL, "pass both arrays of each meter the bank has, and NULL for a meter it lacks");
+    if (!h->hist) return set_err (B200M_E_INVAL, "the histogram plane is off (b200m_tpk_hist_enable)");
+    DeviceGuard g (h->device);
+    cudaStream_t st = h->path.stream (stream);
+    std::vector<unsigned char> buf (h->hist_read_bytes ());
+    B200M_CUDA (cudaMemcpyAsync (buf.data (), h->d_hist, buf.size (), cudaMemcpyDeviceToHost, st));
+    B200M_CUDA (cudaStreamSynchronize (st));
+    const size_t nc = (size_t)h->n_chan * TPK_HIST_BINS * sizeof (uint64_t), ns = (size_t)h->n_chan * sizeof (b200m_ppm_hist_stats);
+    const unsigned char* s0 = buf.data () + h->hist_nm () * nc;
+    int q = 0;
+    if (tp) { memcpy (tp_counts, buf.data (), nc); memcpy (tp_stats, s0, ns); ++q; }
+    if (km) { memcpy (km_counts, buf.data () + q * nc, nc); memcpy (km_stats, s0 + q * ns, ns); }
     return 0;
 }
 

@@ -15,6 +15,8 @@ Album correlation distributions likewise: gather_results collects each rank's pe
 and correlation_albums pools them on the host.
 Album needle distributions too: gather_results collects each rank's per-clip hist and stats of programme_needle, and needle_albums
 pools them on the host; every album value is an integer sum or a maximum, so any split of the clips gives the same result.
+Album true-peak and K-meter distributions the same way: needle_albums pools each rank's per-clip tp_hist / tp_stats and km_hist /
+km_stats of programme_truepeak.
 """
 MIX_WORDS = 1508
 DR14_HISTBINS = 8000
