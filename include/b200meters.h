@@ -795,6 +795,28 @@ int b200m_pw_raw (b200m_pw* h, uint32_t inst, float* powL, float* powR, float* p
  * shared memory for the correlation recurrences and appended to the FFT ring from there.  Read the correlation with
  * b200m_cor_results; do not call b200m_cor_process_* on an attached bank.  cor = NULL detaches. */
 int b200m_pw_attach_cor (b200m_pw* h, b200m_cor* cor);
+/* Cross-spectrum plane (an extension; the reference keeps only the last analysis's spectra): with the plane on, every analysis of an
+ * instance adds, for every bin k = 0 .. fft_bins-1, four terms to its row sums[inst][term][k] (fp64):
+ *   B200M_PW_XSPEC_LL  |L_k|^2,   B200M_PW_XSPEC_RR  |R_k|^2,   B200M_PW_XSPEC_RL_RE  Re (R_k conj L_k),   B200M_PW_XSPEC_RL_IM  Im (R_k conj L_k)
+ * L_k, R_k: the fp32 spectra the analysis forms (gui/fft.c:163-180; bin fft_bins-1 as every other bin, though its ports read 0).
+ * Each term is formed in double from the fp32 parts (exact products, one rounding) and added in analysis order, so atan2 (RL_IM, RL_RE)
+ * has the phasewheel's sign, arg R - arg L (gui/phasewheel.c:1323-1325).  counts[inst][0] counts the analyses added.  An analysis with a
+ * non-finite Re / Im part in either spectrum adds nothing and counts in counts[inst][1] (skipped) instead; it does not depend on db_thresh.
+ * - Every analysis counts, not only the last of a call, whose spectra alone reach the ports: a firing of the 25 Hz clock before the
+ *   last one of a call runs a plane-only analysis.  With blocks of at most ceil (rate / 25) frames a call fires at most once and the
+ *   plane adds no launch.
+ * - Ports, peak, b200m_pw_raw and the stereoscope smoothing are bit-identical with the plane on or off, in both modes; with it off
+ *   the bank runs exactly the kernels it runs without it.
+ * - Ragged blocks add an instance's own analyses only; the fused correlation feed and ragged blocks accumulate exactly as unfused
+ *   and plain blocks do.  b200m_pw_set_mode, b200m_pw_debug_capture and b200m_pw_attach_cor leave the plane alone.
+ * enable != 0: allocates the plane on first use (B200M_E_NOMEM if the device cannot hold 32 fft_bins + 16 bytes per instance) and zeroes
+ * every row and count, also when it was on already; 0: stops accumulating and keeps the memory.  Ordered like the getters. */
+#define B200M_PW_XSPEC_TERMS 4
+enum { B200M_PW_XSPEC_LL = 0, B200M_PW_XSPEC_RR = 1, B200M_PW_XSPEC_RL_RE = 2, B200M_PW_XSPEC_RL_IM = 3 };
+int b200m_pw_xspec_enable (b200m_pw* h, int enable, void* stream);
+/* host sums [n_inst][4][fft_bins] and counts [n_inst][2] (analyses, skipped), in one copy and one synchronisation of the stream,
+ * ordered like b200m_pw_results.  B200M_E_INVAL while the plane has never been enabled. */
+int b200m_pw_xspec_read (b200m_pw* h, double* sums, uint64_t* counts, void* stream);
 /* device pointers of the result planes, for callers that keep the spectra on the GPU */
 int b200m_pw_device_results (b200m_pw* h, const float** d_phase, const float** d_level, const float** d_peak);
 

@@ -228,6 +228,8 @@ _PROTOS = {
     "b200m_pw_results": (C.c_int, [_v, _v, _v, _v, _v]),
     "b200m_pw_raw": (C.c_int, [_v, C.c_uint32, _v, _v, _v, _v, _v]),
     "b200m_pw_device_results": (C.c_int, [_v, C.POINTER(_v), C.POINTER(_v), C.POINTER(_v)]),
+    "b200m_pw_xspec_enable": (C.c_int, [_v, C.c_int, _v]),
+    "b200m_pw_xspec_read": (C.c_int, [_v, _v, _v, _v]),
 }
 EXPORTS = tuple(_PROTOS)
 
@@ -1028,6 +1030,10 @@ class Spectr30(_Bank):
         return s, c.astype(np.int64)
 
 
+# the terms of a cross-spectrum plane row, in order (B200M_PW_XSPEC_LL .. RL_IM): |L_k|^2, |R_k|^2, Re and Im (R_k conj L_k)
+PW_XSPEC_TERMS = ("ll", "rr", "rl_re", "rl_im")
+
+
 class Phasewheel(_Bank):
     """N x (2 x FFTAnalysis + phasewheel process_audio) (gui/fft.c:208-361, gui/phasewheel.c:1307-1342)."""
     _pfx = "pw"
@@ -1076,6 +1082,20 @@ class Phasewheel(_Bank):
         a = [np.empty(self.bins, np.float32) for _ in range(4)]
         _ck(lib().b200m_pw_raw(self.h, inst, *[_np_ptr(v) for v in a], _stream_ptr(stream)))
         return a
+
+    def xspec_enable(self, on=True, stream=None):
+        """the cross-spectrum plane (b200m_pw_xspec_enable): on, every analysis of every instance adds the PW_XSPEC_TERMS of each bin
+        to the instance's row, or counts itself skipped when a spectrum is not finite; (re)enabling zeroes every row and count, off
+        stops adding and keeps them"""
+        _ck(lib().b200m_pw_xspec_enable(self.h, int(bool(on)), _stream_ptr(stream)))
+
+    def xspec(self, stream=None):
+        """(sums float64 [n_inst, 4, fft_bins] in PW_XSPEC_TERMS order, analyses int64 [n_inst], skipped int64 [n_inst]) of the
+        cross-spectrum plane (b200m_pw_xspec_read); raises before the plane was first enabled"""
+        s = np.empty((self.n_inst, 4, self.bins), np.float64); c = np.empty((self.n_inst, 2), np.uint64)
+        _ck(lib().b200m_pw_xspec_read(self.h, _np_ptr(s), _np_ptr(c), _stream_ptr(stream)))
+        c = c.astype(np.int64)
+        return s, c[:, 0].copy(), c[:, 1].copy()
 
 
 class EBUr128(_Bank):
@@ -1594,6 +1614,134 @@ def programme_correlation(x, lengths, rate=48000.0, flp=2e3, tcf=0.3, gate_db=-7
     out.update(_cor_dist(hist, sums))
     if grp is not None:
         out.update(correlation_albums(hist, sums, grp))
+    return out
+
+
+def pw_window(fft_bins):
+    """the phasewheel bank's float32 Hann window of 2 fft_bins points, as b200m_pw_create builds it: .5 - .5 cos (2 pi i / (N - 1))
+    stored as float, then times 2 / (its sum in double), stored as float (gui/fft.c:69-79,122-161)"""
+    N = 2 * int(fft_bins)
+    w = (0.5 - 0.5 * np.cos(2.0 * np.pi / (N - 1.0) * np.arange(N))).astype(np.float32)
+    return (w.astype(np.float64) * (2.0 / w.astype(np.float64).sum())).astype(np.float32)
+
+
+def pw_enbw(fft_bins):
+    """the equivalent noise bandwidth of the bank's window in bins, N sum(w^2) / sum(w)^2 in float64 (about 1.5)"""
+    w = pw_window(fft_bins).astype(np.float64)
+    return w.size * float((w * w).sum()) / float(w.sum()) ** 2
+
+
+def _stereo_band_of_bin(rate, fft_bins):
+    """the 1/3-octave band (index into SPEC_BAND_HZ, -1 for none) of each bin k < fft_bins: lo <= k rate / (2 fft_bins) < hi with
+    lo, hi = centre * 2^(-+1/6); DC is in no band"""
+    f = np.arange(int(fft_bins)) * (float(rate) / (2.0 * int(fft_bins)))
+    lo, hi = SPEC_BAND_HZ * 2.0 ** (-1.0 / 6.0), SPEC_BAND_HZ * 2.0 ** (1.0 / 6.0)
+    band = np.full(f.size, -1, np.int64)
+    for b in range(SPEC_BAND_HZ.size):
+        band[(f >= lo[b]) & (f < hi[b])] = b
+    band[0] = -1
+    return band
+
+
+def stereo_bands(sums, analyses, rate, fft_bins):
+    """Band fields of cross-spectrum rows (sums float64 [N, 4, fft_bins] in PW_XSPEC_TERMS order, analyses [N]): a clip's or an
+    album's.  A band of SPEC_BAND_HZ holds the bins k with lo <= k rate / (2 fft_bins) < hi, lo, hi = centre * 2^(-+1/6) (DC is in
+    none); its sums LL, RR and C = RL_RE + i RL_IM are its bins' sums added in ascending k.  Returns a dict of:
+      band_level_db (float64 [N, 30, 2]): 10 log10 (LL / (analyses * enbw)) for L and the same with RR for R, enbw = pw_enbw (fft_bins):
+        a steady sine of amplitude a well inside the band reads 20 log10 a (programme_spectrum's ltas_db scale);
+      band_corr (Re C / sqrt (LL RR)), band_coherence (|C|^2 / (LL RR)), band_phase (atan2 (Im C, Re C), arg R - arg L);
+      band_balance_db (10 log10 (RR / LL));
+      band_mono_db (10 log10 ((LL + RR + 2 Re C) / (2 (LL + RR)))): the power of (L + R) / 2 against the mean channel power, 0 dB for
+        identical channels, about -3.01 dB for uncorrelated ones and -inf for exact anti-phase;
+    all float64 [N, 30].  NaN where a band has no bin or a denominator is 0 (band_phase: where C is 0), -inf where a log's argument is 0."""
+    sums = np.asarray(sums, np.float64); analyses = np.asarray(analyses, np.int64)
+    bins = int(fft_bins)
+    n = sums.shape[0] if sums.ndim == 3 else -1
+    if n < 0 or sums.shape != (n, 4, bins) or analyses.shape != (n,):
+        raise B200MError("sums and analyses must be [N, 4, %d] and [N] rows of the same N clips" % bins)
+    band = _stereo_band_of_bin(rate, bins)
+    nb = SPEC_BAND_HZ.size
+    acc = np.zeros((n, 4, nb))
+    for k in np.flatnonzero(band >= 0):                  # ascending k: a fixed order of the fp64 sums
+        acc[:, :, band[k]] += sums[:, :, k]
+    empty = np.bincount(band[band >= 0], minlength=nb) == 0
+    LL, RR, CR, CI = acc[:, 0], acc[:, 1], acc[:, 2], acc[:, 3]
+
+    def ratio(num, den):                                 # num / den, NaN where den is 0 or the band is empty
+        with np.errstate(invalid="ignore", divide="ignore"):
+            return np.where((den != 0) & ~empty, num / np.where(den != 0, den, 1.0), np.nan)
+
+    def db(r):                                           # 10 log10 r, -inf at 0 (and below: rounding of an exact 0), NaN stays
+        with np.errstate(invalid="ignore", divide="ignore"):
+            return np.where(r > 0, 10.0 * np.log10(np.where(r > 0, r, 1.0)), np.where(np.isnan(r), np.nan, -np.inf))
+    den = (analyses.astype(np.float64) * pw_enbw(bins))[:, None]
+    level = np.stack([db(ratio(LL, np.broadcast_to(den, LL.shape))), db(ratio(RR, np.broadcast_to(den, RR.shape)))], axis=-1)
+    with np.errstate(invalid="ignore"):
+        llrr = LL * RR
+        corr = ratio(CR, np.sqrt(llrr))
+    coh = ratio(CR * CR + CI * CI, llrr)
+    phase = np.where(empty | ((CR == 0) & (CI == 0)), np.nan, np.arctan2(CI, CR))
+    return dict(band_level_db=level, band_corr=corr, band_coherence=coh, band_phase=phase,
+                band_balance_db=db(ratio(RR, LL)), band_mono_db=db(ratio(LL + RR + 2.0 * CR, 2.0 * (LL + RR))))
+
+
+def stereo_albums(sums, analyses, skipped, groups, rate, fft_bins):
+    """Album cross-spectra from per-clip rows: programme_stereo's sums, analyses and skipped, or those of several banks (shards on
+    several GPUs) concatenated in clip order, e.g. with shard.gather_results.  groups: N album ids (>= 0, or -1 for a clip in no
+    album).  An album's sums are its members' sums added in ascending clip index and its counts the sum of theirs, so the result does
+    not depend on how the clips were split between banks.  Returns a dict for G = max(groups) + 1 albums: album_sums (float64
+    [G, 4, fft_bins]), album_analyses, album_skipped and album_n_clips (int64 [G]), and stereo_bands of the album rows with each
+    field prefixed album_ (album_band_corr, ...)."""
+    sums = np.asarray(sums, np.float64); analyses = np.asarray(analyses, np.int64); skipped = np.asarray(skipped, np.int64)
+    bins = int(fft_bins)
+    n = sums.shape[0] if sums.ndim == 3 else -1
+    if n < 0 or sums.shape != (n, 4, bins) or analyses.shape != (n,) or skipped.shape != (n,):
+        raise B200MError("sums, analyses and skipped must be [N, 4, %d], [N] and [N] rows of the same N clips" % bins)
+    grp = _groups(groups, n)
+    g = int(grp.max()) + 1 if n else 0
+    s, a, k = np.zeros((g, 4, bins)), np.zeros(g, np.int64), np.zeros(g, np.int64)
+    for i in np.flatnonzero(grp >= 0):                 # one clip at a time, in ascending index: a fixed order of the fp64 sums
+        s[grp[i]] += sums[i]
+        a[grp[i]] += analyses[i]
+        k[grp[i]] += skipped[i]
+    out = dict(album_sums=s, album_analyses=a, album_skipped=k,
+               album_n_clips=np.bincount(grp[grp >= 0], minlength=g).astype(np.int64))
+    out.update(("album_" + f, v) for f, v in stereo_bands(s, a, rate, bins).items())
+    return out
+
+
+def programme_stereo(x, lengths, rate=48000.0, fft_bins=2048, block=1024, device=0, groups=None):
+    """Stereo image by frequency band of N stereo clips of different lengths, in one phasewheel bank: per 1/3-octave band, the
+    correlation, coherence, phase, balance and the level lost in the mono downmix (stereo_bands) over the whole clip.
+
+    x: rows 2i, 2i + 1 = L, R of clip i, clip i valid for its first lengths[i] frames: a [2N, >= max(lengths)] float32 numpy array /
+    CPU tensor (host path) or CUDA tensor (device path), or a callable f(offset, nfram) that returns frames offset .. offset +
+    nfram - 1 of every row as such an array.  Frames past a clip's length are never read into a result.  The clips are fed in blocks
+    of `block` frames with clip i's length in block k clamp(lengths[i] - k * block, 0, block) (Phasewheel.process with lengths), so
+    clip i's sums, analyses and skipped are bit-identical to one Phasewheel(1, fft_bins, rate) fed only that clip in blocks of
+    `block` frames with the cross-spectrum plane on (Phasewheel.xspec_enable).
+    Coverage: an analysis takes the last 2 fft_bins frames of the clip, windowed, every ceil(rate / 25) frames of the clip's own clock,
+    starting from a zeroed ring (the first analyses see leading zeros).  When 2 fft_bins < ceil(rate / 25), as with fft_bins 2048 at
+    192 kHz, the frames between two windows are not analysed; a clip's tail after its last analysis is not analysed either.
+    Returns a dict: sums (float64 [N, 4, fft_bins], PW_XSPEC_TERMS), analyses and skipped (int64 [N]; an analysis with a non-finite
+    spectrum is skipped and adds nothing), bin_hz (float64 [fft_bins], k rate / (2 fft_bins)) and the stereo_bands fields ([N, 30]).
+    groups: None, or N album ids (>= 0, or -1 for a clip in no album): the dict then also holds stereo_albums(sums, analyses,
+    skipped, groups, rate, fft_bins)."""
+    ln, blocks = _programme_blocks(x, lengths, block, "no clips")
+    n = ln.size
+    grp = None if groups is None else _groups(groups, n)
+    bank = Phasewheel(n, fft_bins, rate, device)
+    try:
+        bank.xspec_enable()
+        for _, xb, lb in blocks:
+            bank.process(xb, lengths=lb)
+        sums, analyses, skipped = bank.xspec()
+    finally:
+        bank.close()
+    out = dict(sums=sums, analyses=analyses, skipped=skipped, bin_hz=np.arange(int(fft_bins)) * (float(rate) / (2.0 * int(fft_bins))))
+    out.update(stereo_bands(sums, analyses, rate, fft_bins))
+    if grp is not None:
+        out.update(stereo_albums(sums, analyses, skipped, grp, rate, fft_bins))
     return out
 
 

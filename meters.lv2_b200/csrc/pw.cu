@@ -106,19 +106,27 @@ B200M_DEV void stockham_pass (const float2* __restrict__ X, float2* __restrict__
 // half the shared memory of packing L + iR into one N-point transform, which is what lets N = 16384 (gui/phasewheel.c:1116)
 // fit: 2 x M complex ping-pong buffers + the left channel's power / phase = 12 N bytes.
 // RAG (ragged blocks): CTA b analyses instance fire[2 b] with the oldest sample at fire[2 b + 1], its own ring offset when it fired.
-template <bool RAG>
+// XS (the cross-spectrum plane, b200m_pw_xspec_enable): the analysis also adds |L_k|^2, |R_k|^2, Re and Im (R_k conj L_k) of every bin
+// k < bins to xs[inst][4][bins] (fp64, each term rounded once, __dadd_rn in analysis order) and counts itself in xcnt[inst][0], or
+// adds nothing and counts itself in xcnt[inst][1] when a Re / Im part of either spectrum is not finite.  ports = 0: a plane-only
+// analysis (a firing before the last one of a call), no raw, phase, level or peak writes; with RAG the entry's bit 31 says so.
+// The XS form keeps the left channel's Re / Im in sPL / sFL and recomputes its power and phase from them with the expressions that
+// formed them, so the ports get the same bits; the right channel's Re / Im go to the free ping-pong buffer.
+template <bool RAG, bool XS = false>
 __global__ void __launch_bounds__ (PW_THREADS)
 pw_analyze_kernel (const float* __restrict__ ring, int N, int f3, int f4, int f2, int start, const float* __restrict__ window,
                    const float2* __restrict__ tw, float db_thresh, float* __restrict__ rawp /* [inst][4][bins] or NULL */,
                    float* __restrict__ phase, float* __restrict__ level, float* __restrict__ peak, int mode,
-                   const uint32_t* __restrict__ fire)
+                   const uint32_t* __restrict__ fire, double* __restrict__ xs, unsigned long long* __restrict__ xcnt, int ports)
 {
-    extern __shared__ __align__ (16) float2 sm[];          // X, Y: M complex each; then powL[bins], phL[bins]
+    extern __shared__ __align__ (16) float2 sm[];          // X, Y: M complex each; then powL[bins], phL[bins] (XS: ReL[bins], ImL[bins])
     __shared__ float red[PW_THREADS / 32];
     const int M = N / 2, bins = N / 2;
     float2* bufA = sm; float2* bufB = sm + M;
     float* sPL = reinterpret_cast<float*> (sm + 2 * M); float* sFL = sPL + bins;
-    const int inst = RAG ? (int)fire[2 * blockIdx.x] : blockIdx.x, tid = threadIdx.x;
+    int inst = RAG ? (int)fire[2 * blockIdx.x] : blockIdx.x;
+    const int tid = threadIdx.x;
+    if (XS && RAG) { ports = inst >= 0; inst &= 0x7fffffff; }
     if (RAG) start = (int)fire[2 * blockIdx.x + 1];
     float pk = 0.0f;
     for (int ch = 0; ch < 2; ++ch) {
@@ -136,22 +144,42 @@ pw_analyze_kernel (const float* __restrict__ ring, int N, int f3, int f4, int f2
         for (int i = 0; i < f4; ++i) { stockham_pass<4> (X, Y, tw, M, n, s3, sh, tid); __syncthreads (); float2* T = X; X = Y; Y = T; n /= 4; sh += 2; }
         for (int i = 0; i < f2; ++i) { stockham_pass<2> (X, Y, tw, M, n, s3, sh, tid); __syncthreads (); float2* T = X; X = Y; Y = T; n /= 2; sh += 1; }
         // ft_analyze (gui/fft.c:163-180) for this channel, then (right channel) process_audio (gui/phasewheel.c:1313-1331)
-        float* rp = rawp ? rawp + (size_t)inst * 4 * bins : nullptr;
+        float* rp = rawp && (!XS || ports) ? rawp + (size_t)inst * 4 * bins : nullptr;
+        // XS: the left channel's phase is recomputed in the right channel's pass, so a phase is formed here only for raw or the ports
+        const bool want_ph = XS ? (rp || (ch == 1 && mode == 0 && ports)) : (mode == 0 || rp);
+        int bad = 0;                                         // XS: a non-finite Re / Im part in this thread's bins
         for (int k = tid; k < bins; k += PW_THREADS) {
-            float pw_, ph_;
-            if (k == 0) { const float x0 = X[0].x + X[0].y; pw_ = x0 * x0; ph_ = 0.0f; }          // power[0] = out[0]^2, phase[0] = 0
-            else if (k == bins - 1) { pw_ = 0.0f; ph_ = 0.0f; }                                   // never written by ft_analyze (i < data_size - 1): stays as fftx_reset left it
+            float pw_, ph_, xre = 0.0f, xim = 0.0f;
+            if (k == 0) { const float x0 = X[0].x + X[0].y; pw_ = x0 * x0; ph_ = 0.0f; if (XS) xre = x0; }   // power[0] = out[0]^2, phase[0] = 0
+            else if (!XS && k == bins - 1) { pw_ = 0.0f; ph_ = 0.0f; }                            // never written by ft_analyze (i < data_size - 1): stays as fftx_reset left it
             else {
                 const float2 A = X[k], Bm = X[M - k], w = tw[k];
                 const float er = 0.5f * (A.x + Bm.x), ei = 0.5f * (A.y - Bm.y);
                 const float orr = 0.5f * (A.y + Bm.y), oi = -0.5f * (A.x - Bm.x);
                 const float re = er + fmaf (w.x, orr, -w.y * oi), im = ei + fmaf (w.x, oi, w.y * orr);
-                pw_ = fmaf (re, re, im * im);
-                ph_ = (mode == 0 || rp) ? atan2f (im, re) : 0.0f;            // the stereoscope's process_audio never reads ft->phase
+                if (XS) { xre = re; xim = im; }
+                if (XS && k == bins - 1) { pw_ = 0.0f; ph_ = 0.0f; }                              // the plane takes this bin, the ports do not
+                else {
+                    pw_ = fmaf (re, re, im * im);
+                    ph_ = want_ph ? atan2f (im, re) : 0.0f;           // the stereoscope's process_audio never reads ft->phase
+                }
             }
             if (rp) { rp[ch * bins + k] = pw_; rp[(2 + ch) * bins + k] = ph_; }
-            if (ch == 0) { sPL[k] = pw_; sFL[k] = ph_; continue; }
-            const float pl = sPL[k], fl = sFL[k], pr = pw_, fr = ph_;
+            if (ch == 0) {
+                if (XS) { sPL[k] = xre; sFL[k] = xim; }
+                else { sPL[k] = pw_; sFL[k] = ph_; }
+                continue;
+            }
+            float pl, fl;
+            if (XS) {
+                const float lre = sPL[k], lim = sFL[k];
+                bad |= !(finitef_ (lre) && finitef_ (lim) && finitef_ (xre) && finitef_ (xim));
+                Y[k] = make_float2 (xre, xim);                   // Y is free once the transform sits in X
+                if (!ports || k < 1 || k >= bins - 1) continue;
+                pl = fmaf (lre, lre, lim * lim);
+                fl = mode == 0 ? atan2f (lim, lre) : 0.0f;
+            } else { pl = sPL[k]; fl = sFL[k]; }
+            const float pr = pw_, fr = ph_;
             if (k < 1 || k >= bins - 1) continue;
             if (mode == 1) {
                 // stereoscope process_audio (gui/stereoscope.c:713-739): phase[] holds ui->lr[], both outputs are smoothed state
@@ -173,13 +201,28 @@ pw_analyze_kernel (const float* __restrict__ ring, int N, int f3, int f4, int f2
                 level[(size_t)inst * bins + k] = lv;
             }
         }
+        if (XS && ch == 1) {
+            // one CTA owns the instance's row in a launch and launches are stream-ordered: plain read-modify-writes
+            const bool skip = __syncthreads_or (bad);
+            if (!skip) {
+                double* row = xs + (size_t)inst * 4 * bins;
+                for (int k = tid; k < bins; k += PW_THREADS) {
+                    const double lr = sPL[k], li = sFL[k], rr = Y[k].x, ri = Y[k].y;    // exact products in double, each term rounded once
+                    row[k]            = __dadd_rn (row[k],            __dadd_rn (__dmul_rn (lr, lr), __dmul_rn (li, li)));
+                    row[bins + k]     = __dadd_rn (row[bins + k],     __dadd_rn (__dmul_rn (rr, rr), __dmul_rn (ri, ri)));
+                    row[2 * bins + k] = __dadd_rn (row[2 * bins + k], __dadd_rn (__dmul_rn (rr, lr), __dmul_rn (ri, li)));
+                    row[3 * bins + k] = __dadd_rn (row[3 * bins + k], __dsub_rn (__dmul_rn (ri, lr), __dmul_rn (rr, li)));
+                }
+            }
+            if (tid == 0) ++xcnt[2 * inst + (skip ? 1 : 0)];
+        }
         __syncthreads ();                                    // the buffers are reused by the right channel
     }
 #pragma unroll
     for (int o = 16; o; o >>= 1) pk = fmaxf (pk, __shfl_xor_sync (0xffffffffu, pk, o));
     if ((tid & 31) == 0) red[tid >> 5] = pk;
     __syncthreads ();
-    if (tid == 0 && mode == 0) {
+    if (tid == 0 && mode == 0 && (!XS || ports)) {
         for (int i = 1; i < PW_THREADS / 32; ++i) pk = fmaxf (pk, red[i]);
         // ui->peak += .04 * (peak - ui->peak) + 1e-15;  (double arithmetic on a float lvalue, :1333-1335)
         float up = peak[inst];
@@ -216,20 +259,45 @@ struct b200m_pw {
     uint32_t rboff, smps, sps, step;                       // shared ring offset + 25 Hz analysis clock (gui/fft.c:43-64)
     // each instance's ring offset and clock once ragged blocks have moved them apart; empty while every instance agrees (rboff, smps)
     std::vector<uint32_t> rb, sm;
-    // ragged-block scratch: every length nfram (a plain block once the clocks differ), each instance's last firing step, the
-    // firing instances per step; and the upload of rb[n] | len[n] | (instance, ring start) of the firing instances by step
-    std::vector<uint32_t> full, off; std::vector<int> fire;
+    // ragged-block scratch: every length nfram (a plain block once the clocks differ), the (instance word, step) of each analysis,
+    // the analyses per step; and the upload of rb[n] | len[n] | (instance word, ring start) of the analyses by step
+    std::vector<uint32_t> full, off, fire;
     RaggedLen rag;
     int mode = 0;                                          // 0: phasewheel process_audio, 1: stereoscope process_audio
     float *d_ring = nullptr, *d_win = nullptr, *d_raw = nullptr, *d_phase = nullptr, *d_level = nullptr, *d_peak = nullptr;
     float2* d_tw = nullptr;
     b200m_cor* cor = nullptr;                              // attached correlation bank (fused feed), not owned
     BankPath path;
+    // the cross-spectrum plane (b200m_pw_xspec_enable): [n_inst][4][bins] fp64 sums, then [n_inst][2] counts (analyses, skipped), in
+    // one allocation that stays once made; xs: the plane is on
+    double* d_xs = nullptr;
+    bool xs = false;
+    unsigned long long* xs_cnt () const { return (unsigned long long*)(d_xs + (size_t)n_inst * 4 * bins); }
+    size_t xs_bytes () const { return (size_t)n_inst * (4 * bins * sizeof (double) + 2 * sizeof (unsigned long long)); }
+    // the ragged upload's words: rb | len | one (instance, ring start) pair per analysis, the last of each instance's call only, or
+    // with the plane allocated every firing, at most one per step of N frames
+    size_t rag_words () const { return d_xs ? (size_t)2 * n_inst * (1 + (B200M_MAX_BLOCK + N - 1) / N) : (size_t)4 * n_inst; }
 };
 
 // the host path of a phasewheel bank runs on its attached correlation bank's own stream, if it has one (cor_host_stream)
 static cudaStream_t pw_stream (b200m_pw* h, void* stream) { return h->path.last_host ? cor_host_stream (h->cor, h->path.own) : (cudaStream_t)stream; }
 static size_t pw_smem_bytes (uint32_t N) { return (size_t)12 * N; }   // 2 x N/2 float2 + 2 x N/2 float
+
+// one analysis launch of c CTAs: fire = NULL (lock step, every instance, ports: the call's last firing) or the ragged entries
+static void pw_analyze (b200m_pw* h, unsigned c, int start, float db_thresh, const uint32_t* fire, int ports, cudaStream_t st)
+{
+    const size_t smem = pw_smem_bytes (h->N);
+    if (h->xs) {
+        const auto k = fire ? pw_analyze_kernel<true, true> : pw_analyze_kernel<false, true>;
+        k<<<c, PW_THREADS, smem, st>>> (h->d_ring, (int)h->N, h->f3, h->f4, h->f2, start, h->d_win, h->d_tw, db_thresh, h->d_raw, h->d_phase,
+                                        h->d_level, h->d_peak, h->mode, fire, h->d_xs, h->xs_cnt (), ports);
+    } else {
+        const auto k = fire ? pw_analyze_kernel<true> : pw_analyze_kernel<false>;
+        k<<<c, PW_THREADS, smem, st>>> (h->d_ring, (int)h->N, h->f3, h->f4, h->f2, start, h->d_win, h->d_tw, db_thresh, h->d_raw, h->d_phase,
+                                        h->d_level, h->d_peak, h->mode, fire, nullptr, nullptr, 1);
+    }
+    B200M_LAUNCHED (1);
+}
 
 // a plain block while every instance shares one ring offset and clock
 static int pw_lockstep (b200m_pw* h, const float* d_in, size_t stride, uint32_t nfram, float db_thresh, int* fired, cudaStream_t st)
@@ -237,7 +305,7 @@ static int pw_lockstep (b200m_pw* h, const float* d_in, size_t stride, uint32_t 
     // fftx_run walks the block in steps of at most window_size (gui/fft.c:346-360) and process_audio runs ONCE
     // after both channels' fftx_run (gui/phasewheel.c:1310-1313): when several analyses fire inside one call only
     // the last one's spectra survive, so only that one is launched (its ring state is the one at its firing time
-    // because launches execute in stream order).
+    // because launches execute in stream order).  With the cross-spectrum plane on, every earlier firing runs a plane-only analysis.
     int any = 0, last_fire = -1;
     {
         uint32_t sm = h->smps, d = 0; int step = 0;
@@ -262,12 +330,7 @@ static int pw_lockstep (b200m_pw* h, const float* d_in, size_t stride, uint32_t 
         h->smps += n;
         if (h->smps >= h->sps) {                            // :308-313
             h->step = h->smps; h->smps = 0;
-            if (step == last_fire) {
-                pw_analyze_kernel<false><<<h->n_inst, PW_THREADS, pw_smem_bytes (h->N), st>>> (
-                    h->d_ring, (int)h->N, h->f3, h->f4, h->f2, (int)h->rboff, h->d_win, h->d_tw, db_thresh, h->d_raw, h->d_phase, h->d_level, h->d_peak, h->mode,
-                    nullptr);
-                B200M_LAUNCHED (1);
-            }
+            if (step == last_fire || h->xs) pw_analyze (h, h->n_inst, (int)h->rboff, db_thresh, nullptr, step == last_fire, st);
             any = 1;
         }
         done += n; ++step;
@@ -282,40 +345,46 @@ static int pw_lockstep (b200m_pw* h, const float* d_in, size_t stride, uint32_t 
 // Each instance's block is walked in steps of N frames as fftx_run walks it (gui/fft.c:346-360): step s covers its frames
 // [s N, min (len[i], (s + 1) N)).  Per step, one append kernel, then one analysis of the instances whose LAST firing in this call
 // falls in that step (process_audio runs once per call, after fftx_run: gui/phasewheel.c:1310-1313); stream order gives each
-// analysis its ring as it stood when that instance fired.
+// analysis its ring as it stood when that instance fired.  With the cross-spectrum plane on, every firing of an instance is analysed
+// at its step, and all but the last of the call are plane-only (bit 31 of the entry's instance word).
 static int pw_ragged (b200m_pw* h, const float* d_in, size_t stride, uint32_t nfram, const uint32_t* len, bool plain, float db_thresh,
                       int* fired, cudaStream_t st)
 {
     const uint32_t n = h->n_inst, N = h->N;
     if (h->rb.empty ()) { h->rb.assign (n, h->rboff); h->sm.assign (n, h->smps); }
     uint32_t maxlen = 0, nfire = 0;
-    h->fire.assign (n, -1);
+    for (uint32_t i = 0; i < n; ++i) maxlen = std::max (maxlen, len[i]);
+    const uint32_t nsteps = (maxlen + N - 1) / N;
+    // the analyses by step: (instance | plane-only bit, step) pairs, counted per step in off[]
+    h->off.assign (nsteps + 1, 0);
+    h->fire.clear ();
     for (uint32_t i = 0; i < n; ++i) {                     // the host mirror of _fftx_run's clock (gui/fft.c:308-313)
         uint32_t smps = h->sm[i], s = 0;
+        int last = -1;
         for (uint32_t d = 0; d < len[i]; d += N, ++s) {
             smps += std::min (N, len[i] - d);
-            if (smps >= h->sps) { smps = 0; h->fire[i] = (int)s; }
+            if (smps >= h->sps) {
+                smps = 0;
+                if (h->xs && last >= 0) { h->fire.push_back (i | 0x80000000u); h->fire.push_back ((uint32_t)last); ++h->off[last + 1]; }
+                last = (int)s;
+            }
         }
         h->sm[i] = smps;
-        maxlen = std::max (maxlen, len[i]);
-        nfire += h->fire[i] >= 0;
+        if (last >= 0) { h->fire.push_back (i); h->fire.push_back ((uint32_t)last); ++h->off[last + 1]; }
     }
-    const uint32_t nsteps = (maxlen + N - 1) / N;
+    nfire = (uint32_t)(h->fire.size () / 2);
     // upload rb[n] | len[n] | (instance, ring start at its firing) pairs, grouped by firing step (counting sort)
     cudaError_t e = cudaSuccess;
-    uint32_t* w = h->rag.stage ((size_t)4 * n, &e);
+    uint32_t* w = h->rag.stage (h->rag_words (), &e);
     if (!w) return cuda_fail (e, "pw_ragged", __FILE__, __LINE__);
     memcpy (w, h->rb.data (), n * sizeof (uint32_t));
     memcpy (w + n, len, n * sizeof (uint32_t));
-    h->off.assign (nsteps + 1, 0);
-    for (uint32_t i = 0; i < n; ++i) if (h->fire[i] >= 0) ++h->off[h->fire[i] + 1];
     for (uint32_t s = 0; s < nsteps; ++s) h->off[s + 1] += h->off[s];
     {
         std::vector<uint32_t> cur (h->off.begin (), h->off.end () - 1);
-        for (uint32_t i = 0; i < n; ++i) {
-            if (h->fire[i] < 0) continue;
-            const uint32_t f = (uint32_t)h->fire[i], k = cur[f]++;
-            w[2 * n + 2 * k] = i;
+        for (uint32_t q = 0; q < nfire; ++q) {
+            const uint32_t iw = h->fire[2 * q], i = iw & 0x7fffffffu, f = h->fire[2 * q + 1], k = cur[f]++;
+            w[2 * n + 2 * k] = iw;
             w[2 * n + 2 * k + 1] = (h->rb[i] + std::min (N, len[i] - f * N)) % N;          // its ring offset after step f
         }
     }
@@ -331,12 +400,7 @@ static int pw_ragged (b200m_pw* h, const float* d_in, size_t stride, uint32_t nf
         pw_ragged_append_kernel<<<(unsigned)((total + 255) / 256), 256, 0, st>>> (d_in, stride, (int)n, (int)cmax, (int)(s * N), (int)N, h->rag.d,
                                                                                    h->rag.d + n, h->d_ring);
         B200M_LAUNCHED (1);
-        if (const uint32_t c = h->off[s + 1] - h->off[s]) {
-            pw_analyze_kernel<true><<<c, PW_THREADS, pw_smem_bytes (N), st>>> (
-                h->d_ring, (int)N, h->f3, h->f4, h->f2, 0, h->d_win, h->d_tw, db_thresh, h->d_raw, h->d_phase, h->d_level, h->d_peak, h->mode,
-                h->rag.d + 2 * n + 2 * h->off[s]);
-            B200M_LAUNCHED (1);
-        }
+        if (const uint32_t c = h->off[s + 1] - h->off[s]) pw_analyze (h, c, 0, db_thresh, h->rag.d + 2 * n + 2 * h->off[s], 1, st);
     }
     bool agree = true;
     for (uint32_t i = 0; i < n; ++i) {
@@ -422,6 +486,8 @@ int b200m_pw_create (b200m_pw** out, int device, uint32_t n_inst, uint32_t fft_b
     free (win); free (tw);
     if (e == cudaSuccess) e = cudaFuncSetAttribute (pw_analyze_kernel<false>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)pw_smem_bytes (16384));
     if (e == cudaSuccess) e = cudaFuncSetAttribute (pw_analyze_kernel<true>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)pw_smem_bytes (16384));
+    if (e == cudaSuccess) e = cudaFuncSetAttribute (pw_analyze_kernel<false, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)pw_smem_bytes (16384));
+    if (e == cudaSuccess) e = cudaFuncSetAttribute (pw_analyze_kernel<true, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)pw_smem_bytes (16384));
     if (e == cudaSuccess) e = cudaStreamCreateWithFlags (&h->path.own, cudaStreamNonBlocking);
     if (e == cudaSuccess) {
         const size_t n = (size_t)n_inst * fft_bins;       // ui->level[i] = -100, ui->phase[i] = 0 (phasewheel.c:199-202)
@@ -440,6 +506,7 @@ int b200m_pw_destroy (b200m_pw* h)
     DeviceGuard g (h->device);
     cudaDeviceSynchronize ();
     cudaFree (h->d_ring); cudaFree (h->d_win); cudaFree (h->d_tw); cudaFree (h->d_raw); cudaFree (h->d_phase); cudaFree (h->d_level); cudaFree (h->d_peak);
+    cudaFree (h->d_xs);
     h->rag.release (); h->path.release ();
     delete h;
     return 0;
@@ -533,6 +600,43 @@ int b200m_pw_raw (b200m_pw* h, uint32_t inst, float* powL, float* powR, float* p
     for (int q = 0; q < 4; ++q)
         if (dst[q]) B200M_CUDA (cudaMemcpyAsync (dst[q], h->d_raw + ((size_t)inst * 4 + q) * h->bins, h->bins * sizeof (float), cudaMemcpyDeviceToHost, st));
     B200M_CUDA (cudaStreamSynchronize (st));
+    return 0;
+}
+
+int b200m_pw_xspec_enable (b200m_pw* h, int enable, void* stream)
+{
+    if (!h) return set_err (B200M_E_INVAL, "NULL handle");
+    DeviceGuard g (h->device);
+    if (!enable) { h->xs = false; return 0; }              // the plane's memory stays for the next enable
+    if (!h->d_xs) {
+        // the ragged upload grows to one entry per firing: its buffers are made again at the next ragged call
+        B200M_CUDA (cudaDeviceSynchronize ());
+        h->rag.release ();
+        const cudaError_t e = cudaMalloc ((void**)&h->d_xs, h->xs_bytes ());
+        if (e != cudaSuccess) {
+            cudaGetLastError ();                               // a failed allocation is not sticky: later calls must not see it
+            h->d_xs = nullptr;
+            if (e == cudaErrorMemoryAllocation) return set_err (B200M_E_NOMEM, "cross-spectrum plane of %u instances: out of device memory", h->n_inst);
+            return cuda_fail (e, "b200m_pw_xspec_enable", __FILE__, __LINE__);
+        }
+    }
+    B200M_CUDA (cudaMemsetAsync (h->d_xs, 0, h->xs_bytes (), pw_stream (h, stream)));
+    h->xs = true;
+    return 0;
+}
+
+int b200m_pw_xspec_read (b200m_pw* h, double* sums, uint64_t* counts, void* stream)
+{
+    if (!h || !sums || !counts) return set_err (B200M_E_INVAL, "NULL argument");
+    if (!h->d_xs) return set_err (B200M_E_INVAL, "the cross-spectrum plane was never enabled (b200m_pw_xspec_enable)");
+    DeviceGuard g (h->device);
+    cudaStream_t st = pw_stream (h, stream);
+    const size_t ns = (size_t)h->n_inst * 4 * h->bins;
+    std::vector<double> buf (ns + 2 * (size_t)h->n_inst);   // sums, then the counts' bits
+    B200M_CUDA (cudaMemcpyAsync (buf.data (), h->d_xs, h->xs_bytes (), cudaMemcpyDeviceToHost, st));
+    B200M_CUDA (cudaStreamSynchronize (st));
+    memcpy (sums, buf.data (), ns * sizeof (double));
+    memcpy (counts, buf.data () + ns, 2 * (size_t)h->n_inst * sizeof (uint64_t));
     return 0;
 }
 

@@ -17,6 +17,8 @@ Album needle distributions too: gather_results collects each rank's per-clip his
 pools them on the host; every album value is an integer sum or a maximum, so any split of the clips gives the same result.
 Album true-peak and K-meter distributions the same way: needle_albums pools each rank's per-clip tp_hist / tp_stats and km_hist /
 km_stats of programme_truepeak.
+Album stereo images too (gather_results + stereo_albums, no exchange): stereo_albums pools each rank's per-clip sums, analyses and
+skipped of programme_stereo on the host.
 """
 MIX_WORDS = 1508
 DR14_HISTBINS = 8000
