@@ -10,7 +10,8 @@
  *  - every function returns 0 on success or a negative B200M_E_* code; nothing throws.
  *  - audio is planar float32, exactly what an LV2 host connects to an audio port
  *    (src/meters.cc:257-296): channel k (k = inst*nchan + c) of a process call starts at
- *    in + k*stride and holds nfram samples.  `*_process_device` takes a device pointer and is
+ *    in + k*stride and holds nfram samples (interleaved integer PCM converts to it on the device:
+ *    b200m_pcm_planar_device).  `*_process_device` takes a device pointer and is
  *    asynchronous on `stream` (a cudaStream_t, NULL = legacy default stream);
  *    `*_process_host` takes a host pointer (pinned memory recommended: b200m_host_alloc),
  *    performs the host->device copy itself and is asynchronous on the bank's own stream.
@@ -819,6 +820,26 @@ int b200m_pw_xspec_enable (b200m_pw* h, int enable, void* stream);
 int b200m_pw_xspec_read (b200m_pw* h, double* sums, uint64_t* counts, void* stream);
 /* device pointers of the result planes, for callers that keep the spectra on the GPU */
 int b200m_pw_device_results (b200m_pw* h, const float** d_phase, const float** d_level, const float** d_peak);
+
+/* ======================================================================================
+ * PCM input: interleaved integer or float PCM, as a file decodes (frames [t][c], little-endian), to the planar float32 rows every
+ * bank reads, on the device.  Clip i of n_clips starts at in + i * in_stride (bytes) and holds nfram frames of nchan samples; out row
+ * k = i * nchan + c (at out + k * out_stride floats), frame t, is the sample at in + i * in_stride + (t * nchan + c) * bps, scaled by
+ * 2^-(bits - 1), the normalised float read of integer PCM (-full scale reads -1.0):
+ *   B200M_PCM_S16  2 bytes   (float) x * 2^-15, exact
+ *   B200M_PCM_S24  3 bytes   packed, sign-extended 24-bit x, (float) x * 2^-23, exact
+ *   B200M_PCM_S32  4 bytes   x rounded to the nearest float (ties to even), times 2^-31 (exact): INT32_MAX reads 1.0f
+ *   B200M_PCM_F32  4 bytes   a bit copy: NaN payloads, +-Inf, -0 and denormals kept
+ * One launch, asynchronous on `stream`; in and out must not overlap.  in and in_stride must be multiples of the sample size (any
+ * byte for S24, so a WAV data chunk can be converted where it lies).  B200M_E_INVAL, with nothing enqueued: a NULL pointer, an
+ * unknown format, n_clips == 0, nchan outside 1..B200M_PCM_MAX_CHANNELS, nfram outside 1..B200M_MAX_BLOCK, in_stride < nfram *
+ * nchan * bps, a misaligned in or in_stride, out_stride < nfram.  No CUDA device: B200M_E_NODEVICE.  A host caller uploads the raw
+ * bytes itself (pinned memory: b200m_host_alloc) and converts them here.
+ * ====================================================================================== */
+enum { B200M_PCM_S16 = 0, B200M_PCM_S24 = 1, B200M_PCM_S32 = 2, B200M_PCM_F32 = 3 };
+#define B200M_PCM_MAX_CHANNELS 32u   /* the widest instance any bank meters: the weighted EBUr128 bank */
+int b200m_pcm_planar_device (int device, const void* in, int format, uint32_t n_clips, uint32_t nchan, uint32_t nfram,
+                             size_t in_stride, float* out, size_t out_stride, void* stream);
 
 /* ======================================================================================
  * LV2 facade: the library also exports `lv2_descriptor (index)` (the one symbol of the reference's meters.so,

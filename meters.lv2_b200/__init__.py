@@ -230,6 +230,8 @@ _PROTOS = {
     "b200m_pw_device_results": (C.c_int, [_v, C.POINTER(_v), C.POINTER(_v), C.POINTER(_v)]),
     "b200m_pw_xspec_enable": (C.c_int, [_v, C.c_int, _v]),
     "b200m_pw_xspec_read": (C.c_int, [_v, _v, _v, _v]),
+    # PCM input
+    "b200m_pcm_planar_device": (C.c_int, [C.c_int, _v, C.c_int, C.c_uint32, C.c_uint32, C.c_uint32, C.c_size_t, _v, C.c_size_t, _v]),
 }
 EXPORTS = tuple(_PROTOS)
 
@@ -1942,3 +1944,142 @@ def programme_truepeak(x, lengths, rate=48000.0, nchan=2, flags=TPK_TRUEPEAK | T
         out["km_rms"] = st["km"][:, 2].astype(np.float32).reshape(n, per)
         out["km_peak"] = st["km"][:, 3].astype(np.float32).reshape(n, per)
     return out
+
+
+# ---------------------------------------------------------------------------------------------------- PCM input
+PCM_S16, PCM_S24, PCM_S32, PCM_F32 = 0, 1, 2, 3     # B200M_PCM_*
+PCM_MAX_CHANNELS = 32                               # B200M_PCM_MAX_CHANNELS
+PCM_BYTES = (2, 3, 4, 4)                            # bytes per sample of each format
+_PCM_DTYPE = {np.dtype(np.int16): PCM_S16, np.dtype(np.int32): PCM_S32, np.dtype(np.float32): PCM_F32}
+
+
+def _pcm_check(fmt, nchan):
+    if fmt not in (PCM_S16, PCM_S24, PCM_S32, PCM_F32):
+        raise B200MError("unknown PCM format %d" % fmt)
+    if not 1 <= nchan <= PCM_MAX_CHANNELS:
+        raise B200MError("nchan %d outside 1..%d" % (nchan, PCM_MAX_CHANNELS))
+
+
+def _pcm_layout(a, fmt=None, nchan=None):
+    """(fmt, nchan) of a numpy PCM array: int16 / int32 / float32 [N, T, nchan] (PCM_S16 / S32 / F32) or uint8 [N, T, nchan, 3]
+    (PCM_S24, packed little-endian); B200MError if it is neither, or if it disagrees with a given fmt or nchan"""
+    if not isinstance(a, np.ndarray):
+        raise B200MError("PCM data must be a numpy array, not %s" % type(a).__name__)
+    if a.dtype == np.uint8 and a.ndim == 4 and a.shape[3] == 3:
+        f = PCM_S24
+    elif a.dtype in _PCM_DTYPE and a.ndim == 3:
+        f = _PCM_DTYPE[a.dtype]
+    else:
+        raise B200MError("PCM data must be int16, int32 or float32 [N, T, nchan], or uint8 [N, T, nchan, 3] for packed 24-bit; "
+                         "got %s %s" % (a.dtype, a.shape))
+    if fmt is not None and int(fmt) != f:
+        raise B200MError("PCM format %s does not match %s data" % (fmt, a.dtype))
+    if nchan is not None and int(nchan) != a.shape[2]:
+        raise B200MError("nchan %s does not match data of %d channels" % (nchan, a.shape[2]))
+    _pcm_check(f, a.shape[2])
+    if a.shape[0] == 0:
+        raise B200MError("no clips")
+    return f, a.shape[2]
+
+
+def pcm_planar(pcm, fmt, nchan, nfram=None, stream=None):
+    """Interleaved PCM already on the device to the planar float32 rows every bank reads (b200m_pcm_planar_device, one launch).
+
+    pcm: a CUDA tensor [N, ...] of N clips, each clip's bytes contiguous (any dtype: the bytes are read as `fmt`; a uint8 [N, bytes]
+    view of uploaded WAV data chunks works as it lies), holding frames [t][c] of nchan samples of PCM_S16 (int16), PCM_S24 (packed
+    24-bit), PCM_S32 (int32) or PCM_F32 (float32).  nfram: the frames to convert from the start of each clip (default: all it holds).
+    Returns a float32 CUDA tensor [N * nchan, nfram], row i * nchan + c = channel c of clip i scaled by 2^-(bits - 1) (PCM_F32 bit for
+    bit), with a row pitch of a multiple of 64 floats.  Runs on `stream` (default: torch's current stream of pcm's device)."""
+    import torch
+    fmt, nchan = int(fmt), int(nchan)
+    if not (isinstance(pcm, torch.Tensor) and pcm.is_cuda and pcm.dim() >= 1 and pcm.shape[0] > 0 and pcm[0].is_contiguous()):
+        raise B200MError("pcm must be a CUDA tensor [N, ...] of N >= 1 clips, each clip's samples contiguous")
+    _pcm_check(fmt, nchan)
+    n, es = pcm.shape[0], pcm.element_size()
+    clip_bytes = pcm[0].numel() * es
+    in_stride = pcm.stride(0) * es if n > 1 else clip_bytes
+    nfram = clip_bytes // (nchan * PCM_BYTES[fmt]) if nfram is None else int(nfram)
+    if not 1 <= nfram <= MAX_BLOCK:
+        raise B200MError("nfram %d outside 1..%d" % (nfram, MAX_BLOCK))
+    if nfram * nchan * PCM_BYTES[fmt] > clip_bytes:
+        raise B200MError("%d frames of %d channels reach past the clip's %d bytes" % (nfram, nchan, clip_bytes))
+    pitch = (nfram + 63) & ~63
+    out = torch.empty((n * nchan, pitch), dtype=torch.float32, device=pcm.device)
+    st = C.c_void_p(torch.cuda.current_stream(pcm.device).cuda_stream) if stream is None else _stream_ptr(stream)
+    _ck(lib().b200m_pcm_planar_device(pcm.device.index, C.c_void_p(pcm.data_ptr()), fmt, n, nchan, nfram, in_stride,
+                                      C.c_void_p(out.data_ptr()), pitch, st))
+    return out[:, :nfram]
+
+
+class _PcmSource:
+    """pcm_source's callable: block (offset, nfram) of the source through one of two pinned slots to the device, then pcm_planar"""
+
+    def __init__(self, data, fmt, nchan, device):
+        self.data, self.fmt, self.nchan, self.device = data, fmt, nchan, device
+        self.n = None if callable(data) else data.shape[0]
+        self.slots = [None, None]           # pinned uint8 buffers from host_alloc, allocated with the first block
+        self.events = [None, None]          # recorded behind each slot's last copy
+        self.next = 0
+
+    def _block(self, offset, nfram):
+        if callable(self.data):
+            blk = self.data(offset, nfram)
+            _pcm_layout(blk, self.fmt, self.nchan)
+            if self.n is None:
+                self.n = blk.shape[0]
+            if blk.shape[0] != self.n or blk.shape[1] != nfram:
+                raise B200MError("the decoder returned %s for a block of %d clips x %d frames" % (blk.shape, self.n, nfram))
+            return blk
+        if offset < 0 or offset + nfram > self.data.shape[1]:
+            raise B200MError("block of frames %d .. %d reaches past the %d frames of the data" % (offset, offset + nfram - 1,
+                                                                                             self.data.shape[1]))
+        return self.data[:, offset:offset + nfram]
+
+    def __call__(self, offset, nfram):
+        import torch
+        offset, nfram = int(offset), int(nfram)
+        if not 1 <= nfram <= MAX_BLOCK:
+            raise B200MError("nfram %d outside 1..%d" % (nfram, MAX_BLOCK))
+        blk = self._block(offset, nfram)
+        dev = torch.device("cuda", self.device)
+        stream = torch.cuda.current_stream(dev)
+        es = blk.dtype.itemsize
+        clip_bytes = nfram * self.nchan * PCM_BYTES[self.fmt]
+        in_stride = (clip_bytes + 15) & ~15               # each clip's chunk starts at a 16-byte boundary: 16-byte loads
+        nbytes = self.n * in_stride
+        s = self.next
+        self.next ^= 1
+        if self.events[s] is not None:
+            self.events[s].synchronize()                  # the slot's previous copy has run: it may be refilled
+        if self.slots[s] is None or self.slots[s].size < nbytes:
+            self.slots[s] = host_alloc(1, (nbytes + 3) // 4).view(np.uint8).reshape(-1)
+        rows = self.slots[s][:nbytes].view(blk.dtype).reshape(self.n, in_stride // es)
+        np.copyto(rows[:, :clip_bytes // es], blk.reshape(self.n, -1))
+        d = torch.empty((self.n, in_stride), dtype=torch.uint8, device=dev)
+        d.view(-1).copy_(torch.from_numpy(self.slots[s][:nbytes]), non_blocking=True)
+        if self.events[s] is None:
+            self.events[s] = torch.cuda.Event()
+        self.events[s].record(stream)
+        return pcm_planar(d, self.fmt, self.nchan, nfram, stream)
+
+
+def pcm_source(data, nchan=None, fmt=None, device=0):
+    """The block source f(offset, nfram) that every programme_* function takes as x, fed from interleaved PCM on the host.
+
+    data: a numpy array [N, T, nchan] of int16 (PCM_S16), int32 (PCM_S32) or float32 (PCM_F32), or uint8 [N, T, nchan, 3] of packed
+    little-endian 24-bit samples (PCM_S24; e.g. an np.memmap of WAV data chunks); or a callable g(offset, nfram) that returns such an
+    array of nfram frames for a decoder, with nchan and fmt given.  f(offset, nfram) copies frames offset .. offset + nfram - 1 of
+    every clip, as raw bytes, into one of two pinned slots (host_alloc; each clip's chunk at a 16-byte boundary), uploads the slot
+    with an asynchronous copy and converts it on the device (pcm_planar), all on torch's current stream; a slot is refilled only
+    after the copy issued from it before has run.  It returns a fresh float32 CUDA tensor [N * nchan, nfram] (row i * nchan + c =
+    channel c of clip i, row pitch a multiple of 64 floats), so a programme function's results are those of the same clips given as
+    the float32 planar array of pcm_planar's scale.  A block past the data's T frames raises B200MError.  dtype, shape and format
+    are checked here, before any device use."""
+    if callable(data):
+        if nchan is None or fmt is None:
+            raise B200MError("a decoder callable needs nchan and fmt")
+        fmt, nchan = int(fmt), int(nchan)
+        _pcm_check(fmt, nchan)
+    else:
+        fmt, nchan = _pcm_layout(data, fmt, nchan)
+    return _PcmSource(data, fmt, nchan, int(device))
